@@ -1,4 +1,4 @@
-# Thin wrapper: the real build lives in faabric_b200/build.py (nvcc sm_100a + g++)
+# Thin wrapper: the real build lives in faabric_b200/build.py (nvcc sm_90a + g++)
 PY ?= python
 
 .PHONY: all build test test-gpu cpp-test bench clean

@@ -710,7 +710,7 @@ int fb_snapshot_diff_push(const void* mem,
     a.stats = (uint64_t*)statsDev;
     a.updateBase = updateBase;
     if (blocks <= 0) {
-        blocks = 148 * 2;
+        blocks = FB_NUM_SMS * 2;
     }
     return fb::launchSnapshotDiffPush(a, blocks, (cudaStream_t)stream) ==
                cudaSuccess
@@ -728,7 +728,7 @@ int fb_dirty_scan(const void* mem,
 {
     OwnerDeviceGuard ownerGuard(mem);
     if (blocks <= 0) {
-        blocks = 148 * 2;
+        blocks = FB_NUM_SMS * 2;
     }
     return fb::launchDirtyScan((const uint8_t*)mem,
                                (const uint8_t*)base,

@@ -1,6 +1,6 @@
 // Device-communication ABI shared by host C++, CUDA kernels and the C API.
 //
-// Design (B200-first, not a port): an MPI rank is bound to a GPU; every rank
+// Design (GPU-first, not a port): an MPI rank is bound to a GPU; every rank
 // owns a *symmetric heap* (identical layout on every rank) and a *signal pad*,
 // both mapped into every peer's address space over NVLink (single process:
 // peer access / VMM; multi process: CUDA IPC / VMM fds).  Collectives are ONE

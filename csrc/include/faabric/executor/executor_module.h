@@ -77,7 +77,7 @@ class ChainedCallException : public faabric::util::FaabricException
     {}
 };
 
-// Function memory that lives in HBM (B200): executors that return a non-empty
+// Function memory that lives in HBM (GPU): executors that return a non-empty
 // view take the device paths of restore / THREADS fork-join, where the
 // snapshot image, the per-host base image and the merge all stay on the GPUs
 struct DeviceMemoryView

@@ -66,7 +66,7 @@ namespace faabric::runner {
 
 // A whole deployment inside one process: the planner, and one worker that
 // registers each GPU (or any number of virtual hosts) as a separate planner
-// host.  This is the B200 single-box topology - eight GPUs behind one NVSwitch
+// host.  This is the single-box HGX topology - eight GPUs behind NVSwitch
 // are eight "hosts" to the scheduler but share an address space, so RPCs take
 // the in-process fast path and MPI ranks reach each other through peer memory.
 // (The reference needs a docker-compose cluster for the same picture.)

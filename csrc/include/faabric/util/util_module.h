@@ -726,7 +726,7 @@ class SystemConfig
     std::string plannerHost;
     int plannerPort;
 
-    // ---- B200 additions ----
+    // ---- GPU additions ----
     // Comma separated GPU ordinals this worker may use ("" = all visible)
     std::string gpus;
     // cuda | loopback  (loopback = host memory, no GPU required)
@@ -861,7 +861,7 @@ void deltaForEach(const std::vector<uint8_t>& delta,
 // same contract as the reference (include/faabric/util/dirty.h:24-236): every
 // mode reports the same pages for the same writes.  Device memory has no page
 // faults to hook, so DeviceCompareDirtyTracker diffs against the base image with
-// an sm_100a kernel (csrc/kernels/snapshot_kernels.cu: dirtyScanKernel).
+// an sm_90a kernel (csrc/kernels/snapshot_kernels.cu: dirtyScanKernel).
 
 
 namespace faabric::util {
@@ -1451,7 +1451,7 @@ int createFd(size_t size, const std::string& fdLabel);
 void appendDataToFd(int fd, std::span<uint8_t> data);
 
 // -------------------------
-// Device memory (B200)
+// Device memory (GPU)
 // -------------------------
 // Owning handle of cudaMalloc'd (or pinned-host) memory; empty on CPU boxes.
 struct DeviceRegion

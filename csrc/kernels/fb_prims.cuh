@@ -1,4 +1,4 @@
-// Device primitives for the peer-memory collectives (sm_100a).
+// Device primitives for the peer-memory collectives (sm_90a).
 //  * system-scope release/acquire flag ops and a bounded (watchdog) spin
 //  * block-level cross-rank barrier over monotonically increasing flags
 //  * 16-byte vector load/store helpers (peer-safe: no .nc, no L1 staleness)

@@ -1,4 +1,4 @@
-// Host-visible launch interface of every sm_100a kernel in csrc/kernels.
+// Host-visible launch interface of every sm_90a kernel in csrc/kernels.
 // Plain C++ (no device code) so the host runtime can be built with g++ while
 // the kernels are built with nvcc.
 #pragma once
@@ -9,6 +9,10 @@
 #include "faabric/device/comm_abi.h"
 
 namespace fb {
+
+// SMs of the target GPU (H100 SXM).  Default grids are sized from this
+// constant rather than a device query so that every rank derives the same grid.
+#define FB_NUM_SMS 132
 
 // ---------------------------------------------------------------- reduce ----
 struct ReduceArgs

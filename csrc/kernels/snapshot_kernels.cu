@@ -1,4 +1,4 @@
-// Device snapshot kernels (sm_100a).
+// Device snapshot kernels (sm_90a).
 //
 //  * snapshotDiffPushKernel — the fused north-star path: scan (optionally only
 //    the dirty 4 KiB pages), compare the executor's memory with its base image,

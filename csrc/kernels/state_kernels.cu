@@ -105,8 +105,8 @@ cudaError_t launchStatePushDirty(uint8_t* mask,
     if (blocks <= 0) {
         const uint64_t groups = (nBlocks + 31) / 32;
         blocks = (int)((groups + 7) / 8); // 8 warps per CTA, one group per warp...
-        if (blocks > 148 * 4) {
-            blocks = 148 * 4; // ...then grid-stride
+        if (blocks > FB_NUM_SMS * 4) {
+            blocks = FB_NUM_SMS * 4; // ...then grid-stride
         }
         if (blocks < 1) {
             blocks = 1;

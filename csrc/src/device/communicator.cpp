@@ -1837,8 +1837,8 @@ static int groupGrid(const CommConfig& cfg, int nranks, uint64_t vecsPerRank)
     // one rank meets CTA b of every peer at the barriers
     // a lone rank does not synchronise with anybody: two CTAs per SM for an
     // HBM-bound copy; otherwise the grid is bounded by the barrier slots
-    const int slots = nranks == 1 ? 2 * 148 : FB_MAX_BLOCKS / cfg.channels;
-    const int cap = std::min(slots, cfg.groupBlocks > 0 ? cfg.groupBlocks : (nranks == 1 ? 2 * 148 : 128));
+    const int slots = nranks == 1 ? 2 * FB_NUM_SMS : FB_MAX_BLOCKS / cfg.channels;
+    const int cap = std::min(slots, cfg.groupBlocks > 0 ? cfg.groupBlocks : (nranks == 1 ? 2 * FB_NUM_SMS : 128));
     const uint64_t warps = (uint64_t)cfg.threads / 32;
     const uint64_t chunks = (vecsPerRank + fb::fbGroupChunkVecs(nranks) - 1) / fb::fbGroupChunkVecs(nranks);
     const uint64_t want = (chunks + warps * 2 - 1) / (warps * 2); // >= 2 chunks per warp

@@ -1,4 +1,4 @@
-// Loopback device backend: host twins of the sm_100a kernels.
+// Loopback device backend: host twins of the sm_90a kernels.
 //
 // FAABRIC_DEVICE_BACKEND=loopback runs the WHOLE communicator - algorithm
 // choice, staging, chunking, channel slicing, grouped segment tables, p2p

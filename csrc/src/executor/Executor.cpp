@@ -947,7 +947,7 @@ DeviceExecutor::DeviceExecutor(faabric::Message& msg, size_t initialSize, size_t
     if (getGpuIdx() < 0) {
         throw std::runtime_error("DeviceExecutor needs a GPU");
     }
-    // Reserve the maximum up front (HBM is plentiful: 180 GB per B200), expose
+    // Reserve the maximum up front (one device allocation, 80 GB of HBM on an H100), expose
     // `currentSize` of it, like the reference's virtual reservation + mprotect
     memory = faabric::util::allocateDeviceMemory(maxSize, getGpuIdx());
     GpuGuard g(getGpuIdx());

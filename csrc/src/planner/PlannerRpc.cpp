@@ -162,11 +162,10 @@ void PlannerClient::setMessageResult(std::shared_ptr<faabric::Message> msg)
 {
     if (plannerIsInProcess(host)) {
         // No encode / decode, and no convoy on the planner's lock when every
-        // executor thread of a 1024-way fan-in reports at once.  Measured on a
-        // 128-core box (1024 functions, 8 hosts): `direct` (each executor
-        // thread takes the lock) 8.8 ms, `workers` (typed task on the planner's
-        // RPC workers) 3.5 ms, `combine` (whoever arrives first records
-        // everybody's pending results in one acquisition): see profiles/
+        // executor thread of a 1024-way fan-in reports at once: `direct` (each
+        // executor thread takes the lock), `workers` (typed task on the
+        // planner's RPC workers), `combine` (default: whoever arrives first
+        // records everybody's pending results in one acquisition)
         static const int mode = []() {
             const char* v = getenv("FAABRIC_PLANNER_RESULTS");
             std::string m = v == nullptr ? "combine" : v;

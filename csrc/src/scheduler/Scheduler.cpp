@@ -60,9 +60,11 @@ void Scheduler::addHostToGlobalSet(
         req->mutable_host()->set_usedslots(overwriteResources->usedslots());
         req->set_overwrite(true);
     } else if (hostIp == thisHost) {
-        // Execution slots: CPU cores, or slots-per-GPU x GPUs on a GPU box
+        // Execution slots: slots-per-GPU x GPUs on a GPU box, otherwise CPU
+        // cores; an explicit OVERRIDE_CPU_COUNT sets them on either
         int gpus = faabric::util::getUsableGpus();
-        int slots = gpus > 0 ? gpus * conf.slotsPerGpu : (int)faabric::util::getUsableCores();
+        int slots = gpus > 0 && conf.overrideCpuCount <= 0 ? gpus * conf.slotsPerGpu
+                                                            : (int)faabric::util::getUsableCores();
         req->mutable_host()->set_slots(slots);
         req->mutable_host()->set_usedslots(0);
     }

@@ -953,7 +953,7 @@ void DeviceSnapshot::diffAndPush(const uint8_t* mem,
         a.pageStampOut = pushStamps;
         a.pageStamp = pushStamp;
     }
-    DS_CUDA(fb::launchSnapshotDiffPush(a, 296, (cudaStream_t)stream));
+    DS_CUDA(fb::launchSnapshotDiffPush(a, FB_NUM_SMS * 2, (cudaStream_t)stream));
     diffPushCount++;
     globalDiffPushCount.fetch_add(1);
 }
@@ -988,7 +988,7 @@ std::vector<uint8_t> DeviceSnapshot::serializeDelta(const faabric::util::DeltaSe
         auto outDev = faabric::util::allocateDeviceMemory(pages.size() * 4096, device);
         DS_CUDA(cudaMemcpy(listDev.ptr, pages.data(), pages.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
         DS_CUDA(fb::launchPageGather(
-          image, mem, (const uint32_t*)listDev.ptr, (uint32_t)pages.size(), memSize, cfg.xorWithOld ? 1 : 0, outDev.ptr, 296, nullptr));
+          image, mem, (const uint32_t*)listDev.ptr, (uint32_t)pages.size(), memSize, cfg.xorWithOld ? 1 : 0, outDev.ptr, FB_NUM_SMS * 2, nullptr));
         std::vector<uint8_t> compact(pages.size() * 4096);
         DS_CUDA(cudaMemcpy(compact.data(), outDev.ptr, compact.size(), cudaMemcpyDeviceToHost));
         // 3. runs of consecutive pages become one command each
@@ -1039,7 +1039,7 @@ void DeviceSnapshot::syncPagesFrom(const uint8_t* mem, size_t n, uint32_t stamp,
     }
     DeviceGuard g(device);
     ensurePeerAccessTo(device, mem);
-    DS_CUDA(fb::launchPageSync(mem, image, pageStamps(), stamp, n, pageStatsOn(device), 296, (cudaStream_t)stream));
+    DS_CUDA(fb::launchPageSync(mem, image, pageStamps(), stamp, n, pageStatsOn(device), FB_NUM_SMS * 2, (cudaStream_t)stream));
 }
 
 void DeviceSnapshot::pullChangedPages(uint8_t* dst1, uint8_t* dst2, uint32_t since, size_t n, int onDevice, void* stream)
@@ -1053,7 +1053,7 @@ void DeviceSnapshot::pullChangedPages(uint8_t* dst1, uint8_t* dst2, uint32_t sin
     DeviceGuard g(onDevice);
     ensurePeerAccessTo(onDevice, image);
     ensurePeerAccessTo(onDevice, pageStamps());
-    DS_CUDA(fb::launchPagePull(image, dst1, dst2, pageStamps(), since, n, pageStatsOn(onDevice), 296, (cudaStream_t)stream));
+    DS_CUDA(fb::launchPagePull(image, dst1, dst2, pageStamps(), since, n, pageStatsOn(onDevice), FB_NUM_SMS * 2, (cudaStream_t)stream));
 }
 
 uint64_t DeviceSnapshot::takePageCopyCount(int onDevice, void* stream)

@@ -56,15 +56,15 @@ const std::vector<Knob>& knobs()
         { "Dirty tracking", "DIFFING_MODE", "xor", &C::diffingMode },
         { "Planner", "PLANNER_HOST", "planner", &C::plannerHost },
         { "Planner", "PLANNER_PORT", "8080", &C::plannerPort },
-        { "B200", "FAABRIC_GPUS", "", &C::gpus },
-        { "B200", "FAABRIC_DEVICE_BACKEND", "cuda", &C::deviceBackend },
-        { "B200", "FAABRIC_ALLREDUCE_ALGO", "auto", &C::allreduceAlgo },
-        { "B200", "FAABRIC_USE_NVLS", "1", &C::useNvls },
-        { "B200", "FAABRIC_COMM_STREAMS", "2", &C::commStreams },
-        { "B200", "FAABRIC_SYMM_HEAP_BYTES", "1073741824", &C::symmHeapBytes },
-        { "B200", "FAABRIC_SLOTS_PER_GPU", "8", &C::slotsPerGpu },
-        { "B200", "FAABRIC_PORT_OFFSET", "0", &C::portOffset },
-        { "B200", "FAABRIC_CHECKPOINT_DIR", "", &C::checkpointDir },
+        { "GPU", "FAABRIC_GPUS", "", &C::gpus },
+        { "GPU", "FAABRIC_DEVICE_BACKEND", "cuda", &C::deviceBackend },
+        { "GPU", "FAABRIC_ALLREDUCE_ALGO", "auto", &C::allreduceAlgo },
+        { "GPU", "FAABRIC_USE_NVLS", "1", &C::useNvls },
+        { "GPU", "FAABRIC_COMM_STREAMS", "2", &C::commStreams },
+        { "GPU", "FAABRIC_SYMM_HEAP_BYTES", "1073741824", &C::symmHeapBytes },
+        { "GPU", "FAABRIC_SLOTS_PER_GPU", "8", &C::slotsPerGpu },
+        { "GPU", "FAABRIC_PORT_OFFSET", "0", &C::portOffset },
+        { "GPU", "FAABRIC_CHECKPOINT_DIR", "", &C::checkpointDir },
     };
     return table;
 }

@@ -777,7 +777,7 @@ void DeviceCompareDirtyTracker::getDirtyPagesDevice(const uint8_t* mem,
                                                     void* stream)
 {
     cudaError_t e = fb::launchDirtyScan(
-      mem, base, size, pageFlagsDev, countDev, 296, (cudaStream_t)stream);
+      mem, base, size, pageFlagsDev, countDev, FB_NUM_SMS * 2, (cudaStream_t)stream);
     if (e != cudaSuccess) {
         throw std::runtime_error(std::string("dirty scan launch failed: ") +
                                  cudaGetErrorString(e));

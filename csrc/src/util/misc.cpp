@@ -15,6 +15,7 @@
 #include <algorithm>
 #include <arpa/inet.h>
 #include <atomic>
+#include <chrono>
 #include <cstdlib>
 #include <cstring>
 #include <fstream>
@@ -26,6 +27,7 @@
 #include <sstream>
 #include <thread>
 #include <unistd.h>
+#include <unordered_map>
 
 namespace faabric::device {
 int cudaDeviceCountSafe();
@@ -136,25 +138,41 @@ int getUsableGpus()
 }
 
 // --------------------------------------------------------------- network ---
+// Every thread builds its own planner client and resolves PLANNER_HOST, so
+// answers are kept for a while: a fan-out that starts a thousand executor
+// threads then costs a lookup or two, not a thousand serialised ones, each of
+// which may wait for a resolver that cannot answer.  A failure is kept only
+// briefly: callers fall back to ENDPOINT_HOST while a name does not resolve,
+// and a name that starts resolving is picked up within a second.
 static std::mutex hostnameMx;
+static std::unordered_map<std::string, std::pair<std::string, std::chrono::steady_clock::time_point>> hostnameCache;
+static constexpr auto HOSTNAME_CACHE_TTL = std::chrono::seconds(5);
+static constexpr auto HOSTNAME_FAILURE_TTL = std::chrono::seconds(1);
 
 std::string getIPFromHostname(const std::string& hostname)
 {
     std::lock_guard<std::mutex> lk(hostnameMx);
+    auto cached = hostnameCache.find(hostname);
+    if (cached != hostnameCache.end() &&
+        std::chrono::steady_clock::now() - cached->second.second <
+          (cached->second.first.empty() ? HOSTNAME_FAILURE_TTL : HOSTNAME_CACHE_TTL)) {
+        return cached->second.first;
+    }
     addrinfo hints;
     memset(&hints, 0, sizeof(hints));
     hints.ai_family = AF_INET;
     hints.ai_socktype = SOCK_STREAM;
     addrinfo* res = nullptr;
-    if (getaddrinfo(hostname.c_str(), nullptr, &hints, &res) != 0 ||
-        res == nullptr) {
-        return "";
+    std::string ip;
+    if (getaddrinfo(hostname.c_str(), nullptr, &hints, &res) == 0 && res != nullptr) {
+        char buf[INET_ADDRSTRLEN];
+        auto* sa = (sockaddr_in*)res->ai_addr;
+        inet_ntop(AF_INET, &sa->sin_addr, buf, sizeof(buf));
+        freeaddrinfo(res);
+        ip = buf;
     }
-    char buf[INET_ADDRSTRLEN];
-    auto* sa = (sockaddr_in*)res->ai_addr;
-    inet_ntop(AF_INET, &sa->sin_addr, buf, sizeof(buf));
-    freeaddrinfo(res);
-    return buf;
+    hostnameCache[hostname] = { ip, std::chrono::steady_clock::now() };
+    return ip;
 }
 
 std::string getPrimaryIPForThisHost(const std::string& interface)

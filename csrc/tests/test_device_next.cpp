@@ -1,6 +1,6 @@
 // Device-path tests written WITHOUT access to a GPU (the round's GPU budget was
 // spent): tag [unverified] keeps them out of `--tag gpu`, which is what the
-// pytest GPU suite runs.  First thing to do with a B200: run
+// pytest GPU suite runs.  First thing to do with a GPU: run
 //   build/bin/faabric_tests --tag unverified
 // fix what they find, then retag them [gpu].  They skip without a device.
 #include "fixtures.h"

@@ -1,6 +1,6 @@
 """The headline workload on GPUs: all-reduce the 214 gradient tensors of a
 ResNet-50 (int32, SUM) with one fused kernel per tensor, replayed from a CUDA
-graph.  Needs B200s:
+graph.  Needs H100s:
 
     python examples/gradient_sync.py                       # 1 GPU
     torchrun --nproc-per-node 8 examples/gradient_sync.py  # one process per GPU

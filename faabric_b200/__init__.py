@@ -1,4 +1,4 @@
-"""faabric_b200 — a Blackwell (B200, sm_100a) native distributed runtime with
+"""faabric_b200 — a Hopper (H100, sm_90a) native distributed runtime with
 the capabilities of faasm/faabric: Planner / Scheduler / Executor, MpiWorld,
 PointToPointBroker, SnapshotRegistry, StateKeyValue — with ranks bound to GPUs
 and the communication-bound hot paths implemented as hand-written CUDA kernels

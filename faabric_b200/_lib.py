@@ -1,6 +1,6 @@
 """ctypes binding to the in-tree native library ``lib/libfaabric_b200.so``.
 
-The library is built by :mod:`faabric_b200.build` (nvcc sm_100a + g++).  Import
+The library is built by :mod:`faabric_b200.build` (nvcc sm_90a + g++).  Import
 fails loudly if it is missing on a GPU box: there is no Python/eager fallback
 for the device ops.
 """

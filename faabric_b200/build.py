@@ -1,7 +1,7 @@
 """In-tree native build of libfaabric_b200.so (and the C++ binaries).
 
-Every ``.cu`` under ``csrc/kernels`` is compiled by nvcc for sm_100a ONLY
-(``-gencode arch=compute_100a,code=sm_100a -lineinfo``); host C++ is compiled
+Every ``.cu`` under ``csrc/kernels`` is compiled by nvcc for sm_90a ONLY
+(``-gencode arch=compute_90a,code=sm_90a -lineinfo``); host C++ is compiled
 with g++ -std=c++20.  Objects are cached under ``build/obj`` keyed by a hash of
 (source, headers mtime, flags) so incremental rebuilds are fast.  The result is
 written to ``faabric_b200/lib/libfaabric_b200.so`` so it travels with the tree.
@@ -31,7 +31,7 @@ BINDIR = BUILD / "bin"
 CUDA_HOME = Path(os.environ.get("CUDA_HOME", "/usr/local/cuda"))
 NVCC = str(CUDA_HOME / "bin" / "nvcc")
 
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = [
     "-std=c++17",
     "-O3",

@@ -18,7 +18,7 @@ The reference has no counterpart (its all-reduce is always reduce + broadcast,
 
 CLI::
 
-    python -m faabric_b200.parallel.autotune --from-json profiles/tuning_N8.json --out tuning_N8.txt
+    python -m faabric_b200.parallel.autotune --from-json tuning_N8.json --out tuning_N8.txt
     python -m faabric_b200.parallel.autotune --measure --ranks 8 --out tuning_N8.txt   # needs GPUs
 """
 
@@ -92,7 +92,7 @@ def table_from_rows(rows: Iterable[dict], hysteresis: float = 0.03) -> Table:
 
 
 def json_table_from_rows(rows: Iterable[dict]) -> List[dict]:
-    """The same table as ``table_from_rows`` in the JSON shape of ``profiles/tuning_N*.json``."""
+    """The same table as ``table_from_rows`` in the JSON shape of ``tuning_N*.json``."""
     rows = list(rows)
     out = []
     lo = 0
@@ -149,7 +149,7 @@ def native_normalise(text: str) -> str:
 
 
 def load_json_table(path) -> Table:
-    """``profiles/tuning_N*.json`` as written by ``bench.py --mode sweep``."""
+    """``tuning_N*.json`` as written by ``bench.py --mode sweep``."""
     t = json.loads(Path(path).read_text())
     table = [(int(e["max_bytes"]), e["algo"]) for e in t["allreduce"]]
     if table:

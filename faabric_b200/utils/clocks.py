@@ -1,4 +1,4 @@
-"""nvidia-smi clock / throttle sampling during a timed region (B200 profiling
+"""nvidia-smi clock / throttle sampling during a timed region (profiling
 recipe: clocks line)."""
 
 from __future__ import annotations

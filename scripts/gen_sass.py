@@ -49,7 +49,7 @@ def main():
     OUT.mkdir(parents=True, exist_ok=True)
     for old in OUT.glob("*.sass"):
         old.unlink()
-    md = ["# Memory / sync SASS mnemonics per kernel family (cuobjdump -sass, sm_100a)", "",
+    md = ["# Memory / sync SASS mnemonics per kernel family (cuobjdump -sass, sm_90a)", "",
           "Regenerate with `python scripts/gen_sass.py` after a build.  One representative",
           "instantiation per family; counts are static instruction counts.", ""]
     for fam, rx in FAMILIES.items():

@@ -1,4 +1,4 @@
-"""The built library is Blackwell code: sm_100a cubins only, and the kernels
+"""The built library is Hopper code: sm_90a cubins only, and the kernels
 contain the instructions the design depends on (checked from the SASS, no GPU
 needed).  Mnemonics: profiles/sass/MNEMONICS.md."""
 
@@ -25,12 +25,12 @@ def _mnemonics(sass: str) -> set:
     return set(re.findall(r"\b([A-Z][A-Z0-9_]*(?:\.[A-Z0-9_]+)*)\b", sass))
 
 
-def test_only_sm_100a_cubins_are_embedded(native_lib):
+def test_only_sm_90a_cubins_are_embedded(native_lib):
     r = subprocess.run([CUOBJDUMP, "-lelf", str(_lib.lib_path())], capture_output=True, text=True, timeout=120)
     assert r.returncode == 0, r.stderr
     elfs = re.findall(r"ELF file\s+\d+:\s+(\S+)", r.stdout)
     assert len(elfs) >= 6, r.stdout
-    assert all(e.endswith(".sm_100a.cubin") for e in elfs), elfs
+    assert all(e.endswith(".sm_90a.cubin") for e in elfs), elfs
     # no PTX for a JIT fallback on another architecture either
     r = subprocess.run([CUOBJDUMP, "-lptx", str(_lib.lib_path())], capture_output=True, text=True, timeout=120)
     assert "PTX file" not in r.stdout, r.stdout
