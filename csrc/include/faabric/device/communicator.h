@@ -24,6 +24,10 @@
 
 #include "faabric/device/comm_abi.h"
 
+namespace fb {
+struct KernelTable;
+}
+
 namespace faabric::device {
 
 class Bootstrap;
@@ -331,8 +335,9 @@ class Communicator
     uint32_t sbarEpoch_[FB_MAX_CHANNELS] = { 0 };
     uint32_t userSigConsumed_[FB_SIG_USER_WORDS] = { 0 };
     bool loop_ = false;
+    // CUDA launchers, or their host twins on the loopback backend
+    const fb::KernelTable* k_ = nullptr;
     void bindDevice() const;
-    cudaError_t copyD2D(void* dst, const void* src, size_t bytes, cudaStream_t s);
     bool streamSync_ = false;
     bool streamWaitOk_ = false;
     bool streamWriteOk_ = false;
@@ -360,12 +365,20 @@ class Communicator
     struct LocalGroup;
     std::shared_ptr<LocalGroup> localGroup_;
 
+    struct GroupLaunch;
+
+    static std::shared_ptr<Communicator> makeRank(const CommConfig& cfg, int rank, int nranks, int device);
     void computeLayout();
     void initAllocator();
     int blocksFor(uint64_t vecs, int perThread) const;
-    int widthFor(const void* a, const void* b, uint64_t bytes) const;
     FbCommDev devFor(int flags) const;
+    void attach(const std::vector<uint8_t*>& bases,
+                uint8_t* mcBase,
+                uint32_t* err,
+                std::shared_ptr<Backing> backing,
+                const std::string& kind);
     void finishSetup();
+    int launchGroup(const GroupLaunch& l, int dtype, int op, int flags, cudaStream_t s);
     int streamWaitGe(cudaStream_t s, const uint32_t* localWord, uint32_t value);
     int streamBarrier(int flags, cudaStream_t s);
     int sendChunk(const uint8_t* buf, size_t len, int peer, cudaStream_t s);

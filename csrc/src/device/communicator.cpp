@@ -338,7 +338,6 @@ bool Communicator::isLoopbackHeapPointer(const void* p)
 struct Communicator::Backing
 {
     bool vmm = false;
-    bool legacyIpc = false;
     size_t mapSize = 0;
     // per rank (local mode: all ranks; ipc mode: index = rank)
     std::vector<CUmemGenericAllocationHandle> handles;
@@ -352,6 +351,17 @@ struct Communicator::Backing
     std::vector<uint32_t*> errWords;
     std::vector<int> errDevices;
     std::vector<void*> hostAllocs; // loopback backend
+
+    // Binds handles[firstRank + i] (on devices[i]) to the multicast object,
+    // then maps the multicast range for the `access` devices
+    uint8_t* bindMulticast(const DriverApi& api,
+                           int firstRank,
+                           const std::vector<int>& devices,
+                           size_t gran,
+                           const std::vector<int>& access);
+    // Zeroes the signal pad and control areas at `base` and allocates the
+    // rank's error word
+    uint32_t* initDeviceRank(uint8_t* base, size_t controlBytes, int device);
 
     ~Backing()
     {
@@ -458,17 +468,55 @@ static bool multicastSupported(const DriverApi& api, int device)
     return v != 0;
 }
 
-static CUmemAllocationProp vmmProp(int device, bool shareable)
+static CUmemAllocationProp vmmProp(int device, CUmemAllocationHandleType handleType)
 {
     CUmemAllocationProp prop;
     memset(&prop, 0, sizeof(prop));
     prop.type = CU_MEM_ALLOCATION_TYPE_PINNED;
     prop.location.type = CU_MEM_LOCATION_TYPE_DEVICE;
     prop.location.id = device;
-    prop.requestedHandleTypes = shareable
-                                  ? CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR
-                                  : CU_MEM_HANDLE_TYPE_NONE;
+    prop.requestedHandleTypes = handleType;
     return prop;
+}
+
+static CUmulticastObjectProp multicastProp(int nranks, size_t size, CUmemAllocationHandleType handleType)
+{
+    CUmulticastObjectProp mp;
+    memset(&mp, 0, sizeof(mp));
+    mp.numDevices = nranks;
+    mp.size = size;
+    mp.handleTypes = handleType;
+    return mp;
+}
+
+// VMM allocation granularity of a heap of `bytes`.  `mc` is set when every
+// device of `mcDevices` (none: multicast not wanted) supports multicast and
+// the driver reports a multicast granularity; the result then covers both.
+static size_t heapGranularity(const DriverApi& api,
+                              int device,
+                              CUmemAllocationHandleType handleType,
+                              size_t bytes,
+                              int nranks,
+                              const std::vector<int>& mcDevices,
+                              bool& mc)
+{
+    size_t gran = 0;
+    CUmemAllocationProp prop = vmmProp(device, handleType);
+    CU_OK(api, api.cuMemGetAllocationGranularity(&gran, &prop, CU_MEM_ALLOC_GRANULARITY_RECOMMENDED));
+    mc = !mcDevices.empty();
+    for (int d : mcDevices) {
+        mc = mc && multicastSupported(api, d);
+    }
+    if (mc) {
+        CUmulticastObjectProp mp = multicastProp(nranks, bytes, handleType);
+        size_t mcGran = 0;
+        if (api.cuMulticastGetGranularity(&mcGran, &mp, CU_MULTICAST_GRANULARITY_RECOMMENDED) == CUDA_SUCCESS) {
+            gran = std::max(gran, mcGran);
+        } else {
+            mc = false;
+        }
+    }
+    return gran;
 }
 
 static void setAccess(const DriverApi& api,
@@ -488,6 +536,84 @@ static void setAccess(const DriverApi& api,
     CU_OK(api, api.cuMemSetAccess(va, size, descs.data(), descs.size()));
 }
 
+// Reserves an address range into `va`, maps `h` there and opens it to `devices`
+static uint8_t* mapHandle(const DriverApi& api,
+                          CUdeviceptr& va,
+                          CUmemGenericAllocationHandle h,
+                          size_t size,
+                          size_t gran,
+                          const std::vector<int>& devices)
+{
+    CU_OK(api, api.cuMemAddressReserve(&va, size, gran, 0, 0));
+    CU_OK(api, api.cuMemMap(va, size, 0, h, 0));
+    setAccess(api, va, size, devices);
+    return reinterpret_cast<uint8_t*>(va);
+}
+
+uint8_t* Communicator::Backing::bindMulticast(const DriverApi& api,
+                                              int firstRank,
+                                              const std::vector<int>& devices,
+                                              size_t gran,
+                                              const std::vector<int>& access)
+{
+    for (size_t i = 0; i < devices.size(); i++) {
+        CUDA_OK(cudaSetDevice(devices[i]));
+        CU_OK(api, api.cuMulticastBindMem(mcHandle, 0, handles[firstRank + i], 0, mapSize, 0));
+    }
+    mcVas.assign(1, 0);
+    return mapHandle(api, mcVas[0], mcHandle, mapSize, gran, access);
+}
+
+uint32_t* Communicator::Backing::initDeviceRank(uint8_t* base, size_t controlBytes, int device)
+{
+    CUDA_OK(cudaSetDevice(device));
+    CUDA_OK(cudaMemset(base, 0, controlBytes));
+    // Watchdog error word: pinned host memory the kernels can write, so
+    // the host reads it after a stream sync without a device round trip
+    uint32_t* err = nullptr;
+    CUDA_OK(cudaHostAlloc((void**)&err, 256, cudaHostAllocMapped | cudaHostAllocPortable));
+    memset(err, 0, 256);
+    errWords.push_back(err);
+    errDevices.push_back(device);
+    CUDA_OK(cudaDeviceSynchronize());
+    return err;
+}
+
+// Per-rank set-up shared by both wiring modes: configuration, heap layout,
+// allocator
+std::shared_ptr<Communicator> Communicator::makeRank(const CommConfig& cfg, int rank, int nranks, int device)
+{
+    auto c = std::shared_ptr<Communicator>(new Communicator());
+    c->cfg_ = cfg;
+    c->applyTuningFromEnv();
+    c->dev_.rank = rank;
+    c->dev_.nranks = nranks;
+    c->device_ = device;
+    c->computeLayout();
+    c->initAllocator();
+    return c;
+}
+
+// Wiring tail shared by every backing: `bases[p]` is rank p's signal pad,
+// followed by its heap
+void Communicator::attach(const std::vector<uint8_t*>& bases,
+                          uint8_t* mcBase,
+                          uint32_t* err,
+                          std::shared_ptr<Backing> backing,
+                          const std::string& kind)
+{
+    for (int p = 0; p < dev_.nranks; p++) {
+        dev_.sig[p] = reinterpret_cast<uint32_t*>(bases[p]);
+        dev_.heap[p] = bases[p] + SIG_REGION;
+    }
+    dev_.mcHeap = mcBase ? mcBase + SIG_REGION : nullptr;
+    dev_.err = err;
+    dev_.timeoutNs = cfg_.timeoutMs * 1000000ull;
+    backingState_ = std::move(backing);
+    backing_ = kind;
+    finishSetup();
+}
+
 // ---------------------------------------------------------------------------
 // Local (single-process) creation
 // ---------------------------------------------------------------------------
@@ -504,22 +630,14 @@ std::vector<std::shared_ptr<Communicator>> Communicator::createLocal(
     }
     std::vector<std::shared_ptr<Communicator>> comms;
     for (int r = 0; r < nranks; r++) {
-        auto c = std::shared_ptr<Communicator>(new Communicator());
-        c->cfg_ = cfgIn;
-        c->applyTuningFromEnv();
-        c->dev_.rank = r;
-        c->dev_.nranks = nranks;
-        c->device_ = devices[r];
-        c->computeLayout();
-        c->initAllocator();
-        comms.push_back(c);
+        comms.push_back(makeRank(cfgIn, r, nranks, devices[r]));
     }
     const size_t total = SIG_REGION + comms[0]->heapTotal_;
+    auto backing = std::make_shared<Backing>();
+    auto group = std::make_shared<LocalGroup>(nranks);
+    std::vector<uint8_t*> bases(nranks, nullptr);
     if (cfgIn.loopback) {
         // ---- loopback: host memory, host twins of the kernels ----
-        auto backing = std::make_shared<Backing>();
-        auto group = std::make_shared<LocalGroup>(nranks);
-        std::vector<uint8_t*> bases(nranks, nullptr);
         for (int r = 0; r < nranks; r++) {
             void* p = nullptr;
             if (posix_memalign(&p, 4096, total) != 0) {
@@ -540,19 +658,9 @@ std::vector<std::shared_ptr<Communicator>> Communicator::createLocal(
             }
             memset(e, 0, 256);
             backing->hostAllocs.push_back(e);
-            auto& c = comms[r];
-            c->loop_ = true;
-            for (int p = 0; p < nranks; p++) {
-                c->dev_.sig[p] = reinterpret_cast<uint32_t*>(bases[p]);
-                c->dev_.heap[p] = bases[p] + SIG_REGION;
-            }
-            c->dev_.mcHeap = nullptr;
-            c->dev_.err = (uint32_t*)e;
-            c->dev_.timeoutNs = c->cfg_.timeoutMs * 1000000ull;
-            c->backingState_ = backing;
-            c->backing_ = "loopback";
-            c->localGroup_ = group;
-            c->finishSetup();
+            comms[r]->loop_ = true;
+            comms[r]->localGroup_ = group;
+            comms[r]->attach(bases, nullptr, (uint32_t*)e, backing, "loopback");
         }
         return comms;
     }
@@ -560,104 +668,46 @@ std::vector<std::shared_ptr<Communicator>> Communicator::createLocal(
     std::vector<int> distinctDevs(distinct.begin(), distinct.end());
     const bool allDistinct = (int)distinct.size() == nranks;
 
-    auto backing = std::make_shared<Backing>();
-    std::vector<uint8_t*> bases(nranks, nullptr);
-    std::vector<uint8_t*> mcBases(nranks, nullptr);
+    uint8_t* mcBase = nullptr;
     std::string kind = "cudaMalloc+peer";
 
     const DriverApi& api = getDriverApi();
     bool vmmDone = false;
     if (cfgIn.useVmm && api.loaded) {
         try {
-            size_t gran = 0;
-            CUmemAllocationProp p0 = vmmProp(devices[0], false);
-            CU_OK(api,
-                  api.cuMemGetAllocationGranularity(
-                    &gran, &p0, CU_MEM_ALLOC_GRANULARITY_RECOMMENDED));
-            bool wantMc = cfgIn.useMulticast && allDistinct && nranks >= 2;
-            for (int d : distinctDevs) {
-                wantMc = wantMc && multicastSupported(api, d);
-            }
-            CUmulticastObjectProp mcProp;
-            memset(&mcProp, 0, sizeof(mcProp));
-            if (wantMc) {
-                mcProp.numDevices = nranks;
-                mcProp.size = total;
-                mcProp.handleTypes = 0;
-                size_t mcGran = 0;
-                if (api.cuMulticastGetGranularity(
-                      &mcGran, &mcProp, CU_MULTICAST_GRANULARITY_RECOMMENDED) ==
-                    CUDA_SUCCESS) {
-                    gran = std::max(gran, mcGran);
-                } else {
-                    wantMc = false;
-                }
-            }
-            size_t mapSize = roundUp(total, gran);
-            backing->mapSize = mapSize;
+            bool wantMc = false;
+            const bool mcAllowed = cfgIn.useMulticast && allDistinct && nranks >= 2;
+            const size_t gran = heapGranularity(
+              api, devices[0], CU_MEM_HANDLE_TYPE_NONE, total, nranks, mcAllowed ? distinctDevs : std::vector<int>(), wantMc);
+            backing->mapSize = roundUp(total, gran);
             backing->vmm = true;
             backing->handles.assign(nranks, 0);
             backing->vas.assign(nranks, 0);
             for (int r = 0; r < nranks; r++) {
                 CUDA_OK(cudaSetDevice(devices[r]));
                 CUDA_OK(cudaFree(0));
-                CUmemAllocationProp prop = vmmProp(devices[r], false);
-                CU_OK(api,
-                      api.cuMemCreate(&backing->handles[r], mapSize, &prop, 0));
-                CU_OK(api,
-                      api.cuMemAddressReserve(
-                        &backing->vas[r], mapSize, gran, 0, 0));
-                CU_OK(api,
-                      api.cuMemMap(
-                        backing->vas[r], mapSize, 0, backing->handles[r], 0));
-                setAccess(api, backing->vas[r], mapSize, distinctDevs);
-                bases[r] = reinterpret_cast<uint8_t*>(backing->vas[r]);
+                CUmemAllocationProp prop = vmmProp(devices[r], CU_MEM_HANDLE_TYPE_NONE);
+                CU_OK(api, api.cuMemCreate(&backing->handles[r], backing->mapSize, &prop, 0));
+                bases[r] = mapHandle(api, backing->vas[r], backing->handles[r], backing->mapSize, gran, distinctDevs);
             }
             vmmDone = true;
             kind = "vmm";
             if (wantMc) {
                 try {
-                    mcProp.size = mapSize;
-                    CU_OK(api,
-                          api.cuMulticastCreate(&backing->mcHandle, &mcProp));
+                    CUmulticastObjectProp mcProp = multicastProp(nranks, backing->mapSize, CU_MEM_HANDLE_TYPE_NONE);
+                    CU_OK(api, api.cuMulticastCreate(&backing->mcHandle, &mcProp));
                     backing->hasMc = true;
                     for (int r = 0; r < nranks; r++) {
                         CUdevice cd;
                         CU_OK(api, api.cuDeviceGet(&cd, devices[r]));
-                        CU_OK(api,
-                              api.cuMulticastAddDevice(backing->mcHandle, cd));
+                        CU_OK(api, api.cuMulticastAddDevice(backing->mcHandle, cd));
                     }
-                    for (int r = 0; r < nranks; r++) {
-                        CUDA_OK(cudaSetDevice(devices[r]));
-                        CU_OK(api,
-                              api.cuMulticastBindMem(backing->mcHandle,
-                                                     0,
-                                                     backing->handles[r],
-                                                     0,
-                                                     mapSize,
-                                                     0));
-                    }
-                    backing->mcVas.assign(1, 0);
-                    CU_OK(api,
-                          api.cuMemAddressReserve(
-                            &backing->mcVas[0], mapSize, gran, 0, 0));
-                    CU_OK(api,
-                          api.cuMemMap(backing->mcVas[0],
-                                       mapSize,
-                                       0,
-                                       backing->mcHandle,
-                                       0));
-                    setAccess(api, backing->mcVas[0], mapSize, distinctDevs);
-                    for (int r = 0; r < nranks; r++) {
-                        mcBases[r] =
-                          reinterpret_cast<uint8_t*>(backing->mcVas[0]);
-                    }
+                    mcBase = backing->bindMulticast(api, 0, devices, gran, distinctDevs);
                     kind = "vmm+multicast";
                 } catch (const std::exception& e) {
                     fprintf(stderr,
                             "[faabric-b200] multicast unavailable: %s\n",
                             e.what());
-                    std::fill(mcBases.begin(), mcBases.end(), nullptr);
                 }
             }
         } catch (const std::exception& e) {
@@ -700,35 +750,14 @@ std::vector<std::shared_ptr<Communicator>> Communicator::createLocal(
         CUDA_OK(cudaSetDevice(d));
         CUDA_OK(fb::preloadAllKernels());
     }
-
-    // zero the pads + control areas, allocate error words
-    auto group = std::make_shared<LocalGroup>(nranks);
     for (int r = 0; r < nranks; r++) {
-        CUDA_OK(cudaSetDevice(devices[r]));
-        CUDA_OK(cudaMemset(bases[r], 0, SIG_REGION + comms[r]->userOff_));
-        // Watchdog error word: pinned host memory the kernels can write, so
-        // the host reads it after a stream sync without a device round trip
-        uint32_t* err = nullptr;
-        CUDA_OK(cudaHostAlloc((void**)&err, 256, cudaHostAllocMapped | cudaHostAllocPortable));
-        memset(err, 0, 256);
-        backing->errWords.push_back(err);
-        backing->errDevices.push_back(devices[r]);
-        CUDA_OK(cudaDeviceSynchronize());
         auto& c = comms[r];
-        for (int p = 0; p < nranks; p++) {
-            c->dev_.sig[p] = reinterpret_cast<uint32_t*>(bases[p]);
-            c->dev_.heap[p] = bases[p] + SIG_REGION;
-        }
-        c->dev_.mcHeap = mcBases[r] ? mcBases[r] + SIG_REGION : nullptr;
-        c->dev_.err = err;
-        c->dev_.timeoutNs = c->cfg_.timeoutMs * 1000000ull;
-        c->backingState_ = backing;
-        c->backing_ = kind;
+        uint32_t* err = backing->initDeviceRank(bases[r], SIG_REGION + c->userOff_, devices[r]);
         c->localGroup_ = group;
         if (c->cfg_.streamSync < 0) {
             c->cfg_.streamSync = allDistinct ? 0 : 1;
         }
-        c->finishSetup();
+        c->attach(bases, mcBase, err, backing, kind);
     }
     return comms;
 }
@@ -748,14 +777,7 @@ std::shared_ptr<Communicator> Communicator::createIpc(int rank,
     if (!cudaAvailable()) {
         throw std::runtime_error("createIpc: no CUDA device");
     }
-    auto c = std::shared_ptr<Communicator>(new Communicator());
-    c->cfg_ = cfgIn;
-    c->applyTuningFromEnv();
-    c->dev_.rank = rank;
-    c->dev_.nranks = nranks;
-    c->device_ = device;
-    c->computeLayout();
-    c->initAllocator();
+    auto c = makeRank(cfgIn, rank, nranks, device);
     c->bootstrap_ = std::make_shared<Bootstrap>(rank, nranks, jobId);
     Bootstrap& bs = *c->bootstrap_;
 
@@ -768,6 +790,7 @@ std::shared_ptr<Communicator> Communicator::createIpc(int rank,
     std::string kind;
 
     const DriverApi& api = getDriverApi();
+    const CUmemAllocationHandleType fdType = CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR;
     // ---- stage 1: try VMM with POSIX fd export; all ranks must agree ----
     uint8_t vmmOk = 0;
     int myFd = -1;
@@ -776,40 +799,17 @@ std::shared_ptr<Communicator> Communicator::createIpc(int rank,
     uint8_t mcWanted = 0;
     if (cfgIn.useVmm && api.loaded) {
         try {
-            CUmemAllocationProp prop = vmmProp(device, true);
-            CU_OK(api,
-                  api.cuMemGetAllocationGranularity(
-                    &gran, &prop, CU_MEM_ALLOC_GRANULARITY_RECOMMENDED));
-            mcWanted = (cfgIn.useMulticast && nranks >= 2 &&
-                        multicastSupported(api, device))
-                         ? 1
-                         : 0;
-            if (mcWanted) {
-                CUmulticastObjectProp mp;
-                memset(&mp, 0, sizeof(mp));
-                mp.numDevices = nranks;
-                mp.size = total;
-                mp.handleTypes = CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR;
-                size_t mg = 0;
-                if (api.cuMulticastGetGranularity(
-                      &mg, &mp, CU_MULTICAST_GRANULARITY_RECOMMENDED) ==
-                    CUDA_SUCCESS) {
-                    gran = std::max(gran, mg);
-                } else {
-                    mcWanted = 0;
-                }
-            }
+            bool mc = false;
+            const bool mcAllowed = cfgIn.useMulticast && nranks >= 2;
+            gran = heapGranularity(
+              api, device, fdType, total, nranks, mcAllowed ? std::vector<int>{ device } : std::vector<int>(), mc);
+            mcWanted = mc ? 1 : 0;
             mapSize = roundUp(total, gran);
             backing->handles.assign(nranks, 0);
             backing->vas.assign(nranks, 0);
-            CU_OK(api,
-                  api.cuMemCreate(&backing->handles[rank], mapSize, &prop, 0));
-            CU_OK(api,
-                  api.cuMemExportToShareableHandle(
-                    &myFd,
-                    backing->handles[rank],
-                    CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR,
-                    0));
+            CUmemAllocationProp prop = vmmProp(device, fdType);
+            CU_OK(api, api.cuMemCreate(&backing->handles[rank], mapSize, &prop, 0));
+            CU_OK(api, api.cuMemExportToShareableHandle(&myFd, backing->handles[rank], fdType, 0));
             vmmOk = 1;
         } catch (const std::exception& e) {
             fprintf(stderr,
@@ -836,17 +836,10 @@ std::shared_ptr<Communicator> Communicator::createIpc(int rank,
             if (p != rank) {
                 CU_OK(api,
                       api.cuMemImportFromShareableHandle(
-                        &backing->handles[p],
-                        (void*)(uintptr_t)fds[p],
-                        CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR));
+                        &backing->handles[p], (void*)(uintptr_t)fds[p], fdType));
             }
             ::close(fds[p]);
-            CU_OK(api,
-                  api.cuMemAddressReserve(&backing->vas[p], mapSize, gran, 0, 0));
-            CU_OK(api,
-                  api.cuMemMap(backing->vas[p], mapSize, 0, backing->handles[p], 0));
-            setAccess(api, backing->vas[p], mapSize, { device });
-            bases[p] = reinterpret_cast<uint8_t*>(backing->vas[p]);
+            bases[p] = mapHandle(api, backing->vas[p], backing->handles[p], mapSize, gran, { device });
         }
         kind = "vmm-ipc";
         // ---- multicast ----
@@ -855,19 +848,10 @@ std::shared_ptr<Communicator> Communicator::createIpc(int rank,
             int mcFd = -1;
             try {
                 if (rank == 0) {
-                    CUmulticastObjectProp mp;
-                    memset(&mp, 0, sizeof(mp));
-                    mp.numDevices = nranks;
-                    mp.size = mapSize;
-                    mp.handleTypes = CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR;
+                    CUmulticastObjectProp mp = multicastProp(nranks, mapSize, fdType);
                     CU_OK(api, api.cuMulticastCreate(&backing->mcHandle, &mp));
                     backing->hasMc = true;
-                    CU_OK(api,
-                          api.cuMemExportToShareableHandle(
-                            &mcFd,
-                            backing->mcHandle,
-                            CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR,
-                            0));
+                    CU_OK(api, api.cuMemExportToShareableHandle(&mcFd, backing->mcHandle, fdType, 0));
                 }
             } catch (const std::exception& e) {
                 fprintf(stderr,
@@ -890,9 +874,7 @@ std::shared_ptr<Communicator> Communicator::createIpc(int rank,
                     if (rank != 0) {
                         CU_OK(api,
                               api.cuMemImportFromShareableHandle(
-                                &backing->mcHandle,
-                                (void*)(uintptr_t)got,
-                                CU_MEM_HANDLE_TYPE_POSIX_FILE_DESCRIPTOR));
+                                &backing->mcHandle, (void*)(uintptr_t)got, fdType));
                         backing->hasMc = true;
                     }
                     CUdevice cd;
@@ -913,25 +895,9 @@ std::shared_ptr<Communicator> Communicator::createIpc(int rank,
                     }
                 }
                 if (step) {
+                    uint8_t* mapped = nullptr;
                     try {
-                        CU_OK(api,
-                              api.cuMulticastBindMem(backing->mcHandle,
-                                                     0,
-                                                     backing->handles[rank],
-                                                     0,
-                                                     mapSize,
-                                                     0));
-                        backing->mcVas.assign(1, 0);
-                        CU_OK(api,
-                              api.cuMemAddressReserve(
-                                &backing->mcVas[0], mapSize, gran, 0, 0));
-                        CU_OK(api,
-                              api.cuMemMap(backing->mcVas[0],
-                                           mapSize,
-                                           0,
-                                           backing->mcHandle,
-                                           0));
-                        setAccess(api, backing->mcVas[0], mapSize, { device });
+                        mapped = backing->bindMulticast(api, rank, { device }, gran, { device });
                     } catch (const std::exception& e) {
                         fprintf(stderr,
                                 "[faabric-b200] rank %d multicast bind/map "
@@ -945,7 +911,7 @@ std::shared_ptr<Communicator> Communicator::createIpc(int rank,
                         step = step && all[r];
                     }
                     if (step) {
-                        mcBase = reinterpret_cast<uint8_t*>(backing->mcVas[0]);
+                        mcBase = mapped;
                         kind = "vmm-ipc+multicast";
                     }
                 }
@@ -957,7 +923,6 @@ std::shared_ptr<Communicator> Communicator::createIpc(int rank,
             ::close(myFd);
         }
         backing = std::make_shared<Backing>();
-        backing->legacyIpc = true;
         void* p = nullptr;
         CUDA_OK(cudaMalloc(&p, total));
         backing->mallocPtrs.push_back(p);
@@ -982,26 +947,11 @@ std::shared_ptr<Communicator> Communicator::createIpc(int rank,
     }
 
     CUDA_OK(fb::preloadAllKernels());
-    CUDA_OK(cudaMemset(bases[rank], 0, SIG_REGION + c->userOff_));
-    uint32_t* err = nullptr;
-    CUDA_OK(cudaHostAlloc((void**)&err, 256, cudaHostAllocMapped | cudaHostAllocPortable));
-    memset(err, 0, 256);
-    backing->errWords.push_back(err);
-    backing->errDevices.push_back(device);
-    CUDA_OK(cudaDeviceSynchronize());
-    for (int p = 0; p < nranks; p++) {
-        c->dev_.sig[p] = reinterpret_cast<uint32_t*>(bases[p]);
-        c->dev_.heap[p] = bases[p] + SIG_REGION;
-    }
-    c->dev_.mcHeap = mcBase ? mcBase + SIG_REGION : nullptr;
-    c->dev_.err = err;
-    c->dev_.timeoutNs = c->cfg_.timeoutMs * 1000000ull;
-    c->backingState_ = backing;
-    c->backing_ = kind;
+    uint32_t* err = backing->initDeviceRank(bases[rank], SIG_REGION + c->userOff_, device);
     if (c->cfg_.streamSync < 0) {
         c->cfg_.streamSync = 0;
     }
-    c->finishSetup();
+    c->attach(bases, mcBase, err, backing, kind);
     // nobody may touch a peer's pad before it has been zeroed
     bs.barrier();
     return c;
@@ -1012,15 +962,6 @@ void Communicator::bindDevice() const
     if (!loop_) {
         cudaSetDevice(device_);
     }
-}
-
-cudaError_t Communicator::copyD2D(void* dst, const void* src, size_t bytes, cudaStream_t s)
-{
-    if (loop_) {
-        memmove(dst, src, bytes);
-        return cudaSuccess;
-    }
-    return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, s);
 }
 
 cudaStream_t Communicator::internalStream()
@@ -1143,6 +1084,70 @@ uint64_t Communicator::offsetOf(const void* p) const
 }
 
 // ---------------------------------------------------------------------------
+// Kernel tables
+// ---------------------------------------------------------------------------
+namespace {
+cudaError_t cudaReduce(const fb::ReduceArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s)
+{
+    return fb::findReduceLaunchers(dtype, op)->reduce(a, a.comm.nranks, blocks, threads, s);
+}
+
+cudaError_t cudaLL(const fb::LLArgs& a, int dtype, int op, cudaStream_t s)
+{
+    return fb::findReduceLaunchers(dtype, op)->ll(a, s);
+}
+
+cudaError_t cudaGroup(const fb::GroupArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s)
+{
+    return fb::findReduceLaunchers(dtype, op)->group(a, blocks, threads, s);
+}
+
+cudaError_t cudaCopy(void* dst, const void* src, size_t bytes, cudaStream_t s)
+{
+    return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, s);
+}
+
+cudaError_t cudaCopy2D(void* dst, size_t dpitch, const void* src, size_t spitch, size_t width, size_t height, cudaStream_t s)
+{
+    return cudaMemcpy2DAsync(dst, dpitch, src, spitch, width, height, cudaMemcpyDeviceToDevice, s);
+}
+
+const fb::KernelTable CUDA_KERNELS = {
+    .reduce = cudaReduce,
+    .ll = cudaLL,
+    .group = cudaGroup,
+    .move = fb::launchMove,
+    .moveBulk = fb::launchMoveBulk,
+    .barrier = fb::launchBarrier,
+    .p2pSend = fb::launchP2PSend,
+    .p2pPull = fb::launchP2PPull,
+    .putSignal = fb::launchPutSignal,
+    .waitSignal = fb::launchWaitSignal,
+    .waitWord = fb::launchWaitWord,
+    .signalPeers = fb::launchSignalPeers,
+    .copy = cudaCopy,
+    .copy2D = cudaCopy2D,
+};
+
+const fb::KernelTable HOST_KERNELS = {
+    .reduce = fb::host::reduceKernel,
+    .ll = fb::host::llAllReduce,
+    .group = fb::host::groupAllReduce,
+    .move = fb::host::moveKernel,
+    .moveBulk = nullptr,
+    .barrier = fb::host::barrierKernel,
+    .p2pSend = fb::host::p2pSend,
+    .p2pPull = fb::host::p2pPull,
+    .putSignal = fb::host::putSignal,
+    .waitSignal = fb::host::waitSignal,
+    .waitWord = fb::host::waitWord,
+    .signalPeers = fb::host::signalPeers,
+    .copy = fb::host::copy,
+    .copy2D = fb::host::copy2D,
+};
+}
+
+// ---------------------------------------------------------------------------
 // launch helpers
 // ---------------------------------------------------------------------------
 int Communicator::blocksFor(uint64_t vecs, int perThread) const
@@ -1168,13 +1173,6 @@ static int alignWidth(uint64_t v)
         return 4;
     }
     return 1;
-}
-
-int Communicator::widthFor(const void* a, const void* b, uint64_t bytes) const
-{
-    int w = std::min(alignWidth((uint64_t)(uintptr_t)a),
-                     alignWidth((uint64_t)(uintptr_t)b));
-    return std::min(w, alignWidth(bytes));
 }
 
 FbCommDev Communicator::devFor(int flags) const
@@ -1273,8 +1271,7 @@ int Communicator::reduceLike(int kind,
     if (esize == 0) {
         return FB_E_INVALID;
     }
-    const fb::ReduceLaunchers* L = fb::findReduceLaunchers(dtype, op);
-    if (L == nullptr) {
+    if (fb::findReduceLaunchers(dtype, op) == nullptr) {
         return FB_E_UNSUPPORTED;
     }
     bindDevice();
@@ -1388,10 +1385,7 @@ int Communicator::reduceLike(int kind,
                              FB_LL_AREA_BYTES(n);
         stats_.launches++;
         stats_.bytes += bytes;
-        if (loop_) {
-            return fb::host::llAllReduce(a, dtype, op) == 0 ? FB_OK : FB_E_CUDA;
-        }
-        return L->ll(a, s) == cudaSuccess ? FB_OK : FB_E_CUDA;
+        return k_->ll(a, dtype, op, s) == cudaSuccess ? FB_OK : FB_E_CUDA;
     }
 
     // ---- staged / symmetric chunk loop ----
@@ -1434,7 +1428,7 @@ int Communicator::reduceLike(int kind,
         const uint64_t len = std::min<uint64_t>(chunkMax, bytes - done);
         uint64_t sendOff;
         if (stageSend) {
-            if (copyD2D(heapPtr(stageSendOff_), (const uint8_t*)send + done, len, s) != cudaSuccess) {
+            if (k_->copy(heapPtr(stageSendOff_), (const uint8_t*)send + done, len, s) != cudaSuccess) {
                 return FB_E_CUDA;
             }
             stats_.stagedCopies++;
@@ -1539,11 +1533,7 @@ int Communicator::reduceLike(int kind,
                 a.tailOwner = -2;
             }
             int perThread = (n == 8) ? 2 : 4;
-            if (loop_) {
-                ce = fb::host::reduceKernel(a, dtype, op, blocksFor(work, perThread)) == 0 ? cudaSuccess : cudaErrorUnknown;
-            } else {
-                ce = L->reduce(a, n, blocksFor(work, perThread), cfg_.threads, s);
-            }
+            ce = k_->reduce(a, dtype, op, blocksFor(work, perThread), cfg_.threads, s);
         }
         if (ce != cudaSuccess) {
             return FB_E_CUDA;
@@ -1555,7 +1545,7 @@ int Communicator::reduceLike(int kind,
         stats_.bytes += len;
         if (stageRecv && isRootOrAll) {
             uint64_t outLen = (kind == K_REDUCE_SCATTER) ? count * esize : len;
-            if (copyD2D((uint8_t*)recv + done, heapPtr(stageRecvOff_), outLen, s) != cudaSuccess) {
+            if (k_->copy((uint8_t*)recv + done, heapPtr(stageRecvOff_), outLen, s) != cudaSuccess) {
                 return FB_E_CUDA;
             }
             stats_.stagedCopies++;
@@ -1632,17 +1622,19 @@ int Communicator::scan(const void* send,
 // ---------------------------------------------------------------------------
 // Grouped all-reduce
 // ---------------------------------------------------------------------------
+// One launch of the grouped kernel: this rank's segment table
+struct Communicator::GroupLaunch
+{
+    fb::GroupSeg* dSegs = nullptr; // host memory on the loopback backend
+    uint32_t nSegs = 0;
+    uint32_t totalChunks = 0;
+    uint64_t vecsPerRank = 0; // same on every rank: sizes the grid
+    uint64_t bytes = 0;
+};
+
 struct Communicator::GroupPlan
 {
-    struct Launch
-    {
-        fb::GroupSeg* dSegs = nullptr;
-        uint32_t nSegs = 0;
-        uint32_t totalChunks = 0;
-        uint64_t vecsPerRank = 0; // same on every rank: sizes the grid
-        uint64_t bytes = 0;
-    };
-    std::vector<Launch> launches;
+    std::vector<GroupLaunch> launches;
     int dtype = 0;
     int device = 0;
     size_t items = 0;
@@ -1797,7 +1789,7 @@ std::shared_ptr<Communicator::GroupPlan> Communicator::prepareGroup(
         if (rc != FB_OK) {
             return nullptr;
         }
-        GroupPlan::Launch l;
+        GroupLaunch l;
         l.nSegs = (uint32_t)sb.segs.size();
         l.totalChunks = sb.totalChunks;
         l.vecsPerRank = sb.vecsPerRank;
@@ -1845,6 +1837,32 @@ static int groupGrid(const CommConfig& cfg, int nranks, uint64_t vecsPerRank)
     return (int)std::clamp<uint64_t>(want, 1, (uint64_t)cap);
 }
 
+int Communicator::launchGroup(const GroupLaunch& l, int dtype, int op, int flags, cudaStream_t s)
+{
+    const int n = dev_.nranks;
+    const bool ss = streamSync_ && !(flags & FB_FLAG_NOSYNC) && n > 1;
+    fb::GroupArgs a;
+    memset(&a, 0, sizeof(a));
+    a.comm = devFor(flags);
+    a.segs = l.dSegs;
+    a.nSegs = l.nSegs;
+    a.totalChunks = l.totalChunks;
+    a.noSync = ((flags & FB_FLAG_NOSYNC) || ss || n == 1) ? 1 : 0;
+    if (ss && streamBarrier(flags, s) != FB_OK) {
+        return FB_E_CUDA;
+    }
+    if (k_->group(a, dtype, op, groupGrid(cfg_, n, l.vecsPerRank), cfg_.threads, s) != cudaSuccess) {
+        return FB_E_CUDA;
+    }
+    if (ss && streamBarrier(flags, s) != FB_OK) {
+        return FB_E_CUDA;
+    }
+    stats_.launches++;
+    stats_.bytes += l.bytes;
+    stats_.algoCount[FB_ALGO_TWOSHOT]++;
+    return FB_OK;
+}
+
 int Communicator::allReduceGroup(const GroupPlan& plan, int op, int flags, cudaStream_t s)
 {
     NvtxRange nvtxRange("fb::allReduceGroup");
@@ -1853,30 +1871,11 @@ int Communicator::allReduceGroup(const GroupPlan& plan, int op, int flags, cudaS
         return FB_E_UNSUPPORTED;
     }
     bindDevice();
-    const int n = dev_.nranks;
-    const bool ss = streamSync_ && !(flags & FB_FLAG_NOSYNC) && n > 1;
     for (const auto& l : plan.launches) {
-        fb::GroupArgs a;
-        memset(&a, 0, sizeof(a));
-        a.comm = devFor(flags);
-        a.segs = l.dSegs;
-        a.nSegs = l.nSegs;
-        a.totalChunks = l.totalChunks;
-        a.noSync = ((flags & FB_FLAG_NOSYNC) || ss || n == 1) ? 1 : 0;
-        if (ss && streamBarrier(flags, s) != FB_OK) {
-            return FB_E_CUDA;
+        int rc = launchGroup(l, plan.dtype, op, flags, s);
+        if (rc != FB_OK) {
+            return rc;
         }
-        if (loop_) {
-            fb::host::groupAllReduce(a, plan.dtype, op, groupGrid(cfg_, n, l.vecsPerRank));
-        } else if (L->group(a, groupGrid(cfg_, n, l.vecsPerRank), cfg_.threads, s) != cudaSuccess) {
-            return FB_E_CUDA;
-        }
-        if (ss && streamBarrier(flags, s) != FB_OK) {
-            return FB_E_CUDA;
-        }
-        stats_.launches++;
-        stats_.bytes += l.bytes;
-        stats_.algoCount[FB_ALGO_TWOSHOT]++;
     }
     lastAlgo_ = FB_ALGO_TWOSHOT;
     return FB_OK;
@@ -1899,8 +1898,6 @@ int Communicator::allReduceMany(const GroupItem* items,
         return FB_E_UNSUPPORTED;
     }
     bindDevice();
-    const int n = dev_.nranks;
-    const bool ss = streamSync_ && !(flags & FB_FLAG_NOSYNC) && n > 1;
     // try the grouped path batch by batch; anything not symmetric / aligned
     // goes through the per-tensor calls (the choice depends only on arguments
     // that are symmetric across ranks)
@@ -1922,72 +1919,52 @@ int Communicator::allReduceMany(const GroupItem* items,
             }
             continue;
         }
-        if (loop_) {
-            fb::GroupArgs la;
-            memset(&la, 0, sizeof(la));
-            la.comm = devFor(flags);
-            la.segs = sb.segs.data();
-            la.nSegs = (uint32_t)sb.segs.size();
-            la.totalChunks = sb.totalChunks;
-            la.noSync = (flags & FB_FLAG_NOSYNC) ? 1 : 0;
-            fb::host::groupAllReduce(la, dtype, op, groupGrid(cfg_, n, sb.vecsPerRank));
-            stats_.launches++;
-            stats_.bytes += sb.bytes;
-            stats_.algoCount[FB_ALGO_TWOSHOT]++;
-            continue;
-        }
-        // table slot: pinned staging + device copy, recycled after its launch
-        if (manySlots_.empty()) {
-            manySlots_.resize(8);
-        }
-        auto& slotPtr = manySlots_[manyNext_++ % manySlots_.size()];
-        if (!slotPtr) {
-            slotPtr = std::make_shared<ManySlot>();
-            slotPtr->device = device_;
-            if (cudaMalloc((void**)&slotPtr->dSegs, FB_GROUP_MAX_SEGS * sizeof(fb::GroupSeg)) != cudaSuccess ||
-                cudaHostAlloc((void**)&slotPtr->hSegs, FB_GROUP_MAX_SEGS * sizeof(fb::GroupSeg), cudaHostAllocDefault) !=
-                  cudaSuccess ||
-                cudaEventCreateWithFlags(&slotPtr->ev, cudaEventDisableTiming) != cudaSuccess) {
-                cudaGetLastError();
-                slotPtr.reset();
-                return FB_E_CUDA;
+        GroupLaunch l;
+        l.dSegs = sb.segs.data(); // the host twin reads the table in place
+        l.nSegs = (uint32_t)sb.segs.size();
+        l.totalChunks = sb.totalChunks;
+        l.vecsPerRank = sb.vecsPerRank;
+        l.bytes = sb.bytes;
+        ManySlot* slot = nullptr;
+        if (!loop_) {
+            // table slot: pinned staging + device copy, recycled after its launch
+            if (manySlots_.empty()) {
+                manySlots_.resize(8);
             }
-        }
-        ManySlot& slot = *slotPtr;
-        if (slot.used) {
-            cudaEventSynchronize(slot.ev);
-        }
-        if (!sb.segs.empty()) {
-            memcpy(slot.hSegs, sb.segs.data(), sb.segs.size() * sizeof(fb::GroupSeg));
-            if (cudaMemcpyAsync(slot.dSegs, slot.hSegs, sb.segs.size() * sizeof(fb::GroupSeg), cudaMemcpyHostToDevice, s) !=
-                cudaSuccess) {
-                return FB_E_CUDA;
+            auto& slotPtr = manySlots_[manyNext_++ % manySlots_.size()];
+            if (!slotPtr) {
+                slotPtr = std::make_shared<ManySlot>();
+                slotPtr->device = device_;
+                if (cudaMalloc((void**)&slotPtr->dSegs, FB_GROUP_MAX_SEGS * sizeof(fb::GroupSeg)) != cudaSuccess ||
+                    cudaHostAlloc((void**)&slotPtr->hSegs, FB_GROUP_MAX_SEGS * sizeof(fb::GroupSeg), cudaHostAllocDefault) !=
+                      cudaSuccess ||
+                    cudaEventCreateWithFlags(&slotPtr->ev, cudaEventDisableTiming) != cudaSuccess) {
+                    cudaGetLastError();
+                    slotPtr.reset();
+                    return FB_E_CUDA;
+                }
             }
+            slot = slotPtr.get();
+            if (slot->used) {
+                cudaEventSynchronize(slot->ev);
+            }
+            if (!sb.segs.empty()) {
+                memcpy(slot->hSegs, sb.segs.data(), sb.segs.size() * sizeof(fb::GroupSeg));
+                if (cudaMemcpyAsync(slot->dSegs, slot->hSegs, sb.segs.size() * sizeof(fb::GroupSeg), cudaMemcpyHostToDevice, s) !=
+                    cudaSuccess) {
+                    return FB_E_CUDA;
+                }
+            }
+            l.dSegs = slot->dSegs;
         }
-        fb::GroupArgs a;
-        memset(&a, 0, sizeof(a));
-        a.comm = devFor(flags);
-        a.segs = slot.dSegs;
-        a.nSegs = (uint32_t)sb.segs.size();
-        a.totalChunks = sb.totalChunks;
-        a.noSync = ((flags & FB_FLAG_NOSYNC) || ss || n == 1) ? 1 : 0;
-        if (ss && streamBarrier(flags, s) != FB_OK) {
-            return FB_E_CUDA;
+        rc = launchGroup(l, dtype, op, flags, s);
+        if (rc != FB_OK) {
+            return rc;
         }
-        if (loop_) {
-            a.segs = sb.segs.data(); // the host twin reads the table in place
-            fb::host::groupAllReduce(a, dtype, op, groupGrid(cfg_, n, sb.vecsPerRank));
-        } else if (L->group(a, groupGrid(cfg_, n, sb.vecsPerRank), cfg_.threads, s) != cudaSuccess) {
-            return FB_E_CUDA;
+        if (slot != nullptr) {
+            cudaEventRecord(slot->ev, s);
+            slot->used = true;
         }
-        if (ss && streamBarrier(flags, s) != FB_OK) {
-            return FB_E_CUDA;
-        }
-        cudaEventRecord(slot.ev, s);
-        slot.used = true;
-        stats_.launches++;
-        stats_.bytes += sb.bytes;
-        stats_.algoCount[FB_ALGO_TWOSHOT]++;
     }
     lastAlgo_ = FB_ALGO_TWOSHOT;
     return FB_OK;
@@ -2013,9 +1990,7 @@ int Communicator::moveLike(int mode,
     if (chunkBytes == 0) {
         return barrier(s);
     }
-    // what this rank contributes (bytes) and whether it is a source at all
-    const bool rooted = (mode == fb::MOVE_GATHER || mode == fb::MOVE_SCATTER ||
-                         mode == fb::MOVE_BCAST);
+    // whether this rank is a source at all
     const bool isSource =
       (mode == fb::MOVE_ALLGATHER || mode == fb::MOVE_ALLTOALL ||
        mode == fb::MOVE_GATHER) ||
@@ -2023,8 +1998,6 @@ int Communicator::moveLike(int mode,
     // rows x rowBytes describes the source layout per rank
     const int srcRows =
       (mode == fb::MOVE_ALLTOALL || mode == fb::MOVE_SCATTER) ? n : 1;
-
-    (void)rooted;
 
     lastAlgo_ = FB_ALGO_ONESHOT;
     // ---- NVLS fast paths on symmetric buffers ----
@@ -2083,14 +2056,7 @@ int Communicator::moveLike(int mode,
         stats_.algoCount[FB_ALGO_TWOSHOT]++;
         stats_.launches++;
         stats_.bytes += chunkBytes;
-        if (loop_) {
-            return fb::host::moveKernel(a, blocksFor(chunkBytes / 16 / n, 4)) == 0 ? FB_OK : FB_E_CUDA;
-        }
-        return fb::launchMove(
-                 a, 16, blocksFor(chunkBytes / 16 / n, 4), cfg_.threads, s) ==
-                   cudaSuccess
-                 ? FB_OK
-                 : FB_E_CUDA;
+        return k_->move(a, 16, blocksFor(chunkBytes / 16 / n, 4), cfg_.threads, s) == cudaSuccess ? FB_OK : FB_E_CUDA;
     }
 
     // ---- generic pull, staged in pieces when buffers are not symmetric ----
@@ -2128,24 +2094,9 @@ int Communicator::moveLike(int mode,
             if (isSource) {
                 const uint8_t* src =
                   (const uint8_t*)((mode == fb::MOVE_BCAST) ? recv : send);
-                cudaError_t ce;
-                if (srcRows == 1) {
-                    ce = copyD2D(heapPtr(stageSendOff_), src + done, len, s);
-                } else if (loop_) {
-                    for (int row = 0; row < srcRows; row++) {
-                        memcpy(heapPtr(stageSendOff_) + (size_t)row * len, src + done + (size_t)row * chunkBytes, len);
-                    }
-                    ce = cudaSuccess;
-                } else {
-                    ce = cudaMemcpy2DAsync(heapPtr(stageSendOff_),
-                                           len,
-                                           src + done,
-                                           chunkBytes,
-                                           len,
-                                           srcRows,
-                                           cudaMemcpyDeviceToDevice,
-                                           s);
-                }
+                const cudaError_t ce =
+                  srcRows == 1 ? k_->copy(heapPtr(stageSendOff_), src + done, len, s)
+                               : k_->copy2D(heapPtr(stageSendOff_), len, src + done, chunkBytes, len, srcRows, s);
                 if (ce != cudaSuccess) {
                     return FB_E_CUDA;
                 }
@@ -2162,10 +2113,8 @@ int Communicator::moveLike(int mode,
         if (ss && streamBarrier(flags, s) != FB_OK) {
             return FB_E_CUDA;
         }
-        if (loop_) {
-            ce = fb::host::moveKernel(a, blocksFor(words, 2)) == 0 ? cudaSuccess : cudaErrorUnknown;
-        } else if (width == 16 && cfg_.tmaMinBytes > 0 && len >= cfg_.tmaMinBytes &&
-                   fb::moveBulkSupported(a)) {
+        if (k_->moveBulk != nullptr && width == 16 && cfg_.tmaMinBytes > 0 && len >= cfg_.tmaMinBytes &&
+            fb::moveBulkSupported(a)) {
             // Large chunks: the copy engine streams 32 KiB tiles through
             // shared memory; a few CTAs (>= 4 tiles each) saturate the link
             const uint64_t pieces =
@@ -2173,10 +2122,10 @@ int Communicator::moveLike(int mode,
             const uint64_t tiles = pieces * ((len + 32767) / 32768);
             const int maxB = std::min(cfg_.maxBlocks, FB_MAX_BLOCKS / cfg_.channels);
             const int blocks = (int)std::clamp<uint64_t>(tiles / 4, 1, (uint64_t)maxB);
-            ce = fb::launchMoveBulk(a, blocks, s);
+            ce = k_->moveBulk(a, blocks, s);
             stats_.tmaLaunches++;
         } else {
-            ce = fb::launchMove(a, width, blocksFor(words, 2), cfg_.threads, s);
+            ce = k_->move(a, width, blocksFor(words, 2), cfg_.threads, s);
         }
         if (ce != cudaSuccess) {
             return FB_E_CUDA;
@@ -2273,10 +2222,7 @@ int Communicator::barrier(cudaStream_t s)
     if (streamSync_) {
         return streamBarrier(0, s);
     }
-    if (loop_) {
-        return fb::host::barrierKernel(dev_) == 0 ? FB_OK : FB_E_CUDA;
-    }
-    return fb::launchBarrier(dev_, s) == cudaSuccess ? FB_OK : FB_E_CUDA;
+    return k_->barrier(dev_, s) == cudaSuccess ? FB_OK : FB_E_CUDA;
 }
 
 // ---------------------------------------------------------------------------
@@ -2284,6 +2230,7 @@ int Communicator::barrier(cudaStream_t s)
 // ---------------------------------------------------------------------------
 void Communicator::finishSetup()
 {
+    k_ = loop_ ? &HOST_KERNELS : &CUDA_KERNELS;
     if (dev_.heap[dev_.rank] != nullptr && heapTotal_ > 0) {
         std::unique_lock<std::shared_mutex> lk(heapRangesMx);
         heapRanges.emplace_back((const uint8_t*)dev_.heap[dev_.rank], heapTotal_);
@@ -2349,12 +2296,7 @@ int Communicator::streamWaitGe(cudaStream_t s,
         }
         // e.g. not permitted in this capture mode: use the spin kernel
     }
-    if (loop_) {
-        return fb::host::waitFlagGe(dev_, localWord, value, FB_ERR_FLAG_TIMEOUT) ? FB_OK : FB_E_CUDA;
-    }
-    return fb::launchWaitWord(dev_, localWord, value, s) == cudaSuccess
-             ? FB_OK
-             : FB_E_CUDA;
+    return k_->waitWord(dev_, localWord, value, s) == cudaSuccess ? FB_OK : FB_E_CUDA;
 }
 
 // Stream-ordered barrier of one channel: every rank signals every peer from a
@@ -2368,9 +2310,7 @@ int Communicator::streamBarrier(int flags, cudaStream_t s)
     int ch = FB_FLAG_GET_CHANNEL(flags) % cfg_.channels;
     const uint32_t e = ++sbarEpoch_[ch];
     const uint32_t wordOff = FB_SIG_SBAR_OFF + (uint32_t)ch * FB_MAX_RANKS;
-    if (loop_) {
-        fb::host::signalPeers(dev_, wordOff, e);
-    } else if (fb::launchSignalPeers(dev_, wordOff, e, s) != cudaSuccess) {
+    if (k_->signalPeers(dev_, wordOff, e, s) != cudaSuccess) {
         return FB_E_CUDA;
     }
     for (int p = 0; p < n; p++) {
@@ -2524,10 +2464,7 @@ int Communicator::sendChunk(const uint8_t* buf, size_t len, int peer, cudaStream
     stats_.launches++;
     stats_.bytes += len;
     int w = alignWidth((uint64_t)(uintptr_t)buf);
-    if (loop_) {
-        return fb::host::p2pSend(a) == 0 ? FB_OK : FB_E_CUDA;
-    }
-    return fb::launchP2PSend(a, w, p2pBlocks(len), s) == cudaSuccess ? FB_OK : FB_E_CUDA;
+    return k_->p2pSend(a, w, p2pBlocks(len), s) == cudaSuccess ? FB_OK : FB_E_CUDA;
 }
 
 int Communicator::recvChunk(uint8_t* buf, size_t len, int peer, cudaStream_t s)
@@ -2548,10 +2485,7 @@ int Communicator::recvChunk(uint8_t* buf, size_t len, int peer, cudaStream_t s)
     a.peer = peer;
     stats_.launches++;
     int w = alignWidth((uint64_t)(uintptr_t)buf);
-    if (loop_) {
-        return fb::host::p2pPull(a) == 0 ? FB_OK : FB_E_CUDA;
-    }
-    return fb::launchP2PPull(a, w, p2pBlocks(len), s) == cudaSuccess ? FB_OK : FB_E_CUDA;
+    return k_->p2pPull(a, w, p2pBlocks(len), s) == cudaSuccess ? FB_OK : FB_E_CUDA;
 }
 
 int Communicator::send(const void* buf, size_t bytes, int peer, cudaStream_t s)
@@ -2659,11 +2593,7 @@ int Communicator::putSignal(const void* local,
                      alignWidth(dstOffset));
     stats_.launches++;
     stats_.bytes += bytes;
-    if (loop_) {
-        return fb::host::putSignal(a, blocks) == 0 ? FB_OK : FB_E_CUDA;
-    }
-    return fb::launchPutSignal(a, w, blocks, s) == cudaSuccess ? FB_OK
-                                                               : FB_E_CUDA;
+    return k_->putSignal(a, w, blocks, s) == cudaSuccess ? FB_OK : FB_E_CUDA;
 }
 
 int Communicator::waitSignal(int signalIdx, uint32_t count, cudaStream_t s)
@@ -2678,12 +2608,7 @@ int Communicator::waitSignal(int signalIdx, uint32_t count, cudaStream_t s)
           s, dev_.sig[dev_.rank] + FB_SIG_USER_OFF + signalIdx, userSigConsumed_[signalIdx]);
     }
     stats_.launches++;
-    if (loop_) {
-        return fb::host::waitSignal(dev_, signalIdx, count) == 0 ? FB_OK : FB_E_CUDA;
-    }
-    return fb::launchWaitSignal(dev_, signalIdx, count, s) == cudaSuccess
-             ? FB_OK
-             : FB_E_CUDA;
+    return k_->waitSignal(dev_, signalIdx, count, s) == cudaSuccess ? FB_OK : FB_E_CUDA;
 }
 
 } // namespace faabric::device

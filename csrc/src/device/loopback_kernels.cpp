@@ -38,7 +38,7 @@ static inline uint32_t ldAcquire(const uint32_t* p)
     return aw(const_cast<uint32_t*>(p))->load(std::memory_order_acquire);
 }
 
-bool waitFlagGe(const FbCommDev& c, const uint32_t* p, uint32_t target, uint32_t errCode)
+static bool waitFlagGe(const FbCommDev& c, const uint32_t* p, uint32_t target, uint32_t errCode)
 {
     if ((int32_t)(ldAcquire(p) - target) >= 0) {
         return true;
@@ -346,7 +346,7 @@ static void reduceRange(const FbCommDev& c,
 }
 
 // --------------------------------------------------------------- reduce ----
-int reduceKernel(const ReduceArgs& a, int dtype, int op, int blocks)
+cudaError_t reduceKernel(const ReduceArgs& a, int dtype, int op, int blocks, int, cudaStream_t)
 {
     const FbCommDev& c = a.comm;
     bool ok = true;
@@ -384,11 +384,11 @@ int reduceKernel(const ReduceArgs& a, int dtype, int op, int blocks)
     if (!a.noSync) {
         gridBarrier(c, blocks);
     }
-    return 0;
+    return cudaSuccess;
 }
 
 // ------------------------------------------------------------------- LL ----
-int llAllReduce(const LLArgs& a, int dtype, int op)
+cudaError_t llAllReduce(const LLArgs& a, int dtype, int op, cudaStream_t)
 {
     const FbCommDev& c = a.comm;
     const int n = c.nranks;
@@ -456,11 +456,11 @@ int llAllReduce(const LLArgs& a, int dtype, int op)
     for (int b = 0; b < FB_LL_BLOCKS; b++) {
         *(c.sig[c.rank] + FB_SIG_LL_EPOCH_OFF + c.llEpochBase + b) = epochs[b];
     }
-    return 0;
+    return cudaSuccess;
 }
 
 // ---------------------------------------------------------------- group ----
-int groupAllReduce(const GroupArgs& a, int dtype, int op, int blocks)
+cudaError_t groupAllReduce(const GroupArgs& a, int dtype, int op, int blocks, int, cudaStream_t)
 {
     const FbCommDev& c = a.comm;
     bool ok = true;
@@ -486,11 +486,11 @@ int groupAllReduce(const GroupArgs& a, int dtype, int op, int blocks)
     if (!a.noSync) {
         gridBarrier(c, blocks);
     }
-    return 0;
+    return cudaSuccess;
 }
 
 // ----------------------------------------------------------------- move ----
-int moveKernel(const MoveArgs& a, int blocks)
+cudaError_t moveKernel(const MoveArgs& a, int, int blocks, int, cudaStream_t)
 {
     const FbCommDev& c = a.comm;
     const int rank = c.rank;
@@ -540,16 +540,16 @@ int moveKernel(const MoveArgs& a, int blocks)
     if (!a.noSync) {
         gridBarrier(c, blocks);
     }
-    return 0;
+    return cudaSuccess;
 }
 
-int barrierKernel(const FbCommDev& c)
+cudaError_t barrierKernel(const FbCommDev& c, cudaStream_t)
 {
-    return blockBarrier(c, 0) ? 0 : 1;
+    return blockBarrier(c, 0) ? cudaSuccess : cudaErrorUnknown;
 }
 
 // ------------------------------------------------------------------ p2p ----
-int p2pSend(const P2PArgs& a)
+cudaError_t p2pSend(const P2PArgs& a, int, int, cudaStream_t)
 {
     const FbCommDev& c = a.comm;
     if (a.stage && a.bytes > 0) {
@@ -562,10 +562,10 @@ int p2pSend(const P2PArgs& a)
     desc[2] = (uint32_t)(a.bytes & 0xffffffffu);
     desc[3] = (uint32_t)(a.bytes >> 32);
     stRelease(c.sig[a.peer] + FB_P2P_READY_OFF + c.rank, a.seq);
-    return 0;
+    return cudaSuccess;
 }
 
-int p2pPull(const P2PArgs& a)
+cudaError_t p2pPull(const P2PArgs& a, int, int, cudaStream_t)
 {
     const FbCommDev& c = a.comm;
     const uint32_t seen = ldAcquire(c.sig[c.rank] + FB_P2P_READY_OFF + a.peer);
@@ -583,10 +583,10 @@ int p2pPull(const P2PArgs& a)
         memcpy(a.local, c.heap[a.peer] + srcOff, len);
     }
     stRelease(c.sig[a.peer] + FB_P2P_ACK_OFF + c.rank, a.seq);
-    return 0;
+    return cudaSuccess;
 }
 
-int putSignal(const PutArgs& a, int blocks)
+cudaError_t putSignal(const PutArgs& a, int, int blocks, cudaStream_t)
 {
     const FbCommDev& c = a.comm;
     if (a.bytes > 0) {
@@ -594,27 +594,47 @@ int putSignal(const PutArgs& a, int blocks)
     }
     // one increment per "CTA", like the kernel
     aw(c.sig[a.peer] + FB_SIG_USER_OFF + a.signalIdx)->fetch_add((uint32_t)blocks, std::memory_order_release);
-    return 0;
+    return cudaSuccess;
 }
 
-int waitSignal(const FbCommDev& c, int signalIdx, uint32_t addTarget)
+cudaError_t waitSignal(const FbCommDev& c, int signalIdx, uint32_t addTarget, cudaStream_t)
 {
     uint32_t* sigp = c.sig[c.rank] + FB_SIG_USER_OFF + signalIdx;
     uint32_t* consumed = sigp + FB_SIG_USER_WORDS;
     const uint32_t target = *consumed + addTarget;
     bool ok = waitFlagGe(c, sigp, target, FB_ERR_FLAG_TIMEOUT);
     *consumed = target;
-    return ok ? 0 : 1;
+    return ok ? cudaSuccess : cudaErrorUnknown;
 }
 
-int signalPeers(const FbCommDev& c, uint32_t wordOff, uint32_t value)
+cudaError_t signalPeers(const FbCommDev& c, uint32_t wordOff, uint32_t value, cudaStream_t)
 {
     for (int p = 0; p < c.nranks; p++) {
         if (p != c.rank) {
             stRelease(c.sig[p] + wordOff + c.rank, value);
         }
     }
-    return 0;
+    return cudaSuccess;
+}
+
+cudaError_t waitWord(const FbCommDev& c, const uint32_t* word, uint32_t target, cudaStream_t)
+{
+    return waitFlagGe(c, word, target, FB_ERR_FLAG_TIMEOUT) ? cudaSuccess : cudaErrorUnknown;
+}
+
+// ----------------------------------------------------------------- copy ----
+cudaError_t copy(void* dst, const void* src, size_t bytes, cudaStream_t)
+{
+    memmove(dst, src, bytes);
+    return cudaSuccess;
+}
+
+cudaError_t copy2D(void* dst, size_t dpitch, const void* src, size_t spitch, size_t width, size_t height, cudaStream_t)
+{
+    for (size_t row = 0; row < height; row++) {
+        memcpy((uint8_t*)dst + row * dpitch, (const uint8_t*)src + row * spitch, width);
+    }
+    return cudaSuccess;
 }
 
 } // namespace fb::host

@@ -1,26 +1,61 @@
-// Host twins of the collective / p2p kernels (loopback device backend)
+// Launch table of the communicator, and the host twins of the collective / p2p
+// kernels (loopback device backend)
 #pragma once
 
 #include "launch_api.h"
 
 #include <vector>
 
+namespace fb {
+
+// Every launch the communicator makes, chosen once per communicator: the CUDA
+// launchers, or their host twins (which run to completion and ignore the
+// stream).  Reductions are resolved by (dtype, op).
+struct KernelTable
+{
+    cudaError_t (*reduce)(const ReduceArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s);
+    cudaError_t (*ll)(const LLArgs& a, int dtype, int op, cudaStream_t s);
+    cudaError_t (*group)(const GroupArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s);
+    cudaError_t (*move)(const MoveArgs& a, int width, int blocks, int threads, cudaStream_t s);
+    // TMA bulk-copy engine; null on the host
+    cudaError_t (*moveBulk)(const MoveArgs& a, int blocks, cudaStream_t s);
+    cudaError_t (*barrier)(const FbCommDev& c, cudaStream_t s);
+    cudaError_t (*p2pSend)(const P2PArgs& a, int width, int blocks, cudaStream_t s);
+    cudaError_t (*p2pPull)(const P2PArgs& a, int width, int blocks, cudaStream_t s);
+    cudaError_t (*putSignal)(const PutArgs& a, int width, int blocks, cudaStream_t s);
+    cudaError_t (*waitSignal)(const FbCommDev& c, int signalIdx, uint32_t count, cudaStream_t s);
+    cudaError_t (*waitWord)(const FbCommDev& c, const uint32_t* word, uint32_t target, cudaStream_t s);
+    cudaError_t (*signalPeers)(const FbCommDev& c, uint32_t wordOff, uint32_t value, cudaStream_t s);
+    // device-to-device copies: one range, and `height` rows of `width` bytes
+    cudaError_t (*copy)(void* dst, const void* src, size_t bytes, cudaStream_t s);
+    cudaError_t (*copy2D)(void* dst,
+                          size_t dpitch,
+                          const void* src,
+                          size_t spitch,
+                          size_t width,
+                          size_t height,
+                          cudaStream_t s);
+};
+
+}
+
 namespace fb::host {
 
 // true if (dtype, op) has an element-wise reduction
 bool reducible(int dtype, int op);
 
-bool waitFlagGe(const FbCommDev& c, const uint32_t* p, uint32_t target, uint32_t errCode);
-
-int reduceKernel(const ReduceArgs& a, int dtype, int op, int blocks);
-int llAllReduce(const LLArgs& a, int dtype, int op);
-int groupAllReduce(const GroupArgs& a, int dtype, int op, int blocks); // a.segs: HOST memory
-int moveKernel(const MoveArgs& a, int blocks);
-int barrierKernel(const FbCommDev& c);
-int p2pSend(const P2PArgs& a);
-int p2pPull(const P2PArgs& a);
-int putSignal(const PutArgs& a, int blocks);
-int waitSignal(const FbCommDev& c, int signalIdx, uint32_t addTarget);
-int signalPeers(const FbCommDev& c, uint32_t wordOff, uint32_t value);
+cudaError_t reduceKernel(const ReduceArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s);
+cudaError_t llAllReduce(const LLArgs& a, int dtype, int op, cudaStream_t s);
+cudaError_t groupAllReduce(const GroupArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s); // a.segs: HOST memory
+cudaError_t moveKernel(const MoveArgs& a, int width, int blocks, int threads, cudaStream_t s);
+cudaError_t barrierKernel(const FbCommDev& c, cudaStream_t s);
+cudaError_t p2pSend(const P2PArgs& a, int width, int blocks, cudaStream_t s);
+cudaError_t p2pPull(const P2PArgs& a, int width, int blocks, cudaStream_t s);
+cudaError_t putSignal(const PutArgs& a, int width, int blocks, cudaStream_t s);
+cudaError_t waitSignal(const FbCommDev& c, int signalIdx, uint32_t addTarget, cudaStream_t s);
+cudaError_t waitWord(const FbCommDev& c, const uint32_t* word, uint32_t target, cudaStream_t s);
+cudaError_t signalPeers(const FbCommDev& c, uint32_t wordOff, uint32_t value, cudaStream_t s);
+cudaError_t copy(void* dst, const void* src, size_t bytes, cudaStream_t s);
+cudaError_t copy2D(void* dst, size_t dpitch, const void* src, size_t spitch, size_t width, size_t height, cudaStream_t s);
 
 }
