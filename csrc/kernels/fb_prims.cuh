@@ -11,6 +11,8 @@
 #include <cuda_fp16.h>
 #include <stdint.h>
 
+#include <type_traits>
+
 #include "faabric/device/comm_abi.h"
 
 namespace fb {
@@ -201,7 +203,19 @@ struct Reducer
 {
     __device__ __forceinline__ static T apply(T a, T b)
     {
-        if constexpr (OP == FB_OP_MAX) {
+        // Float MAX/MIN use fmax/fmin (a NaN operand is ignored; NaN only if
+        // both are NaN; -0 orders below +0), so the result does not depend on
+        // which rank holds a NaN or a signed zero.  A plain `a > b ? a : b`
+        // keeps a NaN in `b` but drops one in `a`, and returns `b` for ±0.
+        if constexpr (OP == FB_OP_MAX && std::is_same_v<T, float>) {
+            return fmaxf(a, b);
+        } else if constexpr (OP == FB_OP_MAX && std::is_same_v<T, double>) {
+            return fmax(a, b);
+        } else if constexpr (OP == FB_OP_MIN && std::is_same_v<T, float>) {
+            return fminf(a, b);
+        } else if constexpr (OP == FB_OP_MIN && std::is_same_v<T, double>) {
+            return fmin(a, b);
+        } else if constexpr (OP == FB_OP_MAX) {
             return a > b ? a : b;
         } else if constexpr (OP == FB_OP_MIN) {
             return a < b ? a : b;

@@ -14,6 +14,8 @@
 // thread): a call returns when the rank's part of the collective is complete.
 #include "loopback_kernels.h"
 
+#include <faabric/util/reduce_ops.h>
+
 #include <atomic>
 #include <chrono>
 #include <cmath>
@@ -175,21 +177,22 @@ uint16_t floatToBf16(float f)
     return (uint16_t)(x >> 16);
 }
 
+// MAX/MIN/SUM/PROD as the kernels define them (faabric/util/reduce_ops.h)
 template<typename T>
 bool arith(int op, T a, T b, T& out)
 {
     switch (op) {
         case FB_OP_MAX:
-            out = a > b ? a : b;
+            out = faabric::util::reduceMax(a, b);
             return true;
         case FB_OP_MIN:
-            out = a < b ? a : b;
+            out = faabric::util::reduceMin(a, b);
             return true;
         case FB_OP_SUM:
-            out = (T)(a + b);
+            out = faabric::util::reduceSum(a, b);
             return true;
         case FB_OP_PROD:
-            out = (T)(a * b);
+            out = faabric::util::reduceProd(a, b);
             return true;
         case FB_OP_LAND:
             out = (T)((a != (T)0) && (b != (T)0));

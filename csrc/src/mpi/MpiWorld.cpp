@@ -13,6 +13,7 @@
 #include <faabric/util/gids.h>
 #include <faabric/util/logging.h>
 #include <faabric/util/macros.h>
+#include <faabric/util/reduce_ops.h>
 #include <faabric/util/testing.h>
 #include <faabric/util/timing.h>
 
@@ -1849,6 +1850,9 @@ void MpiWorld::reduceScatter(int rank,
 
 // ---- host-side element-wise reduction for every (op, dtype) ----
 namespace {
+// MAX/MIN/SUM/PROD as the device kernels define them (reduce_ops.h): integer
+// SUM/PROD wrap without signed overflow, float MAX/MIN do not depend on the
+// order of the operands (NaN, signed zeros)
 template<typename T>
 void reduceArith(int opId, int count, const uint8_t* inRaw, uint8_t* outRaw)
 {
@@ -1857,22 +1861,22 @@ void reduceArith(int opId, int count, const uint8_t* inRaw, uint8_t* outRaw)
     switch (opId) {
         case FAABRIC_OP_MAX:
             for (int i = 0; i < count; i++) {
-                out[i] = std::max<T>(out[i], in[i]);
+                out[i] = faabric::util::reduceMax(out[i], in[i]);
             }
             break;
         case FAABRIC_OP_MIN:
             for (int i = 0; i < count; i++) {
-                out[i] = std::min<T>(out[i], in[i]);
+                out[i] = faabric::util::reduceMin(out[i], in[i]);
             }
             break;
         case FAABRIC_OP_SUM:
             for (int i = 0; i < count; i++) {
-                out[i] = (T)(out[i] + in[i]);
+                out[i] = faabric::util::reduceSum(out[i], in[i]);
             }
             break;
         case FAABRIC_OP_PROD:
             for (int i = 0; i < count; i++) {
-                out[i] = (T)(out[i] * in[i]);
+                out[i] = faabric::util::reduceProd(out[i], in[i]);
             }
             break;
         case FAABRIC_OP_LAND:
@@ -1981,6 +1985,11 @@ uint16_t floatToHalf(float f, bool bf16)
     uint32_t u;
     memcpy(&u, &f, 4);
     if (bf16) {
+        // NaN stays a (quiet) NaN: the rounding increment below could carry
+        // its payload into the sign bit (0x7fffffff -> 0x8000, i.e. -0.0)
+        if ((u & 0x7fffffffu) > 0x7f800000u) {
+            return (uint16_t)((u >> 16) | 0x40u);
+        }
         // round to nearest even
         uint32_t lsb = (u >> 16) & 1;
         u += 0x7fffu + lsb;
@@ -2024,10 +2033,10 @@ void reduceHalf(int opId, int count, const uint8_t* inRaw, uint8_t* outRaw, bool
         float r;
         switch (opId) {
             case FAABRIC_OP_MAX:
-                r = std::max(a, b);
+                r = faabric::util::reduceMax(a, b);
                 break;
             case FAABRIC_OP_MIN:
-                r = std::min(a, b);
+                r = faabric::util::reduceMin(a, b);
                 break;
             case FAABRIC_OP_SUM:
                 r = a + b;

@@ -4,6 +4,7 @@
 #include <faabric/mpi/MpiWorld.h>
 #include <faabric/util/config.h>
 #include <faabric/util/logging.h>
+#include <faabric/util/reduce_ops.h>
 
 #include <algorithm>
 #include <chrono>
@@ -103,18 +104,19 @@ bool fusedReduceTyped(int opId, const uint8_t* const* srcs, int nSrc, uint8_t* d
         typed[s] = reinterpret_cast<const T*>(srcs[s]);
     }
     T* out = reinterpret_cast<T*>(dst);
+    // same element semantics as op_reduce (faabric/util/reduce_ops.h)
     switch (opId) {
         case FAABRIC_OP_SUM:
-            fusedReduceLoop<T>(typed, nSrc, out, count, [](T a, T b) { return (T)(a + b); });
+            fusedReduceLoop<T>(typed, nSrc, out, count, [](T a, T b) { return faabric::util::reduceSum(a, b); });
             return true;
         case FAABRIC_OP_PROD:
-            fusedReduceLoop<T>(typed, nSrc, out, count, [](T a, T b) { return (T)(a * b); });
+            fusedReduceLoop<T>(typed, nSrc, out, count, [](T a, T b) { return faabric::util::reduceProd(a, b); });
             return true;
         case FAABRIC_OP_MAX:
-            fusedReduceLoop<T>(typed, nSrc, out, count, [](T a, T b) { return a > b ? a : b; });
+            fusedReduceLoop<T>(typed, nSrc, out, count, [](T a, T b) { return faabric::util::reduceMax(a, b); });
             return true;
         case FAABRIC_OP_MIN:
-            fusedReduceLoop<T>(typed, nSrc, out, count, [](T a, T b) { return a < b ? a : b; });
+            fusedReduceLoop<T>(typed, nSrc, out, count, [](T a, T b) { return faabric::util::reduceMin(a, b); });
             return true;
         default:
             return false;

@@ -12,8 +12,10 @@
 #include "launch_api.h"
 
 #include <atomic>
+#include <cmath>
 #include <cstring>
 #include <functional>
+#include <limits>
 #include <numeric>
 #include <random>
 #include <thread>
@@ -204,6 +206,121 @@ TEST_CASE("loopback: reductions over dtypes and ops, pairs included", "[loopback
         }
         // bitwise ops on floats are rejected, identically on every rank
         ok = ok && c.allReduce(f, f, 4, FB_F32, FB_OP_BAND, FB_ALGO_AUTO, FB_FLAG_SYMMETRIC, nullptr) == FB_E_UNSUPPORTED;
+        return ok && c.checkError(nullptr) == 0;
+    });
+    REQUIRE_EQ(fails, 0);
+}
+
+namespace {
+// Full-range integer SUM/PROD: the inputs have the top bit set, so both wrap.
+// Expected values are computed in uint64_t (wrapping by definition) and then
+// truncated to the width of T.
+template<typename T>
+bool wrapSumProd(int rank, int n, Communicator& c, int dtype)
+{
+    const size_t count = 37; // two full vectors and a tail for every width
+    auto input = [](int r, size_t i) {
+        return (uint64_t)0x9e3779b97f4a7c15ull * (uint64_t)(r + 1) + (uint64_t)0xf00d * i | ((uint64_t)1 << 63) |
+               ((uint64_t)1 << (8 * sizeof(T) - 1));
+    };
+    T* s = heapArray<T>(c, count);
+    T* sum = heapArray<T>(c, count);
+    T* prod = heapArray<T>(c, count);
+    for (size_t i = 0; i < count; i++) {
+        s[i] = (T)input(rank, i);
+    }
+    c.hostBarrier();
+    bool ok = c.allReduce(s, sum, count, dtype, FB_OP_SUM, FB_ALGO_ONESHOT, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+    ok = ok && c.allReduce(s, prod, count, dtype, FB_OP_PROD, FB_ALGO_LL, 0, nullptr) == FB_OK;
+    for (size_t i = 0; i < count && ok; i++) {
+        uint64_t es = 0;
+        uint64_t ep = 1;
+        for (int r = 0; r < n; r++) {
+            es += input(r, i);
+            ep *= input(r, i);
+        }
+        ok = sum[i] == (T)es && prod[i] == (T)ep;
+    }
+    c.hostBarrier();
+    c.free(c.offsetOf(prod));
+    c.free(c.offsetOf(sum));
+    c.free(c.offsetOf(s));
+    return ok;
+}
+
+uint16_t bf16Bits(float f)
+{
+    uint32_t u;
+    memcpy(&u, &f, 4);
+    return (uint16_t)(u >> 16); // exact for the small integers used below
+}
+
+float bf16Value(uint16_t h)
+{
+    uint32_t u = (uint32_t)h << 16;
+    float f;
+    memcpy(&f, &u, 4);
+    return f;
+}
+}
+
+TEST_CASE("loopback: integer SUM/PROD wrap and float MAX/MIN ignore where a NaN or -0 sits", "[loopback]")
+{
+    LoopGroup g(4);
+    int fails = g.run([&](int rank, Communicator& c) {
+        const int n = c.size();
+        bool ok = wrapSumProd<int8_t>(rank, n, c, FB_I8);
+        ok = wrapSumProd<uint8_t>(rank, n, c, FB_U8) && ok;
+        ok = wrapSumProd<int16_t>(rank, n, c, FB_I16) && ok;
+        ok = wrapSumProd<uint16_t>(rank, n, c, FB_U16) && ok;
+        ok = wrapSumProd<int32_t>(rank, n, c, FB_I32) && ok;
+        ok = wrapSumProd<uint32_t>(rank, n, c, FB_U32) && ok;
+        ok = wrapSumProd<int64_t>(rank, n, c, FB_I64) && ok;
+        ok = wrapSumProd<uint64_t>(rank, n, c, FB_U64) && ok;
+
+        // rank r holds r + 1; element 0 has a NaN on rank 0, element 1 on rank
+        // n - 1, element 2 on every rank.  MAX/MIN skip a NaN operand, so only
+        // element 2 is NaN: max = {n, n - 1, NaN, n}, min = {2, 1, NaN, 1}.
+        // Elements 4 and 5 are zeros, -0 on rank 0 or on rank n - 1 and +0
+        // elsewhere: -0 orders below +0 wherever it sits, so MAX is +0 and MIN -0
+        const float nan = std::numeric_limits<float>::quiet_NaN();
+        const int count = 6;
+        auto input = [&](int r, int i) {
+            if (i >= 4) {
+                return (i == 4 && r == 0) || (i == 5 && r == n - 1) ? -0.0f : 0.0f;
+            }
+            bool isNan = (i == 0 && r == 0) || (i == 1 && r == n - 1) || i == 2;
+            return isNan ? nan : (float)(r + 1);
+        };
+        const float expMax[count] = { (float)n, (float)(n - 1), nan, (float)n, 0.0f, 0.0f };
+        const float expMin[count] = { 2.0f, 1.0f, nan, 1.0f, -0.0f, -0.0f };
+        auto same = [](float got, float exp) {
+            return std::isnan(exp) ? std::isnan(got) : got == exp && std::signbit(got) == std::signbit(exp);
+        };
+        float* f = heapArray<float>(c, count);
+        float* fMax = heapArray<float>(c, count);
+        float* fMin = heapArray<float>(c, count);
+        uint16_t* h = heapArray<uint16_t>(c, count);
+        uint16_t* hMax = heapArray<uint16_t>(c, count);
+        uint16_t* hMin = heapArray<uint16_t>(c, count);
+        for (int i = 0; i < count; i++) {
+            f[i] = input(rank, i);
+            h[i] = std::isnan(f[i]) ? (uint16_t)0x7fc0 : bf16Bits(f[i]);
+        }
+        c.hostBarrier();
+        for (int algo : { FB_ALGO_LL, FB_ALGO_ONESHOT, FB_ALGO_TWOSHOT }) {
+            ok = ok && c.allReduce(f, fMax, count, FB_F32, FB_OP_MAX, algo, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+            ok = ok && c.allReduce(f, fMin, count, FB_F32, FB_OP_MIN, algo, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+            ok = ok && c.allReduce(h, hMax, count, FB_BF16, FB_OP_MAX, algo, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+            ok = ok && c.allReduce(h, hMin, count, FB_BF16, FB_OP_MIN, algo, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+            for (int i = 0; i < count && ok; i++) {
+                ok = same(fMax[i], expMax[i]) && same(fMin[i], expMin[i]) && same(bf16Value(hMax[i]), expMax[i]) &&
+                     same(bf16Value(hMin[i]), expMin[i]);
+            }
+            if (!ok) {
+                printf("         rank %d algo %d: float MAX/MIN depends on where a NaN or -0 sits\n", rank, algo);
+            }
+        }
         return ok && c.checkError(nullptr) == 0;
     });
     REQUIRE_EQ(fails, 0);

@@ -13,6 +13,9 @@
 #include <faabric/transport/PointToPointBroker.h>
 #include <faabric/util/gids.h>
 
+#include <cmath>
+#include <cstring>
+#include <limits>
 #include <numeric>
 #include <thread>
 
@@ -375,6 +378,154 @@ TEST_CASE("mpi world case: the reduce operators on ints, doubles and long longs"
         a = { 1LL << 41, 9 };
         w.op_reduce(MPI_MIN, MPI_LONG_LONG, 2, BYTES(in.data()), BYTES(a.data()));
         REQUIRE(a == (std::vector<long long>{ 1LL << 40, -7 }));
+    }
+}
+
+namespace {
+// Position i % 6 of rank r: 0 a NaN on rank 0, 1 a NaN on the last rank, 2 a
+// NaN on every rank, 3 -0 on rank 0 (+0 elsewhere), 4 -0 on the last rank,
+// 5 no special value; the other entries hold r + 1
+template<typename T>
+T placed(int r, int n, size_t i)
+{
+    const T nan = std::numeric_limits<T>::quiet_NaN();
+    switch (i % 6) {
+        case 0:
+            return r == 0 ? nan : (T)(r + 1);
+        case 1:
+            return r == n - 1 ? nan : (T)(r + 1);
+        case 2:
+            return nan;
+        case 3:
+            return r == 0 ? (T)-0.0 : (T)0.0;
+        case 4:
+            return r == n - 1 ? (T)-0.0 : (T)0.0;
+        default:
+            return (T)(r + 1);
+    }
+}
+
+// Closed forms: MAX ignores the NaNs and orders -0 below +0
+template<typename T>
+bool placedMaxMinOk(const std::vector<T>& got, int n, bool isMax)
+{
+    for (size_t i = 0; i < got.size(); i++) {
+        T g = got[i];
+        bool ok;
+        switch (i % 6) {
+            case 0:
+                ok = g == (isMax ? (T)n : (T)2);
+                break;
+            case 1:
+                ok = g == (isMax ? (T)(n - 1) : (T)1);
+                break;
+            case 2:
+                ok = std::isnan(g);
+                break;
+            case 3:
+            case 4:
+                ok = g == 0 && std::signbit(g) == !isMax;
+                break;
+            default:
+                ok = g == (isMax ? (T)n : (T)1);
+        }
+        if (!ok) {
+            printf("         %s element %zu: got %g\n", isMax ? "MAX" : "MIN", i, (double)g);
+            return false;
+        }
+    }
+    return true;
+}
+
+uint16_t toBf16(float f)
+{
+    uint32_t u;
+    memcpy(&u, &f, 4);
+    return std::isnan(f) ? (uint16_t)0x7fc0 : (uint16_t)(u >> 16); // exact for the values used here
+}
+
+float fromBf16(uint16_t h)
+{
+    uint32_t u = (uint32_t)h << 16;
+    float f;
+    memcpy(&f, &u, 4);
+    return f;
+}
+
+// Full-range int32: every input has its top bit set, so SUM and PROD wrap
+uint32_t wideInput(int r, size_t i)
+{
+    return (0x9e3779b9u * (uint32_t)(r + 1) + 0x7f4a7c15u * (uint32_t)i) | 0x80000000u;
+}
+}
+
+TEST_CASE("mpi world case: host reductions ignore where a NaN or -0 sits and wrap integers, small and shared-memory sizes", "[mpi][world][cases]")
+{
+    // 5 elements take the message path (op_reduce); 64 Ki + 5 (> 256 KiB)
+    // take the shared-memory fused reduction in a world whose ranks all live
+    // here.  reduce() to the last rank folds the root's own input first, so a
+    // NaN or -0 on the last rank is the accumulator there.
+    const int n = 4;
+    LocalWorld f(n);
+    for (size_t count : { (size_t)5, (size_t)(64 * 1024 + 5) }) {
+        std::vector<std::vector<float>> fin(n, std::vector<float>(count));
+        std::vector<std::vector<double>> din(n, std::vector<double>(count));
+        std::vector<std::vector<uint16_t>> hin(n, std::vector<uint16_t>(count));
+        std::vector<std::vector<int32_t>> iin(n, std::vector<int32_t>(count));
+        for (int r = 0; r < n; r++) {
+            for (size_t i = 0; i < count; i++) {
+                fin[r][i] = placed<float>(r, n, i);
+                din[r][i] = placed<double>(r, n, i);
+                hin[r][i] = toBf16(fin[r][i]);
+                iin[r][i] = (int32_t)wideInput(r, i);
+            }
+        }
+        for (bool isMax : { true, false }) {
+            faabric_op_t* op = isMax ? MPI_MAX : MPI_MIN;
+            std::vector<std::vector<float>> fout(n, std::vector<float>(count));
+            std::vector<std::vector<double>> dout(n, std::vector<double>(count));
+            std::vector<std::vector<uint16_t>> hout(n, std::vector<uint16_t>(count));
+            onEveryRank(f, [&](int r) {
+                f.world.allReduce(r, BYTES(fin[r].data()), BYTES(fout[r].data()), MPI_FLOAT, (int)count, op);
+                f.world.allReduce(r, BYTES(din[r].data()), BYTES(dout[r].data()), MPI_DOUBLE, (int)count, op);
+                f.world.allReduce(r, BYTES(hin[r].data()), BYTES(hout[r].data()), MPI_BFLOAT16, (int)count, op);
+            });
+            for (int r = 0; r < n; r++) {
+                REQUIRE(placedMaxMinOk(fout[r], n, isMax));
+                REQUIRE(placedMaxMinOk(dout[r], n, isMax));
+                std::vector<float> widened(count);
+                for (size_t i = 0; i < count; i++) {
+                    widened[i] = fromBf16(hout[r][i]);
+                }
+                REQUIRE(placedMaxMinOk(widened, n, isMax));
+            }
+            std::vector<float> atRoot(count);
+            std::vector<double> dAtRoot(count);
+            onEveryRank(f, [&](int r) {
+                f.world.reduce(r, n - 1, BYTES(fin[r].data()), r == n - 1 ? BYTES(atRoot.data()) : nullptr, MPI_FLOAT, (int)count, op);
+                f.world.reduce(r, n - 1, BYTES(din[r].data()), r == n - 1 ? BYTES(dAtRoot.data()) : nullptr, MPI_DOUBLE, (int)count, op);
+            });
+            REQUIRE(placedMaxMinOk(atRoot, n, isMax));
+            REQUIRE(placedMaxMinOk(dAtRoot, n, isMax));
+        }
+        for (faabric_op_t* op : { MPI_SUM, MPI_PROD }) {
+            std::vector<std::vector<int32_t>> out(n, std::vector<int32_t>(count));
+            onEveryRank(f, [&](int r) { f.world.allReduce(r, BYTES(iin[r].data()), BYTES(out[r].data()), MPI_INT, (int)count, op); });
+            std::vector<int32_t> atRoot(count);
+            onEveryRank(f, [&](int r) {
+                f.world.reduce(r, n - 1, BYTES(iin[r].data()), r == n - 1 ? BYTES(atRoot.data()) : nullptr, MPI_INT, (int)count, op);
+            });
+            for (size_t i = 0; i < count; i++) {
+                uint32_t e = op == MPI_SUM ? 0u : 1u;
+                for (int r = 0; r < n; r++) {
+                    e = op == MPI_SUM ? e + wideInput(r, i) : e * wideInput(r, i);
+                }
+                REQUIRE_EQ(atRoot[i], (int32_t)e);
+                for (int r = 0; r < n; r++) {
+                    REQUIRE_EQ(out[r][i], (int32_t)e);
+                }
+            }
+        }
     }
 }
 

@@ -42,6 +42,30 @@ for _name, _code in (("uint16", 3), ("uint32", 5), ("uint64", 7)):
     if hasattr(torch, _name):
         _DTYPES[getattr(torch, _name)] = _code
 
+# Every FbDtype by name, with its element size in bytes (fbDtypeSize).  The
+# `dtype=` argument of the reductions takes one of these names: the tensor is
+# then read as raw bytes of that type, which reaches the unsigned integers on
+# any torch version and the MAXLOC/MINLOC {value, int32} pairs (the 16-byte
+# pairs include 4 bytes of padding).
+FB_DTYPES = {
+    "i8": (0, 1),
+    "u8": (1, 1),
+    "i16": (2, 2),
+    "u16": (3, 2),
+    "i32": (4, 4),
+    "u32": (5, 4),
+    "i64": (6, 8),
+    "u64": (7, 8),
+    "f32": (8, 4),
+    "f64": (9, 8),
+    "f16": (10, 2),
+    "bf16": (11, 2),
+    "f64_i32": (12, 16),
+    "f32_i32": (13, 8),
+    "i32_i32": (14, 8),
+    "i64_i32": (15, 16),
+}
+
 OPS = {
     "max": 0,
     "min": 1,
@@ -147,6 +171,21 @@ class Communicator:
         except KeyError:
             raise CommError(f"unsupported dtype {t.dtype}")
 
+    @classmethod
+    def _typed(cls, t: torch.Tensor, dtype: Optional[str]) -> tuple[int, int]:
+        """(element count, FbDtype code) of ``t``, read as ``dtype`` when given
+        (an FbDtype name, see FB_DTYPES) or as its own torch dtype otherwise."""
+        if dtype is None:
+            return t.numel(), cls._dtype(t)
+        try:
+            code, esize = FB_DTYPES[dtype]
+        except KeyError:
+            raise CommError(f"unknown dtype {dtype!r}; one of {', '.join(FB_DTYPES)}")
+        nbytes = t.numel() * t.element_size()
+        if nbytes % esize != 0:
+            raise CommError(f"{nbytes} bytes is not a whole number of {dtype} elements ({esize} bytes)")
+        return nbytes // esize, code
+
     # ------------------------------------------------------------ heap
     def empty(self, shape, dtype=torch.float32) -> torch.Tensor:
         """Allocate a tensor in the symmetric heap.  Call collectively (same
@@ -227,8 +266,9 @@ class Communicator:
         self._lib.fb_comm_host_barrier(self._h)
 
     # ------------------------------------------------------------ collectives
-    def all_reduce(self, send, recv=None, op="sum", algo="auto", stream=None, flags=None, channel=0):
+    def all_reduce(self, send, recv=None, op="sum", algo="auto", stream=None, flags=None, channel=0, dtype=None):
         recv = send if recv is None else recv
+        count, dt = self._typed(send, dtype)
         # only the source needs to be symmetric; the native side stages the
         # destination when a push algorithm needs it
         f = self._sym(send) if flags is None else flags
@@ -237,8 +277,8 @@ class Communicator:
             self._h,
             C.c_void_p(send.data_ptr()),
             C.c_void_p(recv.data_ptr()),
-            send.numel(),
-            self._dtype(send),
+            count,
+            dt,
             OPS[op],
             ALGOS[algo],
             f,
@@ -247,15 +287,16 @@ class Communicator:
         self._check(rc, "all_reduce")
         return recv
 
-    def reduce(self, send, recv, root=0, op="sum", stream=None, flags=None):
+    def reduce(self, send, recv, root=0, op="sum", stream=None, flags=None, dtype=None):
         f = self._sym(send) if flags is None else flags
+        count, dt = self._typed(send, dtype)
         rp = recv.data_ptr() if recv is not None else 0
         rc = self._lib.fb_reduce(
             self._h,
             C.c_void_p(send.data_ptr()),
             C.c_void_p(rp),
-            send.numel(),
-            self._dtype(send),
+            count,
+            dt,
             OPS[op],
             root,
             f,
@@ -264,14 +305,16 @@ class Communicator:
         self._check(rc, "reduce")
         return recv
 
-    def reduce_scatter(self, send, recv, op="sum", stream=None, flags=None):
+    def reduce_scatter(self, send, recv, op="sum", stream=None, flags=None, dtype=None):
         f = self._sym(send) if flags is None else flags
+        count, _ = self._typed(recv, dtype)
+        _, dt = self._typed(send, dtype)
         rc = self._lib.fb_reduce_scatter(
             self._h,
             C.c_void_p(send.data_ptr()),
             C.c_void_p(recv.data_ptr()),
-            recv.numel(),
-            self._dtype(send),
+            count,
+            dt,
             OPS[op],
             f,
             self._stream(stream),
@@ -279,14 +322,15 @@ class Communicator:
         self._check(rc, "reduce_scatter")
         return recv
 
-    def scan(self, send, recv, op="sum", stream=None, flags=None):
+    def scan(self, send, recv, op="sum", stream=None, flags=None, dtype=None):
         f = self._sym(send) if flags is None else flags
+        count, dt = self._typed(send, dtype)
         rc = self._lib.fb_scan(
             self._h,
             C.c_void_p(send.data_ptr()),
             C.c_void_p(recv.data_ptr()),
-            send.numel(),
-            self._dtype(send),
+            count,
+            dt,
             OPS[op],
             f,
             self._stream(stream),
@@ -371,22 +415,24 @@ class Communicator:
         return recv
 
     # ------------------------------------------------- grouped all-reduce
-    def _group_arrays(self, sends, recvs):
+    def _group_arrays(self, sends, recvs, dtype):
         n = len(sends)
         sp = (C.c_void_p * n)(*[t.data_ptr() for t in sends])
         rp = (C.c_void_p * n)(*[t.data_ptr() for t in recvs])
-        cnt = (C.c_uint64 * n)(*[t.numel() for t in sends])
-        return n, sp, rp, cnt
+        typed = [self._typed(t, dtype) for t in sends]
+        if len({dt for _, dt in typed}) != 1:
+            raise CommError("grouped all-reduce: every tensor must have the same dtype")
+        cnt = (C.c_uint64 * n)(*[c for c, _ in typed])
+        return n, sp, rp, cnt, typed[0][1]
 
-    def prepare_group(self, sends, recvs=None) -> "GroupPlan":
+    def prepare_group(self, sends, recvs=None, dtype=None) -> "GroupPlan":
         """Plan ONE launch that all-reduces every tensor of ``sends`` (each with
         per-tensor semantics).  Tensors must live in the symmetric heap at
         16-byte aligned addresses; call collectively with the same list."""
         recvs = sends if recvs is None else recvs
         if len(sends) != len(recvs) or not sends:
             raise CommError("prepare_group: need equally long, non-empty lists")
-        dt = self._dtype(sends[0])
-        n, sp, rp, cnt = self._group_arrays(sends, recvs)
+        n, sp, rp, cnt, dt = self._group_arrays(sends, recvs, dtype)
         h = self._lib.fb_group_prepare(self._h, n, sp, rp, cnt, dt)
         if not h:
             raise CommError(f"prepare_group failed [{_lib.last_error()}]")
@@ -398,12 +444,13 @@ class Communicator:
         )
         self._check(rc, "all_reduce_group")
 
-    def all_reduce_many(self, sends, recvs=None, op="sum", stream=None, channel=0):
+    def all_reduce_many(self, sends, recvs=None, op="sum", stream=None, channel=0, dtype=None):
         """Transient variant of :meth:`prepare_group` + :meth:`all_reduce_group`
         (the table is rebuilt and uploaded in stream order on every call)."""
         recvs = sends if recvs is None else recvs
-        dt = self._dtype(sends[0])
-        n, sp, rp, cnt = self._group_arrays(sends, recvs)
+        if not sends:
+            raise CommError("all_reduce_many: need a non-empty list")
+        n, sp, rp, cnt, dt = self._group_arrays(sends, recvs, dtype)
         f = self._sym(*sends) | ((channel & 0xF) << 8)
         rc = self._lib.fb_allreduce_many(self._h, n, sp, rp, cnt, dt, OPS[op], f, self._stream(stream))
         self._check(rc, "all_reduce_many")
