@@ -625,7 +625,8 @@ const char* fb_error_string(int code)
 // SnapshotData::fillGapsWithBytewiseRegions (reference
 // src/util/snapshot.cpp:259-324) and split out the typed ones.  `fillOp` is
 // FB_MERGE_BYTEWISE or FB_MERGE_XOR.  Returns the number of regions written to
-// `out` (capacity maxOut) and the typed indices in typedOut.
+// `out` (capacity maxOut) and the typed indices in typedOut, FB_E_INVALID for
+// overlapping regions and FB_E_TOO_LARGE when `out` is too small.
 int fb_snapshot_prepare_regions(const FbMergeRegionDev* in,
                                 int nIn,
                                 int fillOp,
@@ -645,6 +646,11 @@ int fb_snapshot_prepare_regions(const FbMergeRegionDev* in,
     uint64_t cursor = 0;
     bool toEnd = false;
     for (const auto& r : regs) {
+        // overlapping regions, or any region after a to-end one, are refused
+        // (SnapshotData::fillGapsWithBytewiseRegions throws on the same input)
+        if (toEnd || r.offset < cursor) {
+            return FB_E_INVALID;
+        }
         if (r.offset > cursor) {
             filled.push_back(
               { cursor, r.offset - cursor, FB_SNAP_RAW, fillOp });
@@ -652,9 +658,9 @@ int fb_snapshot_prepare_regions(const FbMergeRegionDev* in,
         filled.push_back(r);
         if (r.length == 0) {
             toEnd = true;
-            break;
+        } else {
+            cursor = r.offset + r.length;
         }
-        cursor = std::max(cursor, r.offset + r.length);
     }
     if (!toEnd && cursor < size) {
         filled.push_back({ cursor, 0, FB_SNAP_RAW, fillOp });

@@ -249,11 +249,13 @@ struct SnapDiffArgs
     const FbMergeRegionDev* regions; // sorted by offset, gaps already filled
     int32_t nRegions;
     const int32_t* typedIdx; // indices of regions with a typed merge op
-    int32_t nTyped;
+    int32_t nTyped;            // > 0: clean pages before dirty ones are visited too
     const uint8_t* dirtyPages; // 1 byte per 4 KiB page, null => scan everything
-    uint8_t* pageFlagsOut;     // optional: pages that produced a diff
+    // optional: pages in which a diff starts (a changed Bytewise / XOR byte,
+    // or the first byte of a typed scalar that produced a diff)
+    uint8_t* pageFlagsOut;
     uint8_t* chunkFlags;       // optional: 128-byte chunks that produced a diff
-    uint64_t* stats;           // [0]=diff bytes, [1]=pages with diffs
+    uint64_t* stats;           // [0]=diff bytes, [1]=pages flagged as above
     int32_t updateBase;        // also fold the changes into the local base
     // optional: one word per 4 KiB page of `dst`, set to `pageStamp` for every
     // page this launch changed (peers find out what to re-pull at the next fork)

@@ -19,9 +19,12 @@
 //
 // Semantics kept from the reference: Bytewise stores exactly the bytes that
 // differ (byte-exact merge safety between concurrent writers), XOR merges
-// orig^updated with an atomic xor, typed regions merge scalars
-// (Sum: +=new-old, Subtract: -=(old-new), Product: *=new/old, Max/Min).
+// orig^updated with an atomic xor, typed regions merge arrays of scalars
+// (Sum: +=new-old, Subtract: -=(old-new), Product: *=new/old, Max/Min) with
+// the rules of faabric/util/reduce_ops.h (see snapAdd ... snapQuotient).
 #include "snapshot_kernels.cuh"
+
+#include <type_traits>
 
 namespace fb {
 
@@ -387,6 +390,87 @@ __device__ __forceinline__ bool atomicRmwUnalignedSys(uint8_t* d, F f)
     }
 }
 
+// Typed merge rules, the device form of faabric/util/reduce_ops.h (reduceSum,
+// reduceSub, reduceProd, reduceMax, reduceMin, snapshotQuotient): integers
+// wrap, computed in the unsigned type of the same width; float Max/Min are
+// fmax/fmin as in Reducer (fb_prims.cuh), so a NaN operand is ignored and -0
+// orders below +0 whichever writer lands first.
+template<typename T>
+__device__ __forceinline__ T snapAdd(T a, T b)
+{
+    if constexpr (std::is_integral_v<T>) {
+        using U = std::make_unsigned_t<T>;
+        return (T)(U)((U)a + (U)b);
+    } else {
+        return a + b;
+    }
+}
+
+template<typename T>
+__device__ __forceinline__ T snapSub(T a, T b)
+{
+    if constexpr (std::is_integral_v<T>) {
+        using U = std::make_unsigned_t<T>;
+        return (T)(U)((U)a - (U)b);
+    } else {
+        return a - b;
+    }
+}
+
+template<typename T>
+__device__ __forceinline__ T snapMul(T a, T b)
+{
+    if constexpr (std::is_integral_v<T>) {
+        using U = std::make_unsigned_t<T>;
+        return (T)(U)((U)a * (U)b);
+    } else {
+        return a * b;
+    }
+}
+
+template<typename T>
+__device__ __forceinline__ T snapMax(T a, T b)
+{
+    if constexpr (std::is_same_v<T, float>) {
+        return fmaxf(a, b);
+    } else if constexpr (std::is_same_v<T, double>) {
+        return fmax(a, b);
+    } else {
+        return a > b ? a : b;
+    }
+}
+
+template<typename T>
+__device__ __forceinline__ T snapMin(T a, T b)
+{
+    if constexpr (std::is_same_v<T, float>) {
+        return fminf(a, b);
+    } else if constexpr (std::is_same_v<T, double>) {
+        return fmin(a, b);
+    } else {
+        return a < b ? a : b;
+    }
+}
+
+// Product factor for a value that went from o to n: IEEE n / o for floats;
+// for integers 0 when o is 0, a wrapping negation when o is -1, otherwise the
+// truncated quotient
+template<typename T>
+__device__ __forceinline__ T snapQuotient(T n, T o)
+{
+    if constexpr (std::is_integral_v<T>) {
+        if (o == 0) {
+            return 0;
+        }
+        if (o == (T)-1) {
+            return snapSub((T)0, n);
+        }
+        return n / o;
+    } else {
+        return n / o;
+    }
+}
+
 // Merge one scalar.  Returns true if a diff was produced.
 template<typename T>
 __device__ __forceinline__ bool mergeScalar(const SnapDiffArgs& a,
@@ -400,38 +484,44 @@ __device__ __forceinline__ bool mergeScalar(const SnapDiffArgs& a,
     }
     uint8_t* d = a.dst + off;
     const bool aligned = ((uintptr_t)d % sizeof(T)) == 0;
-    constexpr bool isInt = (T)0.5 == (T)0; // integer types truncate
+    constexpr bool isInt = std::is_integral_v<T>;
     switch (op) {
         case FB_MERGE_SUM: {
-            T delta = m - o;
+            T delta = snapSub(m, o);
             if (aligned) {
                 redAddSys(reinterpret_cast<T*>(d), delta);
             } else {
-                if (!atomicRmwUnalignedSys<T>(d, [delta](T c) { return (T)(c + delta); })) {
-                    storeUnaligned<T>(d, (T)(loadUnaligned<T>(d) + delta));
+                if (!atomicRmwUnalignedSys<T>(d, [delta](T c) { return snapAdd(c, delta); })) {
+                    storeUnaligned<T>(d, snapAdd(loadUnaligned<T>(d), delta));
                 }
             }
             break;
         }
         case FB_MERGE_SUBTRACT: {
-            T diff = o - m; // applied as main - diff
+            T diff = snapSub(o, m); // applied as main - diff
             if (aligned) {
-                redAddSys(reinterpret_cast<T*>(d), (T)(-diff));
+                T neg;
+                if constexpr (isInt) {
+                    neg = snapSub((T)0, diff);
+                } else {
+                    neg = -diff;
+                }
+                redAddSys(reinterpret_cast<T*>(d), neg);
             } else {
-                if (!atomicRmwUnalignedSys<T>(d, [diff](T c) { return (T)(c - diff); })) {
-                    storeUnaligned<T>(d, (T)(loadUnaligned<T>(d) - diff));
+                if (!atomicRmwUnalignedSys<T>(d, [diff](T c) { return snapSub(c, diff); })) {
+                    storeUnaligned<T>(d, snapSub(loadUnaligned<T>(d), diff));
                 }
             }
             break;
         }
         case FB_MERGE_PRODUCT: {
-            T q = (o == (T)0) ? (T)0 : (T)(m / o);
+            T q = snapQuotient(m, o);
             if (aligned) {
                 atomicRmwSys<T>(reinterpret_cast<T*>(d),
-                                [q](T c) { return (T)(c * q); });
+                                [q](T c) { return snapMul(c, q); });
             } else {
-                if (!atomicRmwUnalignedSys<T>(d, [q](T c) { return (T)(c * q); })) {
-                    storeUnaligned<T>(d, (T)(loadUnaligned<T>(d) * q));
+                if (!atomicRmwUnalignedSys<T>(d, [q](T c) { return snapMul(c, q); })) {
+                    storeUnaligned<T>(d, snapMul(loadUnaligned<T>(d), q));
                 }
             }
             break;
@@ -442,12 +532,11 @@ __device__ __forceinline__ bool mergeScalar(const SnapDiffArgs& a,
                     redMaxSys(reinterpret_cast<T*>(d), m);
                 } else {
                     atomicRmwSys<T>(reinterpret_cast<T*>(d),
-                                    [m](T c) { return c > m ? c : m; });
+                                    [m](T c) { return snapMax(c, m); });
                 }
             } else {
-                if (!atomicRmwUnalignedSys<T>(d, [m](T c) { return c > m ? c : m; })) {
-                    T c = loadUnaligned<T>(d);
-                    storeUnaligned<T>(d, c > m ? c : m);
+                if (!atomicRmwUnalignedSys<T>(d, [m](T c) { return snapMax(c, m); })) {
+                    storeUnaligned<T>(d, snapMax(loadUnaligned<T>(d), m));
                 }
             }
             break;
@@ -458,12 +547,11 @@ __device__ __forceinline__ bool mergeScalar(const SnapDiffArgs& a,
                     redMinSys(reinterpret_cast<T*>(d), m);
                 } else {
                     atomicRmwSys<T>(reinterpret_cast<T*>(d),
-                                    [m](T c) { return c < m ? c : m; });
+                                    [m](T c) { return snapMin(c, m); });
                 }
             } else {
-                if (!atomicRmwUnalignedSys<T>(d, [m](T c) { return c < m ? c : m; })) {
-                    T c = loadUnaligned<T>(d);
-                    storeUnaligned<T>(d, c < m ? c : m);
+                if (!atomicRmwUnalignedSys<T>(d, [m](T c) { return snapMin(c, m); })) {
+                    storeUnaligned<T>(d, snapMin(loadUnaligned<T>(d), m));
                 }
             }
             break;
@@ -486,6 +574,60 @@ __device__ __forceinline__ bool pageDirty(const SnapDiffArgs& a, uint64_t page)
     return a.dirtyPages == nullptr || a.dirtyPages[page] != 0;
 }
 
+// Typed region: the scalars of `reg` (an array of floor(length / size) of
+// them, cut at the image end) whose first byte lies in [pBeg, pEnd), one lane
+// per scalar.  A scalar is merged when its first or its last page is dirty.
+__device__ __forceinline__ uint32_t warpTyped(const SnapDiffArgs& a,
+                                              const FbMergeRegionDev& reg,
+                                              uint64_t pBeg,
+                                              uint64_t pEnd,
+                                              uint64_t rEnd,
+                                              int lane,
+                                              uint32_t& pageAny)
+{
+    const uint32_t sz =
+      (reg.dataType == FB_SNAP_INT || reg.dataType == FB_SNAP_FLOAT) ? 4 : 8;
+    const uint64_t first = pBeg > reg.offset ? (pBeg - reg.offset + sz - 1) / sz : 0;
+    const uint64_t count = (rEnd - reg.offset) / sz;
+    uint32_t bytes = 0;
+    for (uint64_t k = first + lane; k < count; k += 32) {
+        const uint64_t off = reg.offset + k * sz;
+        if (off >= pEnd) {
+            break;
+        }
+        const uint64_t lastPage = (off + sz - 1) / PAGE;
+        if (!pageDirty(a, off / PAGE) && !pageDirty(a, lastPage)) {
+            continue;
+        }
+        bool d = false;
+        switch (reg.dataType) {
+            case FB_SNAP_INT:
+                d = mergeScalar<int32_t>(a, off, reg.op);
+                break;
+            case FB_SNAP_LONG:
+                d = mergeScalar<int64_t>(a, off, reg.op);
+                break;
+            case FB_SNAP_FLOAT:
+                d = mergeScalar<float>(a, off, reg.op);
+                break;
+            case FB_SNAP_DOUBLE:
+                d = mergeScalar<double>(a, off, reg.op);
+                break;
+            default:
+                break;
+        }
+        if (d) {
+            bytes += sz;
+            // the first page is stamped with the page's other diffs
+            if (a.pageStampOut != nullptr && lastPage != off / PAGE) {
+                a.pageStampOut[lastPage] = a.pageStamp;
+            }
+        }
+    }
+    pageAny |= bytes;
+    return bytes;
+}
+
 // ----------------------------------------------------------------------------
 // The fused kernel
 // ----------------------------------------------------------------------------
@@ -501,9 +643,13 @@ __global__ void __launch_bounds__(512, 2) snapshotDiffPushKernel(
     uint32_t diffBytes = 0;
     uint32_t dirtyPagesSeen = 0;
 
-    // ---- phase 1: Bytewise / XOR regions, page-major, one warp per page ----
+    // ---- page-major, one warp per page: Bytewise / XOR segments of the page
+    // and the typed scalars that start in it, so every diff that starts in a
+    // page is seen by one warp and the page is counted once ----
     for (uint64_t page = warpId; page < nPages; page += nWarps) {
-        if (!pageDirty(a, page)) {
+        const bool dirty = pageDirty(a, page);
+        // a scalar starting on a clean page is merged when its last page is dirty
+        if (!dirty && !(a.nTyped > 0 && page + 1 < nPages && pageDirty(a, page + 1))) {
             continue;
         }
         const uint64_t pBeg = page * PAGE;
@@ -521,11 +667,17 @@ __global__ void __launch_bounds__(512, 2) snapshotDiffPushKernel(
             const uint64_t sEnd = min(pEnd, rEnd);
             if (sBeg < sEnd) {
                 if (reg.op == FB_MERGE_BYTEWISE) {
-                    diffBytes +=
-                      warpSegment<false>(a, sBeg, sEnd, lane, pageAny);
+                    if (dirty) {
+                        diffBytes +=
+                          warpSegment<false>(a, sBeg, sEnd, lane, pageAny);
+                    }
                 } else if (reg.op == FB_MERGE_XOR) {
-                    diffBytes +=
-                      warpSegment<true>(a, sBeg, sEnd, lane, pageAny);
+                    if (dirty) {
+                        diffBytes +=
+                          warpSegment<true>(a, sBeg, sEnd, lane, pageAny);
+                    }
+                } else if (reg.op != FB_MERGE_IGNORE) {
+                    diffBytes += warpTyped(a, reg, pBeg, pEnd, rEnd, lane, pageAny);
                 }
             }
             r++;
@@ -537,56 +689,6 @@ __global__ void __launch_bounds__(512, 2) snapshotDiffPushKernel(
             }
             if (a.pageStampOut != nullptr) {
                 a.pageStampOut[page] = a.pageStamp; // same value from every writer
-            }
-        }
-    }
-
-    // ---- phase 2: typed regions, one thread per scalar ----
-    if (a.nTyped > 0) {
-        const uint64_t tid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-        const uint64_t nThreads = (uint64_t)gridDim.x * blockDim.x;
-        for (int t = 0; t < a.nTyped; t++) {
-            const FbMergeRegionDev reg = a.regions[a.typedIdx[t]];
-            const uint64_t rEnd =
-              reg.length == 0 ? a.size : min(a.size, reg.offset + reg.length);
-            uint32_t sz = (reg.dataType == FB_SNAP_INT ||
-                           reg.dataType == FB_SNAP_FLOAT)
-                            ? 4
-                            : 8;
-            if (reg.offset >= a.size) {
-                continue;
-            }
-            const uint64_t count = (rEnd - reg.offset) / sz;
-            for (uint64_t k = tid; k < count; k += nThreads) {
-                const uint64_t off = reg.offset + k * sz;
-                if (!pageDirty(a, off / PAGE) &&
-                    !pageDirty(a, (off + sz - 1) / PAGE)) {
-                    continue;
-                }
-                bool d = false;
-                switch (reg.dataType) {
-                    case FB_SNAP_INT:
-                        d = mergeScalar<int32_t>(a, off, reg.op);
-                        break;
-                    case FB_SNAP_LONG:
-                        d = mergeScalar<int64_t>(a, off, reg.op);
-                        break;
-                    case FB_SNAP_FLOAT:
-                        d = mergeScalar<float>(a, off, reg.op);
-                        break;
-                    case FB_SNAP_DOUBLE:
-                        d = mergeScalar<double>(a, off, reg.op);
-                        break;
-                    default:
-                        break;
-                }
-                if (d) {
-                    diffBytes += sz;
-                    if (a.pageStampOut != nullptr) {
-                        a.pageStampOut[off / PAGE] = a.pageStamp;
-                        a.pageStampOut[(off + sz - 1) / PAGE] = a.pageStamp;
-                    }
-                }
             }
         }
     }
@@ -999,15 +1101,15 @@ __global__ void __launch_bounds__(256) snapshotApplyKernel(
         T v = loadUnaligned<T>(q);                                             \
         T r = c;                                                               \
         if (d.op == FB_MERGE_SUM)                                              \
-            r = (T)(c + v);                                                    \
+            r = snapAdd(c, v);                                                 \
         else if (d.op == FB_MERGE_SUBTRACT)                                    \
-            r = (T)(c - v);                                                    \
+            r = snapSub(c, v);                                                 \
         else if (d.op == FB_MERGE_PRODUCT)                                     \
-            r = (T)(c * v);                                                    \
+            r = snapMul(c, v);                                                 \
         else if (d.op == FB_MERGE_MAX)                                         \
-            r = c > v ? c : v;                                                 \
+            r = snapMax(c, v);                                                 \
         else if (d.op == FB_MERGE_MIN)                                         \
-            r = c < v ? c : v;                                                 \
+            r = snapMin(c, v);                                                 \
         storeUnaligned<T>(p, r);                                               \
     }
                     if (d.dataType == FB_SNAP_INT)

@@ -1,5 +1,6 @@
 // SnapshotRegistry, SnapshotClient, SnapshotServer, DeviceSnapshot
 #include <filesystem>
+#include <faabric/device/communicator.h>
 #include <faabric/scheduler/Scheduler.h>
 #include <faabric/snapshot/DeviceSnapshot.h>
 #include <faabric/snapshot/SnapshotClient.h>
@@ -876,6 +877,9 @@ void DeviceSnapshot::uploadRegions()
     std::vector<int32_t> typed(cap);
     int nTyped = 0;
     int n = fb_snapshot_prepare_regions(in.data(), (int)in.size(), fillOp, size, out.data(), cap, typed.data(), &nTyped);
+    if (n == FB_E_INVALID) {
+        throw std::runtime_error("Overlapping merge regions");
+    }
     if (n < 0) {
         throw std::runtime_error("Too many merge regions");
     }

@@ -1,5 +1,6 @@
 #include <faabric/util/config.h>
 #include <faabric/util/logging.h>
+#include <faabric/util/reduce_ops.h>
 #include <faabric/util/snapshot.h>
 #include <faabric/util/timing.h>
 
@@ -56,6 +57,9 @@ std::vector<uint8_t> SnapshotDiff::getDataCopy() const
 // ---------------------------------------------------------------------------
 // Typed values
 // ---------------------------------------------------------------------------
+// The merge rules are those of faabric/util/reduce_ops.h: integers wrap,
+// float Max/Min ignore a NaN operand and order -0 below +0.  "Unchanged" is a
+// value comparison, so a NaN always counts as a change and ±0 never does.
 template<typename T>
 bool calculateDiffValue(const uint8_t* original,
                         uint8_t* updated,
@@ -69,13 +73,13 @@ bool calculateDiffValue(const uint8_t* original,
     T toSend = newValue;
     switch (operation) {
         case SnapshotMergeOperation::Sum:
-            toSend = newValue - oldValue;
+            toSend = reduceSub(newValue, oldValue);
             break;
         case SnapshotMergeOperation::Subtract:
-            toSend = oldValue - newValue;
+            toSend = reduceSub(oldValue, newValue);
             break;
         case SnapshotMergeOperation::Product:
-            toSend = newValue / oldValue;
+            toSend = snapshotQuotient(newValue, oldValue);
             break;
         case SnapshotMergeOperation::Max:
         case SnapshotMergeOperation::Min:
@@ -97,15 +101,15 @@ T applyDiffValue(const uint8_t* original,
     T current = unalignedRead<T>(original);
     switch (operation) {
         case SnapshotMergeOperation::Sum:
-            return current + diffValue;
+            return reduceSum(current, diffValue);
         case SnapshotMergeOperation::Subtract:
-            return current - diffValue;
+            return reduceSub(current, diffValue);
         case SnapshotMergeOperation::Product:
-            return current * diffValue;
+            return reduceProd(current, diffValue);
         case SnapshotMergeOperation::Max:
-            return std::max<T>(current, diffValue);
+            return reduceMax(current, diffValue);
         case SnapshotMergeOperation::Min:
-            return std::min<T>(current, diffValue);
+            return reduceMin(current, diffValue);
         default:
             SPDLOG_ERROR("Can't apply merge operation: {}", (int)operation);
             throw std::runtime_error("Can't apply merge operation");
@@ -187,11 +191,12 @@ void SnapshotMergeRegion::addDiffs(std::vector<SnapshotDiff>& diffs,
     if (operation == SnapshotMergeOperation::Ignore) {
         return;
     }
-    if (offset > originalData.size()) {
-        return; // region lies beyond the original image
+    const uint64_t dataEnd = std::min(originalData.size(), updatedData.size());
+    if (offset > dataEnd) {
+        return; // region lies beyond the image or the memory
     }
-    uint64_t regionEnd = length > 0 ? offset + length : originalData.size();
-    regionEnd = std::min<uint64_t>(regionEnd, originalData.size());
+    uint64_t regionEnd = length > 0 ? offset + length : dataEnd;
+    regionEnd = std::min<uint64_t>(regionEnd, dataEnd);
 
     size_t firstPage = getRequiredHostPagesRoundDown(offset);
     size_t lastPage = getRequiredHostPages(regionEnd); // exclusive
@@ -249,22 +254,19 @@ void SnapshotMergeRegion::addDiffs(std::vector<SnapshotDiff>& diffs,
         return;
     }
 
-    // Typed scalar
-    uint8_t* updated = updatedData.data() + offset;
-    const uint8_t* original = originalData.data() + offset;
-    bool changed = false;
+    // Typed regions are arrays of floor(length / sizeof(T)) scalars, one diff
+    // per changed scalar.  A scalar is diffed when its first or its last page
+    // is dirty; trailing bytes and a scalar that would pass the end of the
+    // data produce nothing.
+    uint64_t sz = 0;
     switch (dataType) {
         case SnapshotDataType::Int:
-            changed = calculateDiffValue<int32_t>(original, updated, operation);
+        case SnapshotDataType::Float:
+            sz = 4;
             break;
         case SnapshotDataType::Long:
-            changed = calculateDiffValue<long>(original, updated, operation);
-            break;
-        case SnapshotDataType::Float:
-            changed = calculateDiffValue<float>(original, updated, operation);
-            break;
         case SnapshotDataType::Double:
-            changed = calculateDiffValue<double>(original, updated, operation);
+            sz = 8;
             break;
         default:
             SPDLOG_ERROR("Unsupported merge op combination {} {}",
@@ -272,11 +274,34 @@ void SnapshotMergeRegion::addDiffs(std::vector<SnapshotDiff>& diffs,
                          snapshotMergeOpStr(operation));
             throw std::runtime_error("Unsupported merge op combination");
     }
-    if (changed) {
-        diffs.emplace_back(dataType,
-                           operation,
-                           offset,
-                           std::span<const uint8_t>(updated, (size_t)length));
+    auto pageDirty = [&](uint64_t byte) {
+        size_t p = getRequiredHostPagesRoundDown(byte);
+        return p < dirtyRegions.size() && dirtyRegions[p] != 0;
+    };
+    for (uint64_t off = offset; off + sz <= regionEnd; off += sz) {
+        if (!pageDirty(off) && !pageDirty(off + sz - 1)) {
+            continue;
+        }
+        uint8_t* updated = updatedData.data() + off;
+        const uint8_t* original = originalData.data() + off;
+        bool changed = false;
+        switch (dataType) {
+            case SnapshotDataType::Int:
+                changed = calculateDiffValue<int32_t>(original, updated, operation);
+                break;
+            case SnapshotDataType::Long:
+                changed = calculateDiffValue<long>(original, updated, operation);
+                break;
+            case SnapshotDataType::Float:
+                changed = calculateDiffValue<float>(original, updated, operation);
+                break;
+            default:
+                changed = calculateDiffValue<double>(original, updated, operation);
+                break;
+        }
+        if (changed) {
+            diffs.emplace_back(dataType, operation, off, std::span<const uint8_t>(updated, (size_t)sz));
+        }
     }
 }
 
@@ -464,6 +489,12 @@ void SnapshotData::fillGapsWithBytewiseRegions()
     uint64_t cursor = 0;
     bool reachesEnd = false;
     for (const auto& r : mergeRegions) {
+        // Each byte has one merge operation: overlapping regions, or a region
+        // after one that runs to the end, are refused
+        if (reachesEnd || r.offset < cursor) {
+            SPDLOG_ERROR("Merge region at {} (length {}) overlaps another", r.offset, r.length);
+            throw std::runtime_error("Overlapping merge regions");
+        }
         if (r.offset > cursor) {
             filled.emplace_back(cursor, r.offset - cursor, SnapshotDataType::Raw, fillOp);
         }
@@ -538,29 +569,35 @@ void SnapshotData::applyDiffLocked(const SnapshotDiff& diff)
         xorData(diff.getData(), diff.getOffset());
         return;
     }
-    uint8_t* current = validatedOffsetPtr(diff.getOffset());
+    // A typed diff of L bytes holds floor(L / sizeof(T)) scalars; scalars that
+    // would pass the end of the image are not applied
+    const uint64_t offset = diff.getOffset();
+    uint8_t* current = validatedOffsetPtr(offset);
     const uint8_t* value = diff.getData().data();
+    const uint64_t len = std::min<uint64_t>(diff.getData().size(), size - offset);
+    auto applyAll = [&]<typename T>() {
+        const uint64_t n = len / sizeof(T);
+        for (uint64_t k = 0; k < n; k++) {
+            T v = applyDiffValue<T>(current + k * sizeof(T), value + k * sizeof(T), diff.getOperation());
+            unalignedWrite<T>(v, current + k * sizeof(T));
+        }
+        if (n > 0) {
+            trackedChanges.emplace_back(offset, offset + n * sizeof(T));
+        }
+    };
     switch (diff.getDataType()) {
-        case SnapshotDataType::Int: {
-            int32_t v = applyDiffValue<int32_t>(current, value, diff.getOperation());
-            writeData(std::span<const uint8_t>(reinterpret_cast<const uint8_t*>(&v), sizeof(v)), diff.getOffset());
+        case SnapshotDataType::Int:
+            applyAll.template operator()<int32_t>();
             break;
-        }
-        case SnapshotDataType::Long: {
-            long v = applyDiffValue<long>(current, value, diff.getOperation());
-            writeData(std::span<const uint8_t>(reinterpret_cast<const uint8_t*>(&v), sizeof(v)), diff.getOffset());
+        case SnapshotDataType::Long:
+            applyAll.template operator()<long>();
             break;
-        }
-        case SnapshotDataType::Float: {
-            float v = applyDiffValue<float>(current, value, diff.getOperation());
-            writeData(std::span<const uint8_t>(reinterpret_cast<const uint8_t*>(&v), sizeof(v)), diff.getOffset());
+        case SnapshotDataType::Float:
+            applyAll.template operator()<float>();
             break;
-        }
-        case SnapshotDataType::Double: {
-            double v = applyDiffValue<double>(current, value, diff.getOperation());
-            writeData(std::span<const uint8_t>(reinterpret_cast<const uint8_t*>(&v), sizeof(v)), diff.getOffset());
+        case SnapshotDataType::Double:
+            applyAll.template operator()<double>();
             break;
-        }
         default:
             SPDLOG_ERROR("Unsupported data type for merge: {} {}",
                          snapshotDataTypeStr(diff.getDataType()),

@@ -1,8 +1,34 @@
 """Device snapshot ops: fused diff + merge-op + push, dirty-page detection,
 chunk-run extraction and diff application (csrc/kernels/snapshot_kernels.cu).
 
-Semantics follow the reference's SnapshotData / SnapshotMergeRegion
-(src/util/snapshot.cpp) — enum values are ABI-identical.
+Semantics follow SnapshotData / SnapshotMergeRegion (csrc/src/util/snapshot.cpp),
+the host implementation; enum values are ABI-identical.  Typed merges use the
+rules of faabric/util/reduce_ops.h on both sides:
+
+* a typed region is an array of ``length // size`` scalars; trailing bytes and
+  a scalar that would pass the image end produce nothing.  A scalar is merged
+  when its first or its last 4 KiB page is dirty;
+* a scalar is unchanged when ``new == old`` as values: a NaN always counts as
+  a change, +0 and -0 never do;
+* integer Sum / Subtract / Product wrap (two's complement);
+* the Product factor is ``new / old``: IEEE for floats (±inf or NaN when old
+  is 0); for integers 0 when old is 0, a wrapping negation when old is -1,
+  otherwise truncated;
+* float Max / Min ignore a NaN operand and order -0 below +0, so the merged
+  value does not depend on which writer lands first;
+* regions may not overlap, and no region may follow one that runs to the end
+  (length 0): ``prepare_regions`` raises ``ValueError``;
+* ``pages_with_diffs`` (``stats[1]``) and ``page_flags_out`` count the pages
+  in which a diff starts: a changed Bytewise / XOR byte, or the first byte of
+  a typed scalar that produced a diff.
+
+Concurrent writers into one image agree bit for bit for order-independent
+operations.  A scalar that straddles a 16-byte boundary is merged by a plain
+load / modify / store, so there the last writer wins.
+
+Every launch checks its tensors first: ``diff_push`` and ``dirty_scan`` need
+16-byte aligned, contiguous images, and every flag, page or destination
+buffer must cover the image.
 """
 
 from __future__ import annotations
@@ -42,6 +68,28 @@ class PreparedRegions:
     host: list
 
 
+def _nbytes(t: torch.Tensor) -> int:
+    return t.numel() * t.element_size()
+
+
+def _check_image(name: str, t: torch.Tensor) -> None:
+    # the kernels use 16-byte vector loads / stores and 32-bit atomics on
+    # offsets relative to the image start
+    if not t.is_contiguous():
+        raise ValueError(f"{name} must be contiguous")
+    if t.data_ptr() % 16 != 0:
+        raise ValueError(f"{name} must be 16-byte aligned (address {t.data_ptr():#x})")
+
+
+def _check_covers(name: str, t: Optional[torch.Tensor], nbytes: int) -> None:
+    if t is None:
+        return
+    if not t.is_contiguous():
+        raise ValueError(f"{name} must be contiguous")
+    if _nbytes(t) < nbytes:
+        raise ValueError(f"{name} has {_nbytes(t)} bytes, needs {nbytes}")
+
+
 def _stream(device, stream):
     if stream is None:
         stream = torch.cuda.current_stream(device)
@@ -65,6 +113,8 @@ def prepare_regions(
     n = lib.fb_snapshot_prepare_regions(
         arr, n_in, fill_op, size, out, cap, typed, C.byref(n_typed)
     )
+    if n == -2:  # FB_E_INVALID
+        raise ValueError("overlapping merge regions, or a region after one that runs to the end")
     if n < 0:
         raise RuntimeError("too many merge regions")
     raw = bytes(out)[: n * C.sizeof(FbMergeRegion)]
@@ -92,12 +142,26 @@ def diff_push(
     ``[diff_bytes, pages_with_diffs]`` (uint64 as int64, on device; accumulates)."""
     lib = _lib.load()
     dev = mem.device
-    size = min(mem.numel() * mem.element_size(), orig.numel() * orig.element_size())
+    size = min(_nbytes(mem), _nbytes(orig))
+    n_pages = (size + PAGE - 1) // PAGE
+    _check_image("mem", mem)
+    _check_image("orig", orig)
+    if isinstance(dst, int):
+        if dst % 16 != 0:
+            raise ValueError(f"dst must be 16-byte aligned (address {dst:#x})")
+        dst_ptr = dst
+    else:
+        _check_image("dst", dst)
+        _check_covers("dst", dst, size)
+        dst_ptr = dst.data_ptr()
+    _check_covers("dirty_pages", dirty_pages, n_pages)
+    _check_covers("page_flags_out", page_flags_out, n_pages)
+    _check_covers("chunk_flags", chunk_flags, (size + CHUNK - 1) // CHUNK)
+    _check_covers("stats", stats, 16)
     if regions is None:
         regions = prepare_regions([], size, dev)
     if stats is None:
         stats = torch.zeros(2, dtype=torch.int64, device=dev)
-    dst_ptr = dst if isinstance(dst, int) else dst.data_ptr()
     rc = lib.fb_snapshot_diff_push(
         C.c_void_p(mem.data_ptr()),
         C.c_void_p(orig.data_ptr()),
@@ -125,7 +189,9 @@ def dirty_scan(mem: torch.Tensor, base: torch.Tensor, stream=None):
     count int64[1])."""
     lib = _lib.load()
     dev = mem.device
-    size = min(mem.numel() * mem.element_size(), base.numel() * base.element_size())
+    _check_image("mem", mem)
+    _check_image("base", base)
+    size = min(_nbytes(mem), _nbytes(base))
     n_pages = (size + PAGE - 1) // PAGE
     flags = torch.empty(n_pages, dtype=torch.uint8, device=dev)
     count = torch.zeros(1, dtype=torch.int64, device=dev)
@@ -157,9 +223,11 @@ def flags_or(dst: torch.Tensor, src: torch.Tensor, stream=None):
 
 
 def chunk_runs(chunk_flags: torch.Tensor, total_bytes: int, chunk_bytes: int = CHUNK, max_out: int = 1 << 20, stream=None):
-    """Chunk flags -> sorted list of (offset, length) runs."""
+    """Chunk flags -> sorted list of (offset, length) runs.  Raises
+    ``RuntimeError`` when there are more than ``max_out`` runs."""
     lib = _lib.load()
     dev = chunk_flags.device
+    _check_covers("chunk_flags", chunk_flags, 0)
     out = torch.empty(max_out * C.sizeof(FbDiffDesc), dtype=torch.uint8, device=dev)
     count = torch.zeros(1, dtype=torch.int32, device=dev)
     rc = lib.fb_chunk_runs(
@@ -174,7 +242,9 @@ def chunk_runs(chunk_flags: torch.Tensor, total_bytes: int, chunk_bytes: int = C
     )
     if rc != 0:
         raise RuntimeError("fb_chunk_runs failed")
-    n = min(int(count.item()), max_out)
+    n = int(count.item())
+    if n > max_out:
+        raise RuntimeError(f"{n} chunk runs do not fit max_out={max_out}")
     raw = out[: n * C.sizeof(FbDiffDesc)].cpu().numpy().tobytes()
     descs = (FbDiffDesc * n).from_buffer_copy(raw) if n else []
     return sorted((d.offset, d.length) for d in descs)
@@ -182,9 +252,11 @@ def chunk_runs(chunk_flags: torch.Tensor, total_bytes: int, chunk_bytes: int = C
 
 def apply_diffs(image: torch.Tensor, diffs: Sequence[tuple], stream=None):
     """Apply [(offset, data_type, op, bytes-like / uint8 tensor)] to a device
-    image (SnapshotData::applyDiffs)."""
+    image (SnapshotData::applyDiffs).  A typed diff of L bytes holds L // size
+    scalars."""
     lib = _lib.load()
     dev = image.device
+    _check_covers("image", image, 0)
     n = len(diffs)
     if n == 0:
         return image
