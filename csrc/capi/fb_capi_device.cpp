@@ -612,6 +612,33 @@ int fb_wait_signal(void* h, int signalIdx, uint32_t count, void* stream)
     return COMM(h)->waitSignal(signalIdx, count, (cudaStream_t)stream);
 }
 
+// One-sided atomics on peer's copy of the symmetric heap (Communicator::
+// accumulate / compareAndSwap); `fetchOut` null means no fetch
+int fb_accumulate(void* h,
+                  const void* origin,
+                  uint64_t dstOffset,
+                  uint64_t count,
+                  int dtype,
+                  int op,
+                  int peer,
+                  void* fetchOut,
+                  void* stream)
+{
+    return COMM(h)->accumulate(origin, dstOffset, count, dtype, op, peer, fetchOut, (cudaStream_t)stream);
+}
+
+int fb_compare_and_swap(void* h,
+                        const void* compare,
+                        const void* swap,
+                        void* result,
+                        uint64_t dstOffset,
+                        int dtype,
+                        int peer,
+                        void* stream)
+{
+    return COMM(h)->compareAndSwap(compare, swap, result, dstOffset, dtype, peer, (cudaStream_t)stream);
+}
+
 const char* fb_error_string(int code)
 {
     return Communicator::errorString(code);

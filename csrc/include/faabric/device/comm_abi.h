@@ -122,7 +122,12 @@ typedef enum FbOp {
     FB_OP_MINLOC = 9,
     FB_OP_LXOR = 10,
     FB_OP_BXOR = 11,
-    FB_OP_COUNT = 12
+    FB_OP_COUNT = 12,
+    // One-sided accumulate only (MPI_REPLACE, MPI_NO_OP), outside
+    // [0, FB_OP_COUNT): no collective accepts them.  NO_OP is an atomic read
+    // and needs a fetch buffer.
+    FB_OP_REPLACE = 32,
+    FB_OP_NO_OP = 33
 } FbOp;
 
 typedef enum FbAlgo {

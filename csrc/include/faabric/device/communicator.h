@@ -277,6 +277,33 @@ class Communicator
                   int blocks,
                   cudaStream_t s);
     int waitSignal(int signalIdx, uint32_t count, cudaStream_t s);
+    // ---- one-sided atomics (MPI_Accumulate family) on a peer's symmetric heap.
+    // Stream-ordered, never synchronise the host; `peer == rank()` is allowed.
+    // The target is `count` elements at `dstOffset` in the user part of peer's
+    // heap, each aligned to its size; origin and fetch buffers are device-
+    // accessible and need no alignment.  Each target element is updated
+    // atomically with respect to every other accumulate / compare-and-swap on
+    // any rank.  `op` is any reduction pair of allReduce, FB_OP_REPLACE, or
+    // FB_OP_NO_OP (an atomic read; needs `fetchOut`).  `fetchOut` (null: no
+    // fetch) receives every element's previous value.  FB_E_UNSUPPORTED for
+    // an unsupported pair, FB_E_INVALID for a range outside the heap, a
+    // misaligned target or NO_OP without `fetchOut`.
+    int accumulate(const void* origin,
+                   uint64_t dstOffset,
+                   size_t count,
+                   int dtype,
+                   int op,
+                   int peer,
+                   void* fetchOut,
+                   cudaStream_t s);
+    // One integer element: *result = old; if (old == *compare) target = *swap
+    int compareAndSwap(const void* compare,
+                       const void* swap,
+                       void* result,
+                       uint64_t dstOffset,
+                       int dtype,
+                       int peer,
+                       cudaStream_t s);
 
     // Device watchdog error word (FB_ERR_*); synchronises `s`
     uint32_t checkError(cudaStream_t s);
@@ -381,6 +408,7 @@ class Communicator
     int launchGroup(const GroupLaunch& l, int dtype, int op, int flags, cudaStream_t s);
     int streamWaitGe(cudaStream_t s, const uint32_t* localWord, uint32_t value);
     int streamBarrier(int flags, cudaStream_t s);
+    bool rmaTargetOk(uint64_t dstOffset, uint64_t bytes, size_t align, int peer) const;
     int sendChunk(const uint8_t* buf, size_t len, int peer, cudaStream_t s);
     int recvChunk(uint8_t* buf, size_t len, int peer, cudaStream_t s);
     void abortPendingWaits();

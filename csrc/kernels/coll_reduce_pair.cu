@@ -75,6 +75,9 @@ cudaError_t preloadAllKernels()
     if (e == cudaSuccess) {
         e = preloadSnapshotKernels();
     }
+    if (e == cudaSuccess) {
+        e = preloadRmaKernels();
+    }
     return e;
 }
 

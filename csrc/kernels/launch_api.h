@@ -203,6 +203,47 @@ cudaError_t launchWaitSignal(const FbCommDev& c,
                              cudaStream_t s);
 
 
+// ------------------------------------------------------------------- rma ----
+// One-sided atomics on heap[peer] + dstOff (rma_kernels.cu).  Every target
+// element is updated atomically with respect to every other RMA kernel on any
+// GPU.  Every target element must be aligned to its size (fbDtypeSize: 8 for
+// the 8-byte pairs, 16 for the 16-byte pairs); origin and result buffers need
+// no alignment.  No kernel waits on a peer or takes part in a barrier.
+struct RmaArgs
+{
+    FbCommDev comm;
+    const uint8_t* origin; // count elements (unused for NO_OP)
+    uint8_t* result;       // previous values, or null (no fetch)
+    uint64_t dstOff;
+    uint64_t count;
+    int32_t peer;
+    int32_t pad;
+};
+
+struct RmaCasArgs
+{
+    FbCommDev comm;
+    const uint8_t* compare; // one element each
+    const uint8_t* swap;
+    uint8_t* result;
+    uint64_t dstOff;
+    int32_t peer;
+    int32_t pad;
+};
+
+// (dtype, op) pairs the accumulate kernels implement: every device reduction
+// pair, REPLACE for every dtype, and NO_OP for every dtype when fetching
+bool rmaSupported(int dtype, int op, bool fetch);
+// compare-and-swap: the eight integer dtypes
+bool rmaCasSupported(int dtype);
+// target[i] = op(target[i], origin[i]); a.result[i] = previous target[i] when
+// a.result is not null
+cudaError_t launchRmaAccumulate(const RmaArgs& a, int dtype, int op, cudaStream_t s);
+// result = target; if (target == compare) target = swap
+cudaError_t launchRmaCompareSwap(const RmaCasArgs& a, int dtype, cudaStream_t s);
+cudaError_t preloadRmaKernels();
+
+
 // ------------------------------------------------------------------ nvls ----
 enum NvlsMode
 {

@@ -24,6 +24,8 @@
 // the rules of faabric/util/reduce_ops.h (see snapAdd ... snapQuotient).
 #include "snapshot_kernels.cuh"
 
+#include "fb_atomics.cuh"
+
 #include <type_traits>
 
 namespace fb {
@@ -43,12 +45,6 @@ __device__ __forceinline__ uint32_t byteDiffMask(uint32_t a, uint32_t b)
     m |= (x & 0x00ff0000u) ? 4u : 0u;
     m |= (x & 0xff000000u) ? 8u : 0u;
     return m;
-}
-
-__device__ __forceinline__ void redXorSys(uint32_t* p, uint32_t v)
-{
-    asm volatile("red.relaxed.sys.global.xor.b32 [%0], %1;" ::"l"(p), "r"(v)
-                 : "memory");
 }
 
 // Store only the differing bytes of word `m` (mask from byteDiffMask)
@@ -250,104 +246,6 @@ __device__ __forceinline__ void storeUnaligned(uint8_t* p, T v)
     for (int i = 0; i < (int)sizeof(T); i++) {
         p[i] = b[i];
     }
-}
-
-template<typename T>
-struct AtomicWord;
-template<>
-struct AtomicWord<int32_t>
-{
-    using W = int;
-};
-template<>
-struct AtomicWord<float>
-{
-    using W = int;
-};
-template<>
-struct AtomicWord<int64_t>
-{
-    using W = unsigned long long;
-};
-template<>
-struct AtomicWord<double>
-{
-    using W = unsigned long long;
-};
-
-// Generic CAS-based atomic RMW at system scope (works on peer memory)
-template<typename T, typename F>
-__device__ __forceinline__ void atomicRmwSys(T* addr, F f)
-{
-    using W = typename AtomicWord<T>::W;
-    W* wa = reinterpret_cast<W*>(addr);
-    W old = *reinterpret_cast<volatile W*>(wa);
-    while (true) {
-        T cur;
-        memcpy(&cur, &old, sizeof(T));
-        T nv = f(cur);
-        W nw;
-        memcpy(&nw, &nv, sizeof(T));
-        W prev = atomicCAS_system(wa, old, nw);
-        if (prev == old) {
-            return;
-        }
-        old = prev;
-    }
-}
-
-// Native system-scope reductions where the ISA has them (integers): one
-// fire-and-forget red.* instead of a CAS round trip over NVLink
-__device__ __forceinline__ void redAddSys(int32_t* p, int32_t v)
-{
-    asm volatile("red.relaxed.sys.global.add.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ void redAddSys(int64_t* p, int64_t v)
-{
-    asm volatile("red.relaxed.sys.global.add.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-__device__ __forceinline__ void redMaxSys(int32_t* p, int32_t v)
-{
-    asm volatile("red.relaxed.sys.global.max.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ void redMaxSys(int64_t* p, int64_t v)
-{
-    asm volatile("red.relaxed.sys.global.max.s64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-__device__ __forceinline__ void redMinSys(int32_t* p, int32_t v)
-{
-    asm volatile("red.relaxed.sys.global.min.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-__device__ __forceinline__ void redMinSys(int64_t* p, int64_t v)
-{
-    asm volatile("red.relaxed.sys.global.min.s64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
-}
-// (the hardware f32 add flushes subnormals to zero; the host merge of the
-// reference does not, so float sums keep the exact CAS loop)
-__device__ __forceinline__ void redAddSys(float* p, float v)
-{
-    atomicRmwSys<float>(p, [v](float c) { return c + v; });
-}
-__device__ __forceinline__ void redAddSys(double* p, double v)
-{
-    asm volatile("red.relaxed.sys.global.add.f64 [%0], %1;" ::"l"(p), "d"(v) : "memory");
-}
-
-__device__ __forceinline__ bool cas128Sys(void* p,
-                                          uint64_t c0,
-                                          uint64_t c1,
-                                          uint64_t n0,
-                                          uint64_t n1,
-                                          uint64_t& r0,
-                                          uint64_t& r1)
-{
-    asm volatile("{\n\t.reg .b128 c, n, r;\n\tmov.b128 c, {%2, %3};\n\tmov.b128 n, "
-                 "{%4, %5};\n\tatom.relaxed.sys.global.cas.b128 r, [%6], c, n;\n\tmov.b128 "
-                 "{%0, %1}, r;\n\t}"
-                 : "=l"(r0), "=l"(r1)
-                 : "l"(c0), "l"(c1), "l"(n0), "l"(n1), "l"(p)
-                 : "memory");
-    return r0 == c0 && r1 == c1;
 }
 
 // RMW of a scalar that is NOT naturally aligned (an application may declare a

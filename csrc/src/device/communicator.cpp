@@ -1125,6 +1125,8 @@ const fb::KernelTable CUDA_KERNELS = {
     .waitSignal = fb::launchWaitSignal,
     .waitWord = fb::launchWaitWord,
     .signalPeers = fb::launchSignalPeers,
+    .rmaAccumulate = fb::launchRmaAccumulate,
+    .rmaCompareSwap = fb::launchRmaCompareSwap,
     .copy = cudaCopy,
     .copy2D = cudaCopy2D,
 };
@@ -1142,6 +1144,8 @@ const fb::KernelTable HOST_KERNELS = {
     .waitSignal = fb::host::waitSignal,
     .waitWord = fb::host::waitWord,
     .signalPeers = fb::host::signalPeers,
+    .rmaAccumulate = fb::host::rmaAccumulate,
+    .rmaCompareSwap = fb::host::rmaCompareSwap,
     .copy = fb::host::copy,
     .copy2D = fb::host::copy2D,
 };
@@ -2609,6 +2613,81 @@ int Communicator::waitSignal(int signalIdx, uint32_t count, cudaStream_t s)
     }
     stats_.launches++;
     return k_->waitSignal(dev_, signalIdx, count, s) == cudaSuccess ? FB_OK : FB_E_CUDA;
+}
+
+bool Communicator::rmaTargetOk(uint64_t dstOffset, uint64_t bytes, size_t align, int peer) const
+{
+    return dstOffset >= userOff_ && dstOffset <= heapTotal_ && bytes <= heapTotal_ - dstOffset &&
+           (uintptr_t)(dev_.heap[peer] + dstOffset) % align == 0;
+}
+
+int Communicator::accumulate(const void* origin,
+                             uint64_t dstOffset,
+                             size_t count,
+                             int dtype,
+                             int op,
+                             int peer,
+                             void* fetchOut,
+                             cudaStream_t s)
+{
+    const size_t esize = fbDtypeSize(dtype);
+    if (esize == 0 || peer < 0 || peer >= dev_.nranks) {
+        return FB_E_INVALID;
+    }
+    if (!fb::rmaSupported(dtype, op, true)) {
+        return FB_E_UNSUPPORTED;
+    }
+    if ((op == FB_OP_NO_OP && fetchOut == nullptr) || (op != FB_OP_NO_OP && origin == nullptr && count > 0) ||
+        count > heapTotal_ / esize || !rmaTargetOk(dstOffset, (uint64_t)count * esize, esize, peer)) {
+        return FB_E_INVALID;
+    }
+    if (count == 0) {
+        return FB_OK;
+    }
+    bindDevice();
+    fb::RmaArgs a;
+    memset(&a, 0, sizeof(a));
+    a.comm = dev_;
+    a.origin = (const uint8_t*)origin;
+    a.result = (uint8_t*)fetchOut;
+    a.dstOff = dstOffset;
+    a.count = count;
+    a.peer = peer;
+    stats_.launches++;
+    stats_.bytes += (uint64_t)count * esize;
+    return k_->rmaAccumulate(a, dtype, op, s) == cudaSuccess ? FB_OK : FB_E_CUDA;
+}
+
+int Communicator::compareAndSwap(const void* compare,
+                                 const void* swap,
+                                 void* result,
+                                 uint64_t dstOffset,
+                                 int dtype,
+                                 int peer,
+                                 cudaStream_t s)
+{
+    const size_t esize = fbDtypeSize(dtype);
+    if (esize == 0 || peer < 0 || peer >= dev_.nranks) {
+        return FB_E_INVALID;
+    }
+    if (!fb::rmaCasSupported(dtype)) {
+        return FB_E_UNSUPPORTED;
+    }
+    if (compare == nullptr || swap == nullptr || result == nullptr || !rmaTargetOk(dstOffset, esize, esize, peer)) {
+        return FB_E_INVALID;
+    }
+    bindDevice();
+    fb::RmaCasArgs a;
+    memset(&a, 0, sizeof(a));
+    a.comm = dev_;
+    a.compare = (const uint8_t*)compare;
+    a.swap = (const uint8_t*)swap;
+    a.result = (uint8_t*)result;
+    a.dstOff = dstOffset;
+    a.peer = peer;
+    stats_.launches++;
+    stats_.bytes += esize;
+    return k_->rmaCompareSwap(a, dtype, s) == cudaSuccess ? FB_OK : FB_E_CUDA;
 }
 
 } // namespace faabric::device

@@ -20,6 +20,7 @@
 #include <chrono>
 #include <cmath>
 #include <cstring>
+#include <mutex>
 #include <thread>
 
 namespace fb::host {
@@ -623,6 +624,111 @@ cudaError_t signalPeers(const FbCommDev& c, uint32_t wordOff, uint32_t value, cu
 cudaError_t waitWord(const FbCommDev& c, const uint32_t* word, uint32_t target, cudaStream_t)
 {
     return waitFlagGe(c, word, target, FB_ERR_FLAG_TIMEOUT) ? cudaSuccess : cudaErrorUnknown;
+}
+
+// ------------------------------------------------------------------ rma ----
+// The host twins of rma_kernels.cu.  Every element is one atomic step with
+// respect to the other rank threads: a CAS loop on the enclosing 32-bit word
+// (1, 2 and 4-byte elements) or on the 64-bit element, and a striped lock for
+// 16-byte elements.  The target is naturally aligned (the communicator checks).
+namespace {
+
+// bytes of an element that an update replaces: a 16-byte pair keeps its padding
+size_t rmaKeepBytes(int dtype)
+{
+    return (dtype == FB_F64_I32 || dtype == FB_I64_I32) ? 12 : fbDtypeSize(dtype);
+}
+
+// out = the new value of an element whose current bytes are `cur`
+void rmaCombine(int dtype, int op, const uint8_t* cur, const uint8_t* in, uint8_t* out)
+{
+    const size_t n = fbDtypeSize(dtype);
+    memcpy(out, cur, n);
+    if (op == FB_OP_NO_OP) {
+        return;
+    }
+    uint8_t tmp[16];
+    memcpy(tmp, cur, n);
+    if (op == FB_OP_REPLACE) {
+        memcpy(tmp, in, n);
+    } else {
+        combineElem(dtype, op, tmp, in);
+    }
+    memcpy(out, tmp, rmaKeepBytes(dtype));
+}
+
+std::mutex& rmaStripe(const void* p)
+{
+    static std::mutex stripes[64];
+    return stripes[((uintptr_t)p >> 4) % 64];
+}
+
+// Atomically replaces the n-byte element at p by f(current); `prev` (may be
+// null) receives the value it replaced
+template<typename W, typename F>
+void rmaCasWord(uint8_t* p, size_t n, uint8_t* prev, F f)
+{
+    const uintptr_t addr = (uintptr_t)p;
+    W* wp = reinterpret_cast<W*>(addr & ~(uintptr_t)(sizeof(W) - 1));
+    const size_t shift = addr & (sizeof(W) - 1); // little endian
+    std::atomic_ref<W> ref(*wp);
+    W old = ref.load();
+    while (true) {
+        uint8_t cur[8];
+        uint8_t nv[8];
+        memcpy(cur, (const uint8_t*)&old + shift, n);
+        f(cur, nv);
+        W nw = old;
+        memcpy((uint8_t*)&nw + shift, nv, n);
+        if (nw == old || ref.compare_exchange_weak(old, nw)) {
+            if (prev != nullptr) {
+                memcpy(prev, cur, n);
+            }
+            return;
+        }
+    }
+}
+
+template<typename F>
+void rmaAtomic(uint8_t* p, size_t n, uint8_t* prev, F f)
+{
+    if (n == 16) {
+        std::lock_guard<std::mutex> lk(rmaStripe(p));
+        uint8_t nv[16];
+        f(p, nv);
+        if (prev != nullptr) {
+            memcpy(prev, p, 16);
+        }
+        memcpy(p, nv, 16);
+    } else if (n == 8) {
+        rmaCasWord<uint64_t>(p, n, prev, f);
+    } else {
+        rmaCasWord<uint32_t>(p, n, prev, f);
+    }
+}
+
+} // namespace
+
+cudaError_t rmaAccumulate(const RmaArgs& a, int dtype, int op, cudaStream_t)
+{
+    const size_t n = fbDtypeSize(dtype);
+    uint8_t* tgt = a.comm.heap[a.peer] + a.dstOff;
+    for (uint64_t i = 0; i < a.count; i++) {
+        const uint8_t* in = op == FB_OP_NO_OP ? nullptr : a.origin + i * n;
+        rmaAtomic(tgt + i * n, n, a.result != nullptr ? a.result + i * n : nullptr, [&](const uint8_t* cur, uint8_t* nv) {
+            rmaCombine(dtype, op, cur, in, nv);
+        });
+    }
+    return cudaSuccess;
+}
+
+cudaError_t rmaCompareSwap(const RmaCasArgs& a, int dtype, cudaStream_t)
+{
+    const size_t n = fbDtypeSize(dtype);
+    rmaAtomic(a.comm.heap[a.peer] + a.dstOff, n, a.result, [&](const uint8_t* cur, uint8_t* nv) {
+        memcpy(nv, memcmp(cur, a.compare, n) == 0 ? a.swap : cur, n);
+    });
+    return cudaSuccess;
 }
 
 // ----------------------------------------------------------------- copy ----

@@ -26,6 +26,8 @@ struct KernelTable
     cudaError_t (*waitSignal)(const FbCommDev& c, int signalIdx, uint32_t count, cudaStream_t s);
     cudaError_t (*waitWord)(const FbCommDev& c, const uint32_t* word, uint32_t target, cudaStream_t s);
     cudaError_t (*signalPeers)(const FbCommDev& c, uint32_t wordOff, uint32_t value, cudaStream_t s);
+    cudaError_t (*rmaAccumulate)(const RmaArgs& a, int dtype, int op, cudaStream_t s);
+    cudaError_t (*rmaCompareSwap)(const RmaCasArgs& a, int dtype, cudaStream_t s);
     // device-to-device copies: one range, and `height` rows of `width` bytes
     cudaError_t (*copy)(void* dst, const void* src, size_t bytes, cudaStream_t s);
     cudaError_t (*copy2D)(void* dst,
@@ -55,6 +57,10 @@ cudaError_t putSignal(const PutArgs& a, int width, int blocks, cudaStream_t s);
 cudaError_t waitSignal(const FbCommDev& c, int signalIdx, uint32_t addTarget, cudaStream_t s);
 cudaError_t waitWord(const FbCommDev& c, const uint32_t* word, uint32_t target, cudaStream_t s);
 cudaError_t signalPeers(const FbCommDev& c, uint32_t wordOff, uint32_t value, cudaStream_t s);
+// atomic with respect to the other rank threads: a CAS on the enclosing 32- or
+// 64-bit word, a striped lock for 16-byte elements
+cudaError_t rmaAccumulate(const RmaArgs& a, int dtype, int op, cudaStream_t s);
+cudaError_t rmaCompareSwap(const RmaCasArgs& a, int dtype, cudaStream_t s);
 cudaError_t copy(void* dst, const void* src, size_t bytes, cudaStream_t s);
 cudaError_t copy2D(void* dst, size_t dpitch, const void* src, size_t spitch, size_t width, size_t height, cudaStream_t s);
 

@@ -124,6 +124,8 @@ def load():
     _sig(lib, "fb_allreduce_many", i32, [vp, i32, vpp, vpp, u64p, i32, i32, i32, vp])
     _sig(lib, "fb_put_signal", i32, [vp, vp, u64, u64, i32, i32, i32, vp])
     _sig(lib, "fb_wait_signal", i32, [vp, i32, u32, vp])
+    _sig(lib, "fb_accumulate", i32, [vp, vp, u64, u64, i32, i32, i32, vp, vp])
+    _sig(lib, "fb_compare_and_swap", i32, [vp, vp, vp, vp, u64, i32, i32, vp])
 
     regp = C.POINTER(FbMergeRegion)
     _sig(

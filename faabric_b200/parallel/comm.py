@@ -79,6 +79,10 @@ OPS = {
     "minloc": 9,
     "lxor": 10,
     "bxor": 11,
+    # one-sided accumulate only (FB_OP_REPLACE, FB_OP_NO_OP); every collective
+    # rejects them
+    "replace": 32,
+    "no_op": 33,
 }
 ALGOS = {"auto": 0, "oneshot": 1, "twoshot": 2, "nvls": 3, "ll": 4}
 ALGO_NAMES = {v: k for k, v in ALGOS.items()}
@@ -515,6 +519,86 @@ class Communicator:
             self._lib.fb_wait_signal(self._h, signal, count, self._stream(stream)),
             "wait_signal",
         )
+
+    # ------------------------------------------------------ one-sided atomics
+    def _rma_ptr(self, t, what) -> int:
+        if t is None:
+            return 0
+        if not t.is_cuda or not t.is_contiguous():
+            raise CommError(f"{what} must be a contiguous CUDA tensor")
+        return t.data_ptr()
+
+    def _rma_offset(self, dst_sym, nbytes) -> int:
+        if not dst_sym.is_contiguous() or dst_sym.numel() * dst_sym.element_size() < nbytes:
+            raise CommError(f"dst_sym must be a contiguous symmetric tensor of at least {nbytes} bytes")
+        if not self._lib.fb_comm_in_heap(self._h, C.c_void_p(dst_sym.data_ptr()), max(nbytes, 1)):
+            raise CommError("dst_sym is not in the symmetric heap")
+        return self.heap_offset(dst_sym)
+
+    def accumulate(self, src, dst_sym, peer, op="sum", dtype=None, fetch=None, stream=None):
+        """Atomically combine ``src`` into ``peer``'s copy of the symmetric tensor
+        ``dst_sym``, element by element: ``dst[i] = op(dst[i], src[i])``
+        (MPI_Accumulate).  With ``fetch``, every element's previous value is
+        written there first (MPI_Get_accumulate).  ``op`` is any reduction op
+        of :meth:`all_reduce` for the dtype, ``"replace"``, or ``"no_op"``,
+        an atomic read into ``fetch`` for which ``src`` may be None.  The
+        target elements must be aligned to their size; ``src`` and ``fetch``
+        need no alignment.  Concurrent accumulates from any rank to the same
+        element compose atomically.  Stream-ordered; returns ``fetch``."""
+        if op not in OPS:
+            raise CommError(f"unknown op {op!r}")
+        ref = src if src is not None else fetch
+        if ref is None:
+            raise CommError("accumulate needs src (or fetch for no_op)")
+        count, dt = self._typed(ref, dtype)
+        nbytes = ref.numel() * ref.element_size()
+        if fetch is not None and fetch.numel() * fetch.element_size() != nbytes:
+            raise CommError(f"fetch must hold {nbytes} bytes like src")
+        rc = self._lib.fb_accumulate(
+            self._h,
+            C.c_void_p(self._rma_ptr(src, "src")),
+            self._rma_offset(dst_sym, nbytes),
+            count,
+            dt,
+            OPS[op],
+            peer,
+            C.c_void_p(self._rma_ptr(fetch, "fetch")),
+            self._stream(stream),
+        )
+        self._check(rc, "accumulate")
+        return fetch
+
+    def fetch_and_op(self, src, dst_sym, peer, result, op="sum", dtype=None, stream=None):
+        """MPI_Fetch_and_op: :meth:`accumulate` of ONE element with fetch into
+        ``result`` (``src`` may be None for ``"no_op"``)."""
+        for t, what in ((src, "src"), (result, "result")):
+            if t is not None and self._typed(t, dtype)[0] != 1:
+                raise CommError(f"fetch_and_op: {what} must be exactly one element")
+        return self.accumulate(src, dst_sym, peer, op=op, dtype=dtype, fetch=result, stream=stream)
+
+    def compare_and_swap(self, compare, swap, dst_sym, peer, result, dtype=None, stream=None):
+        """MPI_Compare_and_swap on one integer element of ``peer``'s copy of
+        ``dst_sym``: ``result = old; if old == compare: target = swap``."""
+        dts = set()
+        for t, what in ((compare, "compare"), (swap, "swap"), (result, "result")):
+            count, dt = self._typed(t, dtype)
+            if count != 1:
+                raise CommError(f"compare_and_swap: {what} must be exactly one element")
+            dts.add(dt)
+        if len(dts) != 1:
+            raise CommError("compare_and_swap: compare, swap and result must have one dtype")
+        rc = self._lib.fb_compare_and_swap(
+            self._h,
+            C.c_void_p(self._rma_ptr(compare, "compare")),
+            C.c_void_p(self._rma_ptr(swap, "swap")),
+            C.c_void_p(self._rma_ptr(result, "result")),
+            self._rma_offset(dst_sym, result.numel() * result.element_size()),
+            dts.pop(),
+            peer,
+            self._stream(stream),
+        )
+        self._check(rc, "compare_and_swap")
+        return result
 
 
 class GroupPlan:
