@@ -23,6 +23,8 @@
 #include <faabric/util/memory.h>
 #include <faabric/util/snapshot.h>
 
+#include "../tests/mpi_rma_atomics_body.h"
+
 #include <cuda_runtime.h>
 
 #include <chrono>
@@ -709,6 +711,109 @@ static void registerFunctions()
         EXPECT((rc == MPI_SUCCESS) == oneProcess);
         if (rc == MPI_SUCCESS) {
             MPI_Win_free(&sharedWin);
+        }
+        return 0;
+    });
+
+    // One-sided atomics from every rank onto every rank's window, in this
+    // process or another one (shipped and applied at the fence).  Input:
+    // "host" | "cuda" | "heap" window memory, then ",device" for origin and
+    // result buffers in cudaMalloc memory.
+    mpiFunction("rma-atomics", [](int rank, int size, faabric::Message& msg) {
+        const std::string& in = msg.inputdata();
+        rma_atomics::Setup s;
+        s.window = in.rfind("cuda", 0) == 0   ? rma_atomics::WindowMemory::CudaMalloc
+                   : in.rfind("heap", 0) == 0 ? rma_atomics::WindowMemory::Heap
+                                              : rma_atomics::WindowMemory::Host;
+        s.deviceBuffers = in.find(",device") != std::string::npos;
+        std::string why;
+        int rc = rma_atomics::body(rank, size, msg.mpiworldid(), s, &why);
+        if (rc != 0) {
+            SPDLOG_ERROR("rma-atomics: {}", why);
+            msg.set_outputdata(why);
+        }
+        return rc;
+    });
+
+    // Cost of the MPI one-sided atomics, rank 0 onto rank 1's window, each
+    // call followed by its closing fence.  Input:
+    // "fop|acc;<i32|f32|i64>;<bytes>;<iters>;<heap|cuda>;<host|device>".
+    // Rank 0 reports {"us_per_call", "gb_per_s"}.
+    mpiFunction("bench-rma", [](int rank, int size, faabric::Message& msg) {
+        std::vector<std::string> f;
+        std::string cur;
+        for (char c : msg.inputdata() + ";") {
+            if (c == ';') {
+                f.push_back(cur);
+                cur.clear();
+            } else {
+                cur += c;
+            }
+        }
+        EXPECT(f.size() >= 6 && size >= 2);
+        const bool fop = f[0] == "fop";
+        MPI_Datatype dt = f[1] == "f32" ? MPI_FLOAT : (f[1] == "i64" ? MPI_INT64_T : MPI_INT);
+        const size_t bytes = std::stoul(f[2]);
+        const int iters = std::stoi(f[3]);
+        const bool heap = f[4] == "heap";
+        const bool devBuf = f[5] == "device";
+        const int count = (int)(bytes / dt->size);
+        uint8_t* window = nullptr;
+        if (heap) {
+            EXPECT(MPI_Alloc_mem(bytes, MPI_INFO_FAABRIC_DEVICE, &window) == MPI_SUCCESS);
+        } else {
+            EXPECT(cudaMalloc((void**)&window, bytes) == cudaSuccess);
+        }
+        cudaMemset(window, 0, bytes);
+        cudaDeviceSynchronize();
+        // ones: an add that leaves the target unchanged skips its write on the
+        // CAS paths and would time faster than real work
+        std::vector<uint8_t> hostOrigin(bytes, 0), hostResult(bytes, 0);
+        for (size_t i = 0; i + dt->size <= bytes; i += dt->size) {
+            const float f = 1.0f;
+            const int64_t one = 1;
+            memcpy(hostOrigin.data() + i, dt == MPI_FLOAT ? (const void*)&f : (const void*)&one, dt->size);
+        }
+        uint8_t* origin = hostOrigin.data();
+        uint8_t* result = hostResult.data();
+        if (devBuf) {
+            EXPECT(cudaMalloc((void**)&origin, bytes) == cudaSuccess && cudaMalloc((void**)&result, bytes) == cudaSuccess);
+            cudaMemcpy(origin, hostOrigin.data(), bytes, cudaMemcpyHostToDevice);
+            cudaDeviceSynchronize();
+        }
+        MPI_Win win = nullptr;
+        MPI_Win_create(window, bytes, 1, MPI_INFO_NULL, MPI_COMM_WORLD, &win);
+        MPI_Win_fence(0, win);
+        auto issue = [&]() {
+            if (rank != 0) {
+                return MPI_SUCCESS;
+            }
+            return fop ? MPI_Fetch_and_op(origin, result, dt, 1, 0, MPI_SUM, win)
+                       : MPI_Accumulate(origin, count, dt, 1, 0, count, dt, MPI_SUM, win);
+        };
+        for (int i = 0; i < 3; i++) {
+            EXPECT(issue() == MPI_SUCCESS);
+            MPI_Win_fence(0, win);
+        }
+        auto t0 = std::chrono::steady_clock::now();
+        for (int i = 0; i < iters; i++) {
+            EXPECT(issue() == MPI_SUCCESS);
+            MPI_Win_fence(0, win);
+        }
+        double us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count() / iters;
+        if (rank == 0) {
+            msg.set_outputdata("{\"us_per_call\": " + std::to_string(us) +
+                               ", \"gb_per_s\": " + std::to_string((double)bytes / (us * 1e3)) + "}");
+        }
+        MPI_Win_free(&win);
+        if (devBuf) {
+            cudaFree(origin);
+            cudaFree(result);
+        }
+        if (heap) {
+            MPI_Free_mem(window);
+        } else {
+            cudaFree(window);
         }
         return 0;
     });

@@ -187,7 +187,10 @@ extern "C"
     X(FAABRIC_OP_NULL, 11, faabric_op_null)                                    \
     /* extensions */                                                           \
     X(FAABRIC_OP_LXOR, 12, faabric_op_lxor)                                    \
-    X(FAABRIC_OP_BXOR, 13, faabric_op_bxor)
+    X(FAABRIC_OP_BXOR, 13, faabric_op_bxor)                                    \
+    /* one-sided accumulates only; collectives refuse them with MPI_ERR_OP */  \
+    X(FAABRIC_OP_REPLACE, 14, faabric_op_replace)                              \
+    X(FAABRIC_OP_NO_OP, 15, faabric_op_no_op)
 
 #define FAABRIC_MPI_DECLARE_OP(name, num, var)                                 \
     enum                                                                       \
@@ -211,6 +214,8 @@ extern "C"
 #define MPI_OP_NULL &faabric_op_null
 #define MPI_LXOR &faabric_op_lxor
 #define MPI_BXOR &faabric_op_bxor
+#define MPI_REPLACE &faabric_op_replace
+#define MPI_NO_OP &faabric_op_no_op
 
 #define MPI_STATUS_IGNORE ((MPI_Status*)(0))
 #define MPI_STATUSES_IGNORE ((MPI_Status*)(0))
@@ -333,6 +338,18 @@ extern "C"
                 MPI_Aint target_disp, int target_count, MPI_Datatype target_datatype, MPI_Win win);
     int MPI_Put(const void* origin_addr, int origin_count, MPI_Datatype origin_datatype, int target_rank,
                 MPI_Aint target_disp, int target_count, MPI_Datatype target_datatype, MPI_Win win);
+    /* One-sided atomics: every target element is updated atomically.  Fetched
+     * values are defined after the closing MPI_Win_fence. */
+    int MPI_Accumulate(const void* origin_addr, int origin_count, MPI_Datatype origin_datatype, int target_rank,
+                       MPI_Aint target_disp, int target_count, MPI_Datatype target_datatype, MPI_Op op, MPI_Win win);
+    int MPI_Get_accumulate(const void* origin_addr, int origin_count, MPI_Datatype origin_datatype,
+                           void* result_addr, int result_count, MPI_Datatype result_datatype, int target_rank,
+                           MPI_Aint target_disp, int target_count, MPI_Datatype target_datatype, MPI_Op op,
+                           MPI_Win win);
+    int MPI_Fetch_and_op(const void* origin_addr, void* result_addr, MPI_Datatype datatype, int target_rank,
+                         MPI_Aint target_disp, MPI_Op op, MPI_Win win);
+    int MPI_Compare_and_swap(const void* origin_addr, const void* compare_addr, void* result_addr,
+                             MPI_Datatype datatype, int target_rank, MPI_Aint target_disp, MPI_Win win);
 
 #ifdef __cplusplus
 }

@@ -365,6 +365,37 @@ class MpiWorld
 
     void winGet(int rank, int winId, uint8_t* origin, size_t bytes, int targetRank, int64_t targetDisp);
 
+    // One-sided atomics (MPI_Accumulate family): `count` elements of a
+    // predefined `datatype`, target[i] = op(target[i], origin[i]), each element
+    // atomically.  `result` (null: no fetch) receives the previous values; it
+    // is defined after the closing fence.  Every argument is checked before
+    // anything is applied; returns MPI_SUCCESS or an MPI error code.
+    //   host segment in this process       the host atomics, on this thread
+    //   symmetric heap in this process     Communicator::accumulate, on the
+    //                                      origin rank's stream
+    //   other device memory in this process  the pointer kernel on a GPU that
+    //                                      can address the segment
+    //   rank in another worker process     shipped and applied at the fence
+    int winAccumulate(int rank,
+                      int winId,
+                      const uint8_t* origin,
+                      size_t count,
+                      faabric_datatype_t* datatype,
+                      faabric_op_t* op,
+                      uint8_t* result,
+                      int targetRank,
+                      int64_t targetDisp);
+
+    // One integer element: *result = target; if (target == *compare) target = *origin
+    int winCompareSwap(int rank,
+                       int winId,
+                       const uint8_t* origin,
+                       const uint8_t* compare,
+                       uint8_t* result,
+                       faabric_datatype_t* datatype,
+                       int targetRank,
+                       int64_t targetDisp);
+
     // Window segment of `rank`; false if the window is unknown
     bool winQuery(int winId, int rank, void** base, int64_t* sizeBytes, int* dispUnit);
 
@@ -427,13 +458,27 @@ class MpiWorld
     int getLocalLeader() { return leaderForHost.at(thisHost); }
 
     // ---- one-sided windows ----
+    enum RmaKind : int
+    {
+        RMA_PUT = 0,
+        RMA_GET = 1,
+        RMA_ACCUMULATE = 2,
+        RMA_GET_ACCUMULATE = 3,
+        RMA_COMPARE_SWAP = 4,
+    };
     struct RmaOp
     {
-        int kind; // 0 = put, 1 = get
+        int kind; // RmaKind
         int target;
         uint64_t dispBytes;
         uint64_t bytes;
-        uint8_t* origin;
+        uint8_t* origin; // put / get: the user's buffer
+        // atomics: FbDtype / FbOp, a host copy of the origin (and compare)
+        // values, and where the fetched values go (or null)
+        int dtype = -1;
+        int op = -1;
+        std::vector<uint8_t> data;
+        uint8_t* result = nullptr;
     };
     struct RmaWindow
     {
@@ -446,6 +491,9 @@ class MpiWorld
         // operations queued for other processes, one list per ORIGIN rank
         // (only that rank's thread touches its list)
         std::vector<std::vector<RmaOp>> pending;
+        // (device, stream) pairs each rank launched atomics on this epoch,
+        // waited for by its fence (only that rank's thread touches its list)
+        std::vector<std::vector<std::pair<int, void*>>> streams;
     };
     std::mutex windowsMx;
     std::map<int, std::shared_ptr<RmaWindow>> windows;
@@ -455,6 +503,23 @@ class MpiWorld
     uint8_t* winTargetPtr(RmaWindow& w, int targetRank, int64_t targetDisp, size_t bytes);
     void rmaSendOps(RmaWindow& w, int rank, int peer);
     void rmaRecvOps(RmaWindow& w, int rank, int peer, int nOps);
+    // One atomic operation of `rank` on a segment in this process (the paths
+    // of winAccumulate); `compare` non-null means compare-and-swap
+    void rmaApplyLocal(RmaWindow& w,
+                       int rank,
+                       int targetRank,
+                       uint8_t* target,
+                       size_t count,
+                       int dtype,
+                       int op,
+                       const uint8_t* origin,
+                       const uint8_t* compare,
+                       uint8_t* result);
+    // Communicator of a rank if one is wired already (never creates one)
+    std::shared_ptr<faabric::device::Communicator> wiredDeviceComm(int rank);
+    // Stream of `rank` on `device` for one-sided atomics
+    void* rmaStream(int rank, int device);
+    std::map<std::pair<int, int>, void*> rmaStreams;
 
     // ---- local queues (size x size, lazily created) ----
     std::vector<std::shared_ptr<InMemoryMpiQueue>> localQueues;

@@ -204,31 +204,27 @@ cudaError_t launchWaitSignal(const FbCommDev& c,
 
 
 // ------------------------------------------------------------------- rma ----
-// One-sided atomics on heap[peer] + dstOff (rma_kernels.cu).  Every target
-// element is updated atomically with respect to every other RMA kernel on any
-// GPU.  Every target element must be aligned to its size (fbDtypeSize: 8 for
-// the 8-byte pairs, 16 for the 16-byte pairs); origin and result buffers need
-// no alignment.  No kernel waits on a peer or takes part in a barrier.
+// One-sided atomics on `target` (rma_kernels.cu): any memory the launching GPU
+// can address, e.g. a peer's symmetric heap through its mapping, or a
+// cudaMalloc window.  Every target element is updated atomically with respect
+// to every other RMA kernel on any GPU.  Every target element must be aligned
+// to its size (fbDtypeSize: 8 for the 8-byte pairs, 16 for the 16-byte pairs);
+// origin and result buffers need no alignment.  No kernel waits on a peer or
+// takes part in a barrier.
 struct RmaArgs
 {
-    FbCommDev comm;
+    uint8_t* target;
     const uint8_t* origin; // count elements (unused for NO_OP)
     uint8_t* result;       // previous values, or null (no fetch)
-    uint64_t dstOff;
     uint64_t count;
-    int32_t peer;
-    int32_t pad;
 };
 
 struct RmaCasArgs
 {
-    FbCommDev comm;
+    uint8_t* target;
     const uint8_t* compare; // one element each
     const uint8_t* swap;
     uint8_t* result;
-    uint64_t dstOff;
-    int32_t peer;
-    int32_t pad;
 };
 
 // (dtype, op) pairs the accumulate kernels implement: every device reduction

@@ -1,9 +1,11 @@
 // One-sided atomics (sm_90a): MPI_Accumulate, MPI_Get_accumulate,
-// MPI_Fetch_and_op and MPI_Compare_and_swap on the symmetric heap.
+// MPI_Fetch_and_op and MPI_Compare_and_swap on any memory the launching GPU
+// can address.
 //
 //  * rmaAccumulateKernel<DT, OP, FETCH> — grid-stride over `count` elements:
-//    target[i] = combine(target[i], origin[i]), where target is heap[peer] +
-//    dstOff (a peer mapping over NVLink, or local memory).  combine is the
+//    target[i] = combine(target[i], origin[i]), where target is a pointer (a
+//    peer's symmetric heap through its NVLink mapping, a cudaMalloc window, or
+//    local memory).  combine is the
 //    element-wise rule of the reduce kernels (fb_prims.cuh: reduceElem,
 //    reducePair), REPLACE stores the origin value and NO_OP keeps the target.
 //    FETCH also writes every element's previous value to `result`.
@@ -238,7 +240,7 @@ template<int DT, int OP, bool FETCH>
 __global__ void __launch_bounds__(RMA_THREADS) rmaAccumulateKernel(const RmaArgs a)
 {
     using E = RmaElem<DT>;
-    uint8_t* tgt = a.comm.heap[a.peer] + a.dstOff;
+    uint8_t* tgt = a.target;
     const uint64_t tid = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
     const uint64_t nth = (uint64_t)gridDim.x * blockDim.x;
     uint64_t first = 0;
@@ -281,7 +283,7 @@ template<int DT>
 __global__ void rmaCompareSwapKernel(const RmaCasArgs a)
 {
     using T = typename RmaType<DT>::T;
-    uint8_t* tgt = a.comm.heap[a.peer] + a.dstOff;
+    uint8_t* tgt = a.target;
     const T cmp = ldBytes<T>(a.compare);
     const T swp = ldBytes<T>(a.swap);
     T old;

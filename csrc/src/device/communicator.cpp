@@ -2647,12 +2647,10 @@ int Communicator::accumulate(const void* origin,
     bindDevice();
     fb::RmaArgs a;
     memset(&a, 0, sizeof(a));
-    a.comm = dev_;
+    a.target = dev_.heap[peer] + dstOffset;
     a.origin = (const uint8_t*)origin;
     a.result = (uint8_t*)fetchOut;
-    a.dstOff = dstOffset;
     a.count = count;
-    a.peer = peer;
     stats_.launches++;
     stats_.bytes += (uint64_t)count * esize;
     return k_->rmaAccumulate(a, dtype, op, s) == cudaSuccess ? FB_OK : FB_E_CUDA;
@@ -2679,12 +2677,10 @@ int Communicator::compareAndSwap(const void* compare,
     bindDevice();
     fb::RmaCasArgs a;
     memset(&a, 0, sizeof(a));
-    a.comm = dev_;
+    a.target = dev_.heap[peer] + dstOffset;
     a.compare = (const uint8_t*)compare;
     a.swap = (const uint8_t*)swap;
     a.result = (uint8_t*)result;
-    a.dstOff = dstOffset;
-    a.peer = peer;
     stats_.launches++;
     stats_.bytes += esize;
     return k_->rmaCompareSwap(a, dtype, s) == cudaSuccess ? FB_OK : FB_E_CUDA;

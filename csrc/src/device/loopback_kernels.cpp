@@ -627,10 +627,11 @@ cudaError_t waitWord(const FbCommDev& c, const uint32_t* word, uint32_t target, 
 }
 
 // ------------------------------------------------------------------ rma ----
-// The host twins of rma_kernels.cu.  Every element is one atomic step with
-// respect to the other rank threads: a CAS loop on the enclosing 32-bit word
+// The host twins of rma_kernels.cu, also the implementation of one-sided
+// atomics on host windows.  Every element is one atomic step with respect to
+// the other threads of the process: a CAS loop on the enclosing 32-bit word
 // (1, 2 and 4-byte elements) or on the 64-bit element, and a striped lock for
-// 16-byte elements.  The target is naturally aligned (the communicator checks).
+// 16-byte elements.  The target is naturally aligned (the callers check).
 namespace {
 
 // bytes of an element that an update replaces: a 16-byte pair keeps its padding
@@ -712,7 +713,7 @@ void rmaAtomic(uint8_t* p, size_t n, uint8_t* prev, F f)
 cudaError_t rmaAccumulate(const RmaArgs& a, int dtype, int op, cudaStream_t)
 {
     const size_t n = fbDtypeSize(dtype);
-    uint8_t* tgt = a.comm.heap[a.peer] + a.dstOff;
+    uint8_t* tgt = a.target;
     for (uint64_t i = 0; i < a.count; i++) {
         const uint8_t* in = op == FB_OP_NO_OP ? nullptr : a.origin + i * n;
         rmaAtomic(tgt + i * n, n, a.result != nullptr ? a.result + i * n : nullptr, [&](const uint8_t* cur, uint8_t* nv) {
@@ -725,7 +726,7 @@ cudaError_t rmaAccumulate(const RmaArgs& a, int dtype, int op, cudaStream_t)
 cudaError_t rmaCompareSwap(const RmaCasArgs& a, int dtype, cudaStream_t)
 {
     const size_t n = fbDtypeSize(dtype);
-    rmaAtomic(a.comm.heap[a.peer] + a.dstOff, n, a.result, [&](const uint8_t* cur, uint8_t* nv) {
+    rmaAtomic(a.target, n, a.result, [&](const uint8_t* cur, uint8_t* nv) {
         memcpy(nv, memcmp(cur, a.compare, n) == 0 ? a.swap : cur, n);
     });
     return cudaSuccess;

@@ -224,6 +224,10 @@ int fbOpFor(faabric_op_t* op)
             return FB_OP_LXOR;
         case FAABRIC_OP_BXOR:
             return FB_OP_BXOR;
+        case FAABRIC_OP_REPLACE:
+            return FB_OP_REPLACE;
+        case FAABRIC_OP_NO_OP:
+            return FB_OP_NO_OP;
         default:
             return -1;
     }
@@ -280,6 +284,9 @@ MpiWorld::~MpiWorld()
         if (s != nullptr) {
             cudaStreamDestroy((cudaStream_t)s);
         }
+    }
+    for (auto& [key, s] : rmaStreams) {
+        cudaStreamDestroy((cudaStream_t)s);
     }
     cudaGetLastError();
 }

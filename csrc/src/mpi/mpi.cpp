@@ -52,6 +52,8 @@ struct faabric_op_t faabric_op_minloc = { .id = FAABRIC_OP_MINLOC };
 struct faabric_op_t faabric_op_null = { .id = FAABRIC_OP_NULL };
 struct faabric_op_t faabric_op_lxor = { .id = FAABRIC_OP_LXOR };
 struct faabric_op_t faabric_op_bxor = { .id = FAABRIC_OP_BXOR };
+struct faabric_op_t faabric_op_replace = { .id = FAABRIC_OP_REPLACE };
+struct faabric_op_t faabric_op_no_op = { .id = FAABRIC_OP_NO_OP };
 
 struct faabric_datatype_t* getFaabricDatatypeFromId(int datatypeId)
 {

@@ -157,6 +157,83 @@ std::map<int, faabric_request_t*>& requestTable()
     static thread_local std::map<int, faabric_request_t*> t;
     return t;
 }
+
+// MPI_REPLACE and MPI_NO_OP only exist for one-sided accumulates.  Collectives
+// refuse them up front, before any rank sends, waits or launches.
+bool accumulateOnlyOp(MPI_Op op)
+{
+    return op != nullptr && (op->id == FAABRIC_OP_REPLACE || op->id == FAABRIC_OP_NO_OP);
+}
+
+// A datatype as (predefined base type, base elements per element)
+bool baseTypeOf(MPI_Datatype dt, MPI_Datatype* base, int* per)
+{
+    if (dt == nullptr) {
+        return false;
+    }
+    int baseId = dt->id;
+    *per = 1;
+    if (dt->id >= FAABRIC_DERIVED_TYPE_BASE && !getContiguousType(dt->id, &baseId, per)) {
+        return false;
+    }
+    *base = getFaabricDatatypeFromId(baseId);
+    return *base != nullptr && fbDtypeFor(*base) >= 0;
+}
+
+// The element type and element count shared by the origin / result and the
+// target of an accumulate.  MPI_ERR_ARG unless every buffer has the same base
+// type and the same number of bytes.
+int accumulateShape(const std::vector<std::pair<int, MPI_Datatype>>& sides, MPI_Datatype* base, size_t* count)
+{
+    int fdt = -1;
+    int64_t bytes = -1;
+    for (const auto& [n, dt] : sides) {
+        MPI_Datatype b = nullptr;
+        int per = 0;
+        if (n < 0 || !baseTypeOf(dt, &b, &per)) {
+            return MPI_ERR_ARG;
+        }
+        const int64_t sideBytes = (int64_t)n * dt->size;
+        if ((fdt >= 0 && fbDtypeFor(b) != fdt) || (bytes >= 0 && sideBytes != bytes)) {
+            return MPI_ERR_ARG;
+        }
+        fdt = fbDtypeFor(b);
+        bytes = sideBytes;
+        *base = b;
+    }
+    *count = (size_t)bytes / (size_t)(*base)->size;
+    return MPI_SUCCESS;
+}
+
+int getAccumulate(const void* origin, int originCount, MPI_Datatype originType, void* result, int resultCount,
+                  MPI_Datatype resultType, int targetRank, MPI_Aint targetDisp, int targetCount, MPI_Datatype targetType,
+                  MPI_Op op, MPI_Win win)
+{
+    if (win == nullptr) {
+        return MPI_ERR_WIN;
+    }
+    if (op == nullptr || isUserOp(op)) {
+        return MPI_ERR_OP;
+    }
+    if (op->id == FAABRIC_OP_NO_OP && result == nullptr) {
+        return MPI_ERR_OP; // MPI_NO_OP only fetches
+    }
+    std::vector<std::pair<int, MPI_Datatype>> sides{ { targetCount, targetType } };
+    if (op->id != FAABRIC_OP_NO_OP) {
+        sides.emplace_back(originCount, originType); // (ignored for MPI_NO_OP)
+    }
+    if (result != nullptr) {
+        sides.emplace_back(resultCount, resultType);
+    }
+    MPI_Datatype base = nullptr;
+    size_t count = 0;
+    int rc = accumulateShape(sides, &base, &count);
+    if (rc != MPI_SUCCESS) {
+        return rc;
+    }
+    return getExecutingWorld().winAccumulate(executingContext.getRank(), win->id, (const uint8_t*)origin, count, base, op,
+                                             (uint8_t*)result, targetRank, (int64_t)targetDisp);
+}
 }
 
 extern "C"
@@ -524,6 +601,9 @@ int MPI_Allgatherv(const void* sendbuf, int sendcount, MPI_Datatype sendtype, vo
 int MPI_Reduce(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, int root, MPI_Comm comm)
 {
     SPDLOG_TRACE("MPI - MPI_Reduce all -> {}", root);
+    if (accumulateOnlyOp(op)) {
+        return MPI_ERR_OP;
+    }
     if (auto sub = subOf(comm)) {
         sub->reduce(getExecutingWorld(), executingContext.getRank(), root, (const uint8_t*)resolveInPlace(sendbuf, recvbuf),
                     (uint8_t*)recvbuf, datatype, count, op);
@@ -538,6 +618,9 @@ int MPI_Reduce_scatter(const void* sendbuf, void* recvbuf, const int* recvcounts
                        MPI_Op op, MPI_Comm comm)
 {
     SPDLOG_TRACE("MPI - MPI_Reduce_scatter");
+    if (accumulateOnlyOp(op)) {
+        return MPI_ERR_OP;
+    }
     subCommOnly(comm, "MPI_Reduce_scatter");
     MpiWorld& world = getExecutingWorld();
     int size = world.getSize();
@@ -585,6 +668,9 @@ int MPI_Reduce_scatter(const void* sendbuf, void* recvbuf, const int* recvcounts
 int MPI_Allreduce(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, MPI_Comm comm)
 {
     SPDLOG_TRACE("MPI - MPI_Allreduce");
+    if (accumulateOnlyOp(op)) {
+        return MPI_ERR_OP;
+    }
     if (auto sub = subOf(comm)) {
         sub->allReduce(getExecutingWorld(), executingContext.getRank(), (const uint8_t*)resolveInPlace(sendbuf, recvbuf),
                        (uint8_t*)recvbuf, datatype, count, op);
@@ -598,6 +684,9 @@ int MPI_Allreduce(const void* sendbuf, void* recvbuf, int count, MPI_Datatype da
 int MPI_Scan(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, MPI_Comm comm)
 {
     SPDLOG_TRACE("MPI - MPI_Scan");
+    if (accumulateOnlyOp(op)) {
+        return MPI_ERR_OP;
+    }
     if (auto sub = subOf(comm)) {
         sub->scan(getExecutingWorld(), executingContext.getRank(), (const uint8_t*)resolveInPlace(sendbuf, recvbuf),
                   (uint8_t*)recvbuf, datatype, count, op);
@@ -802,6 +891,9 @@ int MPI_Free_mem(void* base)
 int MPI_Iallreduce(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, MPI_Comm comm, MPI_Request* request)
 {
     SPDLOG_TRACE("MPI - MPI_Iallreduce");
+    if (accumulateOnlyOp(op)) {
+        return MPI_ERR_OP;
+    }
     subCommOnly(comm, "MPI_Iallreduce");
     int id = getExecutingWorld().iAllReduce(executingContext.getRank(),
                                             (uint8_t*)resolveInPlace(sendbuf, recvbuf),
@@ -900,6 +992,56 @@ int MPI_Put(const void* origin_addr, int origin_count, MPI_Datatype origin_datat
     }
     getExecutingWorld().winPut(executingContext.getRank(), win->id, (const uint8_t*)origin_addr, bytes, target_rank, target_disp);
     return MPI_SUCCESS;
+}
+
+int MPI_Accumulate(const void* origin_addr, int origin_count, MPI_Datatype origin_datatype, int target_rank,
+                   MPI_Aint target_disp, int target_count, MPI_Datatype target_datatype, MPI_Op op, MPI_Win win)
+{
+    SPDLOG_TRACE("MPI - MPI_Accumulate");
+    if (op == MPI_NO_OP) {
+        return MPI_ERR_OP; // only MPI_Get_accumulate / MPI_Fetch_and_op take it
+    }
+    return getAccumulate(origin_addr, origin_count, origin_datatype, nullptr, 0, nullptr, target_rank, target_disp,
+                         target_count, target_datatype, op, win);
+}
+
+int MPI_Get_accumulate(const void* origin_addr, int origin_count, MPI_Datatype origin_datatype, void* result_addr,
+                       int result_count, MPI_Datatype result_datatype, int target_rank, MPI_Aint target_disp,
+                       int target_count, MPI_Datatype target_datatype, MPI_Op op, MPI_Win win)
+{
+    SPDLOG_TRACE("MPI - MPI_Get_accumulate");
+    if (result_addr == nullptr && result_count > 0) {
+        return MPI_ERR_ARG;
+    }
+    return getAccumulate(origin_addr, origin_count, origin_datatype, result_addr, result_count, result_datatype,
+                         target_rank, target_disp, target_count, target_datatype, op, win);
+}
+
+int MPI_Fetch_and_op(const void* origin_addr, void* result_addr, MPI_Datatype datatype, int target_rank,
+                     MPI_Aint target_disp, MPI_Op op, MPI_Win win)
+{
+    SPDLOG_TRACE("MPI - MPI_Fetch_and_op");
+    if (result_addr == nullptr) {
+        return MPI_ERR_ARG;
+    }
+    return getAccumulate(origin_addr, 1, datatype, result_addr, 1, datatype, target_rank, target_disp, 1, datatype, op, win);
+}
+
+int MPI_Compare_and_swap(const void* origin_addr, const void* compare_addr, void* result_addr, MPI_Datatype datatype,
+                         int target_rank, MPI_Aint target_disp, MPI_Win win)
+{
+    SPDLOG_TRACE("MPI - MPI_Compare_and_swap");
+    if (win == nullptr) {
+        return MPI_ERR_WIN;
+    }
+    MPI_Datatype base = nullptr;
+    int per = 0;
+    if (!baseTypeOf(datatype, &base, &per) || per != 1) {
+        return MPI_ERR_ARG;
+    }
+    return getExecutingWorld().winCompareSwap(executingContext.getRank(), win->id, (const uint8_t*)origin_addr,
+                                              (const uint8_t*)compare_addr, (uint8_t*)result_addr, base, target_rank,
+                                              (int64_t)target_disp);
 }
 
 int MPI_Win_free(MPI_Win* win)
