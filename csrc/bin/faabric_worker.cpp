@@ -24,6 +24,7 @@
 #include <faabric/util/snapshot.h>
 
 #include "../tests/mpi_rma_atomics_body.h"
+#include "../tests/mpi_rma_passive_body.h"
 
 #include <cuda_runtime.h>
 
@@ -735,6 +736,26 @@ static void registerFunctions()
         return rc;
     });
 
+    // Passive-target synchronisation (locks, flushes, lock-all) with origins
+    // in the target's process and in other ones; shipped operations are
+    // applied by the target's point-to-point server, no fence.  Input as for
+    // rma-atomics.
+    mpiFunction("rma-passive", [](int rank, int size, faabric::Message& msg) {
+        const std::string& in = msg.inputdata();
+        rma_passive::Setup s;
+        s.window = in.rfind("cuda", 0) == 0   ? rma_passive::WindowMemory::CudaMalloc
+                   : in.rfind("heap", 0) == 0 ? rma_passive::WindowMemory::Heap
+                                              : rma_passive::WindowMemory::Host;
+        s.deviceBuffers = in.find(",device") != std::string::npos;
+        std::string why;
+        int rc = rma_passive::body(rank, size, msg.mpiworldid(), s, &why);
+        if (rc != 0) {
+            SPDLOG_ERROR("rma-passive: {}", why);
+            msg.set_outputdata(why);
+        }
+        return rc;
+    });
+
     // Cost of the MPI one-sided atomics, rank 0 onto rank 1's window, each
     // call followed by its closing fence.  Input:
     // "fop|acc;<i32|f32|i64>;<bytes>;<iters>;<heap|cuda>;<host|device>".
@@ -814,6 +835,94 @@ static void registerFunctions()
             MPI_Free_mem(window);
         } else {
             cudaFree(window);
+        }
+        return 0;
+    });
+
+    // Cost of passive-target synchronisation, rank 0 onto rank 1's 8-byte
+    // window.  Input: "<mode>;<heap|cuda|host>;<host|device>;<iters>" with mode
+    //   flush  MPI_Fetch_and_op + MPI_Win_flush inside MPI_Win_lock_all
+    //   fence  MPI_Fetch_and_op + MPI_Win_fence (the same call, fence-based)
+    //   lock   MPI_Win_lock(EXCLUSIVE) + MPI_Win_unlock, nothing in between
+    // Rank 0 reports {"us_per_call"}.
+    mpiFunction("bench-rma-passive", [](int rank, int size, faabric::Message& msg) {
+        std::vector<std::string> f;
+        std::string cur;
+        for (char c : msg.inputdata() + ";") {
+            if (c == ';') {
+                f.push_back(cur);
+                cur.clear();
+            } else {
+                cur += c;
+            }
+        }
+        EXPECT(f.size() >= 4 && size >= 2);
+        const std::string mode = f[0];
+        const int iters = std::stoi(f[3]);
+        const bool devBuf = f[2] == "device";
+        uint8_t* window = nullptr;
+        if (f[1] == "heap") {
+            EXPECT(MPI_Alloc_mem(8, MPI_INFO_FAABRIC_DEVICE, &window) == MPI_SUCCESS);
+            cudaMemset(window, 0, 8);
+        } else if (f[1] == "cuda") {
+            EXPECT(cudaMalloc((void**)&window, 8) == cudaSuccess);
+            cudaMemset(window, 0, 8);
+        } else {
+            window = (uint8_t*)calloc(1, 8);
+        }
+        cudaDeviceSynchronize();
+        int64_t hostBufs[2] = { 1, 0 };
+        int64_t* bufs = hostBufs;
+        if (devBuf) {
+            EXPECT(cudaMalloc((void**)&bufs, 16) == cudaSuccess);
+            cudaMemcpy(bufs, hostBufs, 16, cudaMemcpyHostToDevice);
+            cudaDeviceSynchronize();
+        }
+        MPI_Win win = nullptr;
+        MPI_Win_create(window, 8, 1, MPI_INFO_NULL, MPI_COMM_WORLD, &win);
+        auto step = [&]() {
+            if (mode == "fence") {
+                int rc = rank == 0 ? MPI_Fetch_and_op(bufs, bufs + 1, MPI_INT64_T, 1, 0, MPI_SUM, win) : MPI_SUCCESS;
+                return rc == MPI_SUCCESS ? MPI_Win_fence(0, win) : rc;
+            }
+            if (rank != 0) {
+                return MPI_SUCCESS;
+            }
+            if (mode == "lock") {
+                int rc = MPI_Win_lock(MPI_LOCK_EXCLUSIVE, 1, 0, win);
+                return rc == MPI_SUCCESS ? MPI_Win_unlock(1, win) : rc;
+            }
+            int rc = MPI_Fetch_and_op(bufs, bufs + 1, MPI_INT64_T, 1, 0, MPI_SUM, win);
+            return rc == MPI_SUCCESS ? MPI_Win_flush(1, win) : rc;
+        };
+        const bool epoch = mode == "flush" && rank == 0;
+        if (epoch) {
+            EXPECT(MPI_Win_lock_all(0, win) == MPI_SUCCESS);
+        }
+        for (int i = 0; i < 3; i++) {
+            EXPECT(step() == MPI_SUCCESS);
+        }
+        auto t0 = std::chrono::steady_clock::now();
+        for (int i = 0; i < iters; i++) {
+            EXPECT(step() == MPI_SUCCESS);
+        }
+        double us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count() / iters;
+        if (epoch) {
+            EXPECT(MPI_Win_unlock_all(win) == MPI_SUCCESS);
+        }
+        if (rank == 0) {
+            msg.set_outputdata("{\"us_per_call\": " + std::to_string(us) + "}");
+        }
+        MPI_Win_free(&win);
+        if (devBuf) {
+            cudaFree(bufs);
+        }
+        if (f[1] == "heap") {
+            MPI_Free_mem(window);
+        } else if (f[1] == "cuda") {
+            cudaFree(window);
+        } else {
+            free(window);
         }
         return 0;
     });

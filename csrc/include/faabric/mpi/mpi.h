@@ -21,7 +21,22 @@ extern "C"
 #define MPI_ERR_WIN 4
 #define MPI_ERR_RANK 5
 #define MPI_ERR_ARG 6
+/* a synchronisation call out of place: unlock / flush of a target that is
+ * not locked, a second lock, fence or free inside a passive epoch */
+#define MPI_ERR_RMA_SYNC 7
 #define MPI_MAX_OBJECT_NAME 128
+
+/* passive-target lock types (MPI_Win_lock) */
+#define MPI_LOCK_EXCLUSIVE 234
+#define MPI_LOCK_SHARED 235
+
+/* assert bits of MPI_Win_lock / MPI_Win_lock_all / MPI_Win_fence: NOCHECK
+ * skips the lock, the others are accepted and ignored */
+#define MPI_MODE_NOCHECK 1024
+#define MPI_MODE_NOSTORE 2048
+#define MPI_MODE_NOPUT 4096
+#define MPI_MODE_NOPRECEDE 8192
+#define MPI_MODE_NOSUCCEED 16384
 
     /* ---- opaque-ish handle structs ---- */
     struct faabric_status_public_t
@@ -350,6 +365,18 @@ extern "C"
                          MPI_Aint target_disp, MPI_Op op, MPI_Win win);
     int MPI_Compare_and_swap(const void* origin_addr, const void* compare_addr, void* result_addr,
                              MPI_Datatype datatype, int target_rank, MPI_Aint target_disp, MPI_Win win);
+    /* Passive-target synchronisation.  Inside a lock epoch, operations are
+     * complete at origin and target (fetched values defined) after
+     * MPI_Win_flush* or MPI_Win_unlock* of their target; no fence. */
+    int MPI_Win_lock(int lock_type, int rank, int assert, MPI_Win win);
+    int MPI_Win_unlock(int rank, MPI_Win win);
+    int MPI_Win_lock_all(int assert, MPI_Win win);
+    int MPI_Win_unlock_all(MPI_Win win);
+    int MPI_Win_flush(int rank, MPI_Win win);
+    int MPI_Win_flush_all(MPI_Win win);
+    int MPI_Win_flush_local(int rank, MPI_Win win);
+    int MPI_Win_flush_local_all(MPI_Win win);
+    int MPI_Win_sync(MPI_Win win);
 
 #ifdef __cplusplus
 }

@@ -15,7 +15,10 @@
 #include <faabric/util/queue.h>
 
 #include <atomic>
+#include <condition_variable>
 #include <cstdint>
+#include <deque>
+#include <functional>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -396,6 +399,36 @@ class MpiWorld
                        int targetRank,
                        int64_t targetDisp);
 
+    // ---- passive-target synchronisation (MPI_Win_lock and friends) ----
+    // Locks are reader/writer locks per target segment, held in the target's
+    // process and granted in arrival order; a wait is bounded by the world's
+    // message timeout (MPI_ERR_OTHER).  Inside a lock epoch every operation
+    // takes its usual path; those for a rank in another worker process are
+    // shipped at the next flush / unlock of that rank instead of a fence.
+    // Every call returns MPI_SUCCESS or an MPI error code; MPI_ERR_RMA_SYNC
+    // calls change nothing.
+    int winLock(int rank, int winId, int lockType, int targetRank, int assert);
+
+    int winUnlock(int rank, int winId, int targetRank);
+
+    int winLockAll(int rank, int winId, int assert);
+
+    int winUnlockAll(int rank, int winId);
+
+    // Completes every operation of `rank` to `targetRank` (-1: every locked
+    // target) at origin and target
+    int winFlush(int rank, int winId, int targetRank);
+
+    // True while `rank` holds a lock (or lock-all) epoch on the window
+    bool winInPassiveEpoch(int rank, int winId);
+
+    // A passive-target request from another worker process (a PointToPointCall
+    // RMA_* code); returns the reply
+    static std::string serveRmaRequest(int call, const uint8_t* buffer, size_t bytes);
+
+    // The grant of a lock this process queued for in another one
+    static void serveRmaGrant(const uint8_t* buffer, size_t bytes);
+
     // Window segment of `rank`; false if the window is unknown
     bool winQuery(int winId, int rank, void** base, int64_t* sizeBytes, int* dispUnit);
 
@@ -480,6 +513,36 @@ class MpiWorld
         std::vector<uint8_t> data;
         uint8_t* result = nullptr;
     };
+    // A lock request not granted yet: an origin thread of this process waits
+    // for `granted`, one in another process gets `onGrant` (a message)
+    struct RmaLockWaiter
+    {
+        uint64_t ticket;
+        bool exclusive;
+        std::shared_ptr<bool> granted;
+        std::function<void()> onGrant;
+    };
+    // Reader/writer lock of one target segment
+    struct RmaLock
+    {
+        int exclusive = 0;
+        int shared = 0;
+        std::deque<RmaLockWaiter> waiters;
+    };
+    // Passive epoch of one origin: the targets it locked (NOCHECK: without
+    // taking the lock), or all of them after MPI_Win_lock_all
+    struct RmaEpoch
+    {
+        struct Target
+        {
+            bool exclusive;
+            bool nocheck;
+        };
+        bool all = false;
+        std::map<int, Target> locked;
+        // puts / gets of this epoch went through cudaMemcpy
+        bool deviceCopies = false;
+    };
     struct RmaWindow
     {
         std::mutex mx;
@@ -494,17 +557,29 @@ class MpiWorld
         // (device, stream) pairs each rank launched atomics on this epoch,
         // waited for by its fence (only that rank's thread touches its list)
         std::vector<std::vector<std::pair<int, void*>>> streams;
+        // passive epochs, one per ORIGIN rank (only that rank's thread)
+        std::vector<RmaEpoch> epochs;
+        // lock of each target segment in this process, under lockMx
+        std::mutex lockMx;
+        std::condition_variable lockCv;
+        std::vector<RmaLock> locks;
     };
     std::mutex windowsMx;
     std::map<int, std::shared_ptr<RmaWindow>> windows;
     // windows created so far by each rank (collective order => same ids)
     std::vector<int> windowsCreated;
     std::shared_ptr<RmaWindow> getWindow(int winId);
+    // nullptr if the window is unknown (or freed)
+    std::shared_ptr<RmaWindow> findWindow(int winId);
     uint8_t* winTargetPtr(RmaWindow& w, int targetRank, int64_t targetDisp, size_t bytes);
     void rmaSendOps(RmaWindow& w, int rank, int peer);
     void rmaRecvOps(RmaWindow& w, int rank, int peer, int nOps);
+    // Payload bytes of a shipped atomic on `target`; throws if it is malformed
+    static size_t rmaAtomicPayload(int kind, int dtype, int op, uint64_t bytes, const uint8_t* target);
     // One atomic operation of `rank` on a segment in this process (the paths
-    // of winAccumulate); `compare` non-null means compare-and-swap
+    // of winAccumulate); `compare` non-null means compare-and-swap.  Device
+    // streams that still run it are added to `used`.  `serverPath`: applied
+    // for another process outside any rank thread, on streams of its own.
     void rmaApplyLocal(RmaWindow& w,
                        int rank,
                        int targetRank,
@@ -514,7 +589,17 @@ class MpiWorld
                        int op,
                        const uint8_t* origin,
                        const uint8_t* compare,
-                       uint8_t* result);
+                       uint8_t* result,
+                       std::vector<std::pair<int, void*>>& used,
+                       bool serverPath = false);
+    // Waits for the device streams `rank` used on the window
+    void rmaWaitStreams(RmaWindow& w, int rank);
+    // Takes the lock of a target segment for `rank` (waits for the grant)
+    int rmaAcquire(RmaWindow& w, int winId, int rank, int targetRank, bool exclusive);
+    // Completes `rank`'s operations to `targetRank`; `release` also unlocks
+    int rmaComplete(RmaWindow& w, int winId, int rank, int targetRank, bool release);
+    // Handles a request of serveRmaRequest on this world
+    std::string rmaServe(int call, const uint8_t* buffer, size_t bytes);
     // Communicator of a rank if one is wired already (never creates one)
     std::shared_ptr<faabric::device::Communicator> wiredDeviceComm(int rank);
     // Stream of `rank` on `device` for one-sided atomics
@@ -671,6 +756,9 @@ class MpiWorldRegistry
     MpiWorld& getOrInitialiseWorld(faabric::Message& msg);
 
     MpiWorld& getWorld(int worldId);
+
+    // nullptr if the world does not exist (any more); keeps it alive
+    std::shared_ptr<MpiWorld> findWorld(int worldId);
 
     bool worldExists(int worldId);
 

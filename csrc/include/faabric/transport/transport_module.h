@@ -774,6 +774,14 @@ enum PointToPointCall
     LOCK_GROUP_RECURSIVE = 3,
     UNLOCK_GROUP = 4,
     UNLOCK_GROUP_RECURSIVE = 5,
+    // MPI passive-target one-sided requests to the process of a target rank
+    // (sync; see MpiWorld::serveRmaRequest) and the grant of a queued lock
+    // back to the origin's process (async)
+    RMA_LOCK = 6,
+    RMA_LOCK_CANCEL = 7,
+    RMA_FLUSH = 8,
+    RMA_UNLOCK = 9,
+    RMA_LOCK_GRANT = 10,
 };
 
 }
@@ -813,6 +821,12 @@ class PointToPointClient : public faabric::transport::MessageEndpointClient
                      int groupId,
                      int groupIdx,
                      bool recursive = false);
+
+    // MPI passive-target request (RMA_LOCK, RMA_LOCK_CANCEL, RMA_FLUSH,
+    // RMA_UNLOCK): returns the reply bytes
+    std::vector<uint8_t> rmaRequest(PointToPointCall call, const std::vector<uint8_t>& request);
+
+    void rmaLockGrant(const uint8_t* buffer, size_t bytes);
 
   private:
     void makeCoordinationRequest(int appId,

@@ -67,6 +67,12 @@ MpiWorld& MpiWorldRegistry::getWorld(int worldId)
     return *w.value();
 }
 
+std::shared_ptr<MpiWorld> MpiWorldRegistry::findWorld(int worldId)
+{
+    auto w = worldMap.get(worldId);
+    return w.has_value() ? w.value() : nullptr;
+}
+
 bool MpiWorldRegistry::worldExists(int worldId)
 {
     return worldMap.contains(worldId);

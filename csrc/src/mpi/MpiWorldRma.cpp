@@ -3,6 +3,10 @@
 #include <faabric/device/communicator.h>
 #include <faabric/device/cuda_driver.h>
 #include <faabric/mpi/MpiWorld.h>
+#include <faabric/mpi/MpiWorldRegistry.h>
+#include <faabric/transport/PointToPointCall.h>
+#include <faabric/transport/PointToPointClient.h>
+#include <faabric/util/config.h>
 #include <faabric/util/logging.h>
 #include <faabric/util/macros.h>
 
@@ -12,7 +16,9 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <chrono>
 #include <cstring>
+#include <set>
 #include <stdexcept>
 
 namespace faabric::mpi {
@@ -174,12 +180,19 @@ struct RmaStage
     }
 };
 
+// True if a copy between the two goes through CUDA (without a GPU, the
+// loopback backend's heaps are plain host memory)
+bool cudaCopy(const void* dst, const void* src)
+{
+    return (MpiWorld::isDevicePointer(dst) || MpiWorld::isDevicePointer(src)) && faabric::device::cudaAvailable();
+}
+
 void rmaCopy(void* dst, const void* src, size_t bytes)
 {
     if (bytes == 0) {
         return;
     }
-    if (MpiWorld::isDevicePointer(dst) || MpiWorld::isDevicePointer(src)) {
+    if (cudaCopy(dst, src)) {
         if (cudaMemcpy(dst, src, bytes, cudaMemcpyDefault) != cudaSuccess) {
             cudaGetLastError();
             throw std::runtime_error("Device copy for a one-sided operation failed");
@@ -230,6 +243,8 @@ int MpiWorld::winCreate(int rank, void* base, int64_t sizeBytes, int dispUnit)
             slot = std::make_shared<RmaWindow>();
             slot->pending.resize(size);
             slot->streams.resize(size);
+            slot->epochs.resize(size);
+            slot->locks.resize(size);
         }
         w = slot;
     }
@@ -277,6 +292,13 @@ void MpiWorld::winFree(int rank, int winId)
     }
 }
 
+std::shared_ptr<MpiWorld::RmaWindow> MpiWorld::findWindow(int winId)
+{
+    std::lock_guard<std::mutex> lk(windowsMx);
+    auto it = windows.find(winId);
+    return it == windows.end() || !it->second->filled ? nullptr : it->second;
+}
+
 bool MpiWorld::winQuery(int winId, int rank, void** base, int64_t* sizeBytes, int* dispUnit)
 {
     std::shared_ptr<RmaWindow> w;
@@ -316,8 +338,11 @@ void MpiWorld::winPut(int rank, int winId, const uint8_t* origin, size_t bytes, 
     uint8_t* dst = winTargetPtr(*w, targetRank, targetDisp, bytes);
     if (isLocalRank(targetRank)) {
         // Same address space (or peer-mapped HBM): write it now, the closing
-        // fence publishes it
+        // fence (or flush) publishes it
         rmaCopy(dst, origin, bytes);
+        if (!w->epochs[rank].locked.empty()) {
+            w->epochs[rank].deviceCopies |= cudaCopy(dst, origin);
+        }
         return;
     }
     uint64_t dispBytes = (uint64_t)(dst - (uint8_t*)(uintptr_t)w->bases[targetRank]);
@@ -330,6 +355,9 @@ void MpiWorld::winGet(int rank, int winId, uint8_t* origin, size_t bytes, int ta
     uint8_t* src = winTargetPtr(*w, targetRank, targetDisp, bytes);
     if (isLocalRank(targetRank)) {
         rmaCopy(origin, src, bytes);
+        if (!w->epochs[rank].locked.empty()) {
+            w->epochs[rank].deviceCopies |= cudaCopy(origin, src);
+        }
         return;
     }
     uint64_t dispBytes = (uint64_t)(src - (uint8_t*)(uintptr_t)w->bases[targetRank]);
@@ -348,7 +376,8 @@ std::shared_ptr<faabric::device::Communicator> MpiWorld::wiredDeviceComm(int ran
 void* MpiWorld::rmaStream(int rank, int device)
 {
     // (one stream per rank and device, whatever else is wired: the calls of
-    // one origin on one segment stay in issue order)
+    // one origin on one segment stay in issue order.  Rank -1: the streams of
+    // the passive-target server path)
     std::lock_guard<std::mutex> lk(deviceMx);
     void*& s = rmaStreams[{ rank, device }];
     if (s == nullptr) {
@@ -367,7 +396,9 @@ void MpiWorld::rmaApplyLocal(RmaWindow& w,
                              int op,
                              const uint8_t* origin,
                              const uint8_t* compare,
-                             uint8_t* result)
+                             uint8_t* result,
+                             std::vector<std::pair<int, void*>>& used,
+                             bool serverPath)
 {
     const size_t esize = fbDtypeSize(dtype);
     const size_t bytes = count * esize;
@@ -375,7 +406,6 @@ void MpiWorld::rmaApplyLocal(RmaWindow& w,
         return;
     }
     auto streamUsed = [&](int device, void* s) {
-        auto& used = w.streams[rank];
         if (std::find(used.begin(), used.end(), std::make_pair(device, s)) == used.end()) {
             used.emplace_back(device, s);
         }
@@ -385,7 +415,9 @@ void MpiWorld::rmaApplyLocal(RmaWindow& w,
     auto targetComm = wiredDeviceComm(targetRank);
     if (comm != nullptr && targetComm != nullptr && targetComm->inHeap(target, bytes)) {
         const int device = comm->isLoopback() ? HOST_MEMORY : comm->device();
-        cudaStream_t s = (cudaStream_t)streamForRank(rank);
+        cudaStream_t s = !serverPath               ? (cudaStream_t)streamForRank(rank)
+                         : device == HOST_MEMORY ? nullptr
+                                                 : (cudaStream_t)rmaStream(-1, device);
         DeviceGuard on(device);
         RmaStage st(device, s, bytes, esize, origin, compare, result);
         const uint64_t off = targetComm->offsetOf(target);
@@ -432,7 +464,7 @@ void MpiWorld::rmaApplyLocal(RmaWindow& w,
             cudaGetLastError();
         }
     }
-    cudaStream_t s = (cudaStream_t)rmaStream(rank, device);
+    cudaStream_t s = (cudaStream_t)rmaStream(serverPath ? -1 : rank, device);
     DeviceGuard on(device);
     RmaStage st(device, s, bytes, esize, origin, compare, result);
     cudaError_t e;
@@ -508,7 +540,7 @@ int MpiWorld::winAccumulate(int rank,
         return rc;
     }
     if (isLocalRank(targetRank)) {
-        rmaApplyLocal(*w, rank, targetRank, target, count, dtype, fop, origin, nullptr, result);
+        rmaApplyLocal(*w, rank, targetRank, target, count, dtype, fop, origin, nullptr, result, w->streams[rank]);
         return MPI_SUCCESS;
     }
     if (bytes > (uint64_t)INT32_MAX) {
@@ -551,7 +583,7 @@ int MpiWorld::winCompareSwap(int rank,
         return rc;
     }
     if (isLocalRank(targetRank)) {
-        rmaApplyLocal(*w, rank, targetRank, target, 1, dtype, -1, origin, compare, result);
+        rmaApplyLocal(*w, rank, targetRank, target, 1, dtype, -1, origin, compare, result, w->streams[rank]);
         return MPI_SUCCESS;
     }
     RmaOp q{ RMA_COMPARE_SWAP, targetRank, (uint64_t)(target - (uint8_t*)(uintptr_t)w->bases[targetRank]), esize, nullptr };
@@ -599,6 +631,18 @@ void MpiWorld::rmaSendOps(RmaWindow& w, int rank, int peer)
     }
 }
 
+size_t MpiWorld::rmaAtomicPayload(int kind, int dtype, int op, uint64_t bytes, const uint8_t* target)
+{
+    const bool cas = kind == RMA_COMPARE_SWAP;
+    const size_t esize = fbDtypeSize(dtype);
+    if ((kind != RMA_ACCUMULATE && kind != RMA_GET_ACCUMULATE && !cas) || esize == 0 || bytes % esize != 0 ||
+        (uintptr_t)target % esize != 0 ||
+        (cas ? bytes != esize || !fb::rmaCasSupported(dtype) : !fb::rmaSupported(dtype, op, kind == RMA_GET_ACCUMULATE))) {
+        throw std::runtime_error("Malformed remote one-sided atomic");
+    }
+    return cas ? 2 * esize : (op == FB_OP_NO_OP ? 0 : bytes);
+}
+
 void MpiWorld::rmaRecvOps(RmaWindow& w, int rank, int peer, int nOps)
 {
     faabric_datatype_t* byteType = getFaabricDatatypeFromId(FAABRIC_BYTE);
@@ -621,12 +665,7 @@ void MpiWorld::rmaRecvOps(RmaWindow& w, int rank, int peer, int nOps)
         // Atomics, applied in arrival order through this segment's path
         const bool cas = wire.kind == RMA_COMPARE_SWAP;
         const size_t esize = fbDtypeSize(wire.dtype);
-        if (esize == 0 || wire.bytes % esize != 0 || (uintptr_t)(base + wire.dispBytes) % esize != 0 ||
-            (cas ? wire.bytes != esize || !fb::rmaCasSupported(wire.dtype)
-                 : !fb::rmaSupported(wire.dtype, wire.op, wire.kind == RMA_GET_ACCUMULATE))) {
-            throw std::runtime_error("Malformed remote one-sided atomic");
-        }
-        const size_t dataBytes = cas ? 2 * esize : (wire.op == FB_OP_NO_OP ? 0 : wire.bytes);
+        const size_t dataBytes = rmaAtomicPayload(wire.kind, wire.dtype, wire.op, wire.bytes, base + wire.dispBytes);
         data.resize(dataBytes);
         if (dataBytes > 0) {
             recv(peer, rank, data.data(), byteType, (int)dataBytes, nullptr, MpiMessageType::RMA_DATA);
@@ -642,31 +681,35 @@ void MpiWorld::rmaRecvOps(RmaWindow& w, int rank, int peer, int nOps)
                       wire.op,
                       dataBytes > 0 ? data.data() : nullptr,
                       cas ? data.data() + esize : nullptr,
-                      fetch ? fetched.data() : nullptr);
+                      fetch ? fetched.data() : nullptr,
+                      w.streams[rank]);
         if (fetch) {
             send(rank, peer, fetched.data(), byteType, (int)wire.bytes, MpiMessageType::RMA_DATA);
         }
     }
 }
 
+void MpiWorld::rmaWaitStreams(RmaWindow& w, int rank)
+{
+    auto comm = wiredDeviceComm(rank);
+    for (auto [device, s] : w.streams[rank]) {
+        DeviceGuard on(device);
+        if (comm != nullptr && !comm->isLoopback() && comm->device() == device) {
+            if (!comm->waitStreamFast((cudaStream_t)s)) {
+                throw std::runtime_error("One-sided operation failed on the device");
+            }
+        } else {
+            cudaCheck(cudaStreamSynchronize((cudaStream_t)s), "One-sided operation");
+        }
+    }
+    w.streams[rank].clear();
+}
+
 void MpiWorld::winFence(int rank, int winId)
 {
     auto w = getWindow(winId);
     // Atomics this rank launched on device streams complete first
-    {
-        auto comm = wiredDeviceComm(rank);
-        for (auto [device, s] : w->streams[rank]) {
-            DeviceGuard on(device);
-            if (comm != nullptr && !comm->isLoopback() && comm->device() == device) {
-                if (!comm->waitStreamFast((cudaStream_t)s)) {
-                    throw std::runtime_error("One-sided operation failed on the device");
-                }
-            } else {
-                cudaCheck(cudaStreamSynchronize((cudaStream_t)s), "One-sided operation");
-            }
-        }
-        w->streams[rank].clear();
-    }
+    rmaWaitStreams(*w, rank);
     if (!allRanksLocal()) {
         // How many operations does everybody have for everybody else?
         std::vector<int> outgoing(size, 0), incoming(size, 0);
@@ -693,6 +736,588 @@ void MpiWorld::winFence(int rank, int winId)
         w->pending[rank].clear();
     }
     barrier(rank);
+}
+
+// ---------------------------------------------------------------------------
+// Passive-target synchronisation (MPI_Win_lock, MPI_Win_flush, ...)
+// ---------------------------------------------------------------------------
+namespace {
+// A request to the process of a target rank: this header, then (flush and
+// unlock) nOps times an RmaWireOp followed by its payload
+struct RmaPassiveHeader
+{
+    int32_t worldId;
+    int32_t winId;
+    int32_t origin;
+    int32_t target;
+    int32_t exclusive;
+    int32_t nOps;
+    uint64_t ticket;
+};
+
+// First word of every reply.  A flush / unlock reply goes on with the bytes
+// of its gets and fetches, in request order.
+enum RmaReply : int32_t
+{
+    RMA_REPLY_OK = 0,
+    // lock: queued, the grant follows as RMA_LOCK_GRANT
+    RMA_REPLY_QUEUED = 1,
+    // the world or the window is unknown to the target's process (or freed)
+    RMA_REPLY_NO_WINDOW = 2,
+    RMA_REPLY_FAILED = 3,
+};
+
+std::string replyOf(int32_t status)
+{
+    return std::string((const char*)&status, sizeof(status));
+}
+
+// Grants of locks that origins of this process queued for elsewhere
+struct GrantTable
+{
+    std::mutex mx;
+    std::condition_variable cv;
+    std::set<uint64_t> granted;
+};
+
+GrantTable& grantTable()
+{
+    static GrantTable t;
+    return t;
+}
+
+std::atomic<uint64_t> nextTicket{ 1 };
+
+std::chrono::milliseconds lockTimeout()
+{
+    return std::chrono::milliseconds(faabric::util::getSystemConfig().globalMessageTimeout);
+}
+
+// ---- reader/writer lock of a target segment (caller holds lockMx) ----
+template<class Lock>
+bool lockFits(const Lock& l, bool exclusive)
+{
+    return exclusive ? l.exclusive == 0 && l.shared == 0 : l.exclusive == 0;
+}
+
+// Grants waiters in arrival order while they fit (a shared waiter behind an
+// exclusive one waits too: no starvation); returns the grant messages to send
+template<class Lock>
+std::vector<std::function<void()>> grantWaiters(Lock& l)
+{
+    std::vector<std::function<void()>> sends;
+    while (!l.waiters.empty() && lockFits(l, l.waiters.front().exclusive)) {
+        auto& q = l.waiters.front();
+        (q.exclusive ? l.exclusive : l.shared)++;
+        *q.granted = true;
+        if (q.onGrant) {
+            sends.push_back(std::move(q.onGrant));
+        }
+        l.waiters.pop_front();
+    }
+    return sends;
+}
+
+template<class Lock>
+std::vector<std::function<void()>> releaseLock(Lock& l, bool exclusive)
+{
+    int& held = exclusive ? l.exclusive : l.shared;
+    if (held == 0) {
+        throw std::runtime_error("Releasing a one-sided lock that is not held");
+    }
+    held--;
+    return grantWaiters(l);
+}
+
+// Drops a waiter that gave up; false if it was granted already
+template<class Lock>
+bool dropWaiter(Lock& l, uint64_t ticket)
+{
+    auto it = std::find_if(l.waiters.begin(), l.waiters.end(), [&](const auto& q) { return q.ticket == ticket; });
+    if (it == l.waiters.end()) {
+        return false;
+    }
+    l.waiters.erase(it);
+    return true;
+}
+
+// Wakes the origins of this process and sends the other grants (outside
+// lockMx: a send must not hold up the lock)
+template<class Window>
+void announceGrants(Window& w, const std::vector<std::function<void()>>& sends)
+{
+    w.lockCv.notify_all();
+    for (const auto& send : sends) {
+        try {
+            send();
+        } catch (const std::exception& e) {
+            SPDLOG_ERROR("Could not send a one-sided lock grant: {}", e.what());
+        }
+    }
+}
+
+// One request to the process of a target; the reply's status, the rest of
+// the reply in `rest`
+int32_t rmaCall(const std::string& host, faabric::transport::PointToPointCall call, const std::vector<uint8_t>& request, std::vector<uint8_t>* rest)
+{
+    std::vector<uint8_t> reply;
+    try {
+        reply = faabric::transport::getPointToPointClient(host)->rmaRequest(call, request);
+    } catch (const std::exception& e) {
+        SPDLOG_ERROR("One-sided request to {} failed: {}", host, e.what());
+        return RMA_REPLY_FAILED;
+    }
+    int32_t status = RMA_REPLY_FAILED;
+    if (reply.size() >= sizeof(status)) {
+        memcpy(&status, reply.data(), sizeof(status));
+        if (rest != nullptr) {
+            rest->assign(reply.begin() + sizeof(status), reply.end());
+        }
+    }
+    return status;
+}
+
+int mpiErrorOf(int32_t status)
+{
+    return status == RMA_REPLY_OK ? MPI_SUCCESS : status == RMA_REPLY_NO_WINDOW ? MPI_ERR_WIN : MPI_ERR_OTHER;
+}
+
+template<class V>
+void append(std::vector<uint8_t>& out, const V& v)
+{
+    out.insert(out.end(), (const uint8_t*)&v, (const uint8_t*)&v + sizeof(v));
+}
+}
+
+int MpiWorld::rmaAcquire(RmaWindow& w, int winId, int rank, int targetRank, bool exclusive)
+{
+    const uint64_t ticket = nextTicket++;
+    if (isLocalRank(targetRank)) {
+        auto granted = std::make_shared<bool>(false);
+        std::unique_lock<std::mutex> lk(w.lockMx);
+        RmaLock& l = w.locks[targetRank];
+        l.waiters.push_back(RmaLockWaiter{ ticket, exclusive, granted, nullptr });
+        grantWaiters(l);
+        if (w.lockCv.wait_for(lk, lockTimeout(), [&] { return *granted; })) {
+            return MPI_SUCCESS;
+        }
+        dropWaiter(l, ticket);
+        auto sends = grantWaiters(l);
+        lk.unlock();
+        announceGrants(w, sends);
+        SPDLOG_ERROR("Rank {} timed out waiting for the lock of rank {} on window {}", rank, targetRank, winId);
+        return MPI_ERR_OTHER;
+    }
+    // The lock lives in the target's process: granted there at once, or
+    // queued and granted by a later message
+    const std::string host = getHostForRank(targetRank);
+    std::vector<uint8_t> req;
+    append(req, RmaPassiveHeader{ id, winId, rank, targetRank, exclusive ? 1 : 0, 0, ticket });
+    const int32_t status = rmaCall(host, faabric::transport::PointToPointCall::RMA_LOCK, req, nullptr);
+    if (status != RMA_REPLY_QUEUED) {
+        return mpiErrorOf(status);
+    }
+    GrantTable& g = grantTable();
+    std::unique_lock<std::mutex> lk(g.mx);
+    const bool granted = g.cv.wait_for(lk, lockTimeout(), [&] { return g.granted.count(ticket) > 0; });
+    g.granted.erase(ticket);
+    lk.unlock();
+    if (granted) {
+        return MPI_SUCCESS;
+    }
+    // (the target drops the request, or releases the lock if it was granted
+    // meanwhile)
+    rmaCall(host, faabric::transport::PointToPointCall::RMA_LOCK_CANCEL, req, nullptr);
+    SPDLOG_ERROR("Rank {} timed out waiting for the lock of rank {} on window {}", rank, targetRank, winId);
+    return MPI_ERR_OTHER;
+}
+
+int MpiWorld::rmaComplete(RmaWindow& w, int winId, int rank, int targetRank, bool release)
+{
+    RmaEpoch& e = w.epochs[rank];
+    const RmaEpoch::Target t = e.locked.at(targetRank);
+    const bool unlock = release && !t.nocheck;
+    if (isLocalRank(targetRank)) {
+        // Everything of this origin in this process completes: its device
+        // streams, and copies from pageable memory still in flight
+        rmaWaitStreams(w, rank);
+        if (e.deviceCopies) {
+            cudaCheck(cudaStreamSynchronize(cudaStreamLegacy), "One-sided copy");
+            e.deviceCopies = false;
+        }
+        if (unlock) {
+            std::vector<std::function<void()>> sends;
+            {
+                std::lock_guard<std::mutex> lk(w.lockMx);
+                sends = releaseLock(w.locks[targetRank], t.exclusive);
+            }
+            announceGrants(w, sends);
+        }
+        return MPI_SUCCESS;
+    }
+    // Ship the operations queued for the target; it applies them, waits for
+    // its streams and answers with the fetched values
+    std::vector<uint8_t> req;
+    append(req, RmaPassiveHeader{ id, winId, rank, targetRank, t.exclusive ? 1 : 0, 0, 0 });
+    std::vector<const RmaOp*> replies;
+    size_t replyBytes = 0;
+    int nOps = 0;
+    for (const RmaOp& op : w.pending[rank]) {
+        if (op.target != targetRank) {
+            continue;
+        }
+        append(req, RmaWireOp{ op.kind, op.dtype, op.dispBytes, op.bytes, op.op, 0 });
+        const uint8_t* payload = op.kind == RMA_PUT ? op.origin : op.kind == RMA_GET ? nullptr : op.data.data();
+        const size_t payloadBytes = op.kind == RMA_PUT ? op.bytes : op.kind == RMA_GET ? 0 : op.data.size();
+        if (payloadBytes > 0) {
+            req.resize(req.size() + payloadBytes);
+            rmaCopy(req.data() + req.size() - payloadBytes, payload, payloadBytes);
+        }
+        if (op.kind == RMA_GET || op.kind == RMA_GET_ACCUMULATE || op.kind == RMA_COMPARE_SWAP) {
+            replies.push_back(&op);
+            replyBytes += op.bytes;
+        }
+        nOps++;
+    }
+    if (nOps == 0 && !unlock) {
+        return MPI_SUCCESS;
+    }
+    reinterpret_cast<RmaPassiveHeader*>(req.data())->nOps = nOps;
+    std::vector<uint8_t> fetched;
+    int32_t status = rmaCall(getHostForRank(targetRank),
+                             unlock ? faabric::transport::PointToPointCall::RMA_UNLOCK
+                                    : faabric::transport::PointToPointCall::RMA_FLUSH,
+                             req,
+                             &fetched);
+    if (status == RMA_REPLY_OK && fetched.size() != replyBytes) {
+        status = RMA_REPLY_FAILED;
+    }
+    if (status == RMA_REPLY_OK) {
+        size_t off = 0;
+        bool toDevice = false;
+        for (const RmaOp* op : replies) {
+            uint8_t* dst = op->kind == RMA_GET ? op->origin : op->result;
+            rmaCopy(dst, fetched.data() + off, op->bytes);
+            toDevice |= cudaCopy(dst, nullptr);
+            off += op->bytes;
+        }
+        if (toDevice) {
+            // (a copy from pageable memory may return before its DMA lands)
+            cudaCheck(cudaStreamSynchronize(cudaStreamLegacy), "Returning fetched values");
+        }
+    }
+    auto& pending = w.pending[rank];
+    pending.erase(std::remove_if(pending.begin(), pending.end(), [&](const RmaOp& op) { return op.target == targetRank; }),
+                  pending.end());
+    return mpiErrorOf(status);
+}
+
+int MpiWorld::winLock(int rank, int winId, int lockType, int targetRank, int assert)
+{
+    auto w = findWindow(winId);
+    if (w == nullptr) {
+        return MPI_ERR_WIN;
+    }
+    if (targetRank < 0 || targetRank >= size) {
+        return MPI_ERR_RANK;
+    }
+    if (lockType != MPI_LOCK_EXCLUSIVE && lockType != MPI_LOCK_SHARED) {
+        return MPI_ERR_ARG;
+    }
+    RmaEpoch& e = w->epochs[rank];
+    if (e.all || e.locked.count(targetRank) > 0) {
+        return MPI_ERR_RMA_SYNC;
+    }
+    const bool exclusive = lockType == MPI_LOCK_EXCLUSIVE;
+    const bool nocheck = (assert & MPI_MODE_NOCHECK) != 0;
+    if (!nocheck) {
+        int rc = rmaAcquire(*w, winId, rank, targetRank, exclusive);
+        if (rc != MPI_SUCCESS) {
+            return rc;
+        }
+    }
+    e.locked[targetRank] = RmaEpoch::Target{ exclusive, nocheck };
+    return MPI_SUCCESS;
+}
+
+int MpiWorld::winUnlock(int rank, int winId, int targetRank)
+{
+    auto w = findWindow(winId);
+    if (w == nullptr) {
+        return MPI_ERR_WIN;
+    }
+    if (targetRank < 0 || targetRank >= size) {
+        return MPI_ERR_RANK;
+    }
+    RmaEpoch& e = w->epochs[rank];
+    if (e.all || e.locked.count(targetRank) == 0) {
+        return MPI_ERR_RMA_SYNC;
+    }
+    int rc = rmaComplete(*w, winId, rank, targetRank, true);
+    e.locked.erase(targetRank);
+    return rc;
+}
+
+int MpiWorld::winLockAll(int rank, int winId, int assert)
+{
+    auto w = findWindow(winId);
+    if (w == nullptr) {
+        return MPI_ERR_WIN;
+    }
+    RmaEpoch& e = w->epochs[rank];
+    if (e.all || !e.locked.empty()) {
+        return MPI_ERR_RMA_SYNC;
+    }
+    const bool nocheck = (assert & MPI_MODE_NOCHECK) != 0;
+    // Shared locks in increasing rank order
+    for (int t = 0; t < size; t++) {
+        if (!nocheck) {
+            int rc = rmaAcquire(*w, winId, rank, t, false);
+            if (rc != MPI_SUCCESS) {
+                for (int u = 0; u < t; u++) {
+                    rmaComplete(*w, winId, rank, u, true);
+                }
+                e.locked.clear();
+                return rc;
+            }
+        }
+        e.locked[t] = RmaEpoch::Target{ false, nocheck };
+    }
+    e.all = true;
+    return MPI_SUCCESS;
+}
+
+int MpiWorld::winUnlockAll(int rank, int winId)
+{
+    auto w = findWindow(winId);
+    if (w == nullptr) {
+        return MPI_ERR_WIN;
+    }
+    RmaEpoch& e = w->epochs[rank];
+    if (!e.all) {
+        return MPI_ERR_RMA_SYNC;
+    }
+    int rc = MPI_SUCCESS;
+    for (int t = 0; t < size; t++) {
+        int r = rmaComplete(*w, winId, rank, t, true);
+        rc = rc == MPI_SUCCESS ? r : rc;
+    }
+    e.locked.clear();
+    e.all = false;
+    return rc;
+}
+
+int MpiWorld::winFlush(int rank, int winId, int targetRank)
+{
+    auto w = findWindow(winId);
+    if (w == nullptr) {
+        return MPI_ERR_WIN;
+    }
+    RmaEpoch& e = w->epochs[rank];
+    if (targetRank >= 0 && targetRank < size) {
+        return e.locked.count(targetRank) == 0 ? MPI_ERR_RMA_SYNC : rmaComplete(*w, winId, rank, targetRank, false);
+    }
+    if (targetRank != -1) {
+        return MPI_ERR_RANK;
+    }
+    if (e.locked.empty()) {
+        return MPI_ERR_RMA_SYNC;
+    }
+    int rc = MPI_SUCCESS;
+    for (const auto& [t, how] : e.locked) {
+        int r = rmaComplete(*w, winId, rank, t, false);
+        rc = rc == MPI_SUCCESS ? r : rc;
+    }
+    return rc;
+}
+
+bool MpiWorld::winInPassiveEpoch(int rank, int winId)
+{
+    auto w = findWindow(winId);
+    return w != nullptr && rank >= 0 && rank < size && !w->epochs[rank].locked.empty();
+}
+
+std::string MpiWorld::serveRmaRequest(int call, const uint8_t* buffer, size_t bytes)
+{
+    RmaPassiveHeader h{};
+    if (bytes < sizeof(h)) {
+        return replyOf(RMA_REPLY_FAILED);
+    }
+    memcpy(&h, buffer, sizeof(h));
+    auto world = getMpiWorldRegistry().findWorld(h.worldId);
+    if (world == nullptr) {
+        SPDLOG_WARN("One-sided request for world {}, which this process does not know", h.worldId);
+        return replyOf(RMA_REPLY_NO_WINDOW);
+    }
+    try {
+        return world->rmaServe(call, buffer, bytes);
+    } catch (const std::exception& e) {
+        SPDLOG_ERROR("One-sided request from rank {} to rank {} failed: {}", h.origin, h.target, e.what());
+        return replyOf(RMA_REPLY_FAILED);
+    }
+}
+
+void MpiWorld::serveRmaGrant(const uint8_t* buffer, size_t bytes)
+{
+    uint64_t ticket = 0;
+    if (bytes != sizeof(ticket)) {
+        SPDLOG_ERROR("Malformed one-sided lock grant");
+        return;
+    }
+    memcpy(&ticket, buffer, sizeof(ticket));
+    GrantTable& g = grantTable();
+    {
+        std::lock_guard<std::mutex> lk(g.mx);
+        g.granted.insert(ticket);
+    }
+    g.cv.notify_all();
+}
+
+std::string MpiWorld::rmaServe(int call, const uint8_t* buffer, size_t bytes)
+{
+    using faabric::transport::PointToPointCall;
+    RmaPassiveHeader h{};
+    memcpy(&h, buffer, sizeof(h));
+    auto w = findWindow(h.winId);
+    if (w == nullptr || h.origin < 0 || h.origin >= size || h.target < 0 || h.target >= size || !isLocalRank(h.target)) {
+        SPDLOG_WARN("One-sided request for window {} of rank {} in world {}, which this process does not hold", h.winId, h.target, id);
+        return replyOf(RMA_REPLY_NO_WINDOW);
+    }
+    RmaLock& l = w->locks[h.target];
+    const bool exclusive = h.exclusive != 0;
+    if (call == PointToPointCall::RMA_LOCK) {
+        // Never wait here: a queued request is answered by a grant message
+        const std::string originHost = getHostForRank(h.origin);
+        std::lock_guard<std::mutex> lk(w->lockMx);
+        auto granted = std::make_shared<bool>(false);
+        l.waiters.push_back(RmaLockWaiter{ h.ticket, exclusive, granted, nullptr });
+        grantWaiters(l);
+        if (*granted) {
+            return replyOf(RMA_REPLY_OK);
+        }
+        const uint64_t ticket = h.ticket;
+        l.waiters.back().onGrant = [originHost, ticket] {
+            faabric::transport::getPointToPointClient(originHost)->rmaLockGrant((const uint8_t*)&ticket, sizeof(ticket));
+        };
+        return replyOf(RMA_REPLY_QUEUED);
+    }
+    if (call == PointToPointCall::RMA_LOCK_CANCEL) {
+        std::vector<std::function<void()>> sends;
+        {
+            std::lock_guard<std::mutex> lk(w->lockMx);
+            sends = dropWaiter(l, h.ticket) ? grantWaiters(l) : releaseLock(l, exclusive);
+        }
+        announceGrants(*w, sends);
+        return replyOf(RMA_REPLY_OK);
+    }
+    // Flush / unlock.  An unlock releases the lock even if its operations
+    // fail.
+    struct ReleaseAtExit
+    {
+        MpiWorld::RmaWindow& w;
+        RmaLock& l;
+        bool exclusive;
+        bool armed;
+        ~ReleaseAtExit()
+        {
+            if (!armed) {
+                return;
+            }
+            std::vector<std::function<void()>> sends;
+            {
+                std::lock_guard<std::mutex> lk(w.lockMx);
+                sends = releaseLock(l, exclusive);
+            }
+            announceGrants(w, sends);
+        }
+    } release{ *w, l, exclusive, call == PointToPointCall::RMA_UNLOCK };
+    // Check every operation, then apply them in order
+    struct Item
+    {
+        RmaWireOp wire;
+        const uint8_t* data;
+        size_t replyOff;
+    };
+    uint8_t* base = (uint8_t*)(uintptr_t)w->bases[h.target];
+    const uint64_t segBytes = (uint64_t)w->sizes[h.target];
+    std::vector<Item> items;
+    size_t off = sizeof(h), replyBytes = 0;
+    for (int i = 0; i < h.nOps; i++) {
+        Item it{ {}, nullptr, replyBytes };
+        if (bytes - off < sizeof(it.wire)) {
+            throw std::runtime_error("Truncated one-sided request");
+        }
+        memcpy(&it.wire, buffer + off, sizeof(it.wire));
+        off += sizeof(it.wire);
+        const RmaWireOp& wire = it.wire;
+        if (wire.bytes > segBytes || wire.dispBytes > segBytes - wire.bytes) {
+            throw std::runtime_error("Remote one-sided operation outside this rank's window");
+        }
+        const size_t dataBytes = wire.kind == RMA_PUT   ? wire.bytes
+                                 : wire.kind == RMA_GET ? 0
+                                                        : rmaAtomicPayload(wire.kind, wire.dtype, wire.op, wire.bytes, base + wire.dispBytes);
+        if (bytes - off < dataBytes) {
+            throw std::runtime_error("Truncated one-sided request");
+        }
+        it.data = buffer + off;
+        off += dataBytes;
+        if (wire.kind != RMA_PUT && wire.kind != RMA_ACCUMULATE) {
+            replyBytes += wire.bytes;
+        }
+        items.push_back(it);
+    }
+    std::string reply = replyOf(RMA_REPLY_OK);
+    reply.resize(sizeof(int32_t) + replyBytes);
+    uint8_t* out = (uint8_t*)reply.data() + sizeof(int32_t);
+    // Device work goes on this path's own streams, waited for before the reply
+    std::vector<std::pair<int, void*>> used;
+    auto copy = [&](uint8_t* dst, const uint8_t* src, size_t n) {
+        int device = bufferDevice(dst);
+        device = device == HOST_MEMORY ? bufferDevice(src) : device;
+        if (device == HOST_MEMORY) {
+            memcpy(dst, src, n);
+            return;
+        }
+        if (device == ANY_DEVICE) {
+            cudaCheck(cudaGetDevice(&device), "One-sided copy");
+        }
+        void* s = rmaStream(-1, device);
+        DeviceGuard on(device);
+        cudaCheck(cudaMemcpyAsync(dst, src, n, cudaMemcpyDefault, (cudaStream_t)s), "One-sided copy");
+        if (std::find(used.begin(), used.end(), std::make_pair(device, s)) == used.end()) {
+            used.emplace_back(device, s);
+        }
+    };
+    for (const Item& it : items) {
+        const RmaWireOp& wire = it.wire;
+        uint8_t* target = base + wire.dispBytes;
+        if (wire.kind == RMA_PUT) {
+            copy(target, it.data, wire.bytes);
+        } else if (wire.kind == RMA_GET) {
+            copy(out + it.replyOff, target, wire.bytes);
+        } else {
+            const bool cas = wire.kind == RMA_COMPARE_SWAP;
+            const size_t esize = fbDtypeSize(wire.dtype);
+            const bool hasData = cas || wire.op != FB_OP_NO_OP;
+            rmaApplyLocal(*w,
+                          h.target,
+                          h.target,
+                          target,
+                          wire.bytes / esize,
+                          wire.dtype,
+                          wire.op,
+                          hasData ? it.data : nullptr,
+                          cas ? it.data + esize : nullptr,
+                          wire.kind != RMA_ACCUMULATE ? out + it.replyOff : nullptr,
+                          used,
+                          true);
+        }
+    }
+    for (auto [device, s] : used) {
+        DeviceGuard on(device);
+        cudaCheck(cudaStreamSynchronize((cudaStream_t)s), "One-sided operation");
+    }
+    return reply;
 }
 
 }

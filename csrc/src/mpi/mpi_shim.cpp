@@ -18,6 +18,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <atomic>
 #include <cstring>
 #include <map>
 #include <stdexcept>
@@ -960,7 +961,94 @@ int MPI_Win_fence(int assert, MPI_Win win)
     if (win == nullptr) {
         return MPI_ERR_WIN;
     }
-    getExecutingWorld().winFence(executingContext.getRank(), win->id);
+    MpiWorld& world = getExecutingWorld();
+    if (world.winInPassiveEpoch(executingContext.getRank(), win->id)) {
+        return MPI_ERR_RMA_SYNC;
+    }
+    world.winFence(executingContext.getRank(), win->id);
+    return MPI_SUCCESS;
+}
+
+// ---- passive-target synchronisation; see MpiWorld::winLock ----
+int MPI_Win_lock(int lock_type, int rank, int assert, MPI_Win win)
+{
+    SPDLOG_TRACE("MPI - MPI_Win_lock");
+    if (win == nullptr) {
+        return MPI_ERR_WIN;
+    }
+    return getExecutingWorld().winLock(executingContext.getRank(), win->id, lock_type, rank, assert);
+}
+
+int MPI_Win_unlock(int rank, MPI_Win win)
+{
+    SPDLOG_TRACE("MPI - MPI_Win_unlock");
+    if (win == nullptr) {
+        return MPI_ERR_WIN;
+    }
+    return getExecutingWorld().winUnlock(executingContext.getRank(), win->id, rank);
+}
+
+int MPI_Win_lock_all(int assert, MPI_Win win)
+{
+    SPDLOG_TRACE("MPI - MPI_Win_lock_all");
+    if (win == nullptr) {
+        return MPI_ERR_WIN;
+    }
+    return getExecutingWorld().winLockAll(executingContext.getRank(), win->id, assert);
+}
+
+int MPI_Win_unlock_all(MPI_Win win)
+{
+    SPDLOG_TRACE("MPI - MPI_Win_unlock_all");
+    if (win == nullptr) {
+        return MPI_ERR_WIN;
+    }
+    return getExecutingWorld().winUnlockAll(executingContext.getRank(), win->id);
+}
+
+// (target -1: every target of the epoch)
+static int winFlush(int target, MPI_Win win)
+{
+    if (win == nullptr) {
+        return MPI_ERR_WIN;
+    }
+    return getExecutingWorld().winFlush(executingContext.getRank(), win->id, target);
+}
+
+int MPI_Win_flush(int rank, MPI_Win win)
+{
+    SPDLOG_TRACE("MPI - MPI_Win_flush");
+    return rank < 0 ? MPI_ERR_RANK : winFlush(rank, win);
+}
+
+int MPI_Win_flush_all(MPI_Win win)
+{
+    SPDLOG_TRACE("MPI - MPI_Win_flush_all");
+    return winFlush(-1, win);
+}
+
+// Completing at the target too is allowed: the local variants are the same
+int MPI_Win_flush_local(int rank, MPI_Win win)
+{
+    SPDLOG_TRACE("MPI - MPI_Win_flush_local");
+    return rank < 0 ? MPI_ERR_RANK : winFlush(rank, win);
+}
+
+int MPI_Win_flush_local_all(MPI_Win win)
+{
+    SPDLOG_TRACE("MPI - MPI_Win_flush_local_all");
+    return winFlush(-1, win);
+}
+
+// Loads and stores through MPI_Win_shared_query pointers before the call are
+// ordered before those after it
+int MPI_Win_sync(MPI_Win win)
+{
+    SPDLOG_TRACE("MPI - MPI_Win_sync");
+    if (win == nullptr) {
+        return MPI_ERR_WIN;
+    }
+    std::atomic_thread_fence(std::memory_order_seq_cst);
     return MPI_SUCCESS;
 }
 
@@ -1049,6 +1137,9 @@ int MPI_Win_free(MPI_Win* win)
     SPDLOG_TRACE("MPI - MPI_Win_free");
     if (win == nullptr || *win == nullptr) {
         return MPI_ERR_WIN;
+    }
+    if (getExecutingWorld().winInPassiveEpoch(executingContext.getRank(), (*win)->id)) {
+        return MPI_ERR_RMA_SYNC;
     }
     getExecutingWorld().winFree(executingContext.getRank(), (*win)->id);
     if ((*win)->ownedPtr != nullptr) {

@@ -6,6 +6,7 @@
 #include <faabric/util/logging.h>
 #include <faabric/util/testing.h>
 #include <faabric/device/communicator.h>
+#include <faabric/mpi/MpiWorld.h>
 #include <faabric/util/hwloc.h>
 
 #include <cuda_runtime.h>
@@ -149,6 +150,17 @@ void PointToPointClient::groupUnlock(int appId, int groupId, int groupIdx, bool 
                             groupIdx,
                             recursive ? PointToPointCall::UNLOCK_GROUP_RECURSIVE
                                       : PointToPointCall::UNLOCK_GROUP);
+}
+
+std::vector<uint8_t> PointToPointClient::rmaRequest(PointToPointCall call, const std::vector<uint8_t>& request)
+{
+    Message res = syncSendRaw(call, request.data(), request.size());
+    return std::vector<uint8_t>(res.udata().begin(), res.udata().end());
+}
+
+void PointToPointClient::rmaLockGrant(const uint8_t* buffer, size_t bytes)
+{
+    asyncSend(PointToPointCall::RMA_LOCK_GRANT, buffer, bytes);
 }
 
 static thread_local std::unordered_map<std::string, std::shared_ptr<PointToPointClient>>
@@ -864,6 +876,9 @@ void PointToPointServer::doAsyncRecv(transport::Message& message)
         case PointToPointCall::UNLOCK_GROUP_RECURSIVE:
             recvGroupUnlock(message.udata(), true);
             break;
+        case PointToPointCall::RMA_LOCK_GRANT:
+            faabric::mpi::MpiWorld::serveRmaGrant(message.udata().data(), message.udata().size());
+            break;
         default:
             SPDLOG_ERROR("Invalid async point-to-point header: {}", (int)header);
             throw std::runtime_error("Invalid async point-to-point message");
@@ -875,6 +890,10 @@ std::string PointToPointServer::doSyncRecv(transport::Message& message)
     uint8_t header = message.getMessageCode();
     if (header == PointToPointCall::MAPPING) {
         return doRecvMappings(message.udata());
+    }
+    if (header == PointToPointCall::RMA_LOCK || header == PointToPointCall::RMA_LOCK_CANCEL ||
+        header == PointToPointCall::RMA_FLUSH || header == PointToPointCall::RMA_UNLOCK) {
+        return faabric::mpi::MpiWorld::serveRmaRequest(header, message.udata().data(), message.udata().size());
     }
     SPDLOG_ERROR("Invalid sync point-to-point header: {}", (int)header);
     throw std::runtime_error("Invalid sync point-to-point message");
