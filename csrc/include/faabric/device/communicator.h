@@ -189,6 +189,10 @@ class Communicator
              int op,
              int flags,
              cudaStream_t s);
+    // Data movement.  Local (non-heap) destinations may sit at any alignment,
+    // different on every rank.  With FB_FLAG_SYMMETRIC, every rank passes
+    // the same kind of buffer at the same heap offset, outputs included: an
+    // all-gather output in the heap on one rank is in the heap on all.
     int broadcast(void* buf, size_t bytes, int root, int flags, cudaStream_t s);
     int allGather(const void* send,
                   void* recv,

@@ -1136,7 +1136,7 @@ const fb::KernelTable HOST_KERNELS = {
     .ll = fb::host::llAllReduce,
     .group = fb::host::groupAllReduce,
     .move = fb::host::moveKernel,
-    .moveBulk = nullptr,
+    .moveBulk = fb::host::moveBulk,
     .barrier = fb::host::barrierKernel,
     .p2pSend = fb::host::p2pSend,
     .p2pPull = fb::host::p2pPull,
@@ -2005,10 +2005,15 @@ int Communicator::moveLike(int mode,
 
     lastAlgo_ = FB_ALGO_ONESHOT;
     // ---- NVLS fast paths on symmetric buffers ----
+    // They move 16-byte vectors at the heap offsets of source and output.
+    // Whether the all-gather output lives in the heap is part of the call's
+    // contract, as for the reduce path's output: every rank passes the same
+    // kind of buffer, at the same offset, so every rank takes the same path.
     if (symmetric && hasMulticast() && (chunkBytes % 16) == 0 &&
         chunkBytes >= cfg_.nvlsMinBytes &&
-        ((mode == fb::MOVE_ALLGATHER && inHeap(recv, chunkBytes * n)) ||
-         mode == fb::MOVE_BCAST)) {
+        ((mode == fb::MOVE_ALLGATHER && inHeap(recv, chunkBytes * n) && (offsetOf(send) % 16) == 0 &&
+          (offsetOf(recv) % 16) == 0) ||
+         (mode == fb::MOVE_BCAST && (offsetOf(recv) % 16) == 0))) {
         fb::NvlsArgs a;
         memset(&a, 0, sizeof(a));
         a.comm = devFor(flags);
@@ -2043,9 +2048,10 @@ int Communicator::moveLike(int mode,
     }
 
     // ---- large symmetric broadcast: scatter + allgather in one kernel ----
-    // (it has a barrier between its two steps: not available in stream mode)
+    // (it has a barrier between its two steps: not available in stream mode;
+    // it copies 16-byte words at the buffer's heap offset)
     if (mode == fb::MOVE_BCAST && symmetric && !ss &&
-        chunkBytes >= cfg_.bcast2StepMinBytes && (chunkBytes % 16) == 0) {
+        chunkBytes >= cfg_.bcast2StepMinBytes && (chunkBytes % 16) == 0 && (offsetOf(recv) % 16) == 0) {
         fb::MoveArgs a;
         memset(&a, 0, sizeof(a));
         a.comm = devFor(flags);
@@ -2107,29 +2113,39 @@ int Communicator::moveLike(int mode,
                 stats_.stagedCopies++;
             }
         }
-        int width = std::min({ alignWidth((uint64_t)(uintptr_t)a.recvLocal),
-                               alignWidth(a.sendOff),
-                               alignWidth(len),
-                               alignWidth(a.dstStride),
-                               alignWidth(a.srcStride) });
-        uint64_t words = len / width;
-        cudaError_t ce;
-        if (ss && streamBarrier(flags, s) != FB_OK) {
-            return FB_E_CUDA;
-        }
-        if (k_->moveBulk != nullptr && width == 16 && cfg_.tmaMinBytes > 0 && len >= cfg_.tmaMinBytes &&
-            fb::moveBulkSupported(a)) {
+        // BlockBarrier pairs CTA i of every rank, so the grid, and whether the
+        // TMA kernel is eligible, come from values equal on every rank: the
+        // mode, the lengths, the strides and the source offset.  Only this
+        // rank's destination pointer may differ between ranks (gather passes
+        // none off the root); it narrows this rank's copy width, or sends a
+        // rank whose destination the TMA engine cannot address to the LDG/STG
+        // kernel with the same grid.  Both kernels run the same two barriers.
+        const int sharedWidth =
+          std::min({ alignWidth(a.sendOff), alignWidth(len), alignWidth(a.dstStride), alignWidth(a.srcStride) });
+        const int width = std::min(sharedWidth, alignWidth((uint64_t)(uintptr_t)a.recvLocal));
+        const bool bulk =
+          k_->moveBulk != nullptr && sharedWidth == 16 && cfg_.tmaMinBytes > 0 && len >= cfg_.tmaMinBytes;
+        int blocks;
+        if (bulk) {
             // Large chunks: the copy engine streams 32 KiB tiles through
             // shared memory; a few CTAs (>= 4 tiles each) saturate the link
             const uint64_t pieces =
               (mode == fb::MOVE_SCATTER || mode == fb::MOVE_BCAST) ? 1 : (uint64_t)n;
             const uint64_t tiles = pieces * ((len + 32767) / 32768);
             const int maxB = std::min(cfg_.maxBlocks, FB_MAX_BLOCKS / cfg_.channels);
-            const int blocks = (int)std::clamp<uint64_t>(tiles / 4, 1, (uint64_t)maxB);
+            blocks = (int)std::clamp<uint64_t>(tiles / 4, 1, (uint64_t)maxB);
+        } else {
+            blocks = blocksFor(len / sharedWidth, 2);
+        }
+        cudaError_t ce;
+        if (ss && streamBarrier(flags, s) != FB_OK) {
+            return FB_E_CUDA;
+        }
+        if (bulk && fb::moveBulkSupported(a)) {
             ce = k_->moveBulk(a, blocks, s);
             stats_.tmaLaunches++;
         } else {
-            ce = k_->move(a, width, blocksFor(words, 2), cfg_.threads, s);
+            ce = k_->move(a, width, blocks, cfg_.threads, s);
         }
         if (ce != cudaSuccess) {
             return FB_E_CUDA;

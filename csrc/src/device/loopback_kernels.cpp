@@ -494,51 +494,139 @@ cudaError_t groupAllReduce(const GroupArgs& a, int dtype, int op, int blocks, in
 }
 
 // ----------------------------------------------------------------- move ----
-cudaError_t moveKernel(const MoveArgs& a, int, int blocks, int, cudaStream_t)
+// The CUDA kernels copy in W-byte words.  Every address they touch that way
+// must be W-aligned (a misaligned vector access is a device fault), and every
+// length they copy that way a whole number of words (the kernels drop a
+// remainder).  The twins check the width they are given against the same
+// addresses before they copy, so a host decision that would fault on the GPU
+// fails here, with the error the CUDA launch would report.
+namespace {
+struct MoveCopy
+{
+    uint8_t* dst;
+    const uint8_t* src;
+    uint64_t bytes;
+};
+
+bool wordsOk(const void* p, int w)
+{
+    return ((uintptr_t)p % (uintptr_t)w) == 0;
+}
+
+bool copiesOk(const std::vector<MoveCopy>& cs, int w)
+{
+    for (const MoveCopy& m : cs) {
+        if (!wordsOk(m.dst, w) || !wordsOk(m.src, w) || m.bytes % (uint64_t)w != 0) {
+            return false;
+        }
+    }
+    return true;
+}
+
+void runCopies(const std::vector<MoveCopy>& cs)
+{
+    for (const MoveCopy& m : cs) {
+        memcpy(m.dst, m.src, m.bytes);
+    }
+}
+
+// The copies this rank makes in a one-step pull (moveKernel and moveBulkKernel)
+std::vector<MoveCopy> pullCopies(const MoveArgs& a)
+{
+    const FbCommDev& c = a.comm;
+    const int rank = c.rank;
+    std::vector<MoveCopy> cs;
+    if (a.mode == MOVE_ALLGATHER || a.mode == MOVE_ALLTOALL || (a.mode == MOVE_GATHER && rank == a.root)) {
+        const uint64_t srcExtra = (a.mode == MOVE_ALLTOALL) ? (uint64_t)rank * a.srcStride : 0;
+        for (int p = 0; p < c.nranks; p++) {
+            cs.push_back({ a.recvLocal + (uint64_t)p * a.dstStride, c.heap[p] + a.sendOff + srcExtra, a.chunkBytes });
+        }
+    } else if (a.mode == MOVE_SCATTER) {
+        cs.push_back({ a.recvLocal, c.heap[a.root] + a.sendOff + (uint64_t)rank * a.srcStride, a.chunkBytes });
+    } else if (a.mode == MOVE_BCAST && rank != a.root) {
+        cs.push_back({ a.recvLocal, c.heap[a.root] + a.sendOff, a.chunkBytes });
+    }
+    return cs;
+}
+
+// The copies of step 1 (this rank's slice from the root) or step 2 (every
+// other slice from its owner) of the two-step broadcast
+std::vector<MoveCopy> bcast2StepCopies(const MoveArgs& a, int step)
 {
     const FbCommDev& c = a.comm;
     const int rank = c.rank;
     const int n = c.nranks;
+    const uint64_t total = a.chunkBytes;
+    const uint64_t slice = ((total / n) + 15) & ~(uint64_t)15;
+    auto bounds = [&](int p, uint64_t& b, uint64_t& e) {
+        b = std::min<uint64_t>((uint64_t)p * slice, total);
+        e = (p == n - 1) ? total : std::min<uint64_t>(b + slice, total);
+    };
+    std::vector<MoveCopy> cs;
+    if (rank == a.root) {
+        return cs;
+    }
+    uint64_t b, e;
+    if (step == 1) {
+        bounds(rank, b, e);
+        if (e > b) {
+            cs.push_back({ c.heap[rank] + a.recvOff + b, c.heap[a.root] + a.sendOff + b, e - b });
+        }
+        return cs;
+    }
+    for (int q = 1; q < n; q++) {
+        int p = (rank + q) % n;
+        bounds(p, b, e);
+        if (e <= b) {
+            continue;
+        }
+        const uint8_t* src = (p == a.root) ? c.heap[p] + a.sendOff + b : c.heap[p] + a.recvOff + b;
+        cs.push_back({ c.heap[rank] + a.recvOff + b, src, e - b });
+    }
+    return cs;
+}
+
+// barrier, copies, barrier: the protocol of both one-step pull kernels
+cudaError_t runPull(const MoveArgs& a, const std::vector<MoveCopy>& cs, int blocks)
+{
+    bool ok = true;
+    if (!a.noSync) {
+        ok = gridBarrier(a.comm, blocks);
+    }
+    if (ok) {
+        runCopies(cs);
+    }
+    if (!a.noSync) {
+        gridBarrier(a.comm, blocks);
+    }
+    return cudaSuccess;
+}
+}
+
+cudaError_t moveKernel(const MoveArgs& a, int width, int blocks, int, cudaStream_t)
+{
+    if (a.mode != MOVE_BCAST_2STEP) {
+        const std::vector<MoveCopy> cs = pullCopies(a);
+        if (!copiesOk(cs, width)) {
+            return cudaErrorMisalignedAddress;
+        }
+        return runPull(a, cs, blocks);
+    }
+    const std::vector<MoveCopy> step1 = bcast2StepCopies(a, 1);
+    const std::vector<MoveCopy> step2 = bcast2StepCopies(a, 2);
+    if (!copiesOk(step1, width) || !copiesOk(step2, width)) {
+        return cudaErrorMisalignedAddress;
+    }
+    const FbCommDev& c = a.comm;
     bool ok = true;
     if (!a.noSync) {
         ok = gridBarrier(c, blocks);
     }
     if (ok) {
-        if (a.mode == MOVE_ALLGATHER || a.mode == MOVE_ALLTOALL || (a.mode == MOVE_GATHER && rank == a.root)) {
-            const uint64_t srcExtra = (a.mode == MOVE_ALLTOALL) ? (uint64_t)rank * a.srcStride : 0;
-            for (int p = 0; p < n; p++) {
-                memcpy(a.recvLocal + (uint64_t)p * a.dstStride, c.heap[p] + a.sendOff + srcExtra, a.chunkBytes);
-            }
-        } else if (a.mode == MOVE_SCATTER) {
-            memcpy(a.recvLocal, c.heap[a.root] + a.sendOff + (uint64_t)rank * a.srcStride, a.chunkBytes);
-        } else if (a.mode == MOVE_BCAST) {
-            if (rank != a.root) {
-                memcpy(a.recvLocal, c.heap[a.root] + a.sendOff, a.chunkBytes);
-            }
-        } else if (a.mode == MOVE_BCAST_2STEP) {
-            const uint64_t total = a.chunkBytes;
-            uint64_t slice = ((total / n) + 15) & ~(uint64_t)15;
-            auto bounds = [&](int p, uint64_t& b, uint64_t& e) {
-                b = std::min<uint64_t>((uint64_t)p * slice, total);
-                e = (p == n - 1) ? total : std::min<uint64_t>(b + slice, total);
-            };
-            uint64_t b, e;
-            bounds(rank, b, e);
-            if (rank != a.root && e > b) {
-                memcpy(c.heap[rank] + a.recvOff + b, c.heap[a.root] + a.sendOff + b, e - b);
-            }
-            ok = a.noSync ? true : gridBarrier(c, blocks);
-            if (ok && rank != a.root) {
-                for (int q = 1; q < n; q++) {
-                    int p = (rank + q) % n;
-                    bounds(p, b, e);
-                    if (e <= b) {
-                        continue;
-                    }
-                    const uint8_t* src = (p == a.root) ? c.heap[p] + a.sendOff + b : c.heap[p] + a.recvOff + b;
-                    memcpy(c.heap[rank] + a.recvOff + b, src, e - b);
-                }
-            }
+        runCopies(step1);
+        ok = a.noSync ? true : gridBarrier(c, blocks);
+        if (ok) {
+            runCopies(step2);
         }
     }
     if (!a.noSync) {
@@ -547,15 +635,38 @@ cudaError_t moveKernel(const MoveArgs& a, int, int blocks, int, cudaStream_t)
     return cudaSuccess;
 }
 
+cudaError_t moveBulk(const MoveArgs& a, int blocks, cudaStream_t)
+{
+    // cp.async.bulk moves 16-byte aligned ranges of whole 16-byte units
+    if (!moveBulkSupported(a)) {
+        return cudaErrorMisalignedAddress;
+    }
+    const std::vector<MoveCopy> cs = pullCopies(a);
+    if (!copiesOk(cs, 16)) {
+        return cudaErrorMisalignedAddress;
+    }
+    return runPull(a, cs, blocks);
+}
+
 cudaError_t barrierKernel(const FbCommDev& c, cudaStream_t)
 {
     return blockBarrier(c, 0) ? cudaSuccess : cudaErrorUnknown;
 }
 
 // ------------------------------------------------------------------ p2p ----
-cudaError_t p2pSend(const P2PArgs& a, int, int, cudaStream_t)
+// The p2p and put kernels copy bytes - bytes % W in W-byte words, then the
+// tail byte by byte: with no whole word they touch nothing as a word
+static bool p2pWordsOk(const void* dst, const void* src, uint64_t bytes, int w)
+{
+    return bytes < (uint64_t)w || (wordsOk(dst, w) && wordsOk(src, w));
+}
+
+cudaError_t p2pSend(const P2PArgs& a, int width, int, cudaStream_t)
 {
     const FbCommDev& c = a.comm;
+    if (a.stage && !p2pWordsOk(c.heap[c.rank] + a.srcOff, a.local, a.bytes, width)) {
+        return cudaErrorMisalignedAddress;
+    }
     if (a.stage && a.bytes > 0) {
         memcpy(c.heap[c.rank] + a.srcOff, a.local, a.bytes);
     }
@@ -569,7 +680,7 @@ cudaError_t p2pSend(const P2PArgs& a, int, int, cudaStream_t)
     return cudaSuccess;
 }
 
-cudaError_t p2pPull(const P2PArgs& a, int, int, cudaStream_t)
+cudaError_t p2pPull(const P2PArgs& a, int width, int, cudaStream_t)
 {
     const FbCommDev& c = a.comm;
     const uint32_t seen = ldAcquire(c.sig[c.rank] + FB_P2P_READY_OFF + a.peer);
@@ -583,6 +694,9 @@ cudaError_t p2pPull(const P2PArgs& a, int, int, cudaStream_t)
         }
         len = 0;
     }
+    if (!p2pWordsOk(a.local, c.heap[a.peer] + srcOff, len, width)) {
+        return cudaErrorMisalignedAddress;
+    }
     if (len > 0) {
         memcpy(a.local, c.heap[a.peer] + srcOff, len);
     }
@@ -590,9 +704,12 @@ cudaError_t p2pPull(const P2PArgs& a, int, int, cudaStream_t)
     return cudaSuccess;
 }
 
-cudaError_t putSignal(const PutArgs& a, int, int blocks, cudaStream_t)
+cudaError_t putSignal(const PutArgs& a, int width, int blocks, cudaStream_t)
 {
     const FbCommDev& c = a.comm;
+    if (!p2pWordsOk(c.heap[a.peer] + a.dstOff, a.local, a.bytes, width)) {
+        return cudaErrorMisalignedAddress;
+    }
     if (a.bytes > 0) {
         memcpy(c.heap[a.peer] + a.dstOff, a.local, a.bytes);
     }

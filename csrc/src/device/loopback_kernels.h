@@ -17,7 +17,7 @@ struct KernelTable
     cudaError_t (*ll)(const LLArgs& a, int dtype, int op, cudaStream_t s);
     cudaError_t (*group)(const GroupArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s);
     cudaError_t (*move)(const MoveArgs& a, int width, int blocks, int threads, cudaStream_t s);
-    // TMA bulk-copy engine; null on the host
+    // TMA bulk-copy engine (fixed block size, 16-byte aligned ranges)
     cudaError_t (*moveBulk)(const MoveArgs& a, int blocks, cudaStream_t s);
     cudaError_t (*barrier)(const FbCommDev& c, cudaStream_t s);
     cudaError_t (*p2pSend)(const P2PArgs& a, int width, int blocks, cudaStream_t s);
@@ -49,7 +49,11 @@ bool reducible(int dtype, int op);
 cudaError_t reduceKernel(const ReduceArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s);
 cudaError_t llAllReduce(const LLArgs& a, int dtype, int op, cudaStream_t s);
 cudaError_t groupAllReduce(const GroupArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s); // a.segs: HOST memory
+// The move, p2p and put twins return cudaErrorMisalignedAddress, before they
+// copy or synchronise, when an address the kernel reads or writes in words of
+// `width` bytes is not aligned to it (moveBulk: 16 bytes)
 cudaError_t moveKernel(const MoveArgs& a, int width, int blocks, int threads, cudaStream_t s);
+cudaError_t moveBulk(const MoveArgs& a, int blocks, cudaStream_t s);
 cudaError_t barrierKernel(const FbCommDev& c, cudaStream_t s);
 cudaError_t p2pSend(const P2PArgs& a, int width, int blocks, cudaStream_t s);
 cudaError_t p2pPull(const P2PArgs& a, int width, int blocks, cudaStream_t s);

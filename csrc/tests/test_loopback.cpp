@@ -451,6 +451,319 @@ TEST_CASE("loopback: data movement collectives, staged pieces and the two-step b
     }
 }
 
+// ---------------------------------------------------------------------------
+// Pull collectives whose ranks' destinations differ in alignment.  BlockBarrier
+// pairs CTA i of every rank, so every rank must launch the same number of CTAs
+// (and kernels) whatever its own pointer; a rank that launches more waits for
+// CTAs that never come.  The host twins check the copy width they are given,
+// so a width the CUDA kernel could not use fails here too.
+// ---------------------------------------------------------------------------
+namespace {
+// bytes past a 16-byte boundary of rank r's destination: MISALIGN[r % 5]
+const size_t MISALIGN[] = { 0, 4, 1, 12, 8 };
+
+uint8_t movePat(int rank, size_t i)
+{
+    return (uint8_t)(((uint32_t)i * 2654435761u + (uint32_t)rank * 40503u + 17u) >> 13);
+}
+
+// `bytes` at `misalign` bytes past a 16-byte boundary, between sentinel bytes
+struct Guarded
+{
+    std::vector<uint8_t> store;
+    uint8_t* p;
+    size_t bytes;
+
+    Guarded(size_t bytes, size_t misalign)
+      : store(bytes + 64, 0xa5)
+      , bytes(bytes)
+    {
+        p = reinterpret_cast<uint8_t*>(((uintptr_t)store.data() + 31) & ~(uintptr_t)15) + misalign;
+    }
+
+    bool guardsIntact() const
+    {
+        for (const uint8_t* q = store.data(); q < store.data() + store.size(); q++) {
+            if ((q < p || q >= p + bytes) && *q != 0xa5) {
+                return false;
+            }
+        }
+        return true;
+    }
+};
+
+enum MoveKind
+{
+    MK_ALLGATHER,
+    MK_ALLTOALL,
+    MK_GATHER,
+    MK_SCATTER,
+    MK_BCAST,
+};
+const char* const MOVE_NAMES[] = { "allGather", "allToAll", "gather", "scatter", "broadcast" };
+
+// One pull collective of `per` bytes per rank (pair), sources in the heap
+// (`symmetric`) or in local memory (staged), every destination at its rank's
+// MISALIGN; gather passes a destination on the root only.  Checks the return
+// code, the error word, every destination byte and the sentinels around it.
+// Every rank makes every call, failed or not, so a failure cannot leave the
+// other ranks waiting in hostBarrier.
+bool divergentMove(int rank, Communicator& c, MoveKind kind, size_t per, bool symmetric, int root)
+{
+    const int n = c.size();
+    const size_t srcRows = (kind == MK_ALLTOALL || kind == MK_SCATTER) ? n : 1;
+    const size_t dstBytes = (kind == MK_SCATTER || kind == MK_BCAST) ? per : per * n;
+    const int flags = symmetric ? FB_FLAG_SYMMETRIC : 0;
+    Guarded dst(dstBytes, MISALIGN[rank % 5]);
+    Guarded localSrc(per * srcRows, 0);
+    uint64_t symOff = 0;
+    uint8_t* src = localSrc.p;
+    if (symmetric) {
+        symOff = c.alloc(per * srcRows);
+        src = c.heapPtr(symOff);
+    }
+    for (size_t i = 0; i < per * srcRows; i++) {
+        src[i] = movePat(rank, i);
+    }
+    if (kind == MK_BCAST && rank == root) {
+        memcpy(dst.p, src, per);
+    }
+    c.hostBarrier();
+    int rc = FB_E_INVALID;
+    switch (kind) {
+        case MK_ALLGATHER:
+            rc = c.allGather(src, dst.p, per, flags, nullptr);
+            break;
+        case MK_ALLTOALL:
+            rc = c.allToAll(src, dst.p, per, flags, nullptr);
+            break;
+        case MK_GATHER:
+            rc = c.gather(src, rank == root ? dst.p : nullptr, per, root, flags, nullptr);
+            break;
+        case MK_SCATTER:
+            rc = c.scatter(src, dst.p, per, root, flags, nullptr);
+            break;
+        case MK_BCAST:
+            rc = c.broadcast(dst.p, per, root, 0, nullptr);
+            break;
+    }
+    const uint32_t err = c.checkError(nullptr);
+    bool ok = rc == FB_OK && err == 0 && dst.guardsIntact();
+    for (size_t i = 0; i < dstBytes && ok; i++) {
+        const size_t p = i / per;
+        const size_t k = i % per;
+        uint8_t want = dst.p[i];
+        switch (kind) {
+            case MK_ALLGATHER:
+                want = movePat((int)p, k);
+                break;
+            case MK_ALLTOALL:
+                want = movePat((int)p, (size_t)rank * per + k);
+                break;
+            case MK_GATHER:
+                want = rank == root ? movePat((int)p, k) : 0xa5;
+                break;
+            case MK_SCATTER:
+                want = movePat(root, (size_t)rank * per + i);
+                break;
+            case MK_BCAST:
+                want = movePat(root, i);
+                break;
+        }
+        ok = dst.p[i] == want;
+    }
+    if (!ok) {
+        printf("         rank %d %s of %zu bytes (%s, root %d): rc %d, error word %u\n", rank, MOVE_NAMES[kind], per,
+               symmetric ? "symmetric" : "staged", root, rc, err);
+    }
+    c.hostBarrier();
+    if (symmetric) {
+        c.free(symOff);
+    }
+    return ok;
+}
+}
+
+TEST_CASE("loopback: pull collectives launch one grid when ranks' destinations differ in alignment", "[loopback]")
+{
+    // 8 KiB takes one CTA with 16-byte words and two or more with narrower
+    // ones; with tmaMinBytes = 4 KiB, aligned ranks take the TMA kernel and
+    // the others cannot (its grid is sized from tiles)
+    for (int n : { 2, 3, 4 }) {
+        for (size_t tmaMin : { (size_t)256 << 10, (size_t)4096 }) {
+            LoopGroup g(n);
+            int fails = g.run([&](int rank, Communicator& c) {
+                c.config().maxBlocks = 16;
+                c.config().tmaMinBytes = tmaMin;
+                const uint64_t tmaBefore = c.stats().tmaLaunches;
+                bool ok = true;
+                for (size_t per : { (size_t)8192, (size_t)40016 }) {
+                    for (bool symmetric : { false, true }) {
+                        for (int k = MK_ALLGATHER; k <= MK_BCAST; k++) {
+                            if (symmetric && k == MK_BCAST) {
+                                continue; // a symmetric buffer sits at one offset on every rank
+                            }
+                            ok = divergentMove(rank, c, (MoveKind)k, per, symmetric, n - 1) && ok;
+                        }
+                    }
+                }
+                // rank 0's destinations are aligned: it really ran the TMA twin
+                if (ok && rank == 0 && tmaMin == 4096) {
+                    ok = c.stats().tmaLaunches > tmaBefore;
+                }
+                return ok;
+            });
+            if (fails != 0) {
+                printf("         n %d, tmaMinBytes %zu\n", n, tmaMin);
+            }
+            REQUIRE_EQ(fails, 0);
+        }
+    }
+}
+
+TEST_CASE("loopback: staged pieces stay in step when ranks' destinations differ in alignment", "[loopback]")
+{
+    // 64 KiB of staging: 100000 and 100004 bytes per rank pair take several
+    // pieces; with 100004 the last one is not a multiple of 16 bytes
+    for (int n : { 2, 3, 4 }) {
+        LoopGroup g(n, 4, (size_t)64 << 10);
+        int fails = g.run([&](int rank, Communicator& c) {
+            c.config().maxBlocks = 16;
+            const uint64_t stagedBefore = c.stats().stagedCopies;
+            bool ok = true;
+            for (size_t per : { (size_t)100000, (size_t)100004 }) {
+                for (int k = MK_ALLGATHER; k <= MK_BCAST; k++) {
+                    ok = divergentMove(rank, c, (MoveKind)k, per, false, (int)(per % 3) % n) && ok;
+                }
+            }
+            return ok && c.stats().stagedCopies > stagedBefore;
+        });
+        if (fails != 0) {
+            printf("         n %d\n", n);
+        }
+        REQUIRE_EQ(fails, 0);
+    }
+}
+
+TEST_CASE("loopback: the two-step broadcast only runs on 16-byte aligned heap offsets", "[loopback]")
+{
+    // (total, heap offset mod 16, bcast2StepMinBytes): 16 and 48 bytes give
+    // empty and uneven slices; the two-step kernel moves 16-byte words
+    struct Case
+    {
+        size_t total;
+        size_t misalign;
+        size_t minBytes;
+    };
+    const Case cases[] = {
+        { ((size_t)1 << 20) + 16, 4, (size_t)1 << 20 },  { ((size_t)1 << 20) + 16, 0, (size_t)1 << 20 },
+        { ((size_t)1 << 20) + 48, 8, (size_t)1 << 20 },   { 16, 0, 16 },
+        { 48, 0, 16 },                                    { 4096 + 16, 0, 16 },
+        { 4096 + 16, 12, 16 },                            { ((size_t)1 << 20) + 16 * 5, 0, 16 },
+    };
+    for (int n : { 4, 3, 5 }) {
+        LoopGroup g(n);
+        int fails = g.run([&](int rank, Communicator& c) {
+            bool ok = true;
+            for (const Case& cs : cases) {
+                c.config().bcast2StepMinBytes = cs.minBytes;
+                const int root = (int)(cs.total / 16) % c.size();
+                const uint64_t off = c.alloc(cs.total + 64);
+                uint8_t* base = c.heapPtr(off);
+                uint8_t* buf = base + 16 + cs.misalign;
+                memset(base, 0xa5, cs.total + 64);
+                if (rank == root) {
+                    for (size_t i = 0; i < cs.total; i++) {
+                        buf[i] = movePat(root, i);
+                    }
+                }
+                c.hostBarrier();
+                const int rc = c.broadcast(buf, cs.total, root, FB_FLAG_SYMMETRIC, nullptr);
+                const bool twoStep = c.lastAlgo() == FB_ALGO_TWOSHOT;
+                bool good = rc == FB_OK && c.checkError(nullptr) == 0 && twoStep == (cs.misalign == 0);
+                for (size_t i = 0; i < cs.total + 64 && good; i++) {
+                    const uint8_t* q = base + i;
+                    good = *q == ((q >= buf && q < buf + cs.total) ? movePat(root, (size_t)(q - buf)) : 0xa5);
+                }
+                if (!good) {
+                    printf("         rank %d broadcast of %zu bytes at heap offset +%zu: rc %d, two-step %d\n", rank,
+                           cs.total, cs.misalign, rc, (int)twoStep);
+                }
+                ok = ok && good;
+                c.hostBarrier();
+                c.free(off);
+            }
+            return ok;
+        });
+        if (fails != 0) {
+            printf("         n %d\n", n);
+        }
+        REQUIRE_EQ(fails, 0);
+    }
+}
+
+TEST_CASE("loopback: point-to-point and put-with-signal at every local alignment", "[loopback]")
+{
+    LoopGroup g(3);
+    int fails = g.run([&](int rank, Communicator& c) {
+        const int n = c.size();
+        const int next = (rank + 1) % n;
+        const int prev = (rank + n - 1) % n;
+        // the bounce slot (largest eager chunk) is half the 1 MiB ring
+        const size_t slot = (size_t)512 << 10;
+        bool ok = true;
+        for (size_t misalign : { 0, 1, 4, 12 }) {
+            for (size_t bytes : { (size_t)0, (size_t)1, (size_t)15, (size_t)16, (size_t)17, slot - 1, slot, slot + 1 }) {
+                Guarded out(bytes, misalign);
+                Guarded in(bytes, (misalign * 3) % 16);
+                Guarded in2(bytes, (misalign + 1) % 16);
+                for (size_t i = 0; i < bytes; i++) {
+                    out.p[i] = movePat(rank, i + bytes);
+                }
+                int rc = c.send(out.p, bytes, next, nullptr);
+                rc = rc == FB_OK ? c.recv(in.p, bytes, prev, nullptr) : rc;
+                rc = rc == FB_OK ? c.sendRecv(out.p, bytes, next, in2.p, bytes, prev, nullptr) : rc;
+                bool good = rc == FB_OK && c.checkError(nullptr) == 0 && in.guardsIntact() && in2.guardsIntact();
+                for (size_t i = 0; i < bytes && good; i++) {
+                    good = in.p[i] == movePat(prev, i + bytes) && in2.p[i] == movePat(prev, i + bytes);
+                }
+                if (!good) {
+                    printf("         rank %d p2p of %zu bytes at +%zu: rc %d\n", rank, bytes, misalign, rc);
+                }
+                ok = ok && good;
+            }
+        }
+        // put-with-signal into a symmetric destination at an odd heap offset
+        for (size_t misalign : { 0, 1, 4, 12 }) {
+            for (size_t bytes : { (size_t)1, (size_t)17, (size_t)4099 }) {
+                const uint64_t off = c.alloc(bytes + 64);
+                uint8_t* base = c.heapPtr(off);
+                memset(base, 0xa5, bytes + 64);
+                Guarded out(bytes, (misalign + 4) % 16);
+                for (size_t i = 0; i < bytes; i++) {
+                    out.p[i] = movePat(rank, i);
+                }
+                c.hostBarrier();
+                int rc = c.putSignal(out.p, off + 16 + misalign, bytes, next, 7, 2, nullptr);
+                rc = rc == FB_OK ? c.waitSignal(7, 2, nullptr) : rc;
+                bool good = rc == FB_OK && c.checkError(nullptr) == 0;
+                for (size_t i = 0; i < bytes + 64 && good; i++) {
+                    const bool inside = i >= 16 + misalign && i < 16 + misalign + bytes;
+                    good = base[i] == (inside ? movePat(prev, i - 16 - misalign) : 0xa5);
+                }
+                if (!good) {
+                    printf("         rank %d put of %zu bytes at heap +%zu: rc %d\n", rank, bytes, misalign, rc);
+                }
+                ok = ok && good;
+                c.hostBarrier();
+                c.free(off);
+            }
+        }
+        return ok;
+    });
+    REQUIRE_EQ(fails, 0);
+}
+
 TEST_CASE("loopback: grouped all-reduce equals per-tensor all-reduces", "[loopback]")
 {
     const std::vector<size_t> sizes = { 1, 3, 4, 7, 64, 1000, 4099, 65541, 9408, 2, 33, 300000 };
