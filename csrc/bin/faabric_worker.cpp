@@ -25,6 +25,7 @@
 
 #include "../tests/mpi_rma_atomics_body.h"
 #include "../tests/mpi_rma_passive_body.h"
+#include "../tests/mpi_subcomm_device_body.h"
 
 #include <cuda_runtime.h>
 
@@ -754,6 +755,101 @@ static void registerFunctions()
             msg.set_outputdata(why);
         }
         return rc;
+    });
+
+    // Fused device collectives on sub-communicators (mpi_subcomm_device_body.h).
+    // Input: "heap" (symmetric heap buffers) or "cuda" (cudaMalloc buffers).
+    mpiFunction("subcomm-device", [](int rank, int size, faabric::Message& msg) {
+        subcomm_device::Setup s;
+        s.memory = msg.inputdata().rfind("cuda", 0) == 0 ? subcomm_device::BufferMemory::CudaMalloc
+                                                          : subcomm_device::BufferMemory::Heap;
+        std::string why;
+        int rc = subcomm_device::body(rank, size, msg.mpiworldid(), s, &why);
+        if (rc != 0) {
+            SPDLOG_ERROR("subcomm-device: {}", why);
+            msg.set_outputdata(why);
+        }
+        return rc;
+    });
+
+    // MPI_Allreduce (float32 SUM) on symmetric-heap buffers.  Input:
+    // "<mode>;<bytes>;<iters>" with mode
+    //   fused  on the half communicator of this rank (ranks [0, size/2) and
+    //          [size/2, size)): the fused kernels on a signal slot
+    //   host   the same, after FB_SUB_SLOTS world splits have taken every slot:
+    //          the point-to-point host path
+    //   world  on MPI_COMM_WORLD
+    // Rank 0 reports {"us_per_call", "device_calls"}: the device collectives
+    // of rank 0's process per timed call (one per rank of the process when the
+    // call is fused, 0 on the host path).
+    mpiFunction("bench-subcomm", [](int rank, int size, faabric::Message& msg) {
+        std::vector<std::string> f;
+        std::string cur;
+        for (char c : msg.inputdata() + ";") {
+            if (c == ';') {
+                f.push_back(cur);
+                cur.clear();
+            } else {
+                cur += c;
+            }
+        }
+        EXPECT(f.size() >= 3 && size >= 2);
+        const std::string mode = f[0];
+        const size_t bytes = std::stoul(f[1]);
+        const int iters = std::stoi(f[2]);
+        const int count = (int)(bytes / 4);
+        faabric::mpi::MpiWorld& world = faabric::mpi::getMpiWorldRegistry().getWorld(msg.mpiworldid());
+        float* send = nullptr;
+        float* recv = nullptr;
+        EXPECT(MPI_Alloc_mem(bytes, MPI_INFO_FAABRIC_DEVICE, &send) == MPI_SUCCESS);
+        EXPECT(MPI_Alloc_mem(bytes, MPI_INFO_FAABRIC_DEVICE, &recv) == MPI_SUCCESS);
+        std::vector<float> ones(count, 1.0f);
+        cudaMemcpy(send, ones.data(), bytes, cudaMemcpyHostToDevice);
+        std::vector<MPI_Comm> fill;
+        if (mode == "host") {
+            for (int i = 0; i < FB_SUB_SLOTS; i++) {
+                MPI_Comm c = MPI_COMM_NULL;
+                MPI_Comm_split(MPI_COMM_WORLD, 0, rank, &c);
+                // (a device call: takes a slot)
+                EXPECT(MPI_Allreduce(send, recv, 4, MPI_FLOAT, MPI_SUM, c) == MPI_SUCCESS);
+                fill.push_back(c);
+            }
+        }
+        MPI_Comm comm = MPI_COMM_WORLD;
+        if (mode != "world") {
+            MPI_Comm_split(MPI_COMM_WORLD, rank / (size / 2), rank, &comm);
+        }
+        int n = 0;
+        MPI_Comm_size(comm, &n);
+        for (int i = 0; i < 3; i++) {
+            EXPECT(MPI_Allreduce(send, recv, count, MPI_FLOAT, MPI_SUM, comm) == MPI_SUCCESS);
+        }
+        std::vector<float> out(count);
+        cudaMemcpy(out.data(), recv, bytes, cudaMemcpyDeviceToHost);
+        EXPECT(out[0] == (float)n && out[count - 1] == (float)n);
+        MPI_Barrier(MPI_COMM_WORLD);
+        const uint64_t before = world.getDeviceCollectiveCount();
+        MPI_Barrier(MPI_COMM_WORLD);
+        auto t0 = std::chrono::steady_clock::now();
+        for (int i = 0; i < iters; i++) {
+            EXPECT(MPI_Allreduce(send, recv, count, MPI_FLOAT, MPI_SUM, comm) == MPI_SUCCESS);
+        }
+        const double us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count() / iters;
+        MPI_Barrier(MPI_COMM_WORLD);
+        const uint64_t calls = world.getDeviceCollectiveCount() - before;
+        if (rank == 0) {
+            msg.set_outputdata("{\"us_per_call\": " + std::to_string(us) +
+                               ", \"device_calls\": " + std::to_string((double)calls / iters) + "}");
+        }
+        if (comm != MPI_COMM_WORLD) {
+            MPI_Comm_free(&comm);
+        }
+        for (MPI_Comm& c : fill) {
+            MPI_Comm_free(&c);
+        }
+        MPI_Free_mem(send);
+        MPI_Free_mem(recv);
+        return 0;
     });
 
     // Cost of the MPI one-sided atomics, rank 0 onto rank 1's window, each

@@ -335,7 +335,40 @@ int64_t fb_comm_alloc(void* h, uint64_t bytes)
 
 void fb_comm_free(void* h, uint64_t off)
 {
-    COMM(h)->free(off);
+    try {
+        COMM(h)->free(off);
+    } catch (const std::exception& e) {
+        g_lastError = e.what();
+    }
+}
+
+// A communicator over `members` (ranks of `h`, in child order) using signal
+// slot `slot`; null on failure (fb_last_error).  Release with fb_comm_destroy
+// once the child's last collective has completed: it zeroes the slot pad
+// without waiting for the caller's streams.
+void* fb_comm_subset(void* h, const int* members, int n, int slot)
+{
+    FB_TRY
+    int rc = FB_OK;
+    auto child = COMM(h)->subset(std::vector<int>(members, members + std::max(n, 0)), slot, &rc);
+    if (child == nullptr) {
+        g_lastError = std::string("subset: ") + Communicator::errorString(rc);
+        return nullptr;
+    }
+    auto* c = new FbCommHandle();
+    c->comm = std::move(child);
+    return c;
+    FB_CATCH(nullptr)
+}
+
+uint32_t fb_comm_free_subset_slots(void* h)
+{
+    return COMM(h)->freeSubsetSlots();
+}
+
+int fb_comm_is_subset(void* h)
+{
+    return COMM(h)->isSubset() ? 1 : 0;
 }
 
 void* fb_comm_heap_ptr(void* h, uint64_t off, int rank)

@@ -59,6 +59,23 @@ extern "C" {
 #define FB_SIG_SBAR_WORDS (FB_MAX_CHANNELS * FB_MAX_RANKS)
 #define FB_SIG_TOTAL_WORDS 4096
 #define FB_SIG_BYTES (FB_SIG_TOTAL_WORDS * 4)
+// Sub-communicator slots.  Each rank's signal region holds its own pad
+// followed by FB_SUB_SLOTS more pads of FB_SIG_BYTES: slot s of rank p starts
+// at sig[p] + (s + 1) * FB_SIG_TOTAL_WORDS.  A communicator over a subset of
+// the ranks (Communicator::subset) uses one slot on every member as its pads,
+// so its barrier epochs never mix with the parent's or another child's.
+//
+// Zeroing invariant: a slot pad is zeroed once when the region is created and
+// then by its owner when the owner releases the slot, never when a child is
+// created.  This is correct because every word a peer writes into a rank's
+// pad during a collective is awaited by that rank in the same collective (the
+// in-kernel flag barriers, the per-block epoch words, which only the owner
+// writes, and the stream-ordered barrier: signalPeers + a wait per peer).  So
+// once a rank's last collective on the child has completed, no peer write to
+// its pad is pending, and a free slot is all zeros.  A member that creates its
+// child early may therefore signal a peer that has not created its own yet:
+// zeroing at creation would wipe that signal.
+#define FB_SUB_SLOTS 15
 
 // Error word values written by device watchdogs
 #define FB_ERR_NONE 0u

@@ -13,6 +13,7 @@
 
 #include <cuda_runtime.h>
 
+#include <atomic>
 #include <cstdint>
 #include <cstddef>
 #include <deque>
@@ -117,7 +118,7 @@ struct CommStats
     uint64_t tmaLaunches = 0;
 };
 
-class Communicator
+class Communicator : public std::enable_shared_from_this<Communicator>
 {
   public:
     ~Communicator();
@@ -132,6 +133,31 @@ class Communicator
                                                    int device,
                                                    const std::string& jobId,
                                                    const CommConfig& cfg);
+
+    // ---- sub-communicators ----
+    // Local call: no communication, no allocation.  `members` are ranks of this
+    // communicator, in the order that becomes the child's rank order; this rank
+    // must be one of them.  Every member must pass the same list and slot.
+    // The child runs the same fused kernels over the members' heaps, with slot
+    // `slot` of every member's signal region as its pads (comm_abi.h).  It
+    // supports allReduce (one-shot and two-shot only), reduce, reduceScatter,
+    // scan, the data-movement collectives, barrier and the heap queries, with
+    // child ranks.  Point to point, put-signal, the one-sided atomics, the
+    // grouped all-reduce, hostBarrier and subset return FB_E_UNSUPPORTED;
+    // alloc / free throw std::logic_error (heap allocation is collective over
+    // the whole parent).  A child and its parent share this rank's staging
+    // buffers: calls on both from one rank must be stream-ordered unless the
+    // buffers are symmetric.  Returns null and sets *rc to FB_E_INVALID for an
+    // empty list, a member out of range or repeated, this rank not a member,
+    // or a slot out of range or in use on this rank.  Destroying the child
+    // zeroes this rank's slot pad on a stream of its own, then frees the slot.
+    // Precondition: this rank's last collective on the child has completed
+    // (its stream has been waited for); the destructor does not order itself
+    // after the caller's streams.
+    std::shared_ptr<Communicator> subset(const std::vector<int>& members, int slot, int* rc = nullptr);
+    // bit s set: slot s is free on this rank
+    uint32_t freeSubsetSlots() const;
+    bool isSubset() const { return parent_ != nullptr; }
 
     int rank() const { return dev_.rank; }
     int size() const { return dev_.nranks; }
@@ -314,7 +340,8 @@ class Communicator
     // Same word without synchronising (caller has already waited for `s`)
     uint32_t peekError() const;
     // Host-side barrier between the ranks' host threads / processes
-    void hostBarrier();
+    // (FB_E_UNSUPPORTED on a sub-communicator)
+    int hostBarrier();
     // Last algorithm picked by allReduce (for reporting / tests)
     int lastAlgo() const { return lastAlgo_; }
 
@@ -397,6 +424,12 @@ class Communicator
     std::shared_ptr<LocalGroup> localGroup_;
 
     struct GroupLaunch;
+
+    // sub-communicators: the child holds its parent and the slot it uses;
+    // the parent records which slots are in use on this rank
+    std::shared_ptr<Communicator> parent_;
+    int slot_ = -1;
+    std::atomic<uint32_t> usedSlots_{ 0 };
 
     static std::shared_ptr<Communicator> makeRank(const CommConfig& cfg, int rank, int nranks, int device);
     void computeLayout();

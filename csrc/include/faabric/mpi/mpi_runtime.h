@@ -458,6 +458,33 @@ class MpiWorld
     // Statistics of the device path (collectives that ran as fused kernels)
     uint64_t getDeviceCollectiveCount() const { return deviceCollectives.load(); }
 
+    // ---- device branch of each collective ----
+    // One branch per collective, shared by MPI_COMM_WORLD and the
+    // sub-communicators.  `comm` is this rank's device communicator (the
+    // world's, or a sub-communicator child of it; null: no device path),
+    // `rank` the caller's WORLD rank (it picks the stream), `root` a rank of
+    // `comm`.  The caller has checked that the buffers are device memory.
+    // True when the collective ran as a fused kernel; false when `comm` does
+    // not support it (FB_E_UNSUPPORTED, FB_E_TOO_LARGE): take the host path.
+    using DeviceComm = std::shared_ptr<faabric::device::Communicator>;
+    // The (datatype, op) pair has a device reduction
+    static bool deviceReducible(faabric_datatype_t* dt, faabric_op_t* op);
+    bool deviceBroadcast(const DeviceComm& comm, int rank, int root, uint8_t* buffer, size_t bytes);
+    bool deviceReduce(const DeviceComm& comm, int rank, int root, const uint8_t* send, uint8_t* recv,
+                      faabric_datatype_t* dt, int count, faabric_op_t* op);
+    bool deviceAllReduce(const DeviceComm& comm, int rank, const uint8_t* send, uint8_t* recv,
+                         faabric_datatype_t* dt, int count, faabric_op_t* op);
+    // false for an in-place scan (send == recv)
+    bool deviceScan(const DeviceComm& comm, int rank, const uint8_t* send, uint8_t* recv,
+                    faabric_datatype_t* dt, int count, faabric_op_t* op);
+    // send == nullptr at the root: its chunk already sits in its slot of recv
+    bool deviceGather(const DeviceComm& comm, int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes);
+    // recv == nullptr at the root: its chunk stays where it is in send
+    bool deviceScatter(const DeviceComm& comm, int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes);
+    // false for an in-place all-gather (send is this rank's slot of recv)
+    bool deviceAllGather(const DeviceComm& comm, int rank, const uint8_t* send, uint8_t* recv, size_t bytes);
+    bool deviceAllToAll(const DeviceComm& comm, int rank, const uint8_t* send, uint8_t* recv, size_t chunk);
+
   private:
     int id = -1;
     int size = -1;
@@ -701,8 +728,6 @@ class MpiWorld
     void stageFree(int ownerRank, const void* ownerPtr);
     const uint8_t* peerViewOfStaged(int ownerRank, int viewerRank, const void* ownerPtr);
     void* streamForRank(int rank, int channel = 0);
-    // Returns true if the collective ran on the device path
-    bool tryDeviceAllReduce(int rank, uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count, faabric_op_t* op);
 };
 
 // FbDtype / FbOp for an MPI datatype / op (-1 if there is no device mapping)

@@ -422,7 +422,10 @@ struct Communicator::LocalGroup
     {}
 };
 
-static const size_t SIG_REGION = 64 * 1024; // signal pad, padded
+// this rank's signal pad, then the pads of the sub-communicator slots
+static const size_t SIG_REGION = (size_t)(1 + FB_SUB_SLOTS) * FB_SIG_BYTES;
+static_assert(FB_SIG_SBAR_OFF + FB_SIG_SBAR_WORDS <= FB_SIG_TOTAL_WORDS, "signal pad overflows its slot");
+static_assert(FB_SUB_SLOTS <= 32, "slot masks are 32-bit");
 
 void Communicator::computeLayout()
 {
@@ -981,6 +984,30 @@ cudaStream_t Communicator::internalStream()
 
 Communicator::~Communicator()
 {
+    if (parent_ != nullptr) {
+        // Zero-on-release (comm_abi.h): every collective of this child has
+        // completed on this rank, so no peer write to the pad is pending
+        uint32_t* pad = dev_.sig[dev_.rank];
+        bool zeroed = true;
+        if (loop_) {
+            memset(pad, 0, FB_SIG_BYTES);
+        } else {
+            // a stream of our own: a device-wide synchronise could wait for a
+            // peer's kernel that waits for this rank
+            bindDevice();
+            cudaStream_t t = internalStream();
+            zeroed = t != nullptr && cudaMemsetAsync(pad, 0, FB_SIG_BYTES, t) == cudaSuccess &&
+                     cudaStreamSynchronize(t) == cudaSuccess;
+            if (!zeroed) {
+                // a slot whose pad may hold stale flags is never handed out again
+                fprintf(stderr, "[faabric-b200] rank %d: zeroing sub-communicator slot %d failed\n", dev_.rank, slot_);
+                cudaGetLastError();
+            }
+        }
+        if (zeroed) {
+            parent_->usedSlots_.fetch_and(~(1u << slot_));
+        }
+    }
     if (heapRegistered_) {
         std::unique_lock<std::shared_mutex> lk(heapRangesMx);
         const uint8_t* base = dev_.heap[dev_.rank];
@@ -998,13 +1025,90 @@ Communicator::~Communicator()
     // Backing is shared: freed when the last rank's communicator dies
 }
 
-void Communicator::hostBarrier()
+int Communicator::hostBarrier()
 {
+    if (parent_ != nullptr) {
+        return FB_E_UNSUPPORTED;
+    }
     if (bootstrap_) {
         bootstrap_->barrier();
     } else if (localGroup_) {
         localGroup_->bar.arrive_and_wait();
     }
+    return FB_OK;
+}
+
+// ---------------------------------------------------------------------------
+// Sub-communicators
+// ---------------------------------------------------------------------------
+std::shared_ptr<Communicator> Communicator::subset(const std::vector<int>& members, int slot, int* rcOut)
+{
+    int rcLocal = FB_OK;
+    int& rc = rcOut ? *rcOut : rcLocal;
+    rc = FB_OK;
+    if (parent_ != nullptr) {
+        rc = FB_E_UNSUPPORTED;
+        return nullptr;
+    }
+    const int n = dev_.nranks;
+    int self = -1;
+    uint32_t seen = 0;
+    for (size_t i = 0; i < members.size(); i++) {
+        const int m = members[i];
+        if (m < 0 || m >= n || (seen >> m) & 1u) {
+            rc = FB_E_INVALID;
+            return nullptr;
+        }
+        seen |= 1u << m;
+        if (m == dev_.rank) {
+            self = (int)i;
+        }
+    }
+    if (self < 0 || slot < 0 || slot >= FB_SUB_SLOTS) {
+        rc = FB_E_INVALID;
+        return nullptr;
+    }
+    const uint32_t bit = 1u << slot;
+    if (usedSlots_.fetch_or(bit) & bit) {
+        rc = FB_E_INVALID;
+        return nullptr;
+    }
+    auto c = std::shared_ptr<Communicator>(new Communicator());
+    c->parent_ = shared_from_this();
+    c->slot_ = slot;
+    c->cfg_ = cfg_;
+    c->allReduceTable_ = allReduceTable_;
+    c->device_ = device_;
+    c->backing_ = backing_;
+    c->llOff_ = llOff_;
+    c->mboxOff_ = mboxOff_;
+    c->p2pDescOff_ = p2pDescOff_;
+    c->bounceSlotBytes_ = bounceSlotBytes_;
+    c->stageSendOff_ = stageSendOff_;
+    c->stageRecvOff_ = stageRecvOff_;
+    c->userOff_ = userOff_;
+    c->heapTotal_ = heapTotal_;
+    c->loop_ = loop_;
+    c->k_ = k_;
+    c->streamSync_ = streamSync_;
+    c->streamWaitOk_ = streamWaitOk_;
+    c->streamWriteOk_ = streamWriteOk_;
+    c->dev_.rank = self;
+    c->dev_.nranks = (int32_t)members.size();
+    for (size_t i = 0; i < members.size(); i++) {
+        c->dev_.heap[i] = dev_.heap[members[i]];
+        c->dev_.sig[i] = dev_.sig[members[i]] + (size_t)(slot + 1) * FB_SIG_TOTAL_WORDS;
+    }
+    c->dev_.mcHeap = nullptr;
+    c->dev_.err = dev_.err;
+    c->dev_.timeoutNs = dev_.timeoutNs;
+    return c;
+}
+
+uint32_t Communicator::freeSubsetSlots() const
+{
+    // a child cannot be split further
+    return parent_ != nullptr ? 0u : ~usedSlots_.load() & ((1u << FB_SUB_SLOTS) - 1);
 }
 
 // ---------------------------------------------------------------------------
@@ -1012,6 +1116,9 @@ void Communicator::hostBarrier()
 // ---------------------------------------------------------------------------
 uint64_t Communicator::alloc(size_t bytes, size_t align)
 {
+    if (parent_ != nullptr) {
+        throw std::logic_error("alloc on a sub-communicator: allocate collectively on the parent");
+    }
     std::lock_guard<std::mutex> lk(allocMx_);
     if (align < 256) {
         align = 256;
@@ -1040,6 +1147,9 @@ uint64_t Communicator::alloc(size_t bytes, size_t align)
 
 void Communicator::free(uint64_t offset)
 {
+    if (parent_ != nullptr) {
+        throw std::logic_error("free on a sub-communicator: free collectively on the parent");
+    }
     std::lock_guard<std::mutex> lk(allocMx_);
     auto it = allocated_.find(offset);
     if (it == allocated_.end()) {
@@ -1314,7 +1424,21 @@ int Communicator::reduceLike(int kind,
     const int nvVariant = fb::nvlsVariant(dtype, op);
 
     // ---- algorithm choice ----
-    if (kind == K_ALLREDUCE) {
+    if (kind == K_ALLREDUCE && parent_ != nullptr) {
+        // The LL area and the multicast object belong to the parent's rank set
+        if (algo == FB_ALGO_LL || algo == FB_ALGO_NVLS) {
+            return FB_E_UNSUPPORTED;
+        }
+        if (algo == FB_ALGO_AUTO) {
+            algo = pickAllReduceAlgo(bytes, false);
+            if (algo == FB_ALGO_LL) {
+                algo = bytes <= cfg_.oneShotMaxBytes ? FB_ALGO_ONESHOT : FB_ALGO_TWOSHOT;
+            }
+        }
+        if (algo == FB_ALGO_ONESHOT && symmetric && send == recv) {
+            algo = FB_ALGO_TWOSHOT;
+        }
+    } else if (kind == K_ALLREDUCE) {
         if (algo == FB_ALGO_AUTO) {
             // Element-wise multimem variants (integers, f64) are request-rate
             // bound: AUTO leaves them to the P2P kernels unless the message is
@@ -1776,6 +1900,10 @@ std::shared_ptr<Communicator::GroupPlan> Communicator::prepareGroup(
     int rcLocal = FB_OK;
     int& rc = rcOut ? *rcOut : rcLocal;
     rc = FB_OK;
+    if (parent_ != nullptr) {
+        rc = FB_E_UNSUPPORTED; // see subset()
+        return nullptr;
+    }
     const size_t esize = fbDtypeSize(dtype);
     if (esize == 0) {
         rc = FB_E_INVALID;
@@ -1870,6 +1998,9 @@ int Communicator::launchGroup(const GroupLaunch& l, int dtype, int op, int flags
 int Communicator::allReduceGroup(const GroupPlan& plan, int op, int flags, cudaStream_t s)
 {
     NvtxRange nvtxRange("fb::allReduceGroup");
+    if (parent_ != nullptr) {
+        return FB_E_UNSUPPORTED; // see subset()
+    }
     const fb::ReduceLaunchers* L = fb::findReduceLaunchers(plan.dtype, op);
     if (L == nullptr || L->group == nullptr) {
         return FB_E_UNSUPPORTED;
@@ -1893,6 +2024,9 @@ int Communicator::allReduceMany(const GroupItem* items,
                                 cudaStream_t s)
 {
     NvtxRange nvtxRange("fb::allReduceMany");
+    if (parent_ != nullptr) {
+        return FB_E_UNSUPPORTED; // see subset()
+    }
     const size_t esize = fbDtypeSize(dtype);
     const fb::ReduceLaunchers* L = fb::findReduceLaunchers(dtype, op);
     if (esize == 0) {
@@ -2378,6 +2512,10 @@ bool Communicator::syncStreamBounded(cudaStream_t s, uint64_t timeoutMs)
 
 bool Communicator::waitStreamFast(cudaStream_t s)
 {
+    if (parent_ != nullptr) {
+        // one completion word per rank: its sequence lives in the parent
+        return parent_->waitStreamFast(s);
+    }
     if (loop_) {
         return true;
     }
@@ -2511,6 +2649,9 @@ int Communicator::recvChunk(uint8_t* buf, size_t len, int peer, cudaStream_t s)
 int Communicator::send(const void* buf, size_t bytes, int peer, cudaStream_t s)
 {
     NvtxRange nvtxRange("fb::send");
+    if (parent_ != nullptr) {
+        return FB_E_UNSUPPORTED; // see subset()
+    }
     if (peer < 0 || peer >= dev_.nranks) {
         return FB_E_INVALID;
     }
@@ -2532,6 +2673,9 @@ int Communicator::send(const void* buf, size_t bytes, int peer, cudaStream_t s)
 int Communicator::recv(void* buf, size_t bytes, int peer, cudaStream_t s)
 {
     NvtxRange nvtxRange("fb::recv");
+    if (parent_ != nullptr) {
+        return FB_E_UNSUPPORTED; // see subset()
+    }
     if (peer < 0 || peer >= dev_.nranks) {
         return FB_E_INVALID;
     }
@@ -2557,6 +2701,9 @@ int Communicator::sendRecv(const void* sendBuf,
                            cudaStream_t s)
 {
     NvtxRange nvtxRange("fb::sendRecv");
+    if (parent_ != nullptr) {
+        return FB_E_UNSUPPORTED; // see subset()
+    }
     if (dst < 0 || dst >= dev_.nranks || src < 0 || src >= dev_.nranks) {
         return FB_E_INVALID;
     }
@@ -2596,6 +2743,9 @@ int Communicator::putSignal(const void* local,
                             int blocks,
                             cudaStream_t s)
 {
+    if (parent_ != nullptr) {
+        return FB_E_UNSUPPORTED; // see subset()
+    }
     if (peer < 0 || peer >= dev_.nranks || signalIdx < 0 ||
         signalIdx >= FB_SIG_USER_WORDS || blocks < 1) {
         return FB_E_INVALID;
@@ -2618,6 +2768,9 @@ int Communicator::putSignal(const void* local,
 
 int Communicator::waitSignal(int signalIdx, uint32_t count, cudaStream_t s)
 {
+    if (parent_ != nullptr) {
+        return FB_E_UNSUPPORTED; // see subset()
+    }
     if (signalIdx < 0 || signalIdx >= FB_SIG_USER_WORDS) {
         return FB_E_INVALID;
     }
@@ -2646,6 +2799,9 @@ int Communicator::accumulate(const void* origin,
                              void* fetchOut,
                              cudaStream_t s)
 {
+    if (parent_ != nullptr) {
+        return FB_E_UNSUPPORTED; // see subset()
+    }
     const size_t esize = fbDtypeSize(dtype);
     if (esize == 0 || peer < 0 || peer >= dev_.nranks) {
         return FB_E_INVALID;
@@ -2680,6 +2836,9 @@ int Communicator::compareAndSwap(const void* compare,
                                  int peer,
                                  cudaStream_t s)
 {
+    if (parent_ != nullptr) {
+        return FB_E_UNSUPPORTED; // see subset()
+    }
     const size_t esize = fbDtypeSize(dtype);
     if (esize == 0 || peer < 0 || peer >= dev_.nranks) {
         return FB_E_INVALID;

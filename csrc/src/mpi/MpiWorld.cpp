@@ -684,7 +684,8 @@ void MpiWorld::send(int sendRank,
     msg.messageType = messageType;
     msg.buffer = nullptr;
 
-    const bool onDevice = bytes > 0 && isDevicePointer(buffer);
+    // (the loopback backend's heap is host memory: copied as such)
+    const bool onDevice = bytes > 0 && isDevicePointer(buffer) && !faabric::device::Communicator::isLoopbackHeapPointer(buffer);
     if (isLocal && !faabric::util::isMockMode()) {
         // Eager copy so the caller may reuse its buffer as soon as we return
         if (bytes > 0 && onDevice) {
@@ -800,7 +801,7 @@ void MpiWorld::doRecv(MpiMessage& msg,
     const size_t bytes = payloadSize(msg);
     if (bytes > 0 && msg.buffer != nullptr) {
         const bool srcDev = isDevicePointer(msg.buffer);
-        const bool dstDev = isDevicePointer(buffer);
+        const bool dstDev = isDevicePointer(buffer) && !faabric::device::Communicator::isLoopbackHeapPointer(buffer);
         if (srcDev) {
             // Parked in the sender's heap: read it through OUR mapping
             const uint8_t* src = peerViewOfStaged(msg.sendRank, msg.recvRank, msg.buffer);
@@ -1241,22 +1242,122 @@ static int symFlag(faabric::device::Communicator& c, const void* a, size_t bytes
     return c.inHeap(a, bytes) ? FB_FLAG_SYMMETRIC : 0;
 }
 
-bool MpiWorld::tryDeviceAllReduce(int rank, uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count, faabric_op_t* op)
+bool MpiWorld::deviceReducible(faabric_datatype_t* dt, faabric_op_t* op)
 {
-    int fdt = fbDtypeFor(dt);
-    int fop = fbOpFor(op);
+    return fbDtypeFor(dt) >= 0 && fbOpFor(op) >= 0;
+}
+
+// Runs the device branch of a collective and counts it
+#define FB_DEVICE_BRANCH(call)                                                                                   \
+    do {                                                                                                         \
+        if (!runDevice(comm, streamForRank(rank), [&](faabric::device::Communicator& c, cudaStream_t s) {       \
+                return (call);                                                                                   \
+            })) {                                                                                                \
+            return false;                                                                                        \
+        }                                                                                                        \
+        deviceCollectives.fetch_add(1);                                                                          \
+        return true;                                                                                             \
+    } while (0)
+
+bool MpiWorld::deviceBroadcast(const DeviceComm& comm, int rank, int root, uint8_t* buffer, size_t bytes)
+{
+    FB_DEVICE_BRANCH(c.broadcast(buffer, bytes, root, symFlag(c, buffer, bytes), s));
+}
+
+bool MpiWorld::deviceReduce(const DeviceComm& comm,
+                            int rank,
+                            int root,
+                            const uint8_t* send,
+                            uint8_t* recv,
+                            faabric_datatype_t* dt,
+                            int count,
+                            faabric_op_t* op)
+{
+    // Inputs are staged, so aliasing the root's input and output is safe and
+    // no symmetric offsets are assumed
+    const int fdt = fbDtypeFor(dt);
+    const int fop = fbOpFor(op);
     if (fdt < 0 || fop < 0) {
         return false;
     }
-    auto comm = getDeviceComm(rank);
-    bool ran = runDevice(comm, streamForRank(rank), [&](faabric::device::Communicator& c, cudaStream_t s) {
-        return c.allReduce(send, recv, (size_t)count, fdt, fop, forcedAllReduceAlgo, symFlag(c, send, (size_t)count * dt->size), s);
-    });
-    if (ran) {
-        deviceCollectives.fetch_add(1);
-    }
-    return ran;
+    FB_DEVICE_BRANCH(c.reduce(send, recv, (size_t)count, fdt, fop, root, 0, s));
 }
+
+bool MpiWorld::deviceAllReduce(const DeviceComm& comm,
+                               int rank,
+                               const uint8_t* send,
+                               uint8_t* recv,
+                               faabric_datatype_t* dt,
+                               int count,
+                               faabric_op_t* op)
+{
+    const int fdt = fbDtypeFor(dt);
+    const int fop = fbOpFor(op);
+    if (fdt < 0 || fop < 0) {
+        return false;
+    }
+    // LL and NVLS need the parent's rank set: a forced choice of either means
+    // AUTO on a sub-communicator
+    int algo = forcedAllReduceAlgo;
+    if (comm != nullptr && comm->isSubset() && (algo == FB_ALGO_LL || algo == FB_ALGO_NVLS)) {
+        algo = FB_ALGO_AUTO;
+    }
+    FB_DEVICE_BRANCH(c.allReduce(send, recv, (size_t)count, fdt, fop, algo, symFlag(c, send, (size_t)count * dt->size), s));
+}
+
+bool MpiWorld::deviceScan(const DeviceComm& comm,
+                          int rank,
+                          const uint8_t* send,
+                          uint8_t* recv,
+                          faabric_datatype_t* dt,
+                          int count,
+                          faabric_op_t* op)
+{
+    const int fdt = fbDtypeFor(dt);
+    const int fop = fbOpFor(op);
+    if (send == recv || fdt < 0 || fop < 0) {
+        return false;
+    }
+    FB_DEVICE_BRANCH(c.scan(send, recv, (size_t)count, fdt, fop, symFlag(c, send, (size_t)count * dt->size), s));
+}
+
+bool MpiWorld::deviceGather(const DeviceComm& comm, int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes)
+{
+    // The device-or-host choice must come out the same on every rank, and only
+    // the root knows whether it passed MPI_IN_PLACE: so the root's in-place
+    // case takes the device path too (its chunk already sits in the receive
+    // buffer), and no rank relies on symmetric offsets - every contribution is
+    // staged through the symmetric staging area.
+    if (comm != nullptr && send == nullptr) {
+        send = recv + (size_t)comm->rank() * bytes;
+    }
+    FB_DEVICE_BRANCH(c.gather(send, recv, bytes, root, 0, s));
+}
+
+bool MpiWorld::deviceScatter(const DeviceComm& comm, int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes)
+{
+    // In place at the root: its chunk is copied onto itself (the source is
+    // staged before the kernel reads it)
+    if (comm != nullptr && recv == nullptr) {
+        recv = const_cast<uint8_t*>(send) + (size_t)comm->rank() * bytes;
+    }
+    FB_DEVICE_BRANCH(c.scatter(send, recv, bytes, root, 0, s));
+}
+
+bool MpiWorld::deviceAllGather(const DeviceComm& comm, int rank, const uint8_t* send, uint8_t* recv, size_t bytes)
+{
+    if (comm == nullptr || send == recv + (size_t)comm->rank() * bytes) {
+        return false;
+    }
+    FB_DEVICE_BRANCH(c.allGather(send, recv, bytes, symFlag(c, send, bytes), s));
+}
+
+bool MpiWorld::deviceAllToAll(const DeviceComm& comm, int rank, const uint8_t* send, uint8_t* recv, size_t chunk)
+{
+    FB_DEVICE_BRANCH(c.allToAll(send, recv, chunk, symFlag(c, send, chunk * (size_t)(comm ? comm->size() : 0)), s));
+}
+
+#undef FB_DEVICE_BRANCH
 
 int MpiWorld::iAllReduce(int rank, uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count, faabric_op_t* op)
 {
@@ -1420,11 +1521,7 @@ void MpiWorld::broadcast(int rootRank,
 {
     const size_t bytes = (size_t)count * dataType->size;
     if (bytes > 0 && isDevicePointer(buffer)) {
-        auto comm = getDeviceComm(thisRank);
-        if (runDevice(comm, streamForRank(thisRank), [&](faabric::device::Communicator& c, cudaStream_t s) {
-                return c.broadcast(buffer, bytes, rootRank, symFlag(c, buffer, bytes), s);
-            })) {
-            deviceCollectives.fetch_add(1);
+        if (deviceBroadcast(getDeviceComm(thisRank), thisRank, rootRank, buffer, bytes)) {
             return;
         }
         HostStage st;
@@ -1495,11 +1592,7 @@ void MpiWorld::scatter(int sendRank,
     checkRanksRange(sendRank, recvRank);
     const size_t chunk = (size_t)sendCount * sendType->size;
     if (chunk > 0 && isDevicePointer(recvBuffer)) {
-        auto comm = getDeviceComm(recvRank);
-        if (runDevice(comm, streamForRank(recvRank), [&](faabric::device::Communicator& c, cudaStream_t s) {
-                return c.scatter(sendBuffer, recvBuffer, chunk, sendRank, 0, s);
-            })) {
-            deviceCollectives.fetch_add(1);
+        if (deviceScatter(getDeviceComm(recvRank), recvRank, sendRank, sendBuffer, recvBuffer, chunk)) {
             return;
         }
     }
@@ -1548,21 +1641,11 @@ void MpiWorld::gather(int sendRank,
     // In place: the root's contribution already sits in its slot
     const bool inPlace = isRoot && sendBuffer == recvBuffer;
 
-    // The device-or-host choice must come out the same on every rank, and only
-    // the root knows whether it passed MPI_IN_PLACE: so the root's in-place
-    // case takes the device path too (its chunk already sits in the receive
-    // buffer), and no rank relies on symmetric offsets - every contribution is
-    // staged through the symmetric staging area.
+    // (the root's in-place case takes the device path too: see deviceGather)
     const bool deviceCall = isDevicePointer(isRoot && inPlace ? recvBuffer : sendBuffer);
-    if (sendBytes > 0 && deviceCall) {
-        auto comm = getDeviceComm(sendRank);
-        const uint8_t* contribution = (isRoot && inPlace) ? recvBuffer + (size_t)recvRank * recvBytes : sendBuffer;
-        if (runDevice(comm, streamForRank(sendRank), [&](faabric::device::Communicator& c, cudaStream_t s) {
-                return c.gather(contribution, recvBuffer, sendBytes, recvRank, 0, s);
-            })) {
-            deviceCollectives.fetch_add(1);
-            return;
-        }
+    if (sendBytes > 0 && deviceCall &&
+        deviceGather(getDeviceComm(sendRank), sendRank, recvRank, inPlace ? nullptr : sendBuffer, recvBuffer, sendBytes)) {
+        return;
     }
 
     if (!isDevicePointer(sendBuffer) && !(isRoot && isDevicePointer(recvBuffer)) && sharedMemoryEligible(sendBytes * size)) {
@@ -1642,14 +1725,9 @@ void MpiWorld::allGather(int rank,
 {
     checkRanksRange(0, rank);
     const size_t sendBytes = (size_t)sendCount * sendType->size;
-    if (sendBytes > 0 && isDevicePointer(sendBuffer) && sendBuffer != recvBuffer + (size_t)rank * sendBytes) {
-        auto comm = getDeviceComm(rank);
-        if (runDevice(comm, streamForRank(rank), [&](faabric::device::Communicator& c, cudaStream_t s) {
-                return c.allGather(sendBuffer, recvBuffer, sendBytes, symFlag(c, sendBuffer, sendBytes), s);
-            })) {
-            deviceCollectives.fetch_add(1);
-            return;
-        }
+    if (sendBytes > 0 && isDevicePointer(sendBuffer) && sendBuffer != recvBuffer + (size_t)rank * sendBytes &&
+        deviceAllGather(getDeviceComm(rank), rank, sendBuffer, recvBuffer, sendBytes)) {
+        return;
     }
     if (!isDevicePointer(sendBuffer) && !isDevicePointer(recvBuffer) && sharedMemoryEligible(sendBytes * size)) {
         sharedAllGather(rank, sendBuffer, recvBuffer, sendBytes);
@@ -1676,18 +1754,10 @@ void MpiWorld::reduce(int sendRank,
     const bool inPlace = sendBuffer == recvBuffer;
 
     // Same choice on every rank (only the root can see MPI_IN_PLACE): in-place
-    // at the root stays on the device; inputs are staged, so aliasing the
-    // root's input and output is safe and no symmetric offsets are assumed.
-    if (bytes > 0 && isDevicePointer(sendBuffer)) {
-        int fdt = fbDtypeFor(datatype);
-        int fop = fbOpFor(operation);
-        auto comm = (fdt >= 0 && fop >= 0) ? getDeviceComm(sendRank) : nullptr;
-        if (runDevice(comm, streamForRank(sendRank), [&](faabric::device::Communicator& c, cudaStream_t s) {
-                return c.reduce(sendBuffer, recvBuffer, (size_t)count, fdt, fop, recvRank, 0, s);
-            })) {
-            deviceCollectives.fetch_add(1);
-            return;
-        }
+    // at the root stays on the device
+    if (bytes > 0 && isDevicePointer(sendBuffer) && deviceReducible(datatype, operation) &&
+        deviceReduce(getDeviceComm(sendRank), sendRank, recvRank, sendBuffer, recvBuffer, datatype, count, operation)) {
+        return;
     }
     if (bytes > 0 && (isDevicePointer(sendBuffer) || (isRoot && isDevicePointer(recvBuffer)))) {
         HostStage in, out;
@@ -1802,7 +1872,8 @@ void MpiWorld::allReduce(int rank,
     checkRanksRange(0, rank);
     const size_t bytes = (size_t)count * datatype->size;
     if (bytes > 0 && isDevicePointer(sendBuffer)) {
-        if (tryDeviceAllReduce(rank, sendBuffer, recvBuffer, datatype, count, operation)) {
+        if (deviceReducible(datatype, operation) &&
+            deviceAllReduce(getDeviceComm(rank), rank, sendBuffer, recvBuffer, datatype, count, operation)) {
             return;
         }
         HostStage in, out;
@@ -2163,16 +2234,9 @@ void MpiWorld::scan(int rank,
 {
     checkRanksRange(0, rank);
     const size_t bytes = (size_t)count * datatype->size;
-    if (bytes > 0 && isDevicePointer(sendBuffer) && sendBuffer != recvBuffer) {
-        int fdt = fbDtypeFor(datatype);
-        int fop = fbOpFor(operation);
-        auto comm = (fdt >= 0 && fop >= 0) ? getDeviceComm(rank) : nullptr;
-        if (runDevice(comm, streamForRank(rank), [&](faabric::device::Communicator& c, cudaStream_t s) {
-                return c.scan(sendBuffer, recvBuffer, (size_t)count, fdt, fop, symFlag(c, sendBuffer, bytes), s);
-            })) {
-            deviceCollectives.fetch_add(1);
-            return;
-        }
+    if (bytes > 0 && isDevicePointer(sendBuffer) && sendBuffer != recvBuffer && deviceReducible(datatype, operation) &&
+        deviceScan(getDeviceComm(rank), rank, sendBuffer, recvBuffer, datatype, count, operation)) {
+        return;
     }
     if (bytes > 0 && (isDevicePointer(sendBuffer) || isDevicePointer(recvBuffer))) {
         HostStage in, out;
@@ -2212,11 +2276,7 @@ void MpiWorld::allToAll(int rank,
     checkRanksRange(0, rank);
     const size_t chunk = (size_t)sendCount * sendType->size;
     if (chunk > 0 && isDevicePointer(sendBuffer)) {
-        auto comm = getDeviceComm(rank);
-        if (runDevice(comm, streamForRank(rank), [&](faabric::device::Communicator& c, cudaStream_t s) {
-                return c.allToAll(sendBuffer, recvBuffer, chunk, symFlag(c, sendBuffer, chunk * size), s);
-            })) {
-            deviceCollectives.fetch_add(1);
+        if (deviceAllToAll(getDeviceComm(rank), rank, sendBuffer, recvBuffer, chunk)) {
             return;
         }
         HostStage in, out;

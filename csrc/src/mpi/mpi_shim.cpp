@@ -1394,6 +1394,10 @@ int MPI_Comm_free(MPI_Comm* comm)
     // The predefined communicators (and cartesian views of the world) are not
     // owned by the caller; handles of sub-communicators are
     if ((*comm)->id != FAABRIC_COMM_WORLD && (*comm)->id != FAABRIC_COMM_NULL) {
+        // frees this rank's signal slot of the fused device path
+        if (auto sub = getSubCommunicator((*comm)->id)) {
+            sub->releaseDevice(executingContext.getRank());
+        }
         delete *comm;
     }
     *comm = MPI_COMM_NULL;

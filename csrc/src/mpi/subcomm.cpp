@@ -15,13 +15,19 @@
 namespace faabric::mpi {
 
 namespace {
+// Host memory, or the loopback backend's heap (host memory in the device role)
+bool hostAddressable(const void* p)
+{
+    return !MpiWorld::isDevicePointer(p) || faabric::device::Communicator::isLoopbackHeapPointer(p);
+}
+
 // Host<->host copies must not depend on a CUDA device being present
 void copyBytes(void* dst, const void* src, size_t bytes)
 {
     if (bytes == 0 || dst == src) {
         return;
     }
-    if (MpiWorld::isDevicePointer(dst) || MpiWorld::isDevicePointer(src)) {
+    if (!hostAddressable(dst) || !hostAddressable(src)) {
         if (cudaMemcpy(dst, src, bytes, cudaMemcpyDefault) != cudaSuccess) {
             cudaGetLastError();
             throw std::runtime_error("Device copy inside a sub-communicator collective failed");
@@ -39,7 +45,7 @@ struct HostView
 
     HostView(const uint8_t* p, size_t bytes)
     {
-        if (bytes > 0 && MpiWorld::isDevicePointer(p)) {
+        if (bytes > 0 && !hostAddressable(p)) {
             staged.resize(bytes);
             copyBytes(staged.data(), p, bytes);
             ptr = staged.data();
@@ -91,6 +97,10 @@ void SubCommunicator::barrier(MpiWorld& w, int me)
 
 void SubCommunicator::broadcast(MpiWorld& w, int me, int root, uint8_t* buffer, faabric_datatype_t* dt, int count)
 {
+    const size_t bytes = (size_t)count * dt->size;
+    if (bytes > 0 && MpiWorld::isDevicePointer(buffer) && w.deviceBroadcast(deviceComm(w, me), me, root, buffer, bytes)) {
+        return;
+    }
     // Binomial tree over ranks relative to the root
     const int n = size();
     const int rel = (commRankOf(me) - root + n) % n;
@@ -123,6 +133,10 @@ void SubCommunicator::reduce(MpiWorld& w,
                              faabric_op_t* op)
 {
     const size_t bytes = (size_t)count * dt->size;
+    if (bytes > 0 && MpiWorld::isDevicePointer(send) && MpiWorld::deviceReducible(dt, op) &&
+        w.deviceReduce(deviceComm(w, me), me, root, send, recv, dt, count, op)) {
+        return;
+    }
     const int n = size();
     const int myCommRank = commRankOf(me);
     if (myCommRank != root) {
@@ -155,6 +169,10 @@ void SubCommunicator::allReduce(MpiWorld& w,
                                 int count,
                                 faabric_op_t* op)
 {
+    if (count > 0 && dt->size > 0 && MpiWorld::isDevicePointer(send) && MpiWorld::deviceReducible(dt, op) &&
+        w.deviceAllReduce(deviceComm(w, me), me, send, recv, dt, count, op)) {
+        return;
+    }
     reduce(w, me, 0, send, recv, dt, count, op);
     broadcast(w, me, 0, recv, dt, count);
 }
@@ -168,6 +186,10 @@ void SubCommunicator::scan(MpiWorld& w,
                            faabric_op_t* op)
 {
     const size_t bytes = (size_t)count * dt->size;
+    if (bytes > 0 && MpiWorld::isDevicePointer(send) && send != recv && MpiWorld::deviceReducible(dt, op) &&
+        w.deviceScan(deviceComm(w, me), me, send, recv, dt, count, op)) {
+        return;
+    }
     const int myCommRank = commRankOf(me);
     HostView mine(send, bytes);
     std::vector<uint8_t> acc(mine.ptr, mine.ptr + bytes);
@@ -186,6 +208,11 @@ void SubCommunicator::scan(MpiWorld& w,
 void SubCommunicator::gather(MpiWorld& w, int me, int root, const uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count)
 {
     const size_t bytes = (size_t)count * dt->size;
+    // (the root's in-place contribution sits in recv: it decides from that)
+    if (bytes > 0 && MpiWorld::isDevicePointer(send != nullptr ? send : recv) &&
+        w.deviceGather(deviceComm(w, me), me, root, send, recv, bytes)) {
+        return;
+    }
     if (commRankOf(me) != root) {
         w.send(me, worldRanks[root], send, dt, count);
         return;
@@ -205,6 +232,11 @@ void SubCommunicator::gather(MpiWorld& w, int me, int root, const uint8_t* send,
 void SubCommunicator::scatter(MpiWorld& w, int me, int root, const uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count)
 {
     const size_t bytes = (size_t)count * dt->size;
+    // (an in-place root keeps its chunk in send: it decides from that)
+    if (bytes > 0 && MpiWorld::isDevicePointer(recv != nullptr ? recv : send) &&
+        w.deviceScatter(deviceComm(w, me), me, root, send, recv, bytes)) {
+        return;
+    }
     if (commRankOf(me) != root) {
         w.recv(worldRanks[root], me, recv, dt, count, nullptr);
         return;
@@ -223,6 +255,11 @@ void SubCommunicator::scatter(MpiWorld& w, int me, int root, const uint8_t* send
 
 void SubCommunicator::allGather(MpiWorld& w, int me, const uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count)
 {
+    const size_t bytes = (size_t)count * dt->size;
+    if (bytes > 0 && MpiWorld::isDevicePointer(send) && send != recv + (size_t)commRankOf(me) * bytes &&
+        w.deviceAllGather(deviceComm(w, me), me, send, recv, bytes)) {
+        return;
+    }
     // (an in-place chunk is skipped by the self-copy check)
     gather(w, me, 0, send, recv, dt, count);
     broadcast(w, me, 0, recv, dt, count * size());
@@ -231,6 +268,9 @@ void SubCommunicator::allGather(MpiWorld& w, int me, const uint8_t* send, uint8_
 void SubCommunicator::allToAll(MpiWorld& w, int me, const uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count)
 {
     const size_t bytes = (size_t)count * dt->size;
+    if (bytes > 0 && MpiWorld::isDevicePointer(send) && w.deviceAllToAll(deviceComm(w, me), me, send, recv, bytes)) {
+        return;
+    }
     const int n = size();
     const int myCommRank = commRankOf(me);
     // Sends are eager: ship everything, then collect in rank order
@@ -247,6 +287,53 @@ void SubCommunicator::allToAll(MpiWorld& w, int me, const uint8_t* send, uint8_t
             w.recv(worldRanks[r], me, recv + (size_t)r * bytes, dt, count, nullptr);
         }
     }
+}
+
+std::shared_ptr<faabric::device::Communicator> SubCommunicator::deviceComm(MpiWorld& w, int me)
+{
+    {
+        std::lock_guard<std::mutex> lk(deviceMx);
+        const DeviceState& st = device[me];
+        if (st.decided) {
+            return st.child;
+        }
+    }
+    // Slot agreement, once per rank: the lowest slot free on every member.
+    // The lock is not held across it: the other ranks of this process agree
+    // through the same object.  Members are world ranks, so every child (of a
+    // nested split too) is cut from the world communicator.
+    auto parent = w.getDeviceComm(me);
+    int mask = parent != nullptr ? (int)parent->freeSubsetSlots() : 0;
+    int agreed = 0;
+    allReduce(w, me, (const uint8_t*)&mask, (uint8_t*)&agreed, MPI_INT, 1, MPI_BAND);
+    std::shared_ptr<faabric::device::Communicator> child;
+    if (agreed != 0) {
+        int rc = FB_OK;
+        child = parent->subset(worldRanks, __builtin_ctz((unsigned)agreed), &rc);
+        if (child == nullptr) {
+            // the other members run on the slot: this rank cannot fall back alone
+            SPDLOG_ERROR("Communicator {}: rank {} cannot take agreed slot {} ({})", commId, me,
+                         __builtin_ctz((unsigned)agreed), faabric::device::Communicator::errorString(rc));
+            throw std::runtime_error("Sub-communicator slot agreement failed");
+        }
+    }
+    std::lock_guard<std::mutex> lk(deviceMx);
+    DeviceState& st = device[me];
+    st.decided = true;
+    st.child = child;
+    return child;
+}
+
+void SubCommunicator::releaseDevice(int me)
+{
+    std::shared_ptr<faabric::device::Communicator> child;
+    {
+        std::lock_guard<std::mutex> lk(deviceMx);
+        DeviceState& st = device[me];
+        st.decided = true;
+        child = std::move(st.child);
+    }
+    // (the destructor zeroes this rank's slot pad, then frees the slot)
 }
 
 // ---------------------------------------------------------------------------

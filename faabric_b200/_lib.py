@@ -98,6 +98,9 @@ def load():
     _sig(lib, "fb_comm_in_heap", i32, [vp, vp, u64])
     _sig(lib, "fb_comm_check_error", u32, [vp, vp])
     _sig(lib, "fb_comm_host_barrier", None, [vp])
+    _sig(lib, "fb_comm_subset", vp, [vp, C.POINTER(C.c_int), i32, i32])
+    _sig(lib, "fb_comm_free_subset_slots", u32, [vp])
+    _sig(lib, "fb_comm_is_subset", i32, [vp])
 
     _sig(lib, "fb_allreduce", i32, [vp, vp, vp, u64, i32, i32, i32, i32, vp])
     _sig(lib, "fb_reduce", i32, [vp, vp, vp, u64, i32, i32, i32, i32, vp])

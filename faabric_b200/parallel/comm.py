@@ -131,6 +131,7 @@ class Communicator:
         # of in-kernel spins (ranks sharing a GPU): not CUDA-graph capturable
         self.stream_sync = bool(self._lib.fb_comm_stream_sync(self._h))
         self.stream_wait_supported = bool(self._lib.fb_comm_stream_wait_supported(self._h))
+        self.is_subset = bool(self._lib.fb_comm_is_subset(self._h))
         self._allocs: dict[int, int] = {}
 
     # ------------------------------------------------------------ lifecycle
@@ -190,10 +191,37 @@ class Communicator:
             raise CommError(f"{nbytes} bytes is not a whole number of {dtype} elements ({esize} bytes)")
         return nbytes // esize, code
 
+    # ------------------------------------------------------ sub-communicators
+    def subset(self, members: Sequence[int], slot: int) -> "Communicator":
+        """A communicator over ``members`` (ranks of this one, in the order that
+        becomes the child's rank order; this rank must be one of them).  Every
+        member passes the same list and slot, a slot free on every member (see
+        :meth:`free_subset_slots`).  No communication and no allocation: the
+        child runs the same fused kernels over the members' heaps, so tensors
+        from :meth:`empty` on the parent are symmetric on the child too.
+        Closing the child zeroes this rank's slot pad and frees the slot: close
+        it only after its last collective has completed (synchronise the
+        streams it ran on; :meth:`LocalGroup.subset` groups do that)."""
+        members = [int(m) for m in members]
+        arr = (C.c_int * max(len(members), 1))(*members)
+        h = self._lib.fb_comm_subset(self._h, arr, len(members), int(slot))
+        if not h:
+            raise CommError(f"subset {members} on slot {slot} failed [{_lib.last_error()}]")
+        return Communicator(h, owner=self)
+
+    def free_subset_slots(self) -> int:
+        """Bit s set: sub-communicator slot s is free on this rank."""
+        return int(self._lib.fb_comm_free_subset_slots(self._h))
+
+    def _parent_only(self, what: str):
+        if self.is_subset:
+            raise CommError(f"{what} on a sub-communicator: use the parent communicator")
+
     # ------------------------------------------------------------ heap
     def empty(self, shape, dtype=torch.float32) -> torch.Tensor:
         """Allocate a tensor in the symmetric heap.  Call collectively (same
         order and sizes on every rank) so offsets match across ranks."""
+        self._parent_only("empty")
         if isinstance(shape, int):
             shape = (shape,)
         numel = 1
@@ -217,6 +245,7 @@ class Communicator:
         return t
 
     def free(self, t: torch.Tensor):
+        self._parent_only("free")
         off = self._allocs.pop(t.data_ptr(), None)
         if off is not None:
             self._lib.fb_comm_free(self._h, off)
@@ -267,6 +296,7 @@ class Communicator:
         return int(self._lib.fb_comm_check_error(self._h, self._stream(stream)))
 
     def host_barrier(self):
+        self._parent_only("host_barrier")
         self._lib.fb_comm_host_barrier(self._h)
 
     # ------------------------------------------------------------ collectives
@@ -687,6 +717,22 @@ class LocalGroup:
         self.run(lambda c, r, st: c.barrier())
         return self.check_errors() == [0] * self.size
 
+    def subset(self, members: Sequence[int]) -> "SubGroup":
+        """The ranks ``members`` of this group as a group of their own (child
+        rank i is rank ``members[i]`` here), on the lowest sub-communicator
+        slot free on every member.  Its collectives run the same fused
+        kernels; close it to free the slot."""
+        members = [int(m) for m in members]
+        if not members or any(m < 0 or m >= self.size for m in members):
+            raise CommError(f"subset: members {members} outside a group of {self.size}")
+        free = ~0
+        for m in members:
+            free &= self.comms[m].free_subset_slots()
+        if free == 0:
+            raise CommError(f"subset: no sub-communicator slot is free on every member of {members}")
+        slot = (free & -free).bit_length() - 1
+        return SubGroup(self, members, slot)
+
     def close(self):
         for c in self.comms:
             c.close()
@@ -700,6 +746,38 @@ class LocalGroup:
             self.close()
         except Exception:
             pass
+
+
+class SubGroup(LocalGroup):
+    """Members of a :class:`LocalGroup` as a group of their own (made by
+    :meth:`LocalGroup.subset`).  ``comms[i]`` is the child communicator of
+    parent rank ``members[i]`` and ``streams[i]`` that rank's parent stream, so
+    calls on the child and on the parent issued through ``run`` stay ordered."""
+
+    def __init__(self, parent: LocalGroup, members: Sequence[int], slot: int):
+        self._lib = parent._lib
+        self._h = None
+        self.parent = parent
+        self.members = list(members)
+        self.slot = slot
+        self.devices = [parent.devices[m] for m in self.members]
+        self.streams = [parent.streams[m] for m in self.members]
+        self.comms = []
+        try:
+            for m in self.members:
+                self.comms.append(parent.comms[m].subset(self.members, slot))
+        except Exception:
+            self.close()
+            raise
+        self.size = len(self.members)
+
+    def close(self):
+        # a child frees its slot by zeroing its pad: its kernels must be done
+        if self.comms:
+            self.synchronize()
+        for c in self.comms:
+            c.close()
+        self.comms = []
 
 
 def init_from_env(**cfg) -> Communicator:
