@@ -591,6 +591,96 @@ void* fb_group_prepare(void* h,
     FB_CATCH(nullptr)
 }
 
+// ---- grouped reduce-scatter / all-gather: counts are per-rank counts ----
+static void* groupPrepareKind(void* h,
+                              int n,
+                              const void* const* send,
+                              void* const* recv,
+                              const uint64_t* counts,
+                              int dtype,
+                              Communicator::GroupKind kind)
+{
+    FB_TRY
+    auto items = groupItems(n, send, recv, counts);
+    int rc = FB_OK;
+    auto plan = COMM(h)->prepareGroup(items.data(), items.size(), dtype, &rc, kind);
+    if (!plan) {
+        g_lastError = std::string("prepareGroup: ") + Communicator::errorString(rc);
+        return nullptr;
+    }
+    auto* ph = new FbGroupPlanHandle();
+    ph->plan = plan;
+    return ph;
+    FB_CATCH(nullptr)
+}
+
+void* fb_group_prepare_reduce_scatter(void* h,
+                                      int n,
+                                      const void* const* send,
+                                      void* const* recv,
+                                      const uint64_t* counts,
+                                      int dtype)
+{
+    return groupPrepareKind(h, n, send, recv, counts, dtype, Communicator::GROUP_REDUCE_SCATTER);
+}
+
+void* fb_group_prepare_all_gather(void* h,
+                                  int n,
+                                  const void* const* send,
+                                  void* const* recv,
+                                  const uint64_t* counts,
+                                  int dtype)
+{
+    return groupPrepareKind(h, n, send, recv, counts, dtype, Communicator::GROUP_ALLGATHER);
+}
+
+int fb_group_reduce_scatter(void* h, void* plan, int op, int flags, void* stream)
+{
+    if (plan == nullptr) {
+        return FB_E_INVALID;
+    }
+    return COMM(h)->reduceScatterGroup(*((FbGroupPlanHandle*)plan)->plan, op, flags, (cudaStream_t)stream);
+}
+
+int fb_group_all_gather(void* h, void* plan, int flags, void* stream)
+{
+    if (plan == nullptr) {
+        return FB_E_INVALID;
+    }
+    return COMM(h)->allGatherGroup(*((FbGroupPlanHandle*)plan)->plan, flags, (cudaStream_t)stream);
+}
+
+int fb_reduce_scatter_many(void* h,
+                           int n,
+                           const void* const* send,
+                           void* const* recv,
+                           const uint64_t* counts,
+                           int dtype,
+                           int op,
+                           int flags,
+                           void* stream)
+{
+    FB_TRY
+    auto items = groupItems(n, send, recv, counts);
+    return COMM(h)->reduceScatterMany(items.data(), items.size(), dtype, op, flags, (cudaStream_t)stream);
+    FB_CATCH(FB_E_CUDA)
+}
+
+int fb_all_gather_many(void* h,
+                       int n,
+                       const void* const* send,
+                       void* const* recv,
+                       const uint64_t* counts,
+                       int dtype,
+                       int flags,
+                       void* stream)
+{
+    FB_TRY
+    auto items = groupItems(n, send, recv, counts);
+    return COMM(h)->allGatherMany(items.data(), items.size(), dtype, flags, (cudaStream_t)stream);
+    FB_CATCH(FB_E_CUDA)
+}
+
 int fb_group_allreduce(void* h, void* plan, int op, int flags, void* stream)
 {
     if (plan == nullptr) {

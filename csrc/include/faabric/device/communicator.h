@@ -143,7 +143,8 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     // supports allReduce (one-shot and two-shot only), reduce, reduceScatter,
     // scan, the data-movement collectives, barrier and the heap queries, with
     // child ranks.  Point to point, put-signal, the one-sided atomics, the
-    // grouped all-reduce, hostBarrier and subset return FB_E_UNSUPPORTED;
+    // grouped all-reduce, reduce-scatter and all-gather, hostBarrier and
+    // subset return FB_E_UNSUPPORTED;
     // alloc / free throw std::logic_error (heap allocation is collective over
     // the whole parent).  A child and its parent share this rank's staging
     // buffers: calls on both from one rank must be stream-ordered unless the
@@ -252,20 +253,60 @@ class Communicator : public std::enable_shared_from_this<Communicator>
         size_t count;     // elements
     };
     struct GroupPlan;
+    // What a plan's launches compute.  For the two shard kinds, GroupItem
+    // .count is the per-rank element count (MPI recvcount / sendcount):
+    //   GROUP_REDUCE_SCATTER: send holds size()*count elements; recv gets op
+    //     over every rank p of send_p[rank*count, (rank+1)*count)
+    //     (MPI_Reduce_scatter_block per item)
+    //   GROUP_ALLGATHER: send holds count elements; block p of recv (size()
+    //     *count elements) gets send of rank p (MPI_Allgather per item; a
+    //     byte copy, any dtype)
+    // Shard kinds group an item only if send and recv are in the symmetric
+    // heap and 16-byte aligned, count*esize is a multiple of 16, and recv
+    // overlaps no send of the group on this rank.  The one exception is the
+    // in-place all-gather, send == recv + rank*count*esize.  Items with count
+    // 0 are skipped.
+    enum GroupKind
+    {
+        GROUP_ALLREDUCE = 0,
+        GROUP_REDUCE_SCATTER = 1,
+        GROUP_ALLGATHER = 2
+    };
     // Builds (and uploads) this rank's segment tables.  Collective: every rank
     // must pass the same list (same offsets, same counts).  Returns null and
-    // sets *rc when an item is not symmetric / aligned.
+    // sets *rc when an item is not symmetric / aligned (FB_E_INVALID), or on
+    // a sub-communicator (FB_E_UNSUPPORTED).
     std::shared_ptr<GroupPlan> prepareGroup(const GroupItem* items,
                                             size_t nItems,
                                             int dtype,
-                                            int* rc = nullptr);
+                                            int* rc = nullptr,
+                                            GroupKind kind = GROUP_ALLREDUCE);
+    // A plan of another kind gives FB_E_INVALID
     int allReduceGroup(const GroupPlan& plan, int op, int flags, cudaStream_t s);
+    int reduceScatterGroup(const GroupPlan& plan, int op, int flags, cudaStream_t s);
+    int allGatherGroup(const GroupPlan& plan, int flags, cudaStream_t s);
     // prepare + launch for a transient list (MPI_Iallreduce bursts); falls back
     // to per-item allReduce calls when the list cannot be grouped
     int allReduceMany(const GroupItem* items,
                       size_t nItems,
                       int dtype,
                       int op,
+                      int flags,
+                      cudaStream_t s);
+    // The same for the shard kinds (MPI_Ireduce_scatter_block and
+    // MPI_Iallgather bursts): falls back to per-item reduceScatter /
+    // allGather calls for a list that cannot be grouped, and returns their
+    // errors (reduceScatter refuses shards that are not a multiple of 16
+    // bytes with FB_E_UNSUPPORTED)
+    int reduceScatterMany(const GroupItem* items,
+                          size_t nItems,
+                          int dtype,
+                          int op,
+                          int flags,
+                          cudaStream_t s);
+    int allGatherMany(const GroupItem* items,
+                      size_t nItems,
+                      int dtype,
                       int flags,
                       cudaStream_t s);
     static size_t groupPlanLaunches(const GroupPlan& plan);
@@ -442,7 +483,14 @@ class Communicator : public std::enable_shared_from_this<Communicator>
                 std::shared_ptr<Backing> backing,
                 const std::string& kind);
     void finishSetup();
-    int launchGroup(const GroupLaunch& l, int dtype, int op, int flags, cudaStream_t s);
+    int launchGroup(const GroupLaunch& l, GroupKind kind, int dtype, int op, int flags, cudaStream_t s);
+    int groupMany(GroupKind kind,
+                  const GroupItem* items,
+                  size_t nItems,
+                  int dtype,
+                  int op,
+                  int flags,
+                  cudaStream_t s);
     int streamWaitGe(cudaStream_t s, const uint32_t* localWord, uint32_t value);
     int streamBarrier(int flags, cudaStream_t s);
     bool rmaTargetOk(uint64_t dstOffset, uint64_t bytes, size_t align, int peer) const;

@@ -312,6 +312,28 @@ class MpiWorld
                    int count,
                    faabric_op_t* operation);
 
+    // MPI_Ireduce_scatter_block and MPI_Iallgather, built like iAllReduce: a
+    // burst on symmetric, 16-byte aligned device buffers whose shards are
+    // multiples of 16 bytes is deferred and issued as ONE grouped launch at
+    // the next wait (FAABRIC_MPI_GROUP_IALLREDUCE=0 turns that off); other
+    // device buffers run one stream-ordered device call at issue; host
+    // buffers, and an in-place reduce-scatter (send == recv), complete at
+    // issue.
+    int iReduceScatter(int rank,
+                       uint8_t* sendBuffer,
+                       uint8_t* recvBuffer,
+                       faabric_datatype_t* datatype,
+                       int recvCount,
+                       faabric_op_t* operation);
+
+    int iAllGather(int rank,
+                   const uint8_t* sendBuffer,
+                   faabric_datatype_t* sendType,
+                   int sendCount,
+                   uint8_t* recvBuffer,
+                   faabric_datatype_t* recvType,
+                   int recvCount);
+
     // Symmetric-heap allocation for MPI_Alloc_mem (collective: every rank
     // must allocate the same sizes in the same order)
     void* deviceAlloc(int rank, size_t bytes);
@@ -665,13 +687,16 @@ class MpiWorld
     std::atomic<uint64_t> deviceCollectives = 0;
     // Channel streams MPI_Iallreduce may rotate over (see ensureDeviceComms)
     std::atomic<int> nonBlockingChannels = 1;
-    // MPI_Iallreduce bursts on symmetric device buffers are coalesced into one
-    // grouped kernel at the next wait (FAABRIC_MPI_GROUP_IALLREDUCE=0: one
-    // kernel per call over the channels, the round-1 behaviour)
+    // MPI_Iallreduce (and MPI_Ireduce_scatter_block / MPI_Iallgather) bursts
+    // on symmetric device buffers are coalesced into one grouped kernel at the
+    // next wait (FAABRIC_MPI_GROUP_IALLREDUCE=0: one kernel per call, the
+    // round-1 behaviour)
     bool groupIallreduce = true;
     // FAABRIC_ALLREDUCE_ALGO (FbAlgo; AUTO = measured table / thresholds)
     int forcedAllReduceAlgo = 0;
     void ensureDeviceComms();
+    // Looks up this rank thread's communicator and first stream once
+    void cacheDeviceComm(int rank);
 
     // Host buffers, all ranks in this process: the ranks reduce straight out
     // of each other's buffers (slice-parallel reduce-scatter + all-gather in

@@ -7,6 +7,7 @@
 // Reference algorithms replaced: MpiWorld::{broadcast,scatter,gather,allGather,
 // allToAll,barrier,send,recv} message loops (src/mpi/MpiWorld.cpp:590-1111,
 // 1433-1485,1753-1775).
+#include "coll_group.cuh"
 #include "coll_move.cuh"
 
 namespace fb {
@@ -253,6 +254,102 @@ cudaError_t launchMove(const MoveArgs& a,
         return launchMoveW<4>(a, blocks, threads, s);
     }
     return launchMoveW<1>(a, blocks, threads, s);
+}
+
+// ----------------------------------------------------------------------------
+// Grouped all-gather: one MPI_Allgather per tensor, all in ONE launch per rank
+// (launch_api.h).  A push: each chunk loads this rank's vectors once and
+// stores them into block `rank` of every peer's output.  Entry barrier: every
+// peer's output may be overwritten.  Exit barrier: every push into this
+// rank's output has landed.  In place (send == block `rank` of recv) is safe:
+// only this rank ever writes that block.  Dtype-free: a byte copy.
+// ----------------------------------------------------------------------------
+template<int NR>
+__global__ void __launch_bounds__(512, 1) groupAllGatherKernel(const GroupArgs a)
+{
+    extern __shared__ __align__(16) uint8_t sGroupRaw[];
+    GroupSeg* sSegs = reinterpret_cast<GroupSeg*>(sGroupRaw);
+    const FbCommDev& c = a.comm;
+    const int n = (NR > 0) ? NR : c.nranks;
+    BlockBarrier bar;
+    const bool ok = groupEnter(a, sSegs, bar);
+
+    if (ok && a.nSegs > 0) {
+        constexpr int UNROLL = (NR == 8) ? 2 : (NR == 1 ? 8 : 4);
+        constexpr uint32_t CHUNK = 32u * UNROLL;
+        const uint32_t lane = threadIdx.x & 31;
+        const uint32_t warpsPerCta = blockDim.x >> 5;
+        const uint32_t warpStride = gridDim.x * warpsPerCta;
+        const uint8_t* const in = c.heap[c.rank];
+        int cur = 0;
+        for (uint32_t ch = blockIdx.x * warpsPerCta + (threadIdx.x >> 5);
+             ch < a.totalChunks;
+             ch += warpStride) {
+            cur = groupSegOf(sSegs, a.nSegs, cur, ch);
+            const GroupSeg sg = sSegs[cur];
+            const uint32_t v0 = (ch - sg.chunk0) * CHUNK;
+            const uint8_t* const src = in + sg.sendOff + (uint64_t)v0 * 16;
+            const uint64_t rOff = sg.recvOff + (uint64_t)v0 * 16;
+            const uint32_t rem = sg.nVec - v0;
+            if (rem >= CHUNK) {
+                Vec16 v[UNROLL];
+#pragma unroll
+                for (int u = 0; u < UNROLL; u++) {
+                    v[u] = ldVecStream(src + (uint64_t)(u * 32 + lane) * 16);
+                }
+                if constexpr (NR > 0) {
+#pragma unroll
+                    for (int p = 0; p < NR; p++) {
+#pragma unroll
+                        for (int u = 0; u < UNROLL; u++) {
+                            stVec(c.heap[p] + rOff + (uint64_t)(u * 32 + lane) * 16, v[u]);
+                        }
+                    }
+                } else {
+                    for (int p = 0; p < n; p++) {
+#pragma unroll
+                        for (int u = 0; u < UNROLL; u++) {
+                            stVec(c.heap[p] + rOff + (uint64_t)(u * 32 + lane) * 16, v[u]);
+                        }
+                    }
+                }
+            } else {
+                // ragged end of a shard (or a whole small one)
+#pragma unroll
+                for (int u = 0; u < UNROLL; u++) {
+                    const uint32_t i = (uint32_t)u * 32 + lane;
+                    if (i < rem) {
+                        const Vec16 v = ldVecStream(src + (uint64_t)i * 16);
+                        for (int p = 0; p < n; p++) {
+                            stVec(c.heap[p] + rOff + (uint64_t)i * 16, v);
+                        }
+                    }
+                }
+            }
+        }
+    }
+    groupExit(a, bar);
+}
+
+cudaError_t launchGroupAllGather(const GroupArgs& a,
+                                 int blocks,
+                                 int threads,
+                                 cudaStream_t s)
+{
+    const size_t smem = (size_t)a.nSegs * sizeof(GroupSeg);
+    const int n = a.comm.nranks;
+    if (n == 1) {
+        groupAllGatherKernel<1><<<blocks, threads, smem, s>>>(a);
+    } else if (n == 2) {
+        groupAllGatherKernel<2><<<blocks, threads, smem, s>>>(a);
+    } else if (n == 4) {
+        groupAllGatherKernel<4><<<blocks, threads, smem, s>>>(a);
+    } else if (n == 8) {
+        groupAllGatherKernel<8><<<blocks, threads, smem, s>>>(a);
+    } else {
+        groupAllGatherKernel<0><<<blocks, threads, smem, s>>>(a);
+    }
+    return cudaGetLastError();
 }
 
 // ----------------------------------------------------------------------------
@@ -516,6 +613,11 @@ cudaError_t preloadMoveKernels()
     FB_PRELOAD_W(16)
     FB_PRELOAD_W(4)
     FB_PRELOAD_W(1)
+    FB_PRELOAD((groupAllGatherKernel<0>))
+    FB_PRELOAD((groupAllGatherKernel<1>))
+    FB_PRELOAD((groupAllGatherKernel<2>))
+    FB_PRELOAD((groupAllGatherKernel<4>))
+    FB_PRELOAD((groupAllGatherKernel<8>))
     FB_PRELOAD(barrierKernel)
     FB_PRELOAD(waitSignalKernel)
     FB_PRELOAD(waitWordKernel)

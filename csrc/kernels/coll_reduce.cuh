@@ -6,6 +6,7 @@
 // reads peer HBM over NVLink and applies the op in registers.
 #pragma once
 
+#include "coll_group.cuh"
 #include "fb_prims.cuh"
 #include "launch_api.h"
 
@@ -595,6 +596,128 @@ cudaError_t launchGroup(const GroupArgs& a,
     return cudaGetLastError();
 }
 
+// ----------------------------------------------------------------------------
+// Grouped reduce-scatter: one MPI_Reduce_scatter_block per tensor, all in ONE
+// launch per rank.  A segment is this rank's shard of one tensor (sendOff
+// points at shard `rank` of the input, recvOff at the local output), and a
+// shard is a whole number of 16-byte vectors.  Each chunk gathers its vectors
+// from every peer, reduces them in registers and stores to this rank's output
+// only.  Entry barrier: every input is complete.  Exit barrier: the peers
+// have finished reading this rank's input.
+// ----------------------------------------------------------------------------
+template<typename VR, int NR>
+__global__ void __launch_bounds__(512, 1) groupReduceScatterKernel(
+  const GroupArgs a)
+{
+    extern __shared__ __align__(16) uint8_t sGroupRaw[];
+    GroupSeg* sSegs = reinterpret_cast<GroupSeg*>(sGroupRaw);
+    const FbCommDev& c = a.comm;
+    const int n = (NR > 0) ? NR : c.nranks;
+    BlockBarrier bar;
+    const bool ok = groupEnter(a, sSegs, bar);
+
+    if (ok && a.nSegs > 0) {
+        constexpr int UNROLL = (NR == 8) ? 2 : (NR == 1 ? 8 : 4);
+        constexpr uint32_t CHUNK = 32u * UNROLL;
+        const uint32_t lane = threadIdx.x & 31;
+        const uint32_t warpsPerCta = blockDim.x >> 5;
+        const uint32_t warpStride = gridDim.x * warpsPerCta;
+        uint8_t* const out = c.heap[c.rank];
+        int cur = 0;
+        for (uint32_t ch = blockIdx.x * warpsPerCta + (threadIdx.x >> 5);
+             ch < a.totalChunks;
+             ch += warpStride) {
+            cur = groupSegOf(sSegs, a.nSegs, cur, ch);
+            const GroupSeg sg = sSegs[cur];
+            const uint32_t v0 = (ch - sg.chunk0) * CHUNK;
+            const uint64_t sOff = sg.sendOff + (uint64_t)v0 * 16;
+            uint8_t* const dst = out + sg.recvOff + (uint64_t)v0 * 16;
+            const uint32_t rem = sg.nVec - v0;
+            if (rem >= CHUNK) {
+                Vec16 acc[UNROLL];
+                if constexpr (NR > 0) {
+                    Vec16 v[UNROLL][NR];
+#pragma unroll
+                    for (int u = 0; u < UNROLL; u++) {
+#pragma unroll
+                        for (int p = 0; p < NR; p++) {
+                            v[u][p] = ldVecStream(c.heap[p] + sOff +
+                                                  (uint64_t)(u * 32 + lane) * 16);
+                        }
+                    }
+#pragma unroll
+                    for (int u = 0; u < UNROLL; u++) {
+                        acc[u] = v[u][0];
+#pragma unroll
+                        for (int p = 1; p < NR; p++) {
+                            acc[u] = VR::apply(acc[u], v[u][p]);
+                        }
+                    }
+                } else {
+#pragma unroll
+                    for (int u = 0; u < UNROLL; u++) {
+                        acc[u] = ldVecStream(c.heap[0] + sOff +
+                                             (uint64_t)(u * 32 + lane) * 16);
+                    }
+                    for (int p = 1; p < n; p++) {
+                        Vec16 v[UNROLL];
+#pragma unroll
+                        for (int u = 0; u < UNROLL; u++) {
+                            v[u] = ldVecStream(c.heap[p] + sOff +
+                                               (uint64_t)(u * 32 + lane) * 16);
+                        }
+#pragma unroll
+                        for (int u = 0; u < UNROLL; u++) {
+                            acc[u] = VR::apply(acc[u], v[u]);
+                        }
+                    }
+                }
+#pragma unroll
+                for (int u = 0; u < UNROLL; u++) {
+                    stVec(dst + (uint64_t)(u * 32 + lane) * 16, acc[u]);
+                }
+            } else {
+                // ragged end of a shard (or a whole small one)
+#pragma unroll
+                for (int u = 0; u < UNROLL; u++) {
+                    const uint32_t i = (uint32_t)u * 32 + lane;
+                    if (i < rem) {
+                        Vec16 acc = ldVecStream(c.heap[0] + sOff + (uint64_t)i * 16);
+                        for (int p = 1; p < n; p++) {
+                            Vec16 v = ldVecStream(c.heap[p] + sOff + (uint64_t)i * 16);
+                            acc = VR::apply(acc, v);
+                        }
+                        stVec(dst + (uint64_t)i * 16, acc);
+                    }
+                }
+            }
+        }
+    }
+    groupExit(a, bar);
+}
+
+template<typename VR>
+cudaError_t launchGroupReduceScatter(const GroupArgs& a,
+                                     int blocks,
+                                     int threads,
+                                     cudaStream_t stream)
+{
+    const size_t smem = (size_t)a.nSegs * sizeof(GroupSeg);
+    const int nr = a.comm.nranks;
+    if (nr == 1) {
+        groupReduceScatterKernel<VR, 1><<<blocks, threads, smem, stream>>>(a);
+    } else if (nr == 2) {
+        groupReduceScatterKernel<VR, 2><<<blocks, threads, smem, stream>>>(a);
+    } else if (nr == 4) {
+        groupReduceScatterKernel<VR, 4><<<blocks, threads, smem, stream>>>(a);
+    } else if (nr == 8) {
+        groupReduceScatterKernel<VR, 8><<<blocks, threads, smem, stream>>>(a);
+    } else {
+        groupReduceScatterKernel<VR, 0><<<blocks, threads, smem, stream>>>(a);
+    }
+    return cudaGetLastError();
+}
+
 template<typename VR>
 cudaError_t preloadReduce()
 {
@@ -617,6 +740,11 @@ cudaError_t preloadReduce()
     FB_PRELOAD((groupAllReduceKernel<VR, 2>))
     FB_PRELOAD((groupAllReduceKernel<VR, 4>))
     FB_PRELOAD((groupAllReduceKernel<VR, 8>))
+    FB_PRELOAD((groupReduceScatterKernel<VR, 0>))
+    FB_PRELOAD((groupReduceScatterKernel<VR, 1>))
+    FB_PRELOAD((groupReduceScatterKernel<VR, 2>))
+    FB_PRELOAD((groupReduceScatterKernel<VR, 4>))
+    FB_PRELOAD((groupReduceScatterKernel<VR, 8>))
 #undef FB_PRELOAD
     return e;
 }
@@ -627,6 +755,7 @@ const ReduceLaunchers* launchersFor()
     static const ReduceLaunchers l = { &launchReduce<VR>,
                                        &launchLL<VR>,
                                        &launchGroup<VR>,
+                                       &launchGroupReduceScatter<VR>,
                                        &preloadReduce<VR> };
     return &l;
 }

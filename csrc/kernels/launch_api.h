@@ -107,11 +107,27 @@ typedef cudaError_t (*GroupLaunchFn)(const GroupArgs& a,
                                      int threads,
                                      cudaStream_t stream);
 
+// ---- grouped reduce-scatter and all-gather: equal shards, ONE launch ----
+// The same GroupArgs, with one segment per tensor and rank whose nVec covers
+// a whole shard (shards are multiples of 16 bytes, so tailBytes is 0):
+//   reduce-scatter: sendOff = off(send) + rank*shard, recvOff = off(recv);
+//                   the kernel reduces over every peer's sendOff and stores
+//                   to this rank's heap only.
+//   all-gather:     sendOff = off(send), recvOff = off(recv) + rank*shard;
+//                   the kernel loads locally and pushes to every peer.
+// Both keep the grouped all-reduce's chunking (fbGroupChunkVecs) and its
+// entry and exit barriers.
+cudaError_t launchGroupAllGather(const GroupArgs& a,
+                                 int blocks,
+                                 int threads,
+                                 cudaStream_t stream);
+
 struct ReduceLaunchers
 {
     ReduceLaunchFn reduce;
     LLLaunchFn ll;
     GroupLaunchFn group;
+    GroupLaunchFn groupRs; // grouped reduce-scatter
     // Forces the CUDA module/function load of every variant (lazy loading may
     // otherwise synchronise the context while a peer rank's kernel is spinning
     // on this one => deadlock until the watchdog fires)

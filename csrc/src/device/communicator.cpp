@@ -1212,6 +1212,11 @@ cudaError_t cudaGroup(const fb::GroupArgs& a, int dtype, int op, int blocks, int
     return fb::findReduceLaunchers(dtype, op)->group(a, blocks, threads, s);
 }
 
+cudaError_t cudaGroupReduceScatter(const fb::GroupArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s)
+{
+    return fb::findReduceLaunchers(dtype, op)->groupRs(a, blocks, threads, s);
+}
+
 cudaError_t cudaCopy(void* dst, const void* src, size_t bytes, cudaStream_t s)
 {
     return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, s);
@@ -1226,6 +1231,8 @@ const fb::KernelTable CUDA_KERNELS = {
     .reduce = cudaReduce,
     .ll = cudaLL,
     .group = cudaGroup,
+    .groupReduceScatter = cudaGroupReduceScatter,
+    .groupAllGather = fb::launchGroupAllGather,
     .move = fb::launchMove,
     .moveBulk = fb::launchMoveBulk,
     .barrier = fb::launchBarrier,
@@ -1245,6 +1252,8 @@ const fb::KernelTable HOST_KERNELS = {
     .reduce = fb::host::reduceKernel,
     .ll = fb::host::llAllReduce,
     .group = fb::host::groupAllReduce,
+    .groupReduceScatter = fb::host::groupReduceScatter,
+    .groupAllGather = fb::host::groupAllGather,
     .move = fb::host::moveKernel,
     .moveBulk = fb::host::moveBulk,
     .barrier = fb::host::barrierKernel,
@@ -1763,6 +1772,7 @@ struct Communicator::GroupLaunch
 struct Communicator::GroupPlan
 {
     std::vector<GroupLaunch> launches;
+    GroupKind kind = GROUP_ALLREDUCE;
     int dtype = 0;
     int device = 0;
     size_t items = 0;
@@ -1888,6 +1898,98 @@ static int buildGroupSegs(const Communicator& c,
     return FB_OK;
 }
 
+// This rank's segments of a reduce-scatter or all-gather group: one per item,
+// a whole shard each (see Communicator::GroupKind for the conditions)
+static int buildShardSegs(const Communicator& c,
+                          Communicator::GroupKind kind,
+                          const Communicator::GroupItem* items,
+                          size_t nItems,
+                          size_t esize,
+                          SegBuild& out)
+{
+    const int n = c.size();
+    const int rank = c.rank();
+    const uint32_t chunk = fb::fbGroupChunkVecs(n);
+    const bool rs = kind == Communicator::GROUP_REDUCE_SCATTER;
+    // [begin, end) of every send, by begin: peers read them (reduce-scatter)
+    // or the kernel reads them (all-gather) while outputs are written
+    std::vector<std::pair<uintptr_t, uintptr_t>> sends;
+    for (size_t i = 0; i < nItems; i++) {
+        const uint64_t shard = (uint64_t)items[i].count * esize;
+        if (shard == 0) {
+            continue;
+        }
+        const uint64_t sendBytes = rs ? shard * n : shard;
+        const uint64_t recvBytes = rs ? shard : shard * n;
+        if (shard % 16 != 0 || !c.inHeap(items[i].send, sendBytes) || !c.inHeap(items[i].recv, recvBytes) ||
+            (((uintptr_t)items[i].send | (uintptr_t)items[i].recv) & 15)) {
+            return FB_E_INVALID;
+        }
+        sends.push_back({ (uintptr_t)items[i].send, (uintptr_t)items[i].send + sendBytes });
+    }
+    std::sort(sends.begin(), sends.end());
+    std::vector<uintptr_t> maxEnd(sends.size());
+    for (size_t k = 0; k < sends.size(); k++) {
+        maxEnd[k] = std::max(sends[k].second, k > 0 ? maxEnd[k - 1] : 0);
+    }
+    uint64_t chunks = 0;
+    for (size_t i = 0; i < nItems; i++) {
+        const uint64_t shard = (uint64_t)items[i].count * esize;
+        if (shard == 0) {
+            continue;
+        }
+        const uintptr_t lo = (uintptr_t)items[i].recv;
+        const uintptr_t hi = lo + (rs ? shard : shard * n);
+        // in-place all-gather: the send is block `rank` of its own output
+        const uintptr_t own = (!rs && (uintptr_t)items[i].send == lo + (uint64_t)rank * shard) ? lo + rank * shard : 0;
+        // sends starting below `lo` overlap iff one of them ends above it;
+        // every send starting in [lo, hi) overlaps, except the own in-place one
+        size_t k = std::lower_bound(sends.begin(), sends.end(), std::make_pair(lo, (uintptr_t)0)) - sends.begin();
+        if (k > 0 && maxEnd[k - 1] > lo) {
+            return FB_E_INVALID;
+        }
+        bool ownSeen = false;
+        for (; k < sends.size() && sends[k].first < hi; k++) {
+            if (own != 0 && !ownSeen && sends[k].first == own && sends[k].second == own + shard) {
+                ownSeen = true;
+                continue;
+            }
+            return FB_E_INVALID;
+        }
+        if (shard / 16 > 0xffffffffull) {
+            return FB_E_TOO_LARGE;
+        }
+        fb::GroupSeg sg;
+        memset(&sg, 0, sizeof(sg));
+        sg.nVec = (uint32_t)(shard / 16);
+        sg.sendOff = c.offsetOf(items[i].send) + (rs ? (uint64_t)rank * shard : 0);
+        sg.recvOff = c.offsetOf(items[i].recv) + (rs ? 0 : (uint64_t)rank * shard);
+        sg.chunk0 = (uint32_t)chunks;
+        chunks += ((uint64_t)sg.nVec + chunk - 1) / chunk;
+        if (chunks > 0xffffffffull) {
+            return FB_E_TOO_LARGE;
+        }
+        out.segs.push_back(sg);
+        out.vecsPerRank += sg.nVec;
+        out.bytes += shard * n;
+    }
+    out.totalChunks = (uint32_t)chunks;
+    return FB_OK;
+}
+
+static int buildSegs(const Communicator& c,
+                     Communicator::GroupKind kind,
+                     const Communicator::GroupItem* items,
+                     size_t nItems,
+                     size_t esize,
+                     SegBuild& out)
+{
+    if (kind == Communicator::GROUP_ALLREDUCE) {
+        return buildGroupSegs(c, items, nItems, esize, out);
+    }
+    return buildShardSegs(c, kind, items, nItems, esize, out);
+}
+
 // items per launch: every item yields at most one segment per rank
 static const size_t GROUP_ITEMS_PER_LAUNCH = FB_GROUP_MAX_SEGS - 8;
 
@@ -1895,7 +1997,8 @@ std::shared_ptr<Communicator::GroupPlan> Communicator::prepareGroup(
   const GroupItem* items,
   size_t nItems,
   int dtype,
-  int* rcOut)
+  int* rcOut,
+  GroupKind kind)
 {
     int rcLocal = FB_OK;
     int& rc = rcOut ? *rcOut : rcLocal;
@@ -1905,19 +2008,20 @@ std::shared_ptr<Communicator::GroupPlan> Communicator::prepareGroup(
         return nullptr;
     }
     const size_t esize = fbDtypeSize(dtype);
-    if (esize == 0) {
+    if (esize == 0 || kind < GROUP_ALLREDUCE || kind > GROUP_ALLGATHER) {
         rc = FB_E_INVALID;
         return nullptr;
     }
     bindDevice();
     auto plan = std::make_shared<GroupPlan>();
+    plan->kind = kind;
     plan->dtype = dtype;
     plan->device = device_;
     plan->items = nItems;
     for (size_t begin = 0; begin < nItems; begin += GROUP_ITEMS_PER_LAUNCH) {
         const size_t cnt = std::min(GROUP_ITEMS_PER_LAUNCH, nItems - begin);
         SegBuild sb;
-        rc = buildGroupSegs(*this, items + begin, cnt, esize, sb);
+        rc = buildSegs(*this, kind, items + begin, cnt, esize, sb);
         if (rc != FB_OK) {
             return nullptr;
         }
@@ -1969,7 +2073,7 @@ static int groupGrid(const CommConfig& cfg, int nranks, uint64_t vecsPerRank)
     return (int)std::clamp<uint64_t>(want, 1, (uint64_t)cap);
 }
 
-int Communicator::launchGroup(const GroupLaunch& l, int dtype, int op, int flags, cudaStream_t s)
+int Communicator::launchGroup(const GroupLaunch& l, GroupKind kind, int dtype, int op, int flags, cudaStream_t s)
 {
     const int n = dev_.nranks;
     const bool ss = streamSync_ && !(flags & FB_FLAG_NOSYNC) && n > 1;
@@ -1983,7 +2087,16 @@ int Communicator::launchGroup(const GroupLaunch& l, int dtype, int op, int flags
     if (ss && streamBarrier(flags, s) != FB_OK) {
         return FB_E_CUDA;
     }
-    if (k_->group(a, dtype, op, groupGrid(cfg_, n, l.vecsPerRank), cfg_.threads, s) != cudaSuccess) {
+    const int blocks = groupGrid(cfg_, n, l.vecsPerRank);
+    cudaError_t e;
+    if (kind == GROUP_REDUCE_SCATTER) {
+        e = k_->groupReduceScatter(a, dtype, op, blocks, cfg_.threads, s);
+    } else if (kind == GROUP_ALLGATHER) {
+        e = k_->groupAllGather(a, blocks, cfg_.threads, s);
+    } else {
+        e = k_->group(a, dtype, op, blocks, cfg_.threads, s);
+    }
+    if (e != cudaSuccess) {
         return FB_E_CUDA;
     }
     if (ss && streamBarrier(flags, s) != FB_OK) {
@@ -1991,7 +2104,9 @@ int Communicator::launchGroup(const GroupLaunch& l, int dtype, int op, int flags
     }
     stats_.launches++;
     stats_.bytes += l.bytes;
-    stats_.algoCount[FB_ALGO_TWOSHOT]++;
+    if (kind == GROUP_ALLREDUCE) {
+        stats_.algoCount[FB_ALGO_TWOSHOT]++;
+    }
     return FB_OK;
 }
 
@@ -2001,18 +2116,63 @@ int Communicator::allReduceGroup(const GroupPlan& plan, int op, int flags, cudaS
     if (parent_ != nullptr) {
         return FB_E_UNSUPPORTED; // see subset()
     }
+    if (plan.kind != GROUP_ALLREDUCE) {
+        return FB_E_INVALID;
+    }
     const fb::ReduceLaunchers* L = fb::findReduceLaunchers(plan.dtype, op);
     if (L == nullptr || L->group == nullptr) {
         return FB_E_UNSUPPORTED;
     }
     bindDevice();
     for (const auto& l : plan.launches) {
-        int rc = launchGroup(l, plan.dtype, op, flags, s);
+        int rc = launchGroup(l, GROUP_ALLREDUCE, plan.dtype, op, flags, s);
         if (rc != FB_OK) {
             return rc;
         }
     }
     lastAlgo_ = FB_ALGO_TWOSHOT;
+    return FB_OK;
+}
+
+int Communicator::reduceScatterGroup(const GroupPlan& plan, int op, int flags, cudaStream_t s)
+{
+    NvtxRange nvtxRange("fb::reduceScatterGroup");
+    if (parent_ != nullptr) {
+        return FB_E_UNSUPPORTED; // see subset()
+    }
+    if (plan.kind != GROUP_REDUCE_SCATTER) {
+        return FB_E_INVALID;
+    }
+    const fb::ReduceLaunchers* L = fb::findReduceLaunchers(plan.dtype, op);
+    if (L == nullptr || L->groupRs == nullptr) {
+        return FB_E_UNSUPPORTED;
+    }
+    bindDevice();
+    for (const auto& l : plan.launches) {
+        int rc = launchGroup(l, GROUP_REDUCE_SCATTER, plan.dtype, op, flags, s);
+        if (rc != FB_OK) {
+            return rc;
+        }
+    }
+    return FB_OK;
+}
+
+int Communicator::allGatherGroup(const GroupPlan& plan, int flags, cudaStream_t s)
+{
+    NvtxRange nvtxRange("fb::allGatherGroup");
+    if (parent_ != nullptr) {
+        return FB_E_UNSUPPORTED; // see subset()
+    }
+    if (plan.kind != GROUP_ALLGATHER) {
+        return FB_E_INVALID;
+    }
+    bindDevice();
+    for (const auto& l : plan.launches) {
+        int rc = launchGroup(l, GROUP_ALLGATHER, plan.dtype, -1, flags, s);
+        if (rc != FB_OK) {
+            return rc;
+        }
+    }
     return FB_OK;
 }
 
@@ -2024,17 +2184,51 @@ int Communicator::allReduceMany(const GroupItem* items,
                                 cudaStream_t s)
 {
     NvtxRange nvtxRange("fb::allReduceMany");
+    return groupMany(GROUP_ALLREDUCE, items, nItems, dtype, op, flags, s);
+}
+
+int Communicator::reduceScatterMany(const GroupItem* items,
+                                    size_t nItems,
+                                    int dtype,
+                                    int op,
+                                    int flags,
+                                    cudaStream_t s)
+{
+    NvtxRange nvtxRange("fb::reduceScatterMany");
+    return groupMany(GROUP_REDUCE_SCATTER, items, nItems, dtype, op, flags, s);
+}
+
+int Communicator::allGatherMany(const GroupItem* items, size_t nItems, int dtype, int flags, cudaStream_t s)
+{
+    NvtxRange nvtxRange("fb::allGatherMany");
+    return groupMany(GROUP_ALLGATHER, items, nItems, dtype, -1, flags, s);
+}
+
+int Communicator::groupMany(GroupKind kind,
+                            const GroupItem* items,
+                            size_t nItems,
+                            int dtype,
+                            int op,
+                            int flags,
+                            cudaStream_t s)
+{
     if (parent_ != nullptr) {
         return FB_E_UNSUPPORTED; // see subset()
     }
     const size_t esize = fbDtypeSize(dtype);
-    const fb::ReduceLaunchers* L = fb::findReduceLaunchers(dtype, op);
     if (esize == 0) {
         return FB_E_INVALID;
     }
-    if (L == nullptr) {
-        return FB_E_UNSUPPORTED;
+    // all-gather is a byte copy: any dtype has a kernel
+    bool grouped = true;
+    if (kind != GROUP_ALLGATHER) {
+        const fb::ReduceLaunchers* L = fb::findReduceLaunchers(dtype, op);
+        if (L == nullptr) {
+            return FB_E_UNSUPPORTED;
+        }
+        grouped = (kind == GROUP_ALLREDUCE ? L->group : L->groupRs) != nullptr;
     }
+    const size_t n = (size_t)dev_.nranks;
     bindDevice();
     // try the grouped path batch by batch; anything not symmetric / aligned
     // goes through the per-tensor calls (the choice depends only on arguments
@@ -2042,15 +2236,31 @@ int Communicator::allReduceMany(const GroupItem* items,
     for (size_t begin = 0; begin < nItems; begin += GROUP_ITEMS_PER_LAUNCH) {
         const size_t cnt = std::min(GROUP_ITEMS_PER_LAUNCH, nItems - begin);
         SegBuild sb;
-        int rc = (L->group != nullptr) ? buildGroupSegs(*this, items + begin, cnt, esize, sb)
-                                       : FB_E_UNSUPPORTED;
+        int rc = grouped ? buildSegs(*this, kind, items + begin, cnt, esize, sb) : FB_E_UNSUPPORTED;
         if (rc != FB_OK) {
             for (size_t i = begin; i < begin + cnt; i++) {
+                const GroupItem& it = items[i];
+                const size_t bytes = it.count * esize;
                 int f = flags;
-                if (!inHeap(items[i].send, items[i].count * esize)) {
-                    f &= ~FB_FLAG_SYMMETRIC;
+                int r2 = FB_OK;
+                if (kind == GROUP_ALLREDUCE) {
+                    if (!inHeap(it.send, bytes)) {
+                        f &= ~FB_FLAG_SYMMETRIC;
+                    }
+                    r2 = allReduce(it.send, it.recv, it.count, dtype, op, FB_ALGO_AUTO, f, s);
+                } else if (bytes == 0) {
+                    continue;
+                } else if (kind == GROUP_REDUCE_SCATTER) {
+                    if (!inHeap(it.send, bytes * n)) {
+                        f &= ~FB_FLAG_SYMMETRIC;
+                    }
+                    r2 = reduceScatter(it.send, it.recv, it.count, dtype, op, f, s);
+                } else {
+                    if (!inHeap(it.send, bytes)) {
+                        f &= ~FB_FLAG_SYMMETRIC;
+                    }
+                    r2 = allGather(it.send, it.recv, bytes, f, s);
                 }
-                int r2 = allReduce(items[i].send, items[i].recv, items[i].count, dtype, op, FB_ALGO_AUTO, f, s);
                 if (r2 != FB_OK) {
                     return r2;
                 }
@@ -2095,7 +2305,7 @@ int Communicator::allReduceMany(const GroupItem* items,
             }
             l.dSegs = slot->dSegs;
         }
-        rc = launchGroup(l, dtype, op, flags, s);
+        rc = launchGroup(l, kind, dtype, op, flags, s);
         if (rc != FB_OK) {
             return rc;
         }
@@ -2104,7 +2314,9 @@ int Communicator::allReduceMany(const GroupItem* items,
             slot->used = true;
         }
     }
-    lastAlgo_ = FB_ALGO_TWOSHOT;
+    if (kind == GROUP_ALLREDUCE) {
+        lastAlgo_ = FB_ALGO_TWOSHOT;
+    }
     return FB_OK;
 }
 

@@ -493,6 +493,75 @@ cudaError_t groupAllReduce(const GroupArgs& a, int dtype, int op, int blocks, in
     return cudaSuccess;
 }
 
+// Every segment of the shard kinds is whole 16-byte vectors at 16-byte
+// aligned addresses, as the CUDA kernels load and store them
+static bool shardSegsOk(const GroupArgs& a)
+{
+    const FbCommDev& c = a.comm;
+    for (uint32_t si = 0; si < a.nSegs; si++) {
+        const GroupSeg& sg = a.segs[si];
+        if (sg.tailBytes != 0 || ((uintptr_t)(c.heap[c.rank] + sg.sendOff) & 15) ||
+            ((uintptr_t)(c.heap[c.rank] + sg.recvOff) & 15)) {
+            return false;
+        }
+    }
+    return true;
+}
+
+cudaError_t groupReduceScatter(const GroupArgs& a, int dtype, int op, int blocks, int, cudaStream_t)
+{
+    if (!shardSegsOk(a)) {
+        return cudaErrorMisalignedAddress;
+    }
+    const FbCommDev& c = a.comm;
+    bool ok = true;
+    if (!a.noSync) {
+        ok = gridBarrier(c, blocks);
+    }
+    if (ok) {
+        std::vector<uint8_t> tmp;
+        for (uint32_t si = 0; si < a.nSegs; si++) {
+            const GroupSeg& sg = a.segs[si];
+            const uint64_t bytes = (uint64_t)sg.nVec * 16;
+            tmp.resize(bytes);
+            reduceRange(c, dtype, op, sg.sendOff, bytes, c.nranks, tmp.data());
+            memcpy(c.heap[c.rank] + sg.recvOff, tmp.data(), bytes);
+        }
+    }
+    if (!a.noSync) {
+        gridBarrier(c, blocks);
+    }
+    return cudaSuccess;
+}
+
+cudaError_t groupAllGather(const GroupArgs& a, int blocks, int, cudaStream_t)
+{
+    if (!shardSegsOk(a)) {
+        return cudaErrorMisalignedAddress;
+    }
+    const FbCommDev& c = a.comm;
+    bool ok = true;
+    if (!a.noSync) {
+        ok = gridBarrier(c, blocks);
+    }
+    if (ok) {
+        for (uint32_t si = 0; si < a.nSegs; si++) {
+            const GroupSeg& sg = a.segs[si];
+            const uint8_t* src = c.heap[c.rank] + sg.sendOff;
+            for (int p = 0; p < c.nranks; p++) {
+                uint8_t* dst = c.heap[p] + sg.recvOff;
+                if (dst != src) { // in place: block `rank` is already there
+                    memcpy(dst, src, (uint64_t)sg.nVec * 16);
+                }
+            }
+        }
+    }
+    if (!a.noSync) {
+        gridBarrier(c, blocks);
+    }
+    return cudaSuccess;
+}
+
 // ----------------------------------------------------------------- move ----
 // The CUDA kernels copy in W-byte words.  Every address they touch that way
 // must be W-aligned (a misaligned vector access is a device fault), and every

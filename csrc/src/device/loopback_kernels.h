@@ -16,6 +16,8 @@ struct KernelTable
     cudaError_t (*reduce)(const ReduceArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s);
     cudaError_t (*ll)(const LLArgs& a, int dtype, int op, cudaStream_t s);
     cudaError_t (*group)(const GroupArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s);
+    cudaError_t (*groupReduceScatter)(const GroupArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s);
+    cudaError_t (*groupAllGather)(const GroupArgs& a, int blocks, int threads, cudaStream_t s);
     cudaError_t (*move)(const MoveArgs& a, int width, int blocks, int threads, cudaStream_t s);
     // TMA bulk-copy engine (fixed block size, 16-byte aligned ranges)
     cudaError_t (*moveBulk)(const MoveArgs& a, int blocks, cudaStream_t s);
@@ -49,6 +51,8 @@ bool reducible(int dtype, int op);
 cudaError_t reduceKernel(const ReduceArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s);
 cudaError_t llAllReduce(const LLArgs& a, int dtype, int op, cudaStream_t s);
 cudaError_t groupAllReduce(const GroupArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s); // a.segs: HOST memory
+cudaError_t groupReduceScatter(const GroupArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s);
+cudaError_t groupAllGather(const GroupArgs& a, int blocks, int threads, cudaStream_t s);
 // The move, p2p and put twins return cudaErrorMisalignedAddress, before they
 // copy or synchronise, when an address the kernel reads or writes in words of
 // `width` bytes is not aligned to it (moveBulk: 16 bytes)

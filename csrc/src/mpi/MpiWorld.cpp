@@ -72,8 +72,11 @@ struct RankState
     // Non-blocking device collectives rotate over the communicator's
     // channels (every rank issues the same sequence => same channel)
     uint64_t deviceCollectiveSeq = 0;
-    // MPI_Iallreduce burst on symmetric device buffers: deferred and issued
-    // as ONE grouped kernel at the next wait (or any other device operation)
+    // MPI_Iallreduce, MPI_Ireduce_scatter_block or MPI_Iallgather burst on
+    // symmetric device buffers: deferred and issued as ONE grouped kernel at
+    // the next wait (or any other device operation).  A burst has one key:
+    // (kind, communicator, dtype, op); all-gather bursts are bytes, no op.
+    faabric::device::Communicator::GroupKind groupKind = faabric::device::Communicator::GROUP_ALLREDUCE;
     std::shared_ptr<faabric::device::Communicator> groupComm;
     int groupDtype = -1;
     int groupOp = -1;
@@ -902,10 +905,11 @@ int MpiWorld::irecv(int sendRank,
     return requestId;
 }
 
-// Issues the deferred MPI_Iallreduce burst of this rank thread as one grouped
-// launch (every rank defers and flushes at the same program points)
+// Issues the deferred burst of this rank thread as one grouped launch (every
+// rank defers and flushes at the same program points)
 static void flushPendingGroup()
 {
+    using faabric::device::Communicator;
     if (tls.groupItems.empty()) {
         return;
     }
@@ -920,11 +924,21 @@ static void flushPendingGroup()
     tls.groupRequests.clear();
     tls.groupComm = nullptr;
     cudaSetDevice(comm->device());
-    int rc = comm->allReduceMany(
-      items.data(), items.size(), tls.groupDtype, tls.groupOp, FB_FLAG_SYMMETRIC, (cudaStream_t)tls.groupStream);
+    const cudaStream_t s = (cudaStream_t)tls.groupStream;
+    int rc;
+    const char* what;
+    if (tls.groupKind == Communicator::GROUP_REDUCE_SCATTER) {
+        rc = comm->reduceScatterMany(items.data(), items.size(), tls.groupDtype, tls.groupOp, FB_FLAG_SYMMETRIC, s);
+        what = "reduce-scatter";
+    } else if (tls.groupKind == Communicator::GROUP_ALLGATHER) {
+        rc = comm->allGatherMany(items.data(), items.size(), tls.groupDtype, FB_FLAG_SYMMETRIC, s);
+        what = "all-gather";
+    } else {
+        rc = comm->allReduceMany(items.data(), items.size(), tls.groupDtype, tls.groupOp, FB_FLAG_SYMMETRIC, s);
+        what = "all-reduce";
+    }
     if (rc != FB_OK) {
-        throw std::runtime_error(std::string("Grouped device all-reduce failed: ") +
-                                 faabric::device::Communicator::errorString(rc));
+        throw std::runtime_error(std::string("Grouped device ") + what + " failed: " + Communicator::errorString(rc));
     }
     const uint64_t seq = ++tls.groupLaunchSeq;
     for (int id : reqs) {
@@ -1359,6 +1373,47 @@ bool MpiWorld::deviceAllToAll(const DeviceComm& comm, int rank, const uint8_t* s
 
 #undef FB_DEVICE_BRANCH
 
+void MpiWorld::cacheDeviceComm(int rank)
+{
+    if (!tls.cachedCommValid || tls.cachedCommRank != rank) {
+        tls.cachedComm = getDeviceComm(rank);
+        tls.cachedStream0 = tls.cachedComm != nullptr ? streamForRank(rank, 0) : nullptr;
+        tls.cachedCommRank = rank;
+        tls.cachedCommValid = true;
+    }
+}
+
+// Adds one call to this rank thread's deferred burst, flushing first a burst
+// of another key (or one that is full)
+static void deferToGroup(faabric::device::Communicator::GroupKind kind,
+                         const std::shared_ptr<faabric::device::Communicator>& comm,
+                         int dtype,
+                         int op,
+                         const faabric::device::Communicator::GroupItem& item,
+                         int requestId,
+                         AsyncRequest r,
+                         std::atomic<uint64_t>& counter)
+{
+    if (!tls.groupItems.empty() && (tls.groupKind != kind || tls.groupComm != comm || tls.groupDtype != dtype ||
+                                    tls.groupOp != op || tls.groupItems.size() >= 4096)) {
+        flushPendingGroup();
+    }
+    tls.groupKind = kind;
+    tls.groupComm = comm;
+    tls.groupDtype = dtype;
+    tls.groupOp = op;
+    tls.groupStream = tls.cachedStream0;
+    tls.groupItems.push_back(item);
+    tls.groupRequests.push_back(requestId);
+    tls.deferredCount++; // added to the world's counter at the flush
+    tls.deferredCounter = &counter;
+    r.isDeviceCollective = true;
+    r.deferred = true;
+    r.stream = tls.groupStream;
+    r.comm = comm;
+    tls.requests[requestId] = r;
+}
+
 int MpiWorld::iAllReduce(int rank, uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count, faabric_op_t* op)
 {
     checkRanksRange(0, rank);
@@ -1370,12 +1425,7 @@ int MpiWorld::iAllReduce(int rank, uint8_t* send, uint8_t* recv, faabric_datatyp
     r.recvRank = rank;
     int fdt = fbDtypeFor(dt);
     int fop = fbOpFor(op);
-    if (!tls.cachedCommValid || tls.cachedCommRank != rank) {
-        tls.cachedComm = getDeviceComm(rank);
-        tls.cachedStream0 = tls.cachedComm != nullptr ? streamForRank(rank, 0) : nullptr;
-        tls.cachedCommRank = rank;
-        tls.cachedCommValid = true;
-    }
+    cacheDeviceComm(rank);
     std::shared_ptr<faabric::device::Communicator> comm;
     bool symmetric = false;
     if (bytes > 0 && fdt >= 0 && fop >= 0 && tls.cachedComm != nullptr) {
@@ -1390,23 +1440,14 @@ int MpiWorld::iAllReduce(int rank, uint8_t* send, uint8_t* recv, faabric_datatyp
         // staging area on channel 0
         if (symmetric && ((((uintptr_t)send) | ((uintptr_t)recv)) & 15) == 0 && groupIallreduce) {
             // Deferred: the whole burst becomes ONE kernel at the next wait
-            if (!tls.groupItems.empty() &&
-                (tls.groupComm != comm || tls.groupDtype != fdt || tls.groupOp != fop || tls.groupItems.size() >= 4096)) {
-                flushPendingGroup();
-            }
-            tls.groupComm = comm;
-            tls.groupDtype = fdt;
-            tls.groupOp = fop;
-            tls.groupStream = tls.cachedStream0;
-            tls.groupItems.push_back({ send, recv, (size_t)count });
-            tls.groupRequests.push_back(requestId);
-            tls.deferredCount++; // added to the world's counter at the flush
-            tls.deferredCounter = &deviceCollectives;
-            r.isDeviceCollective = true;
-            r.deferred = true;
-            r.stream = tls.groupStream;
-            r.comm = comm;
-            tls.requests[requestId] = r;
+            deferToGroup(faabric::device::Communicator::GROUP_ALLREDUCE,
+                         comm,
+                         fdt,
+                         fop,
+                         { send, recv, (size_t)count },
+                         requestId,
+                         r,
+                         deviceCollectives);
             return requestId;
         }
         flushPendingGroup();
@@ -1430,6 +1471,119 @@ int MpiWorld::iAllReduce(int rank, uint8_t* send, uint8_t* recv, faabric_datatyp
     }
     // Host path (or unsupported on the device): complete it now
     allReduce(rank, send, recv, dt, count, op);
+    tls.requests[requestId] = r;
+    return requestId;
+}
+
+// Issues one device collective of a non-blocking call on channel 0: the
+// request completes when the stream drains.  False if the device cannot run it.
+static bool issueDeviceRequest(const std::shared_ptr<faabric::device::Communicator>& comm,
+                               void* stream,
+                               std::atomic<uint64_t>& counter,
+                               int requestId,
+                               AsyncRequest& r,
+                               const std::function<int(faabric::device::Communicator&, cudaStream_t)>& fn)
+{
+    flushPendingGroup();
+    cudaStream_t s = (cudaStream_t)stream;
+    cudaSetDevice(comm->device());
+    int rc = fn(*comm, s);
+    if (rc == FB_E_UNSUPPORTED || rc == FB_E_TOO_LARGE) {
+        return false;
+    }
+    if (rc != FB_OK) {
+        throw std::runtime_error(std::string("Device collective failed: ") + faabric::device::Communicator::errorString(rc));
+    }
+    counter.fetch_add(1);
+    r.isDeviceCollective = true;
+    r.stream = s;
+    r.comm = comm;
+    tls.requests[requestId] = r;
+    return true;
+}
+
+int MpiWorld::iReduceScatter(int rank,
+                             uint8_t* send,
+                             uint8_t* recv,
+                             faabric_datatype_t* dt,
+                             int recvCount,
+                             faabric_op_t* op)
+{
+    using faabric::device::Communicator;
+    checkRanksRange(0, rank);
+    const size_t shard = (size_t)recvCount * dt->size;
+    int requestId = tls.nextRequestId++;
+    AsyncRequest r;
+    r.isSend = true; // nothing to drain on wait unless it becomes a device op
+    r.sendRank = rank;
+    r.recvRank = rank;
+    const int fdt = fbDtypeFor(dt);
+    const int fop = fbOpFor(op);
+    cacheDeviceComm(rank);
+    auto comm = tls.cachedComm;
+    // In place, the output overwrites input the peers are still reading: that
+    // case (send == recv) runs the blocking call below
+    if (shard > 0 && fdt >= 0 && fop >= 0 && comm != nullptr && send != recv) {
+        const bool symmetric = comm->inHeap(send, shard * size) && comm->inHeap(recv, shard);
+        if (symmetric && shard % 16 == 0 && ((((uintptr_t)send) | ((uintptr_t)recv)) & 15) == 0 && groupIallreduce) {
+            deferToGroup(Communicator::GROUP_REDUCE_SCATTER,
+                         comm,
+                         fdt,
+                         fop,
+                         { send, recv, (size_t)recvCount },
+                         requestId,
+                         r,
+                         deviceCollectives);
+            return requestId;
+        }
+        if ((symmetric || isDevicePointer(send)) &&
+            issueDeviceRequest(comm, streamForRank(rank, 0), deviceCollectives, requestId, r, [&](Communicator& c, cudaStream_t s) {
+                return c.reduceScatter(send, recv, (size_t)recvCount, fdt, fop, symFlag(c, send, shard * size), s);
+            })) {
+            return requestId;
+        }
+    }
+    // Host buffers, in place, or unsupported on the device: complete it now
+    reduceScatter(rank, send, recv, dt, recvCount, op);
+    tls.requests[requestId] = r;
+    return requestId;
+}
+
+int MpiWorld::iAllGather(int rank,
+                         const uint8_t* send,
+                         faabric_datatype_t* sendType,
+                         int sendCount,
+                         uint8_t* recv,
+                         faabric_datatype_t* recvType,
+                         int recvCount)
+{
+    using faabric::device::Communicator;
+    checkRanksRange(0, rank);
+    const size_t bytes = (size_t)sendCount * sendType->size;
+    int requestId = tls.nextRequestId++;
+    AsyncRequest r;
+    r.isSend = true; // nothing to drain on wait unless it becomes a device op
+    r.sendRank = rank;
+    r.recvRank = rank;
+    cacheDeviceComm(rank);
+    auto comm = tls.cachedComm;
+    if (bytes > 0 && comm != nullptr) {
+        const bool inPlace = send == recv + (size_t)rank * bytes;
+        const bool symmetric = comm->inHeap(send, bytes) && comm->inHeap(recv, bytes * size);
+        if (symmetric && bytes % 16 == 0 && ((((uintptr_t)send) | ((uintptr_t)recv)) & 15) == 0 && groupIallreduce) {
+            // a byte copy: the burst's key is the communicator alone
+            deferToGroup(Communicator::GROUP_ALLGATHER, comm, FB_U8, -1, { send, recv, bytes }, requestId, r, deviceCollectives);
+            return requestId;
+        }
+        if (!inPlace && (symmetric || isDevicePointer(send)) &&
+            issueDeviceRequest(comm, streamForRank(rank, 0), deviceCollectives, requestId, r, [&](Communicator& c, cudaStream_t s) {
+                return c.allGather(send, recv, bytes, symFlag(c, send, bytes), s);
+            })) {
+            return requestId;
+        }
+    }
+    // Host buffers, or unsupported on the device: complete it now
+    allGather(rank, send, sendType, sendCount, recv, recvType, recvCount);
     tls.requests[requestId] = r;
     return requestId;
 }

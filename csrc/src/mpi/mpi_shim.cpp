@@ -908,6 +908,58 @@ int MPI_Iallreduce(const void* sendbuf, void* recvbuf, int count, MPI_Datatype d
     return MPI_SUCCESS;
 }
 
+int MPI_Reduce_scatter_block(const void* sendbuf, void* recvbuf, int recvcount, MPI_Datatype datatype,
+                             MPI_Op op, MPI_Comm comm)
+{
+    SPDLOG_TRACE("MPI - MPI_Reduce_scatter_block");
+    if (accumulateOnlyOp(op)) {
+        return MPI_ERR_OP;
+    }
+    subCommOnly(comm, "MPI_Reduce_scatter_block");
+    getExecutingWorld().reduceScatter(executingContext.getRank(), (uint8_t*)resolveInPlace(sendbuf, recvbuf),
+                                      (uint8_t*)recvbuf, datatype, recvcount, op);
+    return MPI_SUCCESS;
+}
+
+int MPI_Ireduce_scatter_block(const void* sendbuf, void* recvbuf, int recvcount, MPI_Datatype datatype,
+                              MPI_Op op, MPI_Comm comm, MPI_Request* request)
+{
+    SPDLOG_TRACE("MPI - MPI_Ireduce_scatter_block");
+    if (accumulateOnlyOp(op)) {
+        return MPI_ERR_OP;
+    }
+    subCommOnly(comm, "MPI_Ireduce_scatter_block");
+    int id = getExecutingWorld().iReduceScatter(executingContext.getRank(),
+                                                (uint8_t*)resolveInPlace(sendbuf, recvbuf),
+                                                (uint8_t*)recvbuf,
+                                                datatype,
+                                                recvcount,
+                                                op);
+    auto* r = new faabric_request_t{ id };
+    requestTable()[id] = r;
+    *request = r;
+    return MPI_SUCCESS;
+}
+
+int MPI_Iallgather(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                   MPI_Datatype recvtype, MPI_Comm comm, MPI_Request* request)
+{
+    SPDLOG_TRACE("MPI - MPI_Iallgather");
+    subCommOnly(comm, "MPI_Iallgather");
+    int rank = executingContext.getRank();
+    const uint8_t* send = (const uint8_t*)sendbuf;
+    if (sendbuf == MPI_IN_PLACE) {
+        send = (const uint8_t*)recvbuf + (size_t)rank * recvcount * recvtype->size;
+        sendcount = recvcount;
+        sendtype = recvtype;
+    }
+    int id = getExecutingWorld().iAllGather(rank, send, sendtype, sendcount, (uint8_t*)recvbuf, recvtype, recvcount);
+    auto* r = new faabric_request_t{ id };
+    requestTable()[id] = r;
+    *request = r;
+    return MPI_SUCCESS;
+}
+
 int MPI_Get_processor_name(char* name, int* resultlen)
 {
     SPDLOG_TRACE("MPI - MPI_Get_processor_name");

@@ -125,6 +125,12 @@ def load():
     _sig(lib, "fb_group_plan_launches", i32, [vp])
     _sig(lib, "fb_group_plan_free", None, [vp])
     _sig(lib, "fb_allreduce_many", i32, [vp, i32, vpp, vpp, u64p, i32, i32, i32, vp])
+    _sig(lib, "fb_group_prepare_reduce_scatter", vp, [vp, i32, vpp, vpp, u64p, i32])
+    _sig(lib, "fb_group_prepare_all_gather", vp, [vp, i32, vpp, vpp, u64p, i32])
+    _sig(lib, "fb_group_reduce_scatter", i32, [vp, vp, i32, i32, vp])
+    _sig(lib, "fb_group_all_gather", i32, [vp, vp, i32, vp])
+    _sig(lib, "fb_reduce_scatter_many", i32, [vp, i32, vpp, vpp, u64p, i32, i32, i32, vp])
+    _sig(lib, "fb_all_gather_many", i32, [vp, i32, vpp, vpp, u64p, i32, i32, vp])
     _sig(lib, "fb_put_signal", i32, [vp, vp, u64, u64, i32, i32, i32, vp])
     _sig(lib, "fb_wait_signal", i32, [vp, i32, u32, vp])
     _sig(lib, "fb_accumulate", i32, [vp, vp, u64, u64, i32, i32, i32, vp, vp])

@@ -489,6 +489,81 @@ class Communicator:
         rc = self._lib.fb_allreduce_many(self._h, n, sp, rp, cnt, dt, OPS[op], f, self._stream(stream))
         self._check(rc, "all_reduce_many")
 
+    # ------------------------------ grouped reduce-scatter and all-gather
+    def _shard_arrays(self, what, sends, recvs, dtype, gather):
+        """(n, send ptrs, recv ptrs, per-rank counts, FbDtype) of a shard group;
+        raises before any native call when a shape does not fit: reduce-scatter
+        needs send.numel() == size * recv.numel(), all-gather the reverse."""
+        if len(sends) != len(recvs) or not sends:
+            raise CommError(f"{what}: need equally long, non-empty lists")
+        for i, (s, r) in enumerate(zip(sends, recvs)):
+            small, big = (s, r) if gather else (r, s)
+            if big.numel() != self.size * small.numel():
+                raise CommError(
+                    f"{what}: item {i} has {s.numel()} send and {r.numel()} recv elements; "
+                    f"{'recv' if gather else 'send'} must hold {self.size} x {'send' if gather else 'recv'}"
+                )
+        n = len(sends)
+        sp = (C.c_void_p * n)(*[t.data_ptr() for t in sends])
+        rp = (C.c_void_p * n)(*[t.data_ptr() for t in recvs])
+        typed = [self._typed(s if gather else r, dtype) for s, r in zip(sends, recvs)]
+        if len({dt for _, dt in typed}) != 1:
+            raise CommError(f"{what}: every tensor must have the same dtype")
+        cnt = (C.c_uint64 * n)(*[c for c, _ in typed])
+        return n, sp, rp, cnt, typed[0][1]
+
+    def prepare_reduce_scatter_group(self, sends, recvs, dtype=None) -> "GroupPlan":
+        """Plan ONE launch that reduce-scatters every pair of the lists
+        (MPI_Reduce_scatter_block per pair: ``recvs[i]`` gets this rank's
+        shard of the reduction of ``sends[i]`` over the ranks).  Tensors live in
+        the symmetric heap at 16-byte aligned addresses, shards are multiples
+        of 16 bytes, and no output overlaps an input; call collectively with
+        the same lists."""
+        n, sp, rp, cnt, dt = self._shard_arrays("prepare_reduce_scatter_group", sends, recvs, dtype, False)
+        h = self._lib.fb_group_prepare_reduce_scatter(self._h, n, sp, rp, cnt, dt)
+        if not h:
+            raise CommError(f"prepare_reduce_scatter_group failed [{_lib.last_error()}]")
+        return GroupPlan(self, h, n, sum(t.numel() * t.element_size() for t in sends))
+
+    def prepare_all_gather_group(self, sends, recvs, dtype=None) -> "GroupPlan":
+        """Plan ONE launch that all-gathers every pair of the lists
+        (MPI_Allgather per pair: block p of ``recvs[i]`` gets ``sends[i]`` of
+        rank p).  Same conditions as :meth:`prepare_reduce_scatter_group`; in
+        place (``sends[i]`` is block ``rank`` of ``recvs[i]``) is allowed."""
+        n, sp, rp, cnt, dt = self._shard_arrays("prepare_all_gather_group", sends, recvs, dtype, True)
+        h = self._lib.fb_group_prepare_all_gather(self._h, n, sp, rp, cnt, dt)
+        if not h:
+            raise CommError(f"prepare_all_gather_group failed [{_lib.last_error()}]")
+        return GroupPlan(self, h, n, sum(t.numel() * t.element_size() for t in recvs))
+
+    def reduce_scatter_group(self, plan: "GroupPlan", op="sum", stream=None, channel=0, flags=FLAG_SYMMETRIC):
+        rc = self._lib.fb_group_reduce_scatter(
+            self._h, plan._h, OPS[op], flags | ((channel & 0xF) << 8), self._stream(stream)
+        )
+        self._check(rc, "reduce_scatter_group")
+
+    def all_gather_group(self, plan: "GroupPlan", stream=None, channel=0, flags=FLAG_SYMMETRIC):
+        rc = self._lib.fb_group_all_gather(self._h, plan._h, flags | ((channel & 0xF) << 8), self._stream(stream))
+        self._check(rc, "all_gather_group")
+
+    def reduce_scatter_many(self, sends, recvs, op="sum", stream=None, channel=0, dtype=None):
+        """Transient variant of :meth:`prepare_reduce_scatter_group` +
+        :meth:`reduce_scatter_group`; lists that cannot be grouped run one
+        :meth:`reduce_scatter` per pair."""
+        n, sp, rp, cnt, dt = self._shard_arrays("reduce_scatter_many", sends, recvs, dtype, False)
+        f = self._sym(*sends) | ((channel & 0xF) << 8)
+        rc = self._lib.fb_reduce_scatter_many(self._h, n, sp, rp, cnt, dt, OPS[op], f, self._stream(stream))
+        self._check(rc, "reduce_scatter_many")
+
+    def all_gather_many(self, sends, recvs, stream=None, channel=0, dtype=None):
+        """Transient variant of :meth:`prepare_all_gather_group` +
+        :meth:`all_gather_group`; lists that cannot be grouped run one
+        :meth:`all_gather` per pair."""
+        n, sp, rp, cnt, dt = self._shard_arrays("all_gather_many", sends, recvs, dtype, True)
+        f = self._sym(*sends) | ((channel & 0xF) << 8)
+        rc = self._lib.fb_all_gather_many(self._h, n, sp, rp, cnt, dt, f, self._stream(stream))
+        self._check(rc, "all_gather_many")
+
     def send_recv(self, send_buf, dst, recv_buf, src, stream=None):
         rc = self._lib.fb_sendrecv(
             self._h,
@@ -632,7 +707,8 @@ class Communicator:
 
 
 class GroupPlan:
-    """Device-resident segment tables of a grouped all-reduce."""
+    """Device-resident segment tables of a grouped all-reduce, reduce-scatter
+    or all-gather."""
 
     def __init__(self, comm: Communicator, handle, n_tensors: int, nbytes: int):
         self._comm = comm
