@@ -25,6 +25,7 @@
 
 #include "../tests/mpi_rma_atomics_body.h"
 #include "../tests/mpi_rma_passive_body.h"
+#include "../tests/mpi_rma_request_body.h"
 #include "../tests/mpi_subcomm_device_body.h"
 
 #include <cuda_runtime.h>
@@ -757,6 +758,29 @@ static void registerFunctions()
         return rc;
     });
 
+    // Request-based one-sided operations (MPI_Rput, MPI_Rget, MPI_Raccumulate,
+    // MPI_Rget_accumulate) with targets in this process and in other ones.
+    // Input: "host" | "cuda" | "heap" window memory, then ",device" for
+    // origin and result buffers in cudaMalloc memory or ",heapbuf" for
+    // buffers in the origin's symmetric heap.
+    mpiFunction("rma-request", [](int rank, int size, faabric::Message& msg) {
+        const std::string& in = msg.inputdata();
+        rma_request::Setup s;
+        s.window = in.rfind("cuda", 0) == 0   ? rma_request::WindowMemory::CudaMalloc
+                   : in.rfind("heap", 0) == 0 ? rma_request::WindowMemory::Heap
+                                              : rma_request::WindowMemory::Host;
+        s.origin = in.find(",device") != std::string::npos    ? rma_request::Origin::Device
+                   : in.find(",heapbuf") != std::string::npos ? rma_request::Origin::Heap
+                                                              : rma_request::Origin::Host;
+        std::string why;
+        int rc = rma_request::body(rank, size, msg.mpiworldid(), s, &why);
+        if (rc != 0) {
+            SPDLOG_ERROR("rma-request: {}", why);
+            msg.set_outputdata(why);
+        }
+        return rc;
+    });
+
     // Fused device collectives on sub-communicators (mpi_subcomm_device_body.h).
     // Input: "heap" (symmetric heap buffers) or "cuda" (cudaMalloc buffers).
     mpiFunction("subcomm-device", [](int rank, int size, faabric::Message& msg) {
@@ -1020,6 +1044,87 @@ static void registerFunctions()
         } else {
             free(window);
         }
+        return 0;
+    });
+
+    // Cost of request-based puts against plain ones: rank 0 writes K
+    // operations of B bytes from device memory into rank 1's symmetric-heap
+    // window inside MPI_Win_lock_all, then completes them.  Input
+    // "mode;B;K;iters":
+    //   rput  MPI_Rput x K + MPI_Waitall + MPI_Win_flush
+    //   put   MPI_Put x K + MPI_Win_flush
+    // Operation k goes to slot k of the window (slots wrap at 16 MiB).  Rank 0
+    // reports {"us_per_op"}.
+    mpiFunction("bench-rma-request", [](int rank, int size, faabric::Message& msg) {
+        std::vector<std::string> f;
+        std::string cur;
+        for (char c : msg.inputdata() + ";") {
+            if (c == ';') {
+                f.push_back(cur);
+                cur.clear();
+            } else {
+                cur += c;
+            }
+        }
+        EXPECT(f.size() >= 4 && size >= 2);
+        const bool rput = f[0] == "rput";
+        const size_t bytes = std::stoull(f[1]);
+        const int K = std::stoi(f[2]);
+        const int iters = std::stoi(f[3]);
+        EXPECT(bytes > 0 && bytes <= ((size_t)16 << 20) && K > 0 && iters > 0);
+        const size_t slots = std::min<size_t>((size_t)K, ((size_t)16 << 20) / bytes);
+        const size_t winBytes = slots * bytes;
+        uint8_t* window = nullptr;
+        EXPECT(MPI_Alloc_mem(winBytes, MPI_INFO_FAABRIC_DEVICE, &window) == MPI_SUCCESS);
+        uint8_t* src = nullptr;
+        EXPECT(cudaMalloc((void**)&src, (size_t)K * bytes) == cudaSuccess);
+        cudaMemset(src, rank + 1, (size_t)K * bytes);
+        cudaMemset(window, 0, winBytes);
+        cudaDeviceSynchronize();
+        MPI_Win win = nullptr;
+        MPI_Win_create(window, winBytes, 1, MPI_INFO_NULL, MPI_COMM_WORLD, &win);
+        std::vector<MPI_Request> reqs(K, nullptr);
+        auto step = [&]() {
+            for (int k = 0; k < K; k++) {
+                const uint8_t* o = src + (size_t)k * bytes;
+                const MPI_Aint disp = (MPI_Aint)((k % slots) * bytes);
+                int rc = rput ? MPI_Rput(o, (int)bytes, MPI_BYTE, 1, disp, (int)bytes, MPI_BYTE, win, &reqs[k])
+                              : MPI_Put(o, (int)bytes, MPI_BYTE, 1, disp, (int)bytes, MPI_BYTE, win);
+                if (rc != MPI_SUCCESS) {
+                    return rc;
+                }
+            }
+            if (rput) {
+                int rc = MPI_Waitall(K, reqs.data(), MPI_STATUSES_IGNORE);
+                if (rc != MPI_SUCCESS) {
+                    return rc;
+                }
+            }
+            return MPI_Win_flush(1, win);
+        };
+        double us = 0;
+        if (rank == 0) {
+            EXPECT(MPI_Win_lock_all(0, win) == MPI_SUCCESS);
+            for (int i = 0; i < 3; i++) {
+                EXPECT(step() == MPI_SUCCESS);
+            }
+            auto t0 = std::chrono::steady_clock::now();
+            for (int i = 0; i < iters; i++) {
+                EXPECT(step() == MPI_SUCCESS);
+            }
+            us = std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count() / ((double)iters * K);
+            EXPECT(MPI_Win_unlock_all(win) == MPI_SUCCESS);
+            msg.set_outputdata("{\"us_per_op\": " + std::to_string(us) + "}");
+        }
+        MPI_Win_free(&win);
+        if (rank == 1) {
+            // what arrived is rank 0's bytes
+            std::vector<uint8_t> got(winBytes);
+            cudaMemcpy(got.data(), window, winBytes, cudaMemcpyDeviceToHost);
+            EXPECT(std::all_of(got.begin(), got.end(), [](uint8_t b) { return b == 1; }));
+        }
+        cudaFree(src);
+        MPI_Free_mem(window);
         return 0;
     });
 

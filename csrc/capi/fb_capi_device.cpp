@@ -762,6 +762,30 @@ int fb_compare_and_swap(void* h,
     return COMM(h)->compareAndSwap(compare, swap, result, dstOffset, dtype, peer, (cudaStream_t)stream);
 }
 
+// Batched one-sided copies (Communicator::putGetMany): item i copies bytes[i]
+// between local[i] and peer[i]'s symmetric heap at offset[i], towards the
+// heap when get[i] is 0 and out of it otherwise
+int fb_put_get_many(void* h,
+                    int n,
+                    void* const* local,
+                    const uint64_t* offset,
+                    const uint64_t* bytes,
+                    const int32_t* peer,
+                    const int32_t* get,
+                    void* stream)
+{
+    if (n < 0 || (n > 0 && (local == nullptr || offset == nullptr || bytes == nullptr || peer == nullptr || get == nullptr))) {
+        return FB_E_INVALID;
+    }
+    FB_TRY
+    std::vector<Communicator::RmaCopy> items(n);
+    for (int i = 0; i < n; i++) {
+        items[i] = Communicator::RmaCopy{ local[i], offset[i], (size_t)bytes[i], peer[i], get[i] != 0 ? 1 : 0 };
+    }
+    return COMM(h)->putGetMany(items.data(), items.size(), (cudaStream_t)stream);
+    FB_CATCH(FB_E_CUDA)
+}
+
 const char* fb_error_string(int code)
 {
     return Communicator::errorString(code);

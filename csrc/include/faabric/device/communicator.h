@@ -375,6 +375,25 @@ class Communicator : public std::enable_shared_from_this<Communicator>
                        int dtype,
                        int peer,
                        cudaStream_t s);
+    // ---- batched one-sided copies (request-based MPI_Rput / MPI_Rget) ----
+    struct RmaCopy
+    {
+        void* local;     // memory this rank's GPU can load and store
+        uint64_t offset; // user part of peer's symmetric heap
+        size_t bytes;
+        int peer;
+        int get; // 0: local -> peer's heap at offset; 1: the other way
+    };
+    // Every item of the list, as one launch per FB_RMA_COPY_MAX_ITEMS items
+    // (in order, on `s`).  Stream-ordered, never synchronises the host;
+    // `peer == rank()` is allowed; any alignment and length.  Every item is
+    // checked before anything is launched: a peer out of range, a null
+    // `local`, or a range outside the peer's user heap gives FB_E_INVALID; a
+    // sub-communicator gives FB_E_UNSUPPORTED.  Zero-byte items are skipped
+    // (only their peer is checked).
+    // Destinations that overlap within one list (or a destination that
+    // overlaps a source) leave unspecified bytes there.
+    int putGetMany(const RmaCopy* items, size_t n, cudaStream_t s);
 
     // Device watchdog error word (FB_ERR_*); synchronises `s`
     uint32_t checkError(cudaStream_t s);
@@ -442,10 +461,13 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     bool streamWriteOk_ = false;
     cudaStream_t internalStream_ = nullptr;
     uint32_t doneSeq_ = 0;
-    // transient group tables (allReduceMany)
+    // transient group tables (allReduceMany) and copy tables (putGetMany)
     struct ManySlot;
     std::vector<std::shared_ptr<ManySlot>> manySlots_;
     size_t manyNext_ = 0;
+    // The next table slot, free for the host to write (waits for the launch
+    // that used it last); null on a CUDA error
+    ManySlot* nextManySlot();
     uint64_t stageSendOff_ = 0;
     uint64_t stageRecvOff_ = 0;
     uint64_t userOff_ = 0;

@@ -383,6 +383,23 @@ extern "C"
     int MPI_Win_flush_local(int rank, MPI_Win win);
     int MPI_Win_flush_local_all(MPI_Win win);
     int MPI_Win_sync(MPI_Win win);
+    /* Request-based operations, inside a passive epoch that covers the
+     * target.  After MPI_Wait* on the request the origin buffer may be reused
+     * (put, accumulate) or holds the data (get, get-accumulate).
+     * MPI_Win_flush* and MPI_Win_unlock* complete them too. */
+    int MPI_Rput(const void* origin_addr, int origin_count, MPI_Datatype origin_datatype, int target_rank,
+                 MPI_Aint target_disp, int target_count, MPI_Datatype target_datatype, MPI_Win win,
+                 MPI_Request* request);
+    int MPI_Rget(void* origin_addr, int origin_count, MPI_Datatype origin_datatype, int target_rank,
+                 MPI_Aint target_disp, int target_count, MPI_Datatype target_datatype, MPI_Win win,
+                 MPI_Request* request);
+    int MPI_Raccumulate(const void* origin_addr, int origin_count, MPI_Datatype origin_datatype, int target_rank,
+                        MPI_Aint target_disp, int target_count, MPI_Datatype target_datatype, MPI_Op op,
+                        MPI_Win win, MPI_Request* request);
+    int MPI_Rget_accumulate(const void* origin_addr, int origin_count, MPI_Datatype origin_datatype,
+                            void* result_addr, int result_count, MPI_Datatype result_datatype, int target_rank,
+                            MPI_Aint target_disp, int target_count, MPI_Datatype target_datatype, MPI_Op op,
+                            MPI_Win win, MPI_Request* request);
 
 #ifdef __cplusplus
 }

@@ -239,6 +239,11 @@ class MpiWorld
 
     void awaitAsyncRequest(int requestId);
 
+    // MPI_Request_free: drops a request-based one-sided operation's request
+    // (the operation completes at the next flush or unlock); other kinds of
+    // request are kept
+    void freeAsyncRequest(int requestId);
+
     void sendRecv(uint8_t* sendBuffer,
                   int sendCount,
                   faabric_datatype_t* sendDataType,
@@ -444,6 +449,42 @@ class MpiWorld
     // True while `rank` holds a lock (or lock-all) epoch on the window
     bool winInPassiveEpoch(int rank, int winId);
 
+    // ---- request-based operations (MPI_Rput, MPI_Rget, MPI_Raccumulate,
+    // MPI_Rget_accumulate).  Every check runs before anything is issued:
+    // MPI_ERR_WIN (unknown window), MPI_ERR_RANK, MPI_ERR_ARG (a range
+    // outside the target window, or the checks of winAccumulate) and
+    // MPI_ERR_RMA_SYNC (the target is not covered by a passive epoch of
+    // `rank`).  On success *requestId is a request of this rank thread,
+    // completed by awaitAsyncRequest.
+    //   symmetric heap in this process, origin on the origin's GPU (or in
+    //   its heap): deferred into the origin's batch for the window, issued
+    //   as one Communicator::putGetMany at the wait, flush or unlock (or
+    //   when the batch holds a launch's worth)
+    //   other segments in this process: winPut / winGet at issue
+    //   rank in another worker process: queued like MPI_Put, shipped at the
+    //   flush or unlock of the target, or at the wait
+    int winRputGet(int rank, int winId, uint8_t* origin, size_t bytes, int targetRank, int64_t targetDisp, bool get, int* requestId);
+    int winRaccumulate(int rank,
+                       int winId,
+                       const uint8_t* origin,
+                       size_t count,
+                       faabric_datatype_t* datatype,
+                       faabric_op_t* op,
+                       uint8_t* result,
+                       int targetRank,
+                       int64_t targetDisp,
+                       int* requestId);
+
+    // Completion sequences of one origin's request-based operations on one
+    // window, per target: a request numbered at most completed[target] is
+    // complete.  Requests hold it, so a wait after the window is freed
+    // never touches the window.
+    struct RmaProgress
+    {
+        std::vector<uint64_t> issued;
+        std::vector<uint64_t> completed;
+    };
+
     // A passive-target request from another worker process (a PointToPointCall
     // RMA_* code); returns the reply
     static std::string serveRmaRequest(int call, const uint8_t* buffer, size_t bytes);
@@ -612,6 +653,10 @@ class MpiWorld
         std::mutex lockMx;
         std::condition_variable lockCv;
         std::vector<RmaLock> locks;
+        // request-based operations, one entry per ORIGIN rank (only that
+        // rank's thread): deferred heap copies, and completion sequences
+        std::vector<std::vector<faabric::device::Communicator::RmaCopy>> batches;
+        std::vector<std::shared_ptr<RmaProgress>> progress;
     };
     std::mutex windowsMx;
     std::map<int, std::shared_ptr<RmaWindow>> windows;
@@ -647,6 +692,19 @@ class MpiWorld
     int rmaAcquire(RmaWindow& w, int winId, int rank, int targetRank, bool exclusive);
     // Completes `rank`'s operations to `targetRank`; `release` also unlocks
     int rmaComplete(RmaWindow& w, int winId, int rank, int targetRank, bool release);
+    // Issues `rank`'s deferred heap copies on the window (its stream joins
+    // the window's streams of `rank`)
+    void rmaIssueBatch(RmaWindow& w, int rank);
+    // Checks and numbering shared by the request-based calls: MPI_SUCCESS
+    // and the target address, or an MPI error code
+    int rmaRequestTarget(RmaWindow& w, int rank, int targetRank, int64_t targetDisp, size_t bytes, uint8_t** target);
+    // A request of this rank thread for the next operation of `rank` to
+    // `targetRank` (numbered in `progress`; null: it completed at issue)
+    int addRmaRequest(int rank, int winId, int targetRank, std::shared_ptr<RmaProgress> progress);
+    // The wait of a request-based operation whose sequence is not complete:
+    // the batch and streams of `rank` (target in this process), or the flush
+    // of the target (another process)
+    void rmaAwait(int rank, int winId, int targetRank);
     // Handles a request of serveRmaRequest on this world
     std::string rmaServe(int call, const uint8_t* buffer, size_t bytes);
     // Communicator of a rank if one is wired already (never creates one)

@@ -255,6 +255,38 @@ cudaError_t launchRmaAccumulate(const RmaArgs& a, int dtype, int op, cudaStream_
 cudaError_t launchRmaCompareSwap(const RmaCasArgs& a, int dtype, cudaStream_t s);
 cudaError_t preloadRmaKernels();
 
+// Batched copy (rmaCopyManyKernel): every descriptor copies `bytes` from src
+// to dst, two addresses the launching GPU can load and store (its own memory,
+// or a peer's heap through FbCommDev::heap[peer]).  Any alignment, any
+// length.  The warps of the grid stride over the flat chunk space of the
+// table: item i owns chunks [chunk0, chunk0 + fbRmaCopyChunks(bytes)).  No
+// barrier, no flag words: the copy is complete when the stream passes the
+// kernel.  The table is the size of a GroupSeg table, so both share one ring
+// of staging slots.
+struct RmaCopyDesc
+{
+    const uint8_t* src;
+    uint8_t* dst;
+    uint64_t bytes;
+    uint64_t chunk0;
+};
+#define FB_RMA_COPY_MAX_ITEMS FB_GROUP_MAX_SEGS
+#define FB_RMA_COPY_CHUNK 2048 // bytes per warp-chunk (a multiple of 16)
+static inline uint64_t fbRmaCopyChunks(uint64_t bytes)
+{
+    return (bytes + FB_RMA_COPY_CHUNK - 1) / FB_RMA_COPY_CHUNK;
+}
+
+struct RmaCopyArgs
+{
+    const RmaCopyDesc* items; // device memory of the launching GPU
+    uint64_t totalChunks;
+    uint32_t nItems;
+    uint32_t pad;
+};
+
+cudaError_t launchRmaCopyMany(const RmaCopyArgs& a, cudaStream_t s);
+
 
 // ------------------------------------------------------------------ nvls ----
 enum NvlsMode

@@ -19,6 +19,9 @@
 // for 1- and 2-byte elements, or 128-bit for the 16-byte pairs, whose padding
 // is preserved.  Concurrent accumulates from any number of GPUs therefore
 // compose element by element.  The kernels never wait on a peer.
+//
+//  * rmaCopyManyKernel — a table of plain copies (request-based puts and gets
+//    on the symmetric heap): one launch for a whole list, any alignment.
 #include "fb_atomics.cuh"
 #include "fb_prims.cuh"
 #include "launch_api.h"
@@ -297,6 +300,186 @@ __global__ void rmaCompareSwapKernel(const RmaCasArgs a)
     stBytes<T>(a.result, old);
 }
 
+// ---------------------------------------------------------- batched copy ----
+static constexpr int RMA_COPY_THREADS = 256;
+static constexpr int RMA_COPY_UNROLL = 4;
+
+template<int W>
+struct CopyWord;
+template<>
+struct CopyWord<16>
+{
+    using T = Vec16;
+    static __device__ __forceinline__ T ld(const uint8_t* p) { return ldVec(p); }
+    static __device__ __forceinline__ void st(uint8_t* p, const T& v) { stVec(p, v); }
+};
+template<>
+struct CopyWord<8>
+{
+    using T = uint64_t;
+    static __device__ __forceinline__ T ld(const uint8_t* p)
+    {
+        T v;
+        asm volatile("ld.global.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+        return v;
+    }
+    static __device__ __forceinline__ void st(uint8_t* p, T v)
+    {
+        asm volatile("st.global.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+    }
+};
+template<>
+struct CopyWord<4>
+{
+    using T = uint32_t;
+    static __device__ __forceinline__ T ld(const uint8_t* p)
+    {
+        T v;
+        asm volatile("ld.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+        return v;
+    }
+    static __device__ __forceinline__ void st(uint8_t* p, T v)
+    {
+        asm volatile("st.global.u32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+    }
+};
+template<>
+struct CopyWord<2>
+{
+    using T = uint16_t;
+    static __device__ __forceinline__ T ld(const uint8_t* p)
+    {
+        T v;
+        asm volatile("ld.global.u16 %0, [%1];" : "=h"(v) : "l"(p) : "memory");
+        return v;
+    }
+    static __device__ __forceinline__ void st(uint8_t* p, T v)
+    {
+        asm volatile("st.global.u16 [%0], %1;" ::"l"(p), "h"(v) : "memory");
+    }
+};
+template<>
+struct CopyWord<1>
+{
+    using T = uint32_t;
+    static __device__ __forceinline__ T ld(const uint8_t* p)
+    {
+        T v;
+        asm volatile("ld.global.u8 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+        return v;
+    }
+    static __device__ __forceinline__ void st(uint8_t* p, T v)
+    {
+        asm volatile("st.global.u8 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+    }
+};
+
+// n words of W bytes, one warp: RMA_COPY_UNROLL loads in flight per lane
+// before their stores
+template<int W>
+__device__ __forceinline__ void copyWords(const uint8_t* s, uint8_t* d, uint32_t n, uint32_t lane)
+{
+    using C = CopyWord<W>;
+    for (uint32_t base = 0; base < n; base += 32 * RMA_COPY_UNROLL) {
+        typename C::T v[RMA_COPY_UNROLL];
+#pragma unroll
+        for (int u = 0; u < RMA_COPY_UNROLL; u++) {
+            const uint32_t i = base + u * 32 + lane;
+            if (i < n) {
+                v[u] = C::ld(s + (uint64_t)i * W);
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < RMA_COPY_UNROLL; u++) {
+            const uint32_t i = base + u * 32 + lane;
+            if (i < n) {
+                C::st(d + (uint64_t)i * W, v[u]);
+            }
+        }
+    }
+}
+
+// Item that owns chunk `ch`: usually `cur` again (a warp's chunks ascend),
+// otherwise a binary search over chunk0
+__device__ __forceinline__ uint32_t copyItemOf(const RmaCopyDesc* t, uint32_t n, uint32_t cur, uint64_t ch)
+{
+    if (t[cur].chunk0 <= ch && (cur + 1 == n || ch < t[cur + 1].chunk0)) {
+        return cur;
+    }
+    uint32_t lo = 0;
+    uint32_t hi = n - 1;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1) >> 1;
+        if (t[mid].chunk0 <= ch) {
+            lo = mid;
+        } else {
+            hi = mid - 1;
+        }
+    }
+    return lo;
+}
+
+// One chunk of an item: a head of single bytes up to the widest alignment
+// that src and dst share (mod 16), the middle in words of that width, a tail
+// of single bytes
+__global__ void __launch_bounds__(RMA_COPY_THREADS, 2) rmaCopyManyKernel(const RmaCopyArgs a)
+{
+    const uint32_t lane = threadIdx.x & 31;
+    const uint64_t warp = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint64_t nWarps = ((uint64_t)gridDim.x * blockDim.x) >> 5;
+    uint32_t cur = 0;
+    for (uint64_t ch = warp; ch < a.totalChunks; ch += nWarps) {
+        cur = copyItemOf(a.items, a.nItems, cur, ch);
+        const RmaCopyDesc it = a.items[cur];
+        const uint64_t lo = (ch - it.chunk0) * FB_RMA_COPY_CHUNK;
+        const uint64_t len = min((uint64_t)FB_RMA_COPY_CHUNK, it.bytes - lo);
+        const uint8_t* s = it.src + lo;
+        uint8_t* d = it.dst + lo;
+        const uint32_t mis = (uint32_t)(((uintptr_t)s ^ (uintptr_t)d) & 15);
+        const uint32_t w = mis == 0 ? 16 : (mis & -mis);
+        const uint32_t head = (uint32_t)min((uint64_t)((w - ((uintptr_t)s & (w - 1))) & (w - 1)), len);
+        if (lane < head) {
+            d[lane] = s[lane];
+        }
+        const uint32_t n = (uint32_t)((len - head) / w);
+        const uint8_t* sb = s + head;
+        uint8_t* db = d + head;
+        switch (w) {
+            case 16:
+                copyWords<16>(sb, db, n, lane);
+                break;
+            case 8:
+                copyWords<8>(sb, db, n, lane);
+                break;
+            case 4:
+                copyWords<4>(sb, db, n, lane);
+                break;
+            case 2:
+                copyWords<2>(sb, db, n, lane);
+                break;
+            default:
+                copyWords<1>(sb, db, n, lane);
+                break;
+        }
+        const uint32_t done = head + n * w;
+        if (lane < len - done) {
+            d[done + lane] = s[done + lane];
+        }
+    }
+}
+
+cudaError_t launchRmaCopyMany(const RmaCopyArgs& a, cudaStream_t s)
+{
+    if (a.nItems == 0 || a.totalChunks == 0) {
+        return cudaSuccess;
+    }
+    constexpr uint64_t warpsPerBlock = RMA_COPY_THREADS / 32;
+    const uint64_t want = (a.totalChunks + warpsPerBlock - 1) / warpsPerBlock;
+    const unsigned blocks = (unsigned)(want > 2 * FB_NUM_SMS ? 2 * FB_NUM_SMS : want);
+    void* args[] = { const_cast<RmaCopyArgs*>(&a) };
+    return cudaLaunchKernel((const void*)rmaCopyManyKernel, dim3(blocks), dim3(RMA_COPY_THREADS), args, 0, s);
+}
+
 // ------------------------------------------------------------- dispatch ----
 template<int DT, int OP, bool FETCH>
 static const void* kernelOrNull()
@@ -451,6 +634,9 @@ cudaError_t preloadRmaKernels()
         if (e == cudaSuccess && casKernel(dt) != nullptr) {
             e = cudaFuncGetAttributes(&attr, casKernel(dt));
         }
+    }
+    if (e == cudaSuccess) {
+        e = cudaFuncGetAttributes(&attr, (const void*)rmaCopyManyKernel);
     }
     return e;
 }

@@ -1244,6 +1244,7 @@ const fb::KernelTable CUDA_KERNELS = {
     .signalPeers = fb::launchSignalPeers,
     .rmaAccumulate = fb::launchRmaAccumulate,
     .rmaCompareSwap = fb::launchRmaCompareSwap,
+    .rmaCopyMany = fb::launchRmaCopyMany,
     .copy = cudaCopy,
     .copy2D = cudaCopy2D,
 };
@@ -1265,6 +1266,7 @@ const fb::KernelTable HOST_KERNELS = {
     .signalPeers = fb::host::signalPeers,
     .rmaAccumulate = fb::host::rmaAccumulate,
     .rmaCompareSwap = fb::host::rmaCompareSwap,
+    .rmaCopyMany = fb::host::rmaCopyMany,
     .copy = fb::host::copy,
     .copy2D = fb::host::copy2D,
 };
@@ -1819,6 +1821,31 @@ struct Communicator::ManySlot
     }
 };
 
+Communicator::ManySlot* Communicator::nextManySlot()
+{
+    // table slot: pinned staging + device copy, recycled after its launch
+    if (manySlots_.empty()) {
+        manySlots_.resize(8);
+    }
+    auto& slotPtr = manySlots_[manyNext_++ % manySlots_.size()];
+    if (!slotPtr) {
+        slotPtr = std::make_shared<ManySlot>();
+        slotPtr->device = device_;
+        if (cudaMalloc((void**)&slotPtr->dSegs, FB_GROUP_MAX_SEGS * sizeof(fb::GroupSeg)) != cudaSuccess ||
+            cudaHostAlloc((void**)&slotPtr->hSegs, FB_GROUP_MAX_SEGS * sizeof(fb::GroupSeg), cudaHostAllocDefault) !=
+              cudaSuccess ||
+            cudaEventCreateWithFlags(&slotPtr->ev, cudaEventDisableTiming) != cudaSuccess) {
+            cudaGetLastError();
+            slotPtr.reset();
+            return nullptr;
+        }
+    }
+    if (slotPtr->used) {
+        cudaEventSynchronize(slotPtr->ev);
+    }
+    return slotPtr.get();
+}
+
 size_t Communicator::groupPlanLaunches(const GroupPlan& plan)
 {
     return plan.launches.size();
@@ -2275,26 +2302,9 @@ int Communicator::groupMany(GroupKind kind,
         l.bytes = sb.bytes;
         ManySlot* slot = nullptr;
         if (!loop_) {
-            // table slot: pinned staging + device copy, recycled after its launch
-            if (manySlots_.empty()) {
-                manySlots_.resize(8);
-            }
-            auto& slotPtr = manySlots_[manyNext_++ % manySlots_.size()];
-            if (!slotPtr) {
-                slotPtr = std::make_shared<ManySlot>();
-                slotPtr->device = device_;
-                if (cudaMalloc((void**)&slotPtr->dSegs, FB_GROUP_MAX_SEGS * sizeof(fb::GroupSeg)) != cudaSuccess ||
-                    cudaHostAlloc((void**)&slotPtr->hSegs, FB_GROUP_MAX_SEGS * sizeof(fb::GroupSeg), cudaHostAllocDefault) !=
-                      cudaSuccess ||
-                    cudaEventCreateWithFlags(&slotPtr->ev, cudaEventDisableTiming) != cudaSuccess) {
-                    cudaGetLastError();
-                    slotPtr.reset();
-                    return FB_E_CUDA;
-                }
-            }
-            slot = slotPtr.get();
-            if (slot->used) {
-                cudaEventSynchronize(slot->ev);
+            slot = nextManySlot();
+            if (slot == nullptr) {
+                return FB_E_CUDA;
             }
             if (!sb.segs.empty()) {
                 memcpy(slot->hSegs, sb.segs.data(), sb.segs.size() * sizeof(fb::GroupSeg));
@@ -3071,6 +3081,77 @@ int Communicator::compareAndSwap(const void* compare,
     stats_.launches++;
     stats_.bytes += esize;
     return k_->rmaCompareSwap(a, dtype, s) == cudaSuccess ? FB_OK : FB_E_CUDA;
+}
+
+static_assert(sizeof(fb::RmaCopyDesc) == sizeof(fb::GroupSeg) && FB_RMA_COPY_MAX_ITEMS == FB_GROUP_MAX_SEGS,
+              "copy tables share the group tables' staging slots");
+
+int Communicator::putGetMany(const RmaCopy* items, size_t n, cudaStream_t s)
+{
+    if (parent_ != nullptr) {
+        return FB_E_UNSUPPORTED; // see subset()
+    }
+    if (n > 0 && items == nullptr) {
+        return FB_E_INVALID;
+    }
+    for (size_t i = 0; i < n; i++) {
+        const RmaCopy& it = items[i];
+        if (it.peer < 0 || it.peer >= dev_.nranks ||
+            (it.bytes > 0 && (it.local == nullptr || !rmaTargetOk(it.offset, it.bytes, 1, it.peer)))) {
+            return FB_E_INVALID;
+        }
+    }
+    bindDevice();
+    std::vector<fb::RmaCopyDesc> table;
+    table.reserve(std::min<size_t>(n, FB_RMA_COPY_MAX_ITEMS));
+    size_t i = 0;
+    while (i < n) {
+        table.clear();
+        uint64_t chunks = 0;
+        uint64_t bytes = 0;
+        for (; i < n && table.size() < FB_RMA_COPY_MAX_ITEMS; i++) {
+            const RmaCopy& it = items[i];
+            if (it.bytes == 0) {
+                continue;
+            }
+            uint8_t* remote = dev_.heap[it.peer] + it.offset;
+            uint8_t* local = (uint8_t*)it.local;
+            table.push_back(fb::RmaCopyDesc{ it.get ? remote : local, it.get ? local : remote, it.bytes, chunks });
+            chunks += fb::fbRmaCopyChunks(it.bytes);
+            bytes += it.bytes;
+        }
+        if (table.empty()) {
+            break;
+        }
+        fb::RmaCopyArgs a;
+        memset(&a, 0, sizeof(a));
+        a.items = table.data(); // the host twin reads the table in place
+        a.nItems = (uint32_t)table.size();
+        a.totalChunks = chunks;
+        ManySlot* slot = nullptr;
+        if (!loop_) {
+            slot = nextManySlot();
+            if (slot == nullptr) {
+                return FB_E_CUDA;
+            }
+            const size_t tableBytes = table.size() * sizeof(fb::RmaCopyDesc);
+            memcpy(slot->hSegs, table.data(), tableBytes);
+            if (cudaMemcpyAsync(slot->dSegs, slot->hSegs, tableBytes, cudaMemcpyHostToDevice, s) != cudaSuccess) {
+                return FB_E_CUDA;
+            }
+            a.items = reinterpret_cast<const fb::RmaCopyDesc*>(slot->dSegs);
+        }
+        stats_.launches++;
+        stats_.bytes += bytes;
+        if (k_->rmaCopyMany(a, s) != cudaSuccess) {
+            return FB_E_CUDA;
+        }
+        if (slot != nullptr) {
+            cudaEventRecord(slot->ev, s);
+            slot->used = true;
+        }
+    }
+    return FB_OK;
 }
 
 } // namespace faabric::device

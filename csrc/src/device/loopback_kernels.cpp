@@ -918,6 +918,14 @@ cudaError_t rmaCompareSwap(const RmaCasArgs& a, int dtype, cudaStream_t)
     return cudaSuccess;
 }
 
+cudaError_t rmaCopyMany(const RmaCopyArgs& a, cudaStream_t)
+{
+    for (uint32_t i = 0; i < a.nItems; i++) {
+        memmove(a.items[i].dst, a.items[i].src, a.items[i].bytes);
+    }
+    return cudaSuccess;
+}
+
 // ----------------------------------------------------------------- copy ----
 cudaError_t copy(void* dst, const void* src, size_t bytes, cudaStream_t)
 {

@@ -30,6 +30,7 @@ struct KernelTable
     cudaError_t (*signalPeers)(const FbCommDev& c, uint32_t wordOff, uint32_t value, cudaStream_t s);
     cudaError_t (*rmaAccumulate)(const RmaArgs& a, int dtype, int op, cudaStream_t s);
     cudaError_t (*rmaCompareSwap)(const RmaCasArgs& a, int dtype, cudaStream_t s);
+    cudaError_t (*rmaCopyMany)(const RmaCopyArgs& a, cudaStream_t s);
     // device-to-device copies: one range, and `height` rows of `width` bytes
     cudaError_t (*copy)(void* dst, const void* src, size_t bytes, cudaStream_t s);
     cudaError_t (*copy2D)(void* dst,
@@ -69,6 +70,8 @@ cudaError_t signalPeers(const FbCommDev& c, uint32_t wordOff, uint32_t value, cu
 // 64-bit word, a striped lock for 16-byte elements
 cudaError_t rmaAccumulate(const RmaArgs& a, int dtype, int op, cudaStream_t s);
 cudaError_t rmaCompareSwap(const RmaCasArgs& a, int dtype, cudaStream_t s);
+// a.items: HOST memory; one copy per item, in list order
+cudaError_t rmaCopyMany(const RmaCopyArgs& a, cudaStream_t s);
 cudaError_t copy(void* dst, const void* src, size_t bytes, cudaStream_t s);
 cudaError_t copy2D(void* dst, size_t dpitch, const void* src, size_t spitch, size_t width, size_t height, cudaStream_t s);
 

@@ -48,6 +48,13 @@ struct AsyncRequest
     uint64_t groupSeq = 0;
     void* stream = nullptr;
     std::shared_ptr<faabric::device::Communicator> comm;
+    // Request-based one-sided operation (MPI_Rput and friends): complete once
+    // rmaProgress->completed[rmaTarget] reaches rmaSeq
+    bool isRma = false;
+    int rmaWin = -1;
+    int rmaTarget = -1;
+    uint64_t rmaSeq = 0;
+    std::shared_ptr<MpiWorld::RmaProgress> rmaProgress;
 };
 
 struct RankState
@@ -951,11 +958,48 @@ static void flushPendingGroup()
     }
 }
 
+int MpiWorld::addRmaRequest(int rank, int winId, int targetRank, std::shared_ptr<RmaProgress> progress)
+{
+    int requestId = tls.nextRequestId++;
+    AsyncRequest r;
+    r.sendRank = rank;
+    r.isRma = true;
+    r.rmaWin = winId;
+    r.rmaTarget = targetRank;
+    // (no progress: the operation completed at issue)
+    if (progress != nullptr) {
+        r.rmaSeq = ++progress->issued[targetRank];
+        r.rmaProgress = std::move(progress);
+    }
+    tls.requests[requestId] = r;
+    return requestId;
+}
+
+void MpiWorld::freeAsyncRequest(int requestId)
+{
+    // A request-based one-sided operation completes at the next flush or
+    // unlock of its window anyway; the other kinds stay until they are waited
+    auto it = tls.requests.find(requestId);
+    if (it != tls.requests.end() && it->second.isRma) {
+        tls.requests.erase(it);
+    }
+}
+
 void MpiWorld::awaitAsyncRequest(int requestId)
 {
     auto it = tls.requests.find(requestId);
     if (it == tls.requests.end()) {
         // Already satisfied while draining for an earlier wait
+        return;
+    }
+    if (it->second.isRma) {
+        AsyncRequest req = it->second;
+        tls.requests.erase(it);
+        // (completed by an earlier wait, flush or unlock: the window may be
+        // gone, so nothing else is touched)
+        if (req.rmaProgress != nullptr && req.rmaSeq > req.rmaProgress->completed[req.rmaTarget]) {
+            rmaAwait(req.sendRank, req.rmaWin, req.rmaTarget);
+        }
         return;
     }
     if (it->second.isDeviceCollective) {

@@ -187,6 +187,20 @@ bool cudaCopy(const void* dst, const void* src)
     return (MpiWorld::isDevicePointer(dst) || MpiWorld::isDevicePointer(src)) && faabric::device::cudaAvailable();
 }
 
+// Every request of `p` to a target that `covered` names is complete
+template<class F>
+void markComplete(const std::shared_ptr<MpiWorld::RmaProgress>& p, F covered)
+{
+    if (p == nullptr) {
+        return;
+    }
+    for (size_t t = 0; t < p->issued.size(); t++) {
+        if (covered((int)t)) {
+            p->completed[t] = p->issued[t];
+        }
+    }
+}
+
 void rmaCopy(void* dst, const void* src, size_t bytes)
 {
     if (bytes == 0) {
@@ -245,6 +259,8 @@ int MpiWorld::winCreate(int rank, void* base, int64_t sizeBytes, int dispUnit)
             slot->streams.resize(size);
             slot->epochs.resize(size);
             slot->locks.resize(size);
+            slot->batches.resize(size);
+            slot->progress.resize(size);
         }
         w = slot;
     }
@@ -940,11 +956,13 @@ int MpiWorld::rmaComplete(RmaWindow& w, int winId, int rank, int targetRank, boo
     if (isLocalRank(targetRank)) {
         // Everything of this origin in this process completes: its device
         // streams, and copies from pageable memory still in flight
+        rmaIssueBatch(w, rank);
         rmaWaitStreams(w, rank);
         if (e.deviceCopies) {
             cudaCheck(cudaStreamSynchronize(cudaStreamLegacy), "One-sided copy");
             e.deviceCopies = false;
         }
+        markComplete(w.progress[rank], [&](int t) { return isLocalRank(t); });
         if (unlock) {
             std::vector<std::function<void()>> sends;
             {
@@ -980,6 +998,7 @@ int MpiWorld::rmaComplete(RmaWindow& w, int winId, int rank, int targetRank, boo
         nOps++;
     }
     if (nOps == 0 && !unlock) {
+        markComplete(w.progress[rank], [&](int t) { return t == targetRank; });
         return MPI_SUCCESS;
     }
     reinterpret_cast<RmaPassiveHeader*>(req.data())->nOps = nOps;
@@ -1009,6 +1028,9 @@ int MpiWorld::rmaComplete(RmaWindow& w, int winId, int rank, int targetRank, boo
     auto& pending = w.pending[rank];
     pending.erase(std::remove_if(pending.begin(), pending.end(), [&](const RmaOp& op) { return op.target == targetRank; }),
                   pending.end());
+    // The requests to the target are over: done, or failed with this call's
+    // error (a later wait on one of them must not ship anything again)
+    markComplete(w.progress[rank], [&](int t) { return t == targetRank; });
     return mpiErrorOf(status);
 }
 
@@ -1135,6 +1157,154 @@ bool MpiWorld::winInPassiveEpoch(int rank, int winId)
 {
     auto w = findWindow(winId);
     return w != nullptr && rank >= 0 && rank < size && !w->epochs[rank].locked.empty();
+}
+
+// ---------------------------------------------------------------------------
+// Request-based operations (MPI_Rput, MPI_Rget, MPI_Raccumulate,
+// MPI_Rget_accumulate)
+// ---------------------------------------------------------------------------
+void MpiWorld::rmaIssueBatch(RmaWindow& w, int rank)
+{
+    auto& batch = w.batches[rank];
+    if (batch.empty()) {
+        return;
+    }
+    auto comm = wiredDeviceComm(rank);
+    const int device = comm->isLoopback() ? HOST_MEMORY : comm->device();
+    cudaStream_t s = (cudaStream_t)streamForRank(rank);
+    DeviceGuard on(device);
+    const int rc = comm->putGetMany(batch.data(), batch.size(), s);
+    batch.clear();
+    if (rc != FB_OK) {
+        throw std::runtime_error(std::string("Batched one-sided copy failed: ") +
+                                 faabric::device::Communicator::errorString(rc));
+    }
+    auto& used = w.streams[rank];
+    if (device != HOST_MEMORY && std::find(used.begin(), used.end(), std::make_pair(device, (void*)s)) == used.end()) {
+        used.emplace_back(device, (void*)s);
+    }
+}
+
+int MpiWorld::rmaRequestTarget(RmaWindow& w, int rank, int targetRank, int64_t targetDisp, size_t bytes, uint8_t** target)
+{
+    if (targetRank < 0 || targetRank >= size) {
+        return MPI_ERR_RANK;
+    }
+    const int64_t off = targetDisp * (int64_t)w.dispUnits[targetRank];
+    if (targetDisp < 0 || bytes > (uint64_t)w.sizes[targetRank] || off > w.sizes[targetRank] - (int64_t)bytes) {
+        SPDLOG_ERROR("Request-based one-sided access [{}, {}) outside the {}-byte window of rank {}", off, off + (int64_t)bytes, w.sizes[targetRank], targetRank);
+        return MPI_ERR_ARG;
+    }
+    // MPI-3.1 11.3.5: only inside a passive epoch that covers the target
+    if (w.epochs[rank].locked.count(targetRank) == 0) {
+        return MPI_ERR_RMA_SYNC;
+    }
+    *target = (uint8_t*)(uintptr_t)w.bases[targetRank] + off;
+    if (w.progress[rank] == nullptr) {
+        w.progress[rank] = std::make_shared<RmaProgress>();
+        w.progress[rank]->issued.resize(size, 0);
+        w.progress[rank]->completed.resize(size, 0);
+    }
+    return MPI_SUCCESS;
+}
+
+int MpiWorld::winRputGet(int rank, int winId, uint8_t* origin, size_t bytes, int targetRank, int64_t targetDisp, bool get, int* requestId)
+{
+    auto w = findWindow(winId);
+    if (w == nullptr) {
+        return MPI_ERR_WIN;
+    }
+    if (requestId == nullptr || (origin == nullptr && bytes > 0)) {
+        return MPI_ERR_ARG;
+    }
+    uint8_t* target = nullptr;
+    int rc = rmaRequestTarget(*w, rank, targetRank, targetDisp, bytes, &target);
+    if (rc != MPI_SUCCESS) {
+        return rc;
+    }
+    if (isLocalRank(targetRank) && bytes > 0) {
+        // Heap to heap, origin on the origin's GPU: one launch for the batch
+        auto comm = wiredDeviceComm(rank);
+        auto targetComm = wiredDeviceComm(targetRank);
+        const bool originOk =
+          comm != nullptr && (comm->isLoopback() ? faabric::device::Communicator::isLoopbackHeapPointer(origin)
+                                                 : comm->inHeap(origin, bytes) || bufferDevice(origin) == comm->device());
+        if (originOk && targetComm != nullptr && targetComm->inHeap(target, bytes)) {
+            auto& batch = w->batches[rank];
+            batch.push_back(faabric::device::Communicator::RmaCopy{
+              origin, targetComm->offsetOf(target), bytes, targetRank, get ? 1 : 0 });
+            if (batch.size() >= FB_RMA_COPY_MAX_ITEMS) {
+                rmaIssueBatch(*w, rank);
+            }
+            *requestId = addRmaRequest(rank, winId, targetRank, w->progress[rank]);
+            return MPI_SUCCESS;
+        }
+    }
+    // Today's MPI_Put / MPI_Get: a copy now (this process), or queued for
+    // the flush of a target in another process
+    if (get) {
+        winGet(rank, winId, origin, bytes, targetRank, targetDisp);
+    } else {
+        winPut(rank, winId, origin, bytes, targetRank, targetDisp);
+    }
+    if (isLocalRank(targetRank) && cudaCopy(origin, target)) {
+        // complete at issue: a cudaMemcpy that involves pageable memory may
+        // return before its DMA lands, and the request's wait does nothing
+        cudaCheck(cudaStreamSynchronize(cudaStreamLegacy), "Request-based one-sided copy");
+    }
+    *requestId = addRmaRequest(rank, winId, targetRank, isLocalRank(targetRank) ? nullptr : w->progress[rank]);
+    return MPI_SUCCESS;
+}
+
+int MpiWorld::winRaccumulate(int rank,
+                             int winId,
+                             const uint8_t* origin,
+                             size_t count,
+                             faabric_datatype_t* datatype,
+                             faabric_op_t* op,
+                             uint8_t* result,
+                             int targetRank,
+                             int64_t targetDisp,
+                             int* requestId)
+{
+    auto w = findWindow(winId);
+    if (w == nullptr) {
+        return MPI_ERR_WIN;
+    }
+    const int dtype = datatype != nullptr ? fbDtypeFor(datatype) : -1;
+    if (requestId == nullptr || dtype < 0 || count > (size_t)INT64_MAX / fbDtypeSize(dtype)) {
+        return MPI_ERR_ARG;
+    }
+    uint8_t* target = nullptr;
+    int rc = rmaRequestTarget(*w, rank, targetRank, targetDisp, count * fbDtypeSize(dtype), &target);
+    if (rc != MPI_SUCCESS) {
+        return rc;
+    }
+    // (every other check of MPI_Accumulate runs before it applies anything)
+    rc = winAccumulate(rank, winId, origin, count, datatype, op, result, targetRank, targetDisp);
+    if (rc != MPI_SUCCESS) {
+        return rc;
+    }
+    *requestId = addRmaRequest(rank, winId, targetRank, w->progress[rank]);
+    return MPI_SUCCESS;
+}
+
+void MpiWorld::rmaAwait(int rank, int winId, int targetRank)
+{
+    auto w = findWindow(winId);
+    if (w == nullptr) {
+        throw std::runtime_error("Waiting for a one-sided request on a freed window");
+    }
+    if (isLocalRank(targetRank)) {
+        rmaIssueBatch(*w, rank);
+        rmaWaitStreams(*w, rank);
+        markComplete(w->progress[rank], [&](int t) { return isLocalRank(t); });
+        return;
+    }
+    const int rc = rmaComplete(*w, winId, rank, targetRank, false);
+    if (rc != MPI_SUCCESS) {
+        throw std::runtime_error("One-sided request to rank " + std::to_string(targetRank) + " failed");
+    }
 }
 
 std::string MpiWorld::serveRmaRequest(int call, const uint8_t* buffer, size_t bytes)

@@ -206,9 +206,11 @@ int accumulateShape(const std::vector<std::pair<int, MPI_Datatype>>& sides, MPI_
     return MPI_SUCCESS;
 }
 
+// `request` non-null: the request-based form (MPI_Raccumulate,
+// MPI_Rget_accumulate)
 int getAccumulate(const void* origin, int originCount, MPI_Datatype originType, void* result, int resultCount,
                   MPI_Datatype resultType, int targetRank, MPI_Aint targetDisp, int targetCount, MPI_Datatype targetType,
-                  MPI_Op op, MPI_Win win)
+                  MPI_Op op, MPI_Win win, MPI_Request* request = nullptr)
 {
     if (win == nullptr) {
         return MPI_ERR_WIN;
@@ -232,8 +234,42 @@ int getAccumulate(const void* origin, int originCount, MPI_Datatype originType, 
     if (rc != MPI_SUCCESS) {
         return rc;
     }
+    if (request != nullptr) {
+        int id = 0;
+        rc = getExecutingWorld().winRaccumulate(executingContext.getRank(), win->id, (const uint8_t*)origin, count, base,
+                                                op, (uint8_t*)result, targetRank, (int64_t)targetDisp, &id);
+        if (rc == MPI_SUCCESS) {
+            *request = new faabric_request_t{ id };
+            requestTable()[id] = *request;
+        }
+        return rc;
+    }
     return getExecutingWorld().winAccumulate(executingContext.getRank(), win->id, (const uint8_t*)origin, count, base, op,
                                              (uint8_t*)result, targetRank, (int64_t)targetDisp);
+}
+
+// MPI_Rput / MPI_Rget
+int requestPutGet(void* origin, int originCount, MPI_Datatype originType, int targetRank, MPI_Aint targetDisp,
+                  int targetCount, MPI_Datatype targetType, MPI_Win win, MPI_Request* request, bool get)
+{
+    if (win == nullptr) {
+        return MPI_ERR_WIN;
+    }
+    if (request == nullptr || originType == nullptr || targetType == nullptr || originCount < 0 || targetCount < 0) {
+        return MPI_ERR_ARG;
+    }
+    const size_t bytes = (size_t)originCount * originType->size;
+    if (bytes != (size_t)targetCount * targetType->size) {
+        return MPI_ERR_ARG;
+    }
+    int id = 0;
+    int rc = getExecutingWorld().winRputGet(executingContext.getRank(), win->id, (uint8_t*)origin, bytes, targetRank,
+                                            (int64_t)targetDisp, get, &id);
+    if (rc == MPI_SUCCESS) {
+        *request = new faabric_request_t{ id };
+        requestTable()[id] = *request;
+    }
+    return rc;
 }
 }
 
@@ -437,6 +473,7 @@ int MPI_Waitany(int count, MPI_Request array_of_requests[], int* index, MPI_Stat
 int MPI_Request_free(MPI_Request* request)
 {
     if (request != nullptr && *request != nullptr) {
+        getExecutingWorld().freeAsyncRequest((*request)->id);
         requestTable().erase((*request)->id);
         delete *request;
         *request = nullptr;
@@ -1182,6 +1219,57 @@ int MPI_Compare_and_swap(const void* origin_addr, const void* compare_addr, void
     return getExecutingWorld().winCompareSwap(executingContext.getRank(), win->id, (const uint8_t*)origin_addr,
                                               (const uint8_t*)compare_addr, (uint8_t*)result_addr, base, target_rank,
                                               (int64_t)target_disp);
+}
+
+// ---- request-based one-sided operations; see MpiWorld::winRputGet.  They
+// need a passive epoch that covers the target (MPI_ERR_RMA_SYNC otherwise) ----
+int MPI_Rput(const void* origin_addr, int origin_count, MPI_Datatype origin_datatype, int target_rank,
+             MPI_Aint target_disp, int target_count, MPI_Datatype target_datatype, MPI_Win win, MPI_Request* request)
+{
+    SPDLOG_TRACE("MPI - MPI_Rput");
+    return requestPutGet(const_cast<void*>(origin_addr), origin_count, origin_datatype, target_rank, target_disp,
+                         target_count, target_datatype, win, request, false);
+}
+
+int MPI_Rget(void* origin_addr, int origin_count, MPI_Datatype origin_datatype, int target_rank,
+             MPI_Aint target_disp, int target_count, MPI_Datatype target_datatype, MPI_Win win, MPI_Request* request)
+{
+    SPDLOG_TRACE("MPI - MPI_Rget");
+    return requestPutGet(origin_addr, origin_count, origin_datatype, target_rank, target_disp, target_count,
+                         target_datatype, win, request, true);
+}
+
+int MPI_Raccumulate(const void* origin_addr, int origin_count, MPI_Datatype origin_datatype, int target_rank,
+                    MPI_Aint target_disp, int target_count, MPI_Datatype target_datatype, MPI_Op op, MPI_Win win,
+                    MPI_Request* request)
+{
+    SPDLOG_TRACE("MPI - MPI_Raccumulate");
+    if (win == nullptr) {
+        return MPI_ERR_WIN;
+    }
+    if (request == nullptr) {
+        return MPI_ERR_ARG;
+    }
+    if (op == MPI_NO_OP) {
+        return MPI_ERR_OP; // as MPI_Accumulate
+    }
+    return getAccumulate(origin_addr, origin_count, origin_datatype, nullptr, 0, nullptr, target_rank, target_disp,
+                         target_count, target_datatype, op, win, request);
+}
+
+int MPI_Rget_accumulate(const void* origin_addr, int origin_count, MPI_Datatype origin_datatype, void* result_addr,
+                        int result_count, MPI_Datatype result_datatype, int target_rank, MPI_Aint target_disp,
+                        int target_count, MPI_Datatype target_datatype, MPI_Op op, MPI_Win win, MPI_Request* request)
+{
+    SPDLOG_TRACE("MPI - MPI_Rget_accumulate");
+    if (win == nullptr) {
+        return MPI_ERR_WIN;
+    }
+    if (request == nullptr || (result_addr == nullptr && result_count > 0)) {
+        return MPI_ERR_ARG;
+    }
+    return getAccumulate(origin_addr, origin_count, origin_datatype, result_addr, result_count, result_datatype,
+                         target_rank, target_disp, target_count, target_datatype, op, win, request);
 }
 
 int MPI_Win_free(MPI_Win* win)

@@ -640,6 +640,62 @@ class Communicator:
             raise CommError("dst_sym is not in the symmetric heap")
         return self.heap_offset(dst_sym)
 
+    def _put_get_many(self, what, locals_, syms, peers, get, stream):
+        """One batched copy between ``locals_[i]`` and ``peers[i]``'s copy of the
+        symmetric tensor ``syms[i]``; every item is checked before the native
+        call."""
+        self._parent_only(what)
+        n = len(locals_)
+        if len(syms) != n or len(peers) != n:
+            raise CommError(f"{what}: {n} local tensors, {len(syms)} symmetric tensors and {len(peers)} peers")
+        ptrs, offs, nbytes, prs = [], [], [], []
+        for i, (loc, sym, peer) in enumerate(zip(locals_, syms, peers)):
+            if not loc.is_cuda or not loc.is_contiguous() or not sym.is_contiguous():
+                raise CommError(f"{what}: item {i} must be contiguous CUDA tensors")
+            if loc.device.index != self.device:
+                raise CommError(f"{what}: item {i} local tensor is on {loc.device}, not on cuda:{self.device}")
+            nb = loc.numel() * loc.element_size()
+            if sym.numel() * sym.element_size() != nb:
+                raise CommError(
+                    f"{what}: item {i} has {nb} local bytes and {sym.numel() * sym.element_size()} symmetric bytes"
+                )
+            # (an empty item is skipped: only its peer is checked)
+            if nb > 0 and not self._lib.fb_comm_in_heap(self._h, C.c_void_p(sym.data_ptr()), nb):
+                raise CommError(f"{what}: item {i} symmetric tensor is not in the symmetric heap")
+            peer = int(peer)
+            if peer < 0 or peer >= self.size:
+                raise CommError(f"{what}: item {i} peer {peer} outside a communicator of {self.size}")
+            ptrs.append(loc.data_ptr())
+            offs.append(self.heap_offset(sym) if nb > 0 else 0)
+            nbytes.append(nb)
+            prs.append(peer)
+        if n == 0:
+            return
+        rc = self._lib.fb_put_get_many(
+            self._h,
+            n,
+            (C.c_void_p * n)(*ptrs),
+            (C.c_uint64 * n)(*offs),
+            (C.c_uint64 * n)(*nbytes),
+            (C.c_int32 * n)(*prs),
+            (C.c_int32 * n)(*([1 if get else 0] * n)),
+            self._stream(stream),
+        )
+        self._check(rc, what)
+
+    def put_many(self, srcs, dsts_sym, peers, stream=None):
+        """Copy every ``srcs[i]`` into ``peers[i]``'s copy of the symmetric
+        tensor ``dsts_sym[i]`` (byte sizes must match), as one batched launch
+        per 1024 items (MPI_Rput).  Any alignment and length; ``peers[i]`` may
+        be this rank.  Stream-ordered: complete when ``stream`` passes it.
+        Destinations that overlap within one list get unspecified bytes."""
+        self._put_get_many("put_many", srcs, dsts_sym, peers, False, stream)
+
+    def get_many(self, dsts, srcs_sym, peers, stream=None):
+        """Copy ``peers[i]``'s copy of the symmetric tensor ``srcs_sym[i]`` into
+        every ``dsts[i]`` (MPI_Rget); the same rules as :meth:`put_many`."""
+        self._put_get_many("get_many", dsts, srcs_sym, peers, True, stream)
+
     def accumulate(self, src, dst_sym, peer, op="sum", dtype=None, fetch=None, stream=None):
         """Atomically combine ``src`` into ``peer``'s copy of the symmetric tensor
         ``dst_sym``, element by element: ``dst[i] = op(dst[i], src[i])``
