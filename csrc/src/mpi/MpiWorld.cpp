@@ -17,6 +17,8 @@
 #include <faabric/util/testing.h>
 #include <faabric/util/timing.h>
 
+#include "buffers.h"
+
 #include <cuda_runtime.h>
 
 #include <cstring>
@@ -694,8 +696,7 @@ void MpiWorld::send(int sendRank,
     msg.messageType = messageType;
     msg.buffer = nullptr;
 
-    // (the loopback backend's heap is host memory: copied as such)
-    const bool onDevice = bytes > 0 && isDevicePointer(buffer) && !faabric::device::Communicator::isLoopbackHeapPointer(buffer);
+    const bool onDevice = bytes > 0 && !hostAddressable(buffer);
     if (isLocal && !faabric::util::isMockMode()) {
         // Eager copy so the caller may reuse its buffer as soon as we return
         if (bytes > 0 && onDevice) {
@@ -731,7 +732,7 @@ void MpiWorld::send(int sendRank,
         std::vector<uint8_t> hostCopy;
         if (onDevice) {
             hostCopy.resize(bytes);
-            cudaMemcpy(hostCopy.data(), buffer, bytes, cudaMemcpyDeviceToHost);
+            copyBytes(hostCopy.data(), buffer, bytes);
             msg.buffer = hostCopy.data();
         } else {
             msg.buffer = (void*)buffer;
@@ -811,7 +812,7 @@ void MpiWorld::doRecv(MpiMessage& msg,
     const size_t bytes = payloadSize(msg);
     if (bytes > 0 && msg.buffer != nullptr) {
         const bool srcDev = isDevicePointer(msg.buffer);
-        const bool dstDev = isDevicePointer(buffer) && !faabric::device::Communicator::isLoopbackHeapPointer(buffer);
+        const bool dstDev = !hostAddressable(buffer);
         if (srcDev) {
             // Parked in the sender's heap: read it through OUR mapping
             const uint8_t* src = peerViewOfStaged(msg.sendRank, msg.recvRank, msg.buffer);
@@ -912,6 +913,31 @@ int MpiWorld::irecv(int sendRank,
     return requestId;
 }
 
+// Sorts the return code of a device collective: true if it was issued, false
+// if the communicator declines it (FB_E_UNSUPPORTED, FB_E_TOO_LARGE: the host
+// path takes the call); throws on any other error
+static bool deviceIssued(int rc, const char* what = "Device collective")
+{
+    if (rc == FB_OK) {
+        return true;
+    }
+    if (rc == FB_E_UNSUPPORTED || rc == FB_E_TOO_LARGE) {
+        return false;
+    }
+    throw std::runtime_error(std::string(what) + " failed: " + faabric::device::Communicator::errorString(rc));
+}
+
+// Waits for the device collectives issued on `stream`; throws if one failed
+static void awaitDevice(faabric::device::Communicator& comm, void* stream)
+{
+    if (!comm.waitStreamFast((cudaStream_t)stream)) {
+        throw std::runtime_error("Device collective failed at synchronisation");
+    }
+    if (comm.peekError() != 0) {
+        throw std::runtime_error("Device collective watchdog fired (peer missing?)");
+    }
+}
+
 // Issues the deferred burst of this rank thread as one grouped launch (every
 // rank defers and flushes at the same program points)
 static void flushPendingGroup()
@@ -936,16 +962,17 @@ static void flushPendingGroup()
     const char* what;
     if (tls.groupKind == Communicator::GROUP_REDUCE_SCATTER) {
         rc = comm->reduceScatterMany(items.data(), items.size(), tls.groupDtype, tls.groupOp, FB_FLAG_SYMMETRIC, s);
-        what = "reduce-scatter";
+        what = "Grouped device reduce-scatter";
     } else if (tls.groupKind == Communicator::GROUP_ALLGATHER) {
         rc = comm->allGatherMany(items.data(), items.size(), tls.groupDtype, FB_FLAG_SYMMETRIC, s);
-        what = "all-gather";
+        what = "Grouped device all-gather";
     } else {
         rc = comm->allReduceMany(items.data(), items.size(), tls.groupDtype, tls.groupOp, FB_FLAG_SYMMETRIC, s);
-        what = "all-reduce";
+        what = "Grouped device all-reduce";
     }
-    if (rc != FB_OK) {
-        throw std::runtime_error(std::string("Grouped device ") + what + " failed: " + Communicator::errorString(rc));
+    // (the burst's requests have no host path left: declining is an error too)
+    if (!deviceIssued(rc, what)) {
+        throw std::runtime_error(std::string(what) + " declined: " + Communicator::errorString(rc));
     }
     const uint64_t seq = ++tls.groupLaunchSeq;
     for (int id : reqs) {
@@ -1014,15 +1041,10 @@ void MpiWorld::awaitAsyncRequest(int requestId)
             return;
         }
         cudaSetDevice(req.comm->device());
-        if (!req.comm->waitStreamFast((cudaStream_t)req.stream)) {
-            throw std::runtime_error("Device collective failed at synchronisation");
-        }
+        awaitDevice(*req.comm, req.stream);
         if (req.groupSeq != 0) {
             tls.groupCompletedSeq = req.groupSeq;
             tls.groupCompletedStream = req.stream;
-        }
-        if (req.comm->peekError() != 0) {
-            throw std::runtime_error("Device collective watchdog fired (peer missing?)");
         }
         return;
     }
@@ -1267,31 +1289,33 @@ std::shared_ptr<faabric::device::Communicator> MpiWorld::getDeviceComm(int rank)
     return deviceComms[rank];
 }
 
-// Runs `fn(comm, stream)` for a device collective and waits for it
-static bool runDevice(std::shared_ptr<faabric::device::Communicator> comm,
-                      void* stream,
-                      const std::function<int(faabric::device::Communicator&, cudaStream_t)>& fn)
+// Issues `call(comm, stream)`, a device collective, and counts it in
+// `counter`: false if the communicator declines it (the host path takes it)
+template<class Call>
+static bool issueDevice(faabric::device::Communicator& comm, void* stream, std::atomic<uint64_t>& counter, Call&& call)
 {
-    if (comm == nullptr) {
-        return false;
-    }
     // keep the issue order identical on every rank
     flushPendingGroup();
-    cudaSetDevice(comm->device());
-    int rc = fn(*comm, (cudaStream_t)stream);
-    if (rc == FB_E_UNSUPPORTED || rc == FB_E_TOO_LARGE) {
+    cudaSetDevice(comm.device());
+    if (!deviceIssued(call(comm, (cudaStream_t)stream))) {
         return false;
     }
-    if (rc != FB_OK) {
-        throw std::runtime_error(std::string("Device collective failed: ") + faabric::device::Communicator::errorString(rc));
+    counter.fetch_add(1);
+    return true;
+}
+
+// A blocking device collective: issued, then waited for.  False if there is
+// no communicator or it declines the call.
+template<class Call>
+static bool issueAndWait(const std::shared_ptr<faabric::device::Communicator>& comm,
+                         void* stream,
+                         std::atomic<uint64_t>& counter,
+                         Call&& call)
+{
+    if (comm == nullptr || !issueDevice(*comm, stream, counter, call)) {
+        return false;
     }
-    if (!comm->waitStreamFast((cudaStream_t)stream)) {
-        throw std::runtime_error("Device collective failed at synchronisation");
-    }
-    uint32_t err = comm->peekError();
-    if (err != 0) {
-        throw std::runtime_error("Device collective watchdog fired (peer missing?)");
-    }
+    awaitDevice(*comm, stream);
     return true;
 }
 
@@ -1305,21 +1329,11 @@ bool MpiWorld::deviceReducible(faabric_datatype_t* dt, faabric_op_t* op)
     return fbDtypeFor(dt) >= 0 && fbOpFor(op) >= 0;
 }
 
-// Runs the device branch of a collective and counts it
-#define FB_DEVICE_BRANCH(call)                                                                                   \
-    do {                                                                                                         \
-        if (!runDevice(comm, streamForRank(rank), [&](faabric::device::Communicator& c, cudaStream_t s) {       \
-                return (call);                                                                                   \
-            })) {                                                                                                \
-            return false;                                                                                        \
-        }                                                                                                        \
-        deviceCollectives.fetch_add(1);                                                                          \
-        return true;                                                                                             \
-    } while (0)
-
 bool MpiWorld::deviceBroadcast(const DeviceComm& comm, int rank, int root, uint8_t* buffer, size_t bytes)
 {
-    FB_DEVICE_BRANCH(c.broadcast(buffer, bytes, root, symFlag(c, buffer, bytes), s));
+    return issueAndWait(comm, streamForRank(rank), deviceCollectives, [&](auto& c, cudaStream_t s) {
+        return c.broadcast(buffer, bytes, root, symFlag(c, buffer, bytes), s);
+    });
 }
 
 bool MpiWorld::deviceReduce(const DeviceComm& comm,
@@ -1338,7 +1352,9 @@ bool MpiWorld::deviceReduce(const DeviceComm& comm,
     if (fdt < 0 || fop < 0) {
         return false;
     }
-    FB_DEVICE_BRANCH(c.reduce(send, recv, (size_t)count, fdt, fop, root, 0, s));
+    return issueAndWait(comm, streamForRank(rank), deviceCollectives, [&](auto& c, cudaStream_t s) {
+        return c.reduce(send, recv, (size_t)count, fdt, fop, root, 0, s);
+    });
 }
 
 bool MpiWorld::deviceAllReduce(const DeviceComm& comm,
@@ -1360,7 +1376,9 @@ bool MpiWorld::deviceAllReduce(const DeviceComm& comm,
     if (comm != nullptr && comm->isSubset() && (algo == FB_ALGO_LL || algo == FB_ALGO_NVLS)) {
         algo = FB_ALGO_AUTO;
     }
-    FB_DEVICE_BRANCH(c.allReduce(send, recv, (size_t)count, fdt, fop, algo, symFlag(c, send, (size_t)count * dt->size), s));
+    return issueAndWait(comm, streamForRank(rank), deviceCollectives, [&](auto& c, cudaStream_t s) {
+        return c.allReduce(send, recv, (size_t)count, fdt, fop, algo, symFlag(c, send, (size_t)count * dt->size), s);
+    });
 }
 
 bool MpiWorld::deviceScan(const DeviceComm& comm,
@@ -1376,7 +1394,9 @@ bool MpiWorld::deviceScan(const DeviceComm& comm,
     if (send == recv || fdt < 0 || fop < 0) {
         return false;
     }
-    FB_DEVICE_BRANCH(c.scan(send, recv, (size_t)count, fdt, fop, symFlag(c, send, (size_t)count * dt->size), s));
+    return issueAndWait(comm, streamForRank(rank), deviceCollectives, [&](auto& c, cudaStream_t s) {
+        return c.scan(send, recv, (size_t)count, fdt, fop, symFlag(c, send, (size_t)count * dt->size), s);
+    });
 }
 
 bool MpiWorld::deviceGather(const DeviceComm& comm, int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes)
@@ -1389,7 +1409,9 @@ bool MpiWorld::deviceGather(const DeviceComm& comm, int rank, int root, const ui
     if (comm != nullptr && send == nullptr) {
         send = recv + (size_t)comm->rank() * bytes;
     }
-    FB_DEVICE_BRANCH(c.gather(send, recv, bytes, root, 0, s));
+    return issueAndWait(comm, streamForRank(rank), deviceCollectives, [&](auto& c, cudaStream_t s) {
+        return c.gather(send, recv, bytes, root, 0, s);
+    });
 }
 
 bool MpiWorld::deviceScatter(const DeviceComm& comm, int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes)
@@ -1399,7 +1421,9 @@ bool MpiWorld::deviceScatter(const DeviceComm& comm, int rank, int root, const u
     if (comm != nullptr && recv == nullptr) {
         recv = const_cast<uint8_t*>(send) + (size_t)comm->rank() * bytes;
     }
-    FB_DEVICE_BRANCH(c.scatter(send, recv, bytes, root, 0, s));
+    return issueAndWait(comm, streamForRank(rank), deviceCollectives, [&](auto& c, cudaStream_t s) {
+        return c.scatter(send, recv, bytes, root, 0, s);
+    });
 }
 
 bool MpiWorld::deviceAllGather(const DeviceComm& comm, int rank, const uint8_t* send, uint8_t* recv, size_t bytes)
@@ -1407,15 +1431,17 @@ bool MpiWorld::deviceAllGather(const DeviceComm& comm, int rank, const uint8_t* 
     if (comm == nullptr || send == recv + (size_t)comm->rank() * bytes) {
         return false;
     }
-    FB_DEVICE_BRANCH(c.allGather(send, recv, bytes, symFlag(c, send, bytes), s));
+    return issueAndWait(comm, streamForRank(rank), deviceCollectives, [&](auto& c, cudaStream_t s) {
+        return c.allGather(send, recv, bytes, symFlag(c, send, bytes), s);
+    });
 }
 
 bool MpiWorld::deviceAllToAll(const DeviceComm& comm, int rank, const uint8_t* send, uint8_t* recv, size_t chunk)
 {
-    FB_DEVICE_BRANCH(c.allToAll(send, recv, chunk, symFlag(c, send, chunk * (size_t)(comm ? comm->size() : 0)), s));
+    return issueAndWait(comm, streamForRank(rank), deviceCollectives, [&](auto& c, cudaStream_t s) {
+        return c.allToAll(send, recv, chunk, symFlag(c, send, chunk * (size_t)c.size()), s);
+    });
 }
-
-#undef FB_DEVICE_BRANCH
 
 void MpiWorld::cacheDeviceComm(int rank)
 {
@@ -1425,6 +1451,17 @@ void MpiWorld::cacheDeviceComm(int rank)
         tls.cachedCommRank = rank;
         tls.cachedCommValid = true;
     }
+}
+
+// Records the request of a non-blocking collective issued (or, deferred, to be
+// issued) on `stream` of `comm`: waiting for it drains that stream
+static int recordDevice(int requestId, AsyncRequest r, const std::shared_ptr<faabric::device::Communicator>& comm, void* stream)
+{
+    r.isDeviceCollective = true;
+    r.stream = stream;
+    r.comm = comm;
+    tls.requests[requestId] = std::move(r);
+    return requestId;
 }
 
 // Adds one call to this rank thread's deferred burst, flushing first a burst
@@ -1451,38 +1488,56 @@ static void deferToGroup(faabric::device::Communicator::GroupKind kind,
     tls.groupRequests.push_back(requestId);
     tls.deferredCount++; // added to the world's counter at the flush
     tls.deferredCounter = &counter;
-    r.isDeviceCollective = true;
     r.deferred = true;
-    r.stream = tls.groupStream;
-    r.comm = comm;
-    tls.requests[requestId] = r;
+    recordDevice(requestId, std::move(r), comm, tls.groupStream);
+}
+
+// The request of a non-blocking collective, complete as it stands (the call
+// ran on the host) until recordDevice() makes it a device collective
+static AsyncRequest collectiveRequest(int rank)
+{
+    AsyncRequest r;
+    r.isSend = true; // nothing to drain on wait
+    r.sendRank = rank;
+    r.recvRank = rank;
+    return r;
+}
+
+// The buffers of a non-blocking collective on `c`: `symmetric` when both
+// extents lie in its heap (no driver query), `grouped` when the call may also
+// join the deferred burst: grouping on, addresses and shard 16-byte aligned (a
+// shard of 0 puts no condition on the length)
+struct Placement
+{
+    bool symmetric;
+    bool grouped;
+};
+
+static Placement placeCollective(const faabric::device::Communicator& c,
+                                 bool grouping,
+                                 const void* send,
+                                 size_t sendBytes,
+                                 const void* recv,
+                                 size_t recvBytes,
+                                 size_t shardBytes)
+{
+    const bool symmetric = c.inHeap(send, sendBytes) && c.inHeap(recv, recvBytes);
+    return { symmetric, symmetric && grouping && (((uintptr_t)send | (uintptr_t)recv | shardBytes) & 15) == 0 };
 }
 
 int MpiWorld::iAllReduce(int rank, uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count, faabric_op_t* op)
 {
     checkRanksRange(0, rank);
     const size_t bytes = (size_t)count * dt->size;
-    int requestId = tls.nextRequestId++;
-    AsyncRequest r;
-    r.isSend = true; // nothing to drain on wait unless it becomes a device op
-    r.sendRank = rank;
-    r.recvRank = rank;
-    int fdt = fbDtypeFor(dt);
-    int fop = fbOpFor(op);
+    const int requestId = tls.nextRequestId++;
+    AsyncRequest r = collectiveRequest(rank);
+    const int fdt = fbDtypeFor(dt);
+    const int fop = fbOpFor(op);
     cacheDeviceComm(rank);
-    std::shared_ptr<faabric::device::Communicator> comm;
-    bool symmetric = false;
-    if (bytes > 0 && fdt >= 0 && fop >= 0 && tls.cachedComm != nullptr) {
-        // a buffer inside this rank's symmetric heap needs no driver query
-        symmetric = tls.cachedComm->inHeap(send, bytes) && tls.cachedComm->inHeap(recv, bytes);
-        if (symmetric || isDevicePointer(send)) {
-            comm = tls.cachedComm;
-        }
-    }
-    if (comm != nullptr) {
-        // Symmetric buffers may use any channel; others go through the single
-        // staging area on channel 0
-        if (symmetric && ((((uintptr_t)send) | ((uintptr_t)recv)) & 15) == 0 && groupIallreduce) {
+    const auto& comm = tls.cachedComm;
+    if (bytes > 0 && fdt >= 0 && fop >= 0 && comm != nullptr) {
+        const Placement at = placeCollective(*comm, groupIallreduce, send, bytes, recv, bytes, 0);
+        if (at.grouped) {
             // Deferred: the whole burst becomes ONE kernel at the next wait
             deferToGroup(faabric::device::Communicator::GROUP_ALLREDUCE,
                          comm,
@@ -1490,60 +1545,28 @@ int MpiWorld::iAllReduce(int rank, uint8_t* send, uint8_t* recv, faabric_datatyp
                          fop,
                          { send, recv, (size_t)count },
                          requestId,
-                         r,
+                         std::move(r),
                          deviceCollectives);
             return requestId;
         }
-        flushPendingGroup();
-        int nChannels = std::clamp(nonBlockingChannels.load(), 1, std::max(1, comm->config().channels));
-        int channel = symmetric ? (int)(tls.deviceCollectiveSeq++ % (uint64_t)nChannels) : 0;
-        cudaStream_t s = (cudaStream_t)streamForRank(rank, channel);
-        cudaSetDevice(comm->device());
-        int flags = (symmetric ? FB_FLAG_SYMMETRIC : 0) | FB_FLAG_CHANNEL(channel);
-        int rc = comm->allReduce(send, recv, (size_t)count, fdt, fop, forcedAllReduceAlgo, flags, s);
-        if (rc == FB_OK) {
-            deviceCollectives.fetch_add(1);
-            r.isDeviceCollective = true;
-            r.stream = s;
-            r.comm = comm;
-            tls.requests[requestId] = r;
-            return requestId;
-        }
-        if (rc != FB_E_UNSUPPORTED && rc != FB_E_TOO_LARGE) {
-            throw std::runtime_error(std::string("Device collective failed: ") + faabric::device::Communicator::errorString(rc));
+        if (at.symmetric || isDevicePointer(send)) {
+            // Symmetric buffers may use any channel; others go through the
+            // single staging area on channel 0
+            const int nChannels = std::clamp(nonBlockingChannels.load(), 1, std::max(1, comm->config().channels));
+            const int channel = at.symmetric ? (int)(tls.deviceCollectiveSeq++ % (uint64_t)nChannels) : 0;
+            const int flags = (at.symmetric ? FB_FLAG_SYMMETRIC : 0) | FB_FLAG_CHANNEL(channel);
+            void* s = streamForRank(rank, channel);
+            if (issueDevice(*comm, s, deviceCollectives, [&](auto& c, cudaStream_t st) {
+                    return c.allReduce(send, recv, (size_t)count, fdt, fop, forcedAllReduceAlgo, flags, st);
+                })) {
+                return recordDevice(requestId, std::move(r), comm, s);
+            }
         }
     }
     // Host path (or unsupported on the device): complete it now
     allReduce(rank, send, recv, dt, count, op);
-    tls.requests[requestId] = r;
+    tls.requests[requestId] = std::move(r);
     return requestId;
-}
-
-// Issues one device collective of a non-blocking call on channel 0: the
-// request completes when the stream drains.  False if the device cannot run it.
-static bool issueDeviceRequest(const std::shared_ptr<faabric::device::Communicator>& comm,
-                               void* stream,
-                               std::atomic<uint64_t>& counter,
-                               int requestId,
-                               AsyncRequest& r,
-                               const std::function<int(faabric::device::Communicator&, cudaStream_t)>& fn)
-{
-    flushPendingGroup();
-    cudaStream_t s = (cudaStream_t)stream;
-    cudaSetDevice(comm->device());
-    int rc = fn(*comm, s);
-    if (rc == FB_E_UNSUPPORTED || rc == FB_E_TOO_LARGE) {
-        return false;
-    }
-    if (rc != FB_OK) {
-        throw std::runtime_error(std::string("Device collective failed: ") + faabric::device::Communicator::errorString(rc));
-    }
-    counter.fetch_add(1);
-    r.isDeviceCollective = true;
-    r.stream = s;
-    r.comm = comm;
-    tls.requests[requestId] = r;
-    return true;
 }
 
 int MpiWorld::iReduceScatter(int rank,
@@ -1556,40 +1579,37 @@ int MpiWorld::iReduceScatter(int rank,
     using faabric::device::Communicator;
     checkRanksRange(0, rank);
     const size_t shard = (size_t)recvCount * dt->size;
-    int requestId = tls.nextRequestId++;
-    AsyncRequest r;
-    r.isSend = true; // nothing to drain on wait unless it becomes a device op
-    r.sendRank = rank;
-    r.recvRank = rank;
+    const int requestId = tls.nextRequestId++;
+    AsyncRequest r = collectiveRequest(rank);
     const int fdt = fbDtypeFor(dt);
     const int fop = fbOpFor(op);
     cacheDeviceComm(rank);
-    auto comm = tls.cachedComm;
+    const auto& comm = tls.cachedComm;
     // In place, the output overwrites input the peers are still reading: that
     // case (send == recv) runs the blocking call below
     if (shard > 0 && fdt >= 0 && fop >= 0 && comm != nullptr && send != recv) {
-        const bool symmetric = comm->inHeap(send, shard * size) && comm->inHeap(recv, shard);
-        if (symmetric && shard % 16 == 0 && ((((uintptr_t)send) | ((uintptr_t)recv)) & 15) == 0 && groupIallreduce) {
+        const Placement at = placeCollective(*comm, groupIallreduce, send, shard * size, recv, shard, shard);
+        if (at.grouped) {
             deferToGroup(Communicator::GROUP_REDUCE_SCATTER,
                          comm,
                          fdt,
                          fop,
                          { send, recv, (size_t)recvCount },
                          requestId,
-                         r,
+                         std::move(r),
                          deviceCollectives);
             return requestId;
         }
-        if ((symmetric || isDevicePointer(send)) &&
-            issueDeviceRequest(comm, streamForRank(rank, 0), deviceCollectives, requestId, r, [&](Communicator& c, cudaStream_t s) {
-                return c.reduceScatter(send, recv, (size_t)recvCount, fdt, fop, symFlag(c, send, shard * size), s);
+        void* s = tls.cachedStream0;
+        if ((at.symmetric || isDevicePointer(send)) && issueDevice(*comm, s, deviceCollectives, [&](auto& c, cudaStream_t st) {
+                return c.reduceScatter(send, recv, (size_t)recvCount, fdt, fop, symFlag(c, send, shard * size), st);
             })) {
-            return requestId;
+            return recordDevice(requestId, std::move(r), comm, s);
         }
     }
     // Host buffers, in place, or unsupported on the device: complete it now
     reduceScatter(rank, send, recv, dt, recvCount, op);
-    tls.requests[requestId] = r;
+    tls.requests[requestId] = std::move(r);
     return requestId;
 }
 
@@ -1604,31 +1624,29 @@ int MpiWorld::iAllGather(int rank,
     using faabric::device::Communicator;
     checkRanksRange(0, rank);
     const size_t bytes = (size_t)sendCount * sendType->size;
-    int requestId = tls.nextRequestId++;
-    AsyncRequest r;
-    r.isSend = true; // nothing to drain on wait unless it becomes a device op
-    r.sendRank = rank;
-    r.recvRank = rank;
+    const int requestId = tls.nextRequestId++;
+    AsyncRequest r = collectiveRequest(rank);
     cacheDeviceComm(rank);
-    auto comm = tls.cachedComm;
+    const auto& comm = tls.cachedComm;
     if (bytes > 0 && comm != nullptr) {
         const bool inPlace = send == recv + (size_t)rank * bytes;
-        const bool symmetric = comm->inHeap(send, bytes) && comm->inHeap(recv, bytes * size);
-        if (symmetric && bytes % 16 == 0 && ((((uintptr_t)send) | ((uintptr_t)recv)) & 15) == 0 && groupIallreduce) {
+        const Placement at = placeCollective(*comm, groupIallreduce, send, bytes, recv, bytes * size, bytes);
+        if (at.grouped) {
             // a byte copy: the burst's key is the communicator alone
-            deferToGroup(Communicator::GROUP_ALLGATHER, comm, FB_U8, -1, { send, recv, bytes }, requestId, r, deviceCollectives);
+            deferToGroup(Communicator::GROUP_ALLGATHER, comm, FB_U8, -1, { send, recv, bytes }, requestId, std::move(r), deviceCollectives);
             return requestId;
         }
-        if (!inPlace && (symmetric || isDevicePointer(send)) &&
-            issueDeviceRequest(comm, streamForRank(rank, 0), deviceCollectives, requestId, r, [&](Communicator& c, cudaStream_t s) {
-                return c.allGather(send, recv, bytes, symFlag(c, send, bytes), s);
+        void* s = tls.cachedStream0;
+        if (!inPlace && (at.symmetric || isDevicePointer(send)) &&
+            issueDevice(*comm, s, deviceCollectives, [&](auto& c, cudaStream_t st) {
+                return c.allGather(send, recv, bytes, symFlag(c, send, bytes), st);
             })) {
-            return requestId;
+            return recordDevice(requestId, std::move(r), comm, s);
         }
     }
     // Host buffers, or unsupported on the device: complete it now
     allGather(rank, send, sendType, sendCount, recv, recvType, recvCount);
-    tls.requests[requestId] = r;
+    tls.requests[requestId] = std::move(r);
     return requestId;
 }
 
@@ -1660,51 +1678,6 @@ bool MpiWorld::deviceFree(int rank, void* ptr)
     }
     comm->free(comm->offsetOf(ptr));
     return true;
-}
-
-// Stages device buffers through pinned host memory for the host algorithms
-namespace {
-struct HostStage
-{
-    std::vector<uint8_t> data;
-    uint8_t* devicePtr = nullptr;
-    bool active = false;
-
-    // in: copy device -> host now
-    uint8_t* in(const uint8_t* p, size_t bytes)
-    {
-        if (bytes == 0 || !MpiWorld::isDevicePointer(p)) {
-            return const_cast<uint8_t*>(p);
-        }
-        data.resize(bytes);
-        cudaMemcpy(data.data(), p, bytes, cudaMemcpyDeviceToHost);
-        devicePtr = const_cast<uint8_t*>(p);
-        active = true;
-        return data.data();
-    }
-
-    // out: host scratch now, copy host -> device in flush()
-    uint8_t* out(uint8_t* p, size_t bytes, bool preload = false)
-    {
-        if (bytes == 0 || !MpiWorld::isDevicePointer(p)) {
-            return p;
-        }
-        data.resize(bytes);
-        if (preload) {
-            cudaMemcpy(data.data(), p, bytes, cudaMemcpyDeviceToHost);
-        }
-        devicePtr = p;
-        active = true;
-        return data.data();
-    }
-
-    void flush()
-    {
-        if (active) {
-            cudaMemcpy(devicePtr, data.data(), data.size(), cudaMemcpyHostToDevice);
-        }
-    }
-};
 }
 
 // ---------------------------------------------------------------------------
@@ -1964,7 +1937,7 @@ void MpiWorld::reduce(int sendRank,
         reduce(sendRank, recvRank, s, r, datatype, count, operation);
         if (isRoot) {
             if (inPlace) {
-                cudaMemcpy(recvBuffer, s, bytes, cudaMemcpyHostToDevice);
+                copyBytes(recvBuffer, s, bytes);
             } else {
                 out.flush();
             }
@@ -2079,7 +2052,7 @@ void MpiWorld::allReduce(int rank,
         uint8_t* r = sendBuffer == recvBuffer ? s : out.out(recvBuffer, bytes);
         allReduce(rank, s, r, datatype, count, operation);
         if (sendBuffer == recvBuffer) {
-            cudaMemcpy(recvBuffer, s, bytes, cudaMemcpyHostToDevice);
+            copyBytes(recvBuffer, s, bytes);
         } else {
             out.flush();
         }
@@ -2106,10 +2079,9 @@ void MpiWorld::reduceScatter(int rank,
         int fdt = fbDtypeFor(datatype);
         int fop = fbOpFor(operation);
         auto comm = (fdt >= 0 && fop >= 0) ? getDeviceComm(rank) : nullptr;
-        if (runDevice(comm, streamForRank(rank), [&](faabric::device::Communicator& c, cudaStream_t s) {
+        if (issueAndWait(comm, streamForRank(rank), deviceCollectives, [&](auto& c, cudaStream_t s) {
                 return c.reduceScatter(sendBuffer, recvBuffer, (size_t)recvCount, fdt, fop, symFlag(c, sendBuffer, sliceBytes * size), s);
             })) {
-            deviceCollectives.fetch_add(1);
             return;
         }
     }
@@ -2442,7 +2414,7 @@ void MpiWorld::scan(int rank,
         uint8_t* r = sendBuffer == recvBuffer ? s : out.out(recvBuffer, bytes);
         scan(rank, s, r, datatype, count, operation);
         if (sendBuffer == recvBuffer) {
-            cudaMemcpy(recvBuffer, s, bytes, cudaMemcpyHostToDevice);
+            copyBytes(recvBuffer, s, bytes);
         } else {
             out.flush();
         }

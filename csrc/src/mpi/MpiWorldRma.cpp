@@ -10,6 +10,7 @@
 #include <faabric/util/logging.h>
 #include <faabric/util/macros.h>
 
+#include "buffers.h"
 #include "device/loopback_kernels.h"
 #include "launch_api.h"
 
@@ -44,33 +45,6 @@ struct RmaWireOp
     int32_t op;
     int32_t pad;
 };
-
-// Where a buffer lives: a CUDA device, HOST_MEMORY (also the loopback
-// backend's heaps) or ANY_DEVICE (managed memory)
-constexpr int HOST_MEMORY = -1;
-constexpr int ANY_DEVICE = -2;
-
-int bufferDevice(const void* p)
-{
-    if (p == nullptr || faabric::device::Communicator::isLoopbackHeapPointer(p) || !faabric::device::cudaAvailable()) {
-        return HOST_MEMORY;
-    }
-    cudaPointerAttributes attr;
-    if (cudaPointerGetAttributes(&attr, p) != cudaSuccess) {
-        cudaGetLastError();
-        return HOST_MEMORY;
-    }
-    if (attr.type == cudaMemoryTypeDevice) {
-        return attr.device;
-    }
-    return attr.type == cudaMemoryTypeManaged ? ANY_DEVICE : HOST_MEMORY;
-}
-
-bool reachable(const void* p, int device)
-{
-    const int where = bufferDevice(p);
-    return p == nullptr || where == device || where == ANY_DEVICE;
-}
 
 void cudaCheck(cudaError_t e, const char* what)
 {
@@ -127,7 +101,11 @@ struct RmaStage
       , out(resultIn)
     {
         const size_t parts[3] = { origin != nullptr ? bytes : 0, compare != nullptr ? esize : 0, result != nullptr ? bytes : 0 };
-        staged = !reachable(origin, device) || !reachable(compare, device) || !reachable(result, device);
+        auto reachable = [&](const void* p) {
+            const int where = bufferDevice(p);
+            return p == nullptr || where == device || where == ANY_DEVICE;
+        };
+        staged = !reachable(origin) || !reachable(compare) || !reachable(result);
         if (!staged) {
             return;
         }
@@ -180,13 +158,6 @@ struct RmaStage
     }
 };
 
-// True if a copy between the two goes through CUDA (without a GPU, the
-// loopback backend's heaps are plain host memory)
-bool cudaCopy(const void* dst, const void* src)
-{
-    return (MpiWorld::isDevicePointer(dst) || MpiWorld::isDevicePointer(src)) && faabric::device::cudaAvailable();
-}
-
 // Every request of `p` to a target that `covered` names is complete
 template<class F>
 void markComplete(const std::shared_ptr<MpiWorld::RmaProgress>& p, F covered)
@@ -198,21 +169,6 @@ void markComplete(const std::shared_ptr<MpiWorld::RmaProgress>& p, F covered)
         if (covered((int)t)) {
             p->completed[t] = p->issued[t];
         }
-    }
-}
-
-void rmaCopy(void* dst, const void* src, size_t bytes)
-{
-    if (bytes == 0) {
-        return;
-    }
-    if (cudaCopy(dst, src)) {
-        if (cudaMemcpy(dst, src, bytes, cudaMemcpyDefault) != cudaSuccess) {
-            cudaGetLastError();
-            throw std::runtime_error("Device copy for a one-sided operation failed");
-        }
-    } else {
-        memcpy(dst, src, bytes);
     }
 }
 }
@@ -355,9 +311,9 @@ void MpiWorld::winPut(int rank, int winId, const uint8_t* origin, size_t bytes, 
     if (isLocalRank(targetRank)) {
         // Same address space (or peer-mapped HBM): write it now, the closing
         // fence (or flush) publishes it
-        rmaCopy(dst, origin, bytes);
+        copyBytes(dst, origin, bytes);
         if (!w->epochs[rank].locked.empty()) {
-            w->epochs[rank].deviceCopies |= cudaCopy(dst, origin);
+            w->epochs[rank].deviceCopies |= !hostAddressable(dst) || !hostAddressable(origin);
         }
         return;
     }
@@ -370,9 +326,9 @@ void MpiWorld::winGet(int rank, int winId, uint8_t* origin, size_t bytes, int ta
     auto w = getWindow(winId);
     uint8_t* src = winTargetPtr(*w, targetRank, targetDisp, bytes);
     if (isLocalRank(targetRank)) {
-        rmaCopy(origin, src, bytes);
+        copyBytes(origin, src, bytes);
         if (!w->epochs[rank].locked.empty()) {
-            w->epochs[rank].deviceCopies |= cudaCopy(origin, src);
+            w->epochs[rank].deviceCopies |= !hostAddressable(origin) || !hostAddressable(src);
         }
         return;
     }
@@ -572,7 +528,7 @@ int MpiWorld::winAccumulate(int rank,
     q.result = result;
     if (fop != FB_OP_NO_OP) {
         q.data.resize(bytes);
-        rmaCopy(q.data.data(), origin, bytes);
+        copyBytes(q.data.data(), origin, bytes);
     }
     w->pending[rank].push_back(std::move(q));
     return MPI_SUCCESS;
@@ -605,8 +561,8 @@ int MpiWorld::winCompareSwap(int rank,
     RmaOp q{ RMA_COMPARE_SWAP, targetRank, (uint64_t)(target - (uint8_t*)(uintptr_t)w->bases[targetRank]), esize, nullptr };
     q.dtype = dtype;
     q.data.resize(2 * esize);
-    rmaCopy(q.data.data(), origin, esize);
-    rmaCopy(q.data.data() + esize, compare, esize);
+    copyBytes(q.data.data(), origin, esize);
+    copyBytes(q.data.data() + esize, compare, esize);
     q.result = result;
     w->pending[rank].push_back(std::move(q));
     return MPI_SUCCESS;
@@ -642,7 +598,7 @@ void MpiWorld::rmaSendOps(RmaWindow& w, int rank, int peer)
         } else {
             fetched.resize(op->bytes);
             recv(peer, rank, fetched.data(), byteType, (int)op->bytes, nullptr, MpiMessageType::RMA_DATA);
-            rmaCopy(op->result, fetched.data(), op->bytes);
+            copyBytes(op->result, fetched.data(), op->bytes);
         }
     }
 }
@@ -989,7 +945,7 @@ int MpiWorld::rmaComplete(RmaWindow& w, int winId, int rank, int targetRank, boo
         const size_t payloadBytes = op.kind == RMA_PUT ? op.bytes : op.kind == RMA_GET ? 0 : op.data.size();
         if (payloadBytes > 0) {
             req.resize(req.size() + payloadBytes);
-            rmaCopy(req.data() + req.size() - payloadBytes, payload, payloadBytes);
+            copyBytes(req.data() + req.size() - payloadBytes, payload, payloadBytes);
         }
         if (op.kind == RMA_GET || op.kind == RMA_GET_ACCUMULATE || op.kind == RMA_COMPARE_SWAP) {
             replies.push_back(&op);
@@ -1016,8 +972,8 @@ int MpiWorld::rmaComplete(RmaWindow& w, int winId, int rank, int targetRank, boo
         bool toDevice = false;
         for (const RmaOp* op : replies) {
             uint8_t* dst = op->kind == RMA_GET ? op->origin : op->result;
-            rmaCopy(dst, fetched.data() + off, op->bytes);
-            toDevice |= cudaCopy(dst, nullptr);
+            copyBytes(dst, fetched.data() + off, op->bytes);
+            toDevice |= !hostAddressable(dst);
             off += op->bytes;
         }
         if (toDevice) {
@@ -1224,10 +1180,12 @@ int MpiWorld::winRputGet(int rank, int winId, uint8_t* origin, size_t bytes, int
     }
     if (isLocalRank(targetRank) && bytes > 0) {
         // Heap to heap, origin on the origin's GPU: one launch for the batch
+        // (on the loopback backend the origin is in a heap: device-role
+        // memory that memcpy reaches)
         auto comm = wiredDeviceComm(rank);
         auto targetComm = wiredDeviceComm(targetRank);
         const bool originOk =
-          comm != nullptr && (comm->isLoopback() ? faabric::device::Communicator::isLoopbackHeapPointer(origin)
+          comm != nullptr && (comm->isLoopback() ? isDevicePointer(origin) && hostAddressable(origin)
                                                  : comm->inHeap(origin, bytes) || bufferDevice(origin) == comm->device());
         if (originOk && targetComm != nullptr && targetComm->inHeap(target, bytes)) {
             auto& batch = w->batches[rank];
@@ -1247,7 +1205,7 @@ int MpiWorld::winRputGet(int rank, int winId, uint8_t* origin, size_t bytes, int
     } else {
         winPut(rank, winId, origin, bytes, targetRank, targetDisp);
     }
-    if (isLocalRank(targetRank) && cudaCopy(origin, target)) {
+    if (isLocalRank(targetRank) && (!hostAddressable(origin) || !hostAddressable(target))) {
         // complete at issue: a cudaMemcpy that involves pageable memory may
         // return before its DMA lands, and the request's wait does nothing
         cudaCheck(cudaStreamSynchronize(cudaStreamLegacy), "Request-based one-sided copy");

@@ -13,9 +13,8 @@
 #include <faabric/util/config.h>
 #include <faabric/util/logging.h>
 
+#include "buffers.h"
 #include "subcomm.h"
-
-#include <cuda_runtime.h>
 
 #include <algorithm>
 #include <atomic>
@@ -80,19 +79,6 @@ int terminateMpi()
 const void* resolveInPlace(const void* sendbuf, void* recvbuf)
 {
     return sendbuf == MPI_IN_PLACE ? recvbuf : sendbuf;
-}
-
-// Host<->host copies must not depend on a CUDA device being present
-static void copyAny(void* dst, const void* src, size_t bytes)
-{
-    if (bytes == 0 || dst == src) {
-        return;
-    }
-    if (MpiWorld::isDevicePointer(dst) || MpiWorld::isDevicePointer(src)) {
-        cudaMemcpy(dst, src, bytes, cudaMemcpyDefault);
-    } else {
-        memcpy(dst, src, bytes);
-    }
 }
 
 // ---- sub-communicators ----
@@ -577,7 +563,7 @@ int MPI_Gatherv(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void*
             uint8_t* dst = (uint8_t*)recvbuf + (size_t)displs[r] * recvtype->size;
             if (r == root) {
                 if (sendbuf != MPI_IN_PLACE) {
-                    copyAny(dst, sendbuf, (size_t)sendcount * sendtype->size);
+                    copyBytes(dst, sendbuf, (size_t)sendcount * sendtype->size);
                 }
             } else {
                 world.recv(r, root, dst, recvtype, recvcounts[r], nullptr, MpiMessageType::GATHER);
@@ -681,19 +667,14 @@ int MPI_Reduce_scatter(const void* sendbuf, void* recvbuf, const int* recvcounts
             total += (size_t)recvcounts[r];
         }
         std::vector<uint8_t> reduced(rank == 0 ? total * datatype->size : 0);
-        std::vector<uint8_t> hostSend;
-        const uint8_t* src = (const uint8_t*)send;
-        if (MpiWorld::isDevicePointer(src)) {
-            hostSend.resize(total * datatype->size);
-            copyAny(hostSend.data(), src, hostSend.size());
-            src = hostSend.data();
-        }
-        world.reduce(rank, 0, (uint8_t*)src, reduced.data(), datatype, (int)total, op);
+        HostStage hostSend;
+        uint8_t* src = hostSend.in((const uint8_t*)send, total * datatype->size);
+        world.reduce(rank, 0, src, reduced.data(), datatype, (int)total, op);
         if (rank == 0) {
             for (int r = 1; r < size; r++) {
                 world.send(0, r, reduced.data() + offsets[r] * datatype->size, datatype, recvcounts[r], MpiMessageType::SCATTER);
             }
-            copyAny(recvbuf, reduced.data(), (size_t)recvcounts[0] * datatype->size);
+            copyBytes(recvbuf, reduced.data(), (size_t)recvcounts[0] * datatype->size);
         } else {
             world.recv(0, rank, (uint8_t*)recvbuf, datatype, recvcounts[rank], nullptr, MpiMessageType::SCATTER);
         }
@@ -762,7 +743,7 @@ int MPI_Alltoallv(const void* sendbuf, const int sendcounts[], const int sdispls
         uint8_t* dst = (uint8_t*)recvbuf + (size_t)rdispls[r] * recvtype->size;
         const uint8_t* src = (const uint8_t*)sendbuf + (size_t)sdispls[r] * sendtype->size;
         if (r == rank) {
-            copyAny(dst, src, (size_t)sendcounts[r] * sendtype->size);
+            copyBytes(dst, src, (size_t)sendcounts[r] * sendtype->size);
         } else {
             reqs.push_back(world.irecv(r, rank, dst, recvtype, recvcounts[r], MpiMessageType::ALLTOALL));
         }

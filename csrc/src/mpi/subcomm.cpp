@@ -1,60 +1,16 @@
 #include "subcomm.h"
+#include "buffers.h"
 
 #include <faabric/util/logging.h>
 
-#include <cuda_runtime.h>
-
 #include <algorithm>
 #include <atomic>
-#include <cstring>
 #include <map>
 #include <mutex>
 #include <shared_mutex>
 #include <stdexcept>
 
 namespace faabric::mpi {
-
-namespace {
-// Host memory, or the loopback backend's heap (host memory in the device role)
-bool hostAddressable(const void* p)
-{
-    return !MpiWorld::isDevicePointer(p) || faabric::device::Communicator::isLoopbackHeapPointer(p);
-}
-
-// Host<->host copies must not depend on a CUDA device being present
-void copyBytes(void* dst, const void* src, size_t bytes)
-{
-    if (bytes == 0 || dst == src) {
-        return;
-    }
-    if (!hostAddressable(dst) || !hostAddressable(src)) {
-        if (cudaMemcpy(dst, src, bytes, cudaMemcpyDefault) != cudaSuccess) {
-            cudaGetLastError();
-            throw std::runtime_error("Device copy inside a sub-communicator collective failed");
-        }
-    } else {
-        memcpy(dst, src, bytes);
-    }
-}
-
-// Reductions run on the host: device operands are brought over first
-struct HostView
-{
-    std::vector<uint8_t> staged;
-    uint8_t* ptr = nullptr;
-
-    HostView(const uint8_t* p, size_t bytes)
-    {
-        if (bytes > 0 && !hostAddressable(p)) {
-            staged.resize(bytes);
-            copyBytes(staged.data(), p, bytes);
-            ptr = staged.data();
-        } else {
-            ptr = const_cast<uint8_t*>(p);
-        }
-    }
-};
-}
 
 SubCommunicator::SubCommunicator(int commIdIn, int worldIdIn, std::vector<int> worldRanksIn)
   : commId(commIdIn)
@@ -191,8 +147,8 @@ void SubCommunicator::scan(MpiWorld& w,
         return;
     }
     const int myCommRank = commRankOf(me);
-    HostView mine(send, bytes);
-    std::vector<uint8_t> acc(mine.ptr, mine.ptr + bytes);
+    std::vector<uint8_t> acc(bytes);
+    copyBytes(acc.data(), send, bytes);
     if (myCommRank > 0) {
         std::vector<uint8_t> prev(bytes);
         w.recv(worldRanks[myCommRank - 1], me, prev.data(), dt, count, nullptr);

@@ -22,10 +22,23 @@
 #include <faabric/util/testing.h>
 
 #include <atomic>
+#include <cstdlib>
 #include <functional>
 #include <map>
 
 namespace tests {
+
+// The loopback device backend (heaps in host memory, no GPU needed) for the
+// lifetime of the object; the configuration is reset afterwards
+struct LoopbackBackend
+{
+    LoopbackBackend() { setenv("FAABRIC_DEVICE_BACKEND", "loopback", 1); }
+    ~LoopbackBackend()
+    {
+        unsetenv("FAABRIC_DEVICE_BACKEND");
+        faabric::util::getSystemConfig().reset();
+    }
+};
 
 typedef std::function<int(faabric::executor::Executor*, int, int, std::shared_ptr<faabric::BatchExecuteRequest>)>
   TestFunction;

@@ -11,6 +11,7 @@
 
 #include "launch_api.h"
 
+#include <algorithm>
 #include <atomic>
 #include <cmath>
 #include <cstring>
@@ -18,6 +19,7 @@
 #include <limits>
 #include <numeric>
 #include <random>
+#include <set>
 #include <thread>
 
 using faabric::device::CommConfig;
@@ -1044,7 +1046,7 @@ int loopbackMpiBody(int rank, int size)
 TEST_CASE("loopback: the MPI C API dispatches to the device communicator without a GPU", "[loopback][mpi]")
 {
     using namespace tests;
-    setenv("FAABRIC_DEVICE_BACKEND", "loopback", 1);
+    LoopbackBackend loopback;
     const int worldSize = 4;
     {
         ClusterFixture f(worldSize);
@@ -1076,6 +1078,168 @@ TEST_CASE("loopback: the MPI C API dispatches to the device communicator without
         REQUIRE(loopbackDeviceCollectives.load() >= 30u + 5u);
         faabric::mpi::getMpiWorldRegistry().clear();
     }
-    unsetenv("FAABRIC_DEVICE_BACKEND");
-    faabric::util::getSystemConfig().reset();
+}
+
+namespace {
+// Commutative and associative: a op b = a + b + 1, so a missing or stale
+// contribution shows in every element
+void plusOneFn(void* in, void* inout, int* len, MPI_Datatype*)
+{
+    auto* a = (const int*)in;
+    auto* b = (int*)inout;
+    for (int i = 0; i < *len; i++) {
+        b[i] = a[i] + b[i] + 1;
+    }
+}
+
+// Host fallbacks of the MPI C API on MPI_Alloc_mem(MPI_INFO_FAABRIC_DEVICE)
+// memory, which the loopback backend keeps in host memory: a user-defined
+// operation, the own blocks of the v-collectives and uneven reduce-scatter
+// blocks.  Every rank runs every call whatever it finds, so a wrong result
+// cannot leave a peer waiting.
+int loopbackHostFallbackBody(int rank, int size)
+{
+    std::set<int> failedLines;
+    auto check = [&](bool ok, int line) {
+        if (!ok && failedLines.insert(line).second) {
+            printf("         rank %d: check failed at line %d\n", rank, line);
+        }
+    };
+    MPI_Op plusOne = nullptr;
+    check(MPI_Op_create(plusOneFn, 1, &plusOne) == MPI_SUCCESS, __LINE__);
+    const int n = 300;
+    int *a = nullptr, *b = nullptr;
+    check(MPI_Alloc_mem(n * sizeof(int), MPI_INFO_FAABRIC_DEVICE, &a) == MPI_SUCCESS, __LINE__);
+    check(MPI_Alloc_mem(n * sizeof(int), MPI_INFO_FAABRIC_DEVICE, &b) == MPI_SUCCESS, __LINE__);
+    check(faabric::mpi::MpiWorld::isDevicePointer(a) && faabric::mpi::MpiWorld::isDevicePointer(b), __LINE__);
+    auto value = [](int r, int i) { return r * 1000 + i; };
+    // op over ranks [0, last]
+    auto folded = [&](int last, int i) {
+        int v = 0;
+        for (int r = 0; r <= last; r++) {
+            v += value(r, i);
+        }
+        return v + last;
+    };
+    auto fill = [&](int* p, int v) { std::fill(p, p + n, v); };
+    auto load = [&]() {
+        for (int i = 0; i < n; i++) {
+            a[i] = value(rank, i);
+        }
+    };
+
+    load();
+    fill(b, -1);
+    MPI_Allreduce(a, b, n, MPI_INT, plusOne, MPI_COMM_WORLD);
+    for (int i = 0; i < n; i++) {
+        check(b[i] == folded(size - 1, i) && a[i] == value(rank, i), __LINE__);
+    }
+    MPI_Allreduce(MPI_IN_PLACE, a, n, MPI_INT, plusOne, MPI_COMM_WORLD);
+    for (int i = 0; i < n; i++) {
+        check(a[i] == folded(size - 1, i), __LINE__);
+    }
+
+    const int root = 2;
+    load();
+    fill(b, -1);
+    MPI_Reduce(a, rank == root ? b : nullptr, n, MPI_INT, plusOne, root, MPI_COMM_WORLD);
+    for (int i = 0; rank == root && i < n; i++) {
+        check(b[i] == folded(size - 1, i), __LINE__);
+    }
+
+    load();
+    fill(b, -1);
+    MPI_Scan(a, b, n, MPI_INT, plusOne, MPI_COMM_WORLD);
+    for (int i = 0; i < n; i++) {
+        check(b[i] == folded(rank, i), __LINE__);
+    }
+
+    // Gatherv to rank 1: rank r sends r + 1 ints, blocks two apart
+    const int gatherRoot = 1;
+    std::vector<int> counts(size), displs(size);
+    for (int r = 0, off = 0; r < size; r++) {
+        counts[r] = r + 1;
+        displs[r] = off;
+        off += counts[r] + 2;
+    }
+    load();
+    fill(b, -1);
+    MPI_Gatherv(a, rank + 1, MPI_INT, b, counts.data(), displs.data(), MPI_INT, gatherRoot, MPI_COMM_WORLD);
+    for (int r = 0; rank == gatherRoot && r < size; r++) {
+        for (int j = 0; j < counts[r]; j++) {
+            check(b[displs[r] + j] == value(r, j), __LINE__);
+        }
+        check(b[displs[r] + counts[r]] == -1, __LINE__);
+    }
+
+    // Alltoallv: rank s sends (s + d) % 3 + 1 ints to rank d
+    auto pairCount = [](int s, int d) { return (s + d) % 3 + 1; };
+    std::vector<int> sendCounts(size), sendDispls(size), recvCounts(size), recvDispls(size);
+    for (int r = 0, so = 0, ro = 0; r < size; r++) {
+        sendCounts[r] = pairCount(rank, r);
+        recvCounts[r] = pairCount(r, rank);
+        sendDispls[r] = so;
+        recvDispls[r] = ro;
+        so += sendCounts[r];
+        ro += recvCounts[r];
+    }
+    for (int r = 0; r < size; r++) {
+        for (int j = 0; j < sendCounts[r]; j++) {
+            a[sendDispls[r] + j] = value(rank, r * 10 + j);
+        }
+    }
+    fill(b, -1);
+    MPI_Alltoallv(a, sendCounts.data(), sendDispls.data(), MPI_INT, b, recvCounts.data(), recvDispls.data(), MPI_INT,
+                  MPI_COMM_WORLD);
+    for (int r = 0; r < size; r++) {
+        for (int j = 0; j < recvCounts[r]; j++) {
+            check(b[recvDispls[r] + j] == value(r, rank * 10 + j), __LINE__);
+        }
+    }
+
+    // Reduce_scatter with uneven blocks: rank r keeps r + 1 elements
+    load();
+    fill(b, -1);
+    MPI_Reduce_scatter(a, b, counts.data(), MPI_INT, MPI_SUM, MPI_COMM_WORLD);
+    const int first = rank * (rank + 1) / 2;
+    for (int j = 0; j < counts[rank]; j++) {
+        check(b[j] == folded(size - 1, first + j) - (size - 1), __LINE__);
+    }
+    check(b[counts[rank]] == -1, __LINE__);
+
+    check(MPI_Op_free(&plusOne) == MPI_SUCCESS, __LINE__);
+    MPI_Free_mem(a);
+    MPI_Free_mem(b);
+    return (int)failedLines.size();
+}
+}
+
+TEST_CASE("loopback: host fallbacks of the MPI C API on device-role memory without a GPU", "[loopback][mpi]")
+{
+    using namespace tests;
+    LoopbackBackend loopback;
+    const int worldSize = 4;
+    ClusterFixture f(worldSize);
+    REQUIRE_EQ(f.conf.deviceBackend, std::string("loopback"));
+    registerTestFunction("mpi", "loopback-host-fallback", [&](auto*, int, int, auto) {
+        MPI_Init(nullptr, nullptr);
+        int rank = -1, size = -1;
+        MPI_Comm_rank(MPI_COMM_WORLD, &rank);
+        MPI_Comm_size(MPI_COMM_WORLD, &size);
+        int rc = loopbackHostFallbackBody(rank, size);
+        MPI_Finalize();
+        return rc;
+    });
+    auto req = faabric::util::batchExecFactory("mpi", "loopback-host-fallback", 1);
+    req->mutable_messages(0)->set_ismpi(true);
+    req->mutable_messages(0)->set_mpiworldsize(worldSize);
+    f.plannerCli.callFunctions(req);
+    auto status = f.awaitBatch(req, 60000);
+    REQUIRE_EQ(status->messageresults_size(), worldSize);
+    for (auto& m : status->messageresults()) {
+        if (m.returnvalue() != 0) {
+            fbtest::fail(__FILE__, __LINE__, "rank " + std::to_string(m.mpirank()) + " failed");
+        }
+    }
+    faabric::mpi::getMpiWorldRegistry().clear();
 }

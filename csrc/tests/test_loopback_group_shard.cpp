@@ -476,9 +476,7 @@ void runGroupShardMpi(const std::string& name, int worldSize)
 
 TEST_CASE("loopback group shard: MPI_Ireduce_scatter_block and MPI_Iallgather bursts", "[loopback][mpi]")
 {
-    setenv("FAABRIC_DEVICE_BACKEND", "loopback", 1);
+    tests::LoopbackBackend loopback;
     runGroupShardMpi("group-shard-loopback-4", 4);
     runGroupShardMpi("group-shard-loopback-3", 3);
-    unsetenv("FAABRIC_DEVICE_BACKEND");
-    faabric::util::getSystemConfig().reset();
 }

@@ -59,16 +59,6 @@ void runAtomics(const std::string& name, int worldSize, const Setup& s)
     });
 }
 
-struct LoopbackBackend
-{
-    LoopbackBackend() { setenv("FAABRIC_DEVICE_BACKEND", "loopback", 1); }
-    ~LoopbackBackend()
-    {
-        unsetenv("FAABRIC_DEVICE_BACKEND");
-        faabric::util::getSystemConfig().reset();
-    }
-};
-
 // Every reduction call refuses the two accumulate-only ops before any rank
 // sends, waits or launches: a later collective still lines up
 int refusedByCollectives(int rank, int size, bool deviceBuffers, std::string* why)

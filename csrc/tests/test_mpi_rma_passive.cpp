@@ -51,16 +51,6 @@ void runPassive(const std::string& name, int worldSize, const Setup& s)
     faabric::mpi::getMpiWorldRegistry().clear();
 }
 
-struct LoopbackBackend
-{
-    LoopbackBackend() { setenv("FAABRIC_DEVICE_BACKEND", "loopback", 1); }
-    ~LoopbackBackend()
-    {
-        unsetenv("FAABRIC_DEVICE_BACKEND");
-        faabric::util::getSystemConfig().reset();
-    }
-};
-
 // 2 and 4 ranks sharing the GPU, and one rank per GPU when there are several
 std::vector<int> gpuWorldSizes()
 {

@@ -52,16 +52,6 @@ void runRequest(const std::string& name, int worldSize, const Setup& s)
     }
     faabric::mpi::getMpiWorldRegistry().clear();
 }
-
-struct LoopbackBackend
-{
-    LoopbackBackend() { setenv("FAABRIC_DEVICE_BACKEND", "loopback", 1); }
-    ~LoopbackBackend()
-    {
-        unsetenv("FAABRIC_DEVICE_BACKEND");
-        faabric::util::getSystemConfig().reset();
-    }
-};
 }
 
 TEST_CASE("mpi rma request: host windows", "[mpi][rma]")

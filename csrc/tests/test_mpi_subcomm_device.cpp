@@ -49,16 +49,6 @@ void runSubcommDevice(const std::string& name, int worldSize, const Setup& s)
     }
     faabric::mpi::getMpiWorldRegistry().clear();
 }
-
-struct LoopbackBackend
-{
-    LoopbackBackend() { setenv("FAABRIC_DEVICE_BACKEND", "loopback", 1); }
-    ~LoopbackBackend()
-    {
-        unsetenv("FAABRIC_DEVICE_BACKEND");
-        faabric::util::getSystemConfig().reset();
-    }
-};
 }
 
 TEST_CASE("mpi sub-communicators: fused collectives on heap buffers (loopback)", "[mpi][loopback]")
