@@ -184,6 +184,10 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     uint64_t offsetOf(const void* p) const;
     size_t userHeapBytes() const { return cfg_.heapBytes; }
 
+    // True if the reduction kernels implement (FbDtype, FbOp); the reductions
+    // return FB_E_UNSUPPORTED for other pairs
+    static bool reduces(int dtype, int op);
+
     // ---- collectives.  Return 0 or a negative FB_E_* code.  `bytes`-based
     // calls are type-agnostic; reductions take FbDtype / FbOp. ----
     int allReduce(const void* send,
@@ -216,6 +220,9 @@ class Communicator : public std::enable_shared_from_this<Communicator>
              int op,
              int flags,
              cudaStream_t s);
+    // (Reductions with FB_FLAG_SYMMETRIC take heap buffers at any heap
+    // offset: an input, or a pushed output, at an offset that is not a
+    // multiple of 16 goes through the staging copy.)
     // Data movement.  Local (non-heap) destinations may sit at any alignment,
     // different on every rank.  With FB_FLAG_SYMMETRIC, every rank passes
     // the same kind of buffer at the same heap offset, outputs included: an

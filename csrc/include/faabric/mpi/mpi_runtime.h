@@ -345,6 +345,11 @@ class MpiWorld
 
     bool deviceFree(int rank, void* ptr);
 
+    // True if `operation` is defined on `datatype`: a user op, or a built-in
+    // op that op_reduce() implements for the datatype's base type.  The
+    // reduction calls refuse other pairs before any rank communicates.
+    static bool reducible(faabric_datatype_t* datatype, faabric_op_t* operation);
+
     void op_reduce(faabric_op_t* operation,
                    faabric_datatype_t* datatype,
                    int count,

@@ -1379,6 +1379,11 @@ enum ReduceKind
     K_SCAN = 3
 };
 
+bool Communicator::reduces(int dtype, int op)
+{
+    return fb::findReduceLaunchers(dtype, op) != nullptr;
+}
+
 int Communicator::reduceLike(int kind,
                              const void* send,
                              void* recv,
@@ -1416,6 +1421,14 @@ int Communicator::reduceLike(int kind,
     }
     if (symmetric && (!inHeap(send, bytes))) {
         return FB_E_INVALID;
+    }
+    if (symmetric && (offsetOf(send) % 16) != 0) {
+        // The kernels load peers' inputs as 16-byte vectors at heap[p] +
+        // offset: an input at an offset that is not a multiple of 16 goes
+        // through the staging copy.  Offsets are the same on every rank, so
+        // every rank takes the same decision.
+        symmetric = false;
+        flags &= ~FB_FLAG_SYMMETRIC;
     }
     if (symmetric && (kind == K_SCAN || kind == K_REDUCE_SCATTER)) {
         // These read the peers' inputs while every rank writes its output with
@@ -1533,13 +1546,15 @@ int Communicator::reduceLike(int kind,
     // which algorithms write through the symmetric recv offset
     const bool pushes = (algo == FB_ALGO_TWOSHOT) ||
                         (algo == FB_ALGO_NVLS && kind == K_ALLREDUCE);
+    // (whether the output lives in the symmetric heap, and at which offset, is
+    // part of the call's contract: all ranks pass the same kind of buffer, so
+    // a pushed output at an offset that is not a multiple of 16 is staged on
+    // every rank)
+    const bool stageRecvGlobal =
+      pushes && (kind == K_REDUCE || !symmetric || !inHeap(recv, bytes) || (offsetOf(recv) % 16) != 0);
     bool stageRecv = false;
     if (pushes) {
-        if (kind == K_REDUCE) {
-            stageRecv = true; // only the root has a recv buffer
-        } else {
-            stageRecv = !symmetric || !inHeap(recv, bytes);
-        }
+        stageRecv = stageRecvGlobal; // (reduce: only the root has a recv buffer)
     } else if (isRootOrAll && (((uintptr_t)recv) & 15)) {
         stageRecv = true; // vector stores need 16-byte alignment
     }
@@ -1554,9 +1569,6 @@ int Communicator::reduceLike(int kind,
     // barrier epochs advance with it), so it only depends on `symmetric`,
     // `algo`, `kind` and `bytes`; a rank-LOCAL need for output staging (an
     // unaligned destination) must fit one piece
-    // (whether the output lives in the symmetric heap is part of the call's
-    // contract: all ranks pass the same kind of buffer)
-    const bool stageRecvGlobal = pushes && (kind == K_REDUCE || !symmetric || !inHeap(recv, bytes));
     const uint64_t chunkMax =
       (stageSend || stageRecvGlobal) ? (uint64_t)cfg_.stageBytes : bytes;
     if (stageRecv && !stageRecvGlobal && !stageSend && bytes > cfg_.stageBytes) {

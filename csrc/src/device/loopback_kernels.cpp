@@ -350,8 +350,41 @@ static void reduceRange(const FbCommDev& c,
 }
 
 // --------------------------------------------------------------- reduce ----
+// The CUDA kernel loads and stores its vector body [vecBegin, vecEnd) as
+// 16-byte vectors: every address it touches that way must be 16-byte aligned
+// and the body must lie in the whole-vector part of the message.  The
+// element-wise tail has no such condition.
+static bool reduceBodyOk(const ReduceArgs& a)
+{
+    const FbCommDev& c = a.comm;
+    if (a.vecEnd <= a.vecBegin) {
+        return true;
+    }
+    if (a.vecEnd * 16 > a.bytes - (a.bytes & 15)) {
+        return false;
+    }
+    auto aligned = [](const void* p) { return ((uintptr_t)p & 15) == 0; };
+    for (int p = 0; p < a.readRanks; p++) {
+        if (!aligned(c.heap[p] + a.sendOff)) {
+            return false;
+        }
+    }
+    if (a.pushMask == 0) {
+        return aligned(a.recvLocal);
+    }
+    for (int p = 0; p < c.nranks; p++) {
+        if ((a.pushMask & (1u << p)) && !aligned(c.heap[p] + a.recvOff)) {
+            return false;
+        }
+    }
+    return true;
+}
+
 cudaError_t reduceKernel(const ReduceArgs& a, int dtype, int op, int blocks, int, cudaStream_t)
 {
+    if (!reduceBodyOk(a)) {
+        return cudaErrorMisalignedAddress;
+    }
     const FbCommDev& c = a.comm;
     bool ok = true;
     if (!a.noSync) {

@@ -1326,7 +1326,9 @@ static int symFlag(faabric::device::Communicator& c, const void* a, size_t bytes
 
 bool MpiWorld::deviceReducible(faabric_datatype_t* dt, faabric_op_t* op)
 {
-    return fbDtypeFor(dt) >= 0 && fbOpFor(op) >= 0;
+    const int fdt = fbDtypeFor(dt);
+    const int fop = fbOpFor(op);
+    return fdt >= 0 && fop >= 0 && faabric::device::Communicator::reduces(fdt, fop);
 }
 
 bool MpiWorld::deviceBroadcast(const DeviceComm& comm, int rank, int root, uint8_t* buffer, size_t bytes)
@@ -1535,7 +1537,8 @@ int MpiWorld::iAllReduce(int rank, uint8_t* send, uint8_t* recv, faabric_datatyp
     const int fop = fbOpFor(op);
     cacheDeviceComm(rank);
     const auto& comm = tls.cachedComm;
-    if (bytes > 0 && fdt >= 0 && fop >= 0 && comm != nullptr) {
+    // (a pair the kernels lack must not join a burst: the burst has no host path)
+    if (bytes > 0 && deviceReducible(dt, op) && comm != nullptr) {
         const Placement at = placeCollective(*comm, groupIallreduce, send, bytes, recv, bytes, 0);
         if (at.grouped) {
             // Deferred: the whole burst becomes ONE kernel at the next wait
@@ -1550,10 +1553,12 @@ int MpiWorld::iAllReduce(int rank, uint8_t* send, uint8_t* recv, faabric_datatyp
             return requestId;
         }
         if (at.symmetric || isDevicePointer(send)) {
-            // Symmetric buffers may use any channel; others go through the
-            // single staging area on channel 0
+            // Symmetric, 16-byte aligned buffers may use any channel; others
+            // (the communicator stages an unaligned heap buffer too) go
+            // through the single staging area on channel 0
             const int nChannels = std::clamp(nonBlockingChannels.load(), 1, std::max(1, comm->config().channels));
-            const int channel = at.symmetric ? (int)(tls.deviceCollectiveSeq++ % (uint64_t)nChannels) : 0;
+            const bool anyChannel = at.symmetric && (((uintptr_t)send | (uintptr_t)recv) & 15) == 0;
+            const int channel = anyChannel ? (int)(tls.deviceCollectiveSeq++ % (uint64_t)nChannels) : 0;
             const int flags = (at.symmetric ? FB_FLAG_SYMMETRIC : 0) | FB_FLAG_CHANNEL(channel);
             void* s = streamForRank(rank, channel);
             if (issueDevice(*comm, s, deviceCollectives, [&](auto& c, cudaStream_t st) {
@@ -1587,7 +1592,7 @@ int MpiWorld::iReduceScatter(int rank,
     const auto& comm = tls.cachedComm;
     // In place, the output overwrites input the peers are still reading: that
     // case (send == recv) runs the blocking call below
-    if (shard > 0 && fdt >= 0 && fop >= 0 && comm != nullptr && send != recv) {
+    if (shard > 0 && deviceReducible(dt, op) && comm != nullptr && send != recv) {
         const Placement at = placeCollective(*comm, groupIallreduce, send, shard * size, recv, shard, shard);
         if (at.grouped) {
             deferToGroup(Communicator::GROUP_REDUCE_SCATTER,
@@ -2328,71 +2333,108 @@ void MpiWorld::op_reduce(faabric_op_t* operation,
         fn(inBuffer, resultBuffer, &count, &datatype);
         return;
     }
-    if (op < FAABRIC_OP_MAX || op > FAABRIC_OP_BXOR || op == FAABRIC_OP_NULL) {
-        SPDLOG_ERROR("Reduce operation not implemented: {}", op);
-        throw std::runtime_error("Not yet implemented reduce operation");
+    if (!reducible(datatype, operation)) {
+        SPDLOG_ERROR("Unsupported type/op for reduce: type {} op {}", datatype->id, op);
+        throw std::runtime_error("Unsupported type for reduce");
     }
-    const bool isLoc = op == FAABRIC_OP_MAXLOC || op == FAABRIC_OP_MINLOC;
     switch (datatype->id) {
         case FAABRIC_INT8:
         case FAABRIC_CHAR:
-            if (isLoc) break;
             return reduceInt<int8_t>(op, count, inBuffer, resultBuffer);
         case FAABRIC_UINT8:
         case FAABRIC_BYTE:
         case FAABRIC_C_BOOL:
-            if (isLoc) break;
             return reduceInt<uint8_t>(op, count, inBuffer, resultBuffer);
         case FAABRIC_INT16:
-            if (isLoc) break;
             return reduceInt<int16_t>(op, count, inBuffer, resultBuffer);
         case FAABRIC_UINT16:
-            if (isLoc) break;
             return reduceInt<uint16_t>(op, count, inBuffer, resultBuffer);
         case FAABRIC_INT32:
         case FAABRIC_INT:
-            if (isLoc) break;
             return reduceInt<int32_t>(op, count, inBuffer, resultBuffer);
         case FAABRIC_UINT32:
         case FAABRIC_UINT:
-            if (isLoc) break;
             return reduceInt<uint32_t>(op, count, inBuffer, resultBuffer);
         case FAABRIC_INT64:
         case FAABRIC_LONG:
         case FAABRIC_LONG_LONG:
         case FAABRIC_LONG_LONG_INT:
-            if (isLoc) break;
             return reduceInt<int64_t>(op, count, inBuffer, resultBuffer);
         case FAABRIC_UINT64:
-            if (isLoc) break;
             return reduceInt<uint64_t>(op, count, inBuffer, resultBuffer);
         case FAABRIC_FLOAT:
-            if (isLoc || op == FAABRIC_OP_BAND || op == FAABRIC_OP_BOR || op == FAABRIC_OP_BXOR) break;
             return reduceArith<float>(op, count, inBuffer, resultBuffer);
         case FAABRIC_DOUBLE:
-            if (isLoc || op == FAABRIC_OP_BAND || op == FAABRIC_OP_BOR || op == FAABRIC_OP_BXOR) break;
             return reduceArith<double>(op, count, inBuffer, resultBuffer);
         case FAABRIC_HALF:
             return reduceHalf(op, count, inBuffer, resultBuffer, false);
         case FAABRIC_BFLOAT16:
             return reduceHalf(op, count, inBuffer, resultBuffer, true);
         case FAABRIC_DOUBLE_INT:
-            if (!isLoc) break;
             return reduceLoc<double>(op, count, inBuffer, resultBuffer);
         case FAABRIC_FLOAT_INT:
-            if (!isLoc) break;
             return reduceLoc<float>(op, count, inBuffer, resultBuffer);
         case FAABRIC_2INT:
-            if (!isLoc) break;
             return reduceLoc<int32_t>(op, count, inBuffer, resultBuffer);
-        case FAABRIC_LONG_INT:
-            if (!isLoc) break;
-            return reduceLoc<int64_t>(op, count, inBuffer, resultBuffer);
         default:
-            break;
+            return reduceLoc<int64_t>(op, count, inBuffer, resultBuffer); // FAABRIC_LONG_INT
     }
-    SPDLOG_ERROR("Unsupported type/op for reduce: type {} op {}", datatype->id, op);
-    throw std::runtime_error("Unsupported type for reduce");
+}
+
+bool MpiWorld::reducible(faabric_datatype_t* datatype, faabric_op_t* operation)
+{
+    if (operation == nullptr || datatype == nullptr) {
+        return false;
+    }
+    if (isUserOp(operation)) {
+        return true;
+    }
+    int typeId = datatype->id;
+    if (typeId >= FAABRIC_DERIVED_TYPE_BASE) {
+        int per = 0;
+        if (!getContiguousType(datatype->id, &typeId, &per)) {
+            return false;
+        }
+    }
+    const int op = operation->id;
+    if (op < FAABRIC_OP_MAX || op > FAABRIC_OP_BXOR || op == FAABRIC_OP_NULL) {
+        return false;
+    }
+    const bool isLoc = op == FAABRIC_OP_MAXLOC || op == FAABRIC_OP_MINLOC;
+    const bool isBitwise = op == FAABRIC_OP_BAND || op == FAABRIC_OP_BOR || op == FAABRIC_OP_BXOR;
+    const bool isArith = op == FAABRIC_OP_MAX || op == FAABRIC_OP_MIN || op == FAABRIC_OP_SUM || op == FAABRIC_OP_PROD;
+    switch (typeId) {
+        case FAABRIC_INT8:
+        case FAABRIC_CHAR:
+        case FAABRIC_UINT8:
+        case FAABRIC_BYTE:
+        case FAABRIC_C_BOOL:
+        case FAABRIC_INT16:
+        case FAABRIC_UINT16:
+        case FAABRIC_INT32:
+        case FAABRIC_INT:
+        case FAABRIC_UINT32:
+        case FAABRIC_UINT:
+        case FAABRIC_INT64:
+        case FAABRIC_LONG:
+        case FAABRIC_LONG_LONG:
+        case FAABRIC_LONG_LONG_INT:
+        case FAABRIC_UINT64:
+            return !isLoc;
+        case FAABRIC_FLOAT:
+        case FAABRIC_DOUBLE:
+            return !isLoc && !isBitwise;
+        case FAABRIC_HALF:
+        case FAABRIC_BFLOAT16:
+            return isArith;
+        case FAABRIC_DOUBLE_INT:
+        case FAABRIC_FLOAT_INT:
+        case FAABRIC_2INT:
+        case FAABRIC_LONG_INT:
+            return isLoc;
+        default:
+            return false;
+    }
 }
 
 void MpiWorld::scan(int rank,

@@ -145,11 +145,13 @@ std::map<int, faabric_request_t*>& requestTable()
     return t;
 }
 
-// MPI_REPLACE and MPI_NO_OP only exist for one-sided accumulates.  Collectives
-// refuse them up front, before any rank sends, waits or launches.
-bool accumulateOnlyOp(MPI_Op op)
+// The reductions refuse, before any rank sends, waits or launches, and on
+// every kind of buffer alike: MPI_REPLACE and MPI_NO_OP (they only exist for
+// one-sided accumulates) and a built-in op the datatype does not define
+// (MPI_BAND on a float, MPI_SUM on a pair, MPI_MAXLOC on an integer, ...)
+bool refusedReduction(MPI_Op op, MPI_Datatype datatype)
 {
-    return op != nullptr && (op->id == FAABRIC_OP_REPLACE || op->id == FAABRIC_OP_NO_OP);
+    return !MpiWorld::reducible(datatype, op);
 }
 
 // A datatype as (predefined base type, base elements per element)
@@ -625,7 +627,7 @@ int MPI_Allgatherv(const void* sendbuf, int sendcount, MPI_Datatype sendtype, vo
 int MPI_Reduce(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, int root, MPI_Comm comm)
 {
     SPDLOG_TRACE("MPI - MPI_Reduce all -> {}", root);
-    if (accumulateOnlyOp(op)) {
+    if (refusedReduction(op, datatype)) {
         return MPI_ERR_OP;
     }
     if (auto sub = subOf(comm)) {
@@ -642,7 +644,7 @@ int MPI_Reduce_scatter(const void* sendbuf, void* recvbuf, const int* recvcounts
                        MPI_Op op, MPI_Comm comm)
 {
     SPDLOG_TRACE("MPI - MPI_Reduce_scatter");
-    if (accumulateOnlyOp(op)) {
+    if (refusedReduction(op, datatype)) {
         return MPI_ERR_OP;
     }
     subCommOnly(comm, "MPI_Reduce_scatter");
@@ -687,7 +689,7 @@ int MPI_Reduce_scatter(const void* sendbuf, void* recvbuf, const int* recvcounts
 int MPI_Allreduce(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, MPI_Comm comm)
 {
     SPDLOG_TRACE("MPI - MPI_Allreduce");
-    if (accumulateOnlyOp(op)) {
+    if (refusedReduction(op, datatype)) {
         return MPI_ERR_OP;
     }
     if (auto sub = subOf(comm)) {
@@ -703,7 +705,7 @@ int MPI_Allreduce(const void* sendbuf, void* recvbuf, int count, MPI_Datatype da
 int MPI_Scan(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, MPI_Comm comm)
 {
     SPDLOG_TRACE("MPI - MPI_Scan");
-    if (accumulateOnlyOp(op)) {
+    if (refusedReduction(op, datatype)) {
         return MPI_ERR_OP;
     }
     if (auto sub = subOf(comm)) {
@@ -910,7 +912,7 @@ int MPI_Free_mem(void* base)
 int MPI_Iallreduce(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, MPI_Comm comm, MPI_Request* request)
 {
     SPDLOG_TRACE("MPI - MPI_Iallreduce");
-    if (accumulateOnlyOp(op)) {
+    if (refusedReduction(op, datatype)) {
         return MPI_ERR_OP;
     }
     subCommOnly(comm, "MPI_Iallreduce");
@@ -930,7 +932,7 @@ int MPI_Reduce_scatter_block(const void* sendbuf, void* recvbuf, int recvcount, 
                              MPI_Op op, MPI_Comm comm)
 {
     SPDLOG_TRACE("MPI - MPI_Reduce_scatter_block");
-    if (accumulateOnlyOp(op)) {
+    if (refusedReduction(op, datatype)) {
         return MPI_ERR_OP;
     }
     subCommOnly(comm, "MPI_Reduce_scatter_block");
@@ -943,7 +945,7 @@ int MPI_Ireduce_scatter_block(const void* sendbuf, void* recvbuf, int recvcount,
                               MPI_Op op, MPI_Comm comm, MPI_Request* request)
 {
     SPDLOG_TRACE("MPI - MPI_Ireduce_scatter_block");
-    if (accumulateOnlyOp(op)) {
+    if (refusedReduction(op, datatype)) {
         return MPI_ERR_OP;
     }
     subCommOnly(comm, "MPI_Ireduce_scatter_block");

@@ -301,6 +301,10 @@ class Communicator:
 
     # ------------------------------------------------------------ collectives
     def all_reduce(self, send, recv=None, op="sum", algo="auto", stream=None, flags=None, channel=0, dtype=None):
+        """All-reduce ``send`` into ``recv`` (in place when ``recv`` is None).
+        Heap tensors take the symmetric path at any heap offset, the same on
+        every rank; offsets not a multiple of 16 are staged.  So do
+        :meth:`reduce`, :meth:`reduce_scatter` and :meth:`scan`."""
         recv = send if recv is None else recv
         count, dt = self._typed(send, dtype)
         # only the source needs to be symmetric; the native side stages the
