@@ -25,6 +25,7 @@
 
 #include "../tests/mpi_rma_atomics_body.h"
 #include "../tests/mpi_rma_passive_body.h"
+#include "../tests/mpi_rma_accumulate_batch_body.h"
 #include "../tests/mpi_rma_request_body.h"
 #include "../tests/mpi_subcomm_device_body.h"
 
@@ -781,6 +782,21 @@ static void registerFunctions()
         return rc;
     });
 
+    // MPI_Raccumulate / MPI_Rget_accumulate deferred into the request batch
+    // of a symmetric-heap window (mpi_rma_accumulate_batch_body.h).  Input:
+    // "device" for origin and result buffers in cudaMalloc memory, otherwise
+    // in the origin's symmetric heap.
+    mpiFunction("rma-accumulate-batch", [](int rank, int size, faabric::Message& msg) {
+        const auto origin = msg.inputdata().rfind("device", 0) == 0 ? rma_request::Origin::Device : rma_request::Origin::Heap;
+        std::string why;
+        int rc = rma_acc_batch::body(rank, size, msg.mpiworldid(), origin, &why);
+        if (rc != 0) {
+            SPDLOG_ERROR("rma-accumulate-batch: {}", why);
+            msg.set_outputdata(why);
+        }
+        return rc;
+    });
+
     // Fused device collectives on sub-communicators (mpi_subcomm_device_body.h).
     // Input: "heap" (symmetric heap buffers) or "cuda" (cudaMalloc buffers).
     mpiFunction("subcomm-device", [](int rank, int size, faabric::Message& msg) {
@@ -1124,6 +1140,94 @@ static void registerFunctions()
             EXPECT(std::all_of(got.begin(), got.end(), [](uint8_t b) { return b == 1; }));
         }
         cudaFree(src);
+        MPI_Free_mem(window);
+        return 0;
+    });
+
+    // Cost of request-based accumulates against plain ones: rank 0 applies K
+    // int64 SUM operations from device memory to rank 1's symmetric-heap
+    // window inside MPI_Win_lock_all, then completes them.  Input
+    // "mode;pattern;K;iters":
+    //   racc  MPI_Raccumulate / MPI_Rget_accumulate x K + MPI_Waitall + MPI_Win_flush
+    //   acc   MPI_Accumulate / MPI_Get_accumulate x K + MPI_Win_flush
+    //   updates: +1 to counter k of K; tickets: a fetching +1 of one counter
+    // Rank 0 reports {"us_per_op"}; rank 1 checks the counters.
+    mpiFunction("bench-rma-raccumulate", [](int rank, int size, faabric::Message& msg) {
+        std::vector<std::string> f;
+        std::string cur;
+        for (char c : msg.inputdata() + ";") {
+            if (c == ';') {
+                f.push_back(cur);
+                cur.clear();
+            } else {
+                cur += c;
+            }
+        }
+        EXPECT(f.size() >= 4 && size >= 2);
+        const bool racc = f[0] == "racc";
+        const bool tickets = f[1] == "tickets";
+        const int K = std::stoi(f[2]);
+        const int iters = std::stoi(f[3]);
+        EXPECT(K > 0 && K <= (1 << 20) && iters > 0);
+        const size_t winBytes = 8 * (size_t)K;
+        uint8_t* window = nullptr;
+        EXPECT(MPI_Alloc_mem(winBytes, MPI_INFO_FAABRIC_DEVICE, &window) == MPI_SUCCESS);
+        int64_t* buf = nullptr; // [0]: the operand 1; [1 + k]: fetched values
+        EXPECT(cudaMalloc((void**)&buf, 8 * ((size_t)K + 1)) == cudaSuccess);
+        const int64_t one = 1;
+        cudaMemcpy(buf, &one, 8, cudaMemcpyHostToDevice);
+        cudaMemset(window, 0, winBytes);
+        cudaDeviceSynchronize();
+        MPI_Win win = nullptr;
+        MPI_Win_create(window, winBytes, 1, MPI_INFO_NULL, MPI_COMM_WORLD, &win);
+        std::vector<MPI_Request> reqs(K, nullptr);
+        auto step = [&]() {
+            for (int k = 0; k < K; k++) {
+                const MPI_Aint disp = tickets ? 0 : 8 * (MPI_Aint)k;
+                int64_t* res = buf + 1 + k;
+                int rc = tickets ? (racc ? MPI_Rget_accumulate(buf, 1, MPI_INT64_T, res, 1, MPI_INT64_T, 1, disp, 1, MPI_INT64_T,
+                                                               MPI_SUM, win, &reqs[k])
+                                         : MPI_Get_accumulate(buf, 1, MPI_INT64_T, res, 1, MPI_INT64_T, 1, disp, 1, MPI_INT64_T,
+                                                              MPI_SUM, win))
+                                 : (racc ? MPI_Raccumulate(buf, 1, MPI_INT64_T, 1, disp, 1, MPI_INT64_T, MPI_SUM, win, &reqs[k])
+                                         : MPI_Accumulate(buf, 1, MPI_INT64_T, 1, disp, 1, MPI_INT64_T, MPI_SUM, win));
+                if (rc != MPI_SUCCESS) {
+                    return rc;
+                }
+            }
+            if (racc) {
+                int rc = MPI_Waitall(K, reqs.data(), MPI_STATUSES_IGNORE);
+                if (rc != MPI_SUCCESS) {
+                    return rc;
+                }
+            }
+            return MPI_Win_flush(1, win);
+        };
+        const int warm = 3;
+        if (rank == 0) {
+            EXPECT(MPI_Win_lock_all(0, win) == MPI_SUCCESS);
+            for (int i = 0; i < warm; i++) {
+                EXPECT(step() == MPI_SUCCESS);
+            }
+            auto t0 = std::chrono::steady_clock::now();
+            for (int i = 0; i < iters; i++) {
+                EXPECT(step() == MPI_SUCCESS);
+            }
+            double us =
+              std::chrono::duration<double, std::micro>(std::chrono::steady_clock::now() - t0).count() / ((double)iters * K);
+            EXPECT(MPI_Win_unlock_all(win) == MPI_SUCCESS);
+            msg.set_outputdata("{\"us_per_op\": " + std::to_string(us) + "}");
+        }
+        MPI_Win_free(&win);
+        if (rank == 1) {
+            std::vector<int64_t> got(K);
+            cudaMemcpy(got.data(), window, winBytes, cudaMemcpyDeviceToHost);
+            const int64_t calls = warm + iters;
+            for (int k = 0; k < (tickets ? 1 : K); k++) {
+                EXPECT(got[k] == (tickets ? calls * K : calls));
+            }
+        }
+        cudaFree(buf);
         MPI_Free_mem(window);
         return 0;
     });

@@ -786,6 +786,32 @@ int fb_put_get_many(void* h,
     FB_CATCH(FB_E_CUDA)
 }
 
+// Batched one-sided atomics (Communicator::accumulateMany): item i combines
+// count[i] elements of origin[i] into peer[i]'s symmetric heap at offset[i];
+// fetch[i] null means no fetch; `fetch` itself may be null (no item fetches)
+int fb_accumulate_many(void* h,
+                       int n,
+                       const void* const* origin,
+                       void* const* fetch,
+                       const uint64_t* offset,
+                       const uint64_t* count,
+                       const int32_t* peer,
+                       int dtype,
+                       int op,
+                       void* stream)
+{
+    if (n < 0 || (n > 0 && (origin == nullptr || offset == nullptr || count == nullptr || peer == nullptr))) {
+        return FB_E_INVALID;
+    }
+    FB_TRY
+    std::vector<Communicator::RmaAccumulate> items(n);
+    for (int i = 0; i < n; i++) {
+        items[i] = Communicator::RmaAccumulate{ origin[i], fetch != nullptr ? fetch[i] : nullptr, offset[i], (size_t)count[i], peer[i] };
+    }
+    return COMM(h)->accumulateMany(items.data(), items.size(), dtype, op, (cudaStream_t)stream);
+    FB_CATCH(FB_E_CUDA)
+}
+
 const char* fb_error_string(int code)
 {
     return Communicator::errorString(code);

@@ -401,6 +401,38 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     // Destinations that overlap within one list (or a destination that
     // overlaps a source) leave unspecified bytes there.
     int putGetMany(const RmaCopy* items, size_t n, cudaStream_t s);
+    // ---- batched one-sided atomics (request-based MPI_Raccumulate /
+    // MPI_Rget_accumulate) ----
+    struct RmaAccumulate
+    {
+        const void* origin; // count elements (may be null for FB_OP_NO_OP)
+        void* fetch;        // previous values, or null (no fetch)
+        uint64_t offset;    // user part of peer's symmetric heap
+        size_t count;
+        int peer;
+    };
+    // Every item as accumulate() of (dtype, op) would apply it, in list order
+    // where the targets of two items intersect (same peer, intersecting
+    // bytes), and atomically element by element with respect to every other
+    // accumulate on any rank.  Stream-ordered, never synchronises the host.
+    // Every item is checked before anything is launched, by the rules and
+    // codes of accumulate(); zero-count items are skipped (only their peer is
+    // checked); a sub-communicator gives FB_E_UNSUPPORTED.
+    //
+    // Launches, in list order (each counted in stats().launches): a launch
+    // takes the next item unless that item would
+    //  * be its FB_RMA_ACC_MAX_ITEMS + 1-th descriptor (an item longer than
+    //    FB_RMA_ACC_MAX_COUNT elements is that many descriptors),
+    //  * intersect items of two different chains of the launch (a chain: the
+    //    items of the launch connected by intersecting targets), or
+    //  * bring the target bytes of its chain above FB_RMA_ACC_CHAIN_BYTES, or
+    //  * bring the launch's chunk space (one chunk per chain, plus
+    //    fbRmaAccChunks(count) per item) to 2^32 chunks, which takes more
+    //    than 2^39 elements in one launch, far beyond any heap,
+    // in which case it starts the next launch.  So K fetching increments of
+    // one counter are one launch for K <= 1024, and their fetched values are
+    // the counter's successive values in list order.
+    int accumulateMany(const RmaAccumulate* items, size_t n, int dtype, int op, cudaStream_t s);
 
     // Device watchdog error word (FB_ERR_*); synchronises `s`
     uint32_t checkError(cudaStream_t s);
@@ -468,13 +500,19 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     bool streamWriteOk_ = false;
     cudaStream_t internalStream_ = nullptr;
     uint32_t doneSeq_ = 0;
-    // transient group tables (allReduceMany) and copy tables (putGetMany)
+    // transient group tables (allReduceMany) and copy and accumulate tables
+    // (putGetMany, accumulateMany)
     struct ManySlot;
     std::vector<std::shared_ptr<ManySlot>> manySlots_;
     size_t manyNext_ = 0;
     // The next table slot, free for the host to write (waits for the launch
     // that used it last); null on a CUDA error
     ManySlot* nextManySlot();
+    // The table of one batched launch where the kernel reads it: a slot's
+    // device copy (*slot set; pass it to releaseManySlot after the launch),
+    // or `table` itself on the loopback backend.  Null on a CUDA error.
+    const void* stageManyTable(const void* table, size_t bytes, cudaStream_t s, ManySlot** slot);
+    void releaseManySlot(ManySlot* slot, cudaStream_t s);
     uint64_t stageSendOff_ = 0;
     uint64_t stageRecvOff_ = 0;
     uint64_t userOff_ = 0;

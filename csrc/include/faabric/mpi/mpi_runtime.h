@@ -461,11 +461,16 @@ class MpiWorld
     // MPI_ERR_RMA_SYNC (the target is not covered by a passive epoch of
     // `rank`).  On success *requestId is a request of this rank thread,
     // completed by awaitAsyncRequest.
-    //   symmetric heap in this process, origin on the origin's GPU (or in
-    //   its heap): deferred into the origin's batch for the window, issued
-    //   as one Communicator::putGetMany at the wait, flush or unlock (or
-    //   when the batch holds a launch's worth)
-    //   other segments in this process: winPut / winGet at issue
+    //   symmetric heap in this process, origin (and result) on the
+    //   origin's GPU (or in its heap): deferred into the origin's batch for
+    //   the window, in issue order, and issued at the wait, flush or unlock
+    //   (or when the batch holds FB_RMA_COPY_MAX_ITEMS entries): each run of
+    //   copies as one Communicator::putGetMany, each run of accumulates of
+    //   one (dtype, op) as one Communicator::accumulateMany.  Any other
+    //   accumulate-family call of the origin on the window issues the batch
+    //   first, so one origin's accumulates apply in issue order.
+    //   other segments in this process: winPut / winGet / winAccumulate at
+    //   issue
     //   rank in another worker process: queued like MPI_Put, shipped at the
     //   flush or unlock of the target, or at the wait
     int winRputGet(int rank, int winId, uint8_t* origin, size_t bytes, int targetRank, int64_t targetDisp, bool get, int* requestId);
@@ -638,6 +643,15 @@ class MpiWorld
         // puts / gets of this epoch went through cudaMemcpy
         bool deviceCopies = false;
     };
+    // One deferred request-based operation on the symmetric heap: a copy
+    // (dtype < 0) or an accumulate of (dtype, op)
+    struct RmaBatchItem
+    {
+        faabric::device::Communicator::RmaCopy copy;
+        faabric::device::Communicator::RmaAccumulate acc;
+        int dtype = -1;
+        int op = -1;
+    };
     struct RmaWindow
     {
         std::mutex mx;
@@ -659,8 +673,9 @@ class MpiWorld
         std::condition_variable lockCv;
         std::vector<RmaLock> locks;
         // request-based operations, one entry per ORIGIN rank (only that
-        // rank's thread): deferred heap copies, and completion sequences
-        std::vector<std::vector<faabric::device::Communicator::RmaCopy>> batches;
+        // rank's thread): deferred heap copies and accumulates in issue
+        // order, and completion sequences
+        std::vector<std::vector<RmaBatchItem>> batches;
         std::vector<std::shared_ptr<RmaProgress>> progress;
     };
     std::mutex windowsMx;
@@ -697,9 +712,26 @@ class MpiWorld
     int rmaAcquire(RmaWindow& w, int winId, int rank, int targetRank, bool exclusive);
     // Completes `rank`'s operations to `targetRank`; `release` also unlocks
     int rmaComplete(RmaWindow& w, int winId, int rank, int targetRank, bool release);
-    // Issues `rank`'s deferred heap copies on the window (its stream joins
-    // the window's streams of `rank`)
+    // Issues `rank`'s deferred heap copies and accumulates on the window, in
+    // issue order (its stream joins the window's streams of `rank`)
     void rmaIssueBatch(RmaWindow& w, int rank);
+    // Whether an operation of `rank` on `bytes` at `target` (a segment of
+    // `targetRank` in this process), with origin / result buffers `buf` and
+    // `buf2` (each may be null), can join the batch
+    bool rmaBatchable(int rank, int targetRank, const uint8_t* target, size_t bytes, const uint8_t* buf, const uint8_t* buf2);
+    // The checks of winAccumulate: MPI_SUCCESS with the FbDtype, FbOp and
+    // target address (in the target's address space), or an MPI error code
+    int rmaAccumulateArgs(RmaWindow& w,
+                          const uint8_t* origin,
+                          size_t count,
+                          faabric_datatype_t* datatype,
+                          faabric_op_t* op,
+                          uint8_t* result,
+                          int targetRank,
+                          int64_t targetDisp,
+                          int* dtype,
+                          int* fop,
+                          uint8_t** target);
     // Checks and numbering shared by the request-based calls: MPI_SUCCESS
     // and the target address, or an MPI error code
     int rmaRequestTarget(RmaWindow& w, int rank, int targetRank, int64_t targetDisp, size_t bytes, uint8_t** target);

@@ -287,6 +287,55 @@ struct RmaCopyArgs
 
 cudaError_t launchRmaCopyMany(const RmaCopyArgs& a, cudaStream_t s);
 
+// Batched accumulate (rmaAccumulateManyKernel): a table of accumulates of one
+// (dtype, op), each with the element rule of launchRmaAccumulate.  `target`
+// is an address the launching GPU can reach (its own heap, or a peer's heap
+// through FbCommDev::heap[peer]), aligned to the element size; `fetch` is
+// null for an item without fetch (never for NO_OP).
+//
+// Items whose targets intersect must apply in list order, which warps of a
+// grid do not give.  So the host lays the table out as `nChains` chains
+// first, then the free items:
+//  * a chain is a run of consecutive descriptors with the same chunk0 (chain
+//    c has chunk0 == c, c < nChains); one warp applies its items one after the
+//    other, in table order;
+//  * a free item owns the chunks [chunk0, chunk0 + fbRmaAccChunks(count)),
+//    FB_RMA_ACC_CHUNK elements each, spread over the warps of the grid.
+// The launch is complete when the stream passes the kernel.  Unlike
+// launchRmaAccumulate, f16 / bf16 SUM items without fetch take the per-element
+// CAS rule, not 8-wide packed adds: the same results, at a lower rate for
+// large half-precision items (a large one is better issued on its own).
+struct RmaAccDesc
+{
+    const uint8_t* origin;
+    uint8_t* fetch;
+    uint8_t* target;
+    uint32_t count;  // elements
+    uint32_t chunk0; // first chunk (free item), or the chain's chunk
+};
+#define FB_RMA_ACC_MAX_ITEMS FB_GROUP_MAX_SEGS
+#define FB_RMA_ACC_CHUNK 128 // elements per warp-chunk of a free item
+// Largest element count of one descriptor; the host splits longer items
+#define FB_RMA_ACC_MAX_COUNT ((uint32_t)1 << 30)
+// Largest sum of the target bytes of one chain (see Communicator::accumulateMany)
+#define FB_RMA_ACC_CHAIN_BYTES 16384
+static inline uint64_t fbRmaAccChunks(uint64_t count)
+{
+    return (count + FB_RMA_ACC_CHUNK - 1) / FB_RMA_ACC_CHUNK;
+}
+
+struct RmaAccManyArgs
+{
+    const RmaAccDesc* items; // device memory of the launching GPU
+    uint32_t nItems;
+    uint32_t nChainItems; // items [0, nChainItems) belong to chains
+    uint32_t nChains;
+    uint32_t totalChunks; // nChains + the chunks of the free items
+};
+
+// rmaSupported(dtype, op, true) pairs; NO_OP needs a fetch on every item
+cudaError_t launchRmaAccumulateMany(const RmaAccManyArgs& a, int dtype, int op, cudaStream_t s);
+
 
 // ------------------------------------------------------------------ nvls ----
 enum NvlsMode

@@ -22,6 +22,10 @@
 //
 //  * rmaCopyManyKernel — a table of plain copies (request-based puts and gets
 //    on the symmetric heap): one launch for a whole list, any alignment.
+//  * rmaAccumulateManyKernel<DT, OP> — a table of accumulates of one (dtype,
+//    op), with or without fetch per item (MPI_Raccumulate and
+//    MPI_Rget_accumulate bursts): the element rule of rmaAccumulateKernel,
+//    overlapping items applied in list order by one warp (launch_api.h).
 #include "fb_atomics.cuh"
 #include "fb_prims.cuh"
 #include "launch_api.h"
@@ -480,61 +484,159 @@ cudaError_t launchRmaCopyMany(const RmaCopyArgs& a, cudaStream_t s)
     return cudaLaunchKernel((const void*)rmaCopyManyKernel, dim3(blocks), dim3(RMA_COPY_THREADS), args, 0, s);
 }
 
-// ------------------------------------------------------------- dispatch ----
-template<int DT, int OP, bool FETCH>
-static const void* kernelOrNull()
+// ------------------------------------------------------ batched accumulate ----
+// Elements [lo, hi) of one item, by the 32 lanes of a warp: the element rule
+// of rmaAccumulateKernel, with a fetch when the item has a fetch buffer
+template<int DT, int OP>
+__device__ __forceinline__ void accumulateItemRange(const RmaAccDesc& it, uint32_t lo, uint32_t hi, uint32_t lane)
 {
-    if constexpr (rmaOk(DT, OP, FETCH)) {
-        return (const void*)rmaAccumulateKernel<DT, OP, FETCH>;
-    } else {
-        return nullptr;
+    using E = RmaElem<DT>;
+    const bool originAligned = ((uintptr_t)it.origin % sizeof(E)) == 0;
+    const bool fetchAligned = ((uintptr_t)it.fetch % sizeof(E)) == 0;
+    for (uint32_t i = lo + lane; i < hi; i += 32) {
+        E v{};
+        if constexpr (OP != FB_OP_NO_OP) {
+            const uint8_t* o = it.origin + (uint64_t)i * sizeof(E);
+            v = originAligned ? *reinterpret_cast<const E*>(o) : ldBytes<E>(o);
+        }
+        uint8_t* t = it.target + (uint64_t)i * sizeof(E);
+        if constexpr (OP != FB_OP_NO_OP) {
+            if (it.fetch == nullptr) {
+                rmaApply<DT, OP, false>(t, v);
+                continue;
+            }
+        }
+        const E old = rmaApply<DT, OP, true>(t, v);
+        uint8_t* r = it.fetch + (uint64_t)i * sizeof(E);
+        if (fetchAligned) {
+            *reinterpret_cast<E*>(r) = old;
+        } else {
+            stBytes<E>(r, old);
+        }
     }
 }
 
-template<int DT, bool FETCH>
+// One warp per chunk.  Chunk c < nChains is chain c: its items (consecutive
+// descriptors with chunk0 == c) apply one after the other, so overlapping
+// items of one list land in list order, in the target and in the fetched
+// values.  Any other chunk is FB_RMA_ACC_CHUNK elements of one free item.
+template<int DT, int OP>
+__global__ void __launch_bounds__(RMA_THREADS) rmaAccumulateManyKernel(const RmaAccManyArgs a)
+{
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const uint32_t nWarps = (gridDim.x * blockDim.x) >> 5;
+    for (uint32_t ch = warp; ch < a.totalChunks; ch += nWarps) {
+        if (ch < a.nChains) {
+            // the chain's first item: the first chunk0 >= ch among the chains
+            uint32_t lo = 0;
+            uint32_t hi = a.nChainItems;
+            while (lo < hi) {
+                const uint32_t mid = (lo + hi) >> 1;
+                if (a.items[mid].chunk0 < ch) {
+                    lo = mid + 1;
+                } else {
+                    hi = mid;
+                }
+            }
+            for (uint32_t i = lo; i < a.nChainItems && a.items[i].chunk0 == ch; i++) {
+                const RmaAccDesc it = a.items[i];
+                accumulateItemRange<DT, OP>(it, 0, it.count, lane);
+                // the next item's updates of these elements come after these
+                __syncwarp();
+            }
+        } else {
+            // the free item that owns the chunk: the last chunk0 <= ch
+            uint32_t lo = a.nChainItems;
+            uint32_t hi = a.nItems - 1;
+            while (lo < hi) {
+                const uint32_t mid = (lo + hi + 1) >> 1;
+                if (a.items[mid].chunk0 <= ch) {
+                    lo = mid;
+                } else {
+                    hi = mid - 1;
+                }
+            }
+            const RmaAccDesc it = a.items[lo];
+            const uint32_t first = (ch - it.chunk0) * FB_RMA_ACC_CHUNK;
+            accumulateItemRange<DT, OP>(it, first, min(it.count, first + FB_RMA_ACC_CHUNK), lane);
+        }
+    }
+}
+
+// ------------------------------------------------------------- dispatch ----
+// The kernel of one (DT, OP, FETCH), or null where the pair is unsupported
+struct AccumulateKernels
+{
+    template<int DT, int OP, bool FETCH>
+    static const void* get()
+    {
+        if constexpr (rmaOk(DT, OP, FETCH)) {
+            return (const void*)rmaAccumulateKernel<DT, OP, FETCH>;
+        } else {
+            return nullptr;
+        }
+    }
+};
+
+// (one batched kernel per pair: fetching and plain items share a launch)
+struct AccumulateManyKernels
+{
+    template<int DT, int OP, bool>
+    static const void* get()
+    {
+        if constexpr (rmaOk(DT, OP, true)) {
+            return (const void*)rmaAccumulateManyKernel<DT, OP>;
+        } else {
+            return nullptr;
+        }
+    }
+};
+
+template<typename K, int DT, bool FETCH>
 static const void* byOp(int op)
 {
     switch (op) {
         case FB_OP_MAX:
-            return kernelOrNull<DT, FB_OP_MAX, FETCH>();
+            return K::template get<DT, FB_OP_MAX, FETCH>();
         case FB_OP_MIN:
-            return kernelOrNull<DT, FB_OP_MIN, FETCH>();
+            return K::template get<DT, FB_OP_MIN, FETCH>();
         case FB_OP_SUM:
-            return kernelOrNull<DT, FB_OP_SUM, FETCH>();
+            return K::template get<DT, FB_OP_SUM, FETCH>();
         case FB_OP_PROD:
-            return kernelOrNull<DT, FB_OP_PROD, FETCH>();
+            return K::template get<DT, FB_OP_PROD, FETCH>();
         case FB_OP_LAND:
-            return kernelOrNull<DT, FB_OP_LAND, FETCH>();
+            return K::template get<DT, FB_OP_LAND, FETCH>();
         case FB_OP_LOR:
-            return kernelOrNull<DT, FB_OP_LOR, FETCH>();
+            return K::template get<DT, FB_OP_LOR, FETCH>();
         case FB_OP_BAND:
-            return kernelOrNull<DT, FB_OP_BAND, FETCH>();
+            return K::template get<DT, FB_OP_BAND, FETCH>();
         case FB_OP_BOR:
-            return kernelOrNull<DT, FB_OP_BOR, FETCH>();
+            return K::template get<DT, FB_OP_BOR, FETCH>();
         case FB_OP_MAXLOC:
-            return kernelOrNull<DT, FB_OP_MAXLOC, FETCH>();
+            return K::template get<DT, FB_OP_MAXLOC, FETCH>();
         case FB_OP_MINLOC:
-            return kernelOrNull<DT, FB_OP_MINLOC, FETCH>();
+            return K::template get<DT, FB_OP_MINLOC, FETCH>();
         case FB_OP_LXOR:
-            return kernelOrNull<DT, FB_OP_LXOR, FETCH>();
+            return K::template get<DT, FB_OP_LXOR, FETCH>();
         case FB_OP_BXOR:
-            return kernelOrNull<DT, FB_OP_BXOR, FETCH>();
+            return K::template get<DT, FB_OP_BXOR, FETCH>();
         case FB_OP_REPLACE:
-            return kernelOrNull<DT, FB_OP_REPLACE, FETCH>();
+            return K::template get<DT, FB_OP_REPLACE, FETCH>();
         case FB_OP_NO_OP:
-            return kernelOrNull<DT, FB_OP_NO_OP, FETCH>();
+            return K::template get<DT, FB_OP_NO_OP, FETCH>();
         default:
             return nullptr;
     }
 }
 
-template<bool FETCH>
+template<typename K, bool FETCH>
 static const void* byDtype(int dtype, int op)
 {
     switch (dtype) {
 #define FB_RMA_DT(dt)                                                          \
     case dt:                                                                   \
-        return byOp<dt, FETCH>(op);
+        return byOp<K, dt, FETCH>(op);
         FB_RMA_DT(FB_I8)
         FB_RMA_DT(FB_U8)
         FB_RMA_DT(FB_I16)
@@ -559,7 +661,12 @@ static const void* byDtype(int dtype, int op)
 
 static const void* accumulateKernel(int dtype, int op, bool fetch)
 {
-    return fetch ? byDtype<true>(dtype, op) : byDtype<false>(dtype, op);
+    return fetch ? byDtype<AccumulateKernels, true>(dtype, op) : byDtype<AccumulateKernels, false>(dtype, op);
+}
+
+static const void* accumulateManyKernel(int dtype, int op)
+{
+    return byDtype<AccumulateManyKernels, true>(dtype, op);
 }
 
 static const void* casKernel(int dtype)
@@ -608,6 +715,22 @@ cudaError_t launchRmaAccumulate(const RmaArgs& a, int dtype, int op, cudaStream_
     return cudaLaunchKernel(k, dim3(blocks), dim3(RMA_THREADS), args, 0, s);
 }
 
+cudaError_t launchRmaAccumulateMany(const RmaAccManyArgs& a, int dtype, int op, cudaStream_t s)
+{
+    const void* k = accumulateManyKernel(dtype, op);
+    if (k == nullptr) {
+        return cudaErrorInvalidValue;
+    }
+    if (a.nItems == 0 || a.totalChunks == 0) {
+        return cudaSuccess;
+    }
+    constexpr uint32_t warpsPerBlock = RMA_THREADS / 32;
+    const uint32_t want = (a.totalChunks + warpsPerBlock - 1) / warpsPerBlock;
+    const unsigned blocks = want > RMA_MAX_BLOCKS ? RMA_MAX_BLOCKS : want;
+    void* args[] = { const_cast<RmaAccManyArgs*>(&a) };
+    return cudaLaunchKernel(k, dim3(blocks), dim3(RMA_THREADS), args, 0, s);
+}
+
 cudaError_t launchRmaCompareSwap(const RmaCasArgs& a, int dtype, cudaStream_t s)
 {
     const void* k = casKernel(dtype);
@@ -629,6 +752,10 @@ cudaError_t preloadRmaKernels()
                 if (k != nullptr) {
                     e = cudaFuncGetAttributes(&attr, k);
                 }
+            }
+            const void* many = accumulateManyKernel(dt, op);
+            if (e == cudaSuccess && many != nullptr) {
+                e = cudaFuncGetAttributes(&attr, many);
             }
         }
         if (e == cudaSuccess && casKernel(dt) != nullptr) {

@@ -11,6 +11,7 @@
 #include <thread>
 #include <cstdio>
 #include <initializer_list>
+#include <map>
 #include <barrier>
 #include <cstdlib>
 #include <cstring>
@@ -1245,6 +1246,7 @@ const fb::KernelTable CUDA_KERNELS = {
     .rmaAccumulate = fb::launchRmaAccumulate,
     .rmaCompareSwap = fb::launchRmaCompareSwap,
     .rmaCopyMany = fb::launchRmaCopyMany,
+    .rmaAccumulateMany = fb::launchRmaAccumulateMany,
     .copy = cudaCopy,
     .copy2D = cudaCopy2D,
 };
@@ -1267,6 +1269,7 @@ const fb::KernelTable HOST_KERNELS = {
     .rmaAccumulate = fb::host::rmaAccumulate,
     .rmaCompareSwap = fb::host::rmaCompareSwap,
     .rmaCopyMany = fb::host::rmaCopyMany,
+    .rmaAccumulateMany = fb::host::rmaAccumulateMany,
     .copy = fb::host::copy,
     .copy2D = fb::host::copy2D,
 };
@@ -3137,33 +3140,209 @@ int Communicator::putGetMany(const RmaCopy* items, size_t n, cudaStream_t s)
         }
         fb::RmaCopyArgs a;
         memset(&a, 0, sizeof(a));
-        a.items = table.data(); // the host twin reads the table in place
         a.nItems = (uint32_t)table.size();
         a.totalChunks = chunks;
         ManySlot* slot = nullptr;
-        if (!loop_) {
-            slot = nextManySlot();
-            if (slot == nullptr) {
-                return FB_E_CUDA;
-            }
-            const size_t tableBytes = table.size() * sizeof(fb::RmaCopyDesc);
-            memcpy(slot->hSegs, table.data(), tableBytes);
-            if (cudaMemcpyAsync(slot->dSegs, slot->hSegs, tableBytes, cudaMemcpyHostToDevice, s) != cudaSuccess) {
-                return FB_E_CUDA;
-            }
-            a.items = reinterpret_cast<const fb::RmaCopyDesc*>(slot->dSegs);
+        a.items = (const fb::RmaCopyDesc*)stageManyTable(table.data(), table.size() * sizeof(fb::RmaCopyDesc), s, &slot);
+        if (a.items == nullptr) {
+            return FB_E_CUDA;
         }
         stats_.launches++;
         stats_.bytes += bytes;
         if (k_->rmaCopyMany(a, s) != cudaSuccess) {
             return FB_E_CUDA;
         }
-        if (slot != nullptr) {
-            cudaEventRecord(slot->ev, s);
-            slot->used = true;
-        }
+        releaseManySlot(slot, s);
     }
     return FB_OK;
+}
+
+const void* Communicator::stageManyTable(const void* table, size_t bytes, cudaStream_t s, ManySlot** slot)
+{
+    *slot = nullptr;
+    if (loop_) {
+        return table; // the host twins read the table in place
+    }
+    ManySlot* sl = nextManySlot();
+    if (sl == nullptr) {
+        return nullptr;
+    }
+    memcpy(sl->hSegs, table, bytes);
+    if (cudaMemcpyAsync(sl->dSegs, sl->hSegs, bytes, cudaMemcpyHostToDevice, s) != cudaSuccess) {
+        return nullptr;
+    }
+    *slot = sl;
+    return sl->dSegs;
+}
+
+void Communicator::releaseManySlot(ManySlot* slot, cudaStream_t s)
+{
+    if (slot != nullptr) {
+        cudaEventRecord(slot->ev, s);
+        slot->used = true;
+    }
+}
+
+static_assert(sizeof(fb::RmaAccDesc) == sizeof(fb::GroupSeg) && FB_RMA_ACC_MAX_ITEMS == FB_GROUP_MAX_SEGS,
+              "accumulate tables share the group tables' staging slots");
+
+namespace {
+// One launch of accumulateMany being filled, in list order.  Items connected
+// by intersecting targets form a chain; `spans` holds each chain's byte range
+// (the union of its items' ranges, which intersect) by (peer, first byte).
+struct AccLaunch
+{
+    std::vector<std::vector<fb::RmaAccDesc>> chains;
+    std::vector<uint64_t> chainBytes;
+    std::map<std::pair<int, uint64_t>, std::pair<uint64_t, size_t>> spans; // -> (end, chain)
+    size_t items = 0;
+    uint64_t chunks = 0; // an upper bound of the launch's chunk space
+
+    // Adds [off, off + bytes) of peer; false if the item starts the next launch
+    bool add(const fb::RmaAccDesc& d, int peer, uint64_t off, uint64_t bytes)
+    {
+        const uint64_t end = off + bytes;
+        auto it = spans.upper_bound({ peer, off });
+        if (it != spans.begin() && std::prev(it)->first.first == peer && std::prev(it)->second.first > off) {
+            --it;
+        }
+        auto last = it;
+        size_t chain = SIZE_MAX;
+        for (; last != spans.end() && last->first.first == peer && last->first.second < end; ++last) {
+            if (chain != SIZE_MAX && last->second.second != chain) {
+                return false; // joins two chains
+            }
+            chain = last->second.second;
+        }
+        const uint64_t need = chunks + fb::fbRmaAccChunks(d.count) + 1;
+        if (items == FB_RMA_ACC_MAX_ITEMS || need > UINT32_MAX ||
+            (chain != SIZE_MAX && chainBytes[chain] + bytes > FB_RMA_ACC_CHAIN_BYTES)) {
+            return false;
+        }
+        uint64_t lo = off;
+        uint64_t hi = end;
+        if (chain == SIZE_MAX) {
+            chain = chains.size();
+            chains.emplace_back();
+            chainBytes.push_back(0);
+        } else {
+            lo = std::min(lo, it->first.second);
+            hi = std::max(hi, std::prev(last)->second.first);
+            spans.erase(it, last);
+        }
+        spans[{ peer, lo }] = { hi, chain };
+        chains[chain].push_back(d);
+        chainBytes[chain] += bytes;
+        items++;
+        chunks = need;
+        return true;
+    }
+
+    // The table: chains of two or more items first (chain c's items carry
+    // chunk0 = c), then the single items with their chunk ranges
+    fb::RmaAccManyArgs layout(std::vector<fb::RmaAccDesc>& table) const
+    {
+        fb::RmaAccManyArgs a;
+        memset(&a, 0, sizeof(a));
+        table.clear();
+        for (const auto& c : chains) {
+            if (c.size() > 1) {
+                for (fb::RmaAccDesc d : c) {
+                    d.chunk0 = a.nChains;
+                    table.push_back(d);
+                }
+                a.nChains++;
+            }
+        }
+        a.nChainItems = (uint32_t)table.size();
+        uint64_t chunk = a.nChains;
+        for (const auto& c : chains) {
+            if (c.size() == 1) {
+                fb::RmaAccDesc d = c[0];
+                d.chunk0 = (uint32_t)chunk;
+                table.push_back(d);
+                chunk += fb::fbRmaAccChunks(d.count);
+            }
+        }
+        a.nItems = (uint32_t)table.size();
+        a.totalChunks = (uint32_t)chunk;
+        return a;
+    }
+};
+}
+
+int Communicator::accumulateMany(const RmaAccumulate* items, size_t n, int dtype, int op, cudaStream_t s)
+{
+    if (parent_ != nullptr) {
+        return FB_E_UNSUPPORTED; // see subset()
+    }
+    const size_t esize = fbDtypeSize(dtype);
+    if (esize == 0 || (n > 0 && items == nullptr)) {
+        return FB_E_INVALID;
+    }
+    if (!fb::rmaSupported(dtype, op, true)) {
+        return FB_E_UNSUPPORTED;
+    }
+    for (size_t i = 0; i < n; i++) {
+        const RmaAccumulate& it = items[i];
+        if (it.peer < 0 || it.peer >= dev_.nranks) {
+            return FB_E_INVALID;
+        }
+        if (it.count > 0 && ((op == FB_OP_NO_OP && it.fetch == nullptr) || (op != FB_OP_NO_OP && it.origin == nullptr) ||
+                             it.count > heapTotal_ / esize ||
+                             !rmaTargetOk(it.offset, (uint64_t)it.count * esize, esize, it.peer))) {
+            return FB_E_INVALID;
+        }
+    }
+    bindDevice();
+    std::vector<fb::RmaAccDesc> table;
+    table.reserve(FB_RMA_ACC_MAX_ITEMS);
+    AccLaunch launch;
+    uint64_t launchBytes = 0;
+    auto issue = [&]() {
+        if (launch.items == 0) {
+            return FB_OK;
+        }
+        fb::RmaAccManyArgs a = launch.layout(table);
+        ManySlot* slot = nullptr;
+        a.items = (const fb::RmaAccDesc*)stageManyTable(table.data(), table.size() * sizeof(fb::RmaAccDesc), s, &slot);
+        if (a.items == nullptr) {
+            return FB_E_CUDA;
+        }
+        stats_.launches++;
+        stats_.bytes += launchBytes;
+        if (k_->rmaAccumulateMany(a, dtype, op, s) != cudaSuccess) {
+            return FB_E_CUDA;
+        }
+        releaseManySlot(slot, s);
+        launch = AccLaunch();
+        launchBytes = 0;
+        return FB_OK;
+    };
+    for (size_t i = 0; i < n; i++) {
+        const RmaAccumulate& it = items[i];
+        // pieces of at most FB_RMA_ACC_MAX_COUNT elements
+        for (size_t done = 0; done < it.count;) {
+            const uint32_t count = (uint32_t)std::min<size_t>(it.count - done, FB_RMA_ACC_MAX_COUNT);
+            const uint64_t off = it.offset + done * esize;
+            const uint64_t bytes = (uint64_t)count * esize;
+            const fb::RmaAccDesc d{ it.origin == nullptr ? nullptr : (const uint8_t*)it.origin + done * esize,
+                                    it.fetch == nullptr ? nullptr : (uint8_t*)it.fetch + done * esize,
+                                    dev_.heap[it.peer] + off,
+                                    count,
+                                    0 };
+            if (!launch.add(d, it.peer, off, bytes)) {
+                const int rc = issue();
+                if (rc != FB_OK) {
+                    return rc;
+                }
+                launch.add(d, it.peer, off, bytes); // (always fits an empty launch)
+            }
+            launchBytes += bytes;
+            done += count;
+        }
+    }
+    return issue();
 }
 
 } // namespace faabric::device

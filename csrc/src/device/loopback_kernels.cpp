@@ -959,6 +959,15 @@ cudaError_t rmaCopyMany(const RmaCopyArgs& a, cudaStream_t)
     return cudaSuccess;
 }
 
+cudaError_t rmaAccumulateMany(const RmaAccManyArgs& a, int dtype, int op, cudaStream_t s)
+{
+    for (uint32_t i = 0; i < a.nItems; i++) {
+        const RmaAccDesc& it = a.items[i];
+        rmaAccumulate(RmaArgs{ it.target, it.origin, it.fetch, it.count }, dtype, op, s);
+    }
+    return cudaSuccess;
+}
+
 // ----------------------------------------------------------------- copy ----
 cudaError_t copy(void* dst, const void* src, size_t bytes, cudaStream_t)
 {

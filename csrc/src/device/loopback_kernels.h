@@ -31,6 +31,7 @@ struct KernelTable
     cudaError_t (*rmaAccumulate)(const RmaArgs& a, int dtype, int op, cudaStream_t s);
     cudaError_t (*rmaCompareSwap)(const RmaCasArgs& a, int dtype, cudaStream_t s);
     cudaError_t (*rmaCopyMany)(const RmaCopyArgs& a, cudaStream_t s);
+    cudaError_t (*rmaAccumulateMany)(const RmaAccManyArgs& a, int dtype, int op, cudaStream_t s);
     // device-to-device copies: one range, and `height` rows of `width` bytes
     cudaError_t (*copy)(void* dst, const void* src, size_t bytes, cudaStream_t s);
     cudaError_t (*copy2D)(void* dst,
@@ -72,6 +73,8 @@ cudaError_t rmaAccumulate(const RmaArgs& a, int dtype, int op, cudaStream_t s);
 cudaError_t rmaCompareSwap(const RmaCasArgs& a, int dtype, cudaStream_t s);
 // a.items: HOST memory; one copy per item, in list order
 cudaError_t rmaCopyMany(const RmaCopyArgs& a, cudaStream_t s);
+// a.items: HOST memory; one rmaAccumulate per item, in table order
+cudaError_t rmaAccumulateMany(const RmaAccManyArgs& a, int dtype, int op, cudaStream_t s);
 cudaError_t copy(void* dst, const void* src, size_t bytes, cudaStream_t s);
 cudaError_t copy2D(void* dst, size_t dpitch, const void* src, size_t spitch, size_t width, size_t height, cudaStream_t s);
 

@@ -482,6 +482,33 @@ int rmaAtomicTarget(const std::vector<uint64_t>& bases,
 }
 }
 
+int MpiWorld::rmaAccumulateArgs(RmaWindow& w,
+                                const uint8_t* origin,
+                                size_t count,
+                                faabric_datatype_t* datatype,
+                                faabric_op_t* op,
+                                uint8_t* result,
+                                int targetRank,
+                                int64_t targetDisp,
+                                int* dtype,
+                                int* fop,
+                                uint8_t** target)
+{
+    *dtype = datatype != nullptr ? fbDtypeFor(datatype) : -1;
+    *fop = op != nullptr ? fbOpFor(op) : -1;
+    if (*dtype < 0) {
+        return MPI_ERR_ARG;
+    }
+    if (*fop < 0 || !fb::rmaSupported(*dtype, *fop, result != nullptr)) {
+        return MPI_ERR_OP;
+    }
+    const size_t esize = fbDtypeSize(*dtype);
+    if (count > (size_t)INT64_MAX / esize || (origin == nullptr && *fop != FB_OP_NO_OP && count > 0)) {
+        return MPI_ERR_ARG;
+    }
+    return rmaAtomicTarget(w.bases, w.sizes, w.dispUnits, targetRank, targetDisp, count * esize, esize, target);
+}
+
 int MpiWorld::winAccumulate(int rank,
                             int winId,
                             const uint8_t* origin,
@@ -492,26 +519,18 @@ int MpiWorld::winAccumulate(int rank,
                             int targetRank,
                             int64_t targetDisp)
 {
-    const int dtype = datatype != nullptr ? fbDtypeFor(datatype) : -1;
-    const int fop = op != nullptr ? fbOpFor(op) : -1;
-    if (dtype < 0) {
-        return MPI_ERR_ARG;
-    }
-    if (fop < 0 || !fb::rmaSupported(dtype, fop, result != nullptr)) {
-        return MPI_ERR_OP;
-    }
-    const size_t esize = fbDtypeSize(dtype);
-    if (count > (size_t)INT64_MAX / esize || (origin == nullptr && fop != FB_OP_NO_OP && count > 0)) {
-        return MPI_ERR_ARG;
-    }
     auto w = getWindow(winId);
+    int dtype = -1;
+    int fop = -1;
     uint8_t* target = nullptr;
-    const size_t bytes = count * esize;
-    int rc = rmaAtomicTarget(w->bases, w->sizes, w->dispUnits, targetRank, targetDisp, bytes, esize, &target);
+    int rc = rmaAccumulateArgs(*w, origin, count, datatype, op, result, targetRank, targetDisp, &dtype, &fop, &target);
     if (rc != MPI_SUCCESS || count == 0) {
         return rc;
     }
+    const size_t bytes = count * fbDtypeSize(dtype);
     if (isLocalRank(targetRank)) {
+        // after this origin's deferred accumulates (same stream)
+        rmaIssueBatch(*w, rank);
         rmaApplyLocal(*w, rank, targetRank, target, count, dtype, fop, origin, nullptr, result, w->streams[rank]);
         return MPI_SUCCESS;
     }
@@ -555,6 +574,7 @@ int MpiWorld::winCompareSwap(int rank,
         return rc;
     }
     if (isLocalRank(targetRank)) {
+        rmaIssueBatch(*w, rank);
         rmaApplyLocal(*w, rank, targetRank, target, 1, dtype, -1, origin, compare, result, w->streams[rank]);
         return MPI_SUCCESS;
     }
@@ -1129,16 +1149,55 @@ void MpiWorld::rmaIssueBatch(RmaWindow& w, int rank)
     const int device = comm->isLoopback() ? HOST_MEMORY : comm->device();
     cudaStream_t s = (cudaStream_t)streamForRank(rank);
     DeviceGuard on(device);
-    const int rc = comm->putGetMany(batch.data(), batch.size(), s);
+    // runs in issue order: copies, or accumulates of one (dtype, op)
+    std::vector<faabric::device::Communicator::RmaCopy> copies;
+    std::vector<faabric::device::Communicator::RmaAccumulate> accs;
+    int rc = FB_OK;
+    for (size_t i = 0; i < batch.size() && rc == FB_OK;) {
+        size_t j = i;
+        const RmaBatchItem& first = batch[i];
+        if (first.dtype < 0) {
+            copies.clear();
+            for (; j < batch.size() && batch[j].dtype < 0; j++) {
+                copies.push_back(batch[j].copy);
+            }
+            rc = comm->putGetMany(copies.data(), copies.size(), s);
+        } else {
+            accs.clear();
+            for (; j < batch.size() && batch[j].dtype == first.dtype && batch[j].op == first.op; j++) {
+                accs.push_back(batch[j].acc);
+            }
+            rc = comm->accumulateMany(accs.data(), accs.size(), first.dtype, first.op, s);
+        }
+        i = j;
+    }
     batch.clear();
     if (rc != FB_OK) {
-        throw std::runtime_error(std::string("Batched one-sided copy failed: ") +
+        throw std::runtime_error(std::string("Batched one-sided operation failed: ") +
                                  faabric::device::Communicator::errorString(rc));
     }
     auto& used = w.streams[rank];
     if (device != HOST_MEMORY && std::find(used.begin(), used.end(), std::make_pair(device, (void*)s)) == used.end()) {
         used.emplace_back(device, (void*)s);
     }
+}
+
+// Can `rank`'s communicator batch an operation between `buf` (bytes, may be
+// null) and a target of `targetRank` in this process: the target in its
+// symmetric heap, the buffer on the origin's GPU or in its heap (on the
+// loopback backend: in a heap, device-role memory that memcpy reaches)
+bool MpiWorld::rmaBatchable(int rank, int targetRank, const uint8_t* target, size_t bytes, const uint8_t* buf, const uint8_t* buf2)
+{
+    auto comm = wiredDeviceComm(rank);
+    auto targetComm = wiredDeviceComm(targetRank);
+    if (comm == nullptr || targetComm == nullptr || !targetComm->inHeap(target, bytes)) {
+        return false;
+    }
+    auto ok = [&](const uint8_t* p) {
+        return p == nullptr || (comm->isLoopback() ? isDevicePointer(p) && hostAddressable(p)
+                                                   : comm->inHeap(p, bytes) || bufferDevice(p) == comm->device());
+    };
+    return ok(buf) && ok(buf2);
 }
 
 int MpiWorld::rmaRequestTarget(RmaWindow& w, int rank, int targetRank, int64_t targetDisp, size_t bytes, uint8_t** target)
@@ -1182,15 +1241,13 @@ int MpiWorld::winRputGet(int rank, int winId, uint8_t* origin, size_t bytes, int
         // Heap to heap, origin on the origin's GPU: one launch for the batch
         // (on the loopback backend the origin is in a heap: device-role
         // memory that memcpy reaches)
-        auto comm = wiredDeviceComm(rank);
-        auto targetComm = wiredDeviceComm(targetRank);
-        const bool originOk =
-          comm != nullptr && (comm->isLoopback() ? isDevicePointer(origin) && hostAddressable(origin)
-                                                 : comm->inHeap(origin, bytes) || bufferDevice(origin) == comm->device());
-        if (originOk && targetComm != nullptr && targetComm->inHeap(target, bytes)) {
+        if (rmaBatchable(rank, targetRank, target, bytes, origin, nullptr)) {
             auto& batch = w->batches[rank];
-            batch.push_back(faabric::device::Communicator::RmaCopy{
-              origin, targetComm->offsetOf(target), bytes, targetRank, get ? 1 : 0 });
+            RmaBatchItem item;
+            item.copy = faabric::device::Communicator::RmaCopy{
+                origin, wiredDeviceComm(targetRank)->offsetOf(target), bytes, targetRank, get ? 1 : 0
+            };
+            batch.push_back(item);
             if (batch.size() >= FB_RMA_COPY_MAX_ITEMS) {
                 rmaIssueBatch(*w, rank);
             }
@@ -1238,7 +1295,31 @@ int MpiWorld::winRaccumulate(int rank,
     if (rc != MPI_SUCCESS) {
         return rc;
     }
-    // (every other check of MPI_Accumulate runs before it applies anything)
+    int fop = -1;
+    int fdt = -1;
+    rc = rmaAccumulateArgs(*w, origin, count, datatype, op, result, targetRank, targetDisp, &fdt, &fop, &target);
+    if (rc != MPI_SUCCESS) {
+        return rc;
+    }
+    const size_t bytes = count * fbDtypeSize(fdt);
+    if (isLocalRank(targetRank) && count > 0 && rmaBatchable(rank, targetRank, target, bytes, origin, result)) {
+        // Heap target, buffers on the origin's GPU: into the batch, after
+        // this origin's earlier deferred operations on the window
+        auto& batch = w->batches[rank];
+        RmaBatchItem item;
+        item.acc = faabric::device::Communicator::RmaAccumulate{
+            origin, result, wiredDeviceComm(targetRank)->offsetOf(target), count, targetRank
+        };
+        item.dtype = fdt;
+        item.op = fop;
+        batch.push_back(item);
+        if (batch.size() >= FB_RMA_COPY_MAX_ITEMS) {
+            rmaIssueBatch(*w, rank);
+        }
+        *requestId = addRmaRequest(rank, winId, targetRank, w->progress[rank]);
+        return MPI_SUCCESS;
+    }
+    // Today's MPI_Accumulate (which issues the batch first)
     rc = winAccumulate(rank, winId, origin, count, datatype, op, result, targetRank, targetDisp);
     if (rc != MPI_SUCCESS) {
         return rc;

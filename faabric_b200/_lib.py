@@ -137,6 +137,7 @@ def load():
     _sig(lib, "fb_compare_and_swap", i32, [vp, vp, vp, vp, u64, i32, i32, vp])
     i32p = C.POINTER(C.c_int32)
     _sig(lib, "fb_put_get_many", i32, [vp, i32, vpp, u64p, u64p, i32p, i32p, vp])
+    _sig(lib, "fb_accumulate_many", i32, [vp, i32, vpp, vpp, u64p, u64p, i32p, i32, i32, vp])
 
     regp = C.POINTER(FbMergeRegion)
     _sig(

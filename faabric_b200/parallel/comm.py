@@ -733,6 +733,77 @@ class Communicator:
         self._check(rc, "accumulate")
         return fetch
 
+    def accumulate_many(self, srcs, dsts_sym, peers, op="sum", dtype=None, fetches=None, stream=None):
+        """:meth:`accumulate` of every ``srcs[i]`` into ``peers[i]``'s copy of
+        the symmetric tensor ``dsts_sym[i]``, with one ``op`` and dtype for
+        the whole list (MPI_Raccumulate / MPI_Rget_accumulate bursts).
+        ``fetches`` (None, or one tensor or None per item) receive the
+        previous values; ``srcs[i]`` may be None for ``"no_op"``, which needs
+        a fetch on every item.  Items whose targets intersect apply in list
+        order, also in what they fetch.  Typically one launch for up to 1024
+        items; the exact rule is Communicator::accumulateMany's.
+        Stream-ordered; returns ``fetches``."""
+        self._parent_only("accumulate_many")
+        if op not in OPS:
+            raise CommError(f"unknown op {op!r}")
+        n = len(dsts_sym)
+        fl = [None] * n if fetches is None else list(fetches)
+        if len(srcs) != n or len(peers) != n or len(fl) != n:
+            raise CommError(
+                f"accumulate_many: {len(srcs)} sources, {n} symmetric tensors, {len(peers)} peers and {len(fl)} fetches"
+            )
+        ptrs, fptrs, offs, counts, prs, dts = [], [], [], [], [], set()
+        for i, (src, sym, peer, fetch) in enumerate(zip(srcs, dsts_sym, peers, fl)):
+            ref = src if src is not None else fetch
+            if ref is None:
+                raise CommError(f"accumulate_many: item {i} needs src (or fetch for no_op)")
+            if src is None and op != "no_op":
+                raise CommError(f"accumulate_many: item {i} has no src for {op!r}")
+            for t, what in ((src, "src"), (fetch, "fetch")):
+                if t is None:
+                    continue
+                if not t.is_cuda or not t.is_contiguous():
+                    raise CommError(f"accumulate_many: item {i} {what} must be a contiguous CUDA tensor")
+                if t.device.index != self.device:
+                    raise CommError(f"accumulate_many: item {i} {what} is on {t.device}, not on cuda:{self.device}")
+            count, dt = self._typed(ref, dtype)
+            dts.add(dt)
+            nb = ref.numel() * ref.element_size()
+            for t, what in ((fetch, "fetch"), (sym, "symmetric tensor")):
+                if t is not None and t.numel() * t.element_size() != nb:
+                    raise CommError(f"accumulate_many: item {i} {what} holds {t.numel() * t.element_size()} bytes, not {nb}")
+            if not sym.is_contiguous():
+                raise CommError(f"accumulate_many: item {i} symmetric tensor must be contiguous")
+            # (an empty item is skipped: only its peer is checked)
+            if nb > 0 and not self._lib.fb_comm_in_heap(self._h, C.c_void_p(sym.data_ptr()), nb):
+                raise CommError(f"accumulate_many: item {i} symmetric tensor is not in the symmetric heap")
+            peer = int(peer)
+            if peer < 0 or peer >= self.size:
+                raise CommError(f"accumulate_many: item {i} peer {peer} outside a communicator of {self.size}")
+            ptrs.append(src.data_ptr() if src is not None else None)
+            fptrs.append(fetch.data_ptr() if fetch is not None else None)
+            offs.append(self.heap_offset(sym) if nb > 0 else 0)
+            counts.append(count)
+            prs.append(peer)
+        if len(dts) > 1:
+            raise CommError("accumulate_many: every item must have one dtype")
+        if n == 0:
+            return fetches
+        rc = self._lib.fb_accumulate_many(
+            self._h,
+            n,
+            (C.c_void_p * n)(*ptrs),
+            (C.c_void_p * n)(*fptrs),
+            (C.c_uint64 * n)(*offs),
+            (C.c_uint64 * n)(*counts),
+            (C.c_int32 * n)(*prs),
+            dts.pop(),
+            OPS[op],
+            self._stream(stream),
+        )
+        self._check(rc, "accumulate_many")
+        return fetches
+
     def fetch_and_op(self, src, dst_sym, peer, result, op="sum", dtype=None, stream=None):
         """MPI_Fetch_and_op: :meth:`accumulate` of ONE element with fetch into
         ``result`` (``src`` may be None for ``"no_op"``)."""
