@@ -28,6 +28,7 @@
 #include "../tests/mpi_rma_accumulate_batch_body.h"
 #include "../tests/mpi_rma_request_body.h"
 #include "../tests/mpi_subcomm_device_body.h"
+#include "../tests/mpi_group_subcomm_body.h"
 
 #include <cuda_runtime.h>
 
@@ -810,6 +811,112 @@ static void registerFunctions()
             msg.set_outputdata(why);
         }
         return rc;
+    });
+
+    // MPI_Ibcast bursts and the grouped non-blocking collectives on
+    // sub-communicators (mpi_group_subcomm_body.h)
+    mpiFunction("group-subcomm", [](int rank, int size, faabric::Message& msg) {
+        std::string why;
+        int rc = group_subcomm::body(rank, size, msg.mpiworldid(), &why);
+        if (rc != 0) {
+            SPDLOG_ERROR("group-subcomm: {}", why);
+            msg.set_outputdata(why);
+        }
+        return rc;
+    });
+
+    // A list of float32 tensors in one symmetric-heap buffer, each 16-byte
+    // aligned, per step.  Input: "<mode>;<steps>;<count0,count1,...>" with mode
+    //   bcast           one MPI_Bcast per tensor from rank 0 on the world
+    //   ibcast          MPI_Ibcast per tensor + MPI_Waitall on the world
+    //   sub-allreduce   one MPI_Allreduce (SUM, in place) per tensor on the
+    //                   half communicator of this rank (MPI_Comm_split)
+    //   sub-iallreduce  MPI_Iallreduce per tensor + MPI_Waitall on it
+    // Rank 0 reports {"ms_per_step", "us_per_call", "launches_per_step"}:
+    // the device launches of rank 0's communicator for the call (the world's,
+    // or the child's) per step.
+    mpiFunction("bench-group-bcast", [](int rank, int size, faabric::Message& msg) {
+        std::vector<std::string> f;
+        std::string cur;
+        for (char c : msg.inputdata() + ";") {
+            if (c == ';') {
+                f.push_back(cur);
+                cur.clear();
+            } else {
+                cur += c;
+            }
+        }
+        EXPECT(f.size() >= 3 && size >= 2);
+        const std::string mode = f[0];
+        const int steps = std::stoi(f[1]);
+        std::vector<int> counts;
+        for (size_t b = 0, e; b < f[2].size(); b = e + 1) {
+            e = f[2].find(',', b);
+            if (e == std::string::npos) {
+                e = f[2].size();
+            }
+            counts.push_back(std::stoi(f[2].substr(b, e - b)));
+        }
+        size_t total = 0;
+        std::vector<size_t> offs;
+        for (int c : counts) {
+            offs.push_back(total);
+            total += (size_t)(c + 3) / 4 * 4;
+        }
+        faabric::mpi::MpiWorld& world = faabric::mpi::getMpiWorldRegistry().getWorld(msg.mpiworldid());
+        float* buf = nullptr;
+        EXPECT(MPI_Alloc_mem(total * 4, MPI_INFO_FAABRIC_DEVICE, &buf) == MPI_SUCCESS);
+        std::vector<float> init(total, (float)rank);
+        cudaMemcpy(buf, init.data(), total * 4, cudaMemcpyHostToDevice);
+        const bool sub = mode.rfind("sub-", 0) == 0;
+        MPI_Comm comm = MPI_COMM_WORLD;
+        if (sub) {
+            MPI_Comm_split(MPI_COMM_WORLD, rank / (size / 2), rank, &comm);
+        }
+        const int n = (int)counts.size();
+        std::vector<MPI_Request> reqs(n);
+        auto step = [&]() -> int {
+            for (int i = 0; i < n; i++) {
+                float* t = buf + offs[i];
+                if (mode == "bcast") {
+                    EXPECT(MPI_Bcast(t, counts[i], MPI_FLOAT, 0, comm) == MPI_SUCCESS);
+                } else if (mode == "ibcast") {
+                    EXPECT(MPI_Ibcast(t, counts[i], MPI_FLOAT, 0, comm, &reqs[i]) == MPI_SUCCESS);
+                } else if (mode == "sub-allreduce") {
+                    EXPECT(MPI_Allreduce(MPI_IN_PLACE, t, counts[i], MPI_FLOAT, MPI_SUM, comm) == MPI_SUCCESS);
+                } else {
+                    EXPECT(MPI_Iallreduce(MPI_IN_PLACE, t, counts[i], MPI_FLOAT, MPI_SUM, comm, &reqs[i]) == MPI_SUCCESS);
+                }
+            }
+            if (mode == "ibcast" || mode == "sub-iallreduce") {
+                EXPECT(MPI_Waitall(n, reqs.data(), MPI_STATUSES_IGNORE) == MPI_SUCCESS);
+            }
+            return 0;
+        };
+        for (int i = 0; i < 3; i++) {
+            EXPECT(step() == 0);
+        }
+        auto dev = sub ? group_subcomm::childOf(comm, rank) : world.getDeviceComm(rank);
+        EXPECT(dev != nullptr);
+        MPI_Barrier(MPI_COMM_WORLD);
+        const uint64_t l0 = dev->stats().launches;
+        auto t0 = std::chrono::steady_clock::now();
+        for (int i = 0; i < steps; i++) {
+            EXPECT(step() == 0);
+        }
+        const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count() / steps;
+        const double launches = (double)(dev->stats().launches - l0) / steps;
+        MPI_Barrier(MPI_COMM_WORLD);
+        if (rank == 0) {
+            msg.set_outputdata("{\"ms_per_step\": " + std::to_string(ms) + ", \"us_per_call\": " +
+                               std::to_string(ms * 1000.0 / n) + ", \"launches_per_step\": " + std::to_string(launches) +
+                               "}");
+        }
+        if (sub) {
+            MPI_Comm_free(&comm);
+        }
+        MPI_Free_mem(buf);
+        return 0;
     });
 
     // MPI_Allreduce (float32 SUM) on symmetric-heap buffers.  Input:

@@ -345,7 +345,9 @@ void fb_comm_free(void* h, uint64_t off)
 // A communicator over `members` (ranks of `h`, in child order) using signal
 // slot `slot`; null on failure (fb_last_error).  Release with fb_comm_destroy
 // once the child's last collective has completed: it zeroes the slot pad
-// without waiting for the caller's streams.
+// without waiting for the caller's streams.  The child runs every
+// collective and grouped call of Communicator::subset (point to point,
+// put-signal, the one-sided calls and host barriers stay on the parent).
 void* fb_comm_subset(void* h, const int* members, int n, int slot)
 {
     FB_TRY
@@ -678,6 +680,50 @@ int fb_all_gather_many(void* h,
     FB_TRY
     auto items = groupItems(n, send, recv, counts);
     return COMM(h)->allGatherMany(items.data(), items.size(), dtype, flags, (cudaStream_t)stream);
+    FB_CATCH(FB_E_CUDA)
+}
+
+// ---- grouped broadcast: one buffer and byte count per item ----
+static std::vector<Communicator::GroupItem> broadcastItems(int n, void* const* bufs, const uint64_t* bytes)
+{
+    std::vector<Communicator::GroupItem> items((size_t)std::max(n, 0));
+    for (int i = 0; i < n; i++) {
+        items[i].send = bufs[i];
+        items[i].recv = bufs[i];
+        items[i].count = (size_t)bytes[i];
+    }
+    return items;
+}
+
+void* fb_group_prepare_broadcast(void* h, int n, void* const* bufs, const uint64_t* bytes)
+{
+    FB_TRY
+    auto items = broadcastItems(n, bufs, bytes);
+    int rc = FB_OK;
+    auto plan = COMM(h)->prepareGroup(items.data(), items.size(), FB_U8, &rc, Communicator::GROUP_BROADCAST);
+    if (!plan) {
+        g_lastError = std::string("prepareGroup: ") + Communicator::errorString(rc);
+        return nullptr;
+    }
+    auto* ph = new FbGroupPlanHandle();
+    ph->plan = plan;
+    return ph;
+    FB_CATCH(nullptr)
+}
+
+int fb_group_broadcast(void* h, void* plan, int root, int flags, void* stream)
+{
+    if (plan == nullptr) {
+        return FB_E_INVALID;
+    }
+    return COMM(h)->broadcastGroup(*((FbGroupPlanHandle*)plan)->plan, root, flags, (cudaStream_t)stream);
+}
+
+int fb_broadcast_many(void* h, int n, void* const* bufs, const uint64_t* bytes, int root, int flags, void* stream)
+{
+    FB_TRY
+    auto items = broadcastItems(n, bufs, bytes);
+    return COMM(h)->broadcastMany(items.data(), items.size(), root, flags, (cudaStream_t)stream);
     FB_CATCH(FB_E_CUDA)
 }
 

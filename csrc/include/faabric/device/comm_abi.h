@@ -70,7 +70,12 @@ extern "C" {
 // created.  This is correct because every word a peer writes into a rank's
 // pad during a collective is awaited by that rank in the same collective (the
 // in-kernel flag barriers, the per-block epoch words, which only the owner
-// writes, and the stream-ordered barrier: signalPeers + a wait per peer).  So
+// writes, and the stream-ordered barrier: signalPeers + a wait per peer).  The
+// grouped kernels (groupAllReduceKernel, groupReduceScatterKernel,
+// groupAllGatherKernel, groupBroadcastKernel) keep it too: they write a pad
+// only through the entry and exit BlockBarrier syncs, each of which awaits
+// the flag of every peer it signals, or run between two stream-ordered
+// barriers with no in-kernel synchronisation at all.  So
 // once a rank's last collective on the child has completed, no peer write to
 // its pad is pending, and a free slot is all zeros.  A member that creates its
 // child early may therefore signal a peer that has not created its own yet:

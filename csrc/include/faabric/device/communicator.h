@@ -141,10 +141,10 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     // The child runs the same fused kernels over the members' heaps, with slot
     // `slot` of every member's signal region as its pads (comm_abi.h).  It
     // supports allReduce (one-shot and two-shot only), reduce, reduceScatter,
-    // scan, the data-movement collectives, barrier and the heap queries, with
-    // child ranks.  Point to point, put-signal, the one-sided atomics, the
-    // grouped all-reduce, reduce-scatter and all-gather, hostBarrier and
-    // subset return FB_E_UNSUPPORTED;
+    // scan, the data-movement collectives, the grouped calls (plans and
+    // *Many), barrier and the heap queries, with child ranks.  Point to
+    // point, put-signal, the one-sided atomics, hostBarrier and subset return
+    // FB_E_UNSUPPORTED;
     // alloc / free throw std::logic_error (heap allocation is collective over
     // the whole parent).  A child and its parent share this rank's staging
     // buffers: calls on both from one rank must be stream-ordered unless the
@@ -152,6 +152,12 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     // empty list, a member out of range or repeated, this rank not a member,
     // or a slot out of range or in use on this rank.  Destroying the child
     // zeroes this rank's slot pad on a stream of its own, then frees the slot.
+    // A child's *Many tables live in its parent's table ring (on the parent's
+    // device, freed with the parent); a plan prepared on a child owns its
+    // tables and frees them with cudaFree on the child's device when the
+    // last reference to the plan goes.  The ring's host state is shared and
+    // not synchronised: one host thread must drive a rank's parent and all
+    // of its children (as MPI rank threads and LocalGroup.run do).
     // Precondition: this rank's last collective on the child has completed
     // (its stream has been waited for); the destructor does not order itself
     // after the caller's streams.
@@ -268,6 +274,9 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     //   GROUP_ALLGATHER: send holds count elements; block p of recv (size()
     //     *count elements) gets send of rank p (MPI_Allgather per item; a
     //     byte copy, any dtype)
+    //   GROUP_BROADCAST: recv holds count elements (send is not read); every
+    //     rank's recv gets the root's (MPI_Bcast per item; a byte copy, any
+    //     dtype, any length).  Cut into equal ranges like the all-reduce.
     // Shard kinds group an item only if send and recv are in the symmetric
     // heap and 16-byte aligned, count*esize is a multiple of 16, and recv
     // overlaps no send of the group on this rank.  The one exception is the
@@ -277,12 +286,13 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     {
         GROUP_ALLREDUCE = 0,
         GROUP_REDUCE_SCATTER = 1,
-        GROUP_ALLGATHER = 2
+        GROUP_ALLGATHER = 2,
+        GROUP_BROADCAST = 3
     };
     // Builds (and uploads) this rank's segment tables.  Collective: every rank
     // must pass the same list (same offsets, same counts).  Returns null and
-    // sets *rc when an item is not symmetric / aligned (FB_E_INVALID), or on
-    // a sub-communicator (FB_E_UNSUPPORTED).
+    // sets *rc when an item is not symmetric / aligned (FB_E_INVALID).  Works
+    // on a sub-communicator's child as on any other communicator.
     std::shared_ptr<GroupPlan> prepareGroup(const GroupItem* items,
                                             size_t nItems,
                                             int dtype,
@@ -292,6 +302,10 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     int allReduceGroup(const GroupPlan& plan, int op, int flags, cudaStream_t s);
     int reduceScatterGroup(const GroupPlan& plan, int op, int flags, cudaStream_t s);
     int allGatherGroup(const GroupPlan& plan, int flags, cudaStream_t s);
+    // A GROUP_BROADCAST plan from `root` (a rank of this communicator; out of
+    // range: FB_E_INVALID).  The root's buffers are only read.  On a
+    // one-member communicator nothing is launched.
+    int broadcastGroup(const GroupPlan& plan, int root, int flags, cudaStream_t s);
     // prepare + launch for a transient list (MPI_Iallreduce bursts); falls back
     // to per-item allReduce calls when the list cannot be grouped
     int allReduceMany(const GroupItem* items,
@@ -316,6 +330,12 @@ class Communicator : public std::enable_shared_from_this<Communicator>
                       int dtype,
                       int flags,
                       cudaStream_t s);
+    // MPI_Ibcast bursts: item i broadcasts items[i].count BYTES of
+    // items[i].recv from `root` (send is not read).  A batch whose buffers
+    // are not all in the symmetric heap and 16-byte aligned falls back to
+    // per-item broadcast calls.  Root out of range: FB_E_INVALID; one member:
+    // nothing is launched.
+    int broadcastMany(const GroupItem* items, size_t nItems, int root, int flags, cudaStream_t s);
     static size_t groupPlanLaunches(const GroupPlan& plan);
 
     // ---- point to point (per-pair FIFO; no kernel ever spins on a peer) ----

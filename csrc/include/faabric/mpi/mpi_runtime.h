@@ -339,6 +339,13 @@ class MpiWorld
                    faabric_datatype_t* recvType,
                    int recvCount);
 
+    // MPI_Ibcast on the world (root: a world rank), by the same rules:
+    // symmetric, 16-byte aligned device buffers join a burst keyed by (kind,
+    // communicator, root), issued as one grouped launch at the next wait;
+    // other device buffers run one broadcast at issue; host buffers complete
+    // at issue.
+    int iBroadcast(int rank, int root, uint8_t* buffer, faabric_datatype_t* dt, int count);
+
     // Symmetric-heap allocation for MPI_Alloc_mem (collective: every rank
     // must allocate the same sizes in the same order)
     void* deviceAlloc(int rank, size_t bytes);
@@ -557,6 +564,35 @@ class MpiWorld
     // false for an in-place all-gather (send is this rank's slot of recv)
     bool deviceAllGather(const DeviceComm& comm, int rank, const uint8_t* send, uint8_t* recv, size_t bytes);
     bool deviceAllToAll(const DeviceComm& comm, int rank, const uint8_t* send, uint8_t* recv, size_t chunk);
+    // `recvCount` elements of the reduction per member; false for no comm,
+    // a pair the kernels lack, or a call the communicator declines
+    bool deviceReduceScatter(const DeviceComm& comm, int rank, const uint8_t* send, uint8_t* recv,
+                             faabric_datatype_t* dt, int recvCount, faabric_op_t* op);
+
+    // ---- non-blocking collectives on any communicator ----
+    // One function per collective, shared by MPI_COMM_WORLD and the
+    // sub-communicators, each returning a request of this rank thread.
+    // `comm` is this rank's device communicator for the call's members (the
+    // world's, or a sub-communicator's child; null: no device path), `rank`
+    // the caller's WORLD rank, `members` the communicator's size and `host`
+    // the blocking call on the communicator's host path, which completes the
+    // request at issue.  Symmetric, 16-byte aligned device buffers are
+    // deferred into this rank's burst (FAABRIC_MPI_GROUP_IALLREDUCE=0 turns
+    // that off); other device buffers run one device call at issue.
+    using HostPath = std::function<void()>;
+    int nbAllReduce(const DeviceComm& comm, int rank, const uint8_t* send, uint8_t* recv,
+                    faabric_datatype_t* dt, int count, faabric_op_t* op, const HostPath& host);
+    // (send == recv runs `host`: the output would overwrite input the peers
+    // are still reading)
+    int nbReduceScatter(const DeviceComm& comm, int rank, int members, const uint8_t* send, uint8_t* recv,
+                        faabric_datatype_t* dt, int recvCount, faabric_op_t* op, const HostPath& host);
+    int nbAllGather(const DeviceComm& comm, int rank, int members, const uint8_t* send, uint8_t* recv,
+                    size_t bytes, const HostPath& host);
+    // `root` is a rank of `comm`'s communicator (the caller checked it)
+    int nbBroadcast(const DeviceComm& comm, int rank, int root, uint8_t* buffer, size_t bytes, const HostPath& host);
+    // Issues this rank thread's pending burst if it is keyed to `comm`, and
+    // waits for it (before `comm` is released: MPI_Comm_free)
+    void settleDeviceBurst(const DeviceComm& comm);
 
   private:
     int id = -1;

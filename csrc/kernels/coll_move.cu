@@ -353,6 +353,125 @@ cudaError_t launchGroupAllGather(const GroupArgs& a,
 }
 
 // ----------------------------------------------------------------------------
+// Grouped broadcast: one MPI_Bcast per tensor, all in ONE launch per rank
+// (launch_api.h).  The list's vectors are cut into n equal ranges as for the
+// grouped all-reduce; each rank loads its range once from the root's buffer
+// and stores it into every other rank's buffer (a scatter and an all-gather
+// in one pass: the root sends each byte out once).  Entry barrier: the root's
+// data is ready and every output may be overwritten.  Exit barrier: every
+// store into this rank's buffer has landed.  The root's buffer is only read.
+// Buffers that overlap within a list need no check: every store of byte `off`
+// carries the root's byte at `off`, so any overlap leaves the bytes that
+// issuing the broadcasts one by one would.  Dtype-free: a byte copy.
+// ----------------------------------------------------------------------------
+template<int NR>
+__global__ void __launch_bounds__(512, 1) groupBroadcastKernel(const GroupArgs a)
+{
+    extern __shared__ __align__(16) uint8_t sGroupRaw[];
+    GroupSeg* sSegs = reinterpret_cast<GroupSeg*>(sGroupRaw);
+    const FbCommDev& c = a.comm;
+    const int n = (NR > 0) ? NR : c.nranks;
+    const int root = a.root;
+    BlockBarrier bar;
+    const bool ok = groupEnter(a, sSegs, bar);
+
+    if (ok && a.nSegs > 0) {
+        constexpr int UNROLL = (NR == 8) ? 2 : (NR == 1 ? 8 : 4);
+        constexpr uint32_t CHUNK = 32u * UNROLL;
+        const uint32_t lane = threadIdx.x & 31;
+        const uint32_t warpsPerCta = blockDim.x >> 5;
+        const uint32_t warpStride = gridDim.x * warpsPerCta;
+        const uint8_t* const in = c.heap[root];
+        int cur = 0;
+        for (uint32_t ch = blockIdx.x * warpsPerCta + (threadIdx.x >> 5);
+             ch < a.totalChunks;
+             ch += warpStride) {
+            cur = groupSegOf(sSegs, a.nSegs, cur, ch);
+            const GroupSeg sg = sSegs[cur];
+            const uint32_t v0 = (ch - sg.chunk0) * CHUNK;
+            const uint64_t off = sg.sendOff + (uint64_t)v0 * 16;
+            const uint32_t rem = sg.nVec > v0 ? sg.nVec - v0 : 0;
+            if (rem >= CHUNK) {
+                Vec16 v[UNROLL];
+#pragma unroll
+                for (int u = 0; u < UNROLL; u++) {
+                    v[u] = ldVecStream(in + off + (uint64_t)(u * 32 + lane) * 16);
+                }
+                if constexpr (NR > 0) {
+#pragma unroll
+                    for (int p = 0; p < NR; p++) {
+                        if (p != root) {
+#pragma unroll
+                            for (int u = 0; u < UNROLL; u++) {
+                                stVec(c.heap[p] + off + (uint64_t)(u * 32 + lane) * 16, v[u]);
+                            }
+                        }
+                    }
+                } else {
+                    for (int p = 0; p < n; p++) {
+                        if (p != root) {
+#pragma unroll
+                            for (int u = 0; u < UNROLL; u++) {
+                                stVec(c.heap[p] + off + (uint64_t)(u * 32 + lane) * 16, v[u]);
+                            }
+                        }
+                    }
+                }
+            } else {
+                // ragged end of a segment (or a whole small tensor)
+#pragma unroll
+                for (int u = 0; u < UNROLL; u++) {
+                    const uint32_t i = (uint32_t)u * 32 + lane;
+                    if (i < rem) {
+                        const Vec16 v = ldVecStream(in + off + (uint64_t)i * 16);
+                        for (int p = 0; p < n; p++) {
+                            if (p != root) {
+                                stVec(c.heap[p] + off + (uint64_t)i * 16, v);
+                            }
+                        }
+                    }
+                }
+                // the < 16-byte tail rides with the segment's last chunk, a
+                // byte at a time (MPI_Bcast counts are arbitrary)
+                if (sg.tailBytes != 0 && lane == 0 && v0 + CHUNK > sg.nVec) {
+                    const uint64_t t = sg.sendOff + (uint64_t)sg.nVec * 16;
+                    for (uint32_t e = 0; e < sg.tailBytes; e++) {
+                        const uint8_t b = Word<1>::ld(in + t + e);
+                        for (int p = 0; p < n; p++) {
+                            if (p != root) {
+                                Word<1>::st(c.heap[p] + t + e, b);
+                            }
+                        }
+                    }
+                }
+            }
+        }
+    }
+    groupExit(a, bar);
+}
+
+cudaError_t launchGroupBroadcast(const GroupArgs& a,
+                                 int blocks,
+                                 int threads,
+                                 cudaStream_t s)
+{
+    const size_t smem = (size_t)a.nSegs * sizeof(GroupSeg);
+    const int n = a.comm.nranks;
+    if (n == 1) {
+        groupBroadcastKernel<1><<<blocks, threads, smem, s>>>(a);
+    } else if (n == 2) {
+        groupBroadcastKernel<2><<<blocks, threads, smem, s>>>(a);
+    } else if (n == 4) {
+        groupBroadcastKernel<4><<<blocks, threads, smem, s>>>(a);
+    } else if (n == 8) {
+        groupBroadcastKernel<8><<<blocks, threads, smem, s>>>(a);
+    } else {
+        groupBroadcastKernel<0><<<blocks, threads, smem, s>>>(a);
+    }
+    return cudaGetLastError();
+}
+
+// ----------------------------------------------------------------------------
 // Barrier
 // ----------------------------------------------------------------------------
 __global__ void barrierKernel(const FbCommDev c)
@@ -618,6 +737,11 @@ cudaError_t preloadMoveKernels()
     FB_PRELOAD((groupAllGatherKernel<2>))
     FB_PRELOAD((groupAllGatherKernel<4>))
     FB_PRELOAD((groupAllGatherKernel<8>))
+    FB_PRELOAD((groupBroadcastKernel<0>))
+    FB_PRELOAD((groupBroadcastKernel<1>))
+    FB_PRELOAD((groupBroadcastKernel<2>))
+    FB_PRELOAD((groupBroadcastKernel<4>))
+    FB_PRELOAD((groupBroadcastKernel<8>))
     FB_PRELOAD(barrierKernel)
     FB_PRELOAD(waitSignalKernel)
     FB_PRELOAD(waitWordKernel)

@@ -87,7 +87,7 @@ struct GroupArgs
     uint32_t nSegs;
     uint32_t totalChunks;
     int32_t noSync;
-    int32_t pad;
+    int32_t root; // grouped broadcast only: the source rank
 };
 
 // vectors per warp-chunk for a world of n ranks (host and kernel must agree)
@@ -118,6 +118,17 @@ typedef cudaError_t (*GroupLaunchFn)(const GroupArgs& a,
 // Both keep the grouped all-reduce's chunking (fbGroupChunkVecs) and its
 // entry and exit barriers.
 cudaError_t launchGroupAllGather(const GroupArgs& a,
+                                 int blocks,
+                                 int threads,
+                                 cudaStream_t stream);
+
+// ---- grouped broadcast: many MPI_Bcast calls from one root, ONE launch ----
+// GroupArgs.root is the source rank.  The segments are the grouped
+// all-reduce's (this rank's share of the list's flat vector space, with
+// tailBytes 1..15 on a tensor's last segment) with sendOff == recvOff: the
+// kernel loads each vector from the root's heap and stores it into every
+// other rank's heap at the same offset.
+cudaError_t launchGroupBroadcast(const GroupArgs& a,
                                  int blocks,
                                  int threads,
                                  cudaStream_t stream);

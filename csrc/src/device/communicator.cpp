@@ -1234,6 +1234,7 @@ const fb::KernelTable CUDA_KERNELS = {
     .group = cudaGroup,
     .groupReduceScatter = cudaGroupReduceScatter,
     .groupAllGather = fb::launchGroupAllGather,
+    .groupBroadcast = fb::launchGroupBroadcast,
     .move = fb::launchMove,
     .moveBulk = fb::launchMoveBulk,
     .barrier = fb::launchBarrier,
@@ -1257,6 +1258,7 @@ const fb::KernelTable HOST_KERNELS = {
     .group = fb::host::groupAllReduce,
     .groupReduceScatter = fb::host::groupReduceScatter,
     .groupAllGather = fb::host::groupAllGather,
+    .groupBroadcast = fb::host::groupBroadcast,
     .move = fb::host::moveKernel,
     .moveBulk = fb::host::moveBulk,
     .barrier = fb::host::barrierKernel,
@@ -1838,6 +1840,13 @@ struct Communicator::ManySlot
 
 Communicator::ManySlot* Communicator::nextManySlot()
 {
+    // A child stages its tables in its parent's ring: same rank, same device,
+    // same thread.  So a child owns no slot and destroying it frees no memory
+    // (a cudaFree there would wait for the whole device, where a peer sharing
+    // it may spin in a parent collective that waits for this rank).
+    if (parent_ != nullptr) {
+        return parent_->nextManySlot();
+    }
     // table slot: pinned staging + device copy, recycled after its launch
     if (manySlots_.empty()) {
         manySlots_.resize(8);
@@ -1878,11 +1887,14 @@ struct SegBuild
 
 // This rank's share of items[0..n): the concatenation of all tensors (in
 // 16-byte vectors) is cut into nranks equal ranges; a segment is the
-// intersection of one tensor with this rank's range.
+// intersection of one tensor with this rank's range.  A broadcast list has
+// one buffer per item (recv; send is not read): its segments have sendOff ==
+// recvOff.
 static int buildGroupSegs(const Communicator& c,
                           const Communicator::GroupItem* items,
                           size_t nItems,
                           size_t esize,
+                          bool bcast,
                           SegBuild& out)
 {
     const int n = c.size();
@@ -1894,8 +1906,9 @@ static int buildGroupSegs(const Communicator& c,
         if (bytes == 0) {
             continue;
         }
-        if (!c.inHeap(items[i].send, bytes) || !c.inHeap(items[i].recv, bytes) ||
-            (((uintptr_t)items[i].send | (uintptr_t)items[i].recv) & 15)) {
+        const void* send = bcast ? items[i].recv : items[i].send;
+        if (!c.inHeap(send, bytes) || !c.inHeap(items[i].recv, bytes) ||
+            (((uintptr_t)send | (uintptr_t)items[i].recv) & 15)) {
             return FB_E_INVALID;
         }
         V += (bytes + 15) / 16;
@@ -1924,7 +1937,7 @@ static int buildGroupSegs(const Communicator& c,
             sg.nVec = (uint32_t)(std::min(v1, full) > v0 ? std::min(v1, full) - v0 : 0);
             sg.tailBytes = (tail != 0 && v1 == vecs) ? tail : 0;
             if (sg.nVec != 0 || sg.tailBytes != 0) {
-                sg.sendOff = c.offsetOf(items[i].send) + v0 * 16;
+                sg.sendOff = c.offsetOf(bcast ? items[i].recv : items[i].send) + v0 * 16;
                 sg.recvOff = c.offsetOf(items[i].recv) + v0 * 16;
                 sg.chunk0 = (uint32_t)chunks;
                 chunks += ((uint64_t)sg.nVec + (sg.tailBytes ? 1 : 0) + chunk - 1) / chunk;
@@ -2026,8 +2039,8 @@ static int buildSegs(const Communicator& c,
                      size_t esize,
                      SegBuild& out)
 {
-    if (kind == Communicator::GROUP_ALLREDUCE) {
-        return buildGroupSegs(c, items, nItems, esize, out);
+    if (kind == Communicator::GROUP_ALLREDUCE || kind == Communicator::GROUP_BROADCAST) {
+        return buildGroupSegs(c, items, nItems, esize, kind == Communicator::GROUP_BROADCAST, out);
     }
     return buildShardSegs(c, kind, items, nItems, esize, out);
 }
@@ -2045,12 +2058,8 @@ std::shared_ptr<Communicator::GroupPlan> Communicator::prepareGroup(
     int rcLocal = FB_OK;
     int& rc = rcOut ? *rcOut : rcLocal;
     rc = FB_OK;
-    if (parent_ != nullptr) {
-        rc = FB_E_UNSUPPORTED; // see subset()
-        return nullptr;
-    }
     const size_t esize = fbDtypeSize(dtype);
-    if (esize == 0 || kind < GROUP_ALLREDUCE || kind > GROUP_ALLGATHER) {
+    if (esize == 0 || kind < GROUP_ALLREDUCE || kind > GROUP_BROADCAST) {
         rc = FB_E_INVALID;
         return nullptr;
     }
@@ -2117,6 +2126,7 @@ static int groupGrid(const CommConfig& cfg, int nranks, uint64_t vecsPerRank)
 
 int Communicator::launchGroup(const GroupLaunch& l, GroupKind kind, int dtype, int op, int flags, cudaStream_t s)
 {
+    // (a broadcast passes its root as `op`)
     const int n = dev_.nranks;
     const bool ss = streamSync_ && !(flags & FB_FLAG_NOSYNC) && n > 1;
     fb::GroupArgs a;
@@ -2126,6 +2136,7 @@ int Communicator::launchGroup(const GroupLaunch& l, GroupKind kind, int dtype, i
     a.nSegs = l.nSegs;
     a.totalChunks = l.totalChunks;
     a.noSync = ((flags & FB_FLAG_NOSYNC) || ss || n == 1) ? 1 : 0;
+    a.root = kind == GROUP_BROADCAST ? op : 0;
     if (ss && streamBarrier(flags, s) != FB_OK) {
         return FB_E_CUDA;
     }
@@ -2135,6 +2146,8 @@ int Communicator::launchGroup(const GroupLaunch& l, GroupKind kind, int dtype, i
         e = k_->groupReduceScatter(a, dtype, op, blocks, cfg_.threads, s);
     } else if (kind == GROUP_ALLGATHER) {
         e = k_->groupAllGather(a, blocks, cfg_.threads, s);
+    } else if (kind == GROUP_BROADCAST) {
+        e = k_->groupBroadcast(a, blocks, cfg_.threads, s);
     } else {
         e = k_->group(a, dtype, op, blocks, cfg_.threads, s);
     }
@@ -2155,9 +2168,6 @@ int Communicator::launchGroup(const GroupLaunch& l, GroupKind kind, int dtype, i
 int Communicator::allReduceGroup(const GroupPlan& plan, int op, int flags, cudaStream_t s)
 {
     NvtxRange nvtxRange("fb::allReduceGroup");
-    if (parent_ != nullptr) {
-        return FB_E_UNSUPPORTED; // see subset()
-    }
     if (plan.kind != GROUP_ALLREDUCE) {
         return FB_E_INVALID;
     }
@@ -2179,9 +2189,6 @@ int Communicator::allReduceGroup(const GroupPlan& plan, int op, int flags, cudaS
 int Communicator::reduceScatterGroup(const GroupPlan& plan, int op, int flags, cudaStream_t s)
 {
     NvtxRange nvtxRange("fb::reduceScatterGroup");
-    if (parent_ != nullptr) {
-        return FB_E_UNSUPPORTED; // see subset()
-    }
     if (plan.kind != GROUP_REDUCE_SCATTER) {
         return FB_E_INVALID;
     }
@@ -2202,15 +2209,31 @@ int Communicator::reduceScatterGroup(const GroupPlan& plan, int op, int flags, c
 int Communicator::allGatherGroup(const GroupPlan& plan, int flags, cudaStream_t s)
 {
     NvtxRange nvtxRange("fb::allGatherGroup");
-    if (parent_ != nullptr) {
-        return FB_E_UNSUPPORTED; // see subset()
-    }
     if (plan.kind != GROUP_ALLGATHER) {
         return FB_E_INVALID;
     }
     bindDevice();
     for (const auto& l : plan.launches) {
         int rc = launchGroup(l, GROUP_ALLGATHER, plan.dtype, -1, flags, s);
+        if (rc != FB_OK) {
+            return rc;
+        }
+    }
+    return FB_OK;
+}
+
+int Communicator::broadcastGroup(const GroupPlan& plan, int root, int flags, cudaStream_t s)
+{
+    NvtxRange nvtxRange("fb::broadcastGroup");
+    if (plan.kind != GROUP_BROADCAST || root < 0 || root >= dev_.nranks) {
+        return FB_E_INVALID;
+    }
+    if (dev_.nranks == 1) {
+        return FB_OK; // the root's buffers already hold the result
+    }
+    bindDevice();
+    for (const auto& l : plan.launches) {
+        int rc = launchGroup(l, GROUP_BROADCAST, plan.dtype, root, flags, s);
         if (rc != FB_OK) {
             return rc;
         }
@@ -2246,6 +2269,18 @@ int Communicator::allGatherMany(const GroupItem* items, size_t nItems, int dtype
     return groupMany(GROUP_ALLGATHER, items, nItems, dtype, -1, flags, s);
 }
 
+int Communicator::broadcastMany(const GroupItem* items, size_t nItems, int root, int flags, cudaStream_t s)
+{
+    NvtxRange nvtxRange("fb::broadcastMany");
+    if (root < 0 || root >= dev_.nranks) {
+        return FB_E_INVALID;
+    }
+    if (dev_.nranks == 1) {
+        return FB_OK;
+    }
+    return groupMany(GROUP_BROADCAST, items, nItems, FB_U8, root, flags, s);
+}
+
 int Communicator::groupMany(GroupKind kind,
                             const GroupItem* items,
                             size_t nItems,
@@ -2254,16 +2289,13 @@ int Communicator::groupMany(GroupKind kind,
                             int flags,
                             cudaStream_t s)
 {
-    if (parent_ != nullptr) {
-        return FB_E_UNSUPPORTED; // see subset()
-    }
     const size_t esize = fbDtypeSize(dtype);
     if (esize == 0) {
         return FB_E_INVALID;
     }
-    // all-gather is a byte copy: any dtype has a kernel
+    // all-gather and broadcast are byte copies: any dtype has a kernel
     bool grouped = true;
-    if (kind != GROUP_ALLGATHER) {
+    if (kind != GROUP_ALLGATHER && kind != GROUP_BROADCAST) {
         const fb::ReduceLaunchers* L = fb::findReduceLaunchers(dtype, op);
         if (L == nullptr) {
             return FB_E_UNSUPPORTED;
@@ -2292,6 +2324,11 @@ int Communicator::groupMany(GroupKind kind,
                     r2 = allReduce(it.send, it.recv, it.count, dtype, op, FB_ALGO_AUTO, f, s);
                 } else if (bytes == 0) {
                     continue;
+                } else if (kind == GROUP_BROADCAST) {
+                    if (!inHeap(it.recv, bytes)) {
+                        f &= ~FB_FLAG_SYMMETRIC;
+                    }
+                    r2 = broadcast(it.recv, bytes, op, f, s);
                 } else if (kind == GROUP_REDUCE_SCATTER) {
                     if (!inHeap(it.send, bytes * n)) {
                         f &= ~FB_FLAG_SYMMETRIC;

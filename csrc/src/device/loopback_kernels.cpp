@@ -595,6 +595,37 @@ cudaError_t groupAllGather(const GroupArgs& a, int blocks, int, cudaStream_t)
     return cudaSuccess;
 }
 
+cudaError_t groupBroadcast(const GroupArgs& a, int blocks, int, cudaStream_t)
+{
+    const FbCommDev& c = a.comm;
+    // the kernel stores whole vectors at sendOff (== recvOff) on every rank
+    for (uint32_t si = 0; si < a.nSegs; si++) {
+        const GroupSeg& sg = a.segs[si];
+        if (sg.sendOff != sg.recvOff || (sg.nVec != 0 && ((uintptr_t)(c.heap[c.rank] + sg.sendOff) & 15))) {
+            return cudaErrorMisalignedAddress;
+        }
+    }
+    bool ok = true;
+    if (!a.noSync) {
+        ok = gridBarrier(c, blocks);
+    }
+    if (ok) {
+        for (uint32_t si = 0; si < a.nSegs; si++) {
+            const GroupSeg& sg = a.segs[si];
+            const uint8_t* src = c.heap[a.root] + sg.sendOff;
+            for (int p = 0; p < c.nranks; p++) {
+                if (p != a.root) {
+                    memcpy(c.heap[p] + sg.sendOff, src, (uint64_t)sg.nVec * 16 + sg.tailBytes);
+                }
+            }
+        }
+    }
+    if (!a.noSync) {
+        gridBarrier(c, blocks);
+    }
+    return cudaSuccess;
+}
+
 // ----------------------------------------------------------------- move ----
 // The CUDA kernels copy in W-byte words.  Every address they touch that way
 // must be W-aligned (a misaligned vector access is a device fault), and every

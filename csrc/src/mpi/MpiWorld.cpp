@@ -81,10 +81,12 @@ struct RankState
     // Non-blocking device collectives rotate over the communicator's
     // channels (every rank issues the same sequence => same channel)
     uint64_t deviceCollectiveSeq = 0;
-    // MPI_Iallreduce, MPI_Ireduce_scatter_block or MPI_Iallgather burst on
-    // symmetric device buffers: deferred and issued as ONE grouped kernel at
-    // the next wait (or any other device operation).  A burst has one key:
-    // (kind, communicator, dtype, op); all-gather bursts are bytes, no op.
+    // MPI_Iallreduce, MPI_Ireduce_scatter_block, MPI_Iallgather or MPI_Ibcast
+    // burst on symmetric device buffers: deferred and issued as ONE grouped
+    // kernel at the next wait (or any other device operation).  A burst has
+    // one key: (kind, communicator, dtype, op); all-gather and broadcast
+    // bursts are bytes, no op, and a broadcast's root takes the op's place.
+    // The communicator is the world's or a sub-communicator's child.
     faabric::device::Communicator::GroupKind groupKind = faabric::device::Communicator::GROUP_ALLREDUCE;
     std::shared_ptr<faabric::device::Communicator> groupComm;
     int groupDtype = -1;
@@ -418,7 +420,9 @@ void MpiWorld::initialiseRankFromMsg(faabric::Message& msg)
 bool MpiWorld::destroy()
 {
     SPDLOG_TRACE("Destroying MPI world {} (rank {})", id, tls.rank);
-    // Anything still outstanding on this rank is dropped
+    // Anything still outstanding on this rank is dropped, a deferred burst on
+    // MPI_COMM_WORLD included; only a burst on a sub-communicator's child is
+    // issued and waited first (below)
     if (!tls.requests.empty()) {
         SPDLOG_WARN("Destroying world {} with {} outstanding async requests on rank {}", id, tls.requests.size(), tls.rank);
     }
@@ -444,6 +448,15 @@ bool MpiWorld::destroy()
                 (*details)[std::string("mpi-device-algo-") + faabric::device::CommTuning::algoName(a)] =
                   (int)std::min<uint64_t>(st.algoCount[a], INT32_MAX);
             }
+        }
+    }
+    // A burst still deferred on a child is issued and waited, as at
+    // MPI_Comm_free: the child is released with the world's sub-communicators
+    if (!tls.groupItems.empty() && tls.groupComm != nullptr && tls.groupComm->isSubset()) {
+        try {
+            settleDeviceBurst(tls.groupComm);
+        } catch (const std::exception& e) {
+            SPDLOG_ERROR("Rank {}: pending device burst at world teardown failed: {}", tls.rank, e.what());
         }
     }
     tls.reset();
@@ -966,6 +979,9 @@ static void flushPendingGroup()
     } else if (tls.groupKind == Communicator::GROUP_ALLGATHER) {
         rc = comm->allGatherMany(items.data(), items.size(), tls.groupDtype, FB_FLAG_SYMMETRIC, s);
         what = "Grouped device all-gather";
+    } else if (tls.groupKind == Communicator::GROUP_BROADCAST) {
+        rc = comm->broadcastMany(items.data(), items.size(), tls.groupOp, FB_FLAG_SYMMETRIC, s);
+        what = "Grouped device broadcast";
     } else {
         rc = comm->allReduceMany(items.data(), items.size(), tls.groupDtype, tls.groupOp, FB_FLAG_SYMMETRIC, s);
         what = "Grouped device all-reduce";
@@ -1445,6 +1461,25 @@ bool MpiWorld::deviceAllToAll(const DeviceComm& comm, int rank, const uint8_t* s
     });
 }
 
+bool MpiWorld::deviceReduceScatter(const DeviceComm& comm,
+                                   int rank,
+                                   const uint8_t* send,
+                                   uint8_t* recv,
+                                   faabric_datatype_t* dt,
+                                   int recvCount,
+                                   faabric_op_t* op)
+{
+    const int fdt = fbDtypeFor(dt);
+    const int fop = fbOpFor(op);
+    if (fdt < 0 || fop < 0) {
+        return false;
+    }
+    return issueAndWait(comm, streamForRank(rank), deviceCollectives, [&](auto& c, cudaStream_t s) {
+        const size_t shard = (size_t)recvCount * dt->size;
+        return c.reduceScatter(send, recv, (size_t)recvCount, fdt, fop, symFlag(c, send, shard * (size_t)c.size()), s);
+    });
+}
+
 void MpiWorld::cacheDeviceComm(int rank)
 {
     if (!tls.cachedCommValid || tls.cachedCommRank != rank) {
@@ -1530,13 +1565,25 @@ static Placement placeCollective(const faabric::device::Communicator& c,
 int MpiWorld::iAllReduce(int rank, uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count, faabric_op_t* op)
 {
     checkRanksRange(0, rank);
+    cacheDeviceComm(rank);
+    return nbAllReduce(tls.cachedComm, rank, send, recv, dt, count, op, [&] { allReduce(rank, send, recv, dt, count, op); });
+}
+
+int MpiWorld::nbAllReduce(const DeviceComm& comm,
+                          int rank,
+                          const uint8_t* send,
+                          uint8_t* recv,
+                          faabric_datatype_t* dt,
+                          int count,
+                          faabric_op_t* op,
+                          const HostPath& host)
+{
     const size_t bytes = (size_t)count * dt->size;
     const int requestId = tls.nextRequestId++;
     AsyncRequest r = collectiveRequest(rank);
     const int fdt = fbDtypeFor(dt);
     const int fop = fbOpFor(op);
     cacheDeviceComm(rank);
-    const auto& comm = tls.cachedComm;
     // (a pair the kernels lack must not join a burst: the burst has no host path)
     if (bytes > 0 && deviceReducible(dt, op) && comm != nullptr) {
         const Placement at = placeCollective(*comm, groupIallreduce, send, bytes, recv, bytes, 0);
@@ -1569,7 +1616,7 @@ int MpiWorld::iAllReduce(int rank, uint8_t* send, uint8_t* recv, faabric_datatyp
         }
     }
     // Host path (or unsupported on the device): complete it now
-    allReduce(rank, send, recv, dt, count, op);
+    host();
     tls.requests[requestId] = std::move(r);
     return requestId;
 }
@@ -1581,19 +1628,34 @@ int MpiWorld::iReduceScatter(int rank,
                              int recvCount,
                              faabric_op_t* op)
 {
-    using faabric::device::Communicator;
     checkRanksRange(0, rank);
+    cacheDeviceComm(rank);
+    return nbReduceScatter(tls.cachedComm, rank, size, send, recv, dt, recvCount, op, [&] {
+        reduceScatter(rank, send, recv, dt, recvCount, op);
+    });
+}
+
+int MpiWorld::nbReduceScatter(const DeviceComm& comm,
+                              int rank,
+                              int members,
+                              const uint8_t* send,
+                              uint8_t* recv,
+                              faabric_datatype_t* dt,
+                              int recvCount,
+                              faabric_op_t* op,
+                              const HostPath& host)
+{
+    using faabric::device::Communicator;
     const size_t shard = (size_t)recvCount * dt->size;
     const int requestId = tls.nextRequestId++;
     AsyncRequest r = collectiveRequest(rank);
     const int fdt = fbDtypeFor(dt);
     const int fop = fbOpFor(op);
     cacheDeviceComm(rank);
-    const auto& comm = tls.cachedComm;
     // In place, the output overwrites input the peers are still reading: that
     // case (send == recv) runs the blocking call below
     if (shard > 0 && deviceReducible(dt, op) && comm != nullptr && send != recv) {
-        const Placement at = placeCollective(*comm, groupIallreduce, send, shard * size, recv, shard, shard);
+        const Placement at = placeCollective(*comm, groupIallreduce, send, shard * members, recv, shard, shard);
         if (at.grouped) {
             deferToGroup(Communicator::GROUP_REDUCE_SCATTER,
                          comm,
@@ -1607,13 +1669,13 @@ int MpiWorld::iReduceScatter(int rank,
         }
         void* s = tls.cachedStream0;
         if ((at.symmetric || isDevicePointer(send)) && issueDevice(*comm, s, deviceCollectives, [&](auto& c, cudaStream_t st) {
-                return c.reduceScatter(send, recv, (size_t)recvCount, fdt, fop, symFlag(c, send, shard * size), st);
+                return c.reduceScatter(send, recv, (size_t)recvCount, fdt, fop, symFlag(c, send, shard * members), st);
             })) {
             return recordDevice(requestId, std::move(r), comm, s);
         }
     }
     // Host buffers, in place, or unsupported on the device: complete it now
-    reduceScatter(rank, send, recv, dt, recvCount, op);
+    host();
     tls.requests[requestId] = std::move(r);
     return requestId;
 }
@@ -1626,16 +1688,28 @@ int MpiWorld::iAllGather(int rank,
                          faabric_datatype_t* recvType,
                          int recvCount)
 {
-    using faabric::device::Communicator;
     checkRanksRange(0, rank);
-    const size_t bytes = (size_t)sendCount * sendType->size;
+    cacheDeviceComm(rank);
+    return nbAllGather(tls.cachedComm, rank, size, send, recv, (size_t)sendCount * sendType->size, [&] {
+        allGather(rank, send, sendType, sendCount, recv, recvType, recvCount);
+    });
+}
+
+int MpiWorld::nbAllGather(const DeviceComm& comm,
+                          int rank,
+                          int members,
+                          const uint8_t* send,
+                          uint8_t* recv,
+                          size_t bytes,
+                          const HostPath& host)
+{
+    using faabric::device::Communicator;
     const int requestId = tls.nextRequestId++;
     AsyncRequest r = collectiveRequest(rank);
     cacheDeviceComm(rank);
-    const auto& comm = tls.cachedComm;
     if (bytes > 0 && comm != nullptr) {
-        const bool inPlace = send == recv + (size_t)rank * bytes;
-        const Placement at = placeCollective(*comm, groupIallreduce, send, bytes, recv, bytes * size, bytes);
+        const bool inPlace = send == recv + (size_t)comm->rank() * bytes;
+        const Placement at = placeCollective(*comm, groupIallreduce, send, bytes, recv, bytes * members, bytes);
         if (at.grouped) {
             // a byte copy: the burst's key is the communicator alone
             deferToGroup(Communicator::GROUP_ALLGATHER, comm, FB_U8, -1, { send, recv, bytes }, requestId, std::move(r), deviceCollectives);
@@ -1650,9 +1724,57 @@ int MpiWorld::iAllGather(int rank,
         }
     }
     // Host buffers, or unsupported on the device: complete it now
-    allGather(rank, send, sendType, sendCount, recv, recvType, recvCount);
+    host();
     tls.requests[requestId] = std::move(r);
     return requestId;
+}
+
+int MpiWorld::iBroadcast(int rank, int root, uint8_t* buffer, faabric_datatype_t* dt, int count)
+{
+    checkRanksRange(0, rank);
+    cacheDeviceComm(rank);
+    return nbBroadcast(tls.cachedComm, rank, root, buffer, (size_t)count * dt->size, [&] {
+        broadcast(root, rank, buffer, dt, count, MpiMessageType::BROADCAST);
+    });
+}
+
+int MpiWorld::nbBroadcast(const DeviceComm& comm, int rank, int root, uint8_t* buffer, size_t bytes, const HostPath& host)
+{
+    using faabric::device::Communicator;
+    const int requestId = tls.nextRequestId++;
+    AsyncRequest r = collectiveRequest(rank);
+    cacheDeviceComm(rank);
+    if (bytes > 0 && comm != nullptr) {
+        const Placement at = placeCollective(*comm, groupIallreduce, buffer, bytes, buffer, bytes, 0);
+        if (at.grouped) {
+            // a byte copy: the burst's key is (communicator, root); the root
+            // travels in the op slot of the key
+            deferToGroup(Communicator::GROUP_BROADCAST, comm, FB_U8, root, { buffer, buffer, bytes }, requestId, std::move(r),
+                         deviceCollectives);
+            return requestId;
+        }
+        void* s = tls.cachedStream0;
+        if ((at.symmetric || isDevicePointer(buffer)) && issueDevice(*comm, s, deviceCollectives, [&](auto& c, cudaStream_t st) {
+                return c.broadcast(buffer, bytes, root, symFlag(c, buffer, bytes), st);
+            })) {
+            return recordDevice(requestId, std::move(r), comm, s);
+        }
+    }
+    // Host buffers, or unsupported on the device: complete it now
+    host();
+    tls.requests[requestId] = std::move(r);
+    return requestId;
+}
+
+void MpiWorld::settleDeviceBurst(const DeviceComm& comm)
+{
+    if (comm == nullptr || tls.groupItems.empty() || tls.groupComm != comm) {
+        return;
+    }
+    void* stream = tls.groupStream;
+    flushPendingGroup();
+    cudaSetDevice(comm->device());
+    awaitDevice(*comm, stream);
 }
 
 void* MpiWorld::deviceAlloc(int rank, size_t bytes)

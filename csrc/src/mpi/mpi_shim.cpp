@@ -909,23 +909,38 @@ int MPI_Free_mem(void* base)
     return MPI_SUCCESS;
 }
 
+// The request handle of request `id` of this rank thread
+static int handOut(int id, MPI_Request* request)
+{
+    auto* r = new faabric_request_t{ id };
+    requestTable()[id] = r;
+    *request = r;
+    return MPI_SUCCESS;
+}
+
+// Non-blocking collectives on a sub-communicator run the world's rules over
+// the child device communicator; without one (host buffers, or no agreed
+// slot) the host path completes them at issue.  The child is looked up only
+// for device buffers: its slot agreement is collective.
 int MPI_Iallreduce(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, MPI_Comm comm, MPI_Request* request)
 {
     SPDLOG_TRACE("MPI - MPI_Iallreduce");
     if (refusedReduction(op, datatype)) {
         return MPI_ERR_OP;
     }
-    subCommOnly(comm, "MPI_Iallreduce");
-    int id = getExecutingWorld().iAllReduce(executingContext.getRank(),
-                                            (uint8_t*)resolveInPlace(sendbuf, recvbuf),
-                                            (uint8_t*)recvbuf,
-                                            datatype,
-                                            count,
-                                            op);
-    auto* r = new faabric_request_t{ id };
-    requestTable()[id] = r;
-    *request = r;
-    return MPI_SUCCESS;
+    MpiWorld& world = getExecutingWorld();
+    const int rank = executingContext.getRank();
+    const uint8_t* send = (const uint8_t*)resolveInPlace(sendbuf, recvbuf);
+    if (auto sub = subOf(comm)) {
+        auto dev = count > 0 && MpiWorld::isDevicePointer(send) && MpiWorld::deviceReducible(datatype, op)
+                     ? sub->deviceComm(world, rank)
+                     : nullptr;
+        return handOut(world.nbAllReduce(dev, rank, send, (uint8_t*)recvbuf, datatype, count, op, [&] {
+            sub->allReduce(world, rank, send, (uint8_t*)recvbuf, datatype, count, op);
+        }),
+                       request);
+    }
+    return handOut(world.iAllReduce(rank, (uint8_t*)send, (uint8_t*)recvbuf, datatype, count, op), request);
 }
 
 int MPI_Reduce_scatter_block(const void* sendbuf, void* recvbuf, int recvcount, MPI_Datatype datatype,
@@ -935,7 +950,11 @@ int MPI_Reduce_scatter_block(const void* sendbuf, void* recvbuf, int recvcount, 
     if (refusedReduction(op, datatype)) {
         return MPI_ERR_OP;
     }
-    subCommOnly(comm, "MPI_Reduce_scatter_block");
+    if (auto sub = subOf(comm)) {
+        sub->reduceScatter(getExecutingWorld(), executingContext.getRank(), (const uint8_t*)resolveInPlace(sendbuf, recvbuf),
+                           (uint8_t*)recvbuf, datatype, recvcount, op);
+        return MPI_SUCCESS;
+    }
     getExecutingWorld().reduceScatter(executingContext.getRank(), (uint8_t*)resolveInPlace(sendbuf, recvbuf),
                                       (uint8_t*)recvbuf, datatype, recvcount, op);
     return MPI_SUCCESS;
@@ -948,36 +967,64 @@ int MPI_Ireduce_scatter_block(const void* sendbuf, void* recvbuf, int recvcount,
     if (refusedReduction(op, datatype)) {
         return MPI_ERR_OP;
     }
-    subCommOnly(comm, "MPI_Ireduce_scatter_block");
-    int id = getExecutingWorld().iReduceScatter(executingContext.getRank(),
-                                                (uint8_t*)resolveInPlace(sendbuf, recvbuf),
-                                                (uint8_t*)recvbuf,
-                                                datatype,
-                                                recvcount,
-                                                op);
-    auto* r = new faabric_request_t{ id };
-    requestTable()[id] = r;
-    *request = r;
-    return MPI_SUCCESS;
+    MpiWorld& world = getExecutingWorld();
+    const int rank = executingContext.getRank();
+    const uint8_t* send = (const uint8_t*)resolveInPlace(sendbuf, recvbuf);
+    if (auto sub = subOf(comm)) {
+        auto dev = recvcount > 0 && MpiWorld::isDevicePointer(send) && MpiWorld::deviceReducible(datatype, op)
+                     ? sub->deviceComm(world, rank)
+                     : nullptr;
+        return handOut(world.nbReduceScatter(dev, rank, sub->size(), send, (uint8_t*)recvbuf, datatype, recvcount, op, [&] {
+            sub->reduceScatter(world, rank, send, (uint8_t*)recvbuf, datatype, recvcount, op);
+        }),
+                       request);
+    }
+    return handOut(world.iReduceScatter(rank, (uint8_t*)send, (uint8_t*)recvbuf, datatype, recvcount, op), request);
 }
 
 int MPI_Iallgather(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
                    MPI_Datatype recvtype, MPI_Comm comm, MPI_Request* request)
 {
     SPDLOG_TRACE("MPI - MPI_Iallgather");
-    subCommOnly(comm, "MPI_Iallgather");
-    int rank = executingContext.getRank();
+    MpiWorld& world = getExecutingWorld();
+    const int rank = executingContext.getRank();
+    auto sub = subOf(comm);
+    const int commRank = sub != nullptr ? sub->commRankOf(rank) : rank;
     const uint8_t* send = (const uint8_t*)sendbuf;
     if (sendbuf == MPI_IN_PLACE) {
-        send = (const uint8_t*)recvbuf + (size_t)rank * recvcount * recvtype->size;
+        send = (const uint8_t*)recvbuf + (size_t)commRank * recvcount * recvtype->size;
         sendcount = recvcount;
         sendtype = recvtype;
     }
-    int id = getExecutingWorld().iAllGather(rank, send, sendtype, sendcount, (uint8_t*)recvbuf, recvtype, recvcount);
-    auto* r = new faabric_request_t{ id };
-    requestTable()[id] = r;
-    *request = r;
-    return MPI_SUCCESS;
+    if (sub != nullptr) {
+        const size_t bytes = (size_t)sendcount * sendtype->size;
+        auto dev = bytes > 0 && MpiWorld::isDevicePointer(send) ? sub->deviceComm(world, rank) : nullptr;
+        return handOut(world.nbAllGather(dev, rank, sub->size(), send, (uint8_t*)recvbuf, bytes, [&] {
+            sub->allGather(world, rank, send, (uint8_t*)recvbuf, recvtype, recvcount);
+        }),
+                       request);
+    }
+    return handOut(world.iAllGather(rank, send, sendtype, sendcount, (uint8_t*)recvbuf, recvtype, recvcount), request);
+}
+
+int MPI_Ibcast(void* buffer, int count, MPI_Datatype datatype, int root, MPI_Comm comm, MPI_Request* request)
+{
+    SPDLOG_TRACE("MPI - MPI_Ibcast {} -> all", root);
+    MpiWorld& world = getExecutingWorld();
+    const int rank = executingContext.getRank();
+    auto sub = subOf(comm);
+    if (root < 0 || root >= (sub != nullptr ? sub->size() : world.getSize())) {
+        return MPI_ERR_ARG;
+    }
+    if (sub != nullptr) {
+        const size_t bytes = (size_t)count * datatype->size;
+        auto dev = bytes > 0 && MpiWorld::isDevicePointer(buffer) ? sub->deviceComm(world, rank) : nullptr;
+        return handOut(world.nbBroadcast(dev, rank, root, (uint8_t*)buffer, bytes, [&] {
+            sub->broadcast(world, rank, root, (uint8_t*)buffer, datatype, count);
+        }),
+                       request);
+    }
+    return handOut(world.iBroadcast(rank, root, (uint8_t*)buffer, datatype, count), request);
 }
 
 int MPI_Get_processor_name(char* name, int* resultlen)
@@ -1519,6 +1566,8 @@ int MPI_Comm_free(MPI_Comm* comm)
     if ((*comm)->id != FAABRIC_COMM_WORLD && (*comm)->id != FAABRIC_COMM_NULL) {
         // frees this rank's signal slot of the fused device path
         if (auto sub = getSubCommunicator((*comm)->id)) {
+            // a deferred burst on the child is issued and waited first
+            getExecutingWorld().settleDeviceBurst(sub->currentDevice(executingContext.getRank()));
             sub->releaseDevice(executingContext.getRank());
         }
         delete *comm;

@@ -245,6 +245,37 @@ void SubCommunicator::allToAll(MpiWorld& w, int me, const uint8_t* send, uint8_t
     }
 }
 
+void SubCommunicator::reduceScatter(MpiWorld& w,
+                                    int me,
+                                    const uint8_t* send,
+                                    uint8_t* recv,
+                                    faabric_datatype_t* dt,
+                                    int recvCount,
+                                    faabric_op_t* op)
+{
+    const size_t shard = (size_t)recvCount * dt->size;
+    if (shard > 0 && MpiWorld::isDevicePointer(send) && MpiWorld::deviceReducible(dt, op) &&
+        w.deviceReduceScatter(deviceComm(w, me), me, send, recv, dt, recvCount, op)) {
+        return;
+    }
+    // The rank-ordered fold of allReduce on host copies, then each member
+    // keeps its own block (staged first: in place, recv is also the input)
+    const int n = size();
+    HostStage in;
+    const uint8_t* src = in.in(send, shard * (size_t)n);
+    std::vector<uint8_t> full(shard * (size_t)n);
+    reduce(w, me, 0, src, full.data(), dt, recvCount * n, op);
+    broadcast(w, me, 0, full.data(), dt, recvCount * n);
+    copyBytes(recv, full.data() + (size_t)commRankOf(me) * shard, shard);
+}
+
+std::shared_ptr<faabric::device::Communicator> SubCommunicator::currentDevice(int me)
+{
+    std::lock_guard<std::mutex> lk(deviceMx);
+    auto it = device.find(me);
+    return it == device.end() ? nullptr : it->second.child;
+}
+
 std::shared_ptr<faabric::device::Communicator> SubCommunicator::deviceComm(MpiWorld& w, int me)
 {
     {

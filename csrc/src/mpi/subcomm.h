@@ -3,10 +3,12 @@
 // The reference declares these calls and throws "not implemented"
 // (tests/dist/mpi/mpi_native.cpp:686-735).  Here a sub-communicator is an
 // ordered list of world ranks.  On device buffers, MPI_Bcast, MPI_Reduce,
-// MPI_Allreduce, MPI_Scan, MPI_Gather, MPI_Scatter, MPI_Allgather and
-// MPI_Alltoall run the world's fused kernels over a child of the world device
-// communicator (Communicator::subset), on a signal slot the members agree on
-// at their first such call.  Everything else, and every call when no slot is
+// MPI_Allreduce, MPI_Scan, MPI_Gather, MPI_Scatter, MPI_Allgather,
+// MPI_Alltoall and MPI_Reduce_scatter_block run the world's fused kernels over
+// a child of the world device communicator (Communicator::subset), on a
+// signal slot the members agree on at their first such call; MPI_Ibcast,
+// MPI_Iallreduce, MPI_Ireduce_scatter_block and MPI_Iallgather take the
+// world's non-blocking rules (bursts included) over the same child.  Everything else, and every call when no slot is
 // free on all members, is built from the world's point-to-point layer, so it
 // works for ranks in one process (queues / peer memory) and across worker
 // processes (TCP) alike, on host and device buffers.
@@ -62,6 +64,11 @@ class SubCommunicator
 
     void allToAll(MpiWorld& w, int me, const uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count);
 
+    // MPI_Reduce_scatter_block: member r gets block r (recvCount elements) of
+    // the reduction of every member's send (size() * recvCount elements)
+    void reduceScatter(MpiWorld& w, int me, const uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int recvCount,
+                       faabric_op_t* op);
+
     // ---- fused device path ----
     // This rank's child of its world device communicator over the members
     // (null: this communicator stays on the host path).  The first call of a
@@ -69,8 +76,14 @@ class SubCommunicator
     // only from a collective that every member enters with device buffers.
     std::shared_ptr<faabric::device::Communicator> deviceComm(MpiWorld& w, int me);
 
+    // The child of world rank `me` if its slot agreement has run (null
+    // otherwise, or on the host path); never communicates
+    std::shared_ptr<faabric::device::Communicator> currentDevice(int me);
+
     // Releases the child of world rank `me` (MPI_Comm_free); later calls of
-    // that rank take the host path
+    // that rank take the host path.  The caller has completed the rank's
+    // collectives on the child, a deferred burst included
+    // (MpiWorld::settleDeviceBurst).
     void releaseDevice(int me);
 
   private:

@@ -410,35 +410,6 @@ TEST_CASE("loopback group shard: lists that cannot be grouped are refused, *Many
     }
 }
 
-TEST_CASE("loopback group shard: every grouped shard call is refused on a sub-communicator", "[loopback]")
-{
-    ShardGroup g(4);
-    int fails = g.run([&](int rank, Communicator& c) {
-        int32_t* a = (int32_t*)heapBytes(c, 1024);
-        int32_t* b = (int32_t*)heapBytes(c, 1024);
-        c.hostBarrier();
-        auto child = c.subset({ 0, 1, 2, 3 }, 0);
-        bool ok = child != nullptr;
-        Communicator::GroupItem it{ a, b, 16 };
-        int rc = FB_OK;
-        ok = ok && child->prepareGroup(&it, 1, FB_I32, &rc, Communicator::GROUP_REDUCE_SCATTER) == nullptr &&
-             rc == FB_E_UNSUPPORTED;
-        ok = ok && child->prepareGroup(&it, 1, FB_I32, &rc, Communicator::GROUP_ALLGATHER) == nullptr &&
-             rc == FB_E_UNSUPPORTED;
-        auto rsPlan = c.prepareGroup(&it, 1, FB_I32, &rc, Communicator::GROUP_REDUCE_SCATTER);
-        Communicator::GroupItem agIt{ a, b, 4 };
-        auto agPlan = c.prepareGroup(&agIt, 1, FB_I32, &rc, Communicator::GROUP_ALLGATHER);
-        ok = ok && rsPlan && agPlan;
-        ok = ok && child->reduceScatterGroup(*rsPlan, FB_OP_SUM, FB_FLAG_SYMMETRIC, nullptr) == FB_E_UNSUPPORTED;
-        ok = ok && child->allGatherGroup(*agPlan, FB_FLAG_SYMMETRIC, nullptr) == FB_E_UNSUPPORTED;
-        ok = ok && child->reduceScatterMany(&it, 1, FB_I32, FB_OP_SUM, FB_FLAG_SYMMETRIC, nullptr) == FB_E_UNSUPPORTED;
-        ok = ok && child->allGatherMany(&agIt, 1, FB_I32, FB_FLAG_SYMMETRIC, nullptr) == FB_E_UNSUPPORTED;
-        child.reset();
-        return ok;
-    });
-    REQUIRE_EQ(fails, 0);
-}
-
 namespace {
 void runGroupShardMpi(const std::string& name, int worldSize)
 {

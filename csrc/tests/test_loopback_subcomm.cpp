@@ -104,69 +104,6 @@ TEST_CASE("loopback subset: slot masks before and after release", "[loopback]")
     REQUIRE_EQ(comms[0]->freeSubsetSlots(), ALL_SLOTS);
 }
 
-TEST_CASE("loopback subset: child ranks, sizes, heap addressing and refused calls", "[loopback]")
-{
-    auto comms = loopGroup(4);
-    const uint64_t off = comms[0]->alloc(4096);
-    for (int r = 1; r < 4; r++) {
-        REQUIRE_EQ(comms[r]->alloc(4096), off);
-    }
-    const std::vector<int> members{ 3, 0, 2 };
-    auto child = comms[2]->subset(members, 5);
-    REQUIRE(child != nullptr);
-    REQUIRE(child->isSubset() && !comms[2]->isSubset());
-    REQUIRE_EQ(child->rank(), 2);
-    REQUIRE_EQ(child->size(), 3);
-    REQUIRE(!child->hasMulticast());
-    for (int i = 0; i < 3; i++) {
-        REQUIRE(child->heapPtr(off, i) == comms[2]->heapPtr(off, members[i]));
-    }
-    REQUIRE(child->heapPtr(off) == comms[2]->heapPtr(off));
-    REQUIRE(child->inHeap(comms[2]->heapPtr(off), 4096));
-    REQUIRE_EQ(child->offsetOf(comms[2]->heapPtr(off)), off);
-    // slot 5 of member i is the child's pad of child rank i
-    const auto& d = child->devStruct();
-    for (int i = 0; i < 3; i++) {
-        REQUIRE(d.sig[i] == comms[members[i]]->devStruct().sig[members[i]] + 6 * FB_SIG_TOTAL_WORDS);
-    }
-    uint8_t* buf = comms[2]->heapPtr(off);
-    uint32_t word = 0;
-    REQUIRE_EQ(child->send(buf, 16, 0, nullptr), FB_E_UNSUPPORTED);
-    REQUIRE_EQ(child->recv(buf, 16, 0, nullptr), FB_E_UNSUPPORTED);
-    REQUIRE_EQ(child->sendRecv(buf, 16, 0, buf, 16, 0, nullptr), FB_E_UNSUPPORTED);
-    REQUIRE_EQ(child->putSignal(buf, off, 16, 0, 0, 1, nullptr), FB_E_UNSUPPORTED);
-    REQUIRE_EQ(child->waitSignal(0, 1, nullptr), FB_E_UNSUPPORTED);
-    REQUIRE_EQ(child->accumulate(buf, off, 1, FB_I32, FB_OP_SUM, 0, nullptr, nullptr), FB_E_UNSUPPORTED);
-    REQUIRE_EQ(child->compareAndSwap(&word, &word, &word, off, FB_I32, 0, nullptr), FB_E_UNSUPPORTED);
-    Communicator::GroupItem item{ buf, buf, 4 };
-    int rc = FB_OK;
-    REQUIRE(child->prepareGroup(&item, 1, FB_I32, &rc) == nullptr);
-    REQUIRE_EQ(rc, FB_E_UNSUPPORTED);
-    REQUIRE_EQ(child->allReduceMany(&item, 1, FB_I32, FB_OP_SUM, FB_FLAG_SYMMETRIC, nullptr), FB_E_UNSUPPORTED);
-    auto plan = comms[2]->prepareGroup(&item, 1, FB_I32, &rc);
-    REQUIRE(plan != nullptr);
-    REQUIRE_EQ(child->allReduceGroup(*plan, FB_OP_SUM, FB_FLAG_SYMMETRIC, nullptr), FB_E_UNSUPPORTED);
-    REQUIRE_EQ(child->hostBarrier(), FB_E_UNSUPPORTED);
-    REQUIRE_EQ(child->allReduce(buf, buf, 4, FB_I32, FB_OP_SUM, FB_ALGO_LL, FB_FLAG_SYMMETRIC, nullptr), FB_E_UNSUPPORTED);
-    REQUIRE_EQ(child->allReduce(buf, buf, 4, FB_I32, FB_OP_SUM, FB_ALGO_NVLS, FB_FLAG_SYMMETRIC, nullptr), FB_E_UNSUPPORTED);
-    bool threw = false;
-    try {
-        child->alloc(256);
-    } catch (const std::logic_error&) {
-        threw = true;
-    }
-    REQUIRE(threw);
-    threw = false;
-    try {
-        child->free(off);
-    } catch (const std::logic_error&) {
-        threw = true;
-    }
-    REQUIRE(threw);
-    // nothing was launched by the refused calls
-    REQUIRE_EQ(child->stats().launches, 0u);
-}
-
 TEST_CASE("loopback subset: fused collectives over members in child order", "[loopback]")
 {
     auto comms = loopGroup(8);

@@ -131,6 +131,9 @@ def load():
     _sig(lib, "fb_group_all_gather", i32, [vp, vp, i32, vp])
     _sig(lib, "fb_reduce_scatter_many", i32, [vp, i32, vpp, vpp, u64p, i32, i32, i32, vp])
     _sig(lib, "fb_all_gather_many", i32, [vp, i32, vpp, vpp, u64p, i32, i32, vp])
+    _sig(lib, "fb_group_prepare_broadcast", vp, [vp, i32, vpp, u64p])
+    _sig(lib, "fb_group_broadcast", i32, [vp, vp, i32, i32, vp])
+    _sig(lib, "fb_broadcast_many", i32, [vp, i32, vpp, u64p, i32, i32, vp])
     _sig(lib, "fb_put_signal", i32, [vp, vp, u64, u64, i32, i32, i32, vp])
     _sig(lib, "fb_wait_signal", i32, [vp, i32, u32, vp])
     _sig(lib, "fb_accumulate", i32, [vp, vp, u64, u64, i32, i32, i32, vp, vp])

@@ -568,6 +568,49 @@ class Communicator:
         rc = self._lib.fb_all_gather_many(self._h, n, sp, rp, cnt, dt, f, self._stream(stream))
         self._check(rc, "all_gather_many")
 
+    # ------------------------------------------------ grouped broadcast
+    def _bcast_arrays(self, what, bufs, root):
+        """(n, buffer ptrs, byte counts) of a broadcast group; raises before
+        any native call for an empty list, a root outside the communicator or
+        a tensor that is not contiguous."""
+        if not bufs:
+            raise CommError(f"{what}: need a non-empty list")
+        if not 0 <= int(root) < self.size:
+            raise CommError(f"{what}: root {root} outside a communicator of {self.size}")
+        for i, t in enumerate(bufs):
+            if not t.is_contiguous():
+                raise CommError(f"{what}: item {i} must be contiguous")
+        n = len(bufs)
+        bp = (C.c_void_p * n)(*[t.data_ptr() for t in bufs])
+        nb = (C.c_uint64 * n)(*[t.numel() * t.element_size() for t in bufs])
+        return n, bp, nb
+
+    def prepare_broadcast_group(self, bufs) -> "GroupPlan":
+        """Plan ONE launch that broadcasts every tensor of ``bufs`` (MPI_Bcast
+        per tensor, any dtype and length) from the root given to
+        :meth:`broadcast_group`.  Tensors live in the symmetric heap at 16-byte
+        aligned addresses; call collectively with the same list."""
+        n, bp, nb = self._bcast_arrays("prepare_broadcast_group", bufs, 0)
+        h = self._lib.fb_group_prepare_broadcast(self._h, n, bp, nb)
+        if not h:
+            raise CommError(f"prepare_broadcast_group failed [{_lib.last_error()}]")
+        return GroupPlan(self, h, n, sum(nb))
+
+    def broadcast_group(self, plan: "GroupPlan", root=0, stream=None, channel=0, flags=FLAG_SYMMETRIC):
+        rc = self._lib.fb_group_broadcast(
+            self._h, plan._h, int(root), flags | ((channel & 0xF) << 8), self._stream(stream)
+        )
+        self._check(rc, "broadcast_group")
+
+    def broadcast_many(self, bufs, root=0, stream=None, channel=0):
+        """Transient variant of :meth:`prepare_broadcast_group` +
+        :meth:`broadcast_group`; lists that cannot be grouped run one
+        :meth:`broadcast` per tensor."""
+        n, bp, nb = self._bcast_arrays("broadcast_many", bufs, root)
+        f = self._sym(*bufs) | ((channel & 0xF) << 8)
+        rc = self._lib.fb_broadcast_many(self._h, n, bp, nb, int(root), f, self._stream(stream))
+        self._check(rc, "broadcast_many")
+
     def send_recv(self, send_buf, dst, recv_buf, src, stream=None):
         rc = self._lib.fb_sendrecv(
             self._h,
@@ -838,8 +881,8 @@ class Communicator:
 
 
 class GroupPlan:
-    """Device-resident segment tables of a grouped all-reduce, reduce-scatter
-    or all-gather."""
+    """Device-resident segment tables of a grouped all-reduce, reduce-scatter,
+    all-gather or broadcast."""
 
     def __init__(self, comm: Communicator, handle, n_tensors: int, nbytes: int):
         self._comm = comm
