@@ -28,6 +28,7 @@
 #include "../tests/mpi_rma_accumulate_batch_body.h"
 #include "../tests/mpi_rma_request_body.h"
 #include "../tests/mpi_subcomm_device_body.h"
+#include "../tests/mpi_group_alltoall_body.h"
 #include "../tests/mpi_group_subcomm_body.h"
 
 #include <cuda_runtime.h>
@@ -823,6 +824,125 @@ static void registerFunctions()
             msg.set_outputdata(why);
         }
         return rc;
+    });
+
+    // MPI_Ialltoall bursts on the world and on sub-communicators
+    // (mpi_group_alltoall_body.h)
+    mpiFunction("group-alltoall", [](int rank, int size, faabric::Message& msg) {
+        std::string why;
+        int rc = group_alltoall::body(rank, size, msg.mpiworldid(), true, &why);
+        if (rc != 0) {
+            SPDLOG_ERROR("group-alltoall: {}", why);
+            msg.set_outputdata(why);
+        }
+        return rc;
+    });
+
+    // A list of tensors exchanged on the world per step, each one send and one
+    // recv buffer in the symmetric heap.  Input:
+    // "<mode>;<steps>;<bytes0,bytes1,...>" with bytes_i the send bytes of
+    // tensor i on one rank (a multiple of 16 * size) and mode
+    //   alltoall   one MPI_Alltoall per tensor
+    //   ialltoall  MPI_Ialltoall per tensor + MPI_Waitall
+    // Rank 0 reports {"ms_per_step", "us_per_call", "launches_per_step",
+    // "wait_ms_per_step"}: the launches counted on its world device
+    // communicator, and the part of a step spent in MPI_Waitall (where a burst
+    // is issued and completed; 0 for the blocking calls).
+    mpiFunction("bench-group-alltoall", [](int rank, int size, faabric::Message& msg) {
+        std::vector<std::string> f;
+        std::string cur;
+        for (char c : msg.inputdata() + ";") {
+            if (c == ';') {
+                f.push_back(cur);
+                cur.clear();
+            } else {
+                cur += c;
+            }
+        }
+        EXPECT(f.size() >= 3 && size >= 2);
+        const std::string mode = f[0];
+        const int steps = std::stoi(f[1]);
+        std::vector<size_t> bytes;
+        for (size_t b = 0, e; b < f[2].size(); b = e + 1) {
+            e = f[2].find(',', b);
+            if (e == std::string::npos) {
+                e = f[2].size();
+            }
+            bytes.push_back(std::stoull(f[2].substr(b, e - b)));
+        }
+        size_t total = 0;
+        std::vector<size_t> offs;
+        for (size_t b : bytes) {
+            EXPECT(b % (16 * (size_t)size) == 0);
+            offs.push_back(total);
+            total += b;
+        }
+        faabric::mpi::MpiWorld& world = faabric::mpi::getMpiWorldRegistry().getWorld(msg.mpiworldid());
+        uint8_t* send = nullptr;
+        uint8_t* recv = nullptr;
+        EXPECT(MPI_Alloc_mem(total, MPI_INFO_FAABRIC_DEVICE, &send) == MPI_SUCCESS);
+        EXPECT(MPI_Alloc_mem(total, MPI_INFO_FAABRIC_DEVICE, &recv) == MPI_SUCCESS);
+        // (copies from host memory, which wait for this rank only: a device-wide
+        // synchronise could wait for a peer's collective that waits for us)
+        std::vector<uint8_t> init(total, (uint8_t)(rank + 1));
+        cudaMemcpy(send, init.data(), total, cudaMemcpyHostToDevice);
+        std::fill(init.begin(), init.end(), 0);
+        cudaMemcpy(recv, init.data(), total, cudaMemcpyHostToDevice);
+        MPI_Barrier(MPI_COMM_WORLD);
+        const int n = (int)bytes.size();
+        std::vector<MPI_Request> reqs(n);
+        double waitMs = 0;
+        auto step = [&]() -> int {
+            for (int i = 0; i < n; i++) {
+                const int block = (int)(bytes[i] / size);
+                if (mode == "alltoall") {
+                    EXPECT(MPI_Alltoall(send + offs[i], block, MPI_BYTE, recv + offs[i], block, MPI_BYTE, MPI_COMM_WORLD) ==
+                           MPI_SUCCESS);
+                } else {
+                    EXPECT(MPI_Ialltoall(send + offs[i], block, MPI_BYTE, recv + offs[i], block, MPI_BYTE, MPI_COMM_WORLD,
+                                         &reqs[i]) == MPI_SUCCESS);
+                }
+            }
+            if (mode == "ialltoall") {
+                auto w0 = std::chrono::steady_clock::now();
+                EXPECT(MPI_Waitall(n, reqs.data(), MPI_STATUSES_IGNORE) == MPI_SUCCESS);
+                waitMs += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - w0).count();
+            }
+            return 0;
+        };
+        for (int i = 0; i < 3; i++) {
+            EXPECT(step() == 0);
+        }
+        auto dev = world.getDeviceComm(rank);
+        EXPECT(dev != nullptr);
+        MPI_Barrier(MPI_COMM_WORLD);
+        waitMs = 0;
+        const uint64_t l0 = dev->stats().launches;
+        auto t0 = std::chrono::steady_clock::now();
+        for (int i = 0; i < steps; i++) {
+            EXPECT(step() == 0);
+        }
+        const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count() / steps;
+        const double launches = (double)(dev->stats().launches - l0) / steps;
+        MPI_Barrier(MPI_COMM_WORLD);
+        // block p of every recv holds rank p's fill byte
+        std::vector<uint8_t> back(total);
+        cudaMemcpy(back.data(), recv, total, cudaMemcpyDeviceToHost);
+        for (int i = 0; i < n; i++) {
+            const size_t block = bytes[i] / size;
+            for (int p = 0; p < size; p++) {
+                EXPECT(back[offs[i] + p * block] == p + 1 && back[offs[i] + (p + 1) * block - 1] == p + 1);
+            }
+        }
+        if (rank == 0) {
+            msg.set_outputdata("{\"ms_per_step\": " + std::to_string(ms) + ", \"us_per_call\": " +
+                               std::to_string(ms * 1000.0 / n) + ", \"launches_per_step\": " + std::to_string(launches) +
+                               ", \"wait_ms_per_step\": " + std::to_string(waitMs / steps) +
+                               "}");
+        }
+        MPI_Free_mem(recv);
+        MPI_Free_mem(send);
+        return 0;
     });
 
     // A list of float32 tensors in one symmetric-heap buffer, each 16-byte

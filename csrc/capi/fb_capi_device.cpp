@@ -593,7 +593,7 @@ void* fb_group_prepare(void* h,
     FB_CATCH(nullptr)
 }
 
-// ---- grouped reduce-scatter / all-gather: counts are per-rank counts ----
+// ---- grouped reduce-scatter / all-gather / all-to-all: counts are per-rank counts ----
 static void* groupPrepareKind(void* h,
                               int n,
                               const void* const* send,
@@ -636,6 +636,16 @@ void* fb_group_prepare_all_gather(void* h,
     return groupPrepareKind(h, n, send, recv, counts, dtype, Communicator::GROUP_ALLGATHER);
 }
 
+void* fb_group_prepare_all_to_all(void* h,
+                                  int n,
+                                  const void* const* send,
+                                  void* const* recv,
+                                  const uint64_t* counts,
+                                  int dtype)
+{
+    return groupPrepareKind(h, n, send, recv, counts, dtype, Communicator::GROUP_ALLTOALL);
+}
+
 int fb_group_reduce_scatter(void* h, void* plan, int op, int flags, void* stream)
 {
     if (plan == nullptr) {
@@ -650,6 +660,14 @@ int fb_group_all_gather(void* h, void* plan, int flags, void* stream)
         return FB_E_INVALID;
     }
     return COMM(h)->allGatherGroup(*((FbGroupPlanHandle*)plan)->plan, flags, (cudaStream_t)stream);
+}
+
+int fb_group_all_to_all(void* h, void* plan, int flags, void* stream)
+{
+    if (plan == nullptr) {
+        return FB_E_INVALID;
+    }
+    return COMM(h)->allToAllGroup(*((FbGroupPlanHandle*)plan)->plan, flags, (cudaStream_t)stream);
 }
 
 int fb_reduce_scatter_many(void* h,
@@ -680,6 +698,21 @@ int fb_all_gather_many(void* h,
     FB_TRY
     auto items = groupItems(n, send, recv, counts);
     return COMM(h)->allGatherMany(items.data(), items.size(), dtype, flags, (cudaStream_t)stream);
+    FB_CATCH(FB_E_CUDA)
+}
+
+int fb_all_to_all_many(void* h,
+                       int n,
+                       const void* const* send,
+                       void* const* recv,
+                       const uint64_t* counts,
+                       int dtype,
+                       int flags,
+                       void* stream)
+{
+    FB_TRY
+    auto items = groupItems(n, send, recv, counts);
+    return COMM(h)->allToAllMany(items.data(), items.size(), dtype, flags, (cudaStream_t)stream);
     FB_CATCH(FB_E_CUDA)
 }
 

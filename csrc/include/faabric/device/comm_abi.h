@@ -72,7 +72,8 @@ extern "C" {
 // in-kernel flag barriers, the per-block epoch words, which only the owner
 // writes, and the stream-ordered barrier: signalPeers + a wait per peer).  The
 // grouped kernels (groupAllReduceKernel, groupReduceScatterKernel,
-// groupAllGatherKernel, groupBroadcastKernel) keep it too: they write a pad
+// groupAllGatherKernel, groupBroadcastKernel, groupAllToAllKernel) keep it
+// too: they write a pad
 // only through the entry and exit BlockBarrier syncs, each of which awaits
 // the flag of every peer it signals, or run between two stream-ordered
 // barriers with no in-kernel synchronisation at all.  So

@@ -277,17 +277,21 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     //   GROUP_BROADCAST: recv holds count elements (send is not read); every
     //     rank's recv gets the root's (MPI_Bcast per item; a byte copy, any
     //     dtype, any length).  Cut into equal ranges like the all-reduce.
-    // Shard kinds group an item only if send and recv are in the symmetric
-    // heap and 16-byte aligned, count*esize is a multiple of 16, and recv
-    // overlaps no send of the group on this rank.  The one exception is the
-    // in-place all-gather, send == recv + rank*count*esize.  Items with count
-    // 0 are skipped.
+    //   GROUP_ALLTOALL: send and recv hold size()*count elements each; block
+    //     r of recv on rank p gets block p of send on rank r (MPI_Alltoall
+    //     per item; a byte copy, any dtype)
+    // Shard kinds (all but GROUP_ALLREDUCE and GROUP_BROADCAST) group an item
+    // only if send and recv are in the symmetric heap and 16-byte aligned,
+    // count*esize is a multiple of 16, and recv overlaps no send of the group
+    // on this rank.  The one exception is the in-place all-gather, send ==
+    // recv + rank*count*esize.  Items with count 0 are skipped.
     enum GroupKind
     {
         GROUP_ALLREDUCE = 0,
         GROUP_REDUCE_SCATTER = 1,
         GROUP_ALLGATHER = 2,
-        GROUP_BROADCAST = 3
+        GROUP_BROADCAST = 3,
+        GROUP_ALLTOALL = 4
     };
     // Builds (and uploads) this rank's segment tables.  Collective: every rank
     // must pass the same list (same offsets, same counts).  Returns null and
@@ -306,6 +310,9 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     // range: FB_E_INVALID).  The root's buffers are only read.  On a
     // one-member communicator nothing is launched.
     int broadcastGroup(const GroupPlan& plan, int root, int flags, cudaStream_t s);
+    // A GROUP_ALLTOALL plan.  On a one-member communicator it is launched as
+    // a local copy.
+    int allToAllGroup(const GroupPlan& plan, int flags, cudaStream_t s);
     // prepare + launch for a transient list (MPI_Iallreduce bursts); falls back
     // to per-item allReduce calls when the list cannot be grouped
     int allReduceMany(const GroupItem* items,
@@ -336,6 +343,9 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     // per-item broadcast calls.  Root out of range: FB_E_INVALID; one member:
     // nothing is launched.
     int broadcastMany(const GroupItem* items, size_t nItems, int root, int flags, cudaStream_t s);
+    // MPI_Ialltoall bursts (items[i].count elements per block): falls back to
+    // per-item allToAll calls for a list that cannot be grouped
+    int allToAllMany(const GroupItem* items, size_t nItems, int dtype, int flags, cudaStream_t s);
     static size_t groupPlanLaunches(const GroupPlan& plan);
 
     // ---- point to point (per-pair FIFO; no kernel ever spins on a peer) ----

@@ -350,6 +350,10 @@ extern "C"
                        MPI_Datatype recvtype, MPI_Comm comm, MPI_Request* request);
     // A root outside the communicator gives MPI_ERR_ARG
     int MPI_Ibcast(void* buffer, int count, MPI_Datatype datatype, int root, MPI_Comm comm, MPI_Request* request);
+    // MPI_IN_PLACE, or a send block of another byte size than the receive
+    // block, gives MPI_ERR_ARG
+    int MPI_Ialltoall(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                      MPI_Datatype recvtype, MPI_Comm comm, MPI_Request* request);
     int MPI_Free_mem(void* base);
     int MPI_Win_create(void* base, MPI_Aint size, int disp_unit, MPI_Info info, MPI_Comm comm, MPI_Win* win);
     int MPI_Win_allocate_shared(MPI_Aint size, int disp_unit, MPI_Info info, MPI_Comm comm, void* baseptr, MPI_Win* win);

@@ -346,6 +346,19 @@ class MpiWorld
     // at issue.
     int iBroadcast(int rank, int root, uint8_t* buffer, faabric_datatype_t* dt, int count);
 
+    // MPI_Ialltoall on the world, by the same rules: symmetric, 16-byte
+    // aligned device buffers whose block is a multiple of 16 bytes join a
+    // burst keyed by (kind, communicator), issued as one grouped launch at
+    // the next wait; other device buffers run one all-to-all at issue; host
+    // buffers complete at issue.
+    int iAllToAll(int rank,
+                  uint8_t* sendBuffer,
+                  faabric_datatype_t* sendType,
+                  int sendCount,
+                  uint8_t* recvBuffer,
+                  faabric_datatype_t* recvType,
+                  int recvCount);
+
     // Symmetric-heap allocation for MPI_Alloc_mem (collective: every rank
     // must allocate the same sizes in the same order)
     void* deviceAlloc(int rank, size_t bytes);
@@ -590,6 +603,10 @@ class MpiWorld
                     size_t bytes, const HostPath& host);
     // `root` is a rank of `comm`'s communicator (the caller checked it)
     int nbBroadcast(const DeviceComm& comm, int rank, int root, uint8_t* buffer, size_t bytes, const HostPath& host);
+    // `bytes` per block; send and recv hold `members` blocks each and do not
+    // alias (the caller refused MPI_IN_PLACE)
+    int nbAllToAll(const DeviceComm& comm, int rank, int members, const uint8_t* send, uint8_t* recv, size_t bytes,
+                   const HostPath& host);
     // Issues this rank thread's pending burst if it is keyed to `comm`, and
     // waits for it (before `comm` is released: MPI_Comm_free)
     void settleDeviceBurst(const DeviceComm& comm);

@@ -472,6 +472,119 @@ cudaError_t launchGroupBroadcast(const GroupArgs& a,
 }
 
 // ----------------------------------------------------------------------------
+// Grouped all-to-all: one MPI_Alltoall per tensor, all in ONE launch per rank
+// (launch_api.h).  A push: a chunk covers the same vectors of every block of
+// this rank's send; block p goes to this rank's block of peer p's output (the
+// own block is a local copy in the same loop).  Peers are visited from
+// `rank` on, so at each step the ranks store to distinct peers.  Entry
+// barrier: every peer's output may be overwritten.  Exit barrier: every push
+// into this rank's output has landed.  Dtype-free: a byte copy.
+// ----------------------------------------------------------------------------
+template<int NR>
+__global__ void __launch_bounds__(512, 1) groupAllToAllKernel(const GroupArgs a)
+{
+    extern __shared__ __align__(16) uint8_t sGroupRaw[];
+    GroupSeg* sSegs = reinterpret_cast<GroupSeg*>(sGroupRaw);
+    const FbCommDev& c = a.comm;
+    const int n = (NR > 0) ? NR : c.nranks;
+    const int rank = c.rank;
+    BlockBarrier bar;
+    const bool ok = groupEnter(a, sSegs, bar);
+
+    if (ok && a.nSegs > 0) {
+        constexpr int UNROLL = (NR == 8) ? 2 : (NR == 1 ? 8 : 4);
+        constexpr uint32_t CHUNK = 32u * UNROLL;
+        const uint32_t lane = threadIdx.x & 31;
+        const uint32_t warpsPerCta = blockDim.x >> 5;
+        const uint32_t warpStride = gridDim.x * warpsPerCta;
+        const uint8_t* const in = c.heap[rank];
+        int cur = 0;
+        for (uint32_t ch = blockIdx.x * warpsPerCta + (threadIdx.x >> 5);
+             ch < a.totalChunks;
+             ch += warpStride) {
+            cur = groupSegOf(sSegs, a.nSegs, cur, ch);
+            const GroupSeg sg = sSegs[cur];
+            const uint32_t v0 = (ch - sg.chunk0) * CHUNK;
+            const uint64_t block = (uint64_t)sg.nVec * 16;
+            const uint8_t* const src = in + sg.sendOff + (uint64_t)v0 * 16;
+            const uint64_t rOff = sg.recvOff + (uint64_t)v0 * 16;
+            const uint32_t rem = sg.nVec - v0;
+            if constexpr (NR > 0) {
+                if (rem >= CHUNK) {
+                    // every peer's vectors in flight before the first store
+                    Vec16 v[NR][UNROLL];
+#pragma unroll
+                    for (int q = 0; q < NR; q++) {
+                        const int p = (rank + q) & (NR - 1);
+#pragma unroll
+                        for (int u = 0; u < UNROLL; u++) {
+                            v[q][u] = ldVecStream(src + (uint64_t)p * block + (uint64_t)(u * 32 + lane) * 16);
+                        }
+                    }
+#pragma unroll
+                    for (int q = 0; q < NR; q++) {
+                        const int p = (rank + q) & (NR - 1);
+#pragma unroll
+                        for (int u = 0; u < UNROLL; u++) {
+                            stVec(c.heap[p] + rOff + (uint64_t)(u * 32 + lane) * 16, v[q][u]);
+                        }
+                    }
+                    continue;
+                }
+            }
+            // any world size, and the ragged end of a block (or a whole small
+            // one): one peer at a time
+            for (int q = 0; q < n; q++) {
+                const int p = (rank + q < n) ? rank + q : rank + q - n;
+                const uint8_t* const s = src + (uint64_t)p * block;
+                uint8_t* const d = c.heap[p] + rOff;
+                if (rem >= CHUNK) {
+                    Vec16 v[UNROLL];
+#pragma unroll
+                    for (int u = 0; u < UNROLL; u++) {
+                        v[u] = ldVecStream(s + (uint64_t)(u * 32 + lane) * 16);
+                    }
+#pragma unroll
+                    for (int u = 0; u < UNROLL; u++) {
+                        stVec(d + (uint64_t)(u * 32 + lane) * 16, v[u]);
+                    }
+                } else {
+#pragma unroll
+                    for (int u = 0; u < UNROLL; u++) {
+                        const uint32_t i = (uint32_t)u * 32 + lane;
+                        if (i < rem) {
+                            stVec(d + (uint64_t)i * 16, ldVecStream(s + (uint64_t)i * 16));
+                        }
+                    }
+                }
+            }
+        }
+    }
+    groupExit(a, bar);
+}
+
+cudaError_t launchGroupAllToAll(const GroupArgs& a,
+                                int blocks,
+                                int threads,
+                                cudaStream_t s)
+{
+    const size_t smem = (size_t)a.nSegs * sizeof(GroupSeg);
+    const int n = a.comm.nranks;
+    if (n == 1) {
+        groupAllToAllKernel<1><<<blocks, threads, smem, s>>>(a);
+    } else if (n == 2) {
+        groupAllToAllKernel<2><<<blocks, threads, smem, s>>>(a);
+    } else if (n == 4) {
+        groupAllToAllKernel<4><<<blocks, threads, smem, s>>>(a);
+    } else if (n == 8) {
+        groupAllToAllKernel<8><<<blocks, threads, smem, s>>>(a);
+    } else {
+        groupAllToAllKernel<0><<<blocks, threads, smem, s>>>(a);
+    }
+    return cudaGetLastError();
+}
+
+// ----------------------------------------------------------------------------
 // Barrier
 // ----------------------------------------------------------------------------
 __global__ void barrierKernel(const FbCommDev c)
@@ -742,6 +855,11 @@ cudaError_t preloadMoveKernels()
     FB_PRELOAD((groupBroadcastKernel<2>))
     FB_PRELOAD((groupBroadcastKernel<4>))
     FB_PRELOAD((groupBroadcastKernel<8>))
+    FB_PRELOAD((groupAllToAllKernel<0>))
+    FB_PRELOAD((groupAllToAllKernel<1>))
+    FB_PRELOAD((groupAllToAllKernel<2>))
+    FB_PRELOAD((groupAllToAllKernel<4>))
+    FB_PRELOAD((groupAllToAllKernel<8>))
     FB_PRELOAD(barrierKernel)
     FB_PRELOAD(waitSignalKernel)
     FB_PRELOAD(waitWordKernel)

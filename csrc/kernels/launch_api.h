@@ -133,6 +133,16 @@ cudaError_t launchGroupBroadcast(const GroupArgs& a,
                                  int threads,
                                  cudaStream_t stream);
 
+// ---- grouped all-to-all: many equal-block MPI_Alltoall calls, ONE launch ----
+// One segment per tensor with B = nVec * 16 bytes per block: sendOff =
+// off(send), recvOff = off(recv) + rank*B.  A chunk covers the same vectors
+// of every block: block p of this rank's send (sendOff + p*B) is stored at
+// recvOff of peer p.  Keeps fbGroupChunkVecs and the entry and exit barriers.
+cudaError_t launchGroupAllToAll(const GroupArgs& a,
+                                int blocks,
+                                int threads,
+                                cudaStream_t stream);
+
 struct ReduceLaunchers
 {
     ReduceLaunchFn reduce;

@@ -1235,6 +1235,7 @@ const fb::KernelTable CUDA_KERNELS = {
     .groupReduceScatter = cudaGroupReduceScatter,
     .groupAllGather = fb::launchGroupAllGather,
     .groupBroadcast = fb::launchGroupBroadcast,
+    .groupAllToAll = fb::launchGroupAllToAll,
     .move = fb::launchMove,
     .moveBulk = fb::launchMoveBulk,
     .barrier = fb::launchBarrier,
@@ -1259,6 +1260,7 @@ const fb::KernelTable HOST_KERNELS = {
     .groupReduceScatter = fb::host::groupReduceScatter,
     .groupAllGather = fb::host::groupAllGather,
     .groupBroadcast = fb::host::groupBroadcast,
+    .groupAllToAll = fb::host::groupAllToAll,
     .move = fb::host::moveKernel,
     .moveBulk = fb::host::moveBulk,
     .barrier = fb::host::barrierKernel,
@@ -1953,8 +1955,9 @@ static int buildGroupSegs(const Communicator& c,
     return FB_OK;
 }
 
-// This rank's segments of a reduce-scatter or all-gather group: one per item,
-// a whole shard each (see Communicator::GroupKind for the conditions)
+// This rank's segments of a reduce-scatter, all-gather or all-to-all group:
+// one per item, a whole shard (block) each (see Communicator::GroupKind for
+// the conditions)
 static int buildShardSegs(const Communicator& c,
                           Communicator::GroupKind kind,
                           const Communicator::GroupItem* items,
@@ -1966,15 +1969,17 @@ static int buildShardSegs(const Communicator& c,
     const int rank = c.rank();
     const uint32_t chunk = fb::fbGroupChunkVecs(n);
     const bool rs = kind == Communicator::GROUP_REDUCE_SCATTER;
+    const bool a2a = kind == Communicator::GROUP_ALLTOALL;
     // [begin, end) of every send, by begin: peers read them (reduce-scatter)
-    // or the kernel reads them (all-gather) while outputs are written
+    // or the kernel reads them (all-gather, all-to-all) while outputs are
+    // written
     std::vector<std::pair<uintptr_t, uintptr_t>> sends;
     for (size_t i = 0; i < nItems; i++) {
         const uint64_t shard = (uint64_t)items[i].count * esize;
         if (shard == 0) {
             continue;
         }
-        const uint64_t sendBytes = rs ? shard * n : shard;
+        const uint64_t sendBytes = (rs || a2a) ? shard * n : shard;
         const uint64_t recvBytes = rs ? shard : shard * n;
         if (shard % 16 != 0 || !c.inHeap(items[i].send, sendBytes) || !c.inHeap(items[i].recv, recvBytes) ||
             (((uintptr_t)items[i].send | (uintptr_t)items[i].recv) & 15)) {
@@ -1996,7 +2001,8 @@ static int buildShardSegs(const Communicator& c,
         const uintptr_t lo = (uintptr_t)items[i].recv;
         const uintptr_t hi = lo + (rs ? shard : shard * n);
         // in-place all-gather: the send is block `rank` of its own output
-        const uintptr_t own = (!rs && (uintptr_t)items[i].send == lo + (uint64_t)rank * shard) ? lo + rank * shard : 0;
+        const bool gather = kind == Communicator::GROUP_ALLGATHER;
+        const uintptr_t own = (gather && (uintptr_t)items[i].send == lo + (uint64_t)rank * shard) ? lo + rank * shard : 0;
         // sends starting below `lo` overlap iff one of them ends above it;
         // every send starting in [lo, hi) overlaps, except the own in-place one
         size_t k = std::lower_bound(sends.begin(), sends.end(), std::make_pair(lo, (uintptr_t)0)) - sends.begin();
@@ -2025,7 +2031,8 @@ static int buildShardSegs(const Communicator& c,
             return FB_E_TOO_LARGE;
         }
         out.segs.push_back(sg);
-        out.vecsPerRank += sg.nVec;
+        // (an all-to-all chunk stores to every peer: the grid follows the work)
+        out.vecsPerRank += a2a ? (uint64_t)sg.nVec * n : sg.nVec;
         out.bytes += shard * n;
     }
     out.totalChunks = (uint32_t)chunks;
@@ -2059,7 +2066,7 @@ std::shared_ptr<Communicator::GroupPlan> Communicator::prepareGroup(
     int& rc = rcOut ? *rcOut : rcLocal;
     rc = FB_OK;
     const size_t esize = fbDtypeSize(dtype);
-    if (esize == 0 || kind < GROUP_ALLREDUCE || kind > GROUP_BROADCAST) {
+    if (esize == 0 || kind < GROUP_ALLREDUCE || kind > GROUP_ALLTOALL) {
         rc = FB_E_INVALID;
         return nullptr;
     }
@@ -2140,7 +2147,13 @@ int Communicator::launchGroup(const GroupLaunch& l, GroupKind kind, int dtype, i
     if (ss && streamBarrier(flags, s) != FB_OK) {
         return FB_E_CUDA;
     }
-    const int blocks = groupGrid(cfg_, n, l.vecsPerRank);
+    int blocks = groupGrid(cfg_, n, l.vecsPerRank);
+    if (kind == GROUP_ALLTOALL) {
+        // no warp without a chunk (totalChunks is the same on every rank: one
+        // whole block per item)
+        const uint64_t warps = (uint64_t)cfg_.threads / 32;
+        blocks = (int)std::clamp<uint64_t>((l.totalChunks + warps - 1) / warps, 1, (uint64_t)blocks);
+    }
     cudaError_t e;
     if (kind == GROUP_REDUCE_SCATTER) {
         e = k_->groupReduceScatter(a, dtype, op, blocks, cfg_.threads, s);
@@ -2148,6 +2161,8 @@ int Communicator::launchGroup(const GroupLaunch& l, GroupKind kind, int dtype, i
         e = k_->groupAllGather(a, blocks, cfg_.threads, s);
     } else if (kind == GROUP_BROADCAST) {
         e = k_->groupBroadcast(a, blocks, cfg_.threads, s);
+    } else if (kind == GROUP_ALLTOALL) {
+        e = k_->groupAllToAll(a, blocks, cfg_.threads, s);
     } else {
         e = k_->group(a, dtype, op, blocks, cfg_.threads, s);
     }
@@ -2241,6 +2256,22 @@ int Communicator::broadcastGroup(const GroupPlan& plan, int root, int flags, cud
     return FB_OK;
 }
 
+int Communicator::allToAllGroup(const GroupPlan& plan, int flags, cudaStream_t s)
+{
+    NvtxRange nvtxRange("fb::allToAllGroup");
+    if (plan.kind != GROUP_ALLTOALL) {
+        return FB_E_INVALID;
+    }
+    bindDevice();
+    for (const auto& l : plan.launches) {
+        int rc = launchGroup(l, GROUP_ALLTOALL, plan.dtype, -1, flags, s);
+        if (rc != FB_OK) {
+            return rc;
+        }
+    }
+    return FB_OK;
+}
+
 int Communicator::allReduceMany(const GroupItem* items,
                                 size_t nItems,
                                 int dtype,
@@ -2281,6 +2312,12 @@ int Communicator::broadcastMany(const GroupItem* items, size_t nItems, int root,
     return groupMany(GROUP_BROADCAST, items, nItems, FB_U8, root, flags, s);
 }
 
+int Communicator::allToAllMany(const GroupItem* items, size_t nItems, int dtype, int flags, cudaStream_t s)
+{
+    NvtxRange nvtxRange("fb::allToAllMany");
+    return groupMany(GROUP_ALLTOALL, items, nItems, dtype, -1, flags, s);
+}
+
 int Communicator::groupMany(GroupKind kind,
                             const GroupItem* items,
                             size_t nItems,
@@ -2293,9 +2330,10 @@ int Communicator::groupMany(GroupKind kind,
     if (esize == 0) {
         return FB_E_INVALID;
     }
-    // all-gather and broadcast are byte copies: any dtype has a kernel
+    // all-gather, broadcast and all-to-all are byte copies: any dtype has a
+    // kernel
     bool grouped = true;
-    if (kind != GROUP_ALLGATHER && kind != GROUP_BROADCAST) {
+    if (kind == GROUP_ALLREDUCE || kind == GROUP_REDUCE_SCATTER) {
         const fb::ReduceLaunchers* L = fb::findReduceLaunchers(dtype, op);
         if (L == nullptr) {
             return FB_E_UNSUPPORTED;
@@ -2334,6 +2372,11 @@ int Communicator::groupMany(GroupKind kind,
                         f &= ~FB_FLAG_SYMMETRIC;
                     }
                     r2 = reduceScatter(it.send, it.recv, it.count, dtype, op, f, s);
+                } else if (kind == GROUP_ALLTOALL) {
+                    if (!inHeap(it.send, bytes * n)) {
+                        f &= ~FB_FLAG_SYMMETRIC;
+                    }
+                    r2 = allToAll(it.send, it.recv, bytes, f, s);
                 } else {
                     if (!inHeap(it.send, bytes)) {
                         f &= ~FB_FLAG_SYMMETRIC;

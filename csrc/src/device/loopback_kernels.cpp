@@ -626,6 +626,31 @@ cudaError_t groupBroadcast(const GroupArgs& a, int blocks, int, cudaStream_t)
     return cudaSuccess;
 }
 
+cudaError_t groupAllToAll(const GroupArgs& a, int blocks, int, cudaStream_t)
+{
+    if (!shardSegsOk(a)) {
+        return cudaErrorMisalignedAddress;
+    }
+    const FbCommDev& c = a.comm;
+    bool ok = true;
+    if (!a.noSync) {
+        ok = gridBarrier(c, blocks);
+    }
+    if (ok) {
+        for (uint32_t si = 0; si < a.nSegs; si++) {
+            const GroupSeg& sg = a.segs[si];
+            const uint64_t block = (uint64_t)sg.nVec * 16;
+            for (int p = 0; p < c.nranks; p++) {
+                memcpy(c.heap[p] + sg.recvOff, c.heap[c.rank] + sg.sendOff + (uint64_t)p * block, block);
+            }
+        }
+    }
+    if (!a.noSync) {
+        gridBarrier(c, blocks);
+    }
+    return cudaSuccess;
+}
+
 // ----------------------------------------------------------------- move ----
 // The CUDA kernels copy in W-byte words.  Every address they touch that way
 // must be W-aligned (a misaligned vector access is a device fault), and every

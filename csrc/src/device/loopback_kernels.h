@@ -19,6 +19,7 @@ struct KernelTable
     cudaError_t (*groupReduceScatter)(const GroupArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s);
     cudaError_t (*groupAllGather)(const GroupArgs& a, int blocks, int threads, cudaStream_t s);
     cudaError_t (*groupBroadcast)(const GroupArgs& a, int blocks, int threads, cudaStream_t s);
+    cudaError_t (*groupAllToAll)(const GroupArgs& a, int blocks, int threads, cudaStream_t s);
     cudaError_t (*move)(const MoveArgs& a, int width, int blocks, int threads, cudaStream_t s);
     // TMA bulk-copy engine (fixed block size, 16-byte aligned ranges)
     cudaError_t (*moveBulk)(const MoveArgs& a, int blocks, cudaStream_t s);
@@ -57,6 +58,7 @@ cudaError_t groupAllReduce(const GroupArgs& a, int dtype, int op, int blocks, in
 cudaError_t groupReduceScatter(const GroupArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s);
 cudaError_t groupAllGather(const GroupArgs& a, int blocks, int threads, cudaStream_t s);
 cudaError_t groupBroadcast(const GroupArgs& a, int blocks, int threads, cudaStream_t s);
+cudaError_t groupAllToAll(const GroupArgs& a, int blocks, int threads, cudaStream_t s);
 // The move, p2p and put twins return cudaErrorMisalignedAddress, before they
 // copy or synchronise, when an address the kernel reads or writes in words of
 // `width` bytes is not aligned to it (moveBulk: 16 bytes)

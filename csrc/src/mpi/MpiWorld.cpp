@@ -982,6 +982,9 @@ static void flushPendingGroup()
     } else if (tls.groupKind == Communicator::GROUP_BROADCAST) {
         rc = comm->broadcastMany(items.data(), items.size(), tls.groupOp, FB_FLAG_SYMMETRIC, s);
         what = "Grouped device broadcast";
+    } else if (tls.groupKind == Communicator::GROUP_ALLTOALL) {
+        rc = comm->allToAllMany(items.data(), items.size(), tls.groupDtype, FB_FLAG_SYMMETRIC, s);
+        what = "Grouped device all-to-all";
     } else {
         rc = comm->allReduceMany(items.data(), items.size(), tls.groupDtype, tls.groupOp, FB_FLAG_SYMMETRIC, s);
         what = "Grouped device all-reduce";
@@ -1756,6 +1759,54 @@ int MpiWorld::nbBroadcast(const DeviceComm& comm, int rank, int root, uint8_t* b
         void* s = tls.cachedStream0;
         if ((at.symmetric || isDevicePointer(buffer)) && issueDevice(*comm, s, deviceCollectives, [&](auto& c, cudaStream_t st) {
                 return c.broadcast(buffer, bytes, root, symFlag(c, buffer, bytes), st);
+            })) {
+            return recordDevice(requestId, std::move(r), comm, s);
+        }
+    }
+    // Host buffers, or unsupported on the device: complete it now
+    host();
+    tls.requests[requestId] = std::move(r);
+    return requestId;
+}
+
+int MpiWorld::iAllToAll(int rank,
+                        uint8_t* send,
+                        faabric_datatype_t* sendType,
+                        int sendCount,
+                        uint8_t* recv,
+                        faabric_datatype_t* recvType,
+                        int recvCount)
+{
+    checkRanksRange(0, rank);
+    cacheDeviceComm(rank);
+    return nbAllToAll(tls.cachedComm, rank, size, send, recv, (size_t)sendCount * sendType->size, [&] {
+        allToAll(rank, send, sendType, sendCount, recv, recvType, recvCount);
+    });
+}
+
+int MpiWorld::nbAllToAll(const DeviceComm& comm,
+                         int rank,
+                         int members,
+                         const uint8_t* send,
+                         uint8_t* recv,
+                         size_t bytes,
+                         const HostPath& host)
+{
+    using faabric::device::Communicator;
+    const int requestId = tls.nextRequestId++;
+    AsyncRequest r = collectiveRequest(rank);
+    cacheDeviceComm(rank);
+    if (bytes > 0 && comm != nullptr) {
+        const size_t total = bytes * (size_t)members;
+        const Placement at = placeCollective(*comm, groupIallreduce, send, total, recv, total, bytes);
+        if (at.grouped) {
+            // a byte copy: the burst's key is the communicator alone
+            deferToGroup(Communicator::GROUP_ALLTOALL, comm, FB_U8, -1, { send, recv, bytes }, requestId, std::move(r), deviceCollectives);
+            return requestId;
+        }
+        void* s = tls.cachedStream0;
+        if ((at.symmetric || isDevicePointer(send)) && issueDevice(*comm, s, deviceCollectives, [&](auto& c, cudaStream_t st) {
+                return c.allToAll(send, recv, bytes, symFlag(c, send, total), st);
             })) {
             return recordDevice(requestId, std::move(r), comm, s);
         }

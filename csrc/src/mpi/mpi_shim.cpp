@@ -1027,6 +1027,28 @@ int MPI_Ibcast(void* buffer, int count, MPI_Datatype datatype, int root, MPI_Com
     return handOut(world.iBroadcast(rank, root, (uint8_t*)buffer, datatype, count), request);
 }
 
+int MPI_Ialltoall(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                  MPI_Datatype recvtype, MPI_Comm comm, MPI_Request* request)
+{
+    SPDLOG_TRACE("MPI - MPI_Ialltoall");
+    if (sendbuf == MPI_IN_PLACE || (size_t)sendcount * sendtype->size != (size_t)recvcount * recvtype->size) {
+        return MPI_ERR_ARG;
+    }
+    MpiWorld& world = getExecutingWorld();
+    const int rank = executingContext.getRank();
+    const uint8_t* send = (const uint8_t*)sendbuf;
+    if (auto sub = subOf(comm)) {
+        const size_t bytes = (size_t)sendcount * sendtype->size;
+        auto dev = bytes > 0 && MpiWorld::isDevicePointer(send) ? sub->deviceComm(world, rank) : nullptr;
+        return handOut(world.nbAllToAll(dev, rank, sub->size(), send, (uint8_t*)recvbuf, bytes, [&] {
+            sub->allToAll(world, rank, send, (uint8_t*)recvbuf, sendtype, sendcount);
+        }),
+                       request);
+    }
+    return handOut(world.iAllToAll(rank, (uint8_t*)send, sendtype, sendcount, (uint8_t*)recvbuf, recvtype, recvcount),
+                   request);
+}
+
 int MPI_Get_processor_name(char* name, int* resultlen)
 {
     SPDLOG_TRACE("MPI - MPI_Get_processor_name");

@@ -7,9 +7,10 @@
 // MPI_Alltoall and MPI_Reduce_scatter_block run the world's fused kernels over
 // a child of the world device communicator (Communicator::subset), on a
 // signal slot the members agree on at their first such call; MPI_Ibcast,
-// MPI_Iallreduce, MPI_Ireduce_scatter_block and MPI_Iallgather take the
-// world's non-blocking rules (bursts included) over the same child.  Everything else, and every call when no slot is
-// free on all members, is built from the world's point-to-point layer, so it
+// MPI_Iallreduce, MPI_Ireduce_scatter_block, MPI_Iallgather and
+// MPI_Ialltoall take the world's non-blocking rules (bursts included) over
+// the same child.  Everything else, and every call when no slot is free on
+// all members, is built from the world's point-to-point layer, so it
 // works for ranks in one process (queues / peer memory) and across worker
 // processes (TCP) alike, on host and device buffers.
 #pragma once

@@ -134,6 +134,9 @@ def load():
     _sig(lib, "fb_group_prepare_broadcast", vp, [vp, i32, vpp, u64p])
     _sig(lib, "fb_group_broadcast", i32, [vp, vp, i32, i32, vp])
     _sig(lib, "fb_broadcast_many", i32, [vp, i32, vpp, u64p, i32, i32, vp])
+    _sig(lib, "fb_group_prepare_all_to_all", vp, [vp, i32, vpp, vpp, u64p, i32])
+    _sig(lib, "fb_group_all_to_all", i32, [vp, vp, i32, vp])
+    _sig(lib, "fb_all_to_all_many", i32, [vp, i32, vpp, vpp, u64p, i32, i32, vp])
     _sig(lib, "fb_put_signal", i32, [vp, vp, u64, u64, i32, i32, i32, vp])
     _sig(lib, "fb_wait_signal", i32, [vp, i32, u32, vp])
     _sig(lib, "fb_accumulate", i32, [vp, vp, u64, u64, i32, i32, i32, vp, vp])

@@ -611,6 +611,63 @@ class Communicator:
         rc = self._lib.fb_broadcast_many(self._h, n, bp, nb, int(root), f, self._stream(stream))
         self._check(rc, "broadcast_many")
 
+    # ------------------------------------------------ grouped all-to-all
+    def _a2a_arrays(self, what, sends, recvs, dtype):
+        """(n, send ptrs, recv ptrs, per-block counts, FbDtype) of an all-to-all
+        group; raises before any native call unless every item's send and recv
+        have equal numel and element size, numel divisible by ``size`` (in
+        ``dtype`` elements too)."""
+        if len(sends) != len(recvs) or not sends:
+            raise CommError(f"{what}: need equally long, non-empty lists")
+        for i, (s, r) in enumerate(zip(sends, recvs)):
+            if s.numel() != r.numel() or s.numel() % self.size != 0:
+                raise CommError(
+                    f"{what}: item {i} has {s.numel()} send and {r.numel()} recv elements; "
+                    f"both must be equal and divisible by {self.size}"
+                )
+            if s.element_size() != r.element_size():
+                # (the native side sizes recv from the send's elements)
+                raise CommError(
+                    f"{what}: item {i} has {s.element_size()}-byte send and {r.element_size()}-byte recv elements"
+                )
+        n = len(sends)
+        sp = (C.c_void_p * n)(*[t.data_ptr() for t in sends])
+        rp = (C.c_void_p * n)(*[t.data_ptr() for t in recvs])
+        typed = [self._typed(s, dtype) for s in sends]
+        if len({dt for _, dt in typed}) != 1:
+            raise CommError(f"{what}: every tensor must have the same dtype")
+        for i, (c, _) in enumerate(typed):
+            if c % self.size != 0:
+                raise CommError(f"{what}: item {i} has {c} {dtype} elements, not divisible by {self.size}")
+        cnt = (C.c_uint64 * n)(*[c // self.size for c, _ in typed])
+        return n, sp, rp, cnt, typed[0][1]
+
+    def prepare_all_to_all_group(self, sends, recvs, dtype=None) -> "GroupPlan":
+        """Plan ONE launch that exchanges every pair of the lists (MPI_Alltoall
+        per pair: block r of ``recvs[i]`` on rank p gets block p of
+        ``sends[i]`` on rank r, with ``size`` equal blocks per tensor).
+        Tensors live in the symmetric heap at 16-byte aligned addresses, blocks
+        are multiples of 16 bytes, and no output overlaps an input; call
+        collectively with the same lists."""
+        n, sp, rp, cnt, dt = self._a2a_arrays("prepare_all_to_all_group", sends, recvs, dtype)
+        h = self._lib.fb_group_prepare_all_to_all(self._h, n, sp, rp, cnt, dt)
+        if not h:
+            raise CommError(f"prepare_all_to_all_group failed [{_lib.last_error()}]")
+        return GroupPlan(self, h, n, sum(t.numel() * t.element_size() for t in sends))
+
+    def all_to_all_group(self, plan: "GroupPlan", stream=None, channel=0, flags=FLAG_SYMMETRIC):
+        rc = self._lib.fb_group_all_to_all(self._h, plan._h, flags | ((channel & 0xF) << 8), self._stream(stream))
+        self._check(rc, "all_to_all_group")
+
+    def all_to_all_many(self, sends, recvs, stream=None, channel=0, dtype=None):
+        """Transient variant of :meth:`prepare_all_to_all_group` +
+        :meth:`all_to_all_group`; lists that cannot be grouped run one
+        :meth:`all_to_all` per pair."""
+        n, sp, rp, cnt, dt = self._a2a_arrays("all_to_all_many", sends, recvs, dtype)
+        f = self._sym(*sends) | ((channel & 0xF) << 8)
+        rc = self._lib.fb_all_to_all_many(self._h, n, sp, rp, cnt, dt, f, self._stream(stream))
+        self._check(rc, "all_to_all_many")
+
     def send_recv(self, send_buf, dst, recv_buf, src, stream=None):
         rc = self._lib.fb_sendrecv(
             self._h,
@@ -882,7 +939,7 @@ class Communicator:
 
 class GroupPlan:
     """Device-resident segment tables of a grouped all-reduce, reduce-scatter,
-    all-gather or broadcast."""
+    all-gather, broadcast or all-to-all."""
 
     def __init__(self, comm: Communicator, handle, n_tensors: int, nbytes: int):
         self._comm = comm
