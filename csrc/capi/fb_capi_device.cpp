@@ -552,7 +552,7 @@ int fb_comm_sync_bounded(void* h, void* stream, uint64_t timeoutMs)
     return COMM(h)->syncStreamBounded((cudaStream_t)stream, timeoutMs) ? 1 : 0;
 }
 
-// ---- grouped all-reduce ----
+// ---- grouped collectives: `kind` is a Communicator::GroupKind ----
 struct FbGroupPlanHandle
 {
     std::shared_ptr<Communicator::GroupPlan> plan;
@@ -563,7 +563,7 @@ static std::vector<Communicator::GroupItem> groupItems(int n,
                                                        void* const* recv,
                                                        const uint64_t* counts)
 {
-    std::vector<Communicator::GroupItem> items((size_t)n);
+    std::vector<Communicator::GroupItem> items((size_t)std::max(n, 0));
     for (int i = 0; i < n; i++) {
         items[i].send = send[i];
         items[i].recv = recv[i];
@@ -573,6 +573,7 @@ static std::vector<Communicator::GroupItem> groupItems(int n,
 }
 
 void* fb_group_prepare(void* h,
+                       int kind,
                        int n,
                        const void* const* send,
                        void* const* recv,
@@ -582,7 +583,7 @@ void* fb_group_prepare(void* h,
     FB_TRY
     auto items = groupItems(n, send, recv, counts);
     int rc = FB_OK;
-    auto plan = COMM(h)->prepareGroup(items.data(), items.size(), dtype, &rc);
+    auto plan = COMM(h)->prepareGroup(items.data(), items.size(), dtype, &rc, (Communicator::GroupKind)kind);
     if (!plan) {
         g_lastError = std::string("prepareGroup: ") + Communicator::errorString(rc);
         return nullptr;
@@ -593,180 +594,32 @@ void* fb_group_prepare(void* h,
     FB_CATCH(nullptr)
 }
 
-// ---- grouped reduce-scatter / all-gather / all-to-all: counts are per-rank counts ----
-static void* groupPrepareKind(void* h,
-                              int n,
-                              const void* const* send,
-                              void* const* recv,
-                              const uint64_t* counts,
-                              int dtype,
-                              Communicator::GroupKind kind)
+int fb_group_launch(void* h, int kind, void* plan, int op, int root, int flags, void* stream)
+{
+    if (plan == nullptr) {
+        return FB_E_INVALID;
+    }
+    return COMM(h)->runGroup(
+      (Communicator::GroupKind)kind, *((FbGroupPlanHandle*)plan)->plan, op, root, flags, (cudaStream_t)stream);
+}
+
+int fb_group_many(void* h,
+                  int kind,
+                  int n,
+                  const void* const* send,
+                  void* const* recv,
+                  const uint64_t* counts,
+                  int dtype,
+                  int op,
+                  int root,
+                  int flags,
+                  void* stream)
 {
     FB_TRY
     auto items = groupItems(n, send, recv, counts);
-    int rc = FB_OK;
-    auto plan = COMM(h)->prepareGroup(items.data(), items.size(), dtype, &rc, kind);
-    if (!plan) {
-        g_lastError = std::string("prepareGroup: ") + Communicator::errorString(rc);
-        return nullptr;
-    }
-    auto* ph = new FbGroupPlanHandle();
-    ph->plan = plan;
-    return ph;
-    FB_CATCH(nullptr)
-}
-
-void* fb_group_prepare_reduce_scatter(void* h,
-                                      int n,
-                                      const void* const* send,
-                                      void* const* recv,
-                                      const uint64_t* counts,
-                                      int dtype)
-{
-    return groupPrepareKind(h, n, send, recv, counts, dtype, Communicator::GROUP_REDUCE_SCATTER);
-}
-
-void* fb_group_prepare_all_gather(void* h,
-                                  int n,
-                                  const void* const* send,
-                                  void* const* recv,
-                                  const uint64_t* counts,
-                                  int dtype)
-{
-    return groupPrepareKind(h, n, send, recv, counts, dtype, Communicator::GROUP_ALLGATHER);
-}
-
-void* fb_group_prepare_all_to_all(void* h,
-                                  int n,
-                                  const void* const* send,
-                                  void* const* recv,
-                                  const uint64_t* counts,
-                                  int dtype)
-{
-    return groupPrepareKind(h, n, send, recv, counts, dtype, Communicator::GROUP_ALLTOALL);
-}
-
-int fb_group_reduce_scatter(void* h, void* plan, int op, int flags, void* stream)
-{
-    if (plan == nullptr) {
-        return FB_E_INVALID;
-    }
-    return COMM(h)->reduceScatterGroup(*((FbGroupPlanHandle*)plan)->plan, op, flags, (cudaStream_t)stream);
-}
-
-int fb_group_all_gather(void* h, void* plan, int flags, void* stream)
-{
-    if (plan == nullptr) {
-        return FB_E_INVALID;
-    }
-    return COMM(h)->allGatherGroup(*((FbGroupPlanHandle*)plan)->plan, flags, (cudaStream_t)stream);
-}
-
-int fb_group_all_to_all(void* h, void* plan, int flags, void* stream)
-{
-    if (plan == nullptr) {
-        return FB_E_INVALID;
-    }
-    return COMM(h)->allToAllGroup(*((FbGroupPlanHandle*)plan)->plan, flags, (cudaStream_t)stream);
-}
-
-int fb_reduce_scatter_many(void* h,
-                           int n,
-                           const void* const* send,
-                           void* const* recv,
-                           const uint64_t* counts,
-                           int dtype,
-                           int op,
-                           int flags,
-                           void* stream)
-{
-    FB_TRY
-    auto items = groupItems(n, send, recv, counts);
-    return COMM(h)->reduceScatterMany(items.data(), items.size(), dtype, op, flags, (cudaStream_t)stream);
+    return COMM(h)->groupMany(
+      (Communicator::GroupKind)kind, items.data(), items.size(), dtype, op, root, flags, (cudaStream_t)stream);
     FB_CATCH(FB_E_CUDA)
-}
-
-int fb_all_gather_many(void* h,
-                       int n,
-                       const void* const* send,
-                       void* const* recv,
-                       const uint64_t* counts,
-                       int dtype,
-                       int flags,
-                       void* stream)
-{
-    FB_TRY
-    auto items = groupItems(n, send, recv, counts);
-    return COMM(h)->allGatherMany(items.data(), items.size(), dtype, flags, (cudaStream_t)stream);
-    FB_CATCH(FB_E_CUDA)
-}
-
-int fb_all_to_all_many(void* h,
-                       int n,
-                       const void* const* send,
-                       void* const* recv,
-                       const uint64_t* counts,
-                       int dtype,
-                       int flags,
-                       void* stream)
-{
-    FB_TRY
-    auto items = groupItems(n, send, recv, counts);
-    return COMM(h)->allToAllMany(items.data(), items.size(), dtype, flags, (cudaStream_t)stream);
-    FB_CATCH(FB_E_CUDA)
-}
-
-// ---- grouped broadcast: one buffer and byte count per item ----
-static std::vector<Communicator::GroupItem> broadcastItems(int n, void* const* bufs, const uint64_t* bytes)
-{
-    std::vector<Communicator::GroupItem> items((size_t)std::max(n, 0));
-    for (int i = 0; i < n; i++) {
-        items[i].send = bufs[i];
-        items[i].recv = bufs[i];
-        items[i].count = (size_t)bytes[i];
-    }
-    return items;
-}
-
-void* fb_group_prepare_broadcast(void* h, int n, void* const* bufs, const uint64_t* bytes)
-{
-    FB_TRY
-    auto items = broadcastItems(n, bufs, bytes);
-    int rc = FB_OK;
-    auto plan = COMM(h)->prepareGroup(items.data(), items.size(), FB_U8, &rc, Communicator::GROUP_BROADCAST);
-    if (!plan) {
-        g_lastError = std::string("prepareGroup: ") + Communicator::errorString(rc);
-        return nullptr;
-    }
-    auto* ph = new FbGroupPlanHandle();
-    ph->plan = plan;
-    return ph;
-    FB_CATCH(nullptr)
-}
-
-int fb_group_broadcast(void* h, void* plan, int root, int flags, void* stream)
-{
-    if (plan == nullptr) {
-        return FB_E_INVALID;
-    }
-    return COMM(h)->broadcastGroup(*((FbGroupPlanHandle*)plan)->plan, root, flags, (cudaStream_t)stream);
-}
-
-int fb_broadcast_many(void* h, int n, void* const* bufs, const uint64_t* bytes, int root, int flags, void* stream)
-{
-    FB_TRY
-    auto items = broadcastItems(n, bufs, bytes);
-    return COMM(h)->broadcastMany(items.data(), items.size(), root, flags, (cudaStream_t)stream);
-    FB_CATCH(FB_E_CUDA)
-}
-
-int fb_group_allreduce(void* h, void* plan, int op, int flags, void* stream)
-{
-    if (plan == nullptr) {
-        return FB_E_INVALID;
-    }
-    return COMM(h)->allReduceGroup(
-      *((FbGroupPlanHandle*)plan)->plan, op, flags, (cudaStream_t)stream);
 }
 
 int fb_group_plan_launches(void* plan)
@@ -777,23 +630,6 @@ int fb_group_plan_launches(void* plan)
 void fb_group_plan_free(void* plan)
 {
     delete (FbGroupPlanHandle*)plan;
-}
-
-int fb_allreduce_many(void* h,
-                      int n,
-                      const void* const* send,
-                      void* const* recv,
-                      const uint64_t* counts,
-                      int dtype,
-                      int op,
-                      int flags,
-                      void* stream)
-{
-    FB_TRY
-    auto items = groupItems(n, send, recv, counts);
-    return COMM(h)->allReduceMany(
-      items.data(), items.size(), dtype, op, flags, (cudaStream_t)stream);
-    FB_CATCH(FB_E_CUDA)
 }
 
 int fb_put_signal(void* h,

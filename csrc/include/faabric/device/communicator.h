@@ -27,6 +27,7 @@
 
 namespace fb {
 struct KernelTable;
+struct GroupSeg;
 }
 
 namespace faabric::device {
@@ -302,51 +303,38 @@ class Communicator : public std::enable_shared_from_this<Communicator>
                                             int dtype,
                                             int* rc = nullptr,
                                             GroupKind kind = GROUP_ALLREDUCE);
-    // A plan of another kind gives FB_E_INVALID
-    int allReduceGroup(const GroupPlan& plan, int op, int flags, cudaStream_t s);
-    int reduceScatterGroup(const GroupPlan& plan, int op, int flags, cudaStream_t s);
-    int allGatherGroup(const GroupPlan& plan, int flags, cudaStream_t s);
-    // A GROUP_BROADCAST plan from `root` (a rank of this communicator; out of
-    // range: FB_E_INVALID).  The root's buffers are only read.  On a
-    // one-member communicator nothing is launched.
-    int broadcastGroup(const GroupPlan& plan, int root, int flags, cudaStream_t s);
-    // A GROUP_ALLTOALL plan.  On a one-member communicator it is launched as
-    // a local copy.
-    int allToAllGroup(const GroupPlan& plan, int flags, cudaStream_t s);
-    // prepare + launch for a transient list (MPI_Iallreduce bursts); falls back
-    // to per-item allReduce calls when the list cannot be grouped
-    int allReduceMany(const GroupItem* items,
-                      size_t nItems,
-                      int dtype,
-                      int op,
-                      int flags,
-                      cudaStream_t s);
-    // The same for the shard kinds (MPI_Ireduce_scatter_block and
-    // MPI_Iallgather bursts): falls back to per-item reduceScatter /
-    // allGather calls for a list that cannot be grouped, and returns their
-    // errors (reduceScatter refuses shards that are not a multiple of 16
-    // bytes with FB_E_UNSUPPORTED)
-    int reduceScatterMany(const GroupItem* items,
-                          size_t nItems,
-                          int dtype,
-                          int op,
-                          int flags,
-                          cudaStream_t s);
-    int allGatherMany(const GroupItem* items,
-                      size_t nItems,
-                      int dtype,
-                      int flags,
-                      cudaStream_t s);
-    // MPI_Ibcast bursts: item i broadcasts items[i].count BYTES of
-    // items[i].recv from `root` (send is not read).  A batch whose buffers
-    // are not all in the symmetric heap and 16-byte aligned falls back to
-    // per-item broadcast calls.  Root out of range: FB_E_INVALID; one member:
-    // nothing is launched.
-    int broadcastMany(const GroupItem* items, size_t nItems, int root, int flags, cudaStream_t s);
-    // MPI_Ialltoall bursts (items[i].count elements per block): falls back to
-    // per-item allToAll calls for a list that cannot be grouped
-    int allToAllMany(const GroupItem* items, size_t nItems, int dtype, int flags, cudaStream_t s);
+    // Launches a prepared plan of `kind`.  groupMany prepares and launches a
+    // transient list (the MPI bursts), batch by batch; a batch that cannot be
+    // grouped runs as per-item allReduce / reduceScatter / allGather /
+    // broadcast / allToAll calls and returns their errors (reduceScatter
+    // refuses shards that are not a multiple of 16 bytes with
+    // FB_E_UNSUPPORTED).  `op` is read by the reducing kinds (GROUP_ALLREDUCE,
+    // GROUP_REDUCE_SCATTER) only, `root` by GROUP_BROADCAST only.  Both
+    // follow the same rules:
+    //   - a plan of another kind, an unknown kind or a dtype of no size:
+    //     FB_E_INVALID
+    //   - reducing kinds: a (dtype, op) pair with no reduction at all gives
+    //     FB_E_UNSUPPORTED; a pair with no grouped kernel gives
+    //     FB_E_UNSUPPORTED from runGroup, and per-item calls from groupMany
+    //   - GROUP_BROADCAST: a root that is not a rank of this communicator
+    //     gives FB_E_INVALID; the root's buffers are only read; on a
+    //     one-member communicator nothing is launched (FB_OK).  For
+    //     groupMany, pass each buffer as send and recv with FB_U8 and byte
+    //     counts.
+    //   - GROUP_ALLTOALL on a one-member communicator runs as a local copy
+    //   - GROUP_ALLREDUCE sets lastAlgo() to FB_ALGO_TWOSHOT
+    int runGroup(GroupKind kind, const GroupPlan& plan, int op, int root, int flags, cudaStream_t s);
+    int groupMany(GroupKind kind,
+                  const GroupItem* items,
+                  size_t nItems,
+                  int dtype,
+                  int op,
+                  int root,
+                  int flags,
+                  cudaStream_t s);
     static size_t groupPlanLaunches(const GroupPlan& plan);
+    // "all-reduce", "reduce-scatter", "all-gather", "broadcast", "all-to-all"
+    static const char* groupKindName(GroupKind kind);
 
     // ---- point to point (per-pair FIFO; no kernel ever spins on a peer) ----
     // Operations on one ordered pair must be issued in a consistent stream
@@ -530,7 +518,7 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     bool streamWriteOk_ = false;
     cudaStream_t internalStream_ = nullptr;
     uint32_t doneSeq_ = 0;
-    // transient group tables (allReduceMany) and copy and accumulate tables
+    // transient group tables (groupMany) and copy and accumulate tables
     // (putGetMany, accumulateMany)
     struct ManySlot;
     std::vector<std::shared_ptr<ManySlot>> manySlots_;
@@ -580,14 +568,22 @@ class Communicator : public std::enable_shared_from_this<Communicator>
                 std::shared_ptr<Backing> backing,
                 const std::string& kind);
     void finishSetup();
-    int launchGroup(const GroupLaunch& l, GroupKind kind, int dtype, int op, int flags, cudaStream_t s);
-    int groupMany(GroupKind kind,
-                  const GroupItem* items,
-                  size_t nItems,
-                  int dtype,
-                  int op,
-                  int flags,
-                  cudaStream_t s);
+    int launchGroup(const GroupLaunch& l, GroupKind kind, int dtype, int op, int root, int flags, cudaStream_t s);
+    int groupCheck(GroupKind kind, int dtype, int op, int root, bool& grouped) const;
+    int groupBatch(GroupKind kind,
+                   const GroupItem* items,
+                   size_t nItems,
+                   size_t esize,
+                   std::vector<fb::GroupSeg>& segs,
+                   GroupLaunch& l) const;
+    int groupPerItem(GroupKind kind,
+                     const GroupItem* items,
+                     size_t nItems,
+                     int dtype,
+                     int op,
+                     int root,
+                     int flags,
+                     cudaStream_t s);
     int streamWaitGe(cudaStream_t s, const uint32_t* localWord, uint32_t value);
     int streamBarrier(int flags, cudaStream_t s);
     bool rmaTargetOk(uint64_t dstOffset, uint64_t bytes, size_t align, int peer) const;

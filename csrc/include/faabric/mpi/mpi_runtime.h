@@ -612,6 +612,13 @@ class MpiWorld
     void settleDeviceBurst(const DeviceComm& comm);
 
   private:
+    // The request / defer / issue / host skeleton of the nbX functions but
+    // nbAllReduce (which spreads its calls over channels)
+    struct NbCall;
+    template <typename Issue>
+    int nbCollective(const DeviceComm& comm, int rank, bool device, const NbCall& call, Issue&& issue,
+                     const HostPath& host);
+
     int id = -1;
     int size = -1;
     std::string thisHost;

@@ -1778,7 +1778,7 @@ int Communicator::scan(const void* send,
 }
 
 // ---------------------------------------------------------------------------
-// Grouped all-reduce
+// Grouped collectives
 // ---------------------------------------------------------------------------
 // One launch of the grouped kernel: this rank's segment table
 struct Communicator::GroupLaunch
@@ -2039,21 +2039,32 @@ static int buildShardSegs(const Communicator& c,
     return FB_OK;
 }
 
-static int buildSegs(const Communicator& c,
-                     Communicator::GroupKind kind,
-                     const Communicator::GroupItem* items,
-                     size_t nItems,
-                     size_t esize,
-                     SegBuild& out)
-{
-    if (kind == Communicator::GROUP_ALLREDUCE || kind == Communicator::GROUP_BROADCAST) {
-        return buildGroupSegs(c, items, nItems, esize, kind == Communicator::GROUP_BROADCAST, out);
-    }
-    return buildShardSegs(c, kind, items, nItems, esize, out);
-}
-
 // items per launch: every item yields at most one segment per rank
 static const size_t GROUP_ITEMS_PER_LAUNCH = FB_GROUP_MAX_SEGS - 8;
+
+// One launch of items[0..nItems) (at most GROUP_ITEMS_PER_LAUNCH): this rank's
+// segments in `segs`, the launch's sizes in `l` (l.dSegs is left to the caller)
+int Communicator::groupBatch(GroupKind kind,
+                             const GroupItem* items,
+                             size_t nItems,
+                             size_t esize,
+                             std::vector<fb::GroupSeg>& segs,
+                             GroupLaunch& l) const
+{
+    SegBuild sb;
+    const int rc = kind == GROUP_ALLREDUCE || kind == GROUP_BROADCAST
+                     ? buildGroupSegs(*this, items, nItems, esize, kind == GROUP_BROADCAST, sb)
+                     : buildShardSegs(*this, kind, items, nItems, esize, sb);
+    if (rc != FB_OK) {
+        return rc;
+    }
+    segs = std::move(sb.segs);
+    l.nSegs = (uint32_t)segs.size();
+    l.totalChunks = sb.totalChunks;
+    l.vecsPerRank = sb.vecsPerRank;
+    l.bytes = sb.bytes;
+    return FB_OK;
+}
 
 std::shared_ptr<Communicator::GroupPlan> Communicator::prepareGroup(
   const GroupItem* items,
@@ -2077,25 +2088,20 @@ std::shared_ptr<Communicator::GroupPlan> Communicator::prepareGroup(
     plan->device = device_;
     plan->items = nItems;
     for (size_t begin = 0; begin < nItems; begin += GROUP_ITEMS_PER_LAUNCH) {
-        const size_t cnt = std::min(GROUP_ITEMS_PER_LAUNCH, nItems - begin);
-        SegBuild sb;
-        rc = buildSegs(*this, kind, items + begin, cnt, esize, sb);
+        std::vector<fb::GroupSeg> segs;
+        GroupLaunch l;
+        rc = groupBatch(kind, items + begin, std::min(GROUP_ITEMS_PER_LAUNCH, nItems - begin), esize, segs, l);
         if (rc != FB_OK) {
             return nullptr;
         }
-        GroupLaunch l;
-        l.nSegs = (uint32_t)sb.segs.size();
-        l.totalChunks = sb.totalChunks;
-        l.vecsPerRank = sb.vecsPerRank;
-        l.bytes = sb.bytes;
         // (a rank may own nothing of a tiny group: it still takes part in the
         // barriers, with an empty table)
-        const size_t tb = std::max<size_t>(sb.segs.size(), 1) * sizeof(fb::GroupSeg);
+        const size_t tb = std::max<size_t>(segs.size(), 1) * sizeof(fb::GroupSeg);
         if (loop_) {
             plan->hostTables = true;
             l.dSegs = (fb::GroupSeg*)::malloc(tb);
-            if (!sb.segs.empty()) {
-                memcpy(l.dSegs, sb.segs.data(), sb.segs.size() * sizeof(fb::GroupSeg));
+            if (!segs.empty()) {
+                memcpy(l.dSegs, segs.data(), segs.size() * sizeof(fb::GroupSeg));
             }
             plan->launches.push_back(l);
             continue;
@@ -2106,8 +2112,8 @@ std::shared_ptr<Communicator::GroupPlan> Communicator::prepareGroup(
             return nullptr;
         }
         plan->launches.push_back(l);
-        if (!sb.segs.empty() &&
-            cudaMemcpy(l.dSegs, sb.segs.data(), sb.segs.size() * sizeof(fb::GroupSeg), cudaMemcpyHostToDevice) !=
+        if (!segs.empty() &&
+            cudaMemcpy(l.dSegs, segs.data(), segs.size() * sizeof(fb::GroupSeg), cudaMemcpyHostToDevice) !=
               cudaSuccess) {
             cudaGetLastError();
             rc = FB_E_CUDA;
@@ -2131,9 +2137,14 @@ static int groupGrid(const CommConfig& cfg, int nranks, uint64_t vecsPerRank)
     return (int)std::clamp<uint64_t>(want, 1, (uint64_t)cap);
 }
 
-int Communicator::launchGroup(const GroupLaunch& l, GroupKind kind, int dtype, int op, int flags, cudaStream_t s)
+int Communicator::launchGroup(const GroupLaunch& l,
+                              GroupKind kind,
+                              int dtype,
+                              int op,
+                              int root,
+                              int flags,
+                              cudaStream_t s)
 {
-    // (a broadcast passes its root as `op`)
     const int n = dev_.nranks;
     const bool ss = streamSync_ && !(flags & FB_FLAG_NOSYNC) && n > 1;
     fb::GroupArgs a;
@@ -2143,7 +2154,7 @@ int Communicator::launchGroup(const GroupLaunch& l, GroupKind kind, int dtype, i
     a.nSegs = l.nSegs;
     a.totalChunks = l.totalChunks;
     a.noSync = ((flags & FB_FLAG_NOSYNC) || ss || n == 1) ? 1 : 0;
-    a.root = kind == GROUP_BROADCAST ? op : 0;
+    a.root = kind == GROUP_BROADCAST ? root : 0;
     if (ss && streamBarrier(flags, s) != FB_OK) {
         return FB_E_CUDA;
     }
@@ -2180,142 +2191,85 @@ int Communicator::launchGroup(const GroupLaunch& l, GroupKind kind, int dtype, i
     return FB_OK;
 }
 
-int Communicator::allReduceGroup(const GroupPlan& plan, int op, int flags, cudaStream_t s)
+namespace {
+// Indexed by GroupKind: the NVTX ranges of runGroup and groupMany, and the
+// kind's name in messages
+struct GroupKindNames
 {
-    NvtxRange nvtxRange("fb::allReduceGroup");
-    if (plan.kind != GROUP_ALLREDUCE) {
+    const char* run;
+    const char* many;
+    const char* name;
+};
+#define FB_GROUP_NAMES(stem, name) { "fb::" stem "Group", "fb::" stem "Many", name }
+const GroupKindNames kGroupNames[] = {
+    FB_GROUP_NAMES("allReduce", "all-reduce"), FB_GROUP_NAMES("reduceScatter", "reduce-scatter"),
+    FB_GROUP_NAMES("allGather", "all-gather"), FB_GROUP_NAMES("broadcast", "broadcast"),
+    FB_GROUP_NAMES("allToAll", "all-to-all"),
+};
+#undef FB_GROUP_NAMES
+
+// groupCheck: a valid call with nothing to launch
+const int GROUP_NOTHING = 1;
+}
+
+const char* Communicator::groupKindName(GroupKind kind)
+{
+    return kind >= GROUP_ALLREDUCE && kind <= GROUP_ALLTOALL ? kGroupNames[kind].name : "unknown";
+}
+
+// The rules runGroup and groupMany share (see the header).  FB_OK, with
+// `grouped` false when a reducing pair has no grouped kernel; GROUP_NOTHING;
+// or an error code.
+int Communicator::groupCheck(GroupKind kind, int dtype, int op, int root, bool& grouped) const
+{
+    if (fbDtypeSize(dtype) == 0) {
         return FB_E_INVALID;
     }
-    const fb::ReduceLaunchers* L = fb::findReduceLaunchers(plan.dtype, op);
-    if (L == nullptr || L->group == nullptr) {
+    // all-gather, broadcast and all-to-all are byte copies: any dtype has a
+    // kernel
+    grouped = true;
+    if (kind == GROUP_ALLREDUCE || kind == GROUP_REDUCE_SCATTER) {
+        const fb::ReduceLaunchers* L = fb::findReduceLaunchers(dtype, op);
+        if (L == nullptr) {
+            return FB_E_UNSUPPORTED;
+        }
+        grouped = (kind == GROUP_ALLREDUCE ? L->group : L->groupRs) != nullptr;
+    } else if (kind == GROUP_BROADCAST) {
+        if (root < 0 || root >= dev_.nranks) {
+            return FB_E_INVALID;
+        }
+        if (dev_.nranks == 1) {
+            return GROUP_NOTHING; // the root's buffers already hold the result
+        }
+    }
+    return FB_OK;
+}
+
+int Communicator::runGroup(GroupKind kind, const GroupPlan& plan, int op, int root, int flags, cudaStream_t s)
+{
+    if (plan.kind != kind) {
+        return FB_E_INVALID;
+    }
+    NvtxRange nvtxRange(kGroupNames[kind].run);
+    bool grouped = false;
+    int rc = groupCheck(kind, plan.dtype, op, root, grouped);
+    if (rc != FB_OK) {
+        return rc == GROUP_NOTHING ? FB_OK : rc;
+    }
+    if (!grouped) {
         return FB_E_UNSUPPORTED;
     }
     bindDevice();
     for (const auto& l : plan.launches) {
-        int rc = launchGroup(l, GROUP_ALLREDUCE, plan.dtype, op, flags, s);
+        rc = launchGroup(l, kind, plan.dtype, op, root, flags, s);
         if (rc != FB_OK) {
             return rc;
         }
     }
-    lastAlgo_ = FB_ALGO_TWOSHOT;
-    return FB_OK;
-}
-
-int Communicator::reduceScatterGroup(const GroupPlan& plan, int op, int flags, cudaStream_t s)
-{
-    NvtxRange nvtxRange("fb::reduceScatterGroup");
-    if (plan.kind != GROUP_REDUCE_SCATTER) {
-        return FB_E_INVALID;
-    }
-    const fb::ReduceLaunchers* L = fb::findReduceLaunchers(plan.dtype, op);
-    if (L == nullptr || L->groupRs == nullptr) {
-        return FB_E_UNSUPPORTED;
-    }
-    bindDevice();
-    for (const auto& l : plan.launches) {
-        int rc = launchGroup(l, GROUP_REDUCE_SCATTER, plan.dtype, op, flags, s);
-        if (rc != FB_OK) {
-            return rc;
-        }
+    if (kind == GROUP_ALLREDUCE) {
+        lastAlgo_ = FB_ALGO_TWOSHOT;
     }
     return FB_OK;
-}
-
-int Communicator::allGatherGroup(const GroupPlan& plan, int flags, cudaStream_t s)
-{
-    NvtxRange nvtxRange("fb::allGatherGroup");
-    if (plan.kind != GROUP_ALLGATHER) {
-        return FB_E_INVALID;
-    }
-    bindDevice();
-    for (const auto& l : plan.launches) {
-        int rc = launchGroup(l, GROUP_ALLGATHER, plan.dtype, -1, flags, s);
-        if (rc != FB_OK) {
-            return rc;
-        }
-    }
-    return FB_OK;
-}
-
-int Communicator::broadcastGroup(const GroupPlan& plan, int root, int flags, cudaStream_t s)
-{
-    NvtxRange nvtxRange("fb::broadcastGroup");
-    if (plan.kind != GROUP_BROADCAST || root < 0 || root >= dev_.nranks) {
-        return FB_E_INVALID;
-    }
-    if (dev_.nranks == 1) {
-        return FB_OK; // the root's buffers already hold the result
-    }
-    bindDevice();
-    for (const auto& l : plan.launches) {
-        int rc = launchGroup(l, GROUP_BROADCAST, plan.dtype, root, flags, s);
-        if (rc != FB_OK) {
-            return rc;
-        }
-    }
-    return FB_OK;
-}
-
-int Communicator::allToAllGroup(const GroupPlan& plan, int flags, cudaStream_t s)
-{
-    NvtxRange nvtxRange("fb::allToAllGroup");
-    if (plan.kind != GROUP_ALLTOALL) {
-        return FB_E_INVALID;
-    }
-    bindDevice();
-    for (const auto& l : plan.launches) {
-        int rc = launchGroup(l, GROUP_ALLTOALL, plan.dtype, -1, flags, s);
-        if (rc != FB_OK) {
-            return rc;
-        }
-    }
-    return FB_OK;
-}
-
-int Communicator::allReduceMany(const GroupItem* items,
-                                size_t nItems,
-                                int dtype,
-                                int op,
-                                int flags,
-                                cudaStream_t s)
-{
-    NvtxRange nvtxRange("fb::allReduceMany");
-    return groupMany(GROUP_ALLREDUCE, items, nItems, dtype, op, flags, s);
-}
-
-int Communicator::reduceScatterMany(const GroupItem* items,
-                                    size_t nItems,
-                                    int dtype,
-                                    int op,
-                                    int flags,
-                                    cudaStream_t s)
-{
-    NvtxRange nvtxRange("fb::reduceScatterMany");
-    return groupMany(GROUP_REDUCE_SCATTER, items, nItems, dtype, op, flags, s);
-}
-
-int Communicator::allGatherMany(const GroupItem* items, size_t nItems, int dtype, int flags, cudaStream_t s)
-{
-    NvtxRange nvtxRange("fb::allGatherMany");
-    return groupMany(GROUP_ALLGATHER, items, nItems, dtype, -1, flags, s);
-}
-
-int Communicator::broadcastMany(const GroupItem* items, size_t nItems, int root, int flags, cudaStream_t s)
-{
-    NvtxRange nvtxRange("fb::broadcastMany");
-    if (root < 0 || root >= dev_.nranks) {
-        return FB_E_INVALID;
-    }
-    if (dev_.nranks == 1) {
-        return FB_OK;
-    }
-    return groupMany(GROUP_BROADCAST, items, nItems, FB_U8, root, flags, s);
-}
-
-int Communicator::allToAllMany(const GroupItem* items, size_t nItems, int dtype, int flags, cudaStream_t s)
-{
-    NvtxRange nvtxRange("fb::allToAllMany");
-    return groupMany(GROUP_ALLTOALL, items, nItems, dtype, -1, flags, s);
 }
 
 int Communicator::groupMany(GroupKind kind,
@@ -2323,104 +2277,104 @@ int Communicator::groupMany(GroupKind kind,
                             size_t nItems,
                             int dtype,
                             int op,
+                            int root,
                             int flags,
                             cudaStream_t s)
 {
-    const size_t esize = fbDtypeSize(dtype);
-    if (esize == 0) {
+    if (kind < GROUP_ALLREDUCE || kind > GROUP_ALLTOALL) {
         return FB_E_INVALID;
     }
-    // all-gather, broadcast and all-to-all are byte copies: any dtype has a
-    // kernel
-    bool grouped = true;
-    if (kind == GROUP_ALLREDUCE || kind == GROUP_REDUCE_SCATTER) {
-        const fb::ReduceLaunchers* L = fb::findReduceLaunchers(dtype, op);
-        if (L == nullptr) {
-            return FB_E_UNSUPPORTED;
-        }
-        grouped = (kind == GROUP_ALLREDUCE ? L->group : L->groupRs) != nullptr;
+    NvtxRange nvtxRange(kGroupNames[kind].many);
+    bool grouped = false;
+    int rc = groupCheck(kind, dtype, op, root, grouped);
+    if (rc != FB_OK) {
+        return rc == GROUP_NOTHING ? FB_OK : rc;
     }
-    const size_t n = (size_t)dev_.nranks;
+    const size_t esize = fbDtypeSize(dtype);
     bindDevice();
     // try the grouped path batch by batch; anything not symmetric / aligned
     // goes through the per-tensor calls (the choice depends only on arguments
     // that are symmetric across ranks)
     for (size_t begin = 0; begin < nItems; begin += GROUP_ITEMS_PER_LAUNCH) {
         const size_t cnt = std::min(GROUP_ITEMS_PER_LAUNCH, nItems - begin);
-        SegBuild sb;
-        int rc = grouped ? buildSegs(*this, kind, items + begin, cnt, esize, sb) : FB_E_UNSUPPORTED;
+        std::vector<fb::GroupSeg> segs;
+        GroupLaunch l;
+        rc = grouped ? groupBatch(kind, items + begin, cnt, esize, segs, l) : FB_E_UNSUPPORTED;
         if (rc != FB_OK) {
-            for (size_t i = begin; i < begin + cnt; i++) {
-                const GroupItem& it = items[i];
-                const size_t bytes = it.count * esize;
-                int f = flags;
-                int r2 = FB_OK;
-                if (kind == GROUP_ALLREDUCE) {
-                    if (!inHeap(it.send, bytes)) {
-                        f &= ~FB_FLAG_SYMMETRIC;
-                    }
-                    r2 = allReduce(it.send, it.recv, it.count, dtype, op, FB_ALGO_AUTO, f, s);
-                } else if (bytes == 0) {
-                    continue;
-                } else if (kind == GROUP_BROADCAST) {
-                    if (!inHeap(it.recv, bytes)) {
-                        f &= ~FB_FLAG_SYMMETRIC;
-                    }
-                    r2 = broadcast(it.recv, bytes, op, f, s);
-                } else if (kind == GROUP_REDUCE_SCATTER) {
-                    if (!inHeap(it.send, bytes * n)) {
-                        f &= ~FB_FLAG_SYMMETRIC;
-                    }
-                    r2 = reduceScatter(it.send, it.recv, it.count, dtype, op, f, s);
-                } else if (kind == GROUP_ALLTOALL) {
-                    if (!inHeap(it.send, bytes * n)) {
-                        f &= ~FB_FLAG_SYMMETRIC;
-                    }
-                    r2 = allToAll(it.send, it.recv, bytes, f, s);
-                } else {
-                    if (!inHeap(it.send, bytes)) {
-                        f &= ~FB_FLAG_SYMMETRIC;
-                    }
-                    r2 = allGather(it.send, it.recv, bytes, f, s);
-                }
-                if (r2 != FB_OK) {
-                    return r2;
-                }
+            rc = groupPerItem(kind, items + begin, cnt, dtype, op, root, flags, s);
+            if (rc != FB_OK) {
+                return rc;
             }
             continue;
         }
-        GroupLaunch l;
-        l.dSegs = sb.segs.data(); // the host twin reads the table in place
-        l.nSegs = (uint32_t)sb.segs.size();
-        l.totalChunks = sb.totalChunks;
-        l.vecsPerRank = sb.vecsPerRank;
-        l.bytes = sb.bytes;
         ManySlot* slot = nullptr;
-        if (!loop_) {
-            slot = nextManySlot();
-            if (slot == nullptr) {
-                return FB_E_CUDA;
-            }
-            if (!sb.segs.empty()) {
-                memcpy(slot->hSegs, sb.segs.data(), sb.segs.size() * sizeof(fb::GroupSeg));
-                if (cudaMemcpyAsync(slot->dSegs, slot->hSegs, sb.segs.size() * sizeof(fb::GroupSeg), cudaMemcpyHostToDevice, s) !=
-                    cudaSuccess) {
-                    return FB_E_CUDA;
-                }
-            }
-            l.dSegs = slot->dSegs;
+        l.dSegs = (fb::GroupSeg*)stageManyTable(segs.data(), segs.size() * sizeof(fb::GroupSeg), s, &slot);
+        // (on loopback an empty table is a null pointer the kernel never reads)
+        if (l.dSegs == nullptr && !loop_) {
+            return FB_E_CUDA;
         }
-        rc = launchGroup(l, kind, dtype, op, flags, s);
+        rc = launchGroup(l, kind, dtype, op, root, flags, s);
         if (rc != FB_OK) {
             return rc;
         }
-        if (slot != nullptr) {
-            cudaEventRecord(slot->ev, s);
-            slot->used = true;
-        }
+        releaseManySlot(slot, s);
     }
     if (kind == GROUP_ALLREDUCE) {
         lastAlgo_ = FB_ALGO_TWOSHOT;
+    }
+    return FB_OK;
+}
+
+// The per-item calls of a batch that cannot be grouped, in list order; a
+// buffer outside the heap drops FB_FLAG_SYMMETRIC.  Empty items are skipped,
+// except by the all-reduce.
+int Communicator::groupPerItem(GroupKind kind,
+                               const GroupItem* items,
+                               size_t nItems,
+                               int dtype,
+                               int op,
+                               int root,
+                               int flags,
+                               cudaStream_t s)
+{
+    const size_t esize = fbDtypeSize(dtype);
+    const size_t n = (size_t)dev_.nranks;
+    for (size_t i = 0; i < nItems; i++) {
+        const GroupItem& it = items[i];
+        const size_t bytes = it.count * esize;
+        int f = flags;
+        int rc = FB_OK;
+        if (kind == GROUP_ALLREDUCE) {
+            if (!inHeap(it.send, bytes)) {
+                f &= ~FB_FLAG_SYMMETRIC;
+            }
+            rc = allReduce(it.send, it.recv, it.count, dtype, op, FB_ALGO_AUTO, f, s);
+        } else if (bytes == 0) {
+            continue;
+        } else if (kind == GROUP_BROADCAST) {
+            if (!inHeap(it.recv, bytes)) {
+                f &= ~FB_FLAG_SYMMETRIC;
+            }
+            rc = broadcast(it.recv, bytes, root, f, s);
+        } else if (kind == GROUP_REDUCE_SCATTER) {
+            if (!inHeap(it.send, bytes * n)) {
+                f &= ~FB_FLAG_SYMMETRIC;
+            }
+            rc = reduceScatter(it.send, it.recv, it.count, dtype, op, f, s);
+        } else if (kind == GROUP_ALLTOALL) {
+            if (!inHeap(it.send, bytes * n)) {
+                f &= ~FB_FLAG_SYMMETRIC;
+            }
+            rc = allToAll(it.send, it.recv, bytes, f, s);
+        } else {
+            if (!inHeap(it.send, bytes)) {
+                f &= ~FB_FLAG_SYMMETRIC;
+            }
+            rc = allGather(it.send, it.recv, bytes, f, s);
+        }
+        if (rc != FB_OK) {
+            return rc;
+        }
     }
     return FB_OK;
 }
@@ -3247,9 +3201,11 @@ const void* Communicator::stageManyTable(const void* table, size_t bytes, cudaSt
     if (sl == nullptr) {
         return nullptr;
     }
-    memcpy(sl->hSegs, table, bytes);
-    if (cudaMemcpyAsync(sl->dSegs, sl->hSegs, bytes, cudaMemcpyHostToDevice, s) != cudaSuccess) {
-        return nullptr;
+    if (bytes > 0) {
+        memcpy(sl->hSegs, table, bytes);
+        if (cudaMemcpyAsync(sl->dSegs, sl->hSegs, bytes, cudaMemcpyHostToDevice, s) != cudaSuccess) {
+            return nullptr;
+        }
     }
     *slot = sl;
     return sl->dSegs;

@@ -84,13 +84,14 @@ struct RankState
     // MPI_Iallreduce, MPI_Ireduce_scatter_block, MPI_Iallgather or MPI_Ibcast
     // burst on symmetric device buffers: deferred and issued as ONE grouped
     // kernel at the next wait (or any other device operation).  A burst has
-    // one key: (kind, communicator, dtype, op); all-gather and broadcast
-    // bursts are bytes, no op, and a broadcast's root takes the op's place.
-    // The communicator is the world's or a sub-communicator's child.
+    // one key: (kind, communicator, dtype, op, root); the byte-copy kinds are
+    // FB_U8 with op -1, and only a broadcast has a root.  The communicator is
+    // the world's or a sub-communicator's child.
     faabric::device::Communicator::GroupKind groupKind = faabric::device::Communicator::GROUP_ALLREDUCE;
     std::shared_ptr<faabric::device::Communicator> groupComm;
     int groupDtype = -1;
     int groupOp = -1;
+    int groupRoot = 0;
     void* groupStream = nullptr;
     std::vector<faabric::device::Communicator::GroupItem> groupItems;
     std::vector<int> groupRequests;
@@ -971,27 +972,14 @@ static void flushPendingGroup()
     tls.groupComm = nullptr;
     cudaSetDevice(comm->device());
     const cudaStream_t s = (cudaStream_t)tls.groupStream;
-    int rc;
-    const char* what;
-    if (tls.groupKind == Communicator::GROUP_REDUCE_SCATTER) {
-        rc = comm->reduceScatterMany(items.data(), items.size(), tls.groupDtype, tls.groupOp, FB_FLAG_SYMMETRIC, s);
-        what = "Grouped device reduce-scatter";
-    } else if (tls.groupKind == Communicator::GROUP_ALLGATHER) {
-        rc = comm->allGatherMany(items.data(), items.size(), tls.groupDtype, FB_FLAG_SYMMETRIC, s);
-        what = "Grouped device all-gather";
-    } else if (tls.groupKind == Communicator::GROUP_BROADCAST) {
-        rc = comm->broadcastMany(items.data(), items.size(), tls.groupOp, FB_FLAG_SYMMETRIC, s);
-        what = "Grouped device broadcast";
-    } else if (tls.groupKind == Communicator::GROUP_ALLTOALL) {
-        rc = comm->allToAllMany(items.data(), items.size(), tls.groupDtype, FB_FLAG_SYMMETRIC, s);
-        what = "Grouped device all-to-all";
-    } else {
-        rc = comm->allReduceMany(items.data(), items.size(), tls.groupDtype, tls.groupOp, FB_FLAG_SYMMETRIC, s);
-        what = "Grouped device all-reduce";
-    }
-    // (the burst's requests have no host path left: declining is an error too)
-    if (!deviceIssued(rc, what)) {
-        throw std::runtime_error(std::string(what) + " declined: " + Communicator::errorString(rc));
+    const int rc = comm->groupMany(
+      tls.groupKind, items.data(), items.size(), tls.groupDtype, tls.groupOp, tls.groupRoot, FB_FLAG_SYMMETRIC, s);
+    if (rc != FB_OK) {
+        const std::string what = std::string("Grouped device ") + Communicator::groupKindName(tls.groupKind);
+        // (the burst's requests have no host path left: declining is an error too)
+        if (!deviceIssued(rc, what.c_str())) {
+            throw std::runtime_error(what + " declined: " + Communicator::errorString(rc));
+        }
     }
     const uint64_t seq = ++tls.groupLaunchSeq;
     for (int id : reqs) {
@@ -1510,19 +1498,21 @@ static void deferToGroup(faabric::device::Communicator::GroupKind kind,
                          const std::shared_ptr<faabric::device::Communicator>& comm,
                          int dtype,
                          int op,
+                         int root,
                          const faabric::device::Communicator::GroupItem& item,
                          int requestId,
                          AsyncRequest r,
                          std::atomic<uint64_t>& counter)
 {
     if (!tls.groupItems.empty() && (tls.groupKind != kind || tls.groupComm != comm || tls.groupDtype != dtype ||
-                                    tls.groupOp != op || tls.groupItems.size() >= 4096)) {
+                                    tls.groupOp != op || tls.groupRoot != root || tls.groupItems.size() >= 4096)) {
         flushPendingGroup();
     }
     tls.groupKind = kind;
     tls.groupComm = comm;
     tls.groupDtype = dtype;
     tls.groupOp = op;
+    tls.groupRoot = root;
     tls.groupStream = tls.cachedStream0;
     tls.groupItems.push_back(item);
     tls.groupRequests.push_back(requestId);
@@ -1596,6 +1586,7 @@ int MpiWorld::nbAllReduce(const DeviceComm& comm,
                          comm,
                          fdt,
                          fop,
+                         0,
                          { send, recv, (size_t)count },
                          requestId,
                          std::move(r),
@@ -1619,6 +1610,52 @@ int MpiWorld::nbAllReduce(const DeviceComm& comm,
         }
     }
     // Host path (or unsupported on the device): complete it now
+    host();
+    tls.requests[requestId] = std::move(r);
+    return requestId;
+}
+
+// One call of nbReduceScatter, nbAllGather, nbBroadcast or nbAllToAll: the
+// extents of item.send and item.recv and the shard size its placement is
+// judged on, its burst key, its burst item, and whether buffers that cannot
+// join a burst may run the single device call at issue
+struct MpiWorld::NbCall
+{
+    size_t sendBytes;
+    size_t recvBytes;
+    size_t shardBytes;
+    faabric::device::Communicator::GroupKind kind;
+    int dtype;
+    int op;
+    int root;
+    faabric::device::Communicator::GroupItem item;
+    bool direct = true;
+};
+
+// Symmetric, aligned buffers of a call the device takes (`device`) join this
+// rank's burst; other device buffers run `issue` on stream 0; anything else
+// runs `host`, which completes the request at issue
+template <typename Issue>
+int MpiWorld::nbCollective(const DeviceComm& comm, int rank, bool device, const NbCall& call, Issue&& issue,
+                           const HostPath& host)
+{
+    const int requestId = tls.nextRequestId++;
+    AsyncRequest r = collectiveRequest(rank);
+    cacheDeviceComm(rank);
+    if (device && comm != nullptr) {
+        const Placement at = placeCollective(
+          *comm, groupIallreduce, call.item.send, call.sendBytes, call.item.recv, call.recvBytes, call.shardBytes);
+        if (at.grouped) {
+            deferToGroup(call.kind, comm, call.dtype, call.op, call.root, call.item, requestId, std::move(r),
+                         deviceCollectives);
+            return requestId;
+        }
+        void* s = tls.cachedStream0;
+        if (call.direct && (at.symmetric || isDevicePointer(call.item.send)) &&
+            issueDevice(*comm, s, deviceCollectives, issue)) {
+            return recordDevice(requestId, std::move(r), comm, s);
+        }
+    }
     host();
     tls.requests[requestId] = std::move(r);
     return requestId;
@@ -1648,39 +1685,17 @@ int MpiWorld::nbReduceScatter(const DeviceComm& comm,
                               faabric_op_t* op,
                               const HostPath& host)
 {
-    using faabric::device::Communicator;
     const size_t shard = (size_t)recvCount * dt->size;
-    const int requestId = tls.nextRequestId++;
-    AsyncRequest r = collectiveRequest(rank);
     const int fdt = fbDtypeFor(dt);
     const int fop = fbOpFor(op);
-    cacheDeviceComm(rank);
     // In place, the output overwrites input the peers are still reading: that
-    // case (send == recv) runs the blocking call below
-    if (shard > 0 && deviceReducible(dt, op) && comm != nullptr && send != recv) {
-        const Placement at = placeCollective(*comm, groupIallreduce, send, shard * members, recv, shard, shard);
-        if (at.grouped) {
-            deferToGroup(Communicator::GROUP_REDUCE_SCATTER,
-                         comm,
-                         fdt,
-                         fop,
-                         { send, recv, (size_t)recvCount },
-                         requestId,
-                         std::move(r),
-                         deviceCollectives);
-            return requestId;
-        }
-        void* s = tls.cachedStream0;
-        if ((at.symmetric || isDevicePointer(send)) && issueDevice(*comm, s, deviceCollectives, [&](auto& c, cudaStream_t st) {
-                return c.reduceScatter(send, recv, (size_t)recvCount, fdt, fop, symFlag(c, send, shard * members), st);
-            })) {
-            return recordDevice(requestId, std::move(r), comm, s);
-        }
-    }
-    // Host buffers, in place, or unsupported on the device: complete it now
-    host();
-    tls.requests[requestId] = std::move(r);
-    return requestId;
+    // case (send == recv) runs the blocking call
+    const NbCall call{ shard * members, shard, shard, faabric::device::Communicator::GROUP_REDUCE_SCATTER, fdt, fop, 0,
+                       { send, recv, (size_t)recvCount } };
+    const bool device = shard > 0 && deviceReducible(dt, op) && send != recv;
+    return nbCollective(comm, rank, device, call, [&](auto& c, cudaStream_t st) {
+        return c.reduceScatter(send, recv, (size_t)recvCount, fdt, fop, symFlag(c, send, shard * members), st);
+    }, host);
 }
 
 int MpiWorld::iAllGather(int rank,
@@ -1706,30 +1721,14 @@ int MpiWorld::nbAllGather(const DeviceComm& comm,
                           size_t bytes,
                           const HostPath& host)
 {
-    using faabric::device::Communicator;
-    const int requestId = tls.nextRequestId++;
-    AsyncRequest r = collectiveRequest(rank);
-    cacheDeviceComm(rank);
-    if (bytes > 0 && comm != nullptr) {
-        const bool inPlace = send == recv + (size_t)comm->rank() * bytes;
-        const Placement at = placeCollective(*comm, groupIallreduce, send, bytes, recv, bytes * members, bytes);
-        if (at.grouped) {
-            // a byte copy: the burst's key is the communicator alone
-            deferToGroup(Communicator::GROUP_ALLGATHER, comm, FB_U8, -1, { send, recv, bytes }, requestId, std::move(r), deviceCollectives);
-            return requestId;
-        }
-        void* s = tls.cachedStream0;
-        if (!inPlace && (at.symmetric || isDevicePointer(send)) &&
-            issueDevice(*comm, s, deviceCollectives, [&](auto& c, cudaStream_t st) {
-                return c.allGather(send, recv, bytes, symFlag(c, send, bytes), st);
-            })) {
-            return recordDevice(requestId, std::move(r), comm, s);
-        }
-    }
-    // Host buffers, or unsupported on the device: complete it now
-    host();
-    tls.requests[requestId] = std::move(r);
-    return requestId;
+    // a byte copy: the burst's key is the communicator alone.  In place, only
+    // the burst runs it on the device.
+    NbCall call{ bytes, bytes * members, bytes, faabric::device::Communicator::GROUP_ALLGATHER, FB_U8, -1, 0,
+                 { send, recv, bytes } };
+    call.direct = comm == nullptr || send != recv + (size_t)comm->rank() * bytes;
+    return nbCollective(comm, rank, bytes > 0, call, [&](auto& c, cudaStream_t st) {
+        return c.allGather(send, recv, bytes, symFlag(c, send, bytes), st);
+    }, host);
 }
 
 int MpiWorld::iBroadcast(int rank, int root, uint8_t* buffer, faabric_datatype_t* dt, int count)
@@ -1743,30 +1742,12 @@ int MpiWorld::iBroadcast(int rank, int root, uint8_t* buffer, faabric_datatype_t
 
 int MpiWorld::nbBroadcast(const DeviceComm& comm, int rank, int root, uint8_t* buffer, size_t bytes, const HostPath& host)
 {
-    using faabric::device::Communicator;
-    const int requestId = tls.nextRequestId++;
-    AsyncRequest r = collectiveRequest(rank);
-    cacheDeviceComm(rank);
-    if (bytes > 0 && comm != nullptr) {
-        const Placement at = placeCollective(*comm, groupIallreduce, buffer, bytes, buffer, bytes, 0);
-        if (at.grouped) {
-            // a byte copy: the burst's key is (communicator, root); the root
-            // travels in the op slot of the key
-            deferToGroup(Communicator::GROUP_BROADCAST, comm, FB_U8, root, { buffer, buffer, bytes }, requestId, std::move(r),
-                         deviceCollectives);
-            return requestId;
-        }
-        void* s = tls.cachedStream0;
-        if ((at.symmetric || isDevicePointer(buffer)) && issueDevice(*comm, s, deviceCollectives, [&](auto& c, cudaStream_t st) {
-                return c.broadcast(buffer, bytes, root, symFlag(c, buffer, bytes), st);
-            })) {
-            return recordDevice(requestId, std::move(r), comm, s);
-        }
-    }
-    // Host buffers, or unsupported on the device: complete it now
-    host();
-    tls.requests[requestId] = std::move(r);
-    return requestId;
+    // a byte copy: the burst's key is (communicator, root)
+    const NbCall call{ bytes, bytes, 0, faabric::device::Communicator::GROUP_BROADCAST, FB_U8, -1, root,
+                       { buffer, buffer, bytes } };
+    return nbCollective(comm, rank, bytes > 0, call, [&](auto& c, cudaStream_t st) {
+        return c.broadcast(buffer, bytes, root, symFlag(c, buffer, bytes), st);
+    }, host);
 }
 
 int MpiWorld::iAllToAll(int rank,
@@ -1792,29 +1773,13 @@ int MpiWorld::nbAllToAll(const DeviceComm& comm,
                          size_t bytes,
                          const HostPath& host)
 {
-    using faabric::device::Communicator;
-    const int requestId = tls.nextRequestId++;
-    AsyncRequest r = collectiveRequest(rank);
-    cacheDeviceComm(rank);
-    if (bytes > 0 && comm != nullptr) {
-        const size_t total = bytes * (size_t)members;
-        const Placement at = placeCollective(*comm, groupIallreduce, send, total, recv, total, bytes);
-        if (at.grouped) {
-            // a byte copy: the burst's key is the communicator alone
-            deferToGroup(Communicator::GROUP_ALLTOALL, comm, FB_U8, -1, { send, recv, bytes }, requestId, std::move(r), deviceCollectives);
-            return requestId;
-        }
-        void* s = tls.cachedStream0;
-        if ((at.symmetric || isDevicePointer(send)) && issueDevice(*comm, s, deviceCollectives, [&](auto& c, cudaStream_t st) {
-                return c.allToAll(send, recv, bytes, symFlag(c, send, total), st);
-            })) {
-            return recordDevice(requestId, std::move(r), comm, s);
-        }
-    }
-    // Host buffers, or unsupported on the device: complete it now
-    host();
-    tls.requests[requestId] = std::move(r);
-    return requestId;
+    // a byte copy: the burst's key is the communicator alone
+    const size_t total = bytes * (size_t)members;
+    const NbCall call{ total, total, bytes, faabric::device::Communicator::GROUP_ALLTOALL, FB_U8, -1, 0,
+                       { send, recv, bytes } };
+    return nbCollective(comm, rank, bytes > 0, call, [&](auto& c, cudaStream_t st) {
+        return c.allToAll(send, recv, bytes, symFlag(c, send, total), st);
+    }, host);
 }
 
 void MpiWorld::settleDeviceBurst(const DeviceComm& comm)

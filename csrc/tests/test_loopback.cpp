@@ -790,7 +790,7 @@ TEST_CASE("loopback: grouped all-reduce equals per-tensor all-reduces", "[loopba
             int rc = FB_OK;
             auto plan = c.prepareGroup(items.data(), items.size(), FB_I16, &rc);
             bool ok = plan != nullptr && rc == FB_OK && Communicator::groupPlanLaunches(*plan) == 1;
-            ok = ok && c.allReduceGroup(*plan, FB_OP_SUM, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+            ok = ok && c.runGroup(Communicator::GROUP_ALLREDUCE, *plan, FB_OP_SUM, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
             for (size_t t = 0; t < sizes.size() && ok; t++) {
                 for (size_t i = 0; i < sizes[t] && ok; i++) {
                     ok = recvs[t][i] == (int16_t)((i % 97) * n + n * (n - 1) / 2);
@@ -801,7 +801,7 @@ TEST_CASE("loopback: grouped all-reduce equals per-tensor all-reduces", "[loopba
             for (auto& it : items) {
                 it.recv = const_cast<void*>(it.send);
             }
-            ok = ok && c.allReduceMany(items.data(), items.size(), FB_I16, FB_OP_MAX, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+            ok = ok && c.groupMany(Communicator::GROUP_ALLREDUCE, items.data(), items.size(), FB_I16, FB_OP_MAX, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
             for (size_t t = 0; t < sizes.size() && ok; t++) {
                 for (size_t i = 0; i < sizes[t] && ok; i++) {
                     ok = sends[t][i] == (int16_t)((i % 97) + n - 1);
@@ -834,7 +834,7 @@ TEST_CASE("loopback: a group larger than one segment table is split into launche
         int rc = FB_OK;
         auto plan = c.prepareGroup(items.data(), items.size(), FB_I32, &rc);
         bool ok = plan != nullptr && Communicator::groupPlanLaunches(*plan) == 3;
-        ok = ok && c.allReduceGroup(*plan, FB_OP_SUM, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+        ok = ok && c.runGroup(Communicator::GROUP_ALLREDUCE, *plan, FB_OP_SUM, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
         for (size_t i = 0; i < k && ok; i++) {
             for (size_t j = 0; j < 16 && ok; j++) {
                 int32_t own = (int32_t)(i + j) + rank;

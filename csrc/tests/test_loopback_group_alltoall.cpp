@@ -1,4 +1,4 @@
-// Grouped all-to-all (Communicator::allToAllGroup / allToAllMany) on the
+// Grouped all-to-all (Communicator::runGroup / groupMany, GROUP_ALLTOALL) on the
 // loopback backend (no GPU): every byte of the buffers, random guard bytes
 // between blocks included, against an exchange computed on the host at 1-8
 // ranks; launch counts; refusals and fall-backs; a plan on a sub-communicator
@@ -190,10 +190,10 @@ TEST_CASE("loopback group alltoall: plans and transient lists byte-exact at 1-8 
                         int rc = FB_OK;
                         auto plan = c.prepareGroup(list.data(), list.size(), dtype, &rc, Communicator::GROUP_ALLTOALL);
                         if (plan == nullptr || Communicator::groupPlanLaunches(*plan) != 1 ||
-                            c.allToAllGroup(*plan, FB_FLAG_SYMMETRIC, nullptr) != FB_OK) {
+                            c.runGroup(Communicator::GROUP_ALLTOALL, *plan, 0, 0, FB_FLAG_SYMMETRIC, nullptr) != FB_OK) {
                             return false;
                         }
-                    } else if (c.allToAllMany(list.data(), list.size(), dtype, FB_FLAG_SYMMETRIC, nullptr) != FB_OK) {
+                    } else if (c.groupMany(Communicator::GROUP_ALLTOALL, list.data(), list.size(), dtype, 0, 0, FB_FLAG_SYMMETRIC, nullptr) != FB_OK) {
                         return false;
                     }
                     size_t total = 0;
@@ -227,7 +227,7 @@ TEST_CASE("loopback group alltoall: 1017 items take two launches, 1016 one", "[l
             Communicator& c = *reg.comms[r];
             auto g = groupItems(c, reg.at(r), list, 4);
             const uint64_t l0 = c.stats().launches;
-            if (c.allToAllMany(g.data(), g.size(), FB_F32, FB_FLAG_SYMMETRIC, nullptr) != FB_OK) {
+            if (c.groupMany(Communicator::GROUP_ALLTOALL, g.data(), g.size(), FB_F32, 0, 0, FB_FLAG_SYMMETRIC, nullptr) != FB_OK) {
                 return false;
             }
             int rc = FB_OK;
@@ -268,7 +268,7 @@ TEST_CASE("loopback group alltoall: unaligned, off-heap and overlapping lists ar
             bool ok = c.prepareGroup(g.data(), g.size(), FB_U8, &rc, Communicator::GROUP_ALLTOALL) == nullptr &&
                       rc == FB_E_INVALID;
             const uint64_t l0 = c.stats().launches;
-            ok = ok && c.allToAllMany(g.data(), g.size(), FB_U8, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+            ok = ok && c.groupMany(Communicator::GROUP_ALLTOALL, g.data(), g.size(), FB_U8, 0, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
             // one per-item allToAll per item
             return ok && c.stats().launches == l0 + g.size() && c.checkError(nullptr) == 0;
         });
@@ -296,9 +296,9 @@ TEST_CASE("loopback group alltoall: unaligned, off-heap and overlapping lists ar
         auto ag = c.prepareGroup(g.data(), g.size(), FB_U8, &rc, Communicator::GROUP_ALLGATHER);
         const uint64_t l0 = c.stats().launches;
         bool ok = a2a && ag;
-        ok = ok && c.allToAllGroup(*ag, FB_FLAG_SYMMETRIC, nullptr) == FB_E_INVALID;
-        ok = ok && c.allGatherGroup(*a2a, FB_FLAG_SYMMETRIC, nullptr) == FB_E_INVALID;
-        ok = ok && c.broadcastGroup(*a2a, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_E_INVALID;
+        ok = ok && c.runGroup(Communicator::GROUP_ALLTOALL, *ag, 0, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_E_INVALID;
+        ok = ok && c.runGroup(Communicator::GROUP_ALLGATHER, *a2a, 0, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_E_INVALID;
+        ok = ok && c.runGroup(Communicator::GROUP_BROADCAST, *a2a, 0, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_E_INVALID;
         return ok && c.stats().launches == l0;
     });
     REQUIRE_EQ(fails, 0);
@@ -333,7 +333,7 @@ TEST_CASE("loopback group alltoall: a plan on a subset child exchanges among its
         // (16-byte elements: one per block)
         auto plan = child->prepareGroup(&g, 1, FB_F64_I32, &rc, Communicator::GROUP_ALLTOALL);
         const uint64_t l0 = child->stats().launches;
-        const bool ok = plan != nullptr && child->allToAllGroup(*plan, FB_FLAG_SYMMETRIC, nullptr) == FB_OK &&
+        const bool ok = plan != nullptr && child->runGroup(Communicator::GROUP_ALLTOALL, *plan, 0, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_OK &&
                         child->stats().launches == l0 + 1;
         plan.reset();
         child.reset();

@@ -1,4 +1,4 @@
-// Grouped broadcast (Communicator::broadcastGroup / broadcastMany) and the
+// Grouped broadcast (Communicator::runGroup / groupMany, GROUP_BROADCAST) and the
 // grouped calls on sub-communicator children, on the loopback backend (no
 // GPU): results against a closed form at 1-8 ranks, launch counts, refusals
 // and fall-backs, and the MPI program of mpi_group_subcomm_body.h.
@@ -129,14 +129,14 @@ TEST_CASE("loopback group broadcast: plans and transient lists from every root a
             for (int root = 0; root < n && ok; root++) {
                 const uint64_t l0 = c.stats().launches;
                 ok = ok && broadcastCase(c, base, root, [&](auto& items) {
-                    return c.broadcastMany(items.data(), items.size(), root, FB_FLAG_SYMMETRIC, nullptr);
+                    return c.groupMany(Communicator::GROUP_BROADCAST, items.data(), items.size(), FB_U8, 0, root, FB_FLAG_SYMMETRIC, nullptr);
                 });
                 ok = ok && c.stats().launches == l0 + (n > 1 ? 1 : 0);
                 std::shared_ptr<Communicator::GroupPlan> plan;
                 ok = ok && broadcastCase(c, base, root, [&](auto& items) {
                     int rc = FB_OK;
                     plan = c.prepareGroup(items.data(), items.size(), FB_U8, &rc, Communicator::GROUP_BROADCAST);
-                    return plan == nullptr ? rc : c.broadcastGroup(*plan, root, FB_FLAG_SYMMETRIC, nullptr);
+                    return plan == nullptr ? rc : c.runGroup(Communicator::GROUP_BROADCAST, *plan, 0, root, FB_FLAG_SYMMETRIC, nullptr);
                 });
                 ok = ok && plan && Communicator::groupPlanLaunches(*plan) == 1;
                 ok = ok && c.stats().launches == l0 + (n > 1 ? 2 : 0);
@@ -169,7 +169,7 @@ TEST_CASE("loopback group broadcast: 1017 items take two launches, 1016 one", "[
                 list.push_back({ base + i * 32, base + i * 32, 1 + i % 20 });
             }
             const uint64_t l0 = c.stats().launches;
-            ok = ok && c.broadcastMany(list.data(), list.size(), 1, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+            ok = ok && c.groupMany(Communicator::GROUP_BROADCAST, list.data(), list.size(), FB_U8, 0, 1, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
             ok = ok && c.stats().launches == l0 + (cnt == items ? 2 : 1);
             for (size_t i = 0; i < cnt && ok; i++) {
                 for (size_t j = 0; j < 32; j++) {
@@ -204,17 +204,17 @@ TEST_CASE("loopback group broadcast: refusals, and unaligned lists fall back to 
         auto arPlan = c.prepareGroup(&aligned, 1, FB_U8, &rc);
         ok = ok && plan && arPlan;
         const uint64_t l0 = c.stats().launches;
-        ok = ok && c.broadcastGroup(*plan, n, FB_FLAG_SYMMETRIC, nullptr) == FB_E_INVALID;
-        ok = ok && c.broadcastGroup(*plan, -1, FB_FLAG_SYMMETRIC, nullptr) == FB_E_INVALID;
-        ok = ok && c.broadcastGroup(*arPlan, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_E_INVALID;
-        ok = ok && c.broadcastMany(&aligned, 1, n, FB_FLAG_SYMMETRIC, nullptr) == FB_E_INVALID;
+        ok = ok && c.runGroup(Communicator::GROUP_BROADCAST, *plan, 0, n, FB_FLAG_SYMMETRIC, nullptr) == FB_E_INVALID;
+        ok = ok && c.runGroup(Communicator::GROUP_BROADCAST, *plan, 0, -1, FB_FLAG_SYMMETRIC, nullptr) == FB_E_INVALID;
+        ok = ok && c.runGroup(Communicator::GROUP_BROADCAST, *arPlan, 0, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_E_INVALID;
+        ok = ok && c.groupMany(Communicator::GROUP_BROADCAST, &aligned, 1, FB_U8, 0, n, FB_FLAG_SYMMETRIC, nullptr) == FB_E_INVALID;
         ok = ok && c.stats().launches == l0;
         // the unaligned list runs one broadcast per item, with the same bytes
         for (int j = 0; j < 200; j++) {
             base[j] = pattern(r, 0, j);
         }
         Communicator::GroupItem two[2] = { shifted, { base + 100, base + 100, 37 } };
-        ok = ok && c.broadcastMany(two, 2, 2, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+        ok = ok && c.groupMany(Communicator::GROUP_BROADCAST, two, 2, FB_U8, 0, 2, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
         for (int j = 0; j < 200 && ok; j++) {
             const bool in = (j >= 1 && j < 65) || (j >= 100 && j < 137);
             ok = base[j] == (in ? pattern(2, 0, j) : pattern(r, 0, j));
@@ -257,7 +257,7 @@ TEST_CASE("loopback subset group: every grouped kind runs on children of a parit
             }
             Communicator::GroupItem ar[2] = { { buf, buf, 40 }, { buf + 48, buf + 48, 16 } };
             const uint64_t l0 = child->stats().launches;
-            ok = ok && child->allReduceMany(ar, 2, FB_I32, FB_OP_SUM, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+            ok = ok && child->groupMany(Communicator::GROUP_ALLREDUCE, ar, 2, FB_I32, FB_OP_SUM, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
             int sum = 0;
             for (int p : members) {
                 sum += p;
@@ -272,7 +272,7 @@ TEST_CASE("loopback subset group: every grouped kind runs on children of a parit
                 rs[i] = r * 3 + i;
             }
             Communicator::GroupItem rsIt{ rs, rsOut, 4 };
-            ok = ok && child->reduceScatterMany(&rsIt, 1, FB_I32, FB_OP_SUM, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+            ok = ok && child->groupMany(Communicator::GROUP_REDUCE_SCATTER, &rsIt, 1, FB_I32, FB_OP_SUM, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
             for (int j = 0; j < 4 && ok; j++) {
                 ok = rsOut[j] == 3 * sum + m * (cr * 4 + j);
             }
@@ -283,7 +283,7 @@ TEST_CASE("loopback subset group: every grouped kind runs on children of a parit
                 ag[j] = r * 10 + j;
             }
             Communicator::GroupItem agIt{ ag, agOut, 4 };
-            ok = ok && child->allGatherMany(&agIt, 1, FB_I32, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+            ok = ok && child->groupMany(Communicator::GROUP_ALLGATHER, &agIt, 1, FB_I32, 0, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
             for (int q = 0; q < m && ok; q++) {
                 for (int j = 0; j < 4 && ok; j++) {
                     ok = agOut[q * 4 + j] == members[q] * 10 + j;
@@ -296,7 +296,7 @@ TEST_CASE("loopback subset group: every grouped kind runs on children of a parit
             }
             Communicator::GroupItem bcIt{ bc, bc, 21 };
             const int root = round % m;
-            ok = ok && child->broadcastMany(&bcIt, 1, root, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+            ok = ok && child->groupMany(Communicator::GROUP_BROADCAST, &bcIt, 1, FB_U8, 0, root, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
             for (int j = 0; j < 32 && ok; j++) {
                 ok = bc[j] == (j < 21 ? pattern(members[root], round, j) : pattern(r, round, j));
             }
@@ -307,7 +307,7 @@ TEST_CASE("loopback subset group: every grouped kind runs on children of a parit
                 buf[6144 + i] = r;
             }
             Communicator::GroupItem whole{ buf + 6144, buf + 6144, 8 };
-            ok = ok && c.allReduceMany(&whole, 1, FB_I32, FB_OP_SUM, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+            ok = ok && c.groupMany(Communicator::GROUP_ALLREDUCE, &whole, 1, FB_I32, FB_OP_SUM, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
             ok = ok && buf[6144] == n * (n - 1) / 2;
         }
         return ok && c.checkError(nullptr) == 0 && c.freeSubsetSlots() == (1u << FB_SUB_SLOTS) - 1;
@@ -358,11 +358,11 @@ TEST_CASE("loopback subset: child ranks, heap addressing, refused calls and grou
     REQUIRE_EQ(rc, FB_OK);
     auto bplan = child->prepareGroup(&item, 1, FB_U8, &rc, Communicator::GROUP_BROADCAST);
     REQUIRE(bplan != nullptr);
-    REQUIRE_EQ(child->broadcastGroup(*plan, 0, FB_FLAG_SYMMETRIC, nullptr), FB_E_INVALID);
-    REQUIRE_EQ(child->broadcastGroup(*bplan, 3, FB_FLAG_SYMMETRIC, nullptr), FB_E_INVALID);
-    REQUIRE_EQ(child->broadcastGroup(*bplan, -1, FB_FLAG_SYMMETRIC, nullptr), FB_E_INVALID);
-    REQUIRE_EQ(child->allReduceGroup(*bplan, FB_OP_SUM, FB_FLAG_SYMMETRIC, nullptr), FB_E_INVALID);
-    REQUIRE_EQ(child->broadcastMany(&item, 1, 3, FB_FLAG_SYMMETRIC, nullptr), FB_E_INVALID);
+    REQUIRE_EQ(child->runGroup(Communicator::GROUP_BROADCAST, *plan, 0, 0, FB_FLAG_SYMMETRIC, nullptr), FB_E_INVALID);
+    REQUIRE_EQ(child->runGroup(Communicator::GROUP_BROADCAST, *bplan, 0, 3, FB_FLAG_SYMMETRIC, nullptr), FB_E_INVALID);
+    REQUIRE_EQ(child->runGroup(Communicator::GROUP_BROADCAST, *bplan, 0, -1, FB_FLAG_SYMMETRIC, nullptr), FB_E_INVALID);
+    REQUIRE_EQ(child->runGroup(Communicator::GROUP_ALLREDUCE, *bplan, FB_OP_SUM, 0, FB_FLAG_SYMMETRIC, nullptr), FB_E_INVALID);
+    REQUIRE_EQ(child->groupMany(Communicator::GROUP_BROADCAST, &item, 1, FB_U8, 0, 3, FB_FLAG_SYMMETRIC, nullptr), FB_E_INVALID);
     REQUIRE_EQ(child->hostBarrier(), FB_E_UNSUPPORTED);
     REQUIRE_EQ(child->allReduce(buf, buf, 4, FB_I32, FB_OP_SUM, FB_ALGO_LL, FB_FLAG_SYMMETRIC, nullptr), FB_E_UNSUPPORTED);
     REQUIRE_EQ(child->allReduce(buf, buf, 4, FB_I32, FB_OP_SUM, FB_ALGO_NVLS, FB_FLAG_SYMMETRIC, nullptr), FB_E_UNSUPPORTED);

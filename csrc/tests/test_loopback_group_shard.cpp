@@ -148,7 +148,7 @@ TEST_CASE("loopback group shard: reduce-scatter equals per-item reduce-scatters,
                 int rc = FB_OK;
                 auto plan = c.prepareGroup(items.data(), items.size(), k.dtype, &rc, Communicator::GROUP_REDUCE_SCATTER);
                 ok = ok && plan != nullptr && Communicator::groupPlanLaunches(*plan) == 1;
-                ok = ok && c.reduceScatterGroup(*plan, k.op, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+                ok = ok && c.runGroup(Communicator::GROUP_REDUCE_SCATTER, *plan, k.op, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
                 ok = ok && c.stats().launches == l0 + 1;
                 for (size_t t = 0; t < items.size() && ok; t++) {
                     ok = c.reduceScatter(items[t].send, refs[t], items[t].count, k.dtype, k.op, FB_FLAG_SYMMETRIC, nullptr) ==
@@ -160,8 +160,7 @@ TEST_CASE("loopback group shard: reduce-scatter equals per-item reduce-scatters,
                 for (auto& it : items) {
                     memset(it.recv, 0xCD, it.count * es);
                 }
-                ok = ok && c.reduceScatterMany(items.data(), items.size(), k.dtype, k.op,
-                                               FB_FLAG_SYMMETRIC | FB_FLAG_CHANNEL(1), nullptr) == FB_OK;
+                ok = ok && c.groupMany(Communicator::GROUP_REDUCE_SCATTER, items.data(), items.size(), k.dtype, k.op, 0, FB_FLAG_SYMMETRIC | FB_FLAG_CHANNEL(1), nullptr) == FB_OK;
                 for (size_t t = 0; t < items.size() && ok; t++) {
                     ok = memcmp(items[t].recv, refs[t], items[t].count * es) == 0;
                 }
@@ -225,7 +224,7 @@ TEST_CASE("loopback group shard: all-gather with empty items, in place, plan reu
                 fill(step);
                 c.hostBarrier();
                 const uint64_t l0 = c.stats().launches;
-                ok = c.allGatherGroup(*plan, FB_FLAG_SYMMETRIC, nullptr) == FB_OK && c.stats().launches == l0 + 1;
+                ok = c.runGroup(Communicator::GROUP_ALLGATHER, *plan, 0, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_OK && c.stats().launches == l0 + 1;
                 c.hostBarrier();
                 ok = ok && check(step);
             }
@@ -243,14 +242,14 @@ TEST_CASE("loopback group shard: all-gather with empty items, in place, plan reu
             }
             c.hostBarrier();
             auto ipPlan = c.prepareGroup(inPlace.data(), inPlace.size(), FB_I16, &rc, Communicator::GROUP_ALLGATHER);
-            ok = ok && ipPlan != nullptr && c.allGatherGroup(*ipPlan, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+            ok = ok && ipPlan != nullptr && c.runGroup(Communicator::GROUP_ALLGATHER, *ipPlan, 0, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
             c.hostBarrier();
             ok = ok && check(9);
             // and transient
             c.hostBarrier();
             fill(4);
             c.hostBarrier();
-            ok = ok && c.allGatherMany(items.data(), items.size(), FB_I16, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+            ok = ok && c.groupMany(Communicator::GROUP_ALLGATHER, items.data(), items.size(), FB_I16, 0, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
             c.hostBarrier();
             ok = ok && check(4);
             return ok && c.checkError(nullptr) == 0;
@@ -284,10 +283,10 @@ TEST_CASE("loopback group shard: more items than one segment table take two laun
         bool ok = rsPlan != nullptr && agPlan != nullptr && Communicator::groupPlanLaunches(*rsPlan) == 2 &&
                   Communicator::groupPlanLaunches(*agPlan) == 2;
         c.resetStats();
-        ok = ok && c.reduceScatterGroup(*rsPlan, FB_OP_SUM, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+        ok = ok && c.runGroup(Communicator::GROUP_REDUCE_SCATTER, *rsPlan, FB_OP_SUM, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
         ok = ok && c.stats().launches == 2 && c.stats().bytes == k * shard * n * 4;
         c.hostBarrier();
-        ok = ok && c.allGatherGroup(*agPlan, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+        ok = ok && c.runGroup(Communicator::GROUP_ALLGATHER, *agPlan, 0, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
         ok = ok && c.stats().launches == 4 && c.stats().bytes == 2 * k * shard * n * 4;
         c.hostBarrier();
         // all-gather of the reduce-scatter: the all-reduce of the inputs
@@ -299,8 +298,8 @@ TEST_CASE("loopback group shard: more items than one segment table take two laun
         // the transient calls split the same way
         c.hostBarrier();
         c.resetStats();
-        ok = ok && c.reduceScatterMany(rs.data(), rs.size(), FB_I32, FB_OP_SUM, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
-        ok = ok && c.allGatherMany(ag.data(), ag.size(), FB_I32, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+        ok = ok && c.groupMany(Communicator::GROUP_REDUCE_SCATTER, rs.data(), rs.size(), FB_I32, FB_OP_SUM, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+        ok = ok && c.groupMany(Communicator::GROUP_ALLGATHER, ag.data(), ag.size(), FB_I32, 0, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
         ok = ok && c.stats().launches == 4;
         return ok && c.checkError(nullptr) == 0;
     });
@@ -351,15 +350,15 @@ TEST_CASE("loopback group shard: lists that cannot be grouped are refused, *Many
             auto agPlan = c.prepareGroup(&goodAg, 1, FB_I32, &rc, Communicator::GROUP_ALLGATHER);
             auto arPlan = c.prepareGroup(&goodAg, 1, FB_I32, &rc);
             ok = ok && rsPlan && agPlan && arPlan;
-            ok = ok && c.allReduceGroup(*rsPlan, FB_OP_SUM, FB_FLAG_SYMMETRIC, nullptr) == FB_E_INVALID;
-            ok = ok && c.reduceScatterGroup(*agPlan, FB_OP_SUM, FB_FLAG_SYMMETRIC, nullptr) == FB_E_INVALID;
-            ok = ok && c.reduceScatterGroup(*arPlan, FB_OP_SUM, FB_FLAG_SYMMETRIC, nullptr) == FB_E_INVALID;
-            ok = ok && c.allGatherGroup(*rsPlan, FB_FLAG_SYMMETRIC, nullptr) == FB_E_INVALID;
-            ok = ok && c.allGatherGroup(*arPlan, FB_FLAG_SYMMETRIC, nullptr) == FB_E_INVALID;
+            ok = ok && c.runGroup(Communicator::GROUP_ALLREDUCE, *rsPlan, FB_OP_SUM, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_E_INVALID;
+            ok = ok && c.runGroup(Communicator::GROUP_REDUCE_SCATTER, *agPlan, FB_OP_SUM, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_E_INVALID;
+            ok = ok && c.runGroup(Communicator::GROUP_REDUCE_SCATTER, *arPlan, FB_OP_SUM, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_E_INVALID;
+            ok = ok && c.runGroup(Communicator::GROUP_ALLGATHER, *rsPlan, 0, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_E_INVALID;
+            ok = ok && c.runGroup(Communicator::GROUP_ALLGATHER, *arPlan, 0, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_E_INVALID;
             {
                 auto fPlan = c.prepareGroup(&good, 1, FB_F32, &rc, Communicator::GROUP_REDUCE_SCATTER);
-                ok = ok && fPlan && c.reduceScatterGroup(*fPlan, FB_OP_BAND, FB_FLAG_SYMMETRIC, nullptr) == FB_E_UNSUPPORTED;
-                ok = ok && c.reduceScatterMany(&good, 1, FB_F32, FB_OP_BAND, FB_FLAG_SYMMETRIC, nullptr) == FB_E_UNSUPPORTED;
+                ok = ok && fPlan && c.runGroup(Communicator::GROUP_REDUCE_SCATTER, *fPlan, FB_OP_BAND, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_E_UNSUPPORTED;
+                ok = ok && c.groupMany(Communicator::GROUP_REDUCE_SCATTER, &good, 1, FB_F32, FB_OP_BAND, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_E_UNSUPPORTED;
             }
             // *Many runs what cannot be grouped as per-item calls, with their
             // results: an output over its own input (reduce-scatter) ...
@@ -370,7 +369,7 @@ TEST_CASE("loopback group shard: lists that cannot be grouped are refused, *Many
             }
             c.hostBarrier();
             Communicator::GroupItem rsOver{ a, a, cnt };
-            ok = ok && c.reduceScatterMany(&rsOver, 1, FB_I32, FB_OP_SUM, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+            ok = ok && c.groupMany(Communicator::GROUP_REDUCE_SCATTER, &rsOver, 1, FB_I32, FB_OP_SUM, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
             c.hostBarrier();
             for (size_t j = 0; j < cnt && ok; j++) {
                 ok = a[j] == (int32_t)(n * (rank * cnt + j) * 3 + n * (n - 1) / 2);
@@ -382,7 +381,7 @@ TEST_CASE("loopback group shard: lists that cannot be grouped are refused, *Many
             }
             Communicator::GroupItem hostItem{ hs.data(), hr.data(), cnt };
             c.hostBarrier();
-            ok = ok && c.reduceScatterMany(&hostItem, 1, FB_I32, FB_OP_SUM, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+            ok = ok && c.groupMany(Communicator::GROUP_REDUCE_SCATTER, &hostItem, 1, FB_I32, FB_OP_SUM, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
             for (size_t j = 0; j < cnt && ok; j++) {
                 ok = hr[j] == (int32_t)(n * (rank * cnt + j) + n * (n - 1) / 2);
             }
@@ -396,13 +395,13 @@ TEST_CASE("loopback group shard: lists that cannot be grouped are refused, *Many
             }
             Communicator::GroupItem agOdd{ gIn, gOut, odd };
             c.hostBarrier();
-            ok = ok && c.allGatherMany(&agOdd, 1, FB_I32, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
+            ok = ok && c.groupMany(Communicator::GROUP_ALLGATHER, &agOdd, 1, FB_I32, 0, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_OK;
             c.hostBarrier();
             for (size_t i = 0; i < odd * n && ok; i++) {
                 ok = gOut[i] == (int32_t)((i / odd) * 100 + i % odd);
             }
             Communicator::GroupItem rsOdd{ b, b + 64 * n, odd };
-            ok = ok && c.reduceScatterMany(&rsOdd, 1, FB_I32, FB_OP_SUM, FB_FLAG_SYMMETRIC, nullptr) == FB_E_UNSUPPORTED &&
+            ok = ok && c.groupMany(Communicator::GROUP_REDUCE_SCATTER, &rsOdd, 1, FB_I32, FB_OP_SUM, 0, FB_FLAG_SYMMETRIC, nullptr) == FB_E_UNSUPPORTED &&
                  c.reduceScatter(b, b + 64 * n, odd, FB_I32, FB_OP_SUM, FB_FLAG_SYMMETRIC, nullptr) == FB_E_UNSUPPORTED;
             return ok && c.checkError(nullptr) == 0;
         });

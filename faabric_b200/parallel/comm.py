@@ -84,6 +84,8 @@ OPS = {
     "replace": 32,
     "no_op": 33,
 }
+# Communicator::GroupKind
+GROUP_KINDS = {"all_reduce": 0, "reduce_scatter": 1, "all_gather": 2, "broadcast": 3, "all_to_all": 4}
 ALGOS = {"auto": 0, "oneshot": 1, "twoshot": 2, "nvls": 3, "ll": 4}
 ALGO_NAMES = {v: k for k, v in ALGOS.items()}
 FLAG_SYMMETRIC = 1
@@ -452,69 +454,101 @@ class Communicator:
         self._check(rc, "all_to_all")
         return recv
 
-    # ------------------------------------------------- grouped all-reduce
-    def _group_arrays(self, sends, recvs, dtype):
+    # ------------------------------------------------- grouped collectives
+    def _group_items(self, what, kind, sends, recvs, dtype, root=0):
+        """(n, send ptrs, recv ptrs, counts, FbDtype) of a grouped list of
+        ``kind`` (a GROUP_KINDS name); raises before any native call for empty
+        or unequally long lists and for shapes that do not fit the kind:
+        reduce-scatter needs send.numel() == size * recv.numel(), all-gather
+        the reverse; all-to-all needs equal send and recv numel and element
+        size, numel divisible by ``size`` (in ``dtype`` elements too), and
+        counts per block; a broadcast (each buffer as send and recv) needs
+        contiguous tensors and a root in the communicator, and counts bytes."""
+        if len(sends) != len(recvs) or not sends:
+            raise CommError(f"{what}: need equally long, non-empty lists")
+        per = 1
+        if kind == "broadcast":
+            if not 0 <= int(root) < self.size:
+                raise CommError(f"{what}: root {root} outside a communicator of {self.size}")
+            for i, t in enumerate(sends):
+                if not t.is_contiguous():
+                    raise CommError(f"{what}: item {i} must be contiguous")
+            typed = [(t.numel() * t.element_size(), FB_DTYPES["u8"][0]) for t in sends]
+        elif kind == "all_to_all":
+            for i, (s, r) in enumerate(zip(sends, recvs)):
+                if s.numel() != r.numel() or s.numel() % self.size != 0:
+                    raise CommError(
+                        f"{what}: item {i} has {s.numel()} send and {r.numel()} recv elements; "
+                        f"both must be equal and divisible by {self.size}"
+                    )
+                if s.element_size() != r.element_size():
+                    # (the native side sizes recv from the send's elements)
+                    raise CommError(
+                        f"{what}: item {i} has {s.element_size()}-byte send and {r.element_size()}-byte recv elements"
+                    )
+            typed = [self._typed(s, dtype) for s in sends]
+            per = self.size
+        elif kind == "all_reduce":
+            typed = [self._typed(t, dtype) for t in sends]
+        else:
+            gather = kind == "all_gather"
+            for i, (s, r) in enumerate(zip(sends, recvs)):
+                small, big = (s, r) if gather else (r, s)
+                if big.numel() != self.size * small.numel():
+                    raise CommError(
+                        f"{what}: item {i} has {s.numel()} send and {r.numel()} recv elements; "
+                        f"{'recv' if gather else 'send'} must hold {self.size} x {'send' if gather else 'recv'}"
+                    )
+            typed = [self._typed(s if gather else r, dtype) for s, r in zip(sends, recvs)]
+        if len({dt for _, dt in typed}) != 1:
+            raise CommError(f"{what}: every tensor must have the same dtype")
+        for i, (c, _) in enumerate(typed):
+            if c % per != 0:
+                raise CommError(f"{what}: item {i} has {c} {dtype} elements, not divisible by {self.size}")
         n = len(sends)
         sp = (C.c_void_p * n)(*[t.data_ptr() for t in sends])
         rp = (C.c_void_p * n)(*[t.data_ptr() for t in recvs])
-        typed = [self._typed(t, dtype) for t in sends]
-        if len({dt for _, dt in typed}) != 1:
-            raise CommError("grouped all-reduce: every tensor must have the same dtype")
-        cnt = (C.c_uint64 * n)(*[c for c, _ in typed])
+        cnt = (C.c_uint64 * n)(*[c // per for c, _ in typed])
         return n, sp, rp, cnt, typed[0][1]
+
+    def _prepare(self, what, kind, sends, recvs, dtype, sized):
+        """A GroupPlan of ``kind``; ``sized`` is the list whose bytes it moves."""
+        n, sp, rp, cnt, dt = self._group_items(what, kind, sends, recvs, dtype)
+        h = self._lib.fb_group_prepare(self._h, GROUP_KINDS[kind], n, sp, rp, cnt, dt)
+        if not h:
+            raise CommError(f"{what} failed [{_lib.last_error()}]")
+        return GroupPlan(self, h, n, sum(t.numel() * t.element_size() for t in sized))
+
+    def _launch(self, what, kind, plan, op, root, stream, channel, flags):
+        rc = self._lib.fb_group_launch(
+            self._h, GROUP_KINDS[kind], plan._h, op, root, flags | ((channel & 0xF) << 8), self._stream(stream)
+        )
+        self._check(rc, what)
+
+    def _many(self, what, kind, sends, recvs, dtype, op, root, stream, channel):
+        n, sp, rp, cnt, dt = self._group_items(what, kind, sends, recvs, dtype, root)
+        f = self._sym(*sends) | ((channel & 0xF) << 8)
+        fop = OPS[op] if op is not None else 0
+        rc = self._lib.fb_group_many(
+            self._h, GROUP_KINDS[kind], n, sp, rp, cnt, dt, fop, int(root), f, self._stream(stream)
+        )
+        self._check(rc, what)
 
     def prepare_group(self, sends, recvs=None, dtype=None) -> "GroupPlan":
         """Plan ONE launch that all-reduces every tensor of ``sends`` (each with
         per-tensor semantics).  Tensors must live in the symmetric heap at
         16-byte aligned addresses; call collectively with the same list."""
         recvs = sends if recvs is None else recvs
-        if len(sends) != len(recvs) or not sends:
-            raise CommError("prepare_group: need equally long, non-empty lists")
-        n, sp, rp, cnt, dt = self._group_arrays(sends, recvs, dtype)
-        h = self._lib.fb_group_prepare(self._h, n, sp, rp, cnt, dt)
-        if not h:
-            raise CommError(f"prepare_group failed [{_lib.last_error()}]")
-        return GroupPlan(self, h, n, sum(t.numel() * t.element_size() for t in sends))
+        return self._prepare("prepare_group", "all_reduce", sends, recvs, dtype, sends)
 
     def all_reduce_group(self, plan: "GroupPlan", op="sum", stream=None, channel=0, flags=FLAG_SYMMETRIC):
-        rc = self._lib.fb_group_allreduce(
-            self._h, plan._h, OPS[op], flags | ((channel & 0xF) << 8), self._stream(stream)
-        )
-        self._check(rc, "all_reduce_group")
+        self._launch("all_reduce_group", "all_reduce", plan, OPS[op], 0, stream, channel, flags)
 
     def all_reduce_many(self, sends, recvs=None, op="sum", stream=None, channel=0, dtype=None):
         """Transient variant of :meth:`prepare_group` + :meth:`all_reduce_group`
         (the table is rebuilt and uploaded in stream order on every call)."""
         recvs = sends if recvs is None else recvs
-        if not sends:
-            raise CommError("all_reduce_many: need a non-empty list")
-        n, sp, rp, cnt, dt = self._group_arrays(sends, recvs, dtype)
-        f = self._sym(*sends) | ((channel & 0xF) << 8)
-        rc = self._lib.fb_allreduce_many(self._h, n, sp, rp, cnt, dt, OPS[op], f, self._stream(stream))
-        self._check(rc, "all_reduce_many")
-
-    # ------------------------------ grouped reduce-scatter and all-gather
-    def _shard_arrays(self, what, sends, recvs, dtype, gather):
-        """(n, send ptrs, recv ptrs, per-rank counts, FbDtype) of a shard group;
-        raises before any native call when a shape does not fit: reduce-scatter
-        needs send.numel() == size * recv.numel(), all-gather the reverse."""
-        if len(sends) != len(recvs) or not sends:
-            raise CommError(f"{what}: need equally long, non-empty lists")
-        for i, (s, r) in enumerate(zip(sends, recvs)):
-            small, big = (s, r) if gather else (r, s)
-            if big.numel() != self.size * small.numel():
-                raise CommError(
-                    f"{what}: item {i} has {s.numel()} send and {r.numel()} recv elements; "
-                    f"{'recv' if gather else 'send'} must hold {self.size} x {'send' if gather else 'recv'}"
-                )
-        n = len(sends)
-        sp = (C.c_void_p * n)(*[t.data_ptr() for t in sends])
-        rp = (C.c_void_p * n)(*[t.data_ptr() for t in recvs])
-        typed = [self._typed(s if gather else r, dtype) for s, r in zip(sends, recvs)]
-        if len({dt for _, dt in typed}) != 1:
-            raise CommError(f"{what}: every tensor must have the same dtype")
-        cnt = (C.c_uint64 * n)(*[c for c, _ in typed])
-        return n, sp, rp, cnt, typed[0][1]
+        self._many("all_reduce_many", "all_reduce", sends, recvs, dtype, op, 0, stream, channel)
 
     def prepare_reduce_scatter_group(self, sends, recvs, dtype=None) -> "GroupPlan":
         """Plan ONE launch that reduce-scatters every pair of the lists
@@ -523,124 +557,48 @@ class Communicator:
         the symmetric heap at 16-byte aligned addresses, shards are multiples
         of 16 bytes, and no output overlaps an input; call collectively with
         the same lists."""
-        n, sp, rp, cnt, dt = self._shard_arrays("prepare_reduce_scatter_group", sends, recvs, dtype, False)
-        h = self._lib.fb_group_prepare_reduce_scatter(self._h, n, sp, rp, cnt, dt)
-        if not h:
-            raise CommError(f"prepare_reduce_scatter_group failed [{_lib.last_error()}]")
-        return GroupPlan(self, h, n, sum(t.numel() * t.element_size() for t in sends))
+        return self._prepare("prepare_reduce_scatter_group", "reduce_scatter", sends, recvs, dtype, sends)
 
     def prepare_all_gather_group(self, sends, recvs, dtype=None) -> "GroupPlan":
         """Plan ONE launch that all-gathers every pair of the lists
         (MPI_Allgather per pair: block p of ``recvs[i]`` gets ``sends[i]`` of
         rank p).  Same conditions as :meth:`prepare_reduce_scatter_group`; in
         place (``sends[i]`` is block ``rank`` of ``recvs[i]``) is allowed."""
-        n, sp, rp, cnt, dt = self._shard_arrays("prepare_all_gather_group", sends, recvs, dtype, True)
-        h = self._lib.fb_group_prepare_all_gather(self._h, n, sp, rp, cnt, dt)
-        if not h:
-            raise CommError(f"prepare_all_gather_group failed [{_lib.last_error()}]")
-        return GroupPlan(self, h, n, sum(t.numel() * t.element_size() for t in recvs))
+        return self._prepare("prepare_all_gather_group", "all_gather", sends, recvs, dtype, recvs)
 
     def reduce_scatter_group(self, plan: "GroupPlan", op="sum", stream=None, channel=0, flags=FLAG_SYMMETRIC):
-        rc = self._lib.fb_group_reduce_scatter(
-            self._h, plan._h, OPS[op], flags | ((channel & 0xF) << 8), self._stream(stream)
-        )
-        self._check(rc, "reduce_scatter_group")
+        self._launch("reduce_scatter_group", "reduce_scatter", plan, OPS[op], 0, stream, channel, flags)
 
     def all_gather_group(self, plan: "GroupPlan", stream=None, channel=0, flags=FLAG_SYMMETRIC):
-        rc = self._lib.fb_group_all_gather(self._h, plan._h, flags | ((channel & 0xF) << 8), self._stream(stream))
-        self._check(rc, "all_gather_group")
+        self._launch("all_gather_group", "all_gather", plan, 0, 0, stream, channel, flags)
 
     def reduce_scatter_many(self, sends, recvs, op="sum", stream=None, channel=0, dtype=None):
         """Transient variant of :meth:`prepare_reduce_scatter_group` +
         :meth:`reduce_scatter_group`; lists that cannot be grouped run one
         :meth:`reduce_scatter` per pair."""
-        n, sp, rp, cnt, dt = self._shard_arrays("reduce_scatter_many", sends, recvs, dtype, False)
-        f = self._sym(*sends) | ((channel & 0xF) << 8)
-        rc = self._lib.fb_reduce_scatter_many(self._h, n, sp, rp, cnt, dt, OPS[op], f, self._stream(stream))
-        self._check(rc, "reduce_scatter_many")
+        self._many("reduce_scatter_many", "reduce_scatter", sends, recvs, dtype, op, 0, stream, channel)
 
     def all_gather_many(self, sends, recvs, stream=None, channel=0, dtype=None):
         """Transient variant of :meth:`prepare_all_gather_group` +
         :meth:`all_gather_group`; lists that cannot be grouped run one
         :meth:`all_gather` per pair."""
-        n, sp, rp, cnt, dt = self._shard_arrays("all_gather_many", sends, recvs, dtype, True)
-        f = self._sym(*sends) | ((channel & 0xF) << 8)
-        rc = self._lib.fb_all_gather_many(self._h, n, sp, rp, cnt, dt, f, self._stream(stream))
-        self._check(rc, "all_gather_many")
-
-    # ------------------------------------------------ grouped broadcast
-    def _bcast_arrays(self, what, bufs, root):
-        """(n, buffer ptrs, byte counts) of a broadcast group; raises before
-        any native call for an empty list, a root outside the communicator or
-        a tensor that is not contiguous."""
-        if not bufs:
-            raise CommError(f"{what}: need a non-empty list")
-        if not 0 <= int(root) < self.size:
-            raise CommError(f"{what}: root {root} outside a communicator of {self.size}")
-        for i, t in enumerate(bufs):
-            if not t.is_contiguous():
-                raise CommError(f"{what}: item {i} must be contiguous")
-        n = len(bufs)
-        bp = (C.c_void_p * n)(*[t.data_ptr() for t in bufs])
-        nb = (C.c_uint64 * n)(*[t.numel() * t.element_size() for t in bufs])
-        return n, bp, nb
+        self._many("all_gather_many", "all_gather", sends, recvs, dtype, None, 0, stream, channel)
 
     def prepare_broadcast_group(self, bufs) -> "GroupPlan":
         """Plan ONE launch that broadcasts every tensor of ``bufs`` (MPI_Bcast
         per tensor, any dtype and length) from the root given to
         :meth:`broadcast_group`.  Tensors live in the symmetric heap at 16-byte
         aligned addresses; call collectively with the same list."""
-        n, bp, nb = self._bcast_arrays("prepare_broadcast_group", bufs, 0)
-        h = self._lib.fb_group_prepare_broadcast(self._h, n, bp, nb)
-        if not h:
-            raise CommError(f"prepare_broadcast_group failed [{_lib.last_error()}]")
-        return GroupPlan(self, h, n, sum(nb))
+        return self._prepare("prepare_broadcast_group", "broadcast", bufs, bufs, None, bufs)
 
     def broadcast_group(self, plan: "GroupPlan", root=0, stream=None, channel=0, flags=FLAG_SYMMETRIC):
-        rc = self._lib.fb_group_broadcast(
-            self._h, plan._h, int(root), flags | ((channel & 0xF) << 8), self._stream(stream)
-        )
-        self._check(rc, "broadcast_group")
+        self._launch("broadcast_group", "broadcast", plan, 0, int(root), stream, channel, flags)
 
     def broadcast_many(self, bufs, root=0, stream=None, channel=0):
         """Transient variant of :meth:`prepare_broadcast_group` +
         :meth:`broadcast_group`; lists that cannot be grouped run one
         :meth:`broadcast` per tensor."""
-        n, bp, nb = self._bcast_arrays("broadcast_many", bufs, root)
-        f = self._sym(*bufs) | ((channel & 0xF) << 8)
-        rc = self._lib.fb_broadcast_many(self._h, n, bp, nb, int(root), f, self._stream(stream))
-        self._check(rc, "broadcast_many")
-
-    # ------------------------------------------------ grouped all-to-all
-    def _a2a_arrays(self, what, sends, recvs, dtype):
-        """(n, send ptrs, recv ptrs, per-block counts, FbDtype) of an all-to-all
-        group; raises before any native call unless every item's send and recv
-        have equal numel and element size, numel divisible by ``size`` (in
-        ``dtype`` elements too)."""
-        if len(sends) != len(recvs) or not sends:
-            raise CommError(f"{what}: need equally long, non-empty lists")
-        for i, (s, r) in enumerate(zip(sends, recvs)):
-            if s.numel() != r.numel() or s.numel() % self.size != 0:
-                raise CommError(
-                    f"{what}: item {i} has {s.numel()} send and {r.numel()} recv elements; "
-                    f"both must be equal and divisible by {self.size}"
-                )
-            if s.element_size() != r.element_size():
-                # (the native side sizes recv from the send's elements)
-                raise CommError(
-                    f"{what}: item {i} has {s.element_size()}-byte send and {r.element_size()}-byte recv elements"
-                )
-        n = len(sends)
-        sp = (C.c_void_p * n)(*[t.data_ptr() for t in sends])
-        rp = (C.c_void_p * n)(*[t.data_ptr() for t in recvs])
-        typed = [self._typed(s, dtype) for s in sends]
-        if len({dt for _, dt in typed}) != 1:
-            raise CommError(f"{what}: every tensor must have the same dtype")
-        for i, (c, _) in enumerate(typed):
-            if c % self.size != 0:
-                raise CommError(f"{what}: item {i} has {c} {dtype} elements, not divisible by {self.size}")
-        cnt = (C.c_uint64 * n)(*[c // self.size for c, _ in typed])
-        return n, sp, rp, cnt, typed[0][1]
+        self._many("broadcast_many", "broadcast", bufs, bufs, None, None, root, stream, channel)
 
     def prepare_all_to_all_group(self, sends, recvs, dtype=None) -> "GroupPlan":
         """Plan ONE launch that exchanges every pair of the lists (MPI_Alltoall
@@ -649,24 +607,16 @@ class Communicator:
         Tensors live in the symmetric heap at 16-byte aligned addresses, blocks
         are multiples of 16 bytes, and no output overlaps an input; call
         collectively with the same lists."""
-        n, sp, rp, cnt, dt = self._a2a_arrays("prepare_all_to_all_group", sends, recvs, dtype)
-        h = self._lib.fb_group_prepare_all_to_all(self._h, n, sp, rp, cnt, dt)
-        if not h:
-            raise CommError(f"prepare_all_to_all_group failed [{_lib.last_error()}]")
-        return GroupPlan(self, h, n, sum(t.numel() * t.element_size() for t in sends))
+        return self._prepare("prepare_all_to_all_group", "all_to_all", sends, recvs, dtype, sends)
 
     def all_to_all_group(self, plan: "GroupPlan", stream=None, channel=0, flags=FLAG_SYMMETRIC):
-        rc = self._lib.fb_group_all_to_all(self._h, plan._h, flags | ((channel & 0xF) << 8), self._stream(stream))
-        self._check(rc, "all_to_all_group")
+        self._launch("all_to_all_group", "all_to_all", plan, 0, 0, stream, channel, flags)
 
     def all_to_all_many(self, sends, recvs, stream=None, channel=0, dtype=None):
         """Transient variant of :meth:`prepare_all_to_all_group` +
         :meth:`all_to_all_group`; lists that cannot be grouped run one
         :meth:`all_to_all` per pair."""
-        n, sp, rp, cnt, dt = self._a2a_arrays("all_to_all_many", sends, recvs, dtype)
-        f = self._sym(*sends) | ((channel & 0xF) << 8)
-        rc = self._lib.fb_all_to_all_many(self._h, n, sp, rp, cnt, dt, f, self._stream(stream))
-        self._check(rc, "all_to_all_many")
+        self._many("all_to_all_many", "all_to_all", sends, recvs, dtype, None, 0, stream, channel)
 
     def send_recv(self, send_buf, dst, recv_buf, src, stream=None):
         rc = self._lib.fb_sendrecv(

@@ -722,6 +722,9 @@ def test_grouped_rejects_non_symmetric_tensors():
 
     with pytest.raises(CommError):
         c.prepare_group([t])
+    # a recv list shorter than the send list is refused before any native call
+    with pytest.raises(CommError):
+        c.all_reduce_many([t, t], [t])
 
 
 @pytest.mark.parametrize("n", [2, 4])
