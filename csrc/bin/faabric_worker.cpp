@@ -29,6 +29,7 @@
 #include "../tests/mpi_rma_request_body.h"
 #include "../tests/mpi_subcomm_device_body.h"
 #include "../tests/mpi_group_alltoall_body.h"
+#include "../tests/mpi_group_rooted_body.h"
 #include "../tests/mpi_group_subcomm_body.h"
 
 #include <cuda_runtime.h>
@@ -942,6 +943,145 @@ static void registerFunctions()
         }
         MPI_Free_mem(recv);
         MPI_Free_mem(send);
+        return 0;
+    });
+
+    // MPI_Igather and MPI_Iscatter bursts on the world and on
+    // sub-communicators (mpi_group_rooted_body.h)
+    mpiFunction("group-rooted", [](int rank, int size, faabric::Message& msg) {
+        std::string why;
+        int rc = group_rooted::body(rank, size, msg.mpiworldid(), true, &why);
+        if (rc != 0) {
+            SPDLOG_ERROR("group-rooted: {}", why);
+            msg.set_outputdata(why);
+        }
+        return rc;
+    });
+
+    // A list of tensors gathered to or scattered from rank 0 of the world per
+    // step, in device memory (MPI_Alloc_mem).  Input:
+    // "<mode>;<steps>;<bytes0,bytes1,...>" with bytes_i the bytes of tensor i
+    // per rank and mode
+    //   gather / scatter    one MPI_Gather / MPI_Scatter per tensor
+    //   igather / iscatter  MPI_Igather / MPI_Iscatter per tensor + MPI_Waitall
+    // Rank 0 reports {"ms_per_step", "us_per_call", "launches_per_step",
+    // "wait_ms_per_step"}: the launches counted on its world device
+    // communicator, and the part of a step spent in MPI_Waitall.
+    mpiFunction("bench-group-rooted", [](int rank, int size, faabric::Message& msg) {
+        std::vector<std::string> f;
+        std::string cur;
+        for (char c : msg.inputdata() + ";") {
+            if (c == ';') {
+                f.push_back(cur);
+                cur.clear();
+            } else {
+                cur += c;
+            }
+        }
+        EXPECT(f.size() >= 3 && size >= 2);
+        const std::string mode = f[0];
+        const bool gather = mode == "gather" || mode == "igather";
+        const bool nb = mode[0] == 'i';
+        const int steps = std::stoi(f[1]);
+        std::vector<size_t> bytes;
+        for (size_t b = 0, e; b < f[2].size(); b = e + 1) {
+            e = f[2].find(',', b);
+            if (e == std::string::npos) {
+                e = f[2].size();
+            }
+            bytes.push_back(std::stoull(f[2].substr(b, e - b)));
+        }
+        // per tensor: one block at `single`, `size` blocks at `blocks`
+        size_t singleTotal = 0, blockTotal = 0;
+        std::vector<size_t> singleOff, blockOff;
+        for (size_t b : bytes) {
+            singleOff.push_back(singleTotal);
+            blockOff.push_back(blockTotal);
+            singleTotal += b;
+            blockTotal += b * size;
+        }
+        faabric::mpi::MpiWorld& world = faabric::mpi::getMpiWorldRegistry().getWorld(msg.mpiworldid());
+        uint8_t* single = nullptr;
+        uint8_t* blocks = nullptr;
+        EXPECT(MPI_Alloc_mem(singleTotal, MPI_INFO_FAABRIC_DEVICE, &single) == MPI_SUCCESS);
+        EXPECT(MPI_Alloc_mem(blockTotal, MPI_INFO_FAABRIC_DEVICE, &blocks) == MPI_SUCCESS);
+        // (copies from host memory, which wait for this rank only)
+        std::vector<uint8_t> init(blockTotal, 0);
+        if (gather) {
+            std::vector<uint8_t> mine(singleTotal, (uint8_t)(rank + 1));
+            cudaMemcpy(single, mine.data(), singleTotal, cudaMemcpyHostToDevice);
+        } else {
+            for (size_t i = 0; i < bytes.size(); i++) {
+                for (int p = 0; p < size; p++) {
+                    std::fill_n(init.begin() + blockOff[i] + p * bytes[i], bytes[i], (uint8_t)(p + 1));
+                }
+            }
+        }
+        cudaMemcpy(blocks, init.data(), blockTotal, cudaMemcpyHostToDevice);
+        MPI_Barrier(MPI_COMM_WORLD);
+        const int n = (int)bytes.size();
+        std::vector<MPI_Request> reqs(n);
+        double waitMs = 0;
+        auto step = [&]() -> int {
+            for (int i = 0; i < n; i++) {
+                const int b = (int)bytes[i];
+                uint8_t* s1 = single + singleOff[i];
+                uint8_t* sb = blocks + blockOff[i];
+                if (gather) {
+                    EXPECT((nb ? MPI_Igather(s1, b, MPI_BYTE, sb, b, MPI_BYTE, 0, MPI_COMM_WORLD, &reqs[i])
+                               : MPI_Gather(s1, b, MPI_BYTE, sb, b, MPI_BYTE, 0, MPI_COMM_WORLD)) == MPI_SUCCESS);
+                } else {
+                    EXPECT((nb ? MPI_Iscatter(sb, b, MPI_BYTE, s1, b, MPI_BYTE, 0, MPI_COMM_WORLD, &reqs[i])
+                               : MPI_Scatter(sb, b, MPI_BYTE, s1, b, MPI_BYTE, 0, MPI_COMM_WORLD)) == MPI_SUCCESS);
+                }
+            }
+            if (nb) {
+                auto w0 = std::chrono::steady_clock::now();
+                EXPECT(MPI_Waitall(n, reqs.data(), MPI_STATUSES_IGNORE) == MPI_SUCCESS);
+                waitMs += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - w0).count();
+            }
+            return 0;
+        };
+        for (int i = 0; i < 3; i++) {
+            EXPECT(step() == 0);
+        }
+        auto dev = world.getDeviceComm(rank);
+        EXPECT(dev != nullptr);
+        MPI_Barrier(MPI_COMM_WORLD);
+        waitMs = 0;
+        const uint64_t l0 = dev->stats().launches;
+        auto t0 = std::chrono::steady_clock::now();
+        for (int i = 0; i < steps; i++) {
+            EXPECT(step() == 0);
+        }
+        const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count() / steps;
+        const double launches = (double)(dev->stats().launches - l0) / steps;
+        MPI_Barrier(MPI_COMM_WORLD);
+        // gather: block p of the root's output holds rank p's fill byte;
+        // scatter: every rank's tensor holds its own rank's byte
+        if (gather && rank == 0) {
+            std::vector<uint8_t> back(blockTotal);
+            cudaMemcpy(back.data(), blocks, blockTotal, cudaMemcpyDeviceToHost);
+            for (int i = 0; i < n; i++) {
+                for (int p = 0; p < size; p++) {
+                    const size_t o = blockOff[i] + p * bytes[i];
+                    EXPECT(back[o] == p + 1 && back[o + bytes[i] - 1] == p + 1);
+                }
+            }
+        } else if (!gather) {
+            std::vector<uint8_t> back(singleTotal);
+            cudaMemcpy(back.data(), single, singleTotal, cudaMemcpyDeviceToHost);
+            for (int i = 0; i < n; i++) {
+                EXPECT(back[singleOff[i]] == rank + 1 && back[singleOff[i] + bytes[i] - 1] == rank + 1);
+            }
+        }
+        if (rank == 0) {
+            msg.set_outputdata("{\"ms_per_step\": " + std::to_string(ms) + ", \"us_per_call\": " +
+                               std::to_string(ms * 1000.0 / n) + ", \"launches_per_step\": " + std::to_string(launches) +
+                               ", \"wait_ms_per_step\": " + std::to_string(waitMs / steps) + "}");
+        }
+        MPI_Free_mem(blocks);
+        MPI_Free_mem(single);
         return 0;
     });
 

@@ -28,6 +28,7 @@
 namespace fb {
 struct KernelTable;
 struct GroupSeg;
+struct GroupArgs;
 }
 
 namespace faabric::device {
@@ -281,21 +282,48 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     //   GROUP_ALLTOALL: send and recv hold size()*count elements each; block
     //     r of recv on rank p gets block p of send on rank r (MPI_Alltoall
     //     per item; a byte copy, any dtype)
-    // Shard kinds (all but GROUP_ALLREDUCE and GROUP_BROADCAST) group an item
-    // only if send and recv are in the symmetric heap and 16-byte aligned,
-    // count*esize is a multiple of 16, and recv overlaps no send of the group
-    // on this rank.  The one exception is the in-place all-gather, send ==
-    // recv + rank*count*esize.  Items with count 0 are skipped.
+    //   GROUP_GATHER: send holds count elements on every rank; block p of
+    //     the root's recv (size()*count elements) gets send of rank p
+    //     (MPI_Gather per item; a byte copy, any dtype).  recv is read on the
+    //     root only (null elsewhere is fine).  send == recv + root*count*esize
+    //     at the root is in place.
+    //   GROUP_SCATTER: the mirror image: block p of the root's send
+    //     (size()*count elements) goes to recv (count elements) of rank p;
+    //     send is read on the root only; recv == send + root*count*esize at
+    //     the root is in place.
+    // Shard kinds (GROUP_REDUCE_SCATTER, GROUP_ALLGATHER, GROUP_ALLTOALL)
+    // group an item only if send and recv are in the symmetric heap and
+    // 16-byte aligned, count*esize is a multiple of 16, and recv overlaps no
+    // send of the group on this rank.  The one exception is the in-place
+    // all-gather, send == recv + rank*count*esize.  Items with count 0 are
+    // skipped.
+    // Rooted kinds (GROUP_GATHER, GROUP_SCATTER) group every item with count
+    // > 0: buffers are any device memory of this rank, at any alignment and
+    // length, and may differ between ranks.  The data goes through every
+    // rank's staging buffer, so a plan does not depend on the root, and a
+    // launch holds at most CommConfig::stageBytes per rank (rounded to
+    // chunks); a larger item is cut into pieces at the same points on every
+    // rank.
     enum GroupKind
     {
         GROUP_ALLREDUCE = 0,
         GROUP_REDUCE_SCATTER = 1,
         GROUP_ALLGATHER = 2,
         GROUP_BROADCAST = 3,
-        GROUP_ALLTOALL = 4
+        GROUP_ALLTOALL = 4,
+        GROUP_GATHER = 5,
+        GROUP_SCATTER = 6
+    };
+    // Where the next launch of a list starts: an item, and a byte offset in
+    // it (rooted kinds cut items larger than the staging buffer)
+    struct GroupCursor
+    {
+        size_t item = 0;
+        uint64_t offset = 0;
     };
     // Builds (and uploads) this rank's segment tables.  Collective: every rank
-    // must pass the same list (same offsets, same counts).  Returns null and
+    // must pass the same list (same offsets, same counts; the rooted kinds
+    // need the same counts only).  Returns null and
     // sets *rc when an item is not symmetric / aligned (FB_E_INVALID).  Works
     // on a sub-communicator's child as on any other communicator.
     std::shared_ptr<GroupPlan> prepareGroup(const GroupItem* items,
@@ -309,8 +337,8 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     // broadcast / allToAll calls and returns their errors (reduceScatter
     // refuses shards that are not a multiple of 16 bytes with
     // FB_E_UNSUPPORTED).  `op` is read by the reducing kinds (GROUP_ALLREDUCE,
-    // GROUP_REDUCE_SCATTER) only, `root` by GROUP_BROADCAST only.  Both
-    // follow the same rules:
+    // GROUP_REDUCE_SCATTER) only, `root` by GROUP_BROADCAST, GROUP_GATHER and
+    // GROUP_SCATTER only.  Both follow the same rules:
     //   - a plan of another kind, an unknown kind or a dtype of no size:
     //     FB_E_INVALID
     //   - reducing kinds: a (dtype, op) pair with no reduction at all gives
@@ -322,6 +350,15 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     //     groupMany, pass each buffer as send and recv with FB_U8 and byte
     //     counts.
     //   - GROUP_ALLTOALL on a one-member communicator runs as a local copy
+    //   - GROUP_GATHER, GROUP_SCATTER: a root that is not a rank of this
+    //     communicator, or a channel other than 0 (the staging buffers are
+    //     per rank, not per channel), gives FB_E_INVALID; so does a missing
+    //     buffer this rank needs (every rank's own side, and both on the
+    //     root), checked over the whole list before its first launch.  On a
+    //     one-member communicator the launch is a local copy (nothing when in
+    //     place).  With FB_FLAG_NOSYNC nothing orders a peer's staging copy
+    //     against the root's, so the bytes received are unspecified (the
+    //     flag profiles one rank's data path only).
     //   - GROUP_ALLREDUCE sets lastAlgo() to FB_ALGO_TWOSHOT
     int runGroup(GroupKind kind, const GroupPlan& plan, int op, int root, int flags, cudaStream_t s);
     int groupMany(GroupKind kind,
@@ -333,7 +370,8 @@ class Communicator : public std::enable_shared_from_this<Communicator>
                   int flags,
                   cudaStream_t s);
     static size_t groupPlanLaunches(const GroupPlan& plan);
-    // "all-reduce", "reduce-scatter", "all-gather", "broadcast", "all-to-all"
+    // "all-reduce", "reduce-scatter", "all-gather", "broadcast", "all-to-all",
+    // "gather", "scatter"
     static const char* groupKindName(GroupKind kind);
 
     // ---- point to point (per-pair FIFO; no kernel ever spins on a peer) ----
@@ -569,11 +607,13 @@ class Communicator : public std::enable_shared_from_this<Communicator>
                 const std::string& kind);
     void finishSetup();
     int launchGroup(const GroupLaunch& l, GroupKind kind, int dtype, int op, int root, int flags, cudaStream_t s);
-    int groupCheck(GroupKind kind, int dtype, int op, int root, bool& grouped) const;
+    int launchRooted(const GroupLaunch& l, GroupKind kind, fb::GroupArgs& a, bool ss, int flags, cudaStream_t s);
+    int groupCheck(GroupKind kind, int dtype, int op, int root, int flags, bool& grouped) const;
     int groupBatch(GroupKind kind,
                    const GroupItem* items,
                    size_t nItems,
                    size_t esize,
+                   GroupCursor& at,
                    std::vector<fb::GroupSeg>& segs,
                    GroupLaunch& l) const;
     int groupPerItem(GroupKind kind,

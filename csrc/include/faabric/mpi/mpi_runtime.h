@@ -359,6 +359,20 @@ class MpiWorld
                   faabric_datatype_t* recvType,
                   int recvCount);
 
+    // MPI_Igather / MPI_Iscatter on the world (root: a world rank; `bytes`
+    // per rank).  The root's significant buffer and the other ranks' own
+    // buffer are given (null where not significant); in place at the root,
+    // the gather send is block `root` of recv, the scatter recv block `root`
+    // of send.  Device buffers of any placement join a burst keyed by (kind,
+    // communicator, root), issued as one grouped launch per staging buffer
+    // at the next wait (one device call at issue with grouping off); host
+    // buffers complete at issue.  The counts and types are the blocking
+    // call's.
+    int iGather(int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes, faabric_datatype_t* sendType,
+                int sendCount, faabric_datatype_t* recvType, int recvCount);
+    int iScatter(int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes, faabric_datatype_t* sendType,
+                 int sendCount, faabric_datatype_t* recvType, int recvCount);
+
     // Symmetric-heap allocation for MPI_Alloc_mem (collective: every rank
     // must allocate the same sizes in the same order)
     void* deviceAlloc(int rank, size_t bytes);
@@ -607,6 +621,14 @@ class MpiWorld
     // alias (the caller refused MPI_IN_PLACE)
     int nbAllToAll(const DeviceComm& comm, int rank, int members, const uint8_t* send, uint8_t* recv, size_t bytes,
                    const HostPath& host);
+    // `root` is a rank of `comm`'s communicator (the caller checked it);
+    // buffers as for iGather / iScatter.  The caller decides where the call
+    // runs, once: `comm` is null unless this rank's own buffer (gather send,
+    // scatter recv) is device memory.
+    int nbGather(const DeviceComm& comm, int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes,
+                 const HostPath& host);
+    int nbScatter(const DeviceComm& comm, int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes,
+                  const HostPath& host);
     // Issues this rank thread's pending burst if it is keyed to `comm`, and
     // waits for it (before `comm` is released: MPI_Comm_free)
     void settleDeviceBurst(const DeviceComm& comm);

@@ -40,7 +40,9 @@ __device__ __forceinline__ void groupExit(const GroupArgs& a, BlockBarrier& bar)
 
 // Index of the segment that owns chunk `ch`.  A warp's chunks ascend, so the
 // answer is usually `cur` again; otherwise a binary search over chunk0.
-__device__ __forceinline__ int groupSegOf(const GroupSeg* s,
+// (Seg: GroupSeg, or RootedSeg of the grouped gather and scatter)
+template<typename Seg>
+__device__ __forceinline__ int groupSegOf(const Seg* s,
                                           uint32_t nSegs,
                                           int cur,
                                           uint32_t ch)

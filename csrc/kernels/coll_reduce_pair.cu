@@ -64,6 +64,9 @@ cudaError_t preloadAllKernels()
         e = preloadMoveKernels();
     }
     if (e == cudaSuccess) {
+        e = preloadRootedKernels();
+    }
+    if (e == cudaSuccess) {
         e = preloadMoveBulkKernel();
     }
     if (e == cudaSuccess) {

@@ -87,7 +87,12 @@ struct GroupArgs
     uint32_t nSegs;
     uint32_t totalChunks;
     int32_t noSync;
-    int32_t root; // grouped broadcast only: the source rank
+    int32_t root; // grouped broadcast, gather and scatter: the root rank
+    // grouped gather and scatter only: symmetric offset of every rank's
+    // staging buffer, and which GROUP_PHASE_* steps this launch runs
+    uint64_t stageOff;
+    int32_t phase;
+    int32_t pad;
 };
 
 // vectors per warp-chunk for a world of n ranks (host and kernel must agree)
@@ -142,6 +147,40 @@ cudaError_t launchGroupAllToAll(const GroupArgs& a,
                                 int blocks,
                                 int threads,
                                 cudaStream_t stream);
+
+// ---- grouped gather and scatter: many MPI_Gather / MPI_Scatter calls with
+// one root, ONE launch ----
+// User buffers are any memory this rank's GPU can load and store, at any
+// alignment; the peers exchange through their staging buffers (GroupArgs
+// .stageOff).  The table is GroupSeg-sized RootedSeg entries, one per piece
+// of an item (an item larger than a launch's staging room is cut into
+// pieces).  Piece bytes [off, off + CB) with CB = fbGroupChunkVecs(n) * 16
+// are chunk chunk0 + off / CB, and chunk ch's staging slice is [ch * CB,
+// (ch + 1) * CB) of the staging buffer: so the slices follow from the counts
+// alone, and every rank has the same chunk space.
+//   gather:  LOCAL: every non-root copies its send into its own slices;
+//            entry barrier; MOVE: the root copies peer p's slices to block p
+//            of its recv, and its send to block `root` unless send is that
+//            block (in place); exit barrier.
+//   scatter: entry barrier; MOVE: the root copies block p of its send into
+//            peer p's slices, and block `root` to its recv unless recv is
+//            that block (in place); exit barrier; LOCAL: every non-root
+//            copies its slices into its recv.
+// With noSync the launch runs the steps of `phase` with no barrier (the host
+// runs the LOCAL and MOVE steps as two launches around stream barriers).
+struct RootedSeg
+{
+    uint64_t send;   // this rank's send address at the piece (0: not given)
+    uint64_t recv;   // this rank's recv address at the piece (0: not given)
+    uint32_t bytes;  // bytes of the piece per rank
+    uint32_t chunk0; // the piece's first chunk (same field as GroupSeg's)
+    uint64_t stride; // bytes per rank of the whole item: block p at p * stride
+};
+static_assert(sizeof(RootedSeg) == sizeof(GroupSeg), "rooted tables use GroupSeg slots");
+#define GROUP_PHASE_LOCAL 1
+#define GROUP_PHASE_MOVE 2
+cudaError_t launchGroupGather(const GroupArgs& a, int blocks, int threads, cudaStream_t stream);
+cudaError_t launchGroupScatter(const GroupArgs& a, int blocks, int threads, cudaStream_t stream);
 
 struct ReduceLaunchers
 {
@@ -502,6 +541,7 @@ cudaError_t preloadStateKernels();
 // Preload every kernel of the library on the current device (see above)
 cudaError_t preloadAllKernels();
 cudaError_t preloadMoveKernels();
+cudaError_t preloadRootedKernels();
 
 // TMA bulk-copy variant of the pull collectives (coll_move_bulk.cu)
 bool moveBulkSupported(const MoveArgs& a);

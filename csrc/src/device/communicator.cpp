@@ -1236,6 +1236,8 @@ const fb::KernelTable CUDA_KERNELS = {
     .groupAllGather = fb::launchGroupAllGather,
     .groupBroadcast = fb::launchGroupBroadcast,
     .groupAllToAll = fb::launchGroupAllToAll,
+    .groupGather = fb::launchGroupGather,
+    .groupScatter = fb::launchGroupScatter,
     .move = fb::launchMove,
     .moveBulk = fb::launchMoveBulk,
     .barrier = fb::launchBarrier,
@@ -1261,6 +1263,8 @@ const fb::KernelTable HOST_KERNELS = {
     .groupAllGather = fb::host::groupAllGather,
     .groupBroadcast = fb::host::groupBroadcast,
     .groupAllToAll = fb::host::groupAllToAll,
+    .groupGather = fb::host::groupGather,
+    .groupScatter = fb::host::groupScatter,
     .move = fb::host::moveKernel,
     .moveBulk = fb::host::moveBulk,
     .barrier = fb::host::barrierKernel,
@@ -1788,6 +1792,8 @@ struct Communicator::GroupLaunch
     uint32_t totalChunks = 0;
     uint64_t vecsPerRank = 0; // same on every rank: sizes the grid
     uint64_t bytes = 0;
+    // rooted kinds: an item of the launch has no send (bit 0) / no recv (bit 1)
+    uint32_t missing = 0;
 };
 
 struct Communicator::GroupPlan
@@ -2042,19 +2048,77 @@ static int buildShardSegs(const Communicator& c,
 // items per launch: every item yields at most one segment per rank
 static const size_t GROUP_ITEMS_PER_LAUNCH = FB_GROUP_MAX_SEGS - 8;
 
+// The next launch of a gather or scatter list from `at` on, which it
+// advances: pieces of items, one RootedSeg each, while there are segment
+// slots and staging chunks left (launch_api.h).  An item larger than the
+// staging room left is cut at a chunk boundary and goes on in the next
+// launch.  Only the counts decide the cuts, so every rank cuts alike.
+static void buildRootedSegs(const Communicator::GroupItem* items,
+                            size_t nItems,
+                            size_t esize,
+                            int nranks,
+                            size_t stageBytes,
+                            Communicator::GroupCursor& at,
+                            SegBuild& out,
+                            uint32_t& missing)
+{
+    const uint64_t cb = (uint64_t)fb::fbGroupChunkVecs(nranks) * 16;
+    // (a piece's bytes are a uint32)
+    const uint64_t room = std::min<uint64_t>(stageBytes, (uint64_t)1 << 31) / cb;
+    uint64_t chunks = 0;
+    while (at.item < nItems && out.segs.size() < GROUP_ITEMS_PER_LAUNCH && chunks < room) {
+        const Communicator::GroupItem& it = items[at.item];
+        const uint64_t stride = (uint64_t)it.count * esize;
+        if (stride == 0) {
+            at.item++;
+            continue;
+        }
+        const uint64_t len = std::min(stride - at.offset, (room - chunks) * cb);
+        fb::RootedSeg sg;
+        sg.send = it.send != nullptr ? (uint64_t)(uintptr_t)it.send + at.offset : 0;
+        sg.recv = it.recv != nullptr ? (uint64_t)(uintptr_t)it.recv + at.offset : 0;
+        sg.bytes = (uint32_t)len;
+        sg.chunk0 = (uint32_t)chunks;
+        sg.stride = stride;
+        missing |= (it.send == nullptr ? 1u : 0u) | (it.recv == nullptr ? 2u : 0u);
+        fb::GroupSeg raw;
+        memcpy(&raw, &sg, sizeof(raw));
+        out.segs.push_back(raw);
+        chunks += (len + cb - 1) / cb;
+        out.bytes += len * nranks;
+        at.offset += len;
+        if (at.offset == stride) {
+            at.item++;
+            at.offset = 0;
+        }
+    }
+    out.totalChunks = (uint32_t)chunks;
+    out.vecsPerRank = chunks * (cb / 16);
+}
+
 // One launch of items[0..nItems) (at most GROUP_ITEMS_PER_LAUNCH): this rank's
 // segments in `segs`, the launch's sizes in `l` (l.dSegs is left to the caller)
 int Communicator::groupBatch(GroupKind kind,
                              const GroupItem* items,
                              size_t nItems,
                              size_t esize,
+                             GroupCursor& at,
                              std::vector<fb::GroupSeg>& segs,
                              GroupLaunch& l) const
 {
     SegBuild sb;
-    const int rc = kind == GROUP_ALLREDUCE || kind == GROUP_BROADCAST
-                     ? buildGroupSegs(*this, items, nItems, esize, kind == GROUP_BROADCAST, sb)
-                     : buildShardSegs(*this, kind, items, nItems, esize, sb);
+    int rc = FB_OK;
+    if (kind == GROUP_GATHER || kind == GROUP_SCATTER) {
+        buildRootedSegs(items, nItems, esize, dev_.nranks, cfg_.stageBytes, at, sb, l.missing);
+    } else {
+        // a window of GROUP_ITEMS_PER_LAUNCH whole items
+        const size_t begin = at.item;
+        const size_t cnt = std::min(GROUP_ITEMS_PER_LAUNCH, nItems - begin);
+        at.item += cnt;
+        rc = kind == GROUP_ALLREDUCE || kind == GROUP_BROADCAST
+               ? buildGroupSegs(*this, items + begin, cnt, esize, kind == GROUP_BROADCAST, sb)
+               : buildShardSegs(*this, kind, items + begin, cnt, esize, sb);
+    }
     if (rc != FB_OK) {
         return rc;
     }
@@ -2077,7 +2141,7 @@ std::shared_ptr<Communicator::GroupPlan> Communicator::prepareGroup(
     int& rc = rcOut ? *rcOut : rcLocal;
     rc = FB_OK;
     const size_t esize = fbDtypeSize(dtype);
-    if (esize == 0 || kind < GROUP_ALLREDUCE || kind > GROUP_ALLTOALL) {
+    if (esize == 0 || kind < GROUP_ALLREDUCE || kind > GROUP_SCATTER) {
         rc = FB_E_INVALID;
         return nullptr;
     }
@@ -2087,10 +2151,10 @@ std::shared_ptr<Communicator::GroupPlan> Communicator::prepareGroup(
     plan->dtype = dtype;
     plan->device = device_;
     plan->items = nItems;
-    for (size_t begin = 0; begin < nItems; begin += GROUP_ITEMS_PER_LAUNCH) {
+    for (GroupCursor at; at.item < nItems;) {
         std::vector<fb::GroupSeg> segs;
         GroupLaunch l;
-        rc = groupBatch(kind, items + begin, std::min(GROUP_ITEMS_PER_LAUNCH, nItems - begin), esize, segs, l);
+        rc = groupBatch(kind, items, nItems, esize, at, segs, l);
         if (rc != FB_OK) {
             return nullptr;
         }
@@ -2154,7 +2218,10 @@ int Communicator::launchGroup(const GroupLaunch& l,
     a.nSegs = l.nSegs;
     a.totalChunks = l.totalChunks;
     a.noSync = ((flags & FB_FLAG_NOSYNC) || ss || n == 1) ? 1 : 0;
-    a.root = kind == GROUP_BROADCAST ? root : 0;
+    a.root = (kind == GROUP_BROADCAST || kind == GROUP_GATHER || kind == GROUP_SCATTER) ? root : 0;
+    if (kind == GROUP_GATHER || kind == GROUP_SCATTER) {
+        return launchRooted(l, kind, a, ss, flags, s);
+    }
     if (ss && streamBarrier(flags, s) != FB_OK) {
         return FB_E_CUDA;
     }
@@ -2191,6 +2258,56 @@ int Communicator::launchGroup(const GroupLaunch& l,
     return FB_OK;
 }
 
+// Whether this rank lacks a buffer of a gather or scatter list (`missing`:
+// GroupLaunch::missing over the list): every rank needs its own side, the
+// root both.  Checked before the list's first launch.
+static bool rootedMissing(Communicator::GroupKind kind, bool isRoot, uint32_t missing)
+{
+    const uint32_t needed = isRoot ? 3u : (kind == Communicator::GROUP_GATHER ? 1u : 2u);
+    return (missing & needed) != 0;
+}
+
+// A gather or scatter launch.  With stream-ordered barriers the kernel runs
+// as two launches: gather LOCAL, barrier, MOVE, barrier; scatter barrier,
+// MOVE, barrier, LOCAL.
+int Communicator::launchRooted(const GroupLaunch& l, GroupKind kind, fb::GroupArgs& a, bool ss, int flags,
+                               cudaStream_t s)
+{
+    const bool gather = kind == GROUP_GATHER;
+    a.stageOff = stageSendOff_;
+    // no warp without a chunk (as the all-to-all)
+    const uint64_t warps = (uint64_t)cfg_.threads / 32;
+    const int blocks = (int)std::clamp<uint64_t>(
+      (l.totalChunks + warps - 1) / warps, 1, (uint64_t)groupGrid(cfg_, dev_.nranks, l.vecsPerRank));
+    const auto launch = gather ? k_->groupGather : k_->groupScatter;
+    auto run = [&](int phase) {
+        a.phase = phase;
+        return launch(a, blocks, cfg_.threads, s) == cudaSuccess ? FB_OK : FB_E_CUDA;
+    };
+    int rc;
+    if (!ss) {
+        rc = run(GROUP_PHASE_LOCAL | GROUP_PHASE_MOVE);
+    } else if (gather) {
+        rc = run(GROUP_PHASE_LOCAL);
+        rc = rc == FB_OK ? streamBarrier(flags, s) : rc;
+        rc = rc == FB_OK ? run(GROUP_PHASE_MOVE) : rc;
+        rc = rc == FB_OK ? streamBarrier(flags, s) : rc;
+    } else {
+        rc = streamBarrier(flags, s);
+        rc = rc == FB_OK ? run(GROUP_PHASE_MOVE) : rc;
+        rc = rc == FB_OK ? streamBarrier(flags, s) : rc;
+        rc = rc == FB_OK ? run(GROUP_PHASE_LOCAL) : rc;
+    }
+    if (rc != FB_OK) {
+        return FB_E_CUDA;
+    }
+    // (the second launch of a stream-ordered pair is a staging copy)
+    stats_.launches++;
+    stats_.stagedCopies += ss ? 1 : 0;
+    stats_.bytes += l.bytes;
+    return FB_OK;
+}
+
 namespace {
 // Indexed by GroupKind: the NVTX ranges of runGroup and groupMany, and the
 // kind's name in messages
@@ -2204,7 +2321,8 @@ struct GroupKindNames
 const GroupKindNames kGroupNames[] = {
     FB_GROUP_NAMES("allReduce", "all-reduce"), FB_GROUP_NAMES("reduceScatter", "reduce-scatter"),
     FB_GROUP_NAMES("allGather", "all-gather"), FB_GROUP_NAMES("broadcast", "broadcast"),
-    FB_GROUP_NAMES("allToAll", "all-to-all"),
+    FB_GROUP_NAMES("allToAll", "all-to-all"), FB_GROUP_NAMES("gather", "gather"),
+    FB_GROUP_NAMES("scatter", "scatter"),
 };
 #undef FB_GROUP_NAMES
 
@@ -2214,13 +2332,13 @@ const int GROUP_NOTHING = 1;
 
 const char* Communicator::groupKindName(GroupKind kind)
 {
-    return kind >= GROUP_ALLREDUCE && kind <= GROUP_ALLTOALL ? kGroupNames[kind].name : "unknown";
+    return kind >= GROUP_ALLREDUCE && kind <= GROUP_SCATTER ? kGroupNames[kind].name : "unknown";
 }
 
 // The rules runGroup and groupMany share (see the header).  FB_OK, with
 // `grouped` false when a reducing pair has no grouped kernel; GROUP_NOTHING;
 // or an error code.
-int Communicator::groupCheck(GroupKind kind, int dtype, int op, int root, bool& grouped) const
+int Communicator::groupCheck(GroupKind kind, int dtype, int op, int root, int flags, bool& grouped) const
 {
     if (fbDtypeSize(dtype) == 0) {
         return FB_E_INVALID;
@@ -2234,12 +2352,16 @@ int Communicator::groupCheck(GroupKind kind, int dtype, int op, int root, bool& 
             return FB_E_UNSUPPORTED;
         }
         grouped = (kind == GROUP_ALLREDUCE ? L->group : L->groupRs) != nullptr;
-    } else if (kind == GROUP_BROADCAST) {
+    } else if (kind == GROUP_BROADCAST || kind == GROUP_GATHER || kind == GROUP_SCATTER) {
         if (root < 0 || root >= dev_.nranks) {
             return FB_E_INVALID;
         }
-        if (dev_.nranks == 1) {
+        if (kind == GROUP_BROADCAST && dev_.nranks == 1) {
             return GROUP_NOTHING; // the root's buffers already hold the result
+        }
+        // (one staging buffer per rank, shared by the channels)
+        if (kind != GROUP_BROADCAST && FB_FLAG_GET_CHANNEL(flags) != 0) {
+            return FB_E_INVALID;
         }
     }
     return FB_OK;
@@ -2252,12 +2374,21 @@ int Communicator::runGroup(GroupKind kind, const GroupPlan& plan, int op, int ro
     }
     NvtxRange nvtxRange(kGroupNames[kind].run);
     bool grouped = false;
-    int rc = groupCheck(kind, plan.dtype, op, root, grouped);
+    int rc = groupCheck(kind, plan.dtype, op, root, flags, grouped);
     if (rc != FB_OK) {
         return rc == GROUP_NOTHING ? FB_OK : rc;
     }
     if (!grouped) {
         return FB_E_UNSUPPORTED;
+    }
+    if (kind == GROUP_GATHER || kind == GROUP_SCATTER) {
+        uint32_t missing = 0;
+        for (const auto& l : plan.launches) {
+            missing |= l.missing;
+        }
+        if (rootedMissing(kind, dev_.rank == root, missing)) {
+            return FB_E_INVALID;
+        }
     }
     bindDevice();
     for (const auto& l : plan.launches) {
@@ -2281,26 +2412,40 @@ int Communicator::groupMany(GroupKind kind,
                             int flags,
                             cudaStream_t s)
 {
-    if (kind < GROUP_ALLREDUCE || kind > GROUP_ALLTOALL) {
+    if (kind < GROUP_ALLREDUCE || kind > GROUP_SCATTER) {
         return FB_E_INVALID;
     }
     NvtxRange nvtxRange(kGroupNames[kind].many);
     bool grouped = false;
-    int rc = groupCheck(kind, dtype, op, root, grouped);
+    int rc = groupCheck(kind, dtype, op, root, flags, grouped);
     if (rc != FB_OK) {
         return rc == GROUP_NOTHING ? FB_OK : rc;
     }
     const size_t esize = fbDtypeSize(dtype);
+    if (kind == GROUP_GATHER || kind == GROUP_SCATTER) {
+        uint32_t missing = 0;
+        for (size_t i = 0; i < nItems; i++) {
+            if (items[i].count != 0) {
+                missing |= (items[i].send == nullptr ? 1u : 0u) | (items[i].recv == nullptr ? 2u : 0u);
+            }
+        }
+        if (rootedMissing(kind, dev_.rank == root, missing)) {
+            return FB_E_INVALID;
+        }
+    }
     bindDevice();
     // try the grouped path batch by batch; anything not symmetric / aligned
     // goes through the per-tensor calls (the choice depends only on arguments
     // that are symmetric across ranks)
-    for (size_t begin = 0; begin < nItems; begin += GROUP_ITEMS_PER_LAUNCH) {
-        const size_t cnt = std::min(GROUP_ITEMS_PER_LAUNCH, nItems - begin);
+    for (GroupCursor at; at.item < nItems;) {
+        const size_t begin = at.item;
         std::vector<fb::GroupSeg> segs;
         GroupLaunch l;
-        rc = grouped ? groupBatch(kind, items + begin, cnt, esize, segs, l) : FB_E_UNSUPPORTED;
+        rc = grouped ? groupBatch(kind, items, nItems, esize, at, segs, l) : FB_E_UNSUPPORTED;
         if (rc != FB_OK) {
+            // (only the kinds that group a window of whole items fail here)
+            const size_t cnt = std::min(GROUP_ITEMS_PER_LAUNCH, nItems - begin);
+            at = GroupCursor{ begin + cnt, 0 };
             rc = groupPerItem(kind, items + begin, cnt, dtype, op, root, flags, s);
             if (rc != FB_OK) {
                 return rc;

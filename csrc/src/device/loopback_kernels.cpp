@@ -651,6 +651,58 @@ cudaError_t groupAllToAll(const GroupArgs& a, int blocks, int, cudaStream_t)
     return cudaSuccess;
 }
 
+// The twins of groupGatherKernel and groupScatterKernel (RootedSeg tables):
+// a piece's staging slice is its chunks, [chunk0 * CB, chunk0 * CB + bytes)
+static cudaError_t groupRooted(const GroupArgs& a, int blocks, bool gather)
+{
+    const FbCommDev& c = a.comm;
+    const RootedSeg* segs = reinterpret_cast<const RootedSeg*>(a.segs);
+    const uint64_t cb = (uint64_t)fbGroupChunkVecs(c.nranks) * 16;
+    const bool isRoot = c.rank == a.root;
+    auto slice = [&](int p, const RootedSeg& sg) { return c.heap[p] + a.stageOff + sg.chunk0 * cb; };
+    auto user = [](uint64_t addr) { return reinterpret_cast<uint8_t*>(addr); };
+    if (gather && !isRoot && (a.phase & GROUP_PHASE_LOCAL)) {
+        for (uint32_t si = 0; si < a.nSegs; si++) {
+            memcpy(slice(c.rank, segs[si]), user(segs[si].send), segs[si].bytes);
+        }
+    }
+    bool ok = a.noSync || gridBarrier(c, blocks);
+    if (ok && isRoot && (a.phase & GROUP_PHASE_MOVE)) {
+        for (uint32_t si = 0; si < a.nSegs; si++) {
+            const RootedSeg& sg = segs[si];
+            // block p of the root's user buffer, and the root's other buffer
+            uint8_t* const blocked = user(gather ? sg.recv : sg.send);
+            uint8_t* const single = user(gather ? sg.send : sg.recv);
+            for (int p = 0; p < c.nranks; p++) {
+                uint8_t* const blk = blocked + (uint64_t)p * sg.stride;
+                uint8_t* const other = p == a.root ? single : slice(p, sg);
+                if (other != blk) { // in place: the root's block stays
+                    gather ? memcpy(blk, other, sg.bytes) : memcpy(other, blk, sg.bytes);
+                }
+            }
+        }
+    }
+    if (!a.noSync) {
+        ok = gridBarrier(c, blocks) && ok;
+    }
+    if (ok && !gather && !isRoot && (a.phase & GROUP_PHASE_LOCAL)) {
+        for (uint32_t si = 0; si < a.nSegs; si++) {
+            memcpy(user(segs[si].recv), slice(c.rank, segs[si]), segs[si].bytes);
+        }
+    }
+    return cudaSuccess;
+}
+
+cudaError_t groupGather(const GroupArgs& a, int blocks, int, cudaStream_t)
+{
+    return groupRooted(a, blocks, true);
+}
+
+cudaError_t groupScatter(const GroupArgs& a, int blocks, int, cudaStream_t)
+{
+    return groupRooted(a, blocks, false);
+}
+
 // ----------------------------------------------------------------- move ----
 // The CUDA kernels copy in W-byte words.  Every address they touch that way
 // must be W-aligned (a misaligned vector access is a device fault), and every

@@ -1630,6 +1630,9 @@ struct MpiWorld::NbCall
     int root;
     faabric::device::Communicator::GroupItem item;
     bool direct = true;
+    // the kind stages every buffer (gather, scatter): device buffers join
+    // the burst wherever they live
+    bool staged = false;
 };
 
 // Symmetric, aligned buffers of a call the device takes (`device`) join this
@@ -1643,15 +1646,16 @@ int MpiWorld::nbCollective(const DeviceComm& comm, int rank, bool device, const 
     AsyncRequest r = collectiveRequest(rank);
     cacheDeviceComm(rank);
     if (device && comm != nullptr) {
-        const Placement at = placeCollective(
-          *comm, groupIallreduce, call.item.send, call.sendBytes, call.item.recv, call.recvBytes, call.shardBytes);
+        const Placement at = call.staged ? Placement{ false, groupIallreduce }
+                                         : placeCollective(*comm, groupIallreduce, call.item.send, call.sendBytes,
+                                                           call.item.recv, call.recvBytes, call.shardBytes);
         if (at.grouped) {
             deferToGroup(call.kind, comm, call.dtype, call.op, call.root, call.item, requestId, std::move(r),
                          deviceCollectives);
             return requestId;
         }
         void* s = tls.cachedStream0;
-        if (call.direct && (at.symmetric || isDevicePointer(call.item.send)) &&
+        if (call.direct && (call.staged || at.symmetric || isDevicePointer(call.item.send)) &&
             issueDevice(*comm, s, deviceCollectives, issue)) {
             return recordDevice(requestId, std::move(r), comm, s);
         }
@@ -1779,6 +1783,56 @@ int MpiWorld::nbAllToAll(const DeviceComm& comm,
                        { send, recv, bytes } };
     return nbCollective(comm, rank, bytes > 0, call, [&](auto& c, cudaStream_t st) {
         return c.allToAll(send, recv, bytes, symFlag(c, send, total), st);
+    }, host);
+}
+
+int MpiWorld::iGather(int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes, faabric_datatype_t* sendType,
+                      int sendCount, faabric_datatype_t* recvType, int recvCount)
+{
+    checkRanksRange(rank, root);
+    cacheDeviceComm(rank);
+    // (the blocking call takes the root's in-place send as recv itself)
+    const bool inPlace = rank == root && send == recv + (size_t)root * bytes;
+    const DeviceComm dev = bytes > 0 && isDevicePointer(send) ? tls.cachedComm : nullptr;
+    return nbGather(dev, rank, root, send, recv, bytes, [&] {
+        gather(rank, root, inPlace ? recv : send, sendType, sendCount, recv, recvType, recvCount);
+    });
+}
+
+int MpiWorld::nbGather(const DeviceComm& comm, int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes,
+                       const HostPath& host)
+{
+    // a byte copy through the staging buffers: the burst's key is
+    // (communicator, root).  The caller passes `comm` only for a device
+    // send (an in-place root's send lies in its recv).
+    NbCall call{ bytes, bytes, bytes, faabric::device::Communicator::GROUP_GATHER, FB_U8, -1, root,
+                 { send, recv, bytes } };
+    call.staged = true;
+    return nbCollective(comm, rank, bytes > 0, call, [&](auto& c, cudaStream_t st) {
+        return c.gather(send, recv, bytes, root, 0, st);
+    }, host);
+}
+
+int MpiWorld::iScatter(int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes, faabric_datatype_t* sendType,
+                       int sendCount, faabric_datatype_t* recvType, int recvCount)
+{
+    checkRanksRange(root, rank);
+    cacheDeviceComm(rank);
+    const DeviceComm dev = bytes > 0 && isDevicePointer(recv) ? tls.cachedComm : nullptr;
+    return nbScatter(dev, rank, root, send, recv, bytes, [&] {
+        scatter(root, rank, send, sendType, sendCount, recv, recvType, recvCount);
+    });
+}
+
+int MpiWorld::nbScatter(const DeviceComm& comm, int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes,
+                        const HostPath& host)
+{
+    // the mirror of nbGather: `comm` only for a device recv
+    NbCall call{ bytes, bytes, bytes, faabric::device::Communicator::GROUP_SCATTER, FB_U8, -1, root,
+                 { send, recv, bytes } };
+    call.staged = true;
+    return nbCollective(comm, rank, bytes > 0, call, [&](auto& c, cudaStream_t st) {
+        return c.scatter(send, recv, bytes, root, 0, st);
     }, host);
 }
 

@@ -1049,6 +1049,65 @@ int MPI_Ialltoall(const void* sendbuf, int sendcount, MPI_Datatype sendtype, voi
                    request);
 }
 
+int MPI_Igather(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                MPI_Datatype recvtype, int root, MPI_Comm comm, MPI_Request* request)
+{
+    SPDLOG_TRACE("MPI - MPI_Igather all -> {}", root);
+    MpiWorld& world = getExecutingWorld();
+    const int rank = executingContext.getRank();
+    auto sub = subOf(comm);
+    if (root < 0 || root >= (sub != nullptr ? sub->size() : world.getSize())) {
+        return MPI_ERR_ARG;
+    }
+    const bool isRoot = (sub != nullptr ? sub->commRankOf(rank) : rank) == root;
+    const bool inPlace = isRoot && sendbuf == MPI_IN_PLACE;
+    // (the counts that mean something here: the root's receive block)
+    const size_t bytes = inPlace ? (size_t)recvcount * recvtype->size : (size_t)sendcount * sendtype->size;
+    // (recv only means something at the root, send everywhere)
+    uint8_t* recv = (uint8_t*)recvbuf;
+    const uint8_t* send = inPlace ? recv + (size_t)root * bytes : (const uint8_t*)sendbuf;
+    if (sub != nullptr) {
+        auto dev = bytes > 0 && MpiWorld::isDevicePointer(send) ? sub->deviceComm(world, rank) : nullptr;
+        return handOut(world.nbGather(dev, rank, root, send, recv, bytes, [&] {
+            sub->gather(world, rank, root, inPlace ? nullptr : send, recv, isRoot ? recvtype : sendtype,
+                        isRoot ? recvcount : sendcount);
+        }),
+                       request);
+    }
+    return handOut(world.iGather(rank, root, send, recv, bytes, inPlace ? recvtype : sendtype,
+                                 inPlace ? recvcount : sendcount, recvtype, recvcount),
+                   request);
+}
+
+int MPI_Iscatter(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                 MPI_Datatype recvtype, int root, MPI_Comm comm, MPI_Request* request)
+{
+    SPDLOG_TRACE("MPI - MPI_Iscatter {} -> all", root);
+    MpiWorld& world = getExecutingWorld();
+    const int rank = executingContext.getRank();
+    auto sub = subOf(comm);
+    if (root < 0 || root >= (sub != nullptr ? sub->size() : world.getSize())) {
+        return MPI_ERR_ARG;
+    }
+    const bool isRoot = (sub != nullptr ? sub->commRankOf(rank) : rank) == root;
+    const bool inPlace = isRoot && recvbuf == MPI_IN_PLACE;
+    const size_t bytes = isRoot ? (size_t)sendcount * sendtype->size : (size_t)recvcount * recvtype->size;
+    // (send only means something at the root, recv everywhere)
+    const uint8_t* send = (const uint8_t*)sendbuf;
+    uint8_t* recv = inPlace ? const_cast<uint8_t*>(send) + (size_t)root * bytes : (uint8_t*)recvbuf;
+    if (sub != nullptr) {
+        auto dev = bytes > 0 && MpiWorld::isDevicePointer(recv) ? sub->deviceComm(world, rank) : nullptr;
+        return handOut(world.nbScatter(dev, rank, root, send, recv, bytes, [&] {
+            sub->scatter(world, rank, root, send, inPlace ? nullptr : recv, isRoot ? sendtype : recvtype,
+                         isRoot ? sendcount : recvcount);
+        }),
+                       request);
+    }
+    return handOut(world.iScatter(rank, root, send, recv, bytes, sendtype, sendcount, inPlace ? sendtype : recvtype,
+                                  inPlace ? sendcount : recvcount),
+                   request);
+}
+
 int MPI_Get_processor_name(char* name, int* resultlen)
 {
     SPDLOG_TRACE("MPI - MPI_Get_processor_name");

@@ -85,7 +85,15 @@ OPS = {
     "no_op": 33,
 }
 # Communicator::GroupKind
-GROUP_KINDS = {"all_reduce": 0, "reduce_scatter": 1, "all_gather": 2, "broadcast": 3, "all_to_all": 4}
+GROUP_KINDS = {
+    "all_reduce": 0,
+    "reduce_scatter": 1,
+    "all_gather": 2,
+    "broadcast": 3,
+    "all_to_all": 4,
+    "gather": 5,
+    "scatter": 6,
+}
 ALGOS = {"auto": 0, "oneshot": 1, "twoshot": 2, "nvls": 3, "ll": 4}
 ALGO_NAMES = {v: k for k, v in ALGOS.items()}
 FLAG_SYMMETRIC = 1
@@ -463,11 +471,45 @@ class Communicator:
         the reverse; all-to-all needs equal send and recv numel and element
         size, numel divisible by ``size`` (in ``dtype`` elements too), and
         counts per block; a broadcast (each buffer as send and recv) needs
-        contiguous tensors and a root in the communicator, and counts bytes."""
+        contiguous tensors and a root in the communicator, and counts bytes.
+        Gather follows the all-gather rule and scatter the reduce-scatter
+        rule, with a root in the communicator and contiguous tensors on this
+        communicator's GPU; the root's side (gather recvs, scatter sends) may
+        be None off the root, or a list of None."""
+        if kind in ("gather", "scatter"):
+            if not 0 <= int(root) < self.size:
+                raise CommError(f"{what}: root {root} outside a communicator of {self.size}")
+            if kind == "gather" and recvs is None:
+                recvs = [None] * len(sends or [])
+            if kind == "scatter" and sends is None:
+                sends = [None] * len(recvs or [])
         if len(sends) != len(recvs) or not sends:
             raise CommError(f"{what}: need equally long, non-empty lists")
         per = 1
-        if kind == "broadcast":
+        if kind in ("gather", "scatter"):
+            gather = kind == "gather"
+            rooted = self.rank == int(root)
+            for i, (s, r) in enumerate(zip(sends, recvs)):
+                small, big = (s, r) if gather else (r, s)
+                # (the kernels load and store these addresses as they are)
+                for t in (s, r):
+                    if t is not None and (not t.is_cuda or t.device.index != self.device or not t.is_contiguous()):
+                        raise CommError(
+                            f"{what}: item {i} must be contiguous tensors on cuda:{self.device}, not {t.device}"
+                            f"{'' if t.is_contiguous() else ' (non-contiguous)'}"
+                        )
+                if small is None or (big is None and rooted):
+                    raise CommError(f"{what}: item {i} needs a {'send' if gather else 'recv'} on every rank "
+                                    f"and a {'recv' if gather else 'send'} on the root")
+                if big is not None and big.numel() != self.size * small.numel():
+                    raise CommError(
+                        f"{what}: item {i} has {s.numel()} send and {r.numel()} recv elements; "
+                        f"{'recv' if gather else 'send'} must hold {self.size} x {'send' if gather else 'recv'}"
+                    )
+                if big is not None and big.element_size() != small.element_size():
+                    raise CommError(f"{what}: item {i} has send and recv elements of different sizes")
+            typed = [self._typed(s if gather else r, dtype) for s, r in zip(sends, recvs)]
+        elif kind == "broadcast":
             if not 0 <= int(root) < self.size:
                 raise CommError(f"{what}: root {root} outside a communicator of {self.size}")
             for i, t in enumerate(sends):
@@ -506,20 +548,26 @@ class Communicator:
             if c % per != 0:
                 raise CommError(f"{what}: item {i} has {c} {dtype} elements, not divisible by {self.size}")
         n = len(sends)
-        sp = (C.c_void_p * n)(*[t.data_ptr() for t in sends])
-        rp = (C.c_void_p * n)(*[t.data_ptr() for t in recvs])
+        sp = (C.c_void_p * n)(*[t.data_ptr() if t is not None else None for t in sends])
+        rp = (C.c_void_p * n)(*[t.data_ptr() if t is not None else None for t in recvs])
         cnt = (C.c_uint64 * n)(*[c // per for c, _ in typed])
         return n, sp, rp, cnt, typed[0][1]
 
-    def _prepare(self, what, kind, sends, recvs, dtype, sized):
+    def _prepare(self, what, kind, sends, recvs, dtype, sized, root=0):
         """A GroupPlan of ``kind``; ``sized`` is the list whose bytes it moves."""
-        n, sp, rp, cnt, dt = self._group_items(what, kind, sends, recvs, dtype)
+        n, sp, rp, cnt, dt = self._group_items(what, kind, sends, recvs, dtype, root)
         h = self._lib.fb_group_prepare(self._h, GROUP_KINDS[kind], n, sp, rp, cnt, dt)
         if not h:
             raise CommError(f"{what} failed [{_lib.last_error()}]")
-        return GroupPlan(self, h, n, sum(t.numel() * t.element_size() for t in sized))
+        plan = GroupPlan(self, h, n, sum(t.numel() * t.element_size() for t in sized if t is not None))
+        plan.root = int(root)
+        return plan
 
     def _launch(self, what, kind, plan, op, root, stream, channel, flags):
+        if kind in ("gather", "scatter") and int(root) != plan.root:
+            # (the root's side was checked, and on other ranks may be missing,
+            # for the root the plan was prepared for)
+            raise CommError(f"{what}: plan prepared for root {plan.root}, launched with root {root}")
         rc = self._lib.fb_group_launch(
             self._h, GROUP_KINDS[kind], plan._h, op, root, flags | ((channel & 0xF) << 8), self._stream(stream)
         )
@@ -527,7 +575,7 @@ class Communicator:
 
     def _many(self, what, kind, sends, recvs, dtype, op, root, stream, channel):
         n, sp, rp, cnt, dt = self._group_items(what, kind, sends, recvs, dtype, root)
-        f = self._sym(*sends) | ((channel & 0xF) << 8)
+        f = (0 if kind in ("gather", "scatter") else self._sym(*sends)) | ((channel & 0xF) << 8)
         fop = OPS[op] if op is not None else 0
         rc = self._lib.fb_group_many(
             self._h, GROUP_KINDS[kind], n, sp, rp, cnt, dt, fop, int(root), f, self._stream(stream)
@@ -617,6 +665,42 @@ class Communicator:
         :meth:`all_to_all_group`; lists that cannot be grouped run one
         :meth:`all_to_all` per pair."""
         self._many("all_to_all_many", "all_to_all", sends, recvs, dtype, None, 0, stream, channel)
+
+    def prepare_gather_group(self, sends, recvs=None, root=0, dtype=None) -> "GroupPlan":
+        """Plan the launches that gather every pair of the lists to the root
+        given to :meth:`gather_group` (MPI_Gather per pair: block p of
+        ``recvs[i]`` on the root gets ``sends[i]`` of rank p).  Tensors are
+        any device memory at any alignment; ``recvs`` is only read on the
+        root (None elsewhere).  In place (``sends[i]`` is block ``root`` of
+        ``recvs[i]``) is allowed.  The plan launches with this ``root`` only;
+        call collectively with the same counts."""
+        return self._prepare("prepare_gather_group", "gather", sends, recvs, dtype, sends, root)
+
+    def gather_group(self, plan: "GroupPlan", root=0, stream=None, channel=0, flags=0):
+        self._launch("gather_group", "gather", plan, 0, int(root), stream, channel, flags)
+
+    def gather_many(self, sends, recvs=None, root=0, stream=None, channel=0, dtype=None):
+        """Transient variant of :meth:`prepare_gather_group` +
+        :meth:`gather_group`."""
+        self._many("gather_many", "gather", sends, recvs, dtype, None, root, stream, channel)
+
+    def prepare_scatter_group(self, sends, recvs, root=0, dtype=None) -> "GroupPlan":
+        """Plan the launches that scatter every pair of the lists from the
+        root given to :meth:`scatter_group` (MPI_Scatter per pair: ``recvs[i]``
+        of rank p gets block p of ``sends[i]`` on the root).  Tensors are any
+        device memory at any alignment; ``sends`` is only read on the root
+        (None elsewhere).  In place (``recvs[i]`` is block ``root`` of
+        ``sends[i]``) is allowed.  The plan launches with this ``root`` only;
+        call collectively with the same counts."""
+        return self._prepare("prepare_scatter_group", "scatter", sends, recvs, dtype, recvs, root)
+
+    def scatter_group(self, plan: "GroupPlan", root=0, stream=None, channel=0, flags=0):
+        self._launch("scatter_group", "scatter", plan, 0, int(root), stream, channel, flags)
+
+    def scatter_many(self, sends, recvs, root=0, stream=None, channel=0, dtype=None):
+        """Transient variant of :meth:`prepare_scatter_group` +
+        :meth:`scatter_group`."""
+        self._many("scatter_many", "scatter", sends, recvs, dtype, None, root, stream, channel)
 
     def send_recv(self, send_buf, dst, recv_buf, src, stream=None):
         rc = self._lib.fb_sendrecv(
@@ -889,7 +973,7 @@ class Communicator:
 
 class GroupPlan:
     """Device-resident segment tables of a grouped all-reduce, reduce-scatter,
-    all-gather, broadcast or all-to-all."""
+    all-gather, broadcast, all-to-all, gather or scatter."""
 
     def __init__(self, comm: Communicator, handle, n_tensors: int, nbytes: int):
         self._comm = comm
@@ -897,6 +981,8 @@ class GroupPlan:
         self.n_tensors = n_tensors
         self.nbytes = nbytes
         self.launches = int(comm._lib.fb_group_plan_launches(self._h))
+        # gather and scatter: the root the plan was prepared for
+        self.root = 0
 
     def close(self):
         if self._h:
