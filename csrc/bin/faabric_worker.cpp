@@ -29,6 +29,7 @@
 #include "../tests/mpi_rma_request_body.h"
 #include "../tests/mpi_subcomm_device_body.h"
 #include "../tests/mpi_group_alltoall_body.h"
+#include "../tests/mpi_group_reduce_body.h"
 #include "../tests/mpi_group_rooted_body.h"
 #include "../tests/mpi_group_subcomm_body.h"
 
@@ -956,6 +957,110 @@ static void registerFunctions()
             msg.set_outputdata(why);
         }
         return rc;
+    });
+
+    // MPI_Ireduce bursts on the world and on sub-communicators
+    // (mpi_group_reduce_body.h)
+    mpiFunction("group-reduce", [](int rank, int size, faabric::Message& msg) {
+        std::string why;
+        int rc = group_reduce::body(rank, size, msg.mpiworldid(), true, &why);
+        if (rc != 0) {
+            SPDLOG_ERROR("group-reduce: {}", why);
+            msg.set_outputdata(why);
+        }
+        return rc;
+    });
+
+    // A list of float32 tensors summed to rank 0 of the world per step, in
+    // device memory (MPI_Alloc_mem).  Input: "<mode>;<steps>;<count0,count1,
+    // ...>" with count_i the elements of tensor i and mode
+    //   reduce   one MPI_Reduce per tensor
+    //   ireduce  MPI_Ireduce per tensor + MPI_Waitall
+    // Rank 0 reports {"ms_per_step", "us_per_call", "launches_per_step",
+    // "wait_ms_per_step"}: the launches counted on its world device
+    // communicator, and the part of a step spent in MPI_Waitall.
+    mpiFunction("bench-group-reduce", [](int rank, int size, faabric::Message& msg) {
+        std::vector<std::string> f;
+        std::string cur;
+        for (char c : msg.inputdata() + ";") {
+            if (c == ';') {
+                f.push_back(cur);
+                cur.clear();
+            } else {
+                cur += c;
+            }
+        }
+        EXPECT(f.size() >= 3 && size >= 2);
+        const bool nb = f[0] == "ireduce";
+        const int steps = std::stoi(f[1]);
+        std::vector<size_t> counts, offs;
+        size_t total = 0;
+        for (size_t b = 0, e; b < f[2].size(); b = e + 1) {
+            e = f[2].find(',', b);
+            if (e == std::string::npos) {
+                e = f[2].size();
+            }
+            counts.push_back(std::stoull(f[2].substr(b, e - b)));
+            offs.push_back(total);
+            total += counts.back();
+        }
+        faabric::mpi::MpiWorld& world = faabric::mpi::getMpiWorldRegistry().getWorld(msg.mpiworldid());
+        float* send = nullptr;
+        float* recv = nullptr;
+        EXPECT(MPI_Alloc_mem(total * 4, MPI_INFO_FAABRIC_DEVICE, &send) == MPI_SUCCESS);
+        EXPECT(MPI_Alloc_mem(total * 4, MPI_INFO_FAABRIC_DEVICE, &recv) == MPI_SUCCESS);
+        // (copies from host memory, which wait for this rank only)
+        std::vector<float> mine(total, (float)(rank + 1));
+        cudaMemcpy(send, mine.data(), total * 4, cudaMemcpyHostToDevice);
+        MPI_Barrier(MPI_COMM_WORLD);
+        const int n = (int)counts.size();
+        std::vector<MPI_Request> reqs(n);
+        double waitMs = 0;
+        auto step = [&]() -> int {
+            for (int i = 0; i < n; i++) {
+                const int c = (int)counts[i];
+                EXPECT((nb ? MPI_Ireduce(send + offs[i], recv + offs[i], c, MPI_FLOAT, MPI_SUM, 0, MPI_COMM_WORLD,
+                                         &reqs[i])
+                           : MPI_Reduce(send + offs[i], recv + offs[i], c, MPI_FLOAT, MPI_SUM, 0, MPI_COMM_WORLD)) ==
+                       MPI_SUCCESS);
+            }
+            if (nb) {
+                auto w0 = std::chrono::steady_clock::now();
+                EXPECT(MPI_Waitall(n, reqs.data(), MPI_STATUSES_IGNORE) == MPI_SUCCESS);
+                waitMs += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - w0).count();
+            }
+            return 0;
+        };
+        for (int i = 0; i < 3; i++) {
+            EXPECT(step() == 0);
+        }
+        auto dev = world.getDeviceComm(rank);
+        EXPECT(dev != nullptr);
+        MPI_Barrier(MPI_COMM_WORLD);
+        waitMs = 0;
+        const uint64_t l0 = dev->stats().launches;
+        auto t0 = std::chrono::steady_clock::now();
+        for (int i = 0; i < steps; i++) {
+            EXPECT(step() == 0);
+        }
+        const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count() / steps;
+        const double launches = (double)(dev->stats().launches - l0) / steps;
+        MPI_Barrier(MPI_COMM_WORLD);
+        // every element of the root's output is 1 + 2 + ... + size
+        if (rank == 0) {
+            std::vector<float> back(total);
+            cudaMemcpy(back.data(), recv, total * 4, cudaMemcpyDeviceToHost);
+            const float want = (float)(size * (size + 1) / 2);
+            for (int i = 0; i < n; i++) {
+                EXPECT(back[offs[i]] == want && back[offs[i] + counts[i] - 1] == want);
+            }
+            msg.set_outputdata("{\"ms_per_step\": " + std::to_string(ms) + ", \"us_per_call\": " +
+                               std::to_string(ms * 1000.0 / n) + ", \"launches_per_step\": " + std::to_string(launches) +
+                               ", \"wait_ms_per_step\": " + std::to_string(waitMs / steps) + "}");
+        }
+        MPI_Free_mem(recv);
+        MPI_Free_mem(send);
+        return 0;
     });
 
     // A list of tensors gathered to or scattered from rank 0 of the world per

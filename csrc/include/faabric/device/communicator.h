@@ -291,16 +291,24 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     //     (size()*count elements) goes to recv (count elements) of rank p;
     //     send is read on the root only; recv == send + root*count*esize at
     //     the root is in place.
+    //   GROUP_REDUCE: send holds count elements on every rank; the root's
+    //     recv (count elements) gets op over the ranks' sends in rank order,
+    //     acc = send_0, acc = op(acc, send_p) for p = 1..size()-1
+    //     (MPI_Reduce per item).  recv is read on the root only (null
+    //     elsewhere is fine; no other rank's recv is written).  send == recv
+    //     at the root is in place.
     // Shard kinds (GROUP_REDUCE_SCATTER, GROUP_ALLGATHER, GROUP_ALLTOALL)
     // group an item only if send and recv are in the symmetric heap and
     // 16-byte aligned, count*esize is a multiple of 16, and recv overlaps no
     // send of the group on this rank.  The one exception is the in-place
     // all-gather, send == recv + rank*count*esize.  Items with count 0 are
     // skipped.
-    // Rooted kinds (GROUP_GATHER, GROUP_SCATTER) group every item with count
-    // > 0: buffers are any device memory of this rank, at any alignment and
-    // length, and may differ between ranks.  The data goes through every
-    // rank's staging buffer, so a plan does not depend on the root, and a
+    // Rooted kinds (GROUP_GATHER, GROUP_SCATTER, GROUP_REDUCE) group every
+    // item with count > 0: buffers are any device memory of this rank, at
+    // any alignment and length, and may differ between ranks.  The data goes
+    // through every rank's staging buffers (the reduce's results through the
+    // root's second one), so a plan depends on neither the root nor the op,
+    // and a
     // launch holds at most CommConfig::stageBytes per rank (rounded to
     // chunks); a larger item is cut into pieces at the same points on every
     // rank.
@@ -312,7 +320,8 @@ class Communicator : public std::enable_shared_from_this<Communicator>
         GROUP_BROADCAST = 3,
         GROUP_ALLTOALL = 4,
         GROUP_GATHER = 5,
-        GROUP_SCATTER = 6
+        GROUP_SCATTER = 6,
+        GROUP_REDUCE = 7
     };
     // Where the next launch of a list starts: an item, and a byte offset in
     // it (rooted kinds cut items larger than the staging buffer)
@@ -337,8 +346,8 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     // broadcast / allToAll calls and returns their errors (reduceScatter
     // refuses shards that are not a multiple of 16 bytes with
     // FB_E_UNSUPPORTED).  `op` is read by the reducing kinds (GROUP_ALLREDUCE,
-    // GROUP_REDUCE_SCATTER) only, `root` by GROUP_BROADCAST, GROUP_GATHER and
-    // GROUP_SCATTER only.  Both follow the same rules:
+    // GROUP_REDUCE_SCATTER, GROUP_REDUCE) only, `root` by GROUP_BROADCAST and
+    // the rooted kinds only.  Both follow the same rules:
     //   - a plan of another kind, an unknown kind or a dtype of no size:
     //     FB_E_INVALID
     //   - reducing kinds: a (dtype, op) pair with no reduction at all gives
@@ -350,15 +359,17 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     //     groupMany, pass each buffer as send and recv with FB_U8 and byte
     //     counts.
     //   - GROUP_ALLTOALL on a one-member communicator runs as a local copy
-    //   - GROUP_GATHER, GROUP_SCATTER: a root that is not a rank of this
-    //     communicator, or a channel other than 0 (the staging buffers are
-    //     per rank, not per channel), gives FB_E_INVALID; so does a missing
-    //     buffer this rank needs (every rank's own side, and both on the
-    //     root), checked over the whole list before its first launch.  On a
-    //     one-member communicator the launch is a local copy (nothing when in
-    //     place).  With FB_FLAG_NOSYNC nothing orders a peer's staging copy
-    //     against the root's, so the bytes received are unspecified (the
-    //     flag profiles one rank's data path only).
+    //   - GROUP_GATHER, GROUP_SCATTER, GROUP_REDUCE: a root that is not a
+    //     rank of this communicator, or a channel other than 0 (the staging
+    //     buffers are per rank, not per channel), gives FB_E_INVALID; so does
+    //     a missing buffer this rank needs (every rank's own side -- the send
+    //     of a gather or reduce -- and both on the root), checked over the
+    //     whole list before its first launch.  On a one-member communicator
+    //     the launch is a local copy (nothing when in place).  With
+    //     FB_FLAG_NOSYNC nothing orders a peer's staging copy against the
+    //     root's, so the bytes received are unspecified (the flag profiles
+    //     one rank's data path only).  GROUP_REDUCE has a grouped kernel for
+    //     every (dtype, op) pair that has a reduction.
     //   - GROUP_ALLREDUCE sets lastAlgo() to FB_ALGO_TWOSHOT
     int runGroup(GroupKind kind, const GroupPlan& plan, int op, int root, int flags, cudaStream_t s);
     int groupMany(GroupKind kind,
@@ -371,7 +382,7 @@ class Communicator : public std::enable_shared_from_this<Communicator>
                   cudaStream_t s);
     static size_t groupPlanLaunches(const GroupPlan& plan);
     // "all-reduce", "reduce-scatter", "all-gather", "broadcast", "all-to-all",
-    // "gather", "scatter"
+    // "gather", "scatter", "reduce"
     static const char* groupKindName(GroupKind kind);
 
     // ---- point to point (per-pair FIFO; no kernel ever spins on a peer) ----
@@ -607,7 +618,14 @@ class Communicator : public std::enable_shared_from_this<Communicator>
                 const std::string& kind);
     void finishSetup();
     int launchGroup(const GroupLaunch& l, GroupKind kind, int dtype, int op, int root, int flags, cudaStream_t s);
-    int launchRooted(const GroupLaunch& l, GroupKind kind, fb::GroupArgs& a, bool ss, int flags, cudaStream_t s);
+    int launchRooted(const GroupLaunch& l,
+                     GroupKind kind,
+                     int dtype,
+                     int op,
+                     fb::GroupArgs& a,
+                     bool ss,
+                     int flags,
+                     cudaStream_t s);
     int groupCheck(GroupKind kind, int dtype, int op, int root, int flags, bool& grouped) const;
     int groupBatch(GroupKind kind,
                    const GroupItem* items,

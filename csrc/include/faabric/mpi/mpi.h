@@ -359,6 +359,10 @@ extern "C"
                     MPI_Datatype recvtype, int root, MPI_Comm comm, MPI_Request* request);
     int MPI_Iscatter(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
                      MPI_Datatype recvtype, int root, MPI_Comm comm, MPI_Request* request);
+    // A (datatype, op) pair no reduction takes gives MPI_ERR_OP, a root
+    // outside the communicator MPI_ERR_ARG
+    int MPI_Ireduce(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, int root,
+                    MPI_Comm comm, MPI_Request* request);
     int MPI_Free_mem(void* base);
     int MPI_Win_create(void* base, MPI_Aint size, int disp_unit, MPI_Info info, MPI_Comm comm, MPI_Win* win);
     int MPI_Win_allocate_shared(MPI_Aint size, int disp_unit, MPI_Info info, MPI_Comm comm, void* baseptr, MPI_Win* win);

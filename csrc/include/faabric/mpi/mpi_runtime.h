@@ -372,6 +372,14 @@ class MpiWorld
                 int sendCount, faabric_datatype_t* recvType, int recvCount);
     int iScatter(int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes, faabric_datatype_t* sendType,
                  int sendCount, faabric_datatype_t* recvType, int recvCount);
+    // MPI_Ireduce on the world (root: a world rank; send == recv at the root
+    // is in place; recv is not significant off the root).  A device send with
+    // a pair the device reduces joins a burst keyed by (communicator, dtype,
+    // op, root), issued as one grouped launch per staging buffer at the next
+    // wait (one device reduce at issue with grouping off); anything else
+    // completes at issue on the blocking path.
+    int iReduce(int rank, int root, const uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count,
+                faabric_op_t* op);
 
     // Symmetric-heap allocation for MPI_Alloc_mem (collective: every rank
     // must allocate the same sizes in the same order)
@@ -629,6 +637,11 @@ class MpiWorld
                  const HostPath& host);
     int nbScatter(const DeviceComm& comm, int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes,
                   const HostPath& host);
+    // `root` is a rank of `comm`'s communicator (the caller checked it);
+    // buffers as for iReduce.  `comm` is null unless the send is device
+    // memory and deviceReducible(dt, op) holds (judged once, by the caller).
+    int nbReduce(const DeviceComm& comm, int rank, int root, const uint8_t* send, uint8_t* recv,
+                 faabric_datatype_t* dt, int count, faabric_op_t* op, const HostPath& host);
     // Issues this rank thread's pending burst if it is keyed to `comm`, and
     // waits for it (before `comm` is released: MPI_Comm_free)
     void settleDeviceBurst(const DeviceComm& comm);

@@ -718,6 +718,183 @@ cudaError_t launchGroupReduceScatter(const GroupArgs& a,
     return cudaGetLastError();
 }
 
+// ----------------------------------------------------------------------------
+// Grouped reduce: one MPI_Reduce per item, all in ONE launch per rank, through
+// the staging buffers (RootedSeg in launch_api.h: the table, the chunk space
+// and the LOCAL / MOVE / UNSTAGE steps).  User buffers are any memory this
+// rank's GPU can load and store, at any alignment; the staged slices are
+// 16-byte aligned, so the reduction itself always runs on 128-bit vectors.
+// ----------------------------------------------------------------------------
+// MOVE of one chunk: every rank's slice at `sOff` (len bytes) folded in rank
+// order into `dst`; the < 16-byte tail element by element by lane 0
+template<typename VR, int NR, int UNROLL>
+__device__ __forceinline__ void groupReduceChunk(const FbCommDev& c,
+                                                 int n,
+                                                 uint64_t sOff,
+                                                 uint8_t* dst,
+                                                 uint32_t len,
+                                                 uint32_t lane)
+{
+    constexpr uint32_t CHUNK = 32u * UNROLL;
+    const uint32_t nVec = len / 16;
+    if (nVec == CHUNK) {
+        Vec16 acc[UNROLL];
+        if constexpr (NR > 0) {
+            Vec16 v[UNROLL][NR];
+#pragma unroll
+            for (int u = 0; u < UNROLL; u++) {
+#pragma unroll
+                for (int p = 0; p < NR; p++) {
+                    v[u][p] = ldVecStream(c.heap[p] + sOff + (uint64_t)(u * 32 + lane) * 16);
+                }
+            }
+#pragma unroll
+            for (int u = 0; u < UNROLL; u++) {
+                acc[u] = v[u][0];
+#pragma unroll
+                for (int p = 1; p < NR; p++) {
+                    acc[u] = VR::apply(acc[u], v[u][p]);
+                }
+            }
+        } else {
+#pragma unroll
+            for (int u = 0; u < UNROLL; u++) {
+                acc[u] = ldVecStream(c.heap[0] + sOff + (uint64_t)(u * 32 + lane) * 16);
+            }
+            for (int p = 1; p < n; p++) {
+                Vec16 v[UNROLL];
+#pragma unroll
+                for (int u = 0; u < UNROLL; u++) {
+                    v[u] = ldVecStream(c.heap[p] + sOff + (uint64_t)(u * 32 + lane) * 16);
+                }
+#pragma unroll
+                for (int u = 0; u < UNROLL; u++) {
+                    acc[u] = VR::apply(acc[u], v[u]);
+                }
+            }
+        }
+#pragma unroll
+        for (int u = 0; u < UNROLL; u++) {
+            stVec(dst + (uint64_t)(u * 32 + lane) * 16, acc[u]);
+        }
+        return;
+    }
+    // the ragged end of a piece (or a whole small one)
+#pragma unroll
+    for (int u = 0; u < UNROLL; u++) {
+        const uint32_t i = (uint32_t)u * 32 + lane;
+        if (i < nVec) {
+            Vec16 acc = ldVecStream(c.heap[0] + sOff + (uint64_t)i * 16);
+            for (int p = 1; p < n; p++) {
+                acc = VR::apply(acc, ldVecStream(c.heap[p] + sOff + (uint64_t)i * 16));
+            }
+            stVec(dst + (uint64_t)i * 16, acc);
+        }
+    }
+    if (lane == 0) {
+        // (pieces end at element boundaries: chunks are whole elements)
+        using Elem = typename VR::Elem;
+        constexpr uint32_t EB = VR::ELEM_BYTES;
+        for (uint32_t e = nVec * 16; e + EB <= len; e += EB) {
+            Elem acc = ldElemGlobal<Elem>(c.heap[0] + sOff + e);
+            for (int p = 1; p < n; p++) {
+                acc = VR::combine(acc, ldElemGlobal<Elem>(c.heap[p] + sOff + e));
+            }
+            stElemGlobal<Elem>(dst + e, acc);
+        }
+    }
+}
+
+template<typename VR, int NR>
+__global__ void __launch_bounds__(512, 1) groupReduceKernel(const GroupArgs a)
+{
+    extern __shared__ __align__(16) uint8_t sGroupRaw[];
+    constexpr int UNROLL = (NR == 8) ? 2 : (NR == 1 ? 8 : 4);
+    constexpr uint32_t CB = 32u * UNROLL * 16;
+    const FbCommDev& c = a.comm;
+    const int n = (NR > 0) ? NR : c.nranks;
+    const RootedSeg* segs = rootedLoad(a, sGroupRaw);
+    const uint32_t lane = threadIdx.x & 31;
+    const uint32_t warpsPerCta = blockDim.x >> 5;
+    const uint32_t warpStride = gridDim.x * warpsPerCta;
+    const uint32_t first = blockIdx.x * warpsPerCta + (threadIdx.x >> 5);
+    int cur = 0;
+    if (a.phase & GROUP_PHASE_LOCAL) {
+        uint8_t* const stage = c.heap[c.rank] + a.stageOff;
+        for (uint32_t ch = first; ch < a.totalChunks; ch += warpStride) {
+            const RootedChunk k = rootedChunk<UNROLL>(segs, a.nSegs, cur, ch);
+            const uint8_t* const send = reinterpret_cast<const uint8_t*>(k.sg->send) + k.off;
+            if constexpr (NR == 1) {
+                // one rank: the result is the send (nothing to do in place)
+                uint8_t* const recv = reinterpret_cast<uint8_t*>(k.sg->recv) + k.off;
+                if (recv != send) {
+                    rootedCopy<UNROLL>(recv, send, k.len, lane);
+                }
+            } else {
+                rootedCopy<UNROLL>(stage + (uint64_t)ch * CB, send, k.len, lane);
+            }
+        }
+    }
+    if constexpr (NR == 1) {
+        return;
+    }
+    BlockBarrier bar;
+    bool ok = true;
+    if (!a.noSync) {
+        bar.load(c);
+        ok = bar.sync(c);
+    }
+    // Chunk ch is staged, reduced and unstaged by the warp at position
+    // ch % warpStride of the grid on every rank: the same CTA index, which is
+    // what the per-CTA barriers order.  Its owner is (ch % warpStride +
+    // ch / warpStride) % n, which only the chunk and the grid (the same on
+    // every rank) decide: every warp of every rank owns a share of its walk,
+    // also when the walk is a single chunk long.
+    if (ok && (a.phase & GROUP_PHASE_MOVE)) {
+        uint8_t* const out = c.heap[a.root] + a.stageRecvOff;
+        int owner = (int)(first % (uint32_t)n);
+        for (uint32_t ch = first; ch < a.totalChunks; ch += warpStride, owner = owner + 1 == n ? 0 : owner + 1) {
+            if (owner != c.rank) {
+                continue;
+            }
+            const RootedChunk k = rootedChunk<UNROLL>(segs, a.nSegs, cur, ch);
+            groupReduceChunk<VR, NR, UNROLL>(c, n, a.stageOff + (uint64_t)ch * CB, out + (uint64_t)ch * CB, k.len, lane);
+        }
+    }
+    if (!a.noSync) {
+        ok = bar.sync(c) && ok;
+    }
+    if (ok && c.rank == a.root && (a.phase & GROUP_PHASE_UNSTAGE)) {
+        const uint8_t* const res = c.heap[c.rank] + a.stageRecvOff;
+        for (uint32_t ch = first; ch < a.totalChunks; ch += warpStride) {
+            const RootedChunk k = rootedChunk<UNROLL>(segs, a.nSegs, cur, ch);
+            rootedCopy<UNROLL>(reinterpret_cast<uint8_t*>(k.sg->recv) + k.off, res + (uint64_t)ch * CB, k.len, lane);
+        }
+    }
+    if (!a.noSync) {
+        bar.store(c);
+    }
+}
+
+template<typename VR>
+cudaError_t launchGroupReduce(const GroupArgs& a, int blocks, int threads, cudaStream_t stream)
+{
+    const size_t smem = (size_t)a.nSegs * sizeof(RootedSeg);
+    const int nr = a.comm.nranks;
+    if (nr == 1) {
+        groupReduceKernel<VR, 1><<<blocks, threads, smem, stream>>>(a);
+    } else if (nr == 2) {
+        groupReduceKernel<VR, 2><<<blocks, threads, smem, stream>>>(a);
+    } else if (nr == 4) {
+        groupReduceKernel<VR, 4><<<blocks, threads, smem, stream>>>(a);
+    } else if (nr == 8) {
+        groupReduceKernel<VR, 8><<<blocks, threads, smem, stream>>>(a);
+    } else {
+        groupReduceKernel<VR, 0><<<blocks, threads, smem, stream>>>(a);
+    }
+    return cudaGetLastError();
+}
+
 template<typename VR>
 cudaError_t preloadReduce()
 {
@@ -745,6 +922,11 @@ cudaError_t preloadReduce()
     FB_PRELOAD((groupReduceScatterKernel<VR, 2>))
     FB_PRELOAD((groupReduceScatterKernel<VR, 4>))
     FB_PRELOAD((groupReduceScatterKernel<VR, 8>))
+    FB_PRELOAD((groupReduceKernel<VR, 0>))
+    FB_PRELOAD((groupReduceKernel<VR, 1>))
+    FB_PRELOAD((groupReduceKernel<VR, 2>))
+    FB_PRELOAD((groupReduceKernel<VR, 4>))
+    FB_PRELOAD((groupReduceKernel<VR, 8>))
 #undef FB_PRELOAD
     return e;
 }
@@ -756,6 +938,7 @@ const ReduceLaunchers* launchersFor()
                                        &launchLL<VR>,
                                        &launchGroup<VR>,
                                        &launchGroupReduceScatter<VR>,
+                                       &launchGroupReduce<VR>,
                                        &preloadReduce<VR> };
     return &l;
 }

@@ -87,12 +87,15 @@ struct GroupArgs
     uint32_t nSegs;
     uint32_t totalChunks;
     int32_t noSync;
-    int32_t root; // grouped broadcast, gather and scatter: the root rank
-    // grouped gather and scatter only: symmetric offset of every rank's
-    // staging buffer, and which GROUP_PHASE_* steps this launch runs
+    int32_t root; // grouped broadcast, gather, scatter and reduce: the root rank
+    // rooted kinds only: symmetric offset of every rank's staging buffer,
+    // and which GROUP_PHASE_* steps this launch runs
     uint64_t stageOff;
     int32_t phase;
     int32_t pad;
+    // grouped reduce only: symmetric offset of the staging buffer the
+    // results are stored in (the root's)
+    uint64_t stageRecvOff;
 };
 
 // vectors per warp-chunk for a world of n ranks (host and kernel must agree)
@@ -148,8 +151,8 @@ cudaError_t launchGroupAllToAll(const GroupArgs& a,
                                 int threads,
                                 cudaStream_t stream);
 
-// ---- grouped gather and scatter: many MPI_Gather / MPI_Scatter calls with
-// one root, ONE launch ----
+// ---- grouped gather, scatter and reduce: many MPI_Gather / MPI_Scatter /
+// MPI_Reduce calls with one root, ONE launch ----
 // User buffers are any memory this rank's GPU can load and store, at any
 // alignment; the peers exchange through their staging buffers (GroupArgs
 // .stageOff).  The table is GroupSeg-sized RootedSeg entries, one per piece
@@ -166,8 +169,14 @@ cudaError_t launchGroupAllToAll(const GroupArgs& a,
 //            peer p's slices, and block `root` to its recv unless recv is
 //            that block (in place); exit barrier; LOCAL: every non-root
 //            copies its slices into its recv.
+//   reduce:  LOCAL: every rank copies its send into its own slices
+//            (stageOff); entry barrier; MOVE: the owner of chunk ch (one
+//            rank, the same on every rank) folds every rank's slice of ch in
+//            rank order and stores the result into the root's slice of ch at
+//            stageRecvOff; exit barrier; UNSTAGE: the root copies its result
+//            slices into its recv.  One rank: LOCAL copies send to recv.
 // With noSync the launch runs the steps of `phase` with no barrier (the host
-// runs the LOCAL and MOVE steps as two launches around stream barriers).
+// runs the steps as separate launches around stream barriers).
 struct RootedSeg
 {
     uint64_t send;   // this rank's send address at the piece (0: not given)
@@ -179,6 +188,7 @@ struct RootedSeg
 static_assert(sizeof(RootedSeg) == sizeof(GroupSeg), "rooted tables use GroupSeg slots");
 #define GROUP_PHASE_LOCAL 1
 #define GROUP_PHASE_MOVE 2
+#define GROUP_PHASE_UNSTAGE 4
 cudaError_t launchGroupGather(const GroupArgs& a, int blocks, int threads, cudaStream_t stream);
 cudaError_t launchGroupScatter(const GroupArgs& a, int blocks, int threads, cudaStream_t stream);
 
@@ -188,6 +198,7 @@ struct ReduceLaunchers
     LLLaunchFn ll;
     GroupLaunchFn group;
     GroupLaunchFn groupRs; // grouped reduce-scatter
+    GroupLaunchFn groupReduce; // grouped reduce (RootedSeg table)
     // Forces the CUDA module/function load of every variant (lazy loading may
     // otherwise synchronise the context while a peer rank's kernel is spinning
     // on this one => deadlock until the watchdog fires)

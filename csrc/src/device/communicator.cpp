@@ -1218,6 +1218,11 @@ cudaError_t cudaGroupReduceScatter(const fb::GroupArgs& a, int dtype, int op, in
     return fb::findReduceLaunchers(dtype, op)->groupRs(a, blocks, threads, s);
 }
 
+cudaError_t cudaGroupReduce(const fb::GroupArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s)
+{
+    return fb::findReduceLaunchers(dtype, op)->groupReduce(a, blocks, threads, s);
+}
+
 cudaError_t cudaCopy(void* dst, const void* src, size_t bytes, cudaStream_t s)
 {
     return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, s);
@@ -1238,6 +1243,7 @@ const fb::KernelTable CUDA_KERNELS = {
     .groupAllToAll = fb::launchGroupAllToAll,
     .groupGather = fb::launchGroupGather,
     .groupScatter = fb::launchGroupScatter,
+    .groupReduce = cudaGroupReduce,
     .move = fb::launchMove,
     .moveBulk = fb::launchMoveBulk,
     .barrier = fb::launchBarrier,
@@ -1265,6 +1271,7 @@ const fb::KernelTable HOST_KERNELS = {
     .groupAllToAll = fb::host::groupAllToAll,
     .groupGather = fb::host::groupGather,
     .groupScatter = fb::host::groupScatter,
+    .groupReduce = fb::host::groupReduce,
     .move = fb::host::moveKernel,
     .moveBulk = fb::host::moveBulk,
     .barrier = fb::host::barrierKernel,
@@ -2048,7 +2055,14 @@ static int buildShardSegs(const Communicator& c,
 // items per launch: every item yields at most one segment per rank
 static const size_t GROUP_ITEMS_PER_LAUNCH = FB_GROUP_MAX_SEGS - 8;
 
-// The next launch of a gather or scatter list from `at` on, which it
+// Gather, scatter and reduce: the kinds that stage through RootedSeg tables
+static bool rootedKind(Communicator::GroupKind kind)
+{
+    return kind == Communicator::GROUP_GATHER || kind == Communicator::GROUP_SCATTER ||
+           kind == Communicator::GROUP_REDUCE;
+}
+
+// The next launch of a gather, scatter or reduce list from `at` on, which it
 // advances: pieces of items, one RootedSeg each, while there are segment
 // slots and staging chunks left (launch_api.h).  An item larger than the
 // staging room left is cut at a chunk boundary and goes on in the next
@@ -2108,7 +2122,7 @@ int Communicator::groupBatch(GroupKind kind,
 {
     SegBuild sb;
     int rc = FB_OK;
-    if (kind == GROUP_GATHER || kind == GROUP_SCATTER) {
+    if (rootedKind(kind)) {
         buildRootedSegs(items, nItems, esize, dev_.nranks, cfg_.stageBytes, at, sb, l.missing);
     } else {
         // a window of GROUP_ITEMS_PER_LAUNCH whole items
@@ -2141,7 +2155,7 @@ std::shared_ptr<Communicator::GroupPlan> Communicator::prepareGroup(
     int& rc = rcOut ? *rcOut : rcLocal;
     rc = FB_OK;
     const size_t esize = fbDtypeSize(dtype);
-    if (esize == 0 || kind < GROUP_ALLREDUCE || kind > GROUP_SCATTER) {
+    if (esize == 0 || kind < GROUP_ALLREDUCE || kind > GROUP_REDUCE) {
         rc = FB_E_INVALID;
         return nullptr;
     }
@@ -2218,9 +2232,9 @@ int Communicator::launchGroup(const GroupLaunch& l,
     a.nSegs = l.nSegs;
     a.totalChunks = l.totalChunks;
     a.noSync = ((flags & FB_FLAG_NOSYNC) || ss || n == 1) ? 1 : 0;
-    a.root = (kind == GROUP_BROADCAST || kind == GROUP_GATHER || kind == GROUP_SCATTER) ? root : 0;
-    if (kind == GROUP_GATHER || kind == GROUP_SCATTER) {
-        return launchRooted(l, kind, a, ss, flags, s);
+    a.root = (kind == GROUP_BROADCAST || rootedKind(kind)) ? root : 0;
+    if (rootedKind(kind)) {
+        return launchRooted(l, kind, dtype, op, a, ss, flags, s);
     }
     if (ss && streamBarrier(flags, s) != FB_OK) {
         return FB_E_CUDA;
@@ -2258,35 +2272,49 @@ int Communicator::launchGroup(const GroupLaunch& l,
     return FB_OK;
 }
 
-// Whether this rank lacks a buffer of a gather or scatter list (`missing`:
-// GroupLaunch::missing over the list): every rank needs its own side, the
-// root both.  Checked before the list's first launch.
+// Whether this rank lacks a buffer of a gather, scatter or reduce list
+// (`missing`: GroupLaunch::missing over the list): every rank needs its own
+// side (the send of a gather or reduce), the root both.  Checked before the
+// list's first launch.
 static bool rootedMissing(Communicator::GroupKind kind, bool isRoot, uint32_t missing)
 {
-    const uint32_t needed = isRoot ? 3u : (kind == Communicator::GROUP_GATHER ? 1u : 2u);
+    const uint32_t needed = isRoot ? 3u : (kind == Communicator::GROUP_SCATTER ? 2u : 1u);
     return (missing & needed) != 0;
 }
 
-// A gather or scatter launch.  With stream-ordered barriers the kernel runs
-// as two launches: gather LOCAL, barrier, MOVE, barrier; scatter barrier,
-// MOVE, barrier, LOCAL.
-int Communicator::launchRooted(const GroupLaunch& l, GroupKind kind, fb::GroupArgs& a, bool ss, int flags,
-                               cudaStream_t s)
+// A gather, scatter or reduce launch.  With stream-ordered barriers the
+// kernel runs as one launch per step: gather LOCAL, barrier, MOVE, barrier;
+// scatter barrier, MOVE, barrier, LOCAL; reduce LOCAL, barrier, MOVE,
+// barrier, UNSTAGE.
+int Communicator::launchRooted(const GroupLaunch& l, GroupKind kind, int dtype, int op, fb::GroupArgs& a, bool ss,
+                               int flags, cudaStream_t s)
 {
     const bool gather = kind == GROUP_GATHER;
     a.stageOff = stageSendOff_;
+    a.stageRecvOff = stageRecvOff_;
     // no warp without a chunk (as the all-to-all)
     const uint64_t warps = (uint64_t)cfg_.threads / 32;
     const int blocks = (int)std::clamp<uint64_t>(
       (l.totalChunks + warps - 1) / warps, 1, (uint64_t)groupGrid(cfg_, dev_.nranks, l.vecsPerRank));
-    const auto launch = gather ? k_->groupGather : k_->groupScatter;
     auto run = [&](int phase) {
         a.phase = phase;
-        return launch(a, blocks, cfg_.threads, s) == cudaSuccess ? FB_OK : FB_E_CUDA;
+        const cudaError_t e = kind == GROUP_REDUCE ? k_->groupReduce(a, dtype, op, blocks, cfg_.threads, s)
+                              : gather             ? k_->groupGather(a, blocks, cfg_.threads, s)
+                                                   : k_->groupScatter(a, blocks, cfg_.threads, s);
+        return e == cudaSuccess ? FB_OK : FB_E_CUDA;
     };
     int rc;
+    int staged = 1; // launches beyond the first: staging copies
     if (!ss) {
-        rc = run(GROUP_PHASE_LOCAL | GROUP_PHASE_MOVE);
+        rc = run(GROUP_PHASE_LOCAL | GROUP_PHASE_MOVE | GROUP_PHASE_UNSTAGE);
+        staged = 0;
+    } else if (kind == GROUP_REDUCE) {
+        rc = run(GROUP_PHASE_LOCAL);
+        rc = rc == FB_OK ? streamBarrier(flags, s) : rc;
+        rc = rc == FB_OK ? run(GROUP_PHASE_MOVE) : rc;
+        rc = rc == FB_OK ? streamBarrier(flags, s) : rc;
+        rc = rc == FB_OK ? run(GROUP_PHASE_UNSTAGE) : rc;
+        staged = 2;
     } else if (gather) {
         rc = run(GROUP_PHASE_LOCAL);
         rc = rc == FB_OK ? streamBarrier(flags, s) : rc;
@@ -2301,9 +2329,8 @@ int Communicator::launchRooted(const GroupLaunch& l, GroupKind kind, fb::GroupAr
     if (rc != FB_OK) {
         return FB_E_CUDA;
     }
-    // (the second launch of a stream-ordered pair is a staging copy)
     stats_.launches++;
-    stats_.stagedCopies += ss ? 1 : 0;
+    stats_.stagedCopies += staged;
     stats_.bytes += l.bytes;
     return FB_OK;
 }
@@ -2322,7 +2349,7 @@ const GroupKindNames kGroupNames[] = {
     FB_GROUP_NAMES("allReduce", "all-reduce"), FB_GROUP_NAMES("reduceScatter", "reduce-scatter"),
     FB_GROUP_NAMES("allGather", "all-gather"), FB_GROUP_NAMES("broadcast", "broadcast"),
     FB_GROUP_NAMES("allToAll", "all-to-all"), FB_GROUP_NAMES("gather", "gather"),
-    FB_GROUP_NAMES("scatter", "scatter"),
+    FB_GROUP_NAMES("scatter", "scatter"), FB_GROUP_NAMES("reduce", "reduce"),
 };
 #undef FB_GROUP_NAMES
 
@@ -2332,7 +2359,7 @@ const int GROUP_NOTHING = 1;
 
 const char* Communicator::groupKindName(GroupKind kind)
 {
-    return kind >= GROUP_ALLREDUCE && kind <= GROUP_SCATTER ? kGroupNames[kind].name : "unknown";
+    return kind >= GROUP_ALLREDUCE && kind <= GROUP_REDUCE ? kGroupNames[kind].name : "unknown";
 }
 
 // The rules runGroup and groupMany share (see the header).  FB_OK, with
@@ -2346,13 +2373,14 @@ int Communicator::groupCheck(GroupKind kind, int dtype, int op, int root, int fl
     // all-gather, broadcast and all-to-all are byte copies: any dtype has a
     // kernel
     grouped = true;
-    if (kind == GROUP_ALLREDUCE || kind == GROUP_REDUCE_SCATTER) {
+    if (kind == GROUP_ALLREDUCE || kind == GROUP_REDUCE_SCATTER || kind == GROUP_REDUCE) {
         const fb::ReduceLaunchers* L = fb::findReduceLaunchers(dtype, op);
         if (L == nullptr) {
             return FB_E_UNSUPPORTED;
         }
-        grouped = (kind == GROUP_ALLREDUCE ? L->group : L->groupRs) != nullptr;
-    } else if (kind == GROUP_BROADCAST || kind == GROUP_GATHER || kind == GROUP_SCATTER) {
+        grouped = (kind == GROUP_ALLREDUCE ? L->group : kind == GROUP_REDUCE ? L->groupReduce : L->groupRs) != nullptr;
+    }
+    if (kind == GROUP_BROADCAST || rootedKind(kind)) {
         if (root < 0 || root >= dev_.nranks) {
             return FB_E_INVALID;
         }
@@ -2381,7 +2409,7 @@ int Communicator::runGroup(GroupKind kind, const GroupPlan& plan, int op, int ro
     if (!grouped) {
         return FB_E_UNSUPPORTED;
     }
-    if (kind == GROUP_GATHER || kind == GROUP_SCATTER) {
+    if (rootedKind(kind)) {
         uint32_t missing = 0;
         for (const auto& l : plan.launches) {
             missing |= l.missing;
@@ -2412,7 +2440,7 @@ int Communicator::groupMany(GroupKind kind,
                             int flags,
                             cudaStream_t s)
 {
-    if (kind < GROUP_ALLREDUCE || kind > GROUP_SCATTER) {
+    if (kind < GROUP_ALLREDUCE || kind > GROUP_REDUCE) {
         return FB_E_INVALID;
     }
     NvtxRange nvtxRange(kGroupNames[kind].many);
@@ -2422,7 +2450,7 @@ int Communicator::groupMany(GroupKind kind,
         return rc == GROUP_NOTHING ? FB_OK : rc;
     }
     const size_t esize = fbDtypeSize(dtype);
-    if (kind == GROUP_GATHER || kind == GROUP_SCATTER) {
+    if (rootedKind(kind)) {
         uint32_t missing = 0;
         for (size_t i = 0; i < nItems; i++) {
             if (items[i].count != 0) {

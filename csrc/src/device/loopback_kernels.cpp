@@ -703,6 +703,68 @@ cudaError_t groupScatter(const GroupArgs& a, int blocks, int, cudaStream_t)
     return groupRooted(a, blocks, false);
 }
 
+// The twin of groupReduceKernel: every rank stages its pieces; after the
+// entry barrier this rank folds the chunks it owns (the kernel's rule, with
+// the same grid) into the root's result slices; after the exit barrier the
+// root unstages
+cudaError_t groupReduce(const GroupArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t)
+{
+    const FbCommDev& c = a.comm;
+    const RootedSeg* segs = reinterpret_cast<const RootedSeg*>(a.segs);
+    const int n = c.nranks;
+    const uint64_t cb = (uint64_t)fbGroupChunkVecs(n) * 16;
+    const size_t es = fbDtypeSize(dtype);
+    auto user = [](uint64_t addr) { return reinterpret_cast<uint8_t*>(addr); };
+    if (a.phase & GROUP_PHASE_LOCAL) {
+        for (uint32_t si = 0; si < a.nSegs; si++) {
+            const RootedSeg& sg = segs[si];
+            if (n == 1) {
+                if (sg.recv != sg.send) {
+                    memcpy(user(sg.recv), user(sg.send), sg.bytes);
+                }
+            } else {
+                memcpy(c.heap[c.rank] + a.stageOff + sg.chunk0 * cb, user(sg.send), sg.bytes);
+            }
+        }
+    }
+    if (n == 1) {
+        return cudaSuccess;
+    }
+    bool ok = a.noSync || gridBarrier(c, blocks);
+    if (ok && (a.phase & GROUP_PHASE_MOVE)) {
+        const uint64_t warpStride = (uint64_t)blocks * (uint64_t)(threads / 32);
+        for (uint32_t si = 0; si < a.nSegs; si++) {
+            const RootedSeg& sg = segs[si];
+            for (uint64_t off = 0; off < sg.bytes; off += cb) {
+                const uint64_t ch = sg.chunk0 + off / cb;
+                if ((int)((ch % warpStride + ch / warpStride) % (uint64_t)n) != c.rank) {
+                    continue;
+                }
+                const uint64_t len = std::min<uint64_t>(cb, sg.bytes - off);
+                const uint64_t slice = ch * cb;
+                uint8_t* const out = c.heap[a.root] + a.stageRecvOff + slice;
+                memcpy(out, c.heap[0] + a.stageOff + slice, len);
+                for (int p = 1; p < n; p++) {
+                    const uint8_t* in = c.heap[p] + a.stageOff + slice;
+                    for (uint64_t e = 0; e + es <= len; e += es) {
+                        combineElem(dtype, op, out + e, in + e);
+                    }
+                }
+            }
+        }
+    }
+    if (!a.noSync) {
+        ok = gridBarrier(c, blocks) && ok;
+    }
+    if (ok && c.rank == a.root && (a.phase & GROUP_PHASE_UNSTAGE)) {
+        for (uint32_t si = 0; si < a.nSegs; si++) {
+            const RootedSeg& sg = segs[si];
+            memcpy(user(sg.recv), c.heap[c.rank] + a.stageRecvOff + sg.chunk0 * cb, sg.bytes);
+        }
+    }
+    return cudaSuccess;
+}
+
 // ----------------------------------------------------------------- move ----
 // The CUDA kernels copy in W-byte words.  Every address they touch that way
 // must be W-aligned (a misaligned vector access is a device fault), and every

@@ -22,6 +22,7 @@ struct KernelTable
     cudaError_t (*groupAllToAll)(const GroupArgs& a, int blocks, int threads, cudaStream_t s);
     cudaError_t (*groupGather)(const GroupArgs& a, int blocks, int threads, cudaStream_t s);
     cudaError_t (*groupScatter)(const GroupArgs& a, int blocks, int threads, cudaStream_t s);
+    cudaError_t (*groupReduce)(const GroupArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s);
     cudaError_t (*move)(const MoveArgs& a, int width, int blocks, int threads, cudaStream_t s);
     // TMA bulk-copy engine (fixed block size, 16-byte aligned ranges)
     cudaError_t (*moveBulk)(const MoveArgs& a, int blocks, cudaStream_t s);
@@ -63,6 +64,7 @@ cudaError_t groupBroadcast(const GroupArgs& a, int blocks, int threads, cudaStre
 cudaError_t groupAllToAll(const GroupArgs& a, int blocks, int threads, cudaStream_t s);
 cudaError_t groupGather(const GroupArgs& a, int blocks, int threads, cudaStream_t s);
 cudaError_t groupScatter(const GroupArgs& a, int blocks, int threads, cudaStream_t s);
+cudaError_t groupReduce(const GroupArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s);
 // The move, p2p and put twins return cudaErrorMisalignedAddress, before they
 // copy or synchronise, when an address the kernel reads or writes in words of
 // `width` bytes is not aligned to it (moveBulk: 16 bytes)

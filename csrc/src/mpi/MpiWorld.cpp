@@ -1836,6 +1836,33 @@ int MpiWorld::nbScatter(const DeviceComm& comm, int rank, int root, const uint8_
     }, host);
 }
 
+int MpiWorld::iReduce(int rank, int root, const uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count,
+                      faabric_op_t* op)
+{
+    checkRanksRange(rank, root);
+    cacheDeviceComm(rank);
+    const DeviceComm dev = count > 0 && isDevicePointer(send) && deviceReducible(dt, op) ? tls.cachedComm : nullptr;
+    return nbReduce(dev, rank, root, send, recv, dt, count, op, [&] {
+        reduce(rank, root, const_cast<uint8_t*>(send), recv, dt, count, op);
+    });
+}
+
+int MpiWorld::nbReduce(const DeviceComm& comm, int rank, int root, const uint8_t* send, uint8_t* recv,
+                       faabric_datatype_t* dt, int count, faabric_op_t* op, const HostPath& host)
+{
+    // staged like the gather: the burst's key is (communicator, dtype, op,
+    // root)
+    const size_t bytes = (size_t)count * dt->size;
+    const int fdt = fbDtypeFor(dt);
+    const int fop = fbOpFor(op);
+    NbCall call{ bytes, bytes, bytes, faabric::device::Communicator::GROUP_REDUCE, fdt, fop, root,
+                 { send, recv, (size_t)count } };
+    call.staged = true;
+    return nbCollective(comm, rank, bytes > 0, call, [&](auto& c, cudaStream_t st) {
+        return c.reduce(send, recv, (size_t)count, fdt, fop, root, 0, st);
+    }, host);
+}
+
 void MpiWorld::settleDeviceBurst(const DeviceComm& comm)
 {
     if (comm == nullptr || tls.groupItems.empty() || tls.groupComm != comm) {

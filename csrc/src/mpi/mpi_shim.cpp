@@ -1108,6 +1108,32 @@ int MPI_Iscatter(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void
                    request);
 }
 
+int MPI_Ireduce(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, int root,
+                MPI_Comm comm, MPI_Request* request)
+{
+    SPDLOG_TRACE("MPI - MPI_Ireduce all -> {}", root);
+    if (refusedReduction(op, datatype)) {
+        return MPI_ERR_OP;
+    }
+    MpiWorld& world = getExecutingWorld();
+    const int rank = executingContext.getRank();
+    auto sub = subOf(comm);
+    if (root < 0 || root >= (sub != nullptr ? sub->size() : world.getSize())) {
+        return MPI_ERR_ARG;
+    }
+    const uint8_t* send = (const uint8_t*)resolveInPlace(sendbuf, recvbuf);
+    if (sub != nullptr) {
+        auto dev = count > 0 && MpiWorld::isDevicePointer(send) && MpiWorld::deviceReducible(datatype, op)
+                     ? sub->deviceComm(world, rank)
+                     : nullptr;
+        return handOut(world.nbReduce(dev, rank, root, send, (uint8_t*)recvbuf, datatype, count, op, [&] {
+            sub->reduce(world, rank, root, send, (uint8_t*)recvbuf, datatype, count, op);
+        }),
+                       request);
+    }
+    return handOut(world.iReduce(rank, root, send, (uint8_t*)recvbuf, datatype, count, op), request);
+}
+
 int MPI_Get_processor_name(char* name, int* resultlen)
 {
     SPDLOG_TRACE("MPI - MPI_Get_processor_name");

@@ -93,6 +93,7 @@ GROUP_KINDS = {
     "all_to_all": 4,
     "gather": 5,
     "scatter": 6,
+    "reduce": 7,
 }
 ALGOS = {"auto": 0, "oneshot": 1, "twoshot": 2, "nvls": 3, "ll": 4}
 ALGO_NAMES = {v: k for k, v in ALGOS.items()}
@@ -475,18 +476,39 @@ class Communicator:
         Gather follows the all-gather rule and scatter the reduce-scatter
         rule, with a root in the communicator and contiguous tensors on this
         communicator's GPU; the root's side (gather recvs, scatter sends) may
-        be None off the root, or a list of None."""
-        if kind in ("gather", "scatter"):
+        be None off the root, or a list of None.  Reduce needs the rooted
+        rules with equal send and recv numel and element size (recvs as for
+        gather)."""
+        if kind in ("gather", "scatter", "reduce"):
             if not 0 <= int(root) < self.size:
                 raise CommError(f"{what}: root {root} outside a communicator of {self.size}")
-            if kind == "gather" and recvs is None:
+            if kind != "scatter" and recvs is None:
                 recvs = [None] * len(sends or [])
             if kind == "scatter" and sends is None:
                 sends = [None] * len(recvs or [])
         if len(sends) != len(recvs) or not sends:
             raise CommError(f"{what}: need equally long, non-empty lists")
         per = 1
-        if kind in ("gather", "scatter"):
+        if kind == "reduce":
+            rooted = self.rank == int(root)
+            for i, (s, r) in enumerate(zip(sends, recvs)):
+                for t in (s, r):
+                    if t is not None and (not t.is_cuda or t.device.index != self.device or not t.is_contiguous()):
+                        raise CommError(
+                            f"{what}: item {i} must be contiguous tensors on cuda:{self.device}, not {t.device}"
+                            f"{'' if t.is_contiguous() else ' (non-contiguous)'}"
+                        )
+                if s is None or (r is None and rooted):
+                    raise CommError(f"{what}: item {i} needs a send on every rank and a recv on the root")
+                if r is not None and (r.numel() != s.numel() or r.element_size() != s.element_size()):
+                    raise CommError(
+                        f"{what}: item {i} has {s.numel()} send and {r.numel()} recv elements of "
+                        f"{s.element_size()} and {r.element_size()} bytes; both must be equal"
+                    )
+                if r is not None and dtype is None and r.dtype != s.dtype:
+                    raise CommError(f"{what}: item {i} has a {s.dtype} send and a {r.dtype} recv")
+            typed = [self._typed(s, dtype) for s in sends]
+        elif kind in ("gather", "scatter"):
             gather = kind == "gather"
             rooted = self.rank == int(root)
             for i, (s, r) in enumerate(zip(sends, recvs)):
@@ -564,7 +586,7 @@ class Communicator:
         return plan
 
     def _launch(self, what, kind, plan, op, root, stream, channel, flags):
-        if kind in ("gather", "scatter") and int(root) != plan.root:
+        if kind in ("gather", "scatter", "reduce") and int(root) != plan.root:
             # (the root's side was checked, and on other ranks may be missing,
             # for the root the plan was prepared for)
             raise CommError(f"{what}: plan prepared for root {plan.root}, launched with root {root}")
@@ -575,7 +597,7 @@ class Communicator:
 
     def _many(self, what, kind, sends, recvs, dtype, op, root, stream, channel):
         n, sp, rp, cnt, dt = self._group_items(what, kind, sends, recvs, dtype, root)
-        f = (0 if kind in ("gather", "scatter") else self._sym(*sends)) | ((channel & 0xF) << 8)
+        f = (0 if kind in ("gather", "scatter", "reduce") else self._sym(*sends)) | ((channel & 0xF) << 8)
         fop = OPS[op] if op is not None else 0
         rc = self._lib.fb_group_many(
             self._h, GROUP_KINDS[kind], n, sp, rp, cnt, dt, fop, int(root), f, self._stream(stream)
@@ -701,6 +723,25 @@ class Communicator:
         """Transient variant of :meth:`prepare_scatter_group` +
         :meth:`scatter_group`."""
         self._many("scatter_many", "scatter", sends, recvs, dtype, None, root, stream, channel)
+
+    def prepare_reduce_group(self, sends, recvs=None, root=0, dtype=None) -> "GroupPlan":
+        """Plan the launches that reduce every pair of the lists to the root
+        given to :meth:`reduce_group` (MPI_Reduce per pair: ``recvs[i]`` on the
+        root gets the op over ``sends[i]`` of every rank, folded in rank
+        order).  Tensors are any device memory at any alignment; ``recvs`` is
+        only read on the root (None elsewhere) and no other rank's recv is
+        written.  In place (``recvs[i]`` is ``sends[i]``) is allowed.  The
+        dtype is fixed here, the op is given at launch; the plan launches with
+        this ``root`` only.  Call collectively with the same counts."""
+        return self._prepare("prepare_reduce_group", "reduce", sends, recvs, dtype, sends, root)
+
+    def reduce_group(self, plan: "GroupPlan", op="sum", root=0, stream=None, channel=0, flags=0):
+        self._launch("reduce_group", "reduce", plan, OPS[op], int(root), stream, channel, flags)
+
+    def reduce_many(self, sends, recvs=None, op="sum", root=0, stream=None, channel=0, dtype=None):
+        """Transient variant of :meth:`prepare_reduce_group` +
+        :meth:`reduce_group`."""
+        self._many("reduce_many", "reduce", sends, recvs, dtype, op, root, stream, channel)
 
     def send_recv(self, send_buf, dst, recv_buf, src, stream=None):
         rc = self._lib.fb_sendrecv(
