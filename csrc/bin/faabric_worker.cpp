@@ -30,6 +30,7 @@
 #include "../tests/mpi_subcomm_device_body.h"
 #include "../tests/mpi_group_alltoall_body.h"
 #include "../tests/mpi_group_reduce_body.h"
+#include "../tests/mpi_group_scan_body.h"
 #include "../tests/mpi_group_rooted_body.h"
 #include "../tests/mpi_group_subcomm_body.h"
 
@@ -1054,6 +1055,148 @@ static void registerFunctions()
             for (int i = 0; i < n; i++) {
                 EXPECT(back[offs[i]] == want && back[offs[i] + counts[i] - 1] == want);
             }
+            msg.set_outputdata("{\"ms_per_step\": " + std::to_string(ms) + ", \"us_per_call\": " +
+                               std::to_string(ms * 1000.0 / n) + ", \"launches_per_step\": " + std::to_string(launches) +
+                               ", \"wait_ms_per_step\": " + std::to_string(waitMs / steps) + "}");
+        }
+        MPI_Free_mem(recv);
+        MPI_Free_mem(send);
+        return 0;
+    });
+
+    // MPI_Iscan / MPI_Iexscan bursts and MPI_Exscan on the world and on
+    // sub-communicators (mpi_group_scan_body.h)
+    mpiFunction("group-scan", [](int rank, int size, faabric::Message& msg) {
+        std::string why;
+        int rc = group_scan::body(rank, size, msg.mpiworldid(), true, &why);
+        if (rc != 0) {
+            SPDLOG_ERROR("group-scan: {}", why);
+            msg.set_outputdata(why);
+        }
+        return rc;
+    });
+
+    // A list of tensors prefix-summed over the world per step, in device
+    // memory (MPI_Alloc_mem).  Input: "<mode>;<steps>;<dtype>;<count0,count1,
+    // ...>" with count_i the elements of tensor i, dtype "f32" or "i64", and
+    // mode
+    //   scan     one MPI_Scan per tensor
+    //   iscan    MPI_Iscan per tensor + MPI_Waitall
+    //   exscan   one MPI_Exscan per tensor
+    //   iexscan  MPI_Iexscan per tensor + MPI_Waitall
+    // Rank 0 reports {"ms_per_step", "us_per_call", "launches_per_step",
+    // "wait_ms_per_step"}: the launches counted on its world device
+    // communicator, and the part of a step spent in MPI_Waitall.
+    mpiFunction("bench-group-scan", [](int rank, int size, faabric::Message& msg) {
+        std::vector<std::string> f;
+        std::string cur;
+        for (char c : msg.inputdata() + ";") {
+            if (c == ';') {
+                f.push_back(cur);
+                cur.clear();
+            } else {
+                cur += c;
+            }
+        }
+        EXPECT(f.size() >= 4 && size >= 2);
+        const bool nb = f[0] == "iscan" || f[0] == "iexscan";
+        const bool ex = f[0] == "exscan" || f[0] == "iexscan";
+        const int steps = std::stoi(f[1]);
+        const bool i64 = f[2] == "i64";
+        const MPI_Datatype dt = i64 ? MPI_INT64_T : MPI_FLOAT;
+        const size_t es = i64 ? 8 : 4;
+        std::vector<size_t> counts, offs;
+        size_t total = 0;
+        for (size_t b = 0, e; b < f[3].size(); b = e + 1) {
+            e = f[3].find(',', b);
+            if (e == std::string::npos) {
+                e = f[3].size();
+            }
+            counts.push_back(std::stoull(f[3].substr(b, e - b)));
+            offs.push_back(total);
+            total += counts.back();
+        }
+        faabric::mpi::MpiWorld& world = faabric::mpi::getMpiWorldRegistry().getWorld(msg.mpiworldid());
+        uint8_t* send = nullptr;
+        uint8_t* recv = nullptr;
+        EXPECT(MPI_Alloc_mem(total * es, MPI_INFO_FAABRIC_DEVICE, &send) == MPI_SUCCESS);
+        EXPECT(MPI_Alloc_mem(total * es, MPI_INFO_FAABRIC_DEVICE, &recv) == MPI_SUCCESS);
+        // every element of rank r's send is r + 1 (copies from host memory,
+        // which wait for this rank only)
+        std::vector<uint8_t> mine(total * es);
+        for (size_t i = 0; i < total; i++) {
+            if (i64) {
+                const int64_t v = rank + 1;
+                memcpy(&mine[i * 8], &v, 8);
+            } else {
+                const float v = (float)(rank + 1);
+                memcpy(&mine[i * 4], &v, 4);
+            }
+        }
+        cudaMemcpy(send, mine.data(), total * es, cudaMemcpyHostToDevice);
+        MPI_Barrier(MPI_COMM_WORLD);
+        const int n = (int)counts.size();
+        std::vector<MPI_Request> reqs(n);
+        double waitMs = 0;
+        auto step = [&]() -> int {
+            for (int i = 0; i < n; i++) {
+                const int c = (int)counts[i];
+                uint8_t* s = send + offs[i] * es;
+                uint8_t* r = recv + offs[i] * es;
+                int rc;
+                if (nb) {
+                    rc = ex ? MPI_Iexscan(s, r, c, dt, MPI_SUM, MPI_COMM_WORLD, &reqs[i])
+                            : MPI_Iscan(s, r, c, dt, MPI_SUM, MPI_COMM_WORLD, &reqs[i]);
+                } else {
+                    rc = ex ? MPI_Exscan(s, r, c, dt, MPI_SUM, MPI_COMM_WORLD)
+                            : MPI_Scan(s, r, c, dt, MPI_SUM, MPI_COMM_WORLD);
+                }
+                EXPECT(rc == MPI_SUCCESS);
+            }
+            if (nb) {
+                auto w0 = std::chrono::steady_clock::now();
+                EXPECT(MPI_Waitall(n, reqs.data(), MPI_STATUSES_IGNORE) == MPI_SUCCESS);
+                waitMs += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - w0).count();
+            }
+            return 0;
+        };
+        for (int i = 0; i < 3; i++) {
+            EXPECT(step() == 0);
+        }
+        auto dev = world.getDeviceComm(rank);
+        EXPECT(dev != nullptr);
+        MPI_Barrier(MPI_COMM_WORLD);
+        waitMs = 0;
+        const uint64_t l0 = dev->stats().launches;
+        auto t0 = std::chrono::steady_clock::now();
+        for (int i = 0; i < steps; i++) {
+            EXPECT(step() == 0);
+        }
+        const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count() / steps;
+        const double launches = (double)(dev->stats().launches - l0) / steps;
+        MPI_Barrier(MPI_COMM_WORLD);
+        // every element of rank 1's output is 1 (exscan) or 1 + 2 (scan)
+        if (rank == 1) {
+            std::vector<uint8_t> back(total * es);
+            cudaMemcpy(back.data(), recv, total * es, cudaMemcpyDeviceToHost);
+            const double want = ex ? 1.0 : 3.0;
+            for (int i = 0; i < n; i++) {
+                for (size_t e : { offs[i], offs[i] + counts[i] - 1 }) {
+                    double got;
+                    if (i64) {
+                        int64_t v;
+                        memcpy(&v, &back[e * 8], 8);
+                        got = (double)v;
+                    } else {
+                        float v;
+                        memcpy(&v, &back[e * 4], 4);
+                        got = v;
+                    }
+                    EXPECT(got == want);
+                }
+            }
+        }
+        if (rank == 0) {
             msg.set_outputdata("{\"ms_per_step\": " + std::to_string(ms) + ", \"us_per_call\": " +
                                std::to_string(ms * 1000.0 / n) + ", \"launches_per_step\": " + std::to_string(launches) +
                                ", \"wait_ms_per_step\": " + std::to_string(waitMs / steps) + "}");

@@ -297,19 +297,25 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     //     (MPI_Reduce per item).  recv is read on the root only (null
     //     elsewhere is fine; no other rank's recv is written).  send == recv
     //     at the root is in place.
+    //   GROUP_SCAN: send and recv hold count elements on every rank; rank r's
+    //     recv gets op over the sends of ranks 0..r in rank order, acc =
+    //     send_0, acc = op(acc, send_p) for p = 1..r (MPI_Scan per item).
+    //     `root` is ignored.  send == recv is in place, on any rank.
+    //   GROUP_EXSCAN: the same fold over ranks 0..r-1 (MPI_Exscan per item).
+    //     Rank 0's recv is not written; on a one-member communicator nothing
+    //     is written or launched.
     // Shard kinds (GROUP_REDUCE_SCATTER, GROUP_ALLGATHER, GROUP_ALLTOALL)
     // group an item only if send and recv are in the symmetric heap and
     // 16-byte aligned, count*esize is a multiple of 16, and recv overlaps no
     // send of the group on this rank.  The one exception is the in-place
     // all-gather, send == recv + rank*count*esize.  Items with count 0 are
     // skipped.
-    // Rooted kinds (GROUP_GATHER, GROUP_SCATTER, GROUP_REDUCE) group every
-    // item with count > 0: buffers are any device memory of this rank, at
-    // any alignment and length, and may differ between ranks.  The data goes
-    // through every rank's staging buffers (the reduce's results through the
-    // root's second one), so a plan depends on neither the root nor the op,
-    // and a
-    // launch holds at most CommConfig::stageBytes per rank (rounded to
+    // Rooted kinds (GROUP_GATHER, GROUP_SCATTER, GROUP_REDUCE, GROUP_SCAN,
+    // GROUP_EXSCAN) group every item with count > 0: buffers are any device
+    // memory of this rank, at any alignment and length, and may differ
+    // between ranks.  The data goes through every rank's staging buffers (the
+    // reduce's and scan's results through a second one), so a plan depends
+    // on neither the root nor the op, and a launch holds at most CommConfig::stageBytes per rank (rounded to
     // chunks); a larger item is cut into pieces at the same points on every
     // rank.
     enum GroupKind
@@ -321,7 +327,9 @@ class Communicator : public std::enable_shared_from_this<Communicator>
         GROUP_ALLTOALL = 4,
         GROUP_GATHER = 5,
         GROUP_SCATTER = 6,
-        GROUP_REDUCE = 7
+        GROUP_REDUCE = 7,
+        GROUP_SCAN = 8,
+        GROUP_EXSCAN = 9
     };
     // Where the next launch of a list starts: an item, and a byte offset in
     // it (rooted kinds cut items larger than the staging buffer)
@@ -346,8 +354,9 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     // broadcast / allToAll calls and returns their errors (reduceScatter
     // refuses shards that are not a multiple of 16 bytes with
     // FB_E_UNSUPPORTED).  `op` is read by the reducing kinds (GROUP_ALLREDUCE,
-    // GROUP_REDUCE_SCATTER, GROUP_REDUCE) only, `root` by GROUP_BROADCAST and
-    // the rooted kinds only.  Both follow the same rules:
+    // GROUP_REDUCE_SCATTER, GROUP_REDUCE, GROUP_SCAN, GROUP_EXSCAN) only,
+    // `root` by GROUP_BROADCAST, GROUP_GATHER, GROUP_SCATTER and GROUP_REDUCE
+    // only.  Both follow the same rules:
     //   - a plan of another kind, an unknown kind or a dtype of no size:
     //     FB_E_INVALID
     //   - reducing kinds: a (dtype, op) pair with no reduction at all gives
@@ -370,6 +379,10 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     //     root's, so the bytes received are unspecified (the flag profiles
     //     one rank's data path only).  GROUP_REDUCE has a grouped kernel for
     //     every (dtype, op) pair that has a reduction.
+    //   - GROUP_SCAN, GROUP_EXSCAN: as the rooted kinds above, with no root
+    //     (any value is accepted), and every rank needs both its send and
+    //     its recv.  Every (dtype, op) pair that has a reduction has a grouped
+    //     kernel.
     //   - GROUP_ALLREDUCE sets lastAlgo() to FB_ALGO_TWOSHOT
     int runGroup(GroupKind kind, const GroupPlan& plan, int op, int root, int flags, cudaStream_t s);
     int groupMany(GroupKind kind,
@@ -382,7 +395,7 @@ class Communicator : public std::enable_shared_from_this<Communicator>
                   cudaStream_t s);
     static size_t groupPlanLaunches(const GroupPlan& plan);
     // "all-reduce", "reduce-scatter", "all-gather", "broadcast", "all-to-all",
-    // "gather", "scatter", "reduce"
+    // "gather", "scatter", "reduce", "scan", "exscan"
     static const char* groupKindName(GroupKind kind);
 
     // ---- point to point (per-pair FIFO; no kernel ever spins on a peer) ----

@@ -380,6 +380,14 @@ class MpiWorld
     // completes at issue on the blocking path.
     int iReduce(int rank, int root, const uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count,
                 faabric_op_t* op);
+    // MPI_Iscan, or with `exclusive` MPI_Iexscan, on the world (send == recv
+    // is in place, on any rank).  A device send with a pair the device
+    // reduces joins a burst keyed by (kind, communicator, dtype, op), issued
+    // as one grouped launch per staging buffer at the next wait (a one-item
+    // grouped launch at issue with grouping off); anything else completes at
+    // issue on the blocking path.
+    int iScan(int rank, bool exclusive, const uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count,
+              faabric_op_t* op);
 
     // Symmetric-heap allocation for MPI_Alloc_mem (collective: every rank
     // must allocate the same sizes in the same order)
@@ -404,6 +412,17 @@ class MpiWorld
               faabric_datatype_t* datatype,
               int count,
               faabric_op_t* operation);
+
+    // MPI_Exscan: rank r's recv gets op over the sends of ranks 0..r-1 in
+    // rank order; rank 0's recv is not written.  send == recv is in place.  A
+    // device send with a pair the device reduces runs one grouped device
+    // exscan; anything else the host chain.
+    void exscan(int rank,
+                const uint8_t* sendBuffer,
+                uint8_t* recvBuffer,
+                faabric_datatype_t* datatype,
+                int count,
+                faabric_op_t* operation);
 
     void allToAll(int rank,
                   uint8_t* sendBuffer,
@@ -592,6 +611,9 @@ class MpiWorld
     // false for an in-place scan (send == recv)
     bool deviceScan(const DeviceComm& comm, int rank, const uint8_t* send, uint8_t* recv,
                     faabric_datatype_t* dt, int count, faabric_op_t* op);
+    // a one-item grouped exscan (in place allowed), waited for
+    bool deviceExscan(const DeviceComm& comm, int rank, const uint8_t* send, uint8_t* recv,
+                      faabric_datatype_t* dt, int count, faabric_op_t* op);
     // send == nullptr at the root: its chunk already sits in its slot of recv
     bool deviceGather(const DeviceComm& comm, int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes);
     // recv == nullptr at the root: its chunk stays where it is in send
@@ -642,6 +664,10 @@ class MpiWorld
     // memory and deviceReducible(dt, op) holds (judged once, by the caller).
     int nbReduce(const DeviceComm& comm, int rank, int root, const uint8_t* send, uint8_t* recv,
                  faabric_datatype_t* dt, int count, faabric_op_t* op, const HostPath& host);
+    // Buffers as for iScan.  `comm` is null unless the send is device memory
+    // and deviceReducible(dt, op) holds (judged once, by the caller).
+    int nbScan(const DeviceComm& comm, int rank, bool exclusive, const uint8_t* send, uint8_t* recv,
+               faabric_datatype_t* dt, int count, faabric_op_t* op, const HostPath& host);
     // Issues this rank thread's pending burst if it is keyed to `comm`, and
     // waits for it (before `comm` is released: MPI_Comm_free)
     void settleDeviceBurst(const DeviceComm& comm);

@@ -719,49 +719,64 @@ cudaError_t launchGroupReduceScatter(const GroupArgs& a,
 }
 
 // ----------------------------------------------------------------------------
-// Grouped reduce: one MPI_Reduce per item, all in ONE launch per rank, through
-// the staging buffers (RootedSeg in launch_api.h: the table, the chunk space
-// and the LOCAL / MOVE / UNSTAGE steps).  User buffers are any memory this
-// rank's GPU can load and store, at any alignment; the staged slices are
-// 16-byte aligned, so the reduction itself always runs on 128-bit vectors.
+// Grouped reduce and scan: one MPI_Reduce, MPI_Scan or MPI_Exscan per item,
+// all in ONE launch per rank, through the staging buffers (RootedSeg in
+// launch_api.h: the table, the chunk space and the LOCAL / MOVE / UNSTAGE
+// steps).  User buffers are any memory this rank's GPU can load and store, at
+// any alignment; the staged slices are 16-byte aligned, so the reduction
+// itself always runs on 128-bit vectors.
 // ----------------------------------------------------------------------------
-// MOVE of one chunk: every rank's slice at `sOff` (len bytes) folded in rank
-// order into `dst`; the < 16-byte tail element by element by lane 0
-template<typename VR, int NR, int UNROLL>
-__device__ __forceinline__ void groupReduceChunk(const FbCommDev& c,
-                                                 int n,
-                                                 uint64_t sOff,
-                                                 uint8_t* dst,
-                                                 uint32_t len,
-                                                 uint32_t lane)
+// MOVE of one chunk: the slices at `slice` (len bytes) of the staging buffers
+// at `stageOff` of ranks 0..nFold-1 folded in rank order,
+// acc = slice_0, acc = op(acc, slice_p).  After rank p, the running value of
+// every vector goes to out.vec(p, slice + off, v), and of every element of the
+// < 16-byte tail (lane 0) to out.elem(p, slice + off, e); `off` is its byte
+// offset in the chunk.
+template<typename VR, int NR, int UNROLL, typename Out>
+__device__ __forceinline__ void groupFoldChunk(const FbCommDev& c,
+                                               int nFold,
+                                               uint64_t stageOff,
+                                               uint64_t slice,
+                                               uint32_t len,
+                                               uint32_t lane,
+                                               const Out& out)
 {
     constexpr uint32_t CHUNK = 32u * UNROLL;
+    const uint64_t sOff = stageOff + slice;
     const uint32_t nVec = len / 16;
     if (nVec == CHUNK) {
-        Vec16 acc[UNROLL];
         if constexpr (NR > 0) {
             Vec16 v[UNROLL][NR];
 #pragma unroll
             for (int u = 0; u < UNROLL; u++) {
 #pragma unroll
                 for (int p = 0; p < NR; p++) {
-                    v[u][p] = ldVecStream(c.heap[p] + sOff + (uint64_t)(u * 32 + lane) * 16);
+                    if (p < nFold) {
+                        v[u][p] = ldVecStream(c.heap[p] + sOff + (uint64_t)(u * 32 + lane) * 16);
+                    }
                 }
             }
 #pragma unroll
             for (int u = 0; u < UNROLL; u++) {
-                acc[u] = v[u][0];
+                const uint64_t off = slice + (uint64_t)(u * 32 + lane) * 16;
+                Vec16 acc = v[u][0];
+                out.vec(0, off, acc);
 #pragma unroll
                 for (int p = 1; p < NR; p++) {
-                    acc[u] = VR::apply(acc[u], v[u][p]);
+                    if (p < nFold) {
+                        acc = VR::apply(acc, v[u][p]);
+                        out.vec(p, off, acc);
+                    }
                 }
             }
         } else {
+            Vec16 acc[UNROLL];
 #pragma unroll
             for (int u = 0; u < UNROLL; u++) {
                 acc[u] = ldVecStream(c.heap[0] + sOff + (uint64_t)(u * 32 + lane) * 16);
+                out.vec(0, slice + (uint64_t)(u * 32 + lane) * 16, acc[u]);
             }
-            for (int p = 1; p < n; p++) {
+            for (int p = 1; p < nFold; p++) {
                 Vec16 v[UNROLL];
 #pragma unroll
                 for (int u = 0; u < UNROLL; u++) {
@@ -770,12 +785,9 @@ __device__ __forceinline__ void groupReduceChunk(const FbCommDev& c,
 #pragma unroll
                 for (int u = 0; u < UNROLL; u++) {
                     acc[u] = VR::apply(acc[u], v[u]);
+                    out.vec(p, slice + (uint64_t)(u * 32 + lane) * 16, acc[u]);
                 }
             }
-        }
-#pragma unroll
-        for (int u = 0; u < UNROLL; u++) {
-            stVec(dst + (uint64_t)(u * 32 + lane) * 16, acc[u]);
         }
         return;
     }
@@ -785,10 +797,11 @@ __device__ __forceinline__ void groupReduceChunk(const FbCommDev& c,
         const uint32_t i = (uint32_t)u * 32 + lane;
         if (i < nVec) {
             Vec16 acc = ldVecStream(c.heap[0] + sOff + (uint64_t)i * 16);
-            for (int p = 1; p < n; p++) {
+            out.vec(0, slice + (uint64_t)i * 16, acc);
+            for (int p = 1; p < nFold; p++) {
                 acc = VR::apply(acc, ldVecStream(c.heap[p] + sOff + (uint64_t)i * 16));
+                out.vec(p, slice + (uint64_t)i * 16, acc);
             }
-            stVec(dst + (uint64_t)i * 16, acc);
         }
     }
     if (lane == 0) {
@@ -797,11 +810,128 @@ __device__ __forceinline__ void groupReduceChunk(const FbCommDev& c,
         constexpr uint32_t EB = VR::ELEM_BYTES;
         for (uint32_t e = nVec * 16; e + EB <= len; e += EB) {
             Elem acc = ldElemGlobal<Elem>(c.heap[0] + sOff + e);
-            for (int p = 1; p < n; p++) {
+            out.elem(0, slice + e, acc);
+            for (int p = 1; p < nFold; p++) {
                 acc = VR::combine(acc, ldElemGlobal<Elem>(c.heap[p] + sOff + e));
+                out.elem(p, slice + e, acc);
             }
-            stElemGlobal<Elem>(dst + e, acc);
         }
+    }
+}
+
+// The reduce's results: the fold over every rank, into the root's slices
+struct ReduceOut
+{
+    uint8_t* dst; // the root's result staging buffer
+    int last;     // n - 1
+    __device__ __forceinline__ void vec(int p, uint64_t off, const Vec16& v) const
+    {
+        if (p == last) {
+            stVec(dst + off, v);
+        }
+    }
+    template<typename Elem>
+    __device__ __forceinline__ void elem(int p, uint64_t off, Elem v) const
+    {
+        if (p == last) {
+            stElemGlobal<Elem>(dst + off, v);
+        }
+    }
+};
+
+// The scan's results: the fold after rank p into rank p + shift's slices
+// (shift 0: inclusive, 1: exclusive; the caller folds ranks 0..n-1-shift)
+struct ScanOut
+{
+    const FbCommDev& c;
+    uint64_t stageRecvOff;
+    int shift;
+    __device__ __forceinline__ void vec(int p, uint64_t off, const Vec16& v) const
+    {
+        stVec(c.heap[p + shift] + stageRecvOff + off, v);
+    }
+    template<typename Elem>
+    __device__ __forceinline__ void elem(int p, uint64_t off, Elem v) const
+    {
+        stElemGlobal<Elem>(c.heap[p + shift] + stageRecvOff + off, v);
+    }
+};
+
+// This warp's walk of the chunk space: chunk ch is staged, folded and
+// unstaged by the warp at position ch % warpStride of the grid on every rank
+// (the same CTA index, which is what the per-CTA barriers order)
+struct GroupWalk
+{
+    uint32_t first;
+    uint32_t stride;
+    uint32_t lane;
+    __device__ __forceinline__ GroupWalk()
+      : first(blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5))
+      , stride(gridDim.x * (blockDim.x >> 5))
+      , lane(threadIdx.x & 31)
+    {}
+};
+
+// LOCAL: this warp's chunks of every send into its slices of `stage`; on one
+// rank (NR == 1) into the recv instead, nothing in place
+template<int NR, int UNROLL>
+__device__ __forceinline__ void groupStageSends(const GroupArgs& a,
+                                                const RootedSeg* segs,
+                                                const GroupWalk& w,
+                                                int& cur,
+                                                uint8_t* stage)
+{
+    constexpr uint32_t CB = 32u * UNROLL * 16;
+    for (uint32_t ch = w.first; ch < a.totalChunks; ch += w.stride) {
+        const RootedChunk k = rootedChunk<UNROLL>(segs, a.nSegs, cur, ch);
+        const uint8_t* const send = reinterpret_cast<const uint8_t*>(k.sg->send) + k.off;
+        if constexpr (NR == 1) {
+            uint8_t* const recv = reinterpret_cast<uint8_t*>(k.sg->recv) + k.off;
+            if (recv != send) {
+                rootedCopy<UNROLL>(recv, send, k.len, w.lane);
+            }
+        } else {
+            rootedCopy<UNROLL>(stage + (uint64_t)ch * CB, send, k.len, w.lane);
+        }
+    }
+}
+
+// MOVE: the chunks this rank owns, (ch % warpStride + ch / warpStride) % n,
+// which only the chunk and the grid (the same on every rank) decide: every
+// warp of every rank owns a share of its walk, also when the walk is a single
+// chunk long.  Each is folded over ranks 0..nFold-1 into `out`.
+template<typename VR, int NR, int UNROLL, typename Out>
+__device__ __forceinline__ void groupFoldOwned(const GroupArgs& a,
+                                               const RootedSeg* segs,
+                                               const GroupWalk& w,
+                                               int& cur,
+                                               int n,
+                                               int nFold,
+                                               const Out& out)
+{
+    constexpr uint32_t CB = 32u * UNROLL * 16;
+    int owner = (int)(w.first % (uint32_t)n);
+    for (uint32_t ch = w.first; ch < a.totalChunks; ch += w.stride, owner = owner + 1 == n ? 0 : owner + 1) {
+        if (owner != a.comm.rank) {
+            continue;
+        }
+        const RootedChunk k = rootedChunk<UNROLL>(segs, a.nSegs, cur, ch);
+        groupFoldChunk<VR, NR, UNROLL>(a.comm, nFold, a.stageOff, (uint64_t)ch * CB, k.len, w.lane, out);
+    }
+}
+
+// UNSTAGE: this warp's result slices of `res` into every recv
+template<int UNROLL>
+__device__ __forceinline__ void groupUnstage(const GroupArgs& a,
+                                             const RootedSeg* segs,
+                                             const GroupWalk& w,
+                                             int& cur,
+                                             const uint8_t* res)
+{
+    constexpr uint32_t CB = 32u * UNROLL * 16;
+    for (uint32_t ch = w.first; ch < a.totalChunks; ch += w.stride) {
+        const RootedChunk k = rootedChunk<UNROLL>(segs, a.nSegs, cur, ch);
+        rootedCopy<UNROLL>(reinterpret_cast<uint8_t*>(k.sg->recv) + k.off, res + (uint64_t)ch * CB, k.len, w.lane);
     }
 }
 
@@ -810,30 +940,14 @@ __global__ void __launch_bounds__(512, 1) groupReduceKernel(const GroupArgs a)
 {
     extern __shared__ __align__(16) uint8_t sGroupRaw[];
     constexpr int UNROLL = (NR == 8) ? 2 : (NR == 1 ? 8 : 4);
-    constexpr uint32_t CB = 32u * UNROLL * 16;
     const FbCommDev& c = a.comm;
     const int n = (NR > 0) ? NR : c.nranks;
     const RootedSeg* segs = rootedLoad(a, sGroupRaw);
-    const uint32_t lane = threadIdx.x & 31;
-    const uint32_t warpsPerCta = blockDim.x >> 5;
-    const uint32_t warpStride = gridDim.x * warpsPerCta;
-    const uint32_t first = blockIdx.x * warpsPerCta + (threadIdx.x >> 5);
+    const GroupWalk w;
     int cur = 0;
     if (a.phase & GROUP_PHASE_LOCAL) {
-        uint8_t* const stage = c.heap[c.rank] + a.stageOff;
-        for (uint32_t ch = first; ch < a.totalChunks; ch += warpStride) {
-            const RootedChunk k = rootedChunk<UNROLL>(segs, a.nSegs, cur, ch);
-            const uint8_t* const send = reinterpret_cast<const uint8_t*>(k.sg->send) + k.off;
-            if constexpr (NR == 1) {
-                // one rank: the result is the send (nothing to do in place)
-                uint8_t* const recv = reinterpret_cast<uint8_t*>(k.sg->recv) + k.off;
-                if (recv != send) {
-                    rootedCopy<UNROLL>(recv, send, k.len, lane);
-                }
-            } else {
-                rootedCopy<UNROLL>(stage + (uint64_t)ch * CB, send, k.len, lane);
-            }
-        }
+        // (one rank: the result is the send)
+        groupStageSends<NR, UNROLL>(a, segs, w, cur, c.heap[c.rank] + a.stageOff);
     }
     if constexpr (NR == 1) {
         return;
@@ -844,32 +958,57 @@ __global__ void __launch_bounds__(512, 1) groupReduceKernel(const GroupArgs a)
         bar.load(c);
         ok = bar.sync(c);
     }
-    // Chunk ch is staged, reduced and unstaged by the warp at position
-    // ch % warpStride of the grid on every rank: the same CTA index, which is
-    // what the per-CTA barriers order.  Its owner is (ch % warpStride +
-    // ch / warpStride) % n, which only the chunk and the grid (the same on
-    // every rank) decide: every warp of every rank owns a share of its walk,
-    // also when the walk is a single chunk long.
     if (ok && (a.phase & GROUP_PHASE_MOVE)) {
-        uint8_t* const out = c.heap[a.root] + a.stageRecvOff;
-        int owner = (int)(first % (uint32_t)n);
-        for (uint32_t ch = first; ch < a.totalChunks; ch += warpStride, owner = owner + 1 == n ? 0 : owner + 1) {
-            if (owner != c.rank) {
-                continue;
-            }
-            const RootedChunk k = rootedChunk<UNROLL>(segs, a.nSegs, cur, ch);
-            groupReduceChunk<VR, NR, UNROLL>(c, n, a.stageOff + (uint64_t)ch * CB, out + (uint64_t)ch * CB, k.len, lane);
-        }
+        groupFoldOwned<VR, NR, UNROLL>(a, segs, w, cur, n, n, ReduceOut{ c.heap[a.root] + a.stageRecvOff, n - 1 });
     }
     if (!a.noSync) {
         ok = bar.sync(c) && ok;
     }
     if (ok && c.rank == a.root && (a.phase & GROUP_PHASE_UNSTAGE)) {
-        const uint8_t* const res = c.heap[c.rank] + a.stageRecvOff;
-        for (uint32_t ch = first; ch < a.totalChunks; ch += warpStride) {
-            const RootedChunk k = rootedChunk<UNROLL>(segs, a.nSegs, cur, ch);
-            rootedCopy<UNROLL>(reinterpret_cast<uint8_t*>(k.sg->recv) + k.off, res + (uint64_t)ch * CB, k.len, lane);
-        }
+        groupUnstage<UNROLL>(a, segs, w, cur, c.heap[c.rank] + a.stageRecvOff);
+    }
+    if (!a.noSync) {
+        bar.store(c);
+    }
+}
+
+// The scan's steps (a.exclusive: 0 scan, 1 exscan): LOCAL as the reduce's,
+// but an exscan's last rank stages nothing (no rank reads its send); MOVE
+// folds ranks 0..n-1-exclusive and stores the value after rank p into rank
+// p + exclusive's result slices; UNSTAGE on every rank but an exscan's rank
+// 0, whose recv is never written.  One rank: a scan copies send to recv, an
+// exscan does nothing.
+template<typename VR, int NR>
+__global__ void __launch_bounds__(512, 1) groupScanKernel(const GroupArgs a)
+{
+    extern __shared__ __align__(16) uint8_t sGroupRaw[];
+    constexpr int UNROLL = (NR == 8) ? 2 : (NR == 1 ? 8 : 4);
+    const FbCommDev& c = a.comm;
+    const int n = (NR > 0) ? NR : c.nranks;
+    const int ex = a.exclusive;
+    const RootedSeg* segs = rootedLoad(a, sGroupRaw);
+    const GroupWalk w;
+    int cur = 0;
+    if ((a.phase & GROUP_PHASE_LOCAL) && !(ex && c.rank == n - 1)) {
+        groupStageSends<NR, UNROLL>(a, segs, w, cur, c.heap[c.rank] + a.stageOff);
+    }
+    if constexpr (NR == 1) {
+        return;
+    }
+    BlockBarrier bar;
+    bool ok = true;
+    if (!a.noSync) {
+        bar.load(c);
+        ok = bar.sync(c);
+    }
+    if (ok && (a.phase & GROUP_PHASE_MOVE)) {
+        groupFoldOwned<VR, NR, UNROLL>(a, segs, w, cur, n, n - ex, ScanOut{ c, a.stageRecvOff, ex });
+    }
+    if (!a.noSync) {
+        ok = bar.sync(c) && ok;
+    }
+    if (ok && !(ex && c.rank == 0) && (a.phase & GROUP_PHASE_UNSTAGE)) {
+        groupUnstage<UNROLL>(a, segs, w, cur, c.heap[c.rank] + a.stageRecvOff);
     }
     if (!a.noSync) {
         bar.store(c);
@@ -891,6 +1030,25 @@ cudaError_t launchGroupReduce(const GroupArgs& a, int blocks, int threads, cudaS
         groupReduceKernel<VR, 8><<<blocks, threads, smem, stream>>>(a);
     } else {
         groupReduceKernel<VR, 0><<<blocks, threads, smem, stream>>>(a);
+    }
+    return cudaGetLastError();
+}
+
+template<typename VR>
+cudaError_t launchGroupScan(const GroupArgs& a, int blocks, int threads, cudaStream_t stream)
+{
+    const size_t smem = (size_t)a.nSegs * sizeof(RootedSeg);
+    const int nr = a.comm.nranks;
+    if (nr == 1) {
+        groupScanKernel<VR, 1><<<blocks, threads, smem, stream>>>(a);
+    } else if (nr == 2) {
+        groupScanKernel<VR, 2><<<blocks, threads, smem, stream>>>(a);
+    } else if (nr == 4) {
+        groupScanKernel<VR, 4><<<blocks, threads, smem, stream>>>(a);
+    } else if (nr == 8) {
+        groupScanKernel<VR, 8><<<blocks, threads, smem, stream>>>(a);
+    } else {
+        groupScanKernel<VR, 0><<<blocks, threads, smem, stream>>>(a);
     }
     return cudaGetLastError();
 }
@@ -927,6 +1085,11 @@ cudaError_t preloadReduce()
     FB_PRELOAD((groupReduceKernel<VR, 2>))
     FB_PRELOAD((groupReduceKernel<VR, 4>))
     FB_PRELOAD((groupReduceKernel<VR, 8>))
+    FB_PRELOAD((groupScanKernel<VR, 0>))
+    FB_PRELOAD((groupScanKernel<VR, 1>))
+    FB_PRELOAD((groupScanKernel<VR, 2>))
+    FB_PRELOAD((groupScanKernel<VR, 4>))
+    FB_PRELOAD((groupScanKernel<VR, 8>))
 #undef FB_PRELOAD
     return e;
 }
@@ -939,6 +1102,7 @@ const ReduceLaunchers* launchersFor()
                                        &launchGroup<VR>,
                                        &launchGroupReduceScatter<VR>,
                                        &launchGroupReduce<VR>,
+                                       &launchGroupScan<VR>,
                                        &preloadReduce<VR> };
     return &l;
 }

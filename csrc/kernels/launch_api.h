@@ -92,9 +92,9 @@ struct GroupArgs
     // and which GROUP_PHASE_* steps this launch runs
     uint64_t stageOff;
     int32_t phase;
-    int32_t pad;
-    // grouped reduce only: symmetric offset of the staging buffer the
-    // results are stored in (the root's)
+    int32_t exclusive; // grouped scan only: 1 for an exscan
+    // grouped reduce and scan only: symmetric offset of the staging buffer
+    // the results are stored in (the root's, or every rank's own)
     uint64_t stageRecvOff;
 };
 
@@ -151,8 +151,9 @@ cudaError_t launchGroupAllToAll(const GroupArgs& a,
                                 int threads,
                                 cudaStream_t stream);
 
-// ---- grouped gather, scatter and reduce: many MPI_Gather / MPI_Scatter /
-// MPI_Reduce calls with one root, ONE launch ----
+// ---- grouped gather, scatter, reduce and scan: many MPI_Gather /
+// MPI_Scatter / MPI_Reduce calls with one root, or MPI_Scan / MPI_Exscan
+// calls, ONE launch ----
 // User buffers are any memory this rank's GPU can load and store, at any
 // alignment; the peers exchange through their staging buffers (GroupArgs
 // .stageOff).  The table is GroupSeg-sized RootedSeg entries, one per piece
@@ -175,6 +176,12 @@ cudaError_t launchGroupAllToAll(const GroupArgs& a,
 //            rank order and stores the result into the root's slice of ch at
 //            stageRecvOff; exit barrier; UNSTAGE: the root copies its result
 //            slices into its recv.  One rank: LOCAL copies send to recv.
+//   scan:    as the reduce, but MOVE stores the running fold after rank p
+//            into rank p's slice of ch at stageRecvOff (exscan, GroupArgs
+//            .exclusive: rank p+1's, for p <= n-2, and rank n-1's send is
+//            neither staged nor read); UNSTAGE on every rank (exscan: not
+//            rank 0, whose recv is never written).  One rank: a scan's LOCAL
+//            copies send to recv, an exscan does nothing.
 // With noSync the launch runs the steps of `phase` with no barrier (the host
 // runs the steps as separate launches around stream barriers).
 struct RootedSeg
@@ -199,6 +206,7 @@ struct ReduceLaunchers
     GroupLaunchFn group;
     GroupLaunchFn groupRs; // grouped reduce-scatter
     GroupLaunchFn groupReduce; // grouped reduce (RootedSeg table)
+    GroupLaunchFn groupScan;   // grouped scan and exscan (RootedSeg table)
     // Forces the CUDA module/function load of every variant (lazy loading may
     // otherwise synchronise the context while a peer rank's kernel is spinning
     // on this one => deadlock until the watchdog fires)

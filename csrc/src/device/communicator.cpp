@@ -1223,6 +1223,11 @@ cudaError_t cudaGroupReduce(const fb::GroupArgs& a, int dtype, int op, int block
     return fb::findReduceLaunchers(dtype, op)->groupReduce(a, blocks, threads, s);
 }
 
+cudaError_t cudaGroupScan(const fb::GroupArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s)
+{
+    return fb::findReduceLaunchers(dtype, op)->groupScan(a, blocks, threads, s);
+}
+
 cudaError_t cudaCopy(void* dst, const void* src, size_t bytes, cudaStream_t s)
 {
     return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, s);
@@ -1244,6 +1249,7 @@ const fb::KernelTable CUDA_KERNELS = {
     .groupGather = fb::launchGroupGather,
     .groupScatter = fb::launchGroupScatter,
     .groupReduce = cudaGroupReduce,
+    .groupScan = cudaGroupScan,
     .move = fb::launchMove,
     .moveBulk = fb::launchMoveBulk,
     .barrier = fb::launchBarrier,
@@ -1272,6 +1278,7 @@ const fb::KernelTable HOST_KERNELS = {
     .groupGather = fb::host::groupGather,
     .groupScatter = fb::host::groupScatter,
     .groupReduce = fb::host::groupReduce,
+    .groupScan = fb::host::groupScan,
     .move = fb::host::moveKernel,
     .moveBulk = fb::host::moveBulk,
     .barrier = fb::host::barrierKernel,
@@ -2055,14 +2062,20 @@ static int buildShardSegs(const Communicator& c,
 // items per launch: every item yields at most one segment per rank
 static const size_t GROUP_ITEMS_PER_LAUNCH = FB_GROUP_MAX_SEGS - 8;
 
-// Gather, scatter and reduce: the kinds that stage through RootedSeg tables
+// Gather, scatter, reduce, scan and exscan: the kinds that stage through
+// RootedSeg tables
+static bool scanKind(Communicator::GroupKind kind)
+{
+    return kind == Communicator::GROUP_SCAN || kind == Communicator::GROUP_EXSCAN;
+}
+
 static bool rootedKind(Communicator::GroupKind kind)
 {
     return kind == Communicator::GROUP_GATHER || kind == Communicator::GROUP_SCATTER ||
-           kind == Communicator::GROUP_REDUCE;
+           kind == Communicator::GROUP_REDUCE || scanKind(kind);
 }
 
-// The next launch of a gather, scatter or reduce list from `at` on, which it
+// The next launch of a rooted list from `at` on, which it
 // advances: pieces of items, one RootedSeg each, while there are segment
 // slots and staging chunks left (launch_api.h).  An item larger than the
 // staging room left is cut at a chunk boundary and goes on in the next
@@ -2155,7 +2168,7 @@ std::shared_ptr<Communicator::GroupPlan> Communicator::prepareGroup(
     int& rc = rcOut ? *rcOut : rcLocal;
     rc = FB_OK;
     const size_t esize = fbDtypeSize(dtype);
-    if (esize == 0 || kind < GROUP_ALLREDUCE || kind > GROUP_REDUCE) {
+    if (esize == 0 || kind < GROUP_ALLREDUCE || kind > GROUP_EXSCAN) {
         rc = FB_E_INVALID;
         return nullptr;
     }
@@ -2232,7 +2245,8 @@ int Communicator::launchGroup(const GroupLaunch& l,
     a.nSegs = l.nSegs;
     a.totalChunks = l.totalChunks;
     a.noSync = ((flags & FB_FLAG_NOSYNC) || ss || n == 1) ? 1 : 0;
-    a.root = (kind == GROUP_BROADCAST || rootedKind(kind)) ? root : 0;
+    a.root = (kind == GROUP_BROADCAST || (rootedKind(kind) && !scanKind(kind))) ? root : 0;
+    a.exclusive = kind == GROUP_EXSCAN ? 1 : 0;
     if (rootedKind(kind)) {
         return launchRooted(l, kind, dtype, op, a, ss, flags, s);
     }
@@ -2272,24 +2286,28 @@ int Communicator::launchGroup(const GroupLaunch& l,
     return FB_OK;
 }
 
-// Whether this rank lacks a buffer of a gather, scatter or reduce list
-// (`missing`: GroupLaunch::missing over the list): every rank needs its own
-// side (the send of a gather or reduce), the root both.  Checked before the
-// list's first launch.
+// Whether this rank lacks a buffer of a rooted list (`missing`:
+// GroupLaunch::missing over the list): every rank needs its own side (the
+// send of a gather or reduce), the root both, and every rank of a scan or
+// exscan both.  Checked before the list's first launch.
 static bool rootedMissing(Communicator::GroupKind kind, bool isRoot, uint32_t missing)
 {
-    const uint32_t needed = isRoot ? 3u : (kind == Communicator::GROUP_SCATTER ? 2u : 1u);
+    const uint32_t needed = isRoot || scanKind(kind) ? 3u : (kind == Communicator::GROUP_SCATTER ? 2u : 1u);
     return (missing & needed) != 0;
 }
 
-// A gather, scatter or reduce launch.  With stream-ordered barriers the
-// kernel runs as one launch per step: gather LOCAL, barrier, MOVE, barrier;
-// scatter barrier, MOVE, barrier, LOCAL; reduce LOCAL, barrier, MOVE,
-// barrier, UNSTAGE.
+// A rooted launch.  With stream-ordered barriers the kernel runs as one
+// launch per step: gather LOCAL, barrier, MOVE, barrier; scatter barrier,
+// MOVE, barrier, LOCAL; reduce, scan and exscan LOCAL, barrier, MOVE,
+// barrier, UNSTAGE.  A one-member exscan writes nothing: no launch.
 int Communicator::launchRooted(const GroupLaunch& l, GroupKind kind, int dtype, int op, fb::GroupArgs& a, bool ss,
                                int flags, cudaStream_t s)
 {
     const bool gather = kind == GROUP_GATHER;
+    const bool folds = kind == GROUP_REDUCE || scanKind(kind);
+    if (kind == GROUP_EXSCAN && dev_.nranks == 1) {
+        return FB_OK;
+    }
     a.stageOff = stageSendOff_;
     a.stageRecvOff = stageRecvOff_;
     // no warp without a chunk (as the all-to-all)
@@ -2299,6 +2317,7 @@ int Communicator::launchRooted(const GroupLaunch& l, GroupKind kind, int dtype, 
     auto run = [&](int phase) {
         a.phase = phase;
         const cudaError_t e = kind == GROUP_REDUCE ? k_->groupReduce(a, dtype, op, blocks, cfg_.threads, s)
+                              : scanKind(kind)     ? k_->groupScan(a, dtype, op, blocks, cfg_.threads, s)
                               : gather             ? k_->groupGather(a, blocks, cfg_.threads, s)
                                                    : k_->groupScatter(a, blocks, cfg_.threads, s);
         return e == cudaSuccess ? FB_OK : FB_E_CUDA;
@@ -2308,7 +2327,7 @@ int Communicator::launchRooted(const GroupLaunch& l, GroupKind kind, int dtype, 
     if (!ss) {
         rc = run(GROUP_PHASE_LOCAL | GROUP_PHASE_MOVE | GROUP_PHASE_UNSTAGE);
         staged = 0;
-    } else if (kind == GROUP_REDUCE) {
+    } else if (folds) {
         rc = run(GROUP_PHASE_LOCAL);
         rc = rc == FB_OK ? streamBarrier(flags, s) : rc;
         rc = rc == FB_OK ? run(GROUP_PHASE_MOVE) : rc;
@@ -2350,6 +2369,7 @@ const GroupKindNames kGroupNames[] = {
     FB_GROUP_NAMES("allGather", "all-gather"), FB_GROUP_NAMES("broadcast", "broadcast"),
     FB_GROUP_NAMES("allToAll", "all-to-all"), FB_GROUP_NAMES("gather", "gather"),
     FB_GROUP_NAMES("scatter", "scatter"), FB_GROUP_NAMES("reduce", "reduce"),
+    FB_GROUP_NAMES("scan", "scan"), FB_GROUP_NAMES("exscan", "exscan"),
 };
 #undef FB_GROUP_NAMES
 
@@ -2359,7 +2379,7 @@ const int GROUP_NOTHING = 1;
 
 const char* Communicator::groupKindName(GroupKind kind)
 {
-    return kind >= GROUP_ALLREDUCE && kind <= GROUP_REDUCE ? kGroupNames[kind].name : "unknown";
+    return kind >= GROUP_ALLREDUCE && kind <= GROUP_EXSCAN ? kGroupNames[kind].name : "unknown";
 }
 
 // The rules runGroup and groupMany share (see the header).  FB_OK, with
@@ -2373,15 +2393,18 @@ int Communicator::groupCheck(GroupKind kind, int dtype, int op, int root, int fl
     // all-gather, broadcast and all-to-all are byte copies: any dtype has a
     // kernel
     grouped = true;
-    if (kind == GROUP_ALLREDUCE || kind == GROUP_REDUCE_SCATTER || kind == GROUP_REDUCE) {
+    if (kind == GROUP_ALLREDUCE || kind == GROUP_REDUCE_SCATTER || kind == GROUP_REDUCE || scanKind(kind)) {
         const fb::ReduceLaunchers* L = fb::findReduceLaunchers(dtype, op);
         if (L == nullptr) {
             return FB_E_UNSUPPORTED;
         }
-        grouped = (kind == GROUP_ALLREDUCE ? L->group : kind == GROUP_REDUCE ? L->groupReduce : L->groupRs) != nullptr;
+        grouped = (kind == GROUP_ALLREDUCE  ? L->group
+                   : kind == GROUP_REDUCE   ? L->groupReduce
+                   : scanKind(kind)         ? L->groupScan
+                                            : L->groupRs) != nullptr;
     }
     if (kind == GROUP_BROADCAST || rootedKind(kind)) {
-        if (root < 0 || root >= dev_.nranks) {
+        if (!scanKind(kind) && (root < 0 || root >= dev_.nranks)) {
             return FB_E_INVALID;
         }
         if (kind == GROUP_BROADCAST && dev_.nranks == 1) {
@@ -2440,7 +2463,7 @@ int Communicator::groupMany(GroupKind kind,
                             int flags,
                             cudaStream_t s)
 {
-    if (kind < GROUP_ALLREDUCE || kind > GROUP_REDUCE) {
+    if (kind < GROUP_ALLREDUCE || kind > GROUP_EXSCAN) {
         return FB_E_INVALID;
     }
     NvtxRange nvtxRange(kGroupNames[kind].many);

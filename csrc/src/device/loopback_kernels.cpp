@@ -22,6 +22,7 @@
 #include <cstring>
 #include <mutex>
 #include <thread>
+#include <vector>
 
 namespace fb::host {
 
@@ -757,6 +758,73 @@ cudaError_t groupReduce(const GroupArgs& a, int dtype, int op, int blocks, int t
         ok = gridBarrier(c, blocks) && ok;
     }
     if (ok && c.rank == a.root && (a.phase & GROUP_PHASE_UNSTAGE)) {
+        for (uint32_t si = 0; si < a.nSegs; si++) {
+            const RootedSeg& sg = segs[si];
+            memcpy(user(sg.recv), c.heap[c.rank] + a.stageRecvOff + sg.chunk0 * cb, sg.bytes);
+        }
+    }
+    return cudaSuccess;
+}
+
+// The twin of groupScanKernel (a.exclusive: exscan): every rank stages its
+// pieces (an exscan's last rank does not); after the entry barrier this rank
+// folds the chunks it owns in rank order and stores the value after rank p
+// into rank p + exclusive's result slices; after the exit barrier every rank
+// unstages (an exscan's rank 0 does not)
+cudaError_t groupScan(const GroupArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t)
+{
+    const FbCommDev& c = a.comm;
+    const RootedSeg* segs = reinterpret_cast<const RootedSeg*>(a.segs);
+    const int n = c.nranks;
+    const int ex = a.exclusive;
+    const uint64_t cb = (uint64_t)fbGroupChunkVecs(n) * 16;
+    const size_t es = fbDtypeSize(dtype);
+    auto user = [](uint64_t addr) { return reinterpret_cast<uint8_t*>(addr); };
+    if ((a.phase & GROUP_PHASE_LOCAL) && !(ex && c.rank == n - 1)) {
+        for (uint32_t si = 0; si < a.nSegs; si++) {
+            const RootedSeg& sg = segs[si];
+            if (n == 1) {
+                if (sg.recv != sg.send) {
+                    memcpy(user(sg.recv), user(sg.send), sg.bytes);
+                }
+            } else {
+                memcpy(c.heap[c.rank] + a.stageOff + sg.chunk0 * cb, user(sg.send), sg.bytes);
+            }
+        }
+    }
+    if (n == 1) {
+        return cudaSuccess;
+    }
+    bool ok = a.noSync || gridBarrier(c, blocks);
+    if (ok && (a.phase & GROUP_PHASE_MOVE)) {
+        const uint64_t warpStride = (uint64_t)blocks * (uint64_t)(threads / 32);
+        std::vector<uint8_t> acc(cb);
+        for (uint32_t si = 0; si < a.nSegs; si++) {
+            const RootedSeg& sg = segs[si];
+            for (uint64_t off = 0; off < sg.bytes; off += cb) {
+                const uint64_t ch = sg.chunk0 + off / cb;
+                if ((int)((ch % warpStride + ch / warpStride) % (uint64_t)n) != c.rank) {
+                    continue;
+                }
+                const uint64_t len = std::min<uint64_t>(cb, sg.bytes - off);
+                const uint64_t slice = ch * cb;
+                memcpy(acc.data(), c.heap[0] + a.stageOff + slice, len);
+                for (int p = 0; p + ex < n; p++) {
+                    if (p > 0) {
+                        const uint8_t* in = c.heap[p] + a.stageOff + slice;
+                        for (uint64_t e = 0; e + es <= len; e += es) {
+                            combineElem(dtype, op, acc.data() + e, in + e);
+                        }
+                    }
+                    memcpy(c.heap[p + ex] + a.stageRecvOff + slice, acc.data(), len);
+                }
+            }
+        }
+    }
+    if (!a.noSync) {
+        ok = gridBarrier(c, blocks) && ok;
+    }
+    if (ok && !(ex && c.rank == 0) && (a.phase & GROUP_PHASE_UNSTAGE)) {
         for (uint32_t si = 0; si < a.nSegs; si++) {
             const RootedSeg& sg = segs[si];
             memcpy(user(sg.recv), c.heap[c.rank] + a.stageRecvOff + sg.chunk0 * cb, sg.bytes);

@@ -23,6 +23,7 @@ struct KernelTable
     cudaError_t (*groupGather)(const GroupArgs& a, int blocks, int threads, cudaStream_t s);
     cudaError_t (*groupScatter)(const GroupArgs& a, int blocks, int threads, cudaStream_t s);
     cudaError_t (*groupReduce)(const GroupArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s);
+    cudaError_t (*groupScan)(const GroupArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s);
     cudaError_t (*move)(const MoveArgs& a, int width, int blocks, int threads, cudaStream_t s);
     // TMA bulk-copy engine (fixed block size, 16-byte aligned ranges)
     cudaError_t (*moveBulk)(const MoveArgs& a, int blocks, cudaStream_t s);
@@ -65,6 +66,7 @@ cudaError_t groupAllToAll(const GroupArgs& a, int blocks, int threads, cudaStrea
 cudaError_t groupGather(const GroupArgs& a, int blocks, int threads, cudaStream_t s);
 cudaError_t groupScatter(const GroupArgs& a, int blocks, int threads, cudaStream_t s);
 cudaError_t groupReduce(const GroupArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s);
+cudaError_t groupScan(const GroupArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s);
 // The move, p2p and put twins return cudaErrorMisalignedAddress, before they
 // copy or synchronise, when an address the kernel reads or writes in words of
 // `width` bytes is not aligned to it (moveBulk: 16 bytes)

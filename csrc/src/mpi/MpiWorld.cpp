@@ -1408,6 +1408,25 @@ bool MpiWorld::deviceScan(const DeviceComm& comm,
     });
 }
 
+bool MpiWorld::deviceExscan(const DeviceComm& comm,
+                            int rank,
+                            const uint8_t* send,
+                            uint8_t* recv,
+                            faabric_datatype_t* dt,
+                            int count,
+                            faabric_op_t* op)
+{
+    const int fdt = fbDtypeFor(dt);
+    const int fop = fbOpFor(op);
+    if (fdt < 0 || fop < 0) {
+        return false;
+    }
+    const faabric::device::Communicator::GroupItem item{ send, recv, (size_t)count };
+    return issueAndWait(comm, streamForRank(rank), deviceCollectives, [&](auto& c, cudaStream_t s) {
+        return c.groupMany(faabric::device::Communicator::GROUP_EXSCAN, &item, 1, fdt, fop, 0, 0, s);
+    });
+}
+
 bool MpiWorld::deviceGather(const DeviceComm& comm, int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes)
 {
     // The device-or-host choice must come out the same on every rank, and only
@@ -1860,6 +1879,40 @@ int MpiWorld::nbReduce(const DeviceComm& comm, int rank, int root, const uint8_t
     call.staged = true;
     return nbCollective(comm, rank, bytes > 0, call, [&](auto& c, cudaStream_t st) {
         return c.reduce(send, recv, (size_t)count, fdt, fop, root, 0, st);
+    }, host);
+}
+
+int MpiWorld::iScan(int rank, bool exclusive, const uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count,
+                    faabric_op_t* op)
+{
+    checkRanksRange(0, rank);
+    cacheDeviceComm(rank);
+    const DeviceComm dev = count > 0 && isDevicePointer(send) && deviceReducible(dt, op) ? tls.cachedComm : nullptr;
+    return nbScan(dev, rank, exclusive, send, recv, dt, count, op, [&] {
+        if (exclusive) {
+            exscan(rank, send, recv, dt, count, op);
+        } else {
+            scan(rank, const_cast<uint8_t*>(send), recv, dt, count, op);
+        }
+    });
+}
+
+int MpiWorld::nbScan(const DeviceComm& comm, int rank, bool exclusive, const uint8_t* send, uint8_t* recv,
+                     faabric_datatype_t* dt, int count, faabric_op_t* op, const HostPath& host)
+{
+    // staged like the reduce: the burst's key is (kind, communicator, dtype,
+    // op), and in place is each rank's own affair.  At issue (grouping off)
+    // the call is a one-item grouped launch too: the blocking device scan
+    // refuses in place.
+    const size_t bytes = (size_t)count * dt->size;
+    const int fdt = fbDtypeFor(dt);
+    const int fop = fbOpFor(op);
+    const auto kind =
+      exclusive ? faabric::device::Communicator::GROUP_EXSCAN : faabric::device::Communicator::GROUP_SCAN;
+    NbCall call{ bytes, bytes, bytes, kind, fdt, fop, 0, { send, recv, (size_t)count } };
+    call.staged = true;
+    return nbCollective(comm, rank, bytes > 0, call, [&](auto& c, cudaStream_t st) {
+        return c.groupMany(kind, &call.item, 1, fdt, fop, 0, 0, st);
     }, host);
 }
 
@@ -2693,6 +2746,39 @@ void MpiWorld::scan(int rank,
     }
     if (rank < size - 1) {
         send(rank, rank + 1, recvBuffer, datatype, count, MpiMessageType::SCAN);
+    }
+}
+
+void MpiWorld::exscan(int rank,
+                      const uint8_t* sendBuffer,
+                      uint8_t* recvBuffer,
+                      faabric_datatype_t* datatype,
+                      int count,
+                      faabric_op_t* operation)
+{
+    checkRanksRange(0, rank);
+    const size_t bytes = (size_t)count * datatype->size;
+    // (judged on the send alone, alike on every rank: in place is the
+    // grouped kernel's local matter)
+    if (bytes > 0 && isDevicePointer(sendBuffer) && deviceReducible(datatype, operation) &&
+        deviceExscan(getDeviceComm(rank), rank, sendBuffer, recvBuffer, datatype, count, operation)) {
+        return;
+    }
+    // Linear chain r-1 -> r: rank r receives prefix_{r-1} and passes on
+    // op(prefix_{r-1}, send_r), computed before an in-place recv is
+    // overwritten
+    std::vector<uint8_t> acc(bytes);
+    std::vector<uint8_t> prev(bytes);
+    copyBytes(acc.data(), sendBuffer, bytes);
+    if (rank > 0) {
+        recv(rank - 1, rank, prev.data(), datatype, count, nullptr, MpiMessageType::SCAN);
+        op_reduce(operation, datatype, count, prev.data(), acc.data());
+    }
+    if (rank < size - 1) {
+        send(rank, rank + 1, acc.data(), datatype, count, MpiMessageType::SCAN);
+    }
+    if (rank > 0) {
+        copyBytes(recvBuffer, prev.data(), bytes);
     }
 }
 

@@ -718,6 +718,21 @@ int MPI_Scan(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatyp
     return MPI_SUCCESS;
 }
 
+int MPI_Exscan(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, MPI_Comm comm)
+{
+    SPDLOG_TRACE("MPI - MPI_Exscan");
+    if (refusedReduction(op, datatype)) {
+        return MPI_ERR_OP;
+    }
+    const uint8_t* send = (const uint8_t*)resolveInPlace(sendbuf, recvbuf);
+    if (auto sub = subOf(comm)) {
+        sub->exscan(getExecutingWorld(), executingContext.getRank(), send, (uint8_t*)recvbuf, datatype, count, op);
+        return MPI_SUCCESS;
+    }
+    getExecutingWorld().exscan(executingContext.getRank(), send, (uint8_t*)recvbuf, datatype, count, op);
+    return MPI_SUCCESS;
+}
+
 int MPI_Alltoall(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
                  MPI_Datatype recvtype, MPI_Comm comm)
 {
@@ -1132,6 +1147,47 @@ int MPI_Ireduce(const void* sendbuf, void* recvbuf, int count, MPI_Datatype data
                        request);
     }
     return handOut(world.iReduce(rank, root, send, (uint8_t*)recvbuf, datatype, count, op), request);
+}
+
+// MPI_Iscan and MPI_Iexscan.  The device or host choice rests on the send
+// (the recv when in place), which every rank judges alike.
+static int iScanCall(bool exclusive, const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op,
+                     MPI_Comm comm, MPI_Request* request)
+{
+    if (refusedReduction(op, datatype)) {
+        return MPI_ERR_OP;
+    }
+    MpiWorld& world = getExecutingWorld();
+    const int rank = executingContext.getRank();
+    const uint8_t* send = (const uint8_t*)resolveInPlace(sendbuf, recvbuf);
+    if (auto sub = subOf(comm)) {
+        auto dev = count > 0 && MpiWorld::isDevicePointer(send) && MpiWorld::deviceReducible(datatype, op)
+                     ? sub->deviceComm(world, rank)
+                     : nullptr;
+        return handOut(world.nbScan(dev, rank, exclusive, send, (uint8_t*)recvbuf, datatype, count, op, [&] {
+            if (exclusive) {
+                sub->exscan(world, rank, send, (uint8_t*)recvbuf, datatype, count, op);
+            } else {
+                sub->scan(world, rank, send, (uint8_t*)recvbuf, datatype, count, op);
+            }
+        }),
+                       request);
+    }
+    return handOut(world.iScan(rank, exclusive, send, (uint8_t*)recvbuf, datatype, count, op), request);
+}
+
+int MPI_Iscan(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, MPI_Comm comm,
+              MPI_Request* request)
+{
+    SPDLOG_TRACE("MPI - MPI_Iscan");
+    return iScanCall(false, sendbuf, recvbuf, count, datatype, op, comm, request);
+}
+
+int MPI_Iexscan(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, MPI_Comm comm,
+                MPI_Request* request)
+{
+    SPDLOG_TRACE("MPI - MPI_Iexscan");
+    return iScanCall(true, sendbuf, recvbuf, count, datatype, op, comm, request);
 }
 
 int MPI_Get_processor_name(char* name, int* resultlen)

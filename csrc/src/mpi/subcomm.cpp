@@ -161,6 +161,37 @@ void SubCommunicator::scan(MpiWorld& w,
     copyBytes(recv, acc.data(), bytes);
 }
 
+void SubCommunicator::exscan(MpiWorld& w,
+                             int me,
+                             const uint8_t* send,
+                             uint8_t* recv,
+                             faabric_datatype_t* dt,
+                             int count,
+                             faabric_op_t* op)
+{
+    const size_t bytes = (size_t)count * dt->size;
+    // (in place decides nothing: see MpiWorld::exscan)
+    if (bytes > 0 && MpiWorld::isDevicePointer(send) && MpiWorld::deviceReducible(dt, op) &&
+        w.deviceExscan(deviceComm(w, me), me, send, recv, dt, count, op)) {
+        return;
+    }
+    const int myCommRank = commRankOf(me);
+    std::vector<uint8_t> acc(bytes);
+    std::vector<uint8_t> prev(bytes);
+    copyBytes(acc.data(), send, bytes);
+    if (myCommRank > 0) {
+        w.recv(worldRanks[myCommRank - 1], me, prev.data(), dt, count, nullptr);
+        // acc = prefix op mine, before an in-place recv is overwritten
+        w.op_reduce(op, dt, count, prev.data(), acc.data());
+    }
+    if (myCommRank < size() - 1) {
+        w.send(me, worldRanks[myCommRank + 1], acc.data(), dt, count);
+    }
+    if (myCommRank > 0) {
+        copyBytes(recv, prev.data(), bytes);
+    }
+}
+
 void SubCommunicator::gather(MpiWorld& w, int me, int root, const uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count)
 {
     const size_t bytes = (size_t)count * dt->size;

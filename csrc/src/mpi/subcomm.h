@@ -55,6 +55,8 @@ class SubCommunicator
     void allReduce(MpiWorld& w, int me, const uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count, faabric_op_t* op);
 
     void scan(MpiWorld& w, int me, const uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count, faabric_op_t* op);
+    void exscan(MpiWorld& w, int me, const uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count,
+                faabric_op_t* op);
 
     // send == nullptr on the root means "already in place in recv"
     void gather(MpiWorld& w, int me, int root, const uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count);

@@ -94,6 +94,8 @@ GROUP_KINDS = {
     "gather": 5,
     "scatter": 6,
     "reduce": 7,
+    "scan": 8,
+    "exscan": 9,
 }
 ALGOS = {"auto": 0, "oneshot": 1, "twoshot": 2, "nvls": 3, "ll": 4}
 ALGO_NAMES = {v: k for k, v in ALGOS.items()}
@@ -478,7 +480,8 @@ class Communicator:
         communicator's GPU; the root's side (gather recvs, scatter sends) may
         be None off the root, or a list of None.  Reduce needs the rooted
         rules with equal send and recv numel and element size (recvs as for
-        gather)."""
+        gather); scan and exscan the same, with a send and a recv on every
+        rank and no root."""
         if kind in ("gather", "scatter", "reduce"):
             if not 0 <= int(root) < self.size:
                 raise CommError(f"{what}: root {root} outside a communicator of {self.size}")
@@ -486,11 +489,13 @@ class Communicator:
                 recvs = [None] * len(sends or [])
             if kind == "scatter" and sends is None:
                 sends = [None] * len(recvs or [])
+        if kind in ("scan", "exscan") and (sends is None or recvs is None):
+            raise CommError(f"{what}: need equally long, non-empty lists")
         if len(sends) != len(recvs) or not sends:
             raise CommError(f"{what}: need equally long, non-empty lists")
         per = 1
-        if kind == "reduce":
-            rooted = self.rank == int(root)
+        if kind in ("reduce", "scan", "exscan"):
+            rooted = kind != "reduce" or self.rank == int(root)
             for i, (s, r) in enumerate(zip(sends, recvs)):
                 for t in (s, r):
                     if t is not None and (not t.is_cuda or t.device.index != self.device or not t.is_contiguous()):
@@ -499,7 +504,10 @@ class Communicator:
                             f"{'' if t.is_contiguous() else ' (non-contiguous)'}"
                         )
                 if s is None or (r is None and rooted):
-                    raise CommError(f"{what}: item {i} needs a send on every rank and a recv on the root")
+                    raise CommError(
+                        f"{what}: item {i} needs a send on every rank and a recv on "
+                        f"{'the root' if kind == 'reduce' else 'every rank'}"
+                    )
                 if r is not None and (r.numel() != s.numel() or r.element_size() != s.element_size()):
                     raise CommError(
                         f"{what}: item {i} has {s.numel()} send and {r.numel()} recv elements of "
@@ -583,6 +591,7 @@ class Communicator:
             raise CommError(f"{what} failed [{_lib.last_error()}]")
         plan = GroupPlan(self, h, n, sum(t.numel() * t.element_size() for t in sized if t is not None))
         plan.root = int(root)
+        plan.kind = kind
         return plan
 
     def _launch(self, what, kind, plan, op, root, stream, channel, flags):
@@ -597,7 +606,8 @@ class Communicator:
 
     def _many(self, what, kind, sends, recvs, dtype, op, root, stream, channel):
         n, sp, rp, cnt, dt = self._group_items(what, kind, sends, recvs, dtype, root)
-        f = (0 if kind in ("gather", "scatter", "reduce") else self._sym(*sends)) | ((channel & 0xF) << 8)
+        staged = kind in ("gather", "scatter", "reduce", "scan", "exscan")
+        f = (0 if staged else self._sym(*sends)) | ((channel & 0xF) << 8)
         fop = OPS[op] if op is not None else 0
         rc = self._lib.fb_group_many(
             self._h, GROUP_KINDS[kind], n, sp, rp, cnt, dt, fop, int(root), f, self._stream(stream)
@@ -742,6 +752,28 @@ class Communicator:
         """Transient variant of :meth:`prepare_reduce_group` +
         :meth:`reduce_group`."""
         self._many("reduce_many", "reduce", sends, recvs, dtype, op, root, stream, channel)
+
+    def prepare_scan_group(self, sends, recvs, exclusive=False, dtype=None) -> "GroupPlan":
+        """Plan the launches of a prefix reduction of every pair of the lists
+        given to :meth:`scan_group`: MPI_Scan per pair (``recvs[i]`` on rank r
+        gets the op over ``sends[i]`` of ranks 0..r, folded in rank order), or
+        with ``exclusive`` MPI_Exscan (ranks 0..r-1; rank 0's recvs are not
+        written).  Tensors are any device memory at any alignment, and every
+        rank passes both lists; in place (``recvs[i]`` is ``sends[i]``) is
+        allowed on any rank.  The dtype is fixed here, the op is given at
+        launch.  Call collectively with the same counts."""
+        kind = "exscan" if exclusive else "scan"
+        return self._prepare("prepare_scan_group", kind, sends, recvs, dtype, sends)
+
+    def scan_group(self, plan: "GroupPlan", op="sum", stream=None, channel=0, flags=0):
+        if plan.kind not in ("scan", "exscan"):
+            raise CommError(f"scan_group: a {plan.kind} plan")
+        self._launch("scan_group", plan.kind, plan, OPS[op], 0, stream, channel, flags)
+
+    def scan_many(self, sends, recvs, op="sum", exclusive=False, stream=None, channel=0, dtype=None):
+        """Transient variant of :meth:`prepare_scan_group` +
+        :meth:`scan_group`."""
+        self._many("scan_many", "exscan" if exclusive else "scan", sends, recvs, dtype, op, 0, stream, channel)
 
     def send_recv(self, send_buf, dst, recv_buf, src, stream=None):
         rc = self._lib.fb_sendrecv(
@@ -1014,7 +1046,8 @@ class Communicator:
 
 class GroupPlan:
     """Device-resident segment tables of a grouped all-reduce, reduce-scatter,
-    all-gather, broadcast, all-to-all, gather or scatter."""
+    all-gather, broadcast, all-to-all, gather, scatter, reduce, scan or
+    exscan."""
 
     def __init__(self, comm: Communicator, handle, n_tensors: int, nbytes: int):
         self._comm = comm
@@ -1024,6 +1057,8 @@ class GroupPlan:
         self.launches = int(comm._lib.fb_group_plan_launches(self._h))
         # gather and scatter: the root the plan was prepared for
         self.root = 0
+        # the GROUP_KINDS name it was prepared as
+        self.kind = None
 
     def close(self):
         if self._h:
