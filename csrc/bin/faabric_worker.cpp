@@ -33,6 +33,7 @@
 #include "../tests/mpi_group_scan_body.h"
 #include "../tests/mpi_group_rooted_body.h"
 #include "../tests/mpi_group_subcomm_body.h"
+#include "../tests/mpi_persistent_body.h"
 
 #include <cuda_runtime.h>
 
@@ -839,6 +840,163 @@ static void registerFunctions()
             msg.set_outputdata(why);
         }
         return rc;
+    });
+
+    // Persistent collectives of all ten kinds on the world and on
+    // sub-communicators (mpi_persistent_body.h)
+    mpiFunction("persistent-coll", [](int rank, int size, faabric::Message& msg) {
+        std::string why;
+        int rc = persistent_coll::body(rank, size, msg.mpiworldid(), true, true, &why);
+        if (rc != 0) {
+            SPDLOG_ERROR("persistent-coll: {}", why);
+            msg.set_outputdata(why);
+        }
+        return rc;
+    });
+
+    // A list of int32 tensors all-reduced (MPI_SUM) or exchanged all-to-all on
+    // the world per step, in the symmetric heap.  Input:
+    // "<kind>;<mode>;<steps>;<count0,count1,...>" with kind allreduce or
+    // alltoall, count_i the elements of tensor i on one rank (for alltoall a
+    // multiple of 4 * size) and mode
+    //   blocking    one MPI_Allreduce / MPI_Alltoall per tensor
+    //   icall       MPI_Iallreduce / MPI_Ialltoall per tensor + MPI_Waitall
+    //   persistent  MPI_Startall of one persistent request per tensor (made
+    //               once, before the warm-up) + MPI_Waitall
+    // Rank 0 reports {"ms_per_step", "us_per_call", "launches_per_step",
+    // "wait_ms_per_step", "tables_per_step", "digest"}: launches and segment
+    // tables counted on its world device communicator, the part of a step
+    // spent in MPI_Waitall, and an FNV-1a digest of every rank's recv after
+    // the last step (the same seeded sends in every mode).
+    mpiFunction("bench-persistent", [](int rank, int size, faabric::Message& msg) {
+        std::vector<std::string> f;
+        std::string cur;
+        for (char c : msg.inputdata() + ";") {
+            if (c == ';') {
+                f.push_back(cur);
+                cur.clear();
+            } else {
+                cur += c;
+            }
+        }
+        EXPECT(f.size() >= 4 && size >= 2);
+        const bool a2a = f[0] == "alltoall";
+        const std::string mode = f[1];
+        const int steps = std::stoi(f[2]);
+        std::vector<size_t> counts;
+        for (size_t b = 0, e; b < f[3].size(); b = e + 1) {
+            e = f[3].find(',', b);
+            if (e == std::string::npos) {
+                e = f[3].size();
+            }
+            counts.push_back(std::stoull(f[3].substr(b, e - b)));
+        }
+        size_t total = 0;
+        std::vector<size_t> offs;
+        for (size_t c : counts) {
+            EXPECT(!a2a || c % (4 * (size_t)size) == 0);
+            offs.push_back(total);
+            total += c;
+        }
+        faabric::mpi::MpiWorld& world = faabric::mpi::getMpiWorldRegistry().getWorld(msg.mpiworldid());
+        int32_t* send = nullptr;
+        int32_t* recv = nullptr;
+        EXPECT(MPI_Alloc_mem(total * 4, MPI_INFO_FAABRIC_DEVICE, &send) == MPI_SUCCESS);
+        EXPECT(MPI_Alloc_mem(total * 4, MPI_INFO_FAABRIC_DEVICE, &recv) == MPI_SUCCESS);
+        // (copies from host memory, which wait for this rank only: a device-wide
+        // synchronise could wait for a peer's collective that waits for us)
+        std::vector<int32_t> init(total);
+        for (size_t i = 0; i < total; i++) {
+            init[i] = (int32_t)((i * 2654435761u + (size_t)rank * 40503u) & 0xffff);
+        }
+        cudaMemcpy(send, init.data(), total * 4, cudaMemcpyHostToDevice);
+        std::fill(init.begin(), init.end(), 0);
+        cudaMemcpy(recv, init.data(), total * 4, cudaMemcpyHostToDevice);
+        const int n = (int)counts.size();
+        std::vector<MPI_Request> reqs(n, MPI_REQUEST_NULL);
+        auto block = [&](int i) { return (int)(counts[i] / size); };
+        if (mode == "persistent") {
+            for (int i = 0; i < n; i++) {
+                EXPECT((a2a ? MPI_Alltoall_init(send + offs[i], block(i), MPI_INT, recv + offs[i], block(i), MPI_INT,
+                                                MPI_COMM_WORLD, MPI_INFO_NULL, &reqs[i])
+                            : MPI_Allreduce_init(send + offs[i], recv + offs[i], (int)counts[i], MPI_INT, MPI_SUM,
+                                                 MPI_COMM_WORLD, MPI_INFO_NULL, &reqs[i])) == MPI_SUCCESS);
+            }
+        }
+        MPI_Barrier(MPI_COMM_WORLD);
+        double waitMs = 0;
+        auto step = [&]() -> int {
+            if (mode == "persistent") {
+                EXPECT(MPI_Startall(n, reqs.data()) == MPI_SUCCESS);
+            }
+            for (int i = 0; mode != "persistent" && i < n; i++) {
+                int rc;
+                if (mode == "blocking") {
+                    rc = a2a ? MPI_Alltoall(send + offs[i], block(i), MPI_INT, recv + offs[i], block(i), MPI_INT,
+                                            MPI_COMM_WORLD)
+                             : MPI_Allreduce(send + offs[i], recv + offs[i], (int)counts[i], MPI_INT, MPI_SUM,
+                                             MPI_COMM_WORLD);
+                } else {
+                    rc = a2a ? MPI_Ialltoall(send + offs[i], block(i), MPI_INT, recv + offs[i], block(i), MPI_INT,
+                                             MPI_COMM_WORLD, &reqs[i])
+                             : MPI_Iallreduce(send + offs[i], recv + offs[i], (int)counts[i], MPI_INT, MPI_SUM,
+                                              MPI_COMM_WORLD, &reqs[i]);
+                }
+                EXPECT(rc == MPI_SUCCESS);
+            }
+            if (mode != "blocking") {
+                auto w0 = std::chrono::steady_clock::now();
+                EXPECT(MPI_Waitall(n, reqs.data(), MPI_STATUSES_IGNORE) == MPI_SUCCESS);
+                waitMs += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - w0).count();
+            }
+            return 0;
+        };
+        for (int i = 0; i < 3; i++) {
+            EXPECT(step() == 0);
+        }
+        auto dev = world.getDeviceComm(rank);
+        EXPECT(dev != nullptr);
+        MPI_Barrier(MPI_COMM_WORLD);
+        waitMs = 0;
+        const uint64_t l0 = dev->stats().launches;
+        const uint64_t s0 = dev->stats().segTables;
+        auto t0 = std::chrono::steady_clock::now();
+        for (int i = 0; i < steps; i++) {
+            EXPECT(step() == 0);
+        }
+        const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count() / steps;
+        const double launches = (double)(dev->stats().launches - l0) / steps;
+        const double tables = (double)(dev->stats().segTables - s0) / steps;
+        MPI_Barrier(MPI_COMM_WORLD);
+        std::vector<int32_t> back(total);
+        cudaMemcpy(back.data(), recv, total * 4, cudaMemcpyDeviceToHost);
+        uint64_t h = 1469598103934665603ULL;
+        for (int32_t v : back) {
+            h = (h ^ (uint32_t)v) * 1099511628211ULL;
+        }
+        std::vector<uint64_t> digests(size);
+        MPI_Gather(&h, 8, MPI_BYTE, digests.data(), 8, MPI_BYTE, 0, MPI_COMM_WORLD);
+        for (auto& r : reqs) {
+            if (mode == "persistent") {
+                EXPECT(MPI_Request_free(&r) == MPI_SUCCESS);
+            }
+        }
+        if (rank == 0) {
+            uint64_t all = 1469598103934665603ULL;
+            for (uint64_t d : digests) {
+                all = (all ^ d) * 1099511628211ULL;
+            }
+            char hex[17];
+            snprintf(hex, sizeof(hex), "%016llx", (unsigned long long)all);
+            msg.set_outputdata("{\"ms_per_step\": " + std::to_string(ms) + ", \"us_per_call\": " +
+                               std::to_string(ms * 1000.0 / n) + ", \"launches_per_step\": " + std::to_string(launches) +
+                               ", \"tables_per_step\": " + std::to_string(tables) +
+                               ", \"wait_ms_per_step\": " + std::to_string(waitMs / steps) + ", \"digest\": \"" + hex +
+                               "\"}");
+        }
+        MPI_Free_mem(recv);
+        MPI_Free_mem(send);
+        return 0;
     });
 
     // A list of tensors exchanged on the world per step, each one send and one

@@ -118,6 +118,9 @@ struct CommStats
     uint64_t algoCount[FB_ALGO_COUNT] = { 0 };
     uint64_t stagedCopies = 0;
     uint64_t tmaLaunches = 0;
+    // grouped segment tables built and uploaded: one per launch of a plan
+    // prepareGroup makes, one per grouped batch of groupMany
+    uint64_t segTables = 0;
 };
 
 class Communicator : public std::enable_shared_from_this<Communicator>

@@ -24,6 +24,11 @@ extern "C"
 /* a synchronisation call out of place: unlock / flush of a target that is
  * not locked, a second lock, fence or free inside a passive epoch */
 #define MPI_ERR_RMA_SYNC 7
+/* MPI_Start of an active or non-persistent request, MPI_Request_free of an
+ * active persistent one */
+#define MPI_ERR_REQUEST 8
+/* MPI_Start of a persistent request whose communicator was freed */
+#define MPI_ERR_COMM 9
 #define MPI_MAX_OBJECT_NAME 128
 
 /* passive-target lock types (MPI_Win_lock) */
@@ -233,6 +238,7 @@ extern "C"
 #define MPI_NO_OP &faabric_op_no_op
 
 #define MPI_STATUS_IGNORE ((MPI_Status*)(0))
+#define MPI_REQUEST_NULL ((MPI_Request)(0))
 #define MPI_STATUSES_IGNORE ((MPI_Status*)(0))
 
 #define MPI_WIN_BASE 1
@@ -370,6 +376,36 @@ extern "C"
                   MPI_Request* request);
     int MPI_Iexscan(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, MPI_Comm comm,
                     MPI_Request* request);
+    /* Persistent collectives (MPI-4.0).  Each init call refuses what the
+     * matching MPI_I* call refuses, before anything is created, and fixes
+     * where the call runs; info is ignored.  A completed start leaves the
+     * request inactive (a wait on it returns at once, MPI_Waitany skips it);
+     * MPI_Request_free releases an inactive one. */
+    int MPI_Allreduce_init(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op,
+                           MPI_Comm comm, MPI_Info info, MPI_Request* request);
+    int MPI_Reduce_scatter_block_init(const void* sendbuf, void* recvbuf, int recvcount, MPI_Datatype datatype,
+                                      MPI_Op op, MPI_Comm comm, MPI_Info info, MPI_Request* request);
+    int MPI_Allgather_init(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                           MPI_Datatype recvtype, MPI_Comm comm, MPI_Info info, MPI_Request* request);
+    int MPI_Bcast_init(void* buffer, int count, MPI_Datatype datatype, int root, MPI_Comm comm, MPI_Info info,
+                       MPI_Request* request);
+    int MPI_Alltoall_init(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                          MPI_Datatype recvtype, MPI_Comm comm, MPI_Info info, MPI_Request* request);
+    int MPI_Gather_init(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                        MPI_Datatype recvtype, int root, MPI_Comm comm, MPI_Info info, MPI_Request* request);
+    int MPI_Scatter_init(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                         MPI_Datatype recvtype, int root, MPI_Comm comm, MPI_Info info, MPI_Request* request);
+    int MPI_Reduce_init(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, int root,
+                        MPI_Comm comm, MPI_Info info, MPI_Request* request);
+    int MPI_Scan_init(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, MPI_Comm comm,
+                      MPI_Info info, MPI_Request* request);
+    int MPI_Exscan_init(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op,
+                        MPI_Comm comm, MPI_Info info, MPI_Request* request);
+    /* MPI_ERR_REQUEST for an active or non-persistent request, MPI_ERR_COMM
+     * when its communicator was freed; MPI_Startall checks every request
+     * before it starts any */
+    int MPI_Start(MPI_Request* request);
+    int MPI_Startall(int count, MPI_Request array_of_requests[]);
     int MPI_Free_mem(void* base);
     int MPI_Win_create(void* base, MPI_Aint size, int disp_unit, MPI_Info info, MPI_Comm comm, MPI_Win* win);
     int MPI_Win_allocate_shared(MPI_Aint size, int disp_unit, MPI_Info info, MPI_Comm comm, void* baseptr, MPI_Win* win);

@@ -237,12 +237,31 @@ class MpiWorld
               int count,
               MpiMessageType messageType = MpiMessageType::NORMAL);
 
-    void awaitAsyncRequest(int requestId);
+    // True when the request is persistent: it is inactive now and stays
+    // (waiting for an inactive one returns at once)
+    bool awaitAsyncRequest(int requestId);
 
     // MPI_Request_free: drops a request-based one-sided operation's request
-    // (the operation completes at the next flush or unlock); other kinds of
-    // request are kept
-    void freeAsyncRequest(int requestId);
+    // (the operation completes at the next flush or unlock) and an inactive
+    // persistent request, with every cached plan that contains it
+    // (MPI_ERR_REQUEST for an active one); other kinds of request are kept
+    int freeAsyncRequest(int requestId);
+
+    // ---- persistent collectives (MPI_*_init, MPI_Start) ----
+    // An init call runs the non-blocking call's nbX function with
+    // `persistentComm` set to its MPI communicator's id: the call and where
+    // it runs (the burst, one device call, or the host path) are fixed then,
+    // and nothing is issued.  MPI_Start runs it the way the non-blocking call
+    // would have: MPI_SUCCESS, MPI_ERR_REQUEST (not a persistent request, or
+    // an active one) or MPI_ERR_COMM (its communicator was freed).
+    int startCheck(int requestId);
+    int startPersistent(int requestId);
+    // An inactive persistent request (MPI_Waitany skips it)
+    bool persistentInactive(int requestId);
+    // MPI_Comm_free of `commId` (after settleDeviceBurst on `child`): its
+    // persistent requests of this rank thread cannot start again, and the
+    // cached plans on `child` are dropped
+    void persistentCommFreed(int commId, const std::shared_ptr<faabric::device::Communicator>& child);
 
     void sendRecv(uint8_t* sendBuffer,
                   int sendCount,
@@ -315,7 +334,8 @@ class MpiWorld
                    uint8_t* recvBuffer,
                    faabric_datatype_t* datatype,
                    int count,
-                   faabric_op_t* operation);
+                   faabric_op_t* operation,
+                   int persistentComm = 0);
 
     // MPI_Ireduce_scatter_block and MPI_Iallgather, built like iAllReduce: a
     // burst on symmetric, 16-byte aligned device buffers whose shards are
@@ -329,7 +349,8 @@ class MpiWorld
                        uint8_t* recvBuffer,
                        faabric_datatype_t* datatype,
                        int recvCount,
-                       faabric_op_t* operation);
+                       faabric_op_t* operation,
+                       int persistentComm = 0);
 
     int iAllGather(int rank,
                    const uint8_t* sendBuffer,
@@ -337,14 +358,15 @@ class MpiWorld
                    int sendCount,
                    uint8_t* recvBuffer,
                    faabric_datatype_t* recvType,
-                   int recvCount);
+                   int recvCount,
+                   int persistentComm = 0);
 
     // MPI_Ibcast on the world (root: a world rank), by the same rules:
     // symmetric, 16-byte aligned device buffers join a burst keyed by (kind,
     // communicator, root), issued as one grouped launch at the next wait;
     // other device buffers run one broadcast at issue; host buffers complete
     // at issue.
-    int iBroadcast(int rank, int root, uint8_t* buffer, faabric_datatype_t* dt, int count);
+    int iBroadcast(int rank, int root, uint8_t* buffer, faabric_datatype_t* dt, int count, int persistentComm = 0);
 
     // MPI_Ialltoall on the world, by the same rules: symmetric, 16-byte
     // aligned device buffers whose block is a multiple of 16 bytes join a
@@ -357,7 +379,8 @@ class MpiWorld
                   int sendCount,
                   uint8_t* recvBuffer,
                   faabric_datatype_t* recvType,
-                  int recvCount);
+                  int recvCount,
+                  int persistentComm = 0);
 
     // MPI_Igather / MPI_Iscatter on the world (root: a world rank; `bytes`
     // per rank).  The root's significant buffer and the other ranks' own
@@ -369,9 +392,9 @@ class MpiWorld
     // buffers complete at issue.  The counts and types are the blocking
     // call's.
     int iGather(int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes, faabric_datatype_t* sendType,
-                int sendCount, faabric_datatype_t* recvType, int recvCount);
+                int sendCount, faabric_datatype_t* recvType, int recvCount, int persistentComm = 0);
     int iScatter(int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes, faabric_datatype_t* sendType,
-                 int sendCount, faabric_datatype_t* recvType, int recvCount);
+                 int sendCount, faabric_datatype_t* recvType, int recvCount, int persistentComm = 0);
     // MPI_Ireduce on the world (root: a world rank; send == recv at the root
     // is in place; recv is not significant off the root).  A device send with
     // a pair the device reduces joins a burst keyed by (communicator, dtype,
@@ -379,7 +402,7 @@ class MpiWorld
     // wait (one device reduce at issue with grouping off); anything else
     // completes at issue on the blocking path.
     int iReduce(int rank, int root, const uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count,
-                faabric_op_t* op);
+                faabric_op_t* op, int persistentComm = 0);
     // MPI_Iscan, or with `exclusive` MPI_Iexscan, on the world (send == recv
     // is in place, on any rank).  A device send with a pair the device
     // reduces joins a burst keyed by (kind, communicator, dtype, op), issued
@@ -387,7 +410,7 @@ class MpiWorld
     // grouped launch at issue with grouping off); anything else completes at
     // issue on the blocking path.
     int iScan(int rank, bool exclusive, const uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count,
-              faabric_op_t* op);
+              faabric_op_t* op, int persistentComm = 0);
 
     // Symmetric-heap allocation for MPI_Alloc_mem (collective: every rank
     // must allocate the same sizes in the same order)
@@ -636,38 +659,40 @@ class MpiWorld
     // request at issue.  Symmetric, 16-byte aligned device buffers are
     // deferred into this rank's burst (FAABRIC_MPI_GROUP_IALLREDUCE=0 turns
     // that off); other device buffers run one device call at issue.
+    // `persistentComm` is 0, or the MPI communicator id of a persistent init
+    // (see startPersistent): then `host` must own what it captures.
     using HostPath = std::function<void()>;
     int nbAllReduce(const DeviceComm& comm, int rank, const uint8_t* send, uint8_t* recv,
-                    faabric_datatype_t* dt, int count, faabric_op_t* op, const HostPath& host);
+                    faabric_datatype_t* dt, int count, faabric_op_t* op, const HostPath& host, int persistentComm = 0);
     // (send == recv runs `host`: the output would overwrite input the peers
     // are still reading)
     int nbReduceScatter(const DeviceComm& comm, int rank, int members, const uint8_t* send, uint8_t* recv,
-                        faabric_datatype_t* dt, int recvCount, faabric_op_t* op, const HostPath& host);
+                        faabric_datatype_t* dt, int recvCount, faabric_op_t* op, const HostPath& host, int persistentComm = 0);
     int nbAllGather(const DeviceComm& comm, int rank, int members, const uint8_t* send, uint8_t* recv,
-                    size_t bytes, const HostPath& host);
+                    size_t bytes, const HostPath& host, int persistentComm = 0);
     // `root` is a rank of `comm`'s communicator (the caller checked it)
-    int nbBroadcast(const DeviceComm& comm, int rank, int root, uint8_t* buffer, size_t bytes, const HostPath& host);
+    int nbBroadcast(const DeviceComm& comm, int rank, int root, uint8_t* buffer, size_t bytes, const HostPath& host, int persistentComm = 0);
     // `bytes` per block; send and recv hold `members` blocks each and do not
     // alias (the caller refused MPI_IN_PLACE)
     int nbAllToAll(const DeviceComm& comm, int rank, int members, const uint8_t* send, uint8_t* recv, size_t bytes,
-                   const HostPath& host);
+                   const HostPath& host, int persistentComm = 0);
     // `root` is a rank of `comm`'s communicator (the caller checked it);
     // buffers as for iGather / iScatter.  The caller decides where the call
     // runs, once: `comm` is null unless this rank's own buffer (gather send,
     // scatter recv) is device memory.
     int nbGather(const DeviceComm& comm, int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes,
-                 const HostPath& host);
+                 const HostPath& host, int persistentComm = 0);
     int nbScatter(const DeviceComm& comm, int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes,
-                  const HostPath& host);
+                  const HostPath& host, int persistentComm = 0);
     // `root` is a rank of `comm`'s communicator (the caller checked it);
     // buffers as for iReduce.  `comm` is null unless the send is device
     // memory and deviceReducible(dt, op) holds (judged once, by the caller).
     int nbReduce(const DeviceComm& comm, int rank, int root, const uint8_t* send, uint8_t* recv,
-                 faabric_datatype_t* dt, int count, faabric_op_t* op, const HostPath& host);
+                 faabric_datatype_t* dt, int count, faabric_op_t* op, const HostPath& host, int persistentComm = 0);
     // Buffers as for iScan.  `comm` is null unless the send is device memory
     // and deviceReducible(dt, op) holds (judged once, by the caller).
     int nbScan(const DeviceComm& comm, int rank, bool exclusive, const uint8_t* send, uint8_t* recv,
-               faabric_datatype_t* dt, int count, faabric_op_t* op, const HostPath& host);
+               faabric_datatype_t* dt, int count, faabric_op_t* op, const HostPath& host, int persistentComm = 0);
     // Issues this rank thread's pending burst if it is keyed to `comm`, and
     // waits for it (before `comm` is released: MPI_Comm_free)
     void settleDeviceBurst(const DeviceComm& comm);
@@ -678,7 +703,15 @@ class MpiWorld
     struct NbCall;
     template <typename Issue>
     int nbCollective(const DeviceComm& comm, int rank, bool device, const NbCall& call, Issue&& issue,
-                     const HostPath& host);
+                     const HostPath& host, int persistentComm);
+    // The direct device all-reduce of nbAllReduce, on the stream it sets;
+    // false when the communicator declines it
+    bool allReduceAtIssue(const DeviceComm& comm, int rank, bool symmetric, const uint8_t* send, uint8_t* recv,
+                          int count, int fdt, int fop, void** stream);
+
+    // awaitAsyncRequest for any request but an inactive persistent one:
+    // completes it and drops it
+    void awaitRequest(int requestId);
 
     int id = -1;
     int size = -1;

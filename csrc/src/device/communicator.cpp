@@ -2185,6 +2185,7 @@ std::shared_ptr<Communicator::GroupPlan> Communicator::prepareGroup(
         if (rc != FB_OK) {
             return nullptr;
         }
+        stats_.segTables++;
         // (a rank may own nothing of a tiny group: it still takes part in the
         // barriers, with an empty table)
         const size_t tb = std::max<size_t>(segs.size(), 1) * sizeof(fb::GroupSeg);
@@ -2503,6 +2504,7 @@ int Communicator::groupMany(GroupKind kind,
             }
             continue;
         }
+        stats_.segTables++;
         ManySlot* slot = nullptr;
         l.dSegs = (fb::GroupSeg*)stageManyTable(segs.data(), segs.size() * sizeof(fb::GroupSeg), s, &slot);
         // (on loopback an empty table is a null pointer the kernel never reads)

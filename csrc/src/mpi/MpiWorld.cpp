@@ -24,6 +24,7 @@
 #include <cstring>
 #include <deque>
 #include <functional>
+#include <list>
 #include <poll.h>
 #include <unistd.h>
 
@@ -33,6 +34,48 @@ namespace faabric::mpi {
 // Per-rank (= per-thread) state
 // ---------------------------------------------------------------------------
 namespace {
+// Where a non-blocking collective runs: deferred into this rank thread's
+// burst, one device call at issue, or the blocking host path at issue
+enum class Route
+{
+    Grouped,
+    Direct,
+    Host
+};
+
+// A persistent collective (MPI_*_init): the call and its route, fixed at
+// init.  `active` from MPI_Start until the wait that completes the start.
+struct PersistentColl
+{
+    Route route;
+    faabric::device::Communicator::GroupKind kind;
+    std::shared_ptr<faabric::device::Communicator> comm;
+    int dtype;
+    int op;
+    int root;
+    faabric::device::Communicator::GroupItem item;
+    int rank;
+    int commId;
+    // Direct: issues the device call and sets the stream it went out on;
+    // false when the communicator declines it
+    std::function<bool(void**)> direct;
+    std::function<void()> host;
+    bool active = false;
+    bool commFreed = false;
+};
+
+// A plan of a burst made only of persistent starts, and its key
+struct CachedPlan
+{
+    faabric::device::Communicator::GroupKind kind;
+    const faabric::device::Communicator* comm;
+    int dtype;
+    int op;
+    int root;
+    std::vector<int> requests;
+    std::shared_ptr<faabric::device::Communicator::GroupPlan> plan;
+};
+
 struct AsyncRequest
 {
     bool isSend = false;
@@ -57,6 +100,8 @@ struct AsyncRequest
     int rmaTarget = -1;
     uint64_t rmaSeq = 0;
     std::shared_ptr<MpiWorld::RmaProgress> rmaProgress;
+    // Persistent collective (started, or inactive when nothing else is set)
+    std::shared_ptr<PersistentColl> persistent;
 };
 
 struct RankState
@@ -95,6 +140,14 @@ struct RankState
     void* groupStream = nullptr;
     std::vector<faabric::device::Communicator::GroupItem> groupItems;
     std::vector<int> groupRequests;
+    // every call of the pending burst is a persistent start
+    bool groupAllPersistent = false;
+    // Plans of such bursts, most recently used first, and plans dropped from
+    // the cache.  A dropped plan's device tables are freed with the rank
+    // state, at world teardown: a cudaFree waits for the whole device, where
+    // a peer sharing it may wait for this rank.
+    std::list<CachedPlan> plans;
+    std::vector<std::shared_ptr<faabric::device::Communicator::GroupPlan>> retiredPlans;
     // grouped launches go out on one stream, in order: once a request of
     // launch k was waited for, every request of launches <= k is complete
     uint64_t groupLaunchSeq = 0;
@@ -126,6 +179,9 @@ struct RankState
         groupComm = nullptr;
         groupItems.clear();
         groupRequests.clear();
+        groupAllPersistent = false;
+        plans.clear();
+        retiredPlans.clear();
         cachedComm = nullptr;
         cachedStream0 = nullptr;
         cachedCommRank = -1;
@@ -952,6 +1008,70 @@ static void awaitDevice(faabric::device::Communicator& comm, void* stream)
     }
 }
 
+static AsyncRequest collectiveRequest(int rank);
+
+// Plans a rank thread keeps for its bursts of persistent starts
+constexpr size_t kPlanCacheSize = 64;
+
+// Moves the cached plans `drop` selects out of the cache
+template <typename Drop>
+static void retirePlans(Drop&& drop)
+{
+    for (auto it = tls.plans.begin(); it != tls.plans.end();) {
+        if (drop(*it)) {
+            tls.retiredPlans.push_back(std::move(it->plan));
+            it = tls.plans.erase(it);
+        } else {
+            ++it;
+        }
+    }
+}
+
+// The pending burst, made only of persistent starts (requests `reqs`), as a
+// plan prepared once for its key: (kind, communicator, dtype, op, root, the
+// ordered requests).  The cache is this rank's alone, so one rank may hit
+// where a peer misses, has evicted the plan or is refused by prepareGroup.
+// The barriers still pair up: a plan depends only on its list, which the
+// requests fix, and prepareGroup cuts a list into launches exactly as
+// groupMany does, so a cached plan, a new one and groupMany issue the same
+// launches on every rank.
+static int runPersistentBurst(faabric::device::Communicator& comm,
+                              const std::vector<faabric::device::Communicator::GroupItem>& items,
+                              const std::vector<int>& reqs,
+                              cudaStream_t s)
+{
+    auto it = std::find_if(tls.plans.begin(), tls.plans.end(), [&](const CachedPlan& p) {
+        return p.kind == tls.groupKind && p.comm == &comm && p.dtype == tls.groupDtype && p.op == tls.groupOp &&
+               p.root == tls.groupRoot && p.requests == reqs;
+    });
+    if (it != tls.plans.end()) {
+        tls.plans.splice(tls.plans.begin(), tls.plans, it);
+    } else {
+        int rc = FB_OK;
+        auto plan = comm.prepareGroup(items.data(), items.size(), tls.groupDtype, &rc, tls.groupKind);
+        if (plan == nullptr) {
+            return comm.groupMany(
+              tls.groupKind, items.data(), items.size(), tls.groupDtype, tls.groupOp, tls.groupRoot, FB_FLAG_SYMMETRIC, s);
+        }
+        tls.plans.push_front(
+          CachedPlan{ tls.groupKind, &comm, tls.groupDtype, tls.groupOp, tls.groupRoot, reqs, std::move(plan) });
+        if (tls.plans.size() > kPlanCacheSize) {
+            tls.retiredPlans.push_back(std::move(tls.plans.back().plan));
+            tls.plans.pop_back();
+        }
+    }
+    const int rc = comm.runGroup(tls.groupKind, *tls.plans.front().plan, tls.groupOp, tls.groupRoot, FB_FLAG_SYMMETRIC, s);
+    if (rc == FB_E_UNSUPPORTED) {
+        // (a pair with no grouped kernel, refused before any launch:
+        // groupMany runs it as per-item calls)
+        tls.retiredPlans.push_back(std::move(tls.plans.front().plan));
+        tls.plans.pop_front();
+        return comm.groupMany(
+          tls.groupKind, items.data(), items.size(), tls.groupDtype, tls.groupOp, tls.groupRoot, FB_FLAG_SYMMETRIC, s);
+    }
+    return rc;
+}
+
 // Issues the deferred burst of this rank thread as one grouped launch (every
 // rank defers and flushes at the same program points)
 static void flushPendingGroup()
@@ -972,8 +1092,9 @@ static void flushPendingGroup()
     tls.groupComm = nullptr;
     cudaSetDevice(comm->device());
     const cudaStream_t s = (cudaStream_t)tls.groupStream;
-    const int rc = comm->groupMany(
-      tls.groupKind, items.data(), items.size(), tls.groupDtype, tls.groupOp, tls.groupRoot, FB_FLAG_SYMMETRIC, s);
+    const int rc = tls.groupAllPersistent ? runPersistentBurst(*comm, items, reqs, s)
+                                          : comm->groupMany(tls.groupKind, items.data(), items.size(), tls.groupDtype,
+                                                            tls.groupOp, tls.groupRoot, FB_FLAG_SYMMETRIC, s);
     if (rc != FB_OK) {
         const std::string what = std::string("Grouped device ") + Communicator::groupKindName(tls.groupKind);
         // (the burst's requests have no host path left: declining is an error too)
@@ -1009,17 +1130,46 @@ int MpiWorld::addRmaRequest(int rank, int winId, int targetRank, std::shared_ptr
     return requestId;
 }
 
-void MpiWorld::freeAsyncRequest(int requestId)
+int MpiWorld::freeAsyncRequest(int requestId)
 {
     // A request-based one-sided operation completes at the next flush or
     // unlock of its window anyway; the other kinds stay until they are waited
     auto it = tls.requests.find(requestId);
     if (it != tls.requests.end() && it->second.isRma) {
         tls.requests.erase(it);
+    } else if (it != tls.requests.end() && it->second.persistent != nullptr) {
+        if (it->second.persistent->active) {
+            return MPI_ERR_REQUEST;
+        }
+        tls.requests.erase(it);
+        retirePlans([&](const CachedPlan& p) {
+            return std::find(p.requests.begin(), p.requests.end(), requestId) != p.requests.end();
+        });
     }
+    return MPI_SUCCESS;
 }
 
-void MpiWorld::awaitAsyncRequest(int requestId)
+bool MpiWorld::awaitAsyncRequest(int requestId)
+{
+    auto it = tls.requests.find(requestId);
+    if (it == tls.requests.end() || it->second.persistent == nullptr) {
+        awaitRequest(requestId);
+        return false;
+    }
+    std::shared_ptr<PersistentColl> p = it->second.persistent;
+    if (p->active) {
+        // the start completes as the non-blocking call would; the request
+        // stays, inactive
+        awaitRequest(requestId);
+        p->active = false;
+        AsyncRequest idle = collectiveRequest(p->rank);
+        idle.persistent = std::move(p);
+        tls.requests[requestId] = std::move(idle);
+    }
+    return true;
+}
+
+void MpiWorld::awaitRequest(int requestId)
 {
     auto it = tls.requests.find(requestId);
     if (it == tls.requests.end()) {
@@ -1527,6 +1677,7 @@ static void deferToGroup(faabric::device::Communicator::GroupKind kind,
                                     tls.groupOp != op || tls.groupRoot != root || tls.groupItems.size() >= 4096)) {
         flushPendingGroup();
     }
+    tls.groupAllPersistent = (tls.groupItems.empty() || tls.groupAllPersistent) && r.persistent != nullptr;
     tls.groupKind = kind;
     tls.groupComm = comm;
     tls.groupDtype = dtype;
@@ -1574,11 +1725,23 @@ static Placement placeCollective(const faabric::device::Communicator& c,
     return { symmetric, symmetric && grouping && (((uintptr_t)send | (uintptr_t)recv | shardBytes) & 15) == 0 };
 }
 
-int MpiWorld::iAllReduce(int rank, uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count, faabric_op_t* op)
+int MpiWorld::iAllReduce(int rank, uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count, faabric_op_t* op,
+                         int persistentComm)
 {
     checkRanksRange(0, rank);
     cacheDeviceComm(rank);
-    return nbAllReduce(tls.cachedComm, rank, send, recv, dt, count, op, [&] { allReduce(rank, send, recv, dt, count, op); });
+    return nbAllReduce(tls.cachedComm, rank, send, recv, dt, count, op,
+                       [=, this] { allReduce(rank, send, recv, dt, count, op); }, persistentComm);
+}
+
+// Records an inactive persistent request of this rank thread
+static int addPersistent(PersistentColl p)
+{
+    const int requestId = tls.nextRequestId++;
+    AsyncRequest r = collectiveRequest(p.rank);
+    r.persistent = std::make_shared<PersistentColl>(std::move(p));
+    tls.requests[requestId] = std::move(r);
+    return requestId;
 }
 
 int MpiWorld::nbAllReduce(const DeviceComm& comm,
@@ -1588,50 +1751,61 @@ int MpiWorld::nbAllReduce(const DeviceComm& comm,
                           faabric_datatype_t* dt,
                           int count,
                           faabric_op_t* op,
-                          const HostPath& host)
+                          const HostPath& host,
+                          int persistentComm)
 {
     const size_t bytes = (size_t)count * dt->size;
-    const int requestId = tls.nextRequestId++;
-    AsyncRequest r = collectiveRequest(rank);
     const int fdt = fbDtypeFor(dt);
     const int fop = fbOpFor(op);
     cacheDeviceComm(rank);
+    Route route = Route::Host;
+    bool symmetric = false;
     // (a pair the kernels lack must not join a burst: the burst has no host path)
     if (bytes > 0 && deviceReducible(dt, op) && comm != nullptr) {
         const Placement at = placeCollective(*comm, groupIallreduce, send, bytes, recv, bytes, 0);
-        if (at.grouped) {
-            // Deferred: the whole burst becomes ONE kernel at the next wait
-            deferToGroup(faabric::device::Communicator::GROUP_ALLREDUCE,
-                         comm,
-                         fdt,
-                         fop,
-                         0,
-                         { send, recv, (size_t)count },
-                         requestId,
-                         std::move(r),
-                         deviceCollectives);
-            return requestId;
-        }
-        if (at.symmetric || isDevicePointer(send)) {
-            // Symmetric, 16-byte aligned buffers may use any channel; others
-            // (the communicator stages an unaligned heap buffer too) go
-            // through the single staging area on channel 0
-            const int nChannels = std::clamp(nonBlockingChannels.load(), 1, std::max(1, comm->config().channels));
-            const bool anyChannel = at.symmetric && (((uintptr_t)send | (uintptr_t)recv) & 15) == 0;
-            const int channel = anyChannel ? (int)(tls.deviceCollectiveSeq++ % (uint64_t)nChannels) : 0;
-            const int flags = (at.symmetric ? FB_FLAG_SYMMETRIC : 0) | FB_FLAG_CHANNEL(channel);
-            void* s = streamForRank(rank, channel);
-            if (issueDevice(*comm, s, deviceCollectives, [&](auto& c, cudaStream_t st) {
-                    return c.allReduce(send, recv, (size_t)count, fdt, fop, forcedAllReduceAlgo, flags, st);
-                })) {
-                return recordDevice(requestId, std::move(r), comm, s);
-            }
-        }
+        symmetric = at.symmetric;
+        route = at.grouped ? Route::Grouped : (at.symmetric || isDevicePointer(send)) ? Route::Direct : Route::Host;
+    }
+    const faabric::device::Communicator::GroupItem item{ send, recv, (size_t)count };
+    if (persistentComm != 0) {
+        PersistentColl p{ route, faabric::device::Communicator::GROUP_ALLREDUCE, comm, fdt, fop, 0, item, rank,
+                          persistentComm };
+        p.direct = [=, this](void** s) { return allReduceAtIssue(comm, rank, symmetric, send, recv, count, fdt, fop, s); };
+        p.host = host;
+        return addPersistent(std::move(p));
+    }
+    const int requestId = tls.nextRequestId++;
+    AsyncRequest r = collectiveRequest(rank);
+    if (route == Route::Grouped) {
+        // Deferred: the whole burst becomes ONE kernel at the next wait
+        deferToGroup(faabric::device::Communicator::GROUP_ALLREDUCE, comm, fdt, fop, 0, item, requestId, std::move(r),
+                     deviceCollectives);
+        return requestId;
+    }
+    void* s = nullptr;
+    if (route == Route::Direct && allReduceAtIssue(comm, rank, symmetric, send, recv, count, fdt, fop, &s)) {
+        return recordDevice(requestId, std::move(r), comm, s);
     }
     // Host path (or unsupported on the device): complete it now
     host();
     tls.requests[requestId] = std::move(r);
     return requestId;
+}
+
+bool MpiWorld::allReduceAtIssue(const DeviceComm& comm, int rank, bool symmetric, const uint8_t* send, uint8_t* recv,
+                                int count, int fdt, int fop, void** stream)
+{
+    // Symmetric, 16-byte aligned buffers may use any channel; others (the
+    // communicator stages an unaligned heap buffer too) go through the
+    // single staging area on channel 0
+    const int nChannels = std::clamp(nonBlockingChannels.load(), 1, std::max(1, comm->config().channels));
+    const bool anyChannel = symmetric && (((uintptr_t)send | (uintptr_t)recv) & 15) == 0;
+    const int channel = anyChannel ? (int)(tls.deviceCollectiveSeq++ % (uint64_t)nChannels) : 0;
+    const int flags = (symmetric ? FB_FLAG_SYMMETRIC : 0) | FB_FLAG_CHANNEL(channel);
+    *stream = streamForRank(rank, channel);
+    return issueDevice(*comm, *stream, deviceCollectives, [&](auto& c, cudaStream_t st) {
+        return c.allReduce(send, recv, (size_t)count, fdt, fop, forcedAllReduceAlgo, flags, st);
+    });
 }
 
 // One call of nbReduceScatter, nbAllGather, nbBroadcast or nbAllToAll: the
@@ -1659,29 +1833,102 @@ struct MpiWorld::NbCall
 // runs `host`, which completes the request at issue
 template <typename Issue>
 int MpiWorld::nbCollective(const DeviceComm& comm, int rank, bool device, const NbCall& call, Issue&& issue,
-                           const HostPath& host)
+                           const HostPath& host, int persistentComm)
 {
-    const int requestId = tls.nextRequestId++;
-    AsyncRequest r = collectiveRequest(rank);
     cacheDeviceComm(rank);
+    Route route = Route::Host;
     if (device && comm != nullptr) {
         const Placement at = call.staged ? Placement{ false, groupIallreduce }
                                          : placeCollective(*comm, groupIallreduce, call.item.send, call.sendBytes,
                                                            call.item.recv, call.recvBytes, call.shardBytes);
         if (at.grouped) {
-            deferToGroup(call.kind, comm, call.dtype, call.op, call.root, call.item, requestId, std::move(r),
-                         deviceCollectives);
-            return requestId;
+            route = Route::Grouped;
+        } else if (call.direct && (call.staged || at.symmetric || isDevicePointer(call.item.send))) {
+            route = Route::Direct;
         }
-        void* s = tls.cachedStream0;
-        if (call.direct && (call.staged || at.symmetric || isDevicePointer(call.item.send)) &&
-            issueDevice(*comm, s, deviceCollectives, issue)) {
-            return recordDevice(requestId, std::move(r), comm, s);
-        }
+    }
+    if (persistentComm != 0) {
+        PersistentColl p{ route, call.kind, comm, call.dtype, call.op, call.root, call.item, rank, persistentComm };
+        p.direct = [this, comm, issue](void** s) {
+            *s = tls.cachedStream0;
+            return issueDevice(*comm, *s, deviceCollectives, issue);
+        };
+        p.host = host;
+        return addPersistent(std::move(p));
+    }
+    const int requestId = tls.nextRequestId++;
+    AsyncRequest r = collectiveRequest(rank);
+    if (route == Route::Grouped) {
+        deferToGroup(call.kind, comm, call.dtype, call.op, call.root, call.item, requestId, std::move(r),
+                     deviceCollectives);
+        return requestId;
+    }
+    void* s = tls.cachedStream0;
+    if (route == Route::Direct && issueDevice(*comm, s, deviceCollectives, issue)) {
+        return recordDevice(requestId, std::move(r), comm, s);
     }
     host();
     tls.requests[requestId] = std::move(r);
     return requestId;
+}
+
+int MpiWorld::startCheck(int requestId)
+{
+    auto it = tls.requests.find(requestId);
+    if (it == tls.requests.end() || it->second.persistent == nullptr) {
+        return MPI_ERR_REQUEST;
+    }
+    if (it->second.persistent->commFreed) {
+        return MPI_ERR_COMM;
+    }
+    return it->second.persistent->active ? MPI_ERR_REQUEST : MPI_SUCCESS;
+}
+
+int MpiWorld::startPersistent(int requestId)
+{
+    const int rc = startCheck(requestId);
+    if (rc != MPI_SUCCESS) {
+        return rc;
+    }
+    std::shared_ptr<PersistentColl> p = tls.requests[requestId].persistent;
+    cacheDeviceComm(p->rank);
+    AsyncRequest r = collectiveRequest(p->rank);
+    r.persistent = p;
+    p->active = true;
+    if (p->route == Route::Grouped) {
+        deferToGroup(p->kind, p->comm, p->dtype, p->op, p->root, p->item, requestId, std::move(r), deviceCollectives);
+        return MPI_SUCCESS;
+    }
+    void* s = nullptr;
+    if (p->route == Route::Direct && p->direct(&s)) {
+        recordDevice(requestId, std::move(r), p->comm, s);
+        return MPI_SUCCESS;
+    }
+    p->host();
+    tls.requests[requestId] = std::move(r);
+    return MPI_SUCCESS;
+}
+
+bool MpiWorld::persistentInactive(int requestId)
+{
+    auto it = tls.requests.find(requestId);
+    return it != tls.requests.end() && it->second.persistent != nullptr && !it->second.persistent->active;
+}
+
+void MpiWorld::persistentCommFreed(int commId, const DeviceComm& child)
+{
+    for (auto& [id, r] : tls.requests) {
+        if (r.persistent != nullptr && r.persistent->commId == commId) {
+            r.persistent->commFreed = true;
+            // (what the call holds of the communicator goes with it)
+            r.persistent->comm = nullptr;
+            r.persistent->direct = nullptr;
+            r.persistent->host = nullptr;
+        }
+    }
+    if (child != nullptr) {
+        retirePlans([&](const CachedPlan& p) { return p.comm == child.get(); });
+    }
 }
 
 int MpiWorld::iReduceScatter(int rank,
@@ -1689,13 +1936,14 @@ int MpiWorld::iReduceScatter(int rank,
                              uint8_t* recv,
                              faabric_datatype_t* dt,
                              int recvCount,
-                             faabric_op_t* op)
+                             faabric_op_t* op,
+                             int persistentComm)
 {
     checkRanksRange(0, rank);
     cacheDeviceComm(rank);
-    return nbReduceScatter(tls.cachedComm, rank, size, send, recv, dt, recvCount, op, [&] {
+    return nbReduceScatter(tls.cachedComm, rank, size, send, recv, dt, recvCount, op, [=, this] {
         reduceScatter(rank, send, recv, dt, recvCount, op);
-    });
+    }, persistentComm);
 }
 
 int MpiWorld::nbReduceScatter(const DeviceComm& comm,
@@ -1706,7 +1954,7 @@ int MpiWorld::nbReduceScatter(const DeviceComm& comm,
                               faabric_datatype_t* dt,
                               int recvCount,
                               faabric_op_t* op,
-                              const HostPath& host)
+                              const HostPath& host, int persistentComm)
 {
     const size_t shard = (size_t)recvCount * dt->size;
     const int fdt = fbDtypeFor(dt);
@@ -1716,9 +1964,9 @@ int MpiWorld::nbReduceScatter(const DeviceComm& comm,
     const NbCall call{ shard * members, shard, shard, faabric::device::Communicator::GROUP_REDUCE_SCATTER, fdt, fop, 0,
                        { send, recv, (size_t)recvCount } };
     const bool device = shard > 0 && deviceReducible(dt, op) && send != recv;
-    return nbCollective(comm, rank, device, call, [&](auto& c, cudaStream_t st) {
+    return nbCollective(comm, rank, device, call, [=](auto& c, cudaStream_t st) {
         return c.reduceScatter(send, recv, (size_t)recvCount, fdt, fop, symFlag(c, send, shard * members), st);
-    }, host);
+    }, host, persistentComm);
 }
 
 int MpiWorld::iAllGather(int rank,
@@ -1727,13 +1975,14 @@ int MpiWorld::iAllGather(int rank,
                          int sendCount,
                          uint8_t* recv,
                          faabric_datatype_t* recvType,
-                         int recvCount)
+                         int recvCount,
+                         int persistentComm)
 {
     checkRanksRange(0, rank);
     cacheDeviceComm(rank);
-    return nbAllGather(tls.cachedComm, rank, size, send, recv, (size_t)sendCount * sendType->size, [&] {
+    return nbAllGather(tls.cachedComm, rank, size, send, recv, (size_t)sendCount * sendType->size, [=, this] {
         allGather(rank, send, sendType, sendCount, recv, recvType, recvCount);
-    });
+    }, persistentComm);
 }
 
 int MpiWorld::nbAllGather(const DeviceComm& comm,
@@ -1742,35 +1991,35 @@ int MpiWorld::nbAllGather(const DeviceComm& comm,
                           const uint8_t* send,
                           uint8_t* recv,
                           size_t bytes,
-                          const HostPath& host)
+                          const HostPath& host, int persistentComm)
 {
     // a byte copy: the burst's key is the communicator alone.  In place, only
     // the burst runs it on the device.
     NbCall call{ bytes, bytes * members, bytes, faabric::device::Communicator::GROUP_ALLGATHER, FB_U8, -1, 0,
                  { send, recv, bytes } };
     call.direct = comm == nullptr || send != recv + (size_t)comm->rank() * bytes;
-    return nbCollective(comm, rank, bytes > 0, call, [&](auto& c, cudaStream_t st) {
+    return nbCollective(comm, rank, bytes > 0, call, [=](auto& c, cudaStream_t st) {
         return c.allGather(send, recv, bytes, symFlag(c, send, bytes), st);
-    }, host);
+    }, host, persistentComm);
 }
 
-int MpiWorld::iBroadcast(int rank, int root, uint8_t* buffer, faabric_datatype_t* dt, int count)
+int MpiWorld::iBroadcast(int rank, int root, uint8_t* buffer, faabric_datatype_t* dt, int count, int persistentComm)
 {
     checkRanksRange(0, rank);
     cacheDeviceComm(rank);
-    return nbBroadcast(tls.cachedComm, rank, root, buffer, (size_t)count * dt->size, [&] {
+    return nbBroadcast(tls.cachedComm, rank, root, buffer, (size_t)count * dt->size, [=, this] {
         broadcast(root, rank, buffer, dt, count, MpiMessageType::BROADCAST);
-    });
+    }, persistentComm);
 }
 
-int MpiWorld::nbBroadcast(const DeviceComm& comm, int rank, int root, uint8_t* buffer, size_t bytes, const HostPath& host)
+int MpiWorld::nbBroadcast(const DeviceComm& comm, int rank, int root, uint8_t* buffer, size_t bytes, const HostPath& host, int persistentComm)
 {
     // a byte copy: the burst's key is (communicator, root)
     const NbCall call{ bytes, bytes, 0, faabric::device::Communicator::GROUP_BROADCAST, FB_U8, -1, root,
                        { buffer, buffer, bytes } };
-    return nbCollective(comm, rank, bytes > 0, call, [&](auto& c, cudaStream_t st) {
+    return nbCollective(comm, rank, bytes > 0, call, [=](auto& c, cudaStream_t st) {
         return c.broadcast(buffer, bytes, root, symFlag(c, buffer, bytes), st);
-    }, host);
+    }, host, persistentComm);
 }
 
 int MpiWorld::iAllToAll(int rank,
@@ -1779,13 +2028,14 @@ int MpiWorld::iAllToAll(int rank,
                         int sendCount,
                         uint8_t* recv,
                         faabric_datatype_t* recvType,
-                        int recvCount)
+                        int recvCount,
+                        int persistentComm)
 {
     checkRanksRange(0, rank);
     cacheDeviceComm(rank);
-    return nbAllToAll(tls.cachedComm, rank, size, send, recv, (size_t)sendCount * sendType->size, [&] {
+    return nbAllToAll(tls.cachedComm, rank, size, send, recv, (size_t)sendCount * sendType->size, [=, this] {
         allToAll(rank, send, sendType, sendCount, recv, recvType, recvCount);
-    });
+    }, persistentComm);
 }
 
 int MpiWorld::nbAllToAll(const DeviceComm& comm,
@@ -1794,32 +2044,32 @@ int MpiWorld::nbAllToAll(const DeviceComm& comm,
                          const uint8_t* send,
                          uint8_t* recv,
                          size_t bytes,
-                         const HostPath& host)
+                         const HostPath& host, int persistentComm)
 {
     // a byte copy: the burst's key is the communicator alone
     const size_t total = bytes * (size_t)members;
     const NbCall call{ total, total, bytes, faabric::device::Communicator::GROUP_ALLTOALL, FB_U8, -1, 0,
                        { send, recv, bytes } };
-    return nbCollective(comm, rank, bytes > 0, call, [&](auto& c, cudaStream_t st) {
+    return nbCollective(comm, rank, bytes > 0, call, [=](auto& c, cudaStream_t st) {
         return c.allToAll(send, recv, bytes, symFlag(c, send, total), st);
-    }, host);
+    }, host, persistentComm);
 }
 
 int MpiWorld::iGather(int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes, faabric_datatype_t* sendType,
-                      int sendCount, faabric_datatype_t* recvType, int recvCount)
+                      int sendCount, faabric_datatype_t* recvType, int recvCount, int persistentComm)
 {
     checkRanksRange(rank, root);
     cacheDeviceComm(rank);
     // (the blocking call takes the root's in-place send as recv itself)
     const bool inPlace = rank == root && send == recv + (size_t)root * bytes;
     const DeviceComm dev = bytes > 0 && isDevicePointer(send) ? tls.cachedComm : nullptr;
-    return nbGather(dev, rank, root, send, recv, bytes, [&] {
+    return nbGather(dev, rank, root, send, recv, bytes, [=, this] {
         gather(rank, root, inPlace ? recv : send, sendType, sendCount, recv, recvType, recvCount);
-    });
+    }, persistentComm);
 }
 
 int MpiWorld::nbGather(const DeviceComm& comm, int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes,
-                       const HostPath& host)
+                       const HostPath& host, int persistentComm)
 {
     // a byte copy through the staging buffers: the burst's key is
     // (communicator, root).  The caller passes `comm` only for a device
@@ -1827,47 +2077,47 @@ int MpiWorld::nbGather(const DeviceComm& comm, int rank, int root, const uint8_t
     NbCall call{ bytes, bytes, bytes, faabric::device::Communicator::GROUP_GATHER, FB_U8, -1, root,
                  { send, recv, bytes } };
     call.staged = true;
-    return nbCollective(comm, rank, bytes > 0, call, [&](auto& c, cudaStream_t st) {
+    return nbCollective(comm, rank, bytes > 0, call, [=](auto& c, cudaStream_t st) {
         return c.gather(send, recv, bytes, root, 0, st);
-    }, host);
+    }, host, persistentComm);
 }
 
 int MpiWorld::iScatter(int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes, faabric_datatype_t* sendType,
-                       int sendCount, faabric_datatype_t* recvType, int recvCount)
+                       int sendCount, faabric_datatype_t* recvType, int recvCount, int persistentComm)
 {
     checkRanksRange(root, rank);
     cacheDeviceComm(rank);
     const DeviceComm dev = bytes > 0 && isDevicePointer(recv) ? tls.cachedComm : nullptr;
-    return nbScatter(dev, rank, root, send, recv, bytes, [&] {
+    return nbScatter(dev, rank, root, send, recv, bytes, [=, this] {
         scatter(root, rank, send, sendType, sendCount, recv, recvType, recvCount);
-    });
+    }, persistentComm);
 }
 
 int MpiWorld::nbScatter(const DeviceComm& comm, int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes,
-                        const HostPath& host)
+                        const HostPath& host, int persistentComm)
 {
     // the mirror of nbGather: `comm` only for a device recv
     NbCall call{ bytes, bytes, bytes, faabric::device::Communicator::GROUP_SCATTER, FB_U8, -1, root,
                  { send, recv, bytes } };
     call.staged = true;
-    return nbCollective(comm, rank, bytes > 0, call, [&](auto& c, cudaStream_t st) {
+    return nbCollective(comm, rank, bytes > 0, call, [=](auto& c, cudaStream_t st) {
         return c.scatter(send, recv, bytes, root, 0, st);
-    }, host);
+    }, host, persistentComm);
 }
 
 int MpiWorld::iReduce(int rank, int root, const uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count,
-                      faabric_op_t* op)
+                      faabric_op_t* op, int persistentComm)
 {
     checkRanksRange(rank, root);
     cacheDeviceComm(rank);
     const DeviceComm dev = count > 0 && isDevicePointer(send) && deviceReducible(dt, op) ? tls.cachedComm : nullptr;
-    return nbReduce(dev, rank, root, send, recv, dt, count, op, [&] {
+    return nbReduce(dev, rank, root, send, recv, dt, count, op, [=, this] {
         reduce(rank, root, const_cast<uint8_t*>(send), recv, dt, count, op);
-    });
+    }, persistentComm);
 }
 
 int MpiWorld::nbReduce(const DeviceComm& comm, int rank, int root, const uint8_t* send, uint8_t* recv,
-                       faabric_datatype_t* dt, int count, faabric_op_t* op, const HostPath& host)
+                       faabric_datatype_t* dt, int count, faabric_op_t* op, const HostPath& host, int persistentComm)
 {
     // staged like the gather: the burst's key is (communicator, dtype, op,
     // root)
@@ -1877,28 +2127,28 @@ int MpiWorld::nbReduce(const DeviceComm& comm, int rank, int root, const uint8_t
     NbCall call{ bytes, bytes, bytes, faabric::device::Communicator::GROUP_REDUCE, fdt, fop, root,
                  { send, recv, (size_t)count } };
     call.staged = true;
-    return nbCollective(comm, rank, bytes > 0, call, [&](auto& c, cudaStream_t st) {
+    return nbCollective(comm, rank, bytes > 0, call, [=](auto& c, cudaStream_t st) {
         return c.reduce(send, recv, (size_t)count, fdt, fop, root, 0, st);
-    }, host);
+    }, host, persistentComm);
 }
 
 int MpiWorld::iScan(int rank, bool exclusive, const uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int count,
-                    faabric_op_t* op)
+                    faabric_op_t* op, int persistentComm)
 {
     checkRanksRange(0, rank);
     cacheDeviceComm(rank);
     const DeviceComm dev = count > 0 && isDevicePointer(send) && deviceReducible(dt, op) ? tls.cachedComm : nullptr;
-    return nbScan(dev, rank, exclusive, send, recv, dt, count, op, [&] {
+    return nbScan(dev, rank, exclusive, send, recv, dt, count, op, [=, this] {
         if (exclusive) {
             exscan(rank, send, recv, dt, count, op);
         } else {
             scan(rank, const_cast<uint8_t*>(send), recv, dt, count, op);
         }
-    });
+    }, persistentComm);
 }
 
 int MpiWorld::nbScan(const DeviceComm& comm, int rank, bool exclusive, const uint8_t* send, uint8_t* recv,
-                     faabric_datatype_t* dt, int count, faabric_op_t* op, const HostPath& host)
+                     faabric_datatype_t* dt, int count, faabric_op_t* op, const HostPath& host, int persistentComm)
 {
     // staged like the reduce: the burst's key is (kind, communicator, dtype,
     // op), and in place is each rank's own affair.  At issue (grouping off)
@@ -1911,9 +2161,9 @@ int MpiWorld::nbScan(const DeviceComm& comm, int rank, bool exclusive, const uin
       exclusive ? faabric::device::Communicator::GROUP_EXSCAN : faabric::device::Communicator::GROUP_SCAN;
     NbCall call{ bytes, bytes, bytes, kind, fdt, fop, 0, { send, recv, (size_t)count } };
     call.staged = true;
-    return nbCollective(comm, rank, bytes > 0, call, [&](auto& c, cudaStream_t st) {
+    return nbCollective(comm, rank, bytes > 0, call, [=](auto& c, cudaStream_t st) {
         return c.groupMany(kind, &call.item, 1, fdt, fop, 0, 0, st);
-    }, host);
+    }, host, persistentComm);
 }
 
 void MpiWorld::settleDeviceBurst(const DeviceComm& comm)

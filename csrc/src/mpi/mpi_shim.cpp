@@ -428,7 +428,10 @@ int MPI_Wait(MPI_Request* request, MPI_Status* status)
     }
     int id = (*request)->id;
     SPDLOG_TRACE("MPI - MPI_Wait {}", id);
-    getExecutingWorld().awaitAsyncRequest(id);
+    if (getExecutingWorld().awaitAsyncRequest(id)) {
+        // a persistent request stays, inactive
+        return MPI_SUCCESS;
+    }
     requestTable().erase(id);
     delete *request;
     *request = nullptr;
@@ -446,9 +449,9 @@ int MPI_Waitall(int count, MPI_Request array_of_requests[], MPI_Status* array_of
 int MPI_Waitany(int count, MPI_Request array_of_requests[], int* index, MPI_Status* status)
 {
     // Completion is in posting order per pair, so the first live request is
-    // as good a choice as any
+    // as good a choice as any (inactive persistent requests are not live)
     for (int i = 0; i < count; i++) {
-        if (array_of_requests[i] != nullptr) {
+        if (array_of_requests[i] != nullptr && !getExecutingWorld().persistentInactive(array_of_requests[i]->id)) {
             MPI_Wait(&array_of_requests[i], status);
             *index = i;
             return MPI_SUCCESS;
@@ -461,7 +464,10 @@ int MPI_Waitany(int count, MPI_Request array_of_requests[], int* index, MPI_Stat
 int MPI_Request_free(MPI_Request* request)
 {
     if (request != nullptr && *request != nullptr) {
-        getExecutingWorld().freeAsyncRequest((*request)->id);
+        const int rc = getExecutingWorld().freeAsyncRequest((*request)->id);
+        if (rc != MPI_SUCCESS) {
+            return rc;
+        }
         requestTable().erase((*request)->id);
         delete *request;
         *request = nullptr;
@@ -937,7 +943,7 @@ static int handOut(int id, MPI_Request* request)
 // the child device communicator; without one (host buffers, or no agreed
 // slot) the host path completes them at issue.  The child is looked up only
 // for device buffers: its slot agreement is collective.
-int MPI_Iallreduce(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, MPI_Comm comm, MPI_Request* request)
+static int iAllreduceCall(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, MPI_Comm comm, MPI_Request* request, int persistentComm)
 {
     SPDLOG_TRACE("MPI - MPI_Iallreduce");
     if (refusedReduction(op, datatype)) {
@@ -950,12 +956,17 @@ int MPI_Iallreduce(const void* sendbuf, void* recvbuf, int count, MPI_Datatype d
         auto dev = count > 0 && MpiWorld::isDevicePointer(send) && MpiWorld::deviceReducible(datatype, op)
                      ? sub->deviceComm(world, rank)
                      : nullptr;
-        return handOut(world.nbAllReduce(dev, rank, send, (uint8_t*)recvbuf, datatype, count, op, [&] {
+        return handOut(world.nbAllReduce(dev, rank, send, (uint8_t*)recvbuf, datatype, count, op, [=, &world] {
             sub->allReduce(world, rank, send, (uint8_t*)recvbuf, datatype, count, op);
-        }),
+        }, persistentComm),
                        request);
     }
-    return handOut(world.iAllReduce(rank, (uint8_t*)send, (uint8_t*)recvbuf, datatype, count, op), request);
+    return handOut(world.iAllReduce(rank, (uint8_t*)send, (uint8_t*)recvbuf, datatype, count, op, persistentComm), request);
+}
+
+int MPI_Iallreduce(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, MPI_Comm comm, MPI_Request* request)
+{
+    return iAllreduceCall(sendbuf, recvbuf, count, datatype, op, comm, request, 0);
 }
 
 int MPI_Reduce_scatter_block(const void* sendbuf, void* recvbuf, int recvcount, MPI_Datatype datatype,
@@ -975,8 +986,8 @@ int MPI_Reduce_scatter_block(const void* sendbuf, void* recvbuf, int recvcount, 
     return MPI_SUCCESS;
 }
 
-int MPI_Ireduce_scatter_block(const void* sendbuf, void* recvbuf, int recvcount, MPI_Datatype datatype,
-                              MPI_Op op, MPI_Comm comm, MPI_Request* request)
+static int iReduceScatterBlockCall(const void* sendbuf, void* recvbuf, int recvcount, MPI_Datatype datatype,
+                              MPI_Op op, MPI_Comm comm, MPI_Request* request, int persistentComm)
 {
     SPDLOG_TRACE("MPI - MPI_Ireduce_scatter_block");
     if (refusedReduction(op, datatype)) {
@@ -989,16 +1000,22 @@ int MPI_Ireduce_scatter_block(const void* sendbuf, void* recvbuf, int recvcount,
         auto dev = recvcount > 0 && MpiWorld::isDevicePointer(send) && MpiWorld::deviceReducible(datatype, op)
                      ? sub->deviceComm(world, rank)
                      : nullptr;
-        return handOut(world.nbReduceScatter(dev, rank, sub->size(), send, (uint8_t*)recvbuf, datatype, recvcount, op, [&] {
+        return handOut(world.nbReduceScatter(dev, rank, sub->size(), send, (uint8_t*)recvbuf, datatype, recvcount, op, [=, &world] {
             sub->reduceScatter(world, rank, send, (uint8_t*)recvbuf, datatype, recvcount, op);
-        }),
+        }, persistentComm),
                        request);
     }
-    return handOut(world.iReduceScatter(rank, (uint8_t*)send, (uint8_t*)recvbuf, datatype, recvcount, op), request);
+    return handOut(world.iReduceScatter(rank, (uint8_t*)send, (uint8_t*)recvbuf, datatype, recvcount, op, persistentComm), request);
 }
 
-int MPI_Iallgather(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
-                   MPI_Datatype recvtype, MPI_Comm comm, MPI_Request* request)
+int MPI_Ireduce_scatter_block(const void* sendbuf, void* recvbuf, int recvcount, MPI_Datatype datatype,
+                              MPI_Op op, MPI_Comm comm, MPI_Request* request)
+{
+    return iReduceScatterBlockCall(sendbuf, recvbuf, recvcount, datatype, op, comm, request, 0);
+}
+
+static int iAllgatherCall(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                   MPI_Datatype recvtype, MPI_Comm comm, MPI_Request* request, int persistentComm)
 {
     SPDLOG_TRACE("MPI - MPI_Iallgather");
     MpiWorld& world = getExecutingWorld();
@@ -1014,15 +1031,21 @@ int MPI_Iallgather(const void* sendbuf, int sendcount, MPI_Datatype sendtype, vo
     if (sub != nullptr) {
         const size_t bytes = (size_t)sendcount * sendtype->size;
         auto dev = bytes > 0 && MpiWorld::isDevicePointer(send) ? sub->deviceComm(world, rank) : nullptr;
-        return handOut(world.nbAllGather(dev, rank, sub->size(), send, (uint8_t*)recvbuf, bytes, [&] {
+        return handOut(world.nbAllGather(dev, rank, sub->size(), send, (uint8_t*)recvbuf, bytes, [=, &world] {
             sub->allGather(world, rank, send, (uint8_t*)recvbuf, recvtype, recvcount);
-        }),
+        }, persistentComm),
                        request);
     }
-    return handOut(world.iAllGather(rank, send, sendtype, sendcount, (uint8_t*)recvbuf, recvtype, recvcount), request);
+    return handOut(world.iAllGather(rank, send, sendtype, sendcount, (uint8_t*)recvbuf, recvtype, recvcount, persistentComm), request);
 }
 
-int MPI_Ibcast(void* buffer, int count, MPI_Datatype datatype, int root, MPI_Comm comm, MPI_Request* request)
+int MPI_Iallgather(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                   MPI_Datatype recvtype, MPI_Comm comm, MPI_Request* request)
+{
+    return iAllgatherCall(sendbuf, sendcount, sendtype, recvbuf, recvcount, recvtype, comm, request, 0);
+}
+
+static int iBcastCall(void* buffer, int count, MPI_Datatype datatype, int root, MPI_Comm comm, MPI_Request* request, int persistentComm)
 {
     SPDLOG_TRACE("MPI - MPI_Ibcast {} -> all", root);
     MpiWorld& world = getExecutingWorld();
@@ -1034,16 +1057,21 @@ int MPI_Ibcast(void* buffer, int count, MPI_Datatype datatype, int root, MPI_Com
     if (sub != nullptr) {
         const size_t bytes = (size_t)count * datatype->size;
         auto dev = bytes > 0 && MpiWorld::isDevicePointer(buffer) ? sub->deviceComm(world, rank) : nullptr;
-        return handOut(world.nbBroadcast(dev, rank, root, (uint8_t*)buffer, bytes, [&] {
+        return handOut(world.nbBroadcast(dev, rank, root, (uint8_t*)buffer, bytes, [=, &world] {
             sub->broadcast(world, rank, root, (uint8_t*)buffer, datatype, count);
-        }),
+        }, persistentComm),
                        request);
     }
-    return handOut(world.iBroadcast(rank, root, (uint8_t*)buffer, datatype, count), request);
+    return handOut(world.iBroadcast(rank, root, (uint8_t*)buffer, datatype, count, persistentComm), request);
 }
 
-int MPI_Ialltoall(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
-                  MPI_Datatype recvtype, MPI_Comm comm, MPI_Request* request)
+int MPI_Ibcast(void* buffer, int count, MPI_Datatype datatype, int root, MPI_Comm comm, MPI_Request* request)
+{
+    return iBcastCall(buffer, count, datatype, root, comm, request, 0);
+}
+
+static int iAlltoallCall(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                  MPI_Datatype recvtype, MPI_Comm comm, MPI_Request* request, int persistentComm)
 {
     SPDLOG_TRACE("MPI - MPI_Ialltoall");
     if (sendbuf == MPI_IN_PLACE || (size_t)sendcount * sendtype->size != (size_t)recvcount * recvtype->size) {
@@ -1055,17 +1083,23 @@ int MPI_Ialltoall(const void* sendbuf, int sendcount, MPI_Datatype sendtype, voi
     if (auto sub = subOf(comm)) {
         const size_t bytes = (size_t)sendcount * sendtype->size;
         auto dev = bytes > 0 && MpiWorld::isDevicePointer(send) ? sub->deviceComm(world, rank) : nullptr;
-        return handOut(world.nbAllToAll(dev, rank, sub->size(), send, (uint8_t*)recvbuf, bytes, [&] {
+        return handOut(world.nbAllToAll(dev, rank, sub->size(), send, (uint8_t*)recvbuf, bytes, [=, &world] {
             sub->allToAll(world, rank, send, (uint8_t*)recvbuf, sendtype, sendcount);
-        }),
+        }, persistentComm),
                        request);
     }
-    return handOut(world.iAllToAll(rank, (uint8_t*)send, sendtype, sendcount, (uint8_t*)recvbuf, recvtype, recvcount),
+    return handOut(world.iAllToAll(rank, (uint8_t*)send, sendtype, sendcount, (uint8_t*)recvbuf, recvtype, recvcount, persistentComm),
                    request);
 }
 
-int MPI_Igather(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
-                MPI_Datatype recvtype, int root, MPI_Comm comm, MPI_Request* request)
+int MPI_Ialltoall(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                  MPI_Datatype recvtype, MPI_Comm comm, MPI_Request* request)
+{
+    return iAlltoallCall(sendbuf, sendcount, sendtype, recvbuf, recvcount, recvtype, comm, request, 0);
+}
+
+static int iGatherCall(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                MPI_Datatype recvtype, int root, MPI_Comm comm, MPI_Request* request, int persistentComm)
 {
     SPDLOG_TRACE("MPI - MPI_Igather all -> {}", root);
     MpiWorld& world = getExecutingWorld();
@@ -1083,19 +1117,25 @@ int MPI_Igather(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void*
     const uint8_t* send = inPlace ? recv + (size_t)root * bytes : (const uint8_t*)sendbuf;
     if (sub != nullptr) {
         auto dev = bytes > 0 && MpiWorld::isDevicePointer(send) ? sub->deviceComm(world, rank) : nullptr;
-        return handOut(world.nbGather(dev, rank, root, send, recv, bytes, [&] {
+        return handOut(world.nbGather(dev, rank, root, send, recv, bytes, [=, &world] {
             sub->gather(world, rank, root, inPlace ? nullptr : send, recv, isRoot ? recvtype : sendtype,
                         isRoot ? recvcount : sendcount);
-        }),
+        }, persistentComm),
                        request);
     }
     return handOut(world.iGather(rank, root, send, recv, bytes, inPlace ? recvtype : sendtype,
-                                 inPlace ? recvcount : sendcount, recvtype, recvcount),
+                                 inPlace ? recvcount : sendcount, recvtype, recvcount, persistentComm),
                    request);
 }
 
-int MPI_Iscatter(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
-                 MPI_Datatype recvtype, int root, MPI_Comm comm, MPI_Request* request)
+int MPI_Igather(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                MPI_Datatype recvtype, int root, MPI_Comm comm, MPI_Request* request)
+{
+    return iGatherCall(sendbuf, sendcount, sendtype, recvbuf, recvcount, recvtype, root, comm, request, 0);
+}
+
+static int iScatterCall(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                 MPI_Datatype recvtype, int root, MPI_Comm comm, MPI_Request* request, int persistentComm)
 {
     SPDLOG_TRACE("MPI - MPI_Iscatter {} -> all", root);
     MpiWorld& world = getExecutingWorld();
@@ -1112,19 +1152,25 @@ int MPI_Iscatter(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void
     uint8_t* recv = inPlace ? const_cast<uint8_t*>(send) + (size_t)root * bytes : (uint8_t*)recvbuf;
     if (sub != nullptr) {
         auto dev = bytes > 0 && MpiWorld::isDevicePointer(recv) ? sub->deviceComm(world, rank) : nullptr;
-        return handOut(world.nbScatter(dev, rank, root, send, recv, bytes, [&] {
+        return handOut(world.nbScatter(dev, rank, root, send, recv, bytes, [=, &world] {
             sub->scatter(world, rank, root, send, inPlace ? nullptr : recv, isRoot ? sendtype : recvtype,
                          isRoot ? sendcount : recvcount);
-        }),
+        }, persistentComm),
                        request);
     }
     return handOut(world.iScatter(rank, root, send, recv, bytes, sendtype, sendcount, inPlace ? sendtype : recvtype,
-                                  inPlace ? sendcount : recvcount),
+                                  inPlace ? sendcount : recvcount, persistentComm),
                    request);
 }
 
-int MPI_Ireduce(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, int root,
-                MPI_Comm comm, MPI_Request* request)
+int MPI_Iscatter(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                 MPI_Datatype recvtype, int root, MPI_Comm comm, MPI_Request* request)
+{
+    return iScatterCall(sendbuf, sendcount, sendtype, recvbuf, recvcount, recvtype, root, comm, request, 0);
+}
+
+static int iReduceCall(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, int root,
+                MPI_Comm comm, MPI_Request* request, int persistentComm)
 {
     SPDLOG_TRACE("MPI - MPI_Ireduce all -> {}", root);
     if (refusedReduction(op, datatype)) {
@@ -1141,18 +1187,24 @@ int MPI_Ireduce(const void* sendbuf, void* recvbuf, int count, MPI_Datatype data
         auto dev = count > 0 && MpiWorld::isDevicePointer(send) && MpiWorld::deviceReducible(datatype, op)
                      ? sub->deviceComm(world, rank)
                      : nullptr;
-        return handOut(world.nbReduce(dev, rank, root, send, (uint8_t*)recvbuf, datatype, count, op, [&] {
+        return handOut(world.nbReduce(dev, rank, root, send, (uint8_t*)recvbuf, datatype, count, op, [=, &world] {
             sub->reduce(world, rank, root, send, (uint8_t*)recvbuf, datatype, count, op);
-        }),
+        }, persistentComm),
                        request);
     }
-    return handOut(world.iReduce(rank, root, send, (uint8_t*)recvbuf, datatype, count, op), request);
+    return handOut(world.iReduce(rank, root, send, (uint8_t*)recvbuf, datatype, count, op, persistentComm), request);
+}
+
+int MPI_Ireduce(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, int root,
+                MPI_Comm comm, MPI_Request* request)
+{
+    return iReduceCall(sendbuf, recvbuf, count, datatype, op, root, comm, request, 0);
 }
 
 // MPI_Iscan and MPI_Iexscan.  The device or host choice rests on the send
 // (the recv when in place), which every rank judges alike.
 static int iScanCall(bool exclusive, const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op,
-                     MPI_Comm comm, MPI_Request* request)
+                     MPI_Comm comm, MPI_Request* request, int persistentComm = 0)
 {
     if (refusedReduction(op, datatype)) {
         return MPI_ERR_OP;
@@ -1164,16 +1216,16 @@ static int iScanCall(bool exclusive, const void* sendbuf, void* recvbuf, int cou
         auto dev = count > 0 && MpiWorld::isDevicePointer(send) && MpiWorld::deviceReducible(datatype, op)
                      ? sub->deviceComm(world, rank)
                      : nullptr;
-        return handOut(world.nbScan(dev, rank, exclusive, send, (uint8_t*)recvbuf, datatype, count, op, [&] {
+        return handOut(world.nbScan(dev, rank, exclusive, send, (uint8_t*)recvbuf, datatype, count, op, [=, &world] {
             if (exclusive) {
                 sub->exscan(world, rank, send, (uint8_t*)recvbuf, datatype, count, op);
             } else {
                 sub->scan(world, rank, send, (uint8_t*)recvbuf, datatype, count, op);
             }
-        }),
+        }, persistentComm),
                        request);
     }
-    return handOut(world.iScan(rank, exclusive, send, (uint8_t*)recvbuf, datatype, count, op), request);
+    return handOut(world.iScan(rank, exclusive, send, (uint8_t*)recvbuf, datatype, count, op, persistentComm), request);
 }
 
 int MPI_Iscan(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, MPI_Comm comm,
@@ -1188,6 +1240,109 @@ int MPI_Iexscan(const void* sendbuf, void* recvbuf, int count, MPI_Datatype data
 {
     SPDLOG_TRACE("MPI - MPI_Iexscan");
     return iScanCall(true, sendbuf, recvbuf, count, datatype, op, comm, request);
+}
+
+// ---- persistent collectives (MPI-4.0): each init validates as the matching
+// non-blocking call and fixes where the call runs; MPI_Start issues it as
+// that call would.  The info argument is accepted and ignored. ----
+// The MPI communicator id a persistent request belongs to
+static int persistentCommOf(MPI_Comm comm)
+{
+    return comm != nullptr ? comm->id : FAABRIC_COMM_WORLD;
+}
+
+int MPI_Allreduce_init(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, MPI_Comm comm,
+                       MPI_Info info, MPI_Request* request)
+{
+    return iAllreduceCall(sendbuf, recvbuf, count, datatype, op, comm, request, persistentCommOf(comm));
+}
+
+int MPI_Reduce_scatter_block_init(const void* sendbuf, void* recvbuf, int recvcount, MPI_Datatype datatype, MPI_Op op,
+                                  MPI_Comm comm, MPI_Info info, MPI_Request* request)
+{
+    return iReduceScatterBlockCall(sendbuf, recvbuf, recvcount, datatype, op, comm, request, persistentCommOf(comm));
+}
+
+int MPI_Allgather_init(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                       MPI_Datatype recvtype, MPI_Comm comm, MPI_Info info, MPI_Request* request)
+{
+    return iAllgatherCall(sendbuf, sendcount, sendtype, recvbuf, recvcount, recvtype, comm, request,
+                          persistentCommOf(comm));
+}
+
+int MPI_Bcast_init(void* buffer, int count, MPI_Datatype datatype, int root, MPI_Comm comm, MPI_Info info,
+                   MPI_Request* request)
+{
+    return iBcastCall(buffer, count, datatype, root, comm, request, persistentCommOf(comm));
+}
+
+int MPI_Alltoall_init(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                      MPI_Datatype recvtype, MPI_Comm comm, MPI_Info info, MPI_Request* request)
+{
+    return iAlltoallCall(sendbuf, sendcount, sendtype, recvbuf, recvcount, recvtype, comm, request,
+                         persistentCommOf(comm));
+}
+
+int MPI_Gather_init(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                    MPI_Datatype recvtype, int root, MPI_Comm comm, MPI_Info info, MPI_Request* request)
+{
+    return iGatherCall(sendbuf, sendcount, sendtype, recvbuf, recvcount, recvtype, root, comm, request,
+                       persistentCommOf(comm));
+}
+
+int MPI_Scatter_init(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                     MPI_Datatype recvtype, int root, MPI_Comm comm, MPI_Info info, MPI_Request* request)
+{
+    return iScatterCall(sendbuf, sendcount, sendtype, recvbuf, recvcount, recvtype, root, comm, request,
+                        persistentCommOf(comm));
+}
+
+int MPI_Reduce_init(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, int root,
+                    MPI_Comm comm, MPI_Info info, MPI_Request* request)
+{
+    return iReduceCall(sendbuf, recvbuf, count, datatype, op, root, comm, request, persistentCommOf(comm));
+}
+
+int MPI_Scan_init(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, MPI_Comm comm,
+                  MPI_Info info, MPI_Request* request)
+{
+    return iScanCall(false, sendbuf, recvbuf, count, datatype, op, comm, request, persistentCommOf(comm));
+}
+
+int MPI_Exscan_init(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, MPI_Comm comm,
+                    MPI_Info info, MPI_Request* request)
+{
+    return iScanCall(true, sendbuf, recvbuf, count, datatype, op, comm, request, persistentCommOf(comm));
+}
+
+int MPI_Start(MPI_Request* request)
+{
+    if (request == nullptr || *request == nullptr) {
+        return MPI_ERR_REQUEST;
+    }
+    return getExecutingWorld().startPersistent((*request)->id);
+}
+
+int MPI_Startall(int count, MPI_Request array_of_requests[])
+{
+    // every request is checked before any is started
+    MpiWorld& world = getExecutingWorld();
+    for (int i = 0; i < count; i++) {
+        if (array_of_requests[i] == nullptr) {
+            return MPI_ERR_REQUEST;
+        }
+        const int rc = world.startCheck(array_of_requests[i]->id);
+        if (rc != MPI_SUCCESS) {
+            return rc;
+        }
+    }
+    for (int i = 0; i < count; i++) {
+        const int rc = world.startPersistent(array_of_requests[i]->id);
+        if (rc != MPI_SUCCESS) {
+            return rc;
+        }
+    }
+    return MPI_SUCCESS;
 }
 
 int MPI_Get_processor_name(char* name, int* resultlen)
@@ -1729,8 +1884,11 @@ int MPI_Comm_free(MPI_Comm* comm)
     if ((*comm)->id != FAABRIC_COMM_WORLD && (*comm)->id != FAABRIC_COMM_NULL) {
         // frees this rank's signal slot of the fused device path
         if (auto sub = getSubCommunicator((*comm)->id)) {
-            // a deferred burst on the child is issued and waited first
-            getExecutingWorld().settleDeviceBurst(sub->currentDevice(executingContext.getRank()));
+            // a deferred burst on the child is issued and waited first; its
+            // persistent requests cannot start again
+            auto child = sub->currentDevice(executingContext.getRank());
+            getExecutingWorld().settleDeviceBurst(child);
+            getExecutingWorld().persistentCommFreed((*comm)->id, child);
             sub->releaseDevice(executingContext.getRank());
         }
         delete *comm;
