@@ -31,6 +31,7 @@
 #include "../tests/mpi_group_alltoall_body.h"
 #include "../tests/mpi_group_reduce_body.h"
 #include "../tests/mpi_group_scan_body.h"
+#include "../tests/mpi_neighbor_body.h"
 #include "../tests/mpi_group_rooted_body.h"
 #include "../tests/mpi_group_subcomm_body.h"
 #include "../tests/mpi_persistent_body.h"
@@ -1232,6 +1233,172 @@ static void registerFunctions()
             msg.set_outputdata(why);
         }
         return rc;
+    });
+
+    // The distributed-graph topology and the neighbourhood collectives on the
+    // world and on a split (mpi_neighbor_body.h)
+    mpiFunction("neighbor-coll", [](int rank, int size, faabric::Message& msg) {
+        std::string why;
+        int rc = neighbor_coll::body(rank, size, msg.mpiworldid(), true, &why);
+        if (rc != 0) {
+            SPDLOG_ERROR("neighbor-coll: {}", why);
+            msg.set_outputdata(why);
+        }
+        return rc;
+    });
+
+    // A neighbourhood exchange of `fields` fp32 fields per step over the
+    // world, in device memory (MPI_Alloc_mem).  Input: "<mode>;<steps>;
+    // <graph>;<block bytes>;<fields>" with graph "halo" (periodic 4-neighbour
+    // grid of 2x1, 2x2 or 4x2 ranks: left, right, down, up) or "ring" (each
+    // rank sends to the next), and mode
+    //   p2p       per field an MPI_Isend per out-edge and an MPI_Irecv per
+    //             in-edge, one MPI_Waitall per step (self-edges: a device copy)
+    //   blocking  one MPI_Neighbor_alltoall per field
+    //   burst     one MPI_Ineighbor_alltoall per field + MPI_Waitall
+    // Rank 0 reports {"ms_per_step", "launches_per_step"}: the launches on
+    // its world device communicator and on the graph's child.  Every rank
+    // checks the first and last word of every received block.
+    mpiFunction("bench-neighbor", [](int rank, int size, faabric::Message& msg) {
+        std::vector<std::string> f;
+        std::string cur;
+        for (char c : msg.inputdata() + ";") {
+            if (c == ';') {
+                f.push_back(cur);
+                cur.clear();
+            } else {
+                cur += c;
+            }
+        }
+        EXPECT(f.size() >= 5 && size >= 2);
+        const std::string mode = f[0];
+        const int steps = std::stoi(f[1]);
+        const size_t block = std::stoull(f[3]);
+        const int fields = std::stoi(f[4]);
+        const int words = (int)(block / 4);
+        std::vector<int> src, dst;
+        if (f[2] == "halo") {
+            const int px = size == 8 ? 4 : 2;
+            const int py = size / px;
+            const int x = rank % px, y = rank / px;
+            dst = { (x + px - 1) % px + y * px, (x + 1) % px + y * px, x + (y + py - 1) % py * px,
+                    x + (y + 1) % py * px };
+            src = dst;
+        } else {
+            dst = { (rank + 1) % size };
+            src = { (rank + size - 1) % size };
+        }
+        // in-edge j: (source, index of the edge in the source's destinations),
+        // for the check; every rank's lists follow the same rule
+        auto dstOf = [&](int r) {
+            if (f[2] != "halo") {
+                return std::vector<int>{ (r + 1) % size };
+            }
+            const int px = size == 8 ? 4 : 2;
+            const int py = size / px;
+            const int x = r % px, y = r / px;
+            return std::vector<int>{ (x + px - 1) % px + y * px, (x + 1) % px + y * px, x + (y + py - 1) % py * px,
+                                     x + (y + 1) % py * px };
+        };
+        std::vector<std::pair<int, int>> in;
+        std::map<int, int> seen;
+        for (int s : src) {
+            int k = seen[s]++;
+            const auto d = dstOf(s);
+            for (size_t i = 0; i < d.size(); i++) {
+                if (d[i] == rank && k-- == 0) {
+                    in.push_back({ s, (int)i });
+                    break;
+                }
+            }
+        }
+        EXPECT(in.size() == src.size());
+        MPI_Comm graph = MPI_COMM_NULL;
+        EXPECT(MPI_Dist_graph_create_adjacent(MPI_COMM_WORLD, (int)src.size(), src.data(), MPI_UNWEIGHTED,
+                                              (int)dst.size(), dst.data(), MPI_UNWEIGHTED, MPI_INFO_NULL, 0,
+                                              &graph) == MPI_SUCCESS);
+        const size_t sendBytes = block * dst.size();
+        const size_t recvBytes = block * src.size();
+        std::vector<uint8_t*> sends(fields), recvs(fields);
+        for (int i = 0; i < fields; i++) {
+            EXPECT(MPI_Alloc_mem(sendBytes, MPI_INFO_FAABRIC_DEVICE, &sends[i]) == MPI_SUCCESS);
+            EXPECT(MPI_Alloc_mem(recvBytes, MPI_INFO_FAABRIC_DEVICE, &recvs[i]) == MPI_SUCCESS);
+            // word w of block b of field i on rank r: r * 1000000 + i * 1000 + b
+            std::vector<int32_t> mine(words * dst.size());
+            for (size_t b = 0; b < dst.size(); b++) {
+                std::fill(mine.begin() + b * words, mine.begin() + (b + 1) * words, rank * 1000000 + i * 1000 + (int)b);
+            }
+            cudaMemcpy(sends[i], mine.data(), sendBytes, cudaMemcpyHostToDevice);
+            cudaMemset(recvs[i], 0xff, recvBytes);
+        }
+        MPI_Barrier(MPI_COMM_WORLD);
+        std::vector<MPI_Request> reqs;
+        auto step = [&]() -> int {
+            reqs.clear();
+            for (int i = 0; i < fields; i++) {
+                if (mode == "p2p") {
+                    for (size_t j = 0; j < in.size(); j++) {
+                        if (in[j].first != rank) {
+                            reqs.emplace_back();
+                            EXPECT(MPI_Irecv(recvs[i] + j * block, words, MPI_FLOAT, in[j].first, i, MPI_COMM_WORLD,
+                                             &reqs.back()) == MPI_SUCCESS);
+                        } else {
+                            cudaMemcpy(recvs[i] + j * block, sends[i] + (size_t)in[j].second * block, block,
+                                       cudaMemcpyDeviceToDevice);
+                        }
+                    }
+                    for (size_t k = 0; k < dst.size(); k++) {
+                        if (dst[k] != rank) {
+                            reqs.emplace_back();
+                            EXPECT(MPI_Isend(sends[i] + k * block, words, MPI_FLOAT, dst[k], i, MPI_COMM_WORLD,
+                                             &reqs.back()) == MPI_SUCCESS);
+                        }
+                    }
+                } else if (mode == "blocking") {
+                    EXPECT(MPI_Neighbor_alltoall(sends[i], words, MPI_FLOAT, recvs[i], words, MPI_FLOAT, graph) ==
+                           MPI_SUCCESS);
+                } else {
+                    reqs.emplace_back();
+                    EXPECT(MPI_Ineighbor_alltoall(sends[i], words, MPI_FLOAT, recvs[i], words, MPI_FLOAT, graph,
+                                                  &reqs.back()) == MPI_SUCCESS);
+                }
+            }
+            EXPECT(MPI_Waitall((int)reqs.size(), reqs.data(), MPI_STATUSES_IGNORE) == MPI_SUCCESS);
+            return 0;
+        };
+        for (int i = 0; i < 3; i++) {
+            EXPECT(step() == 0);
+        }
+        auto worldDev = faabric::mpi::getMpiWorldRegistry().getWorld(msg.mpiworldid()).getDeviceComm(rank);
+        auto launches = [&]() {
+            auto child = faabric::mpi::getSubCommunicator(graph->id)->currentDevice(rank);
+            return (worldDev ? worldDev->stats().launches : 0) + (child ? child->stats().launches : 0);
+        };
+        MPI_Barrier(MPI_COMM_WORLD);
+        const uint64_t l0 = launches();
+        auto t0 = std::chrono::steady_clock::now();
+        for (int i = 0; i < steps; i++) {
+            EXPECT(step() == 0);
+        }
+        const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count() / steps;
+        const double perStep = (double)(launches() - l0) / steps;
+        MPI_Barrier(MPI_COMM_WORLD);
+        for (int i = 0; i < fields; i++) {
+            std::vector<int32_t> back(words * src.size());
+            cudaMemcpy(back.data(), recvs[i], recvBytes, cudaMemcpyDeviceToHost);
+            for (size_t j = 0; j < in.size(); j++) {
+                const int32_t want = in[j].first * 1000000 + i * 1000 + in[j].second;
+                EXPECT(back[j * words] == want && back[(j + 1) * words - 1] == want);
+            }
+            MPI_Free_mem(sends[i]);
+            MPI_Free_mem(recvs[i]);
+        }
+        MPI_Comm_free(&graph);
+        if (rank == 0) {
+            msg.set_outputdata("{\"ms_per_step\": " + std::to_string(ms) + ", \"launches_per_step\": " +
+                               std::to_string(perStep) + "}");
+        }
+        return 0;
     });
 
     // A list of tensors prefix-summed over the world per step, in device

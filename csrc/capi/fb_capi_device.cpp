@@ -632,6 +632,24 @@ void fb_group_plan_free(void* plan)
     delete (FbGroupPlanHandle*)plan;
 }
 
+// Communicator::setNeighbors: in-edge j is (srcs[j], idxs[j])
+int fb_comm_set_neighbors(void* h,
+                          int nIn,
+                          const int* srcs,
+                          const int* idxs,
+                          int outDegree,
+                          int maxOutDegree,
+                          int maxInDegree)
+{
+    FB_TRY
+    std::vector<std::pair<int, int>> in((size_t)std::max(nIn, 0));
+    for (int j = 0; j < nIn; j++) {
+        in[j] = { srcs[j], idxs[j] };
+    }
+    return COMM(h)->setNeighbors(in, outDegree, maxOutDegree, maxInDegree);
+    FB_CATCH(FB_E_INVALID)
+}
+
 int fb_put_signal(void* h,
                   const void* local,
                   uint64_t dstOffset,

@@ -313,6 +313,22 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     // send of the group on this rank.  The one exception is the in-place
     // all-gather, send == recv + rank*count*esize.  Items with count 0 are
     // skipped.
+    //   GROUP_NEIGHBOR_ALLGATHER: over the topology of setNeighbors, send
+    //     holds count elements and recv indeg*count; block j of recv gets
+    //     the send of in-edge j's source (MPI_Neighbor_allgather per item)
+    //   GROUP_NEIGHBOR_ALLTOALL: send holds outdeg*count elements and recv
+    //     indeg*count; block j of recv gets block idx of the send of in-edge
+    //     j = (source, idx) (MPI_Neighbor_alltoall per item)
+    //   Both are byte copies of any dtype, with buffers of any device memory
+    //   at any alignment (a rank's send is not read when its out-degree is
+    //   0, nor its recv written when its in-degree is 0; either may then be
+    //   null).  Every rank stages its send blocks, then pulls its in-edges'
+    //   blocks from their sources' staging.  A launch holds at most
+    //   CommConfig::stageBytes of staging per rank (the all-to-all: the
+    //   largest out-degree times the launch's blocks), so a larger list is
+    //   cut into several launches, at the same points on every rank.  A rank
+    //   with no edge still takes part in every launch; a graph with no edge
+    //   launches nothing.
     // Rooted kinds (GROUP_GATHER, GROUP_SCATTER, GROUP_REDUCE, GROUP_SCAN,
     // GROUP_EXSCAN) group every item with count > 0: buffers are any device
     // memory of this rank, at any alignment and length, and may differ
@@ -332,7 +348,9 @@ class Communicator : public std::enable_shared_from_this<Communicator>
         GROUP_SCATTER = 6,
         GROUP_REDUCE = 7,
         GROUP_SCAN = 8,
-        GROUP_EXSCAN = 9
+        GROUP_EXSCAN = 9,
+        GROUP_NEIGHBOR_ALLGATHER = 10,
+        GROUP_NEIGHBOR_ALLTOALL = 11
     };
     // Where the next launch of a list starts: an item, and a byte offset in
     // it (rooted kinds cut items larger than the staging buffer)
@@ -386,6 +404,12 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     //     (any value is accepted), and every rank needs both its send and
     //     its recv.  Every (dtype, op) pair that has a reduction has a grouped
     //     kernel.
+    //   - GROUP_NEIGHBOR_ALLGATHER, GROUP_NEIGHBOR_ALLTOALL: a communicator
+    //     without a topology, a channel other than 0, or a missing buffer
+    //     this rank needs (the send with an out-edge, the recv with an
+    //     in-edge) gives FB_E_INVALID, checked over the whole list before
+    //     its first launch; `op` and `root` are ignored.  On a one-member
+    //     communicator the launch is a local copy.
     //   - GROUP_ALLREDUCE sets lastAlgo() to FB_ALGO_TWOSHOT
     int runGroup(GroupKind kind, const GroupPlan& plan, int op, int root, int flags, cudaStream_t s);
     int groupMany(GroupKind kind,
@@ -398,8 +422,26 @@ class Communicator : public std::enable_shared_from_this<Communicator>
                   cudaStream_t s);
     static size_t groupPlanLaunches(const GroupPlan& plan);
     // "all-reduce", "reduce-scatter", "all-gather", "broadcast", "all-to-all",
-    // "gather", "scatter", "reduce", "scan", "exscan"
+    // "gather", "scatter", "reduce", "scan", "exscan", "neighbor-allgather",
+    // "neighbor-alltoall"
     static const char* groupKindName(GroupKind kind);
+
+    // ---- neighbourhood topology of the neighbour kinds ----
+    // This rank's in-edges in recv-block order, each (source rank, index of
+    // the edge among the source's out-edges), and its out-degree.  The
+    // largest out-degree and in-degree over every member must be passed
+    // alike by every member: the staging layout and the launch cuts follow
+    // from them.  Self-edges and multi-edges are allowed.  Local call, set
+    // once, before the first neighbour call; the caller checks that the
+    // members' edges agree (a source's out-edges are the in-edges naming
+    // it).  FB_E_INVALID for a second call, a source outside the
+    // communicator, an index outside [0, maxOutDegree), a degree above its
+    // maximum, or more than FB_NEIGHBOR_MAX_IN_DEGREE in-edges.
+    int setNeighbors(const std::vector<std::pair<int, int>>& inEdges,
+                     int outDegree,
+                     int maxOutDegree,
+                     int maxInDegree);
+    bool hasNeighbors() const { return topo_ != nullptr; }
 
     // ---- point to point (per-pair FIFO; no kernel ever spins on a peer) ----
     // Operations on one ordered pair must be issued in a consistent stream
@@ -615,6 +657,8 @@ class Communicator : public std::enable_shared_from_this<Communicator>
     std::shared_ptr<LocalGroup> localGroup_;
 
     struct GroupLaunch;
+    struct NeighborTopo;
+    std::shared_ptr<const NeighborTopo> topo_;
 
     // sub-communicators: the child holds its parent and the slot it uses;
     // the parent records which slots are in use on this rank
@@ -643,6 +687,7 @@ class Communicator : public std::enable_shared_from_this<Communicator>
                      int flags,
                      cudaStream_t s);
     int groupCheck(GroupKind kind, int dtype, int op, int root, int flags, bool& grouped) const;
+    int launchNeighbor(const GroupLaunch& l, GroupKind kind, fb::GroupArgs& a, bool ss, int flags, cudaStream_t s);
     int groupBatch(GroupKind kind,
                    const GroupItem* items,
                    size_t nItems,
@@ -683,6 +728,13 @@ class Communicator : public std::enable_shared_from_this<Communicator>
                  int flags,
                  cudaStream_t s);
 };
+
+// Largest in-degree of a neighbour topology.  The in-edges share the
+// FB_GROUP_MAX_SEGS-entry segment table of every launch with the pieces, four
+// edges per entry: up to an in-degree of 32 a launch holds 1016 pieces, at
+// this limit 24, so a list of many items on a high-degree graph takes several
+// launches.  (The MPI layer runs graphs above the limit on its host path.)
+#define FB_NEIGHBOR_MAX_IN_DEGREE 4000
 
 // Error codes
 #define FB_OK 0

@@ -29,6 +29,9 @@ extern "C"
 #define MPI_ERR_REQUEST 8
 /* MPI_Start of a persistent request whose communicator was freed */
 #define MPI_ERR_COMM 9
+/* a neighbourhood call on a communicator without a dist-graph topology, or a
+ * graph whose two sides of an edge disagree */
+#define MPI_ERR_TOPOLOGY 10
 #define MPI_MAX_OBJECT_NAME 128
 
 /* passive-target lock types (MPI_Win_lock) */
@@ -181,6 +184,8 @@ extern "C"
 #define FAABRIC_INFO_NULL 1
 #define FAABRIC_INFO_DEVICE 2
     extern struct faabric_info_t faabric_info_null;
+    extern int faabric_unweighted;
+    extern int faabric_weights_empty;
     extern struct faabric_info_t faabric_info_device;
 #define MPI_INFO_NULL &faabric_info_null
 // Extension: MPI_Alloc_mem with this info allocates from the rank's symmetric
@@ -191,6 +196,11 @@ extern "C"
 #define MPI_UNDEFINED -1
 #define MPI_MAX_PROCESSOR_NAME 256
 #define MPI_CART_MAX_DIMENSIONS 2
+/* MPI_Topo_test: a communicator made by MPI_Dist_graph_create_adjacent */
+#define MPI_DIST_GRAPH 3
+/* weight sentinels of MPI_Dist_graph_create_adjacent (distinct addresses) */
+#define MPI_UNWEIGHTED ((int*)&faabric_unweighted)
+#define MPI_WEIGHTS_EMPTY ((int*)&faabric_weights_empty)
 
     /* ---- reduce operations ---- */
 #define FAABRIC_MPI_OPS(X)                                                     \
@@ -376,6 +386,37 @@ extern "C"
                   MPI_Request* request);
     int MPI_Iexscan(const void* sendbuf, void* recvbuf, int count, MPI_Datatype datatype, MPI_Op op, MPI_Comm comm,
                     MPI_Request* request);
+    /* Distributed-graph topology (MPI-3.1 7.5.4) and neighbourhood
+     * collectives (7.6).  MPI_Dist_graph_create_adjacent is collective over
+     * comm_old (the world or any sub-communicator): every member gathers the
+     * whole graph and checks it alike, so all return MPI_ERR_RANK for a rank
+     * outside comm_old, MPI_ERR_ARG for a negative degree, or
+     * MPI_ERR_TOPOLOGY for an edge s -> d listed a different number of times
+     * in s's destinations and d's sources, with *comm_dist_graph set to
+     * MPI_COMM_NULL.  Self-edges and multi-edges are allowed; info and
+     * reorder are ignored (ranks are those of comm_old). */
+    int MPI_Dist_graph_create_adjacent(MPI_Comm comm_old, int indegree, const int sources[], const int sourceweights[],
+                                       int outdegree, const int destinations[], const int destweights[], MPI_Info info,
+                                       int reorder, MPI_Comm* comm_dist_graph);
+    int MPI_Dist_graph_neighbors_count(MPI_Comm comm, int* indegree, int* outdegree, int* weighted);
+    int MPI_Dist_graph_neighbors(MPI_Comm comm, int maxindegree, int sources[], int sourceweights[], int maxoutdegree,
+                                 int destinations[], int destweights[]);
+    /* MPI_DIST_GRAPH, or MPI_UNDEFINED for every other communicator */
+    int MPI_Topo_test(MPI_Comm comm, int* status);
+    /* Recv block j gets the send of sources[j] (all-gather), or the block of
+     * sources[j]'s send for this rank's edge (all-to-all: send block i goes to
+     * destinations[i]).  A block is recvcount x recvtype bytes.
+     * MPI_IN_PLACE or a send block of another byte size gives MPI_ERR_ARG, a
+     * communicator without a dist-graph topology MPI_ERR_TOPOLOGY, both before
+     * anything is sent or launched. */
+    int MPI_Neighbor_allgather(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                               MPI_Datatype recvtype, MPI_Comm comm);
+    int MPI_Neighbor_alltoall(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                              MPI_Datatype recvtype, MPI_Comm comm);
+    int MPI_Ineighbor_allgather(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf,
+                                int recvcount, MPI_Datatype recvtype, MPI_Comm comm, MPI_Request* request);
+    int MPI_Ineighbor_alltoall(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                               MPI_Datatype recvtype, MPI_Comm comm, MPI_Request* request);
     /* Persistent collectives (MPI-4.0).  Each init call refuses what the
      * matching MPI_I* call refuses, before anything is created, and fixes
      * where the call runs; info is ignored.  A completed start leaves the

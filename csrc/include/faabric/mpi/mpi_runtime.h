@@ -693,6 +693,16 @@ class MpiWorld
     // and deviceReducible(dt, op) holds (judged once, by the caller).
     int nbScan(const DeviceComm& comm, int rank, bool exclusive, const uint8_t* send, uint8_t* recv,
                faabric_datatype_t* dt, int count, faabric_op_t* op, const HostPath& host, int persistentComm = 0);
+    // MPI_Ineighbor_allgather / MPI_Ineighbor_alltoall on a dist-graph
+    // communicator's child (`kind` a neighbour GroupKind): `bytes` per block,
+    // the send and recv sized by this rank's degrees.  Every device call
+    // stages, so device buffers join the burst wherever they live.  `comm`
+    // is null unless the call runs on the device (judged once, by the caller).
+    int nbNeighbor(const DeviceComm& comm, int rank, faabric::device::Communicator::GroupKind kind,
+                   const uint8_t* send, uint8_t* recv, size_t bytes, const HostPath& host);
+    // The blocking call: one grouped launch, waited for (false: no comm)
+    bool deviceNeighbor(const DeviceComm& comm, int rank, faabric::device::Communicator::GroupKind kind,
+                        const uint8_t* send, uint8_t* recv, size_t bytes);
     // Issues this rank thread's pending burst if it is keyed to `comm`, and
     // waits for it (before `comm` is released: MPI_Comm_free)
     void settleDeviceBurst(const DeviceComm& comm);

@@ -67,6 +67,9 @@ cudaError_t preloadAllKernels()
         e = preloadRootedKernels();
     }
     if (e == cudaSuccess) {
+        e = preloadNeighborKernels();
+    }
+    if (e == cudaSuccess) {
         e = preloadMoveBulkKernel();
     }
     if (e == cudaSuccess) {

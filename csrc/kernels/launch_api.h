@@ -96,6 +96,10 @@ struct GroupArgs
     // grouped reduce and scan only: symmetric offset of the staging buffer
     // the results are stored in (the root's, or every rank's own)
     uint64_t stageRecvOff;
+    // neighbour kinds only (see NeighborEdge): this rank's in-edges, which
+    // follow the segments in the table, and the send blocks it stages
+    uint32_t nEdges;
+    uint32_t outDeg;
 };
 
 // vectors per warp-chunk for a world of n ranks (host and kernel must agree)
@@ -198,6 +202,33 @@ static_assert(sizeof(RootedSeg) == sizeof(GroupSeg), "rooted tables use GroupSeg
 #define GROUP_PHASE_UNSTAGE 4
 cudaError_t launchGroupGather(const GroupArgs& a, int blocks, int threads, cudaStream_t stream);
 cudaError_t launchGroupScatter(const GroupArgs& a, int blocks, int threads, cudaStream_t stream);
+
+// ---- grouped neighbourhood all-gather and all-to-all: many
+// MPI_Neighbor_allgather / MPI_Neighbor_alltoall calls, ONE launch ----
+// A staged pull over a fixed graph.  The table holds nSegs RootedSeg pieces
+// (bytes of one block, the same on every rank; stride = the item's block
+// bytes; chunk0 counts the launch's piece chunks, T = totalChunks in all,
+// CB = FB_NEIGHBOR_CHUNK) and then this rank's nEdges in-edges, four
+// NeighborEdge per GroupSeg slot.  Staging holds slots of T chunks: piece
+// chunk g of slot k is chunk k * T + g.
+//   LOCAL: all-to-all: send block k goes to slot k, k < outDeg; all-gather:
+//          the send goes to slot 0 when outDeg > 0.
+//   entry barrier
+//   MOVE:  in-edge j = (src, idx) fills recv block j from src's slot idx
+//          (all-gather: slot 0).  One rank: straight from its send, no
+//          staging and no barrier.
+//   exit barrier
+// With noSync the launch runs the steps of `phase` with no barrier.
+#define FB_NEIGHBOR_CHUNK 2048
+struct NeighborEdge
+{
+    uint32_t src; // source rank
+    uint32_t idx; // this edge's index among the source's out-edges
+};
+// GroupSeg slots of n in-edges (a macro: the kernel needs it too)
+#define FB_NEIGHBOR_EDGE_SLOTS(n) (((uint32_t)(n) + 3u) / 4u)
+cudaError_t launchGroupNeighbor(const GroupArgs& a, bool allToAll, int blocks, int threads, cudaStream_t stream);
+cudaError_t preloadNeighborKernels();
 
 struct ReduceLaunchers
 {

@@ -1250,6 +1250,7 @@ const fb::KernelTable CUDA_KERNELS = {
     .groupScatter = fb::launchGroupScatter,
     .groupReduce = cudaGroupReduce,
     .groupScan = cudaGroupScan,
+    .groupNeighbor = fb::launchGroupNeighbor,
     .move = fb::launchMove,
     .moveBulk = fb::launchMoveBulk,
     .barrier = fb::launchBarrier,
@@ -1279,6 +1280,7 @@ const fb::KernelTable HOST_KERNELS = {
     .groupScatter = fb::host::groupScatter,
     .groupReduce = fb::host::groupReduce,
     .groupScan = fb::host::groupScan,
+    .groupNeighbor = fb::host::groupNeighbor,
     .move = fb::host::moveKernel,
     .moveBulk = fb::host::moveBulk,
     .barrier = fb::host::barrierKernel,
@@ -1810,6 +1812,16 @@ struct Communicator::GroupLaunch
     uint32_t missing = 0;
 };
 
+// A neighbourhood topology (setNeighbors)
+struct Communicator::NeighborTopo
+{
+    std::vector<fb::NeighborEdge> in; // recv-block order
+    uint32_t outDeg = 0;
+    // the same on every member
+    uint32_t maxOutDeg = 0;
+    uint32_t maxInDeg = 0;
+};
+
 struct Communicator::GroupPlan
 {
     std::vector<GroupLaunch> launches;
@@ -2075,25 +2087,54 @@ static bool rootedKind(Communicator::GroupKind kind)
            kind == Communicator::GROUP_REDUCE || scanKind(kind);
 }
 
-// The next launch of a rooted list from `at` on, which it
+static bool neighborKind(Communicator::GroupKind kind)
+{
+    return kind == Communicator::GROUP_NEIGHBOR_ALLGATHER || kind == Communicator::GROUP_NEIGHBOR_ALLTOALL;
+}
+
+int Communicator::setNeighbors(const std::vector<std::pair<int, int>>& inEdges,
+                               int outDegree,
+                               int maxOutDegree,
+                               int maxInDegree)
+{
+    if (topo_ != nullptr || outDegree < 0 || outDegree > maxOutDegree || (int64_t)inEdges.size() > maxInDegree ||
+        maxInDegree > FB_NEIGHBOR_MAX_IN_DEGREE) {
+        return FB_E_INVALID;
+    }
+    auto t = std::make_shared<NeighborTopo>();
+    for (const auto& [src, idx] : inEdges) {
+        if (src < 0 || src >= dev_.nranks || idx < 0 || idx >= maxOutDegree) {
+            return FB_E_INVALID;
+        }
+        t->in.push_back(fb::NeighborEdge{ (uint32_t)src, (uint32_t)idx });
+    }
+    t->outDeg = (uint32_t)outDegree;
+    t->maxOutDeg = (uint32_t)maxOutDegree;
+    t->maxInDeg = (uint32_t)maxInDegree;
+    topo_ = std::move(t);
+    return FB_OK;
+}
+
+// The next launch of a rooted or neighbour list from `at` on, which it
 // advances: pieces of items, one RootedSeg each, while there are segment
-// slots and staging chunks left (launch_api.h).  An item larger than the
-// staging room left is cut at a chunk boundary and goes on in the next
-// launch.  Only the counts decide the cuts, so every rank cuts alike.
+// slots (`maxPieces`) and staging chunks (`room` chunks of `cb` bytes) left
+// (launch_api.h).  An item larger than the staging room left is cut at a
+// chunk boundary and goes on in the next launch.  Only the counts and the
+// arguments, which are the same on every rank, decide the cuts, so every
+// rank cuts alike.  `fanout`: copies of a piece the launch moves.
 static void buildRootedSegs(const Communicator::GroupItem* items,
                             size_t nItems,
                             size_t esize,
-                            int nranks,
-                            size_t stageBytes,
+                            uint64_t cb,
+                            uint64_t room,
+                            size_t maxPieces,
+                            uint64_t fanout,
                             Communicator::GroupCursor& at,
                             SegBuild& out,
                             uint32_t& missing)
 {
-    const uint64_t cb = (uint64_t)fb::fbGroupChunkVecs(nranks) * 16;
-    // (a piece's bytes are a uint32)
-    const uint64_t room = std::min<uint64_t>(stageBytes, (uint64_t)1 << 31) / cb;
     uint64_t chunks = 0;
-    while (at.item < nItems && out.segs.size() < GROUP_ITEMS_PER_LAUNCH && chunks < room) {
+    while (at.item < nItems && out.segs.size() < maxPieces && chunks < room) {
         const Communicator::GroupItem& it = items[at.item];
         const uint64_t stride = (uint64_t)it.count * esize;
         if (stride == 0) {
@@ -2112,7 +2153,7 @@ static void buildRootedSegs(const Communicator::GroupItem* items,
         memcpy(&raw, &sg, sizeof(raw));
         out.segs.push_back(raw);
         chunks += (len + cb - 1) / cb;
-        out.bytes += len * nranks;
+        out.bytes += len * fanout;
         at.offset += len;
         if (at.offset == stride) {
             at.item++;
@@ -2135,8 +2176,35 @@ int Communicator::groupBatch(GroupKind kind,
 {
     SegBuild sb;
     int rc = FB_OK;
+    size_t pieces = 0; // entries before the neighbour kinds' in-edges
+    // (a piece's bytes are a uint32)
+    const uint64_t stage = std::min<uint64_t>(cfg_.stageBytes, (uint64_t)1 << 31);
     if (rootedKind(kind)) {
-        buildRootedSegs(items, nItems, esize, dev_.nranks, cfg_.stageBytes, at, sb, l.missing);
+        const uint64_t cb = (uint64_t)fb::fbGroupChunkVecs(dev_.nranks) * 16;
+        buildRootedSegs(items, nItems, esize, cb, stage / cb, GROUP_ITEMS_PER_LAUNCH, dev_.nranks, at, sb, l.missing);
+    } else if (neighborKind(kind)) {
+        // The staging room is shared by the largest out-degree's slots
+        // (all-to-all) and the segment slots by the largest in-degree's
+        // edges, which follow the pieces in the table
+        if (topo_ == nullptr) {
+            return FB_E_INVALID;
+        }
+        const uint64_t slots = kind == GROUP_NEIGHBOR_ALLTOALL ? std::max<uint32_t>(topo_->maxOutDeg, 1) : 1;
+        const uint64_t room = stage / FB_NEIGHBOR_CHUNK / slots;
+        if (room == 0) {
+            return FB_E_TOO_LARGE;
+        }
+        const size_t maxPieces =
+          std::min<size_t>(GROUP_ITEMS_PER_LAUNCH, FB_GROUP_MAX_SEGS - FB_NEIGHBOR_EDGE_SLOTS(topo_->maxInDeg));
+        buildRootedSegs(items, nItems, esize, FB_NEIGHBOR_CHUNK, room, maxPieces, topo_->in.size(), at, sb, l.missing);
+        pieces = sb.segs.size();
+        const auto& in = topo_->in;
+        for (size_t e = 0; e < in.size(); e += 4) {
+            fb::GroupSeg raw;
+            memset(&raw, 0, sizeof(raw));
+            memcpy(&raw, in.data() + e, std::min<size_t>(4, in.size() - e) * sizeof(fb::NeighborEdge));
+            sb.segs.push_back(raw);
+        }
     } else {
         // a window of GROUP_ITEMS_PER_LAUNCH whole items
         const size_t begin = at.item;
@@ -2150,7 +2218,7 @@ int Communicator::groupBatch(GroupKind kind,
         return rc;
     }
     segs = std::move(sb.segs);
-    l.nSegs = (uint32_t)segs.size();
+    l.nSegs = (uint32_t)(neighborKind(kind) ? pieces : segs.size());
     l.totalChunks = sb.totalChunks;
     l.vecsPerRank = sb.vecsPerRank;
     l.bytes = sb.bytes;
@@ -2168,7 +2236,7 @@ std::shared_ptr<Communicator::GroupPlan> Communicator::prepareGroup(
     int& rc = rcOut ? *rcOut : rcLocal;
     rc = FB_OK;
     const size_t esize = fbDtypeSize(dtype);
-    if (esize == 0 || kind < GROUP_ALLREDUCE || kind > GROUP_EXSCAN) {
+    if (esize == 0 || kind < GROUP_ALLREDUCE || kind > GROUP_NEIGHBOR_ALLTOALL) {
         rc = FB_E_INVALID;
         return nullptr;
     }
@@ -2250,6 +2318,9 @@ int Communicator::launchGroup(const GroupLaunch& l,
     a.exclusive = kind == GROUP_EXSCAN ? 1 : 0;
     if (rootedKind(kind)) {
         return launchRooted(l, kind, dtype, op, a, ss, flags, s);
+    }
+    if (neighborKind(kind)) {
+        return launchNeighbor(l, kind, a, ss, flags, s);
     }
     if (ss && streamBarrier(flags, s) != FB_OK) {
         return FB_E_CUDA;
@@ -2355,6 +2426,50 @@ int Communicator::launchRooted(const GroupLaunch& l, GroupKind kind, int dtype, 
     return FB_OK;
 }
 
+// A neighbour launch.  With stream-ordered barriers the kernel runs as two
+// launches: LOCAL, barrier, MOVE, barrier.  The grid follows from the launch's
+// chunks and the largest degrees, the same on every rank.
+int Communicator::launchNeighbor(const GroupLaunch& l, GroupKind kind, fb::GroupArgs& a, bool ss, int flags,
+                                 cudaStream_t s)
+{
+    const NeighborTopo& t = *topo_;
+    a.stageOff = stageSendOff_;
+    a.nEdges = (uint32_t)t.in.size();
+    a.outDeg = t.outDeg;
+    const uint64_t warps = (uint64_t)cfg_.threads / 32;
+    const uint64_t units = (uint64_t)l.totalChunks * std::max(t.maxOutDeg, t.maxInDeg);
+    const int blocks = (int)std::clamp<uint64_t>(
+      (units + warps - 1) / warps, 1, (uint64_t)groupGrid(cfg_, dev_.nranks, units * (FB_NEIGHBOR_CHUNK / 16)));
+    const bool a2a = kind == GROUP_NEIGHBOR_ALLTOALL;
+    auto run = [&](int phase) {
+        a.phase = phase;
+        return k_->groupNeighbor(a, a2a, blocks, cfg_.threads, s) == cudaSuccess ? FB_OK : FB_E_CUDA;
+    };
+    int rc;
+    if (!ss) {
+        rc = run(GROUP_PHASE_LOCAL | GROUP_PHASE_MOVE);
+    } else {
+        rc = run(GROUP_PHASE_LOCAL);
+        rc = rc == FB_OK ? streamBarrier(flags, s) : rc;
+        rc = rc == FB_OK ? run(GROUP_PHASE_MOVE) : rc;
+        rc = rc == FB_OK ? streamBarrier(flags, s) : rc;
+        stats_.stagedCopies++;
+    }
+    if (rc != FB_OK) {
+        return FB_E_CUDA;
+    }
+    stats_.launches++;
+    stats_.bytes += l.bytes;
+    return FB_OK;
+}
+
+// Whether this rank lacks a buffer of a neighbour list (`missing` as for the
+// rooted kinds): the send with an out-edge, the recv with an in-edge
+static bool neighborMissing(uint32_t outDeg, size_t inDeg, uint32_t missing)
+{
+    return (missing & ((outDeg > 0 ? 1u : 0u) | (inDeg > 0 ? 2u : 0u))) != 0;
+}
+
 namespace {
 // Indexed by GroupKind: the NVTX ranges of runGroup and groupMany, and the
 // kind's name in messages
@@ -2371,6 +2486,8 @@ const GroupKindNames kGroupNames[] = {
     FB_GROUP_NAMES("allToAll", "all-to-all"), FB_GROUP_NAMES("gather", "gather"),
     FB_GROUP_NAMES("scatter", "scatter"), FB_GROUP_NAMES("reduce", "reduce"),
     FB_GROUP_NAMES("scan", "scan"), FB_GROUP_NAMES("exscan", "exscan"),
+    FB_GROUP_NAMES("neighborAllGather", "neighbor-allgather"),
+    FB_GROUP_NAMES("neighborAllToAll", "neighbor-alltoall"),
 };
 #undef FB_GROUP_NAMES
 
@@ -2380,7 +2497,7 @@ const int GROUP_NOTHING = 1;
 
 const char* Communicator::groupKindName(GroupKind kind)
 {
-    return kind >= GROUP_ALLREDUCE && kind <= GROUP_EXSCAN ? kGroupNames[kind].name : "unknown";
+    return kind >= GROUP_ALLREDUCE && kind <= GROUP_NEIGHBOR_ALLTOALL ? kGroupNames[kind].name : "unknown";
 }
 
 // The rules runGroup and groupMany share (see the header).  FB_OK, with
@@ -2416,6 +2533,19 @@ int Communicator::groupCheck(GroupKind kind, int dtype, int op, int root, int fl
             return FB_E_INVALID;
         }
     }
+    if (neighborKind(kind)) {
+        if (topo_ == nullptr || FB_FLAG_GET_CHANNEL(flags) != 0) {
+            return FB_E_INVALID;
+        }
+        // (the all-to-all stages a chunk per slot at least)
+        const uint64_t slots = kind == GROUP_NEIGHBOR_ALLTOALL ? std::max<uint32_t>(topo_->maxOutDeg, 1) : 1;
+        if (std::min<uint64_t>(cfg_.stageBytes, (uint64_t)1 << 31) / FB_NEIGHBOR_CHUNK < slots) {
+            return FB_E_TOO_LARGE;
+        }
+        if (topo_->maxInDeg == 0) {
+            return GROUP_NOTHING; // no member has an edge
+        }
+    }
     return FB_OK;
 }
 
@@ -2442,6 +2572,15 @@ int Communicator::runGroup(GroupKind kind, const GroupPlan& plan, int op, int ro
             return FB_E_INVALID;
         }
     }
+    if (neighborKind(kind)) {
+        uint32_t missing = 0;
+        for (const auto& l : plan.launches) {
+            missing |= l.missing;
+        }
+        if (neighborMissing(topo_->outDeg, topo_->in.size(), missing)) {
+            return FB_E_INVALID;
+        }
+    }
     bindDevice();
     for (const auto& l : plan.launches) {
         rc = launchGroup(l, kind, plan.dtype, op, root, flags, s);
@@ -2464,7 +2603,7 @@ int Communicator::groupMany(GroupKind kind,
                             int flags,
                             cudaStream_t s)
 {
-    if (kind < GROUP_ALLREDUCE || kind > GROUP_EXSCAN) {
+    if (kind < GROUP_ALLREDUCE || kind > GROUP_NEIGHBOR_ALLTOALL) {
         return FB_E_INVALID;
     }
     NvtxRange nvtxRange(kGroupNames[kind].many);
@@ -2474,14 +2613,15 @@ int Communicator::groupMany(GroupKind kind,
         return rc == GROUP_NOTHING ? FB_OK : rc;
     }
     const size_t esize = fbDtypeSize(dtype);
-    if (rootedKind(kind)) {
+    if (rootedKind(kind) || neighborKind(kind)) {
         uint32_t missing = 0;
         for (size_t i = 0; i < nItems; i++) {
             if (items[i].count != 0) {
                 missing |= (items[i].send == nullptr ? 1u : 0u) | (items[i].recv == nullptr ? 2u : 0u);
             }
         }
-        if (rootedMissing(kind, dev_.rank == root, missing)) {
+        if (rootedKind(kind) ? rootedMissing(kind, dev_.rank == root, missing)
+                             : neighborMissing(topo_->outDeg, topo_->in.size(), missing)) {
             return FB_E_INVALID;
         }
     }

@@ -704,6 +704,48 @@ cudaError_t groupScatter(const GroupArgs& a, int blocks, int, cudaStream_t)
     return groupRooted(a, blocks, false);
 }
 
+// The twin of groupNeighborKernel: a piece of staging slot k is its chunks of
+// the slot, [(k * T + chunk0) * CB, ... + bytes)
+cudaError_t groupNeighbor(const GroupArgs& a, bool allToAll, int blocks, int, cudaStream_t)
+{
+    const FbCommDev& c = a.comm;
+    if ((uintptr_t)(c.heap[c.rank] + a.stageOff) & 15) {
+        return cudaErrorMisalignedAddress;
+    }
+    const RootedSeg* segs = reinterpret_cast<const RootedSeg*>(a.segs);
+    const NeighborEdge* edges = reinterpret_cast<const NeighborEdge*>(segs + a.nSegs);
+    const uint64_t T = a.totalChunks;
+    const bool direct = c.nranks == 1;
+    auto slot = [&](int p, uint64_t k, const RootedSeg& sg) {
+        return c.heap[p] + a.stageOff + (k * T + sg.chunk0) * FB_NEIGHBOR_CHUNK;
+    };
+    auto user = [](uint64_t addr) { return reinterpret_cast<uint8_t*>(addr); };
+    if (!direct && (a.phase & GROUP_PHASE_LOCAL)) {
+        const uint32_t slots = allToAll ? a.outDeg : std::min(a.outDeg, 1u);
+        for (uint32_t si = 0; si < a.nSegs; si++) {
+            for (uint32_t k = 0; k < slots; k++) {
+                memcpy(slot(c.rank, k, segs[si]), user(segs[si].send) + (allToAll ? k * segs[si].stride : 0),
+                       segs[si].bytes);
+            }
+        }
+    }
+    bool ok = a.noSync || gridBarrier(c, blocks);
+    if (ok && (a.phase & GROUP_PHASE_MOVE)) {
+        for (uint32_t si = 0; si < a.nSegs; si++) {
+            const RootedSeg& sg = segs[si];
+            for (uint32_t j = 0; j < a.nEdges; j++) {
+                const uint64_t k = allToAll ? edges[j].idx : 0;
+                const uint8_t* src = direct ? user(sg.send) + k * sg.stride : slot(edges[j].src, k, sg);
+                memcpy(user(sg.recv) + j * sg.stride, src, sg.bytes);
+            }
+        }
+    }
+    if (!a.noSync) {
+        gridBarrier(c, blocks);
+    }
+    return cudaSuccess;
+}
+
 // The twin of groupReduceKernel: every rank stages its pieces; after the
 // entry barrier this rank folds the chunks it owns (the kernel's rule, with
 // the same grid) into the root's result slices; after the exit barrier the

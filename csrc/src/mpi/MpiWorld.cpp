@@ -2055,6 +2055,28 @@ int MpiWorld::nbAllToAll(const DeviceComm& comm,
     }, host, persistentComm);
 }
 
+int MpiWorld::nbNeighbor(const DeviceComm& comm, int rank, faabric::device::Communicator::GroupKind kind,
+                         const uint8_t* send, uint8_t* recv, size_t bytes, const HostPath& host)
+{
+    // a byte copy through the staging buffers: the burst's key is
+    // (kind, communicator)
+    NbCall call{ bytes, bytes, bytes, kind, FB_U8, -1, 0, { send, recv, bytes } };
+    call.staged = true;
+    return nbCollective(comm, rank, bytes > 0, call, [=](auto& c, cudaStream_t st) {
+        const faabric::device::Communicator::GroupItem item{ send, recv, bytes };
+        return c.groupMany(kind, &item, 1, FB_U8, 0, 0, 0, st);
+    }, host, 0);
+}
+
+bool MpiWorld::deviceNeighbor(const DeviceComm& comm, int rank, faabric::device::Communicator::GroupKind kind,
+                              const uint8_t* send, uint8_t* recv, size_t bytes)
+{
+    return issueAndWait(comm, streamForRank(rank), deviceCollectives, [&](auto& c, cudaStream_t s) {
+        const faabric::device::Communicator::GroupItem item{ send, recv, bytes };
+        return c.groupMany(kind, &item, 1, FB_U8, 0, 0, 0, s);
+    });
+}
+
 int MpiWorld::iGather(int rank, int root, const uint8_t* send, uint8_t* recv, size_t bytes, faabric_datatype_t* sendType,
                       int sendCount, faabric_datatype_t* recvType, int recvCount, int persistentComm)
 {

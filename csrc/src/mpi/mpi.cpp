@@ -37,6 +37,8 @@ struct faabric_datatype_t faabric_type_2int = { .id = FAABRIC_2INT, .size = 8 };
 struct faabric_datatype_t faabric_type_long_int = { .id = FAABRIC_LONG_INT, .size = 16 };
 
 struct faabric_info_t faabric_info_null = { .id = FAABRIC_INFO_NULL };
+int faabric_unweighted = 0;
+int faabric_weights_empty = 0;
 struct faabric_info_t faabric_info_device = { .id = FAABRIC_INFO_DEVICE };
 
 struct faabric_op_t faabric_op_max = { .id = FAABRIC_OP_MAX };

@@ -1897,4 +1897,244 @@ int MPI_Comm_free(MPI_Comm* comm)
     return MPI_SUCCESS;
 }
 
+
+// ---------------------------------------------------------------------------
+// Distributed-graph topology and neighbourhood collectives
+// ---------------------------------------------------------------------------
+int MPI_Dist_graph_create_adjacent(MPI_Comm comm_old, int indegree, const int sources[], const int sourceweights[],
+                                   int outdegree, const int destinations[], const int destweights[], MPI_Info info,
+                                   int reorder, MPI_Comm* comm_dist_graph)
+{
+    SPDLOG_TRACE("MPI - MPI_Dist_graph_create_adjacent");
+    (void)info;
+    (void)reorder;
+    if (comm_dist_graph == nullptr) {
+        return MPI_ERR_ARG;
+    }
+    *comm_dist_graph = MPI_COMM_NULL;
+    const int parentId = comm_old->id;
+    const int seq = commCreateSeq[parentId]++;
+    const std::vector<int> members = ranksOf(comm_old);
+    const int n = (int)members.size();
+    // Every member learns the whole graph (degrees, then the padded lists)
+    // and checks it alike, so every member returns the same verdict
+    int mine[2] = { indegree, outdegree };
+    std::vector<int> degs(2 * (size_t)n);
+    MPI_Allgather(mine, 2, MPI_INT, degs.data(), 2, MPI_INT, comm_old);
+    int maxIn = 0, maxOut = 0;
+    for (int r = 0; r < n; r++) {
+        if (degs[2 * r] < 0 || degs[2 * r + 1] < 0) {
+            return MPI_ERR_ARG;
+        }
+        maxIn = std::max(maxIn, degs[2 * r]);
+        maxOut = std::max(maxOut, degs[2 * r + 1]);
+    }
+    const int width = std::max(maxIn + maxOut, 1);
+    std::vector<int> row(width, -1);
+    std::copy(sources, sources + indegree, row.begin());
+    std::copy(destinations, destinations + outdegree, row.begin() + maxIn);
+    std::vector<int> all((size_t)width * n);
+    MPI_Allgather(row.data(), width, MPI_INT, all.data(), width, MPI_INT, comm_old);
+    auto g = std::make_shared<SubCommunicator::Graph>();
+    g->sources.resize(n);
+    g->destinations.resize(n);
+    g->in.resize(n);
+    g->maxIn = maxIn;
+    g->maxOut = maxOut;
+    bool badRank = false;
+    for (int r = 0; r < n; r++) {
+        const int* base = all.data() + (size_t)width * r;
+        g->sources[r].assign(base, base + degs[2 * r]);
+        g->destinations[r].assign(base + maxIn, base + maxIn + degs[2 * r + 1]);
+        for (int x : g->sources[r]) {
+            badRank |= x < 0 || x >= n;
+        }
+        for (int x : g->destinations[r]) {
+            badRank |= x < 0 || x >= n;
+        }
+    }
+    if (badRank) {
+        return MPI_ERR_RANK;
+    }
+    // the k-th occurrence of s in d's sources pairs with the k-th occurrence
+    // of d in s's destinations (MPI-3.1 7.6); the counts must agree
+    std::vector<std::map<int, std::vector<int>>> outPos(n);
+    for (int s = 0; s < n; s++) {
+        for (size_t i = 0; i < g->destinations[s].size(); i++) {
+            outPos[s][g->destinations[s][i]].push_back((int)i);
+        }
+    }
+    for (int d = 0; d < n; d++) {
+        std::map<int, int> seen;
+        for (int s : g->sources[d]) {
+            const int k = seen[s]++;
+            const auto& pos = outPos[s][d];
+            if (k >= (int)pos.size()) {
+                return MPI_ERR_TOPOLOGY;
+            }
+            g->in[d].push_back({ s, pos[k] });
+        }
+        for (const auto& [s, k] : seen) {
+            if (k != (int)outPos[s][d].size()) {
+                return MPI_ERR_TOPOLOGY;
+            }
+        }
+    }
+    for (int s = 0; s < n; s++) {
+        for (const auto& [d, pos] : outPos[s]) {
+            if (std::count(g->sources[d].begin(), g->sources[d].end(), s) != (long)pos.size()) {
+                return MPI_ERR_TOPOLOGY;
+            }
+        }
+    }
+    // a discriminator of its own: never the same id as a split of the members
+    const int id = deriveCommId(executingContext.getWorldId(), parentId, seq, hashRanks(members) ^ 0x6469737467726170ULL);
+    auto sub = registerSubCommunicator(id, executingContext.getWorldId(), members);
+    sub->setGraph(g);
+    const int cr = sub->commRankOf(executingContext.getRank());
+    {
+        auto graph = sub->graph();
+        std::lock_guard<std::mutex> lk(sub->graphMx);
+        auto& w = graph->weights[cr];
+        w.weighted = sourceweights != MPI_UNWEIGHTED && destweights != MPI_UNWEIGHTED;
+        if (w.weighted) {
+            w.sources.assign(indegree, 0);
+            w.destinations.assign(outdegree, 0);
+            if (sourceweights != MPI_WEIGHTS_EMPTY && sourceweights != nullptr) {
+                w.sources.assign(sourceweights, sourceweights + indegree);
+            }
+            if (destweights != MPI_WEIGHTS_EMPTY && destweights != nullptr) {
+                w.destinations.assign(destweights, destweights + outdegree);
+            }
+        }
+    }
+    *comm_dist_graph = new faabric_communicator_t{ id };
+    return MPI_SUCCESS;
+}
+
+// The graph of a dist-graph communicator, or null
+static std::shared_ptr<SubCommunicator::Graph> graphOf(MPI_Comm comm, std::shared_ptr<SubCommunicator>* subOut = nullptr)
+{
+    if (comm == nullptr || comm->id == FAABRIC_COMM_NULL || comm->id == FAABRIC_COMM_WORLD) {
+        return nullptr;
+    }
+    auto sub = getSubCommunicator(comm->id);
+    if (subOut != nullptr) {
+        *subOut = sub;
+    }
+    return sub != nullptr ? sub->graph() : nullptr;
+}
+
+int MPI_Topo_test(MPI_Comm comm, int* status)
+{
+    *status = graphOf(comm) != nullptr ? MPI_DIST_GRAPH : MPI_UNDEFINED;
+    return MPI_SUCCESS;
+}
+
+int MPI_Dist_graph_neighbors_count(MPI_Comm comm, int* indegree, int* outdegree, int* weighted)
+{
+    std::shared_ptr<SubCommunicator> sub;
+    auto g = graphOf(comm, &sub);
+    if (g == nullptr) {
+        return MPI_ERR_TOPOLOGY;
+    }
+    const int cr = sub->commRankOf(executingContext.getRank());
+    *indegree = (int)g->sources[cr].size();
+    *outdegree = (int)g->destinations[cr].size();
+    std::lock_guard<std::mutex> lk(sub->graphMx);
+    *weighted = g->weights[cr].weighted ? 1 : 0;
+    return MPI_SUCCESS;
+}
+
+int MPI_Dist_graph_neighbors(MPI_Comm comm, int maxindegree, int sources[], int sourceweights[], int maxoutdegree,
+                             int destinations[], int destweights[])
+{
+    std::shared_ptr<SubCommunicator> sub;
+    auto g = graphOf(comm, &sub);
+    if (g == nullptr) {
+        return MPI_ERR_TOPOLOGY;
+    }
+    const int cr = sub->commRankOf(executingContext.getRank());
+    const auto& src = g->sources[cr];
+    const auto& dst = g->destinations[cr];
+    if (maxindegree < (int)src.size() || maxoutdegree < (int)dst.size()) {
+        return MPI_ERR_ARG;
+    }
+    std::copy(src.begin(), src.end(), sources);
+    std::copy(dst.begin(), dst.end(), destinations);
+    std::lock_guard<std::mutex> lk(sub->graphMx);
+    const auto& w = g->weights[cr];
+    if (w.weighted && sourceweights != MPI_UNWEIGHTED && sourceweights != nullptr) {
+        std::copy(w.sources.begin(), w.sources.end(), sourceweights);
+    }
+    if (w.weighted && destweights != MPI_UNWEIGHTED && destweights != nullptr) {
+        std::copy(w.destinations.begin(), w.destinations.end(), destweights);
+    }
+    return MPI_SUCCESS;
+}
+
+// Blocking (request == nullptr) and non-blocking neighbourhood calls.  Where
+// the call runs follows the sub-communicator rule, judged on the send, or on
+// the recv for a rank without out-edges; a graph whose in-degree the device
+// layer refuses stays on the host path (every member knows it alike).
+static int neighborCall(bool allToAll, const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf,
+                        int recvcount, MPI_Datatype recvtype, MPI_Comm comm, MPI_Request* request)
+{
+    if (sendbuf == MPI_IN_PLACE || (size_t)sendcount * sendtype->size != (size_t)recvcount * recvtype->size) {
+        return MPI_ERR_ARG;
+    }
+    std::shared_ptr<SubCommunicator> sub;
+    auto g = graphOf(comm, &sub);
+    if (g == nullptr) {
+        return MPI_ERR_TOPOLOGY;
+    }
+    MpiWorld& world = getExecutingWorld();
+    const int rank = executingContext.getRank();
+    const int cr = sub->commRankOf(rank);
+    const size_t bytes = (size_t)recvcount * recvtype->size;
+    const uint8_t* send = (const uint8_t*)sendbuf;
+    uint8_t* recv = (uint8_t*)recvbuf;
+    const void* judged = g->destinations[cr].empty() ? (const void*)recv : (const void*)send;
+    const bool device = bytes > 0 && g->maxIn <= FB_NEIGHBOR_MAX_IN_DEGREE && MpiWorld::isDevicePointer(judged);
+    auto dev = device ? sub->deviceComm(world, rank) : nullptr;
+    const auto kind = allToAll ? faabric::device::Communicator::GROUP_NEIGHBOR_ALLTOALL
+                               : faabric::device::Communicator::GROUP_NEIGHBOR_ALLGATHER;
+    auto host = [=, &world] { sub->neighborExchange(world, rank, allToAll, send, recv, recvtype, recvcount); };
+    if (request == nullptr) {
+        if (!world.deviceNeighbor(dev, rank, kind, send, recv, bytes)) {
+            host();
+        }
+        return MPI_SUCCESS;
+    }
+    return handOut(world.nbNeighbor(dev, rank, kind, send, recv, bytes, host), request);
+}
+
+int MPI_Neighbor_allgather(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                           MPI_Datatype recvtype, MPI_Comm comm)
+{
+    SPDLOG_TRACE("MPI - MPI_Neighbor_allgather");
+    return neighborCall(false, sendbuf, sendcount, sendtype, recvbuf, recvcount, recvtype, comm, nullptr);
+}
+
+int MPI_Neighbor_alltoall(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                          MPI_Datatype recvtype, MPI_Comm comm)
+{
+    SPDLOG_TRACE("MPI - MPI_Neighbor_alltoall");
+    return neighborCall(true, sendbuf, sendcount, sendtype, recvbuf, recvcount, recvtype, comm, nullptr);
+}
+
+int MPI_Ineighbor_allgather(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                            MPI_Datatype recvtype, MPI_Comm comm, MPI_Request* request)
+{
+    SPDLOG_TRACE("MPI - MPI_Ineighbor_allgather");
+    return neighborCall(false, sendbuf, sendcount, sendtype, recvbuf, recvcount, recvtype, comm, request);
+}
+
+int MPI_Ineighbor_alltoall(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
+                           MPI_Datatype recvtype, MPI_Comm comm, MPI_Request* request)
+{
+    SPDLOG_TRACE("MPI - MPI_Ineighbor_alltoall");
+    return neighborCall(true, sendbuf, sendcount, sendtype, recvbuf, recvcount, recvtype, comm, request);
+}
+
 } // extern "C"

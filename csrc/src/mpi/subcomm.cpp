@@ -300,6 +300,36 @@ void SubCommunicator::reduceScatter(MpiWorld& w,
     copyBytes(recv, full.data() + (size_t)commRankOf(me) * shard, shard);
 }
 
+void SubCommunicator::setGraph(std::shared_ptr<Graph> g)
+{
+    std::lock_guard<std::mutex> lk(graphMx);
+    if (topo == nullptr) {
+        topo = std::move(g);
+    }
+}
+
+void SubCommunicator::neighborExchange(MpiWorld& w, int me, bool allToAll, const uint8_t* send, uint8_t* recv,
+                                       faabric_datatype_t* dt, int count)
+{
+    const size_t bytes = (size_t)count * dt->size;
+    const int cr = commRankOf(me);
+    const auto& dst = topo->destinations[cr];
+    const auto& in = topo->in[cr];
+    for (size_t i = 0; i < dst.size(); i++) {
+        if (dst[i] != cr) {
+            w.send(me, worldRanks[dst[i]], send + (allToAll ? i * bytes : 0), dt, count);
+        }
+    }
+    for (size_t j = 0; j < in.size(); j++) {
+        const auto [src, idx] = in[j];
+        if (src == cr) {
+            copyBytes(recv + j * bytes, send + (allToAll ? (size_t)idx * bytes : 0), bytes);
+        } else {
+            w.recv(worldRanks[src], me, recv + j * bytes, dt, count, nullptr);
+        }
+    }
+}
+
 std::shared_ptr<faabric::device::Communicator> SubCommunicator::currentDevice(int me)
 {
     std::lock_guard<std::mutex> lk(deviceMx);
@@ -333,6 +363,17 @@ std::shared_ptr<faabric::device::Communicator> SubCommunicator::deviceComm(MpiWo
             SPDLOG_ERROR("Communicator {}: rank {} cannot take agreed slot {} ({})", commId, me,
                          __builtin_ctz((unsigned)agreed), faabric::device::Communicator::errorString(rc));
             throw std::runtime_error("Sub-communicator slot agreement failed");
+        }
+        // a dist-graph communicator's child carries its topology (the
+        // caller routes graphs the device cannot take to the host path)
+        if (topo != nullptr && topo->maxIn <= FB_NEIGHBOR_MAX_IN_DEGREE) {
+            const int cr = commRankOf(me);
+            const int trc = child->setNeighbors(topo->in[cr], (int)topo->destinations[cr].size(), topo->maxOut,
+                                                topo->maxIn);
+            if (trc != FB_OK) {
+                throw std::runtime_error(std::string("Sub-communicator topology refused: ") +
+                                         faabric::device::Communicator::errorString(trc));
+            }
         }
     }
     std::lock_guard<std::mutex> lk(deviceMx);

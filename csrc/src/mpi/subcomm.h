@@ -72,6 +72,40 @@ class SubCommunicator
     void reduceScatter(MpiWorld& w, int me, const uint8_t* send, uint8_t* recv, faabric_datatype_t* dt, int recvCount,
                        faabric_op_t* op);
 
+    // ---- distributed-graph topology (MPI_Dist_graph_create_adjacent) ----
+    // The whole graph, which every member gathered and checked alike: per
+    // comm rank its sources and destinations, and its in-edges in recv-block
+    // order as (source comm rank, index of the edge in the source's
+    // destinations)
+    struct Graph
+    {
+        std::vector<std::vector<int>> sources, destinations;
+        std::vector<std::vector<std::pair<int, int>>> in;
+        int maxOut = 0, maxIn = 0;
+        // each member's weights, as it passed them (set by that member,
+        // under graphMx)
+        struct Weights
+        {
+            bool weighted = false;
+            std::vector<int> sources, destinations;
+        };
+        std::map<int, Weights> weights;
+    };
+    // Null for a communicator without one
+    std::shared_ptr<Graph> graph() const { return topo; }
+    // Set by the creating call, before the handle is handed out; a second
+    // member of this process finds it already set
+    void setGraph(std::shared_ptr<Graph> g);
+    std::mutex graphMx;
+
+    // MPI_Neighbor_allgather / MPI_Neighbor_alltoall on the host path, built
+    // from the world's point-to-point layer: every out-edge's block is sent
+    // (eagerly, in destination order), then every in-edge's block received
+    // (in source order), so the k-th of several edges between two ranks pairs
+    // with the k-th; self-edges are local copies.  `count` x `dt` per block.
+    void neighborExchange(MpiWorld& w, int me, bool allToAll, const uint8_t* send, uint8_t* recv,
+                          faabric_datatype_t* dt, int count);
+
     // ---- fused device path ----
     // This rank's child of its world device communicator over the members
     // (null: this communicator stays on the host path).  The first call of a
@@ -93,6 +127,7 @@ class SubCommunicator
     int commId;
     int world;
     std::vector<int> worldRanks;
+    std::shared_ptr<Graph> topo;
 
     // Per world rank of this process: the slot agreement has run (`decided`)
     // and its result (null child: host path).  Shared by the process's ranks.

@@ -96,6 +96,8 @@ GROUP_KINDS = {
     "reduce": 7,
     "scan": 8,
     "exscan": 9,
+    "neighbor_all_gather": 10,
+    "neighbor_all_to_all": 11,
 }
 ALGOS = {"auto": 0, "oneshot": 1, "twoshot": 2, "nvls": 3, "ll": 4}
 ALGO_NAMES = {v: k for k, v in ALGOS.items()}
@@ -105,6 +107,56 @@ FLAG_NOSYNC = 2
 
 class CommError(RuntimeError):
     pass
+
+
+def neighbor_in_edges(sources_per_rank, destinations_per_rank):
+    """Every rank's in-edges of a distributed graph given by its adjacency
+    lists (MPI_Dist_graph_create_adjacent's ``sources`` and ``destinations``
+    of every rank): ``out[d][j]`` is ``(s, idx)`` for the j-th source s of
+    rank d, where idx is the position of the matching edge in s's
+    destinations.  The k-th occurrence of s in d's sources pairs with the
+    k-th occurrence of d in s's destinations (MPI-3.1 section 7.6), so
+    self-edges and multi-edges are allowed.  Raises CommError for lists of
+    different lengths, a rank outside the graph, or an edge s -> d whose
+    multiplicity in s's destinations differs from that of s in d's sources."""
+    src = [[int(x) for x in v] for v in sources_per_rank]
+    dst = [[int(x) for x in v] for v in destinations_per_rank]
+    n = len(src)
+    if len(dst) != n:
+        raise CommError(f"neighbor_in_edges: {n} source lists and {len(dst)} destination lists")
+    for what, lists in (("source", src), ("destination", dst)):
+        for r, v in enumerate(lists):
+            for x in v:
+                if not 0 <= x < n:
+                    raise CommError(f"neighbor_in_edges: rank {r} names {what} {x} outside a graph of {n}")
+    # positions of d in s's destinations, in order
+    out_pos = [{} for _ in range(n)]
+    for s, v in enumerate(dst):
+        for i, d in enumerate(v):
+            out_pos[s].setdefault(d, []).append(i)
+    in_count = [{} for _ in range(n)]
+    for d, v in enumerate(src):
+        for s in v:
+            in_count[d][s] = in_count[d].get(s, 0) + 1
+    for s in range(n):
+        for d in range(n):
+            a = len(out_pos[s].get(d, ()))
+            b = in_count[d].get(s, 0)
+            if a != b:
+                raise CommError(
+                    f"neighbor_in_edges: edge {s} -> {d} is {a} times in {s}'s destinations "
+                    f"and {b} times in {d}'s sources"
+                )
+    edges = []
+    for d, v in enumerate(src):
+        seen = {}
+        mine = []
+        for s in v:
+            k = seen.get(s, 0)
+            seen[s] = k + 1
+            mine.append((s, out_pos[s][d][k]))
+        edges.append(mine)
+    return edges
 
 
 class _CudaBuf:
@@ -146,6 +198,8 @@ class Communicator:
         self.stream_wait_supported = bool(self._lib.fb_comm_stream_wait_supported(self._h))
         self.is_subset = bool(self._lib.fb_comm_is_subset(self._h))
         self._allocs: dict[int, int] = {}
+        # (in-degree, out-degree) once set_neighbors has run
+        self._neighbors: Optional[tuple[int, int]] = None
 
     # ------------------------------------------------------------ lifecycle
     def close(self):
@@ -775,6 +829,124 @@ class Communicator:
         :meth:`scan_group`."""
         self._many("scan_many", "exscan" if exclusive else "scan", sends, recvs, dtype, op, 0, stream, channel)
 
+    # -------------------------------------------- neighbourhood collectives
+    def set_neighbors(self, in_edges, out_degree: int, max_out_degree: int, max_in_degree: int):
+        """Set this rank's neighbourhood topology, once, before the first
+        neighbour call: its in-edges in recv-block order, each ``(source rank,
+        index of the edge among the source's out-edges)`` (see
+        :func:`neighbor_in_edges`), its out-degree, and the largest out- and
+        in-degree over every member, which every member passes alike.
+        :meth:`LocalGroup.set_neighbors` does this for a whole group."""
+        in_edges = [(int(s), int(i)) for s, i in in_edges]
+        n = len(in_edges)
+        srcs = (C.c_int * max(n, 1))(*[s for s, _ in in_edges])
+        idxs = (C.c_int * max(n, 1))(*[i for _, i in in_edges])
+        rc = self._lib.fb_comm_set_neighbors(
+            self._h, n, srcs, idxs, int(out_degree), int(max_out_degree), int(max_in_degree)
+        )
+        self._check(rc, "set_neighbors")
+        self._neighbors = (n, int(out_degree))
+
+    def _neighbor_items(self, what, kind, sends, recvs, counts, dtype):
+        """(n, send ptrs, recv ptrs, counts, FbDtype) of a neighbour list;
+        raises before any native call.  Item i moves blocks of ``counts[i]``
+        elements (in ``dtype``): the all-gather's send holds one block, the
+        all-to-all's one per out-edge, and every recv one per in-edge, all
+        contiguous tensors on this communicator's GPU.  ``counts`` may be
+        left out where the tensors tell the count: always for the
+        all-gather, and for the all-to-all on a rank with an edge."""
+        if self._neighbors is None:
+            raise CommError(f"{what}: no neighbourhood topology; call set_neighbors first")
+        indeg, outdeg = self._neighbors
+        if sends is None or recvs is None or len(sends) != len(recvs) or not sends:
+            raise CommError(f"{what}: need equally long, non-empty lists")
+        if counts is not None and len(counts) != len(sends):
+            raise CommError(f"{what}: {len(counts)} counts for {len(sends)} items")
+        a2a = kind == "neighbor_all_to_all"
+        typed = []
+        for i, (s, r) in enumerate(zip(sends, recvs)):
+            for t in (s, r):
+                if not t.is_cuda or t.device.index != self.device or not t.is_contiguous():
+                    raise CommError(
+                        f"{what}: item {i} must be contiguous tensors on cuda:{self.device}, not {t.device}"
+                        f"{'' if t.is_contiguous() else ' (non-contiguous)'}"
+                    )
+            if dtype is None and r.dtype != s.dtype:
+                raise CommError(f"{what}: item {i} has a {s.dtype} send and a {r.dtype} recv")
+            ns, code = self._typed(s, dtype)
+            nr, _ = self._typed(r, dtype)
+            if counts is not None:
+                c = int(counts[i])
+            elif not a2a:
+                c = ns
+            elif outdeg or indeg:
+                c = ns // outdeg if outdeg else nr // indeg
+            else:
+                raise CommError(f"{what}: item {i}: this rank has no edge, so pass counts")
+            blocks = outdeg if a2a else 1
+            if c < 0 or ns != c * blocks or nr != c * indeg:
+                raise CommError(
+                    f"{what}: item {i} has {ns} send and {nr} recv elements; with blocks of {c}, "
+                    f"send must hold {blocks} and recv {indeg} blocks"
+                )
+            typed.append((c, code))
+        if len({dt for _, dt in typed}) != 1:
+            raise CommError(f"{what}: every tensor must have the same dtype")
+        n = len(sends)
+        sp = (C.c_void_p * n)(*[t.data_ptr() or None for t in sends])
+        rp = (C.c_void_p * n)(*[t.data_ptr() or None for t in recvs])
+        cnt = (C.c_uint64 * n)(*[c for c, _ in typed])
+        return n, sp, rp, cnt, typed[0][1]
+
+    def _prepare_neighbor(self, what, kind, sends, recvs, counts, dtype) -> "GroupPlan":
+        n, sp, rp, cnt, dt = self._neighbor_items(what, kind, sends, recvs, counts, dtype)
+        h = self._lib.fb_group_prepare(self._h, GROUP_KINDS[kind], n, sp, rp, cnt, dt)
+        if not h:
+            raise CommError(f"{what} failed [{_lib.last_error()}]")
+        plan = GroupPlan(self, h, n, sum(t.numel() * t.element_size() for t in recvs))
+        plan.kind = kind
+        return plan
+
+    def _neighbor_many(self, what, kind, sends, recvs, counts, dtype, stream):
+        n, sp, rp, cnt, dt = self._neighbor_items(what, kind, sends, recvs, counts, dtype)
+        rc = self._lib.fb_group_many(self._h, GROUP_KINDS[kind], n, sp, rp, cnt, dt, 0, 0, 0, self._stream(stream))
+        self._check(rc, what)
+
+    def prepare_neighbor_all_gather_group(self, sends, recvs, counts=None, dtype=None) -> "GroupPlan":
+        """Plan the launches of MPI_Neighbor_allgather per pair of the lists
+        over this communicator's topology (:meth:`set_neighbors`): block j of
+        ``recvs[i]`` gets ``sends[i]`` of in-edge j's source.  Tensors are any
+        device memory at any alignment.  Call collectively with the same
+        counts; every member takes part, edges or not."""
+        return self._prepare_neighbor(
+            "prepare_neighbor_all_gather_group", "neighbor_all_gather", sends, recvs, counts, dtype
+        )
+
+    def neighbor_all_gather_group(self, plan: "GroupPlan", stream=None, flags=0):
+        self._launch("neighbor_all_gather_group", "neighbor_all_gather", plan, 0, 0, stream, 0, flags)
+
+    def neighbor_all_gather_many(self, sends, recvs, counts=None, stream=None, dtype=None):
+        """Transient variant of :meth:`prepare_neighbor_all_gather_group` +
+        :meth:`neighbor_all_gather_group`."""
+        self._neighbor_many("neighbor_all_gather_many", "neighbor_all_gather", sends, recvs, counts, dtype, stream)
+
+    def prepare_neighbor_all_to_all_group(self, sends, recvs, counts=None, dtype=None) -> "GroupPlan":
+        """Plan the launches of MPI_Neighbor_alltoall per pair of the lists
+        over this communicator's topology: block j of ``recvs[i]`` gets block
+        idx of ``sends[i]`` on the source of in-edge j = (source, idx).
+        Otherwise as :meth:`prepare_neighbor_all_gather_group`."""
+        return self._prepare_neighbor(
+            "prepare_neighbor_all_to_all_group", "neighbor_all_to_all", sends, recvs, counts, dtype
+        )
+
+    def neighbor_all_to_all_group(self, plan: "GroupPlan", stream=None, flags=0):
+        self._launch("neighbor_all_to_all_group", "neighbor_all_to_all", plan, 0, 0, stream, 0, flags)
+
+    def neighbor_all_to_all_many(self, sends, recvs, counts=None, stream=None, dtype=None):
+        """Transient variant of :meth:`prepare_neighbor_all_to_all_group` +
+        :meth:`neighbor_all_to_all_group`."""
+        self._neighbor_many("neighbor_all_to_all_many", "neighbor_all_to_all", sends, recvs, counts, dtype, stream)
+
     def send_recv(self, send_buf, dst, recv_buf, src, stream=None):
         rc = self._lib.fb_sendrecv(
             self._h,
@@ -1046,8 +1218,8 @@ class Communicator:
 
 class GroupPlan:
     """Device-resident segment tables of a grouped all-reduce, reduce-scatter,
-    all-gather, broadcast, all-to-all, gather, scatter, reduce, scan or
-    exscan."""
+    all-gather, broadcast, all-to-all, gather, scatter, reduce, scan, exscan,
+    neighbourhood all-gather or neighbourhood all-to-all."""
 
     def __init__(self, comm: Communicator, handle, n_tensors: int, nbytes: int):
         self._comm = comm
@@ -1135,6 +1307,17 @@ class LocalGroup:
         e.g. their streams alias one hardware queue or a tool serialises them."""
         self.run(lambda c, r, st: c.barrier())
         return self.check_errors() == [0] * self.size
+
+    def set_neighbors(self, sources_per_rank, destinations_per_rank):
+        """Give every rank the neighbourhood topology of the graph with these
+        adjacency lists (see :func:`neighbor_in_edges`, which checks it)."""
+        edges = neighbor_in_edges(sources_per_rank, destinations_per_rank)
+        if len(edges) != self.size:
+            raise CommError(f"set_neighbors: a graph of {len(edges)} ranks for a group of {self.size}")
+        max_out = max(len(v) for v in destinations_per_rank)
+        max_in = max(len(v) for v in edges)
+        for r, c in enumerate(self.comms):
+            c.set_neighbors(edges[r], len(destinations_per_rank[r]), max_out, max_in)
 
     def subset(self, members: Sequence[int]) -> "SubGroup":
         """The ranks ``members`` of this group as a group of their own (child
