@@ -32,6 +32,7 @@
 #include "../tests/mpi_group_reduce_body.h"
 #include "../tests/mpi_group_scan_body.h"
 #include "../tests/mpi_neighbor_body.h"
+#include "../tests/mpi_neighbor_v_body.h"
 #include "../tests/mpi_group_rooted_body.h"
 #include "../tests/mpi_group_subcomm_body.h"
 #include "../tests/mpi_persistent_body.h"
@@ -1245,6 +1246,180 @@ static void registerFunctions()
             msg.set_outputdata(why);
         }
         return rc;
+    });
+
+    // The neighbourhood v-collectives on the world and on a split
+    // (mpi_neighbor_v_body.h)
+    mpiFunction("neighbor-v-coll", [](int rank, int size, faabric::Message& msg) {
+        std::string why;
+        int rc = neighbor_v_coll::body(rank, size, msg.mpiworldid(), true, &why);
+        if (rc != 0) {
+            SPDLOG_ERROR("neighbor-v-coll: {}", why);
+            msg.set_outputdata(why);
+        }
+        return rc;
+    });
+
+    // An irregular halo of `fields` fp32 fields per step over the world, in
+    // device memory (MPI_Alloc_mem): the periodic 4-neighbour grid of
+    // bench-neighbor (left, right, down, up), where the face rank r sends on
+    // out-edge k has `face * (1 + (r + k) % 4) / 4` bytes (input "irregular";
+    // "equal": `face` bytes on every edge).  Input: "<mode>;<steps>;<faces>;
+    // <face bytes>;<fields>" with mode
+    //   p2p       per field an MPI_Isend per out-edge and an MPI_Irecv per
+    //             in-edge, one MPI_Waitall per step (self-edges: a device copy)
+    //   blocking  one MPI_Neighbor_alltoallv per field
+    //   burst     one MPI_Ineighbor_alltoallv per field + MPI_Waitall
+    //   equal     one MPI_Ineighbor_alltoall per field + MPI_Waitall (faces
+    //             must be "equal")
+    // Rank 0 reports {"ms_per_step", "launches_per_step"} (launches on its
+    // world device communicator and on the graph's child).  Every rank checks
+    // every word of every received face.
+    mpiFunction("bench-neighbor-v", [](int rank, int size, faabric::Message& msg) {
+        std::vector<std::string> f;
+        std::string cur;
+        for (char c : msg.inputdata() + ";") {
+            if (c == ';') {
+                f.push_back(cur);
+                cur.clear();
+            } else {
+                cur += c;
+            }
+        }
+        EXPECT(f.size() >= 5 && size >= 2);
+        const std::string mode = f[0];
+        const int steps = std::stoi(f[1]);
+        const bool irregular = f[2] == "irregular";
+        const size_t face = std::stoull(f[3]);
+        const int fields = std::stoi(f[4]);
+        EXPECT(!(irregular && mode == "equal"));
+        const int px = size == 8 ? 4 : 2;
+        const int py = size / px;
+        auto dstOf = [&](int r) {
+            const int x = r % px, y = r / px;
+            return std::vector<int>{ (x + px - 1) % px + y * px, (x + 1) % px + y * px, x + (y + py - 1) % py * px,
+                                     x + (y + 1) % py * px };
+        };
+        // words on out-edge k of rank r
+        auto words = [&](int r, int k) { return (int)((irregular ? face * (1 + (r + k) % 4) / 4 : face) / 4); };
+        const std::vector<int> dst = dstOf(rank);
+        const std::vector<int> src = dst;
+        std::vector<std::pair<int, int>> in;
+        std::map<int, int> seen;
+        for (int s : src) {
+            int k = seen[s]++;
+            const auto d = dstOf(s);
+            for (size_t i = 0; i < d.size(); i++) {
+                if (d[i] == rank && k-- == 0) {
+                    in.push_back({ s, (int)i });
+                    break;
+                }
+            }
+        }
+        EXPECT(in.size() == src.size());
+        MPI_Comm graph = MPI_COMM_NULL;
+        EXPECT(MPI_Dist_graph_create_adjacent(MPI_COMM_WORLD, (int)src.size(), src.data(), MPI_UNWEIGHTED,
+                                              (int)dst.size(), dst.data(), MPI_UNWEIGHTED, MPI_INFO_NULL, 0,
+                                              &graph) == MPI_SUCCESS);
+        std::vector<int> sc, sd, rc, rd;
+        int sTotal = 0, rTotal = 0;
+        for (size_t k = 0; k < dst.size(); k++) {
+            sc.push_back(words(rank, (int)k));
+            sd.push_back(sTotal);
+            sTotal += sc.back();
+        }
+        for (auto [s, idx] : in) {
+            rc.push_back(words(s, idx));
+            rd.push_back(rTotal);
+            rTotal += rc.back();
+        }
+        std::vector<float*> sends(fields), recvs(fields);
+        for (int i = 0; i < fields; i++) {
+            EXPECT(MPI_Alloc_mem((MPI_Aint)sTotal * 4, MPI_INFO_FAABRIC_DEVICE, &sends[i]) == MPI_SUCCESS);
+            EXPECT(MPI_Alloc_mem((MPI_Aint)rTotal * 4, MPI_INFO_FAABRIC_DEVICE, &recvs[i]) == MPI_SUCCESS);
+            // word w of face k of field i on rank r: r * 1000000 + i * 1000 + k
+            // (as an int32 bit pattern)
+            std::vector<int32_t> mine(sTotal);
+            for (size_t k = 0; k < dst.size(); k++) {
+                std::fill(mine.begin() + sd[k], mine.begin() + sd[k] + sc[k], rank * 1000000 + i * 1000 + (int)k);
+            }
+            cudaMemcpy(sends[i], mine.data(), (size_t)sTotal * 4, cudaMemcpyHostToDevice);
+            cudaMemset(recvs[i], 0xff, (size_t)rTotal * 4);
+        }
+        MPI_Barrier(MPI_COMM_WORLD);
+        std::vector<MPI_Request> reqs;
+        auto step = [&]() -> int {
+            reqs.clear();
+            for (int i = 0; i < fields; i++) {
+                if (mode == "p2p") {
+                    for (size_t j = 0; j < in.size(); j++) {
+                        if (in[j].first != rank) {
+                            reqs.emplace_back();
+                            EXPECT(MPI_Irecv(recvs[i] + rd[j], rc[j], MPI_FLOAT, in[j].first, i, MPI_COMM_WORLD,
+                                             &reqs.back()) == MPI_SUCCESS);
+                        } else {
+                            cudaMemcpy(recvs[i] + rd[j], sends[i] + sd[in[j].second], (size_t)rc[j] * 4,
+                                       cudaMemcpyDeviceToDevice);
+                        }
+                    }
+                    for (size_t k = 0; k < dst.size(); k++) {
+                        if (dst[k] != rank) {
+                            reqs.emplace_back();
+                            EXPECT(MPI_Isend(sends[i] + sd[k], sc[k], MPI_FLOAT, dst[k], i, MPI_COMM_WORLD,
+                                             &reqs.back()) == MPI_SUCCESS);
+                        }
+                    }
+                } else if (mode == "blocking") {
+                    EXPECT(MPI_Neighbor_alltoallv(sends[i], sc.data(), sd.data(), MPI_FLOAT, recvs[i], rc.data(),
+                                                  rd.data(), MPI_FLOAT, graph) == MPI_SUCCESS);
+                } else if (mode == "burst") {
+                    reqs.emplace_back();
+                    EXPECT(MPI_Ineighbor_alltoallv(sends[i], sc.data(), sd.data(), MPI_FLOAT, recvs[i], rc.data(),
+                                                   rd.data(), MPI_FLOAT, graph, &reqs.back()) == MPI_SUCCESS);
+                } else {
+                    reqs.emplace_back();
+                    EXPECT(MPI_Ineighbor_alltoall(sends[i], sc[0], MPI_FLOAT, recvs[i], rc[0], MPI_FLOAT, graph,
+                                                  &reqs.back()) == MPI_SUCCESS);
+                }
+            }
+            EXPECT(MPI_Waitall((int)reqs.size(), reqs.data(), MPI_STATUSES_IGNORE) == MPI_SUCCESS);
+            return 0;
+        };
+        for (int i = 0; i < 3; i++) {
+            EXPECT(step() == 0);
+        }
+        auto worldDev = faabric::mpi::getMpiWorldRegistry().getWorld(msg.mpiworldid()).getDeviceComm(rank);
+        auto launches = [&]() {
+            auto child = faabric::mpi::getSubCommunicator(graph->id)->currentDevice(rank);
+            return (worldDev ? worldDev->stats().launches : 0) + (child ? child->stats().launches : 0);
+        };
+        MPI_Barrier(MPI_COMM_WORLD);
+        const uint64_t l0 = launches();
+        auto t0 = std::chrono::steady_clock::now();
+        for (int i = 0; i < steps; i++) {
+            EXPECT(step() == 0);
+        }
+        const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count() / steps;
+        const double perStep = (double)(launches() - l0) / steps;
+        MPI_Barrier(MPI_COMM_WORLD);
+        for (int i = 0; i < fields; i++) {
+            std::vector<int32_t> back(rTotal);
+            cudaMemcpy(back.data(), recvs[i], (size_t)rTotal * 4, cudaMemcpyDeviceToHost);
+            for (size_t j = 0; j < in.size(); j++) {
+                const int32_t want = in[j].first * 1000000 + i * 1000 + in[j].second;
+                for (int w = 0; w < rc[j]; w++) {
+                    EXPECT(back[rd[j] + w] == want);
+                }
+            }
+            MPI_Free_mem(sends[i]);
+            MPI_Free_mem(recvs[i]);
+        }
+        MPI_Comm_free(&graph);
+        if (rank == 0) {
+            msg.set_outputdata("{\"ms_per_step\": " + std::to_string(ms) + ", \"launches_per_step\": " +
+                               std::to_string(perStep) + "}");
+        }
+        return 0;
     });
 
     // A neighbourhood exchange of `fields` fp32 fields per step over the

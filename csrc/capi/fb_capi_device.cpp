@@ -632,6 +632,108 @@ void fb_group_plan_free(void* plan)
     delete (FbGroupPlanHandle*)plan;
 }
 
+// ---- grouped neighbourhood v-collectives: item i's counts and
+// displacements are row i of `sendWidth` (send) and `recvWidth` (recv)
+// entries; the rows must cover this rank's degrees (the all-gather reads one
+// send count and no send displacement) ----
+static int neighborVItems(void* h,
+                          int kind,
+                          int n,
+                          const void* const* send,
+                          void* const* recv,
+                          const uint64_t* sendCounts,
+                          const uint64_t* sendDispls,
+                          int sendWidth,
+                          const uint64_t* recvCounts,
+                          const uint64_t* recvDispls,
+                          int recvWidth,
+                          std::vector<Communicator::NeighborVItem>& items)
+{
+    static_assert(sizeof(size_t) == sizeof(uint64_t), "counts are passed as size_t");
+    const auto [inDeg, outDeg] = COMM(h)->neighborDegrees();
+    const int sends = kind == Communicator::GROUP_NEIGHBOR_ALLTOALLV ? outDeg : std::min(outDeg, 1);
+    if (n < 0 || sendWidth < sends || recvWidth < inDeg) {
+        return FB_E_INVALID;
+    }
+    items.resize((size_t)n);
+    for (int i = 0; i < n; i++) {
+        const size_t so = (size_t)i * sendWidth;
+        const size_t ro = (size_t)i * recvWidth;
+        items[i] = { send[i],
+                     recv[i],
+                     sendCounts ? (const size_t*)sendCounts + so : nullptr,
+                     sendDispls ? (const size_t*)sendDispls + so : nullptr,
+                     recvCounts ? (const size_t*)recvCounts + ro : nullptr,
+                     recvDispls ? (const size_t*)recvDispls + ro : nullptr };
+    }
+    return FB_OK;
+}
+
+#define FB_NEIGHBOR_V_ARGS                                                                                             \
+    void *h, int kind, int n, const void *const *send, void *const *recv, const uint64_t *sendCounts,                \
+      const uint64_t *sendDispls, int sendWidth, const uint64_t *recvCounts, const uint64_t *recvDispls,             \
+      int recvWidth, int dtype
+#define FB_NEIGHBOR_V_ITEMS(items)                                                                                     \
+    neighborVItems(h, kind, n, send, recv, sendCounts, sendDispls, sendWidth, recvCounts, recvDispls, recvWidth, items)
+
+// Communicator::neighborVStreams: the number of windows (at most `cap`
+// written to `out`), or an FB_E_* code
+int fb_neighbor_v_streams(FB_NEIGHBOR_V_ARGS, uint64_t* out, int cap)
+{
+    FB_TRY
+    std::vector<Communicator::NeighborVItem> items;
+    int rc = FB_NEIGHBOR_V_ITEMS(items);
+    std::vector<uint64_t> streams;
+    rc = rc == FB_OK ? COMM(h)->neighborVStreams((Communicator::GroupKind)kind, items.data(), items.size(), dtype,
+                                                 streams)
+                     : rc;
+    if (rc != FB_OK) {
+        return rc;
+    }
+    for (size_t w = 0; w < streams.size() && (int)w < cap; w++) {
+        out[w] = streams[w];
+    }
+    return (int)streams.size();
+    FB_CATCH(FB_E_INVALID)
+}
+
+void* fb_group_prepare_v(FB_NEIGHBOR_V_ARGS, const uint64_t* agreed, int nAgreed)
+{
+    FB_TRY
+    std::vector<Communicator::NeighborVItem> items;
+    int rc = FB_NEIGHBOR_V_ITEMS(items);
+    std::shared_ptr<Communicator::GroupPlan> plan;
+    if (rc == FB_OK) {
+        plan = COMM(h)->prepareGroup(items.data(), items.size(), dtype,
+                                     std::vector<uint64_t>(agreed, agreed + std::max(nAgreed, 0)), &rc,
+                                     (Communicator::GroupKind)kind);
+    }
+    if (!plan) {
+        g_lastError = std::string("prepareGroup: ") + Communicator::errorString(rc);
+        return nullptr;
+    }
+    auto* ph = new FbGroupPlanHandle();
+    ph->plan = plan;
+    return ph;
+    FB_CATCH(nullptr)
+}
+
+int fb_group_many_v(FB_NEIGHBOR_V_ARGS, const uint64_t* agreed, int nAgreed, int flags, void* stream)
+{
+    FB_TRY
+    std::vector<Communicator::NeighborVItem> items;
+    const int rc = FB_NEIGHBOR_V_ITEMS(items);
+    if (rc != FB_OK) {
+        return rc;
+    }
+    return COMM(h)->groupMany((Communicator::GroupKind)kind, items.data(), items.size(), dtype,
+                              std::vector<uint64_t>(agreed, agreed + std::max(nAgreed, 0)), flags,
+                              (cudaStream_t)stream);
+    FB_CATCH(FB_E_CUDA)
+}
+#undef FB_NEIGHBOR_V_ARGS
+#undef FB_NEIGHBOR_V_ITEMS
+
 // Communicator::setNeighbors: in-edge j is (srcs[j], idxs[j])
 int fb_comm_set_neighbors(void* h,
                           int nIn,

@@ -350,7 +350,9 @@ class Communicator : public std::enable_shared_from_this<Communicator>
         GROUP_SCAN = 8,
         GROUP_EXSCAN = 9,
         GROUP_NEIGHBOR_ALLGATHER = 10,
-        GROUP_NEIGHBOR_ALLTOALL = 11
+        GROUP_NEIGHBOR_ALLTOALL = 11,
+        GROUP_NEIGHBOR_ALLGATHERV = 12,
+        GROUP_NEIGHBOR_ALLTOALLV = 13
     };
     // Where the next launch of a list starts: an item, and a byte offset in
     // it (rooted kinds cut items larger than the staging buffer)
@@ -420,11 +422,80 @@ class Communicator : public std::enable_shared_from_this<Communicator>
                   int root,
                   int flags,
                   cudaStream_t s);
+    // Kernel launches of a plan (a v plan's launch window runs as several
+    // rounds)
     static size_t groupPlanLaunches(const GroupPlan& plan);
     // "all-reduce", "reduce-scatter", "all-gather", "broadcast", "all-to-all",
     // "gather", "scatter", "reduce", "scan", "exscan", "neighbor-allgather",
-    // "neighbor-alltoall"
+    // "neighbor-alltoall", "neighbor-allgatherv", "neighbor-alltoallv"
     static const char* groupKindName(GroupKind kind);
+
+    // ---- grouped neighbourhood v-collectives ----
+    // One MPI_Neighbor_allgatherv / MPI_Neighbor_alltoallv call of a list over
+    // the topology of setNeighbors, with counts and displacements in elements
+    // of the list's dtype:
+    //   GROUP_NEIGHBOR_ALLGATHERV: send holds sendCounts[0] elements (one
+    //     count; sendDispls is not read); recv block j (recvCounts[j]
+    //     elements at recvDispls[j]) gets the send of in-edge j's source
+    //   GROUP_NEIGHBOR_ALLTOALLV: send block i (sendCounts[i] elements at
+    //     sendDispls[i]) goes to out-edge i; recv block j gets the send block
+    //     idx of in-edge j = (source, idx)
+    // The arrays hold an entry per out-edge and per in-edge of this rank (none
+    // are read for a degree of 0), and are read only by the call that takes
+    // the item.  A block's count must equal the count its peer gives for the
+    // same edge, as MPI requires.  Byte copies of any dtype, buffers in any
+    // device memory at any alignment; a buffer may be null where all its
+    // counts are 0.
+    struct NeighborVItem
+    {
+        const void* send;
+        void* recv;
+        const size_t* sendCounts;
+        const size_t* sendDispls;
+        const size_t* recvCounts;
+        const size_t* recvDispls;
+    };
+    // A v list runs in launch windows of whole items, cut from the largest
+    // degrees alone, so every member cuts alike.  Stream k of a rank in a
+    // window is the concatenation, in item order, of its edge-k blocks; a
+    // launch moves at most the staging room of every stream (a round), so a
+    // window takes ceil(M / W) launches, where M is its largest stream over
+    // every member and W the room of one staging slot (CommConfig::stageBytes
+    // over the largest out-degree for the all-to-all, rounded to
+    // FB_NEIGHBOR_CHUNK, and at most M rounded up to it).  A rank knows only
+    // its own streams, so M is agreed by the caller:
+    //   neighborVStreams: this rank's largest stream of every window, in
+    //     bytes (local; `out` gets one entry per window, none when no member
+    //     has an edge);
+    //   the caller takes the elementwise maximum over every member and passes
+    //     it as `agreed` to prepareGroup / groupMany, which refuse a list whose
+    //     agreement is shorter or longer than its windows or below one of this
+    //     rank's own streams (FB_E_INVALID).  A window whose agreement is 0
+    //     launches nothing.
+    // Refusals, all before any launch: the rules of the equal-block neighbour
+    // kinds (a communicator without a topology or a channel other than 0:
+    // FB_E_INVALID), a missing count array or buffer that this rank needs
+    // (FB_E_INVALID), and degrees too large for one item per window
+    // (FB_E_TOO_LARGE: the largest out-degree plus in-degree above
+    // FB_NEIGHBOR_V_MAX_DEGREE).  runGroup launches a v plan like any other.
+    int neighborVStreams(GroupKind kind,
+                         const NeighborVItem* items,
+                         size_t nItems,
+                         int dtype,
+                         std::vector<uint64_t>& out) const;
+    std::shared_ptr<GroupPlan> prepareGroup(const NeighborVItem* items,
+                                            size_t nItems,
+                                            int dtype,
+                                            const std::vector<uint64_t>& agreed,
+                                            int* rc,
+                                            GroupKind kind);
+    int groupMany(GroupKind kind,
+                  const NeighborVItem* items,
+                  size_t nItems,
+                  int dtype,
+                  const std::vector<uint64_t>& agreed,
+                  int flags,
+                  cudaStream_t s);
 
     // ---- neighbourhood topology of the neighbour kinds ----
     // This rank's in-edges in recv-block order, each (source rank, index of
@@ -442,6 +513,8 @@ class Communicator : public std::enable_shared_from_this<Communicator>
                      int maxOutDegree,
                      int maxInDegree);
     bool hasNeighbors() const { return topo_ != nullptr; }
+    // This rank's (in-degree, out-degree); (0, 0) without a topology
+    std::pair<int, int> neighborDegrees() const;
 
     // ---- point to point (per-pair FIFO; no kernel ever spins on a peer) ----
     // Operations on one ordered pair must be issued in a consistent stream
@@ -688,6 +761,16 @@ class Communicator : public std::enable_shared_from_this<Communicator>
                      cudaStream_t s);
     int groupCheck(GroupKind kind, int dtype, int op, int root, int flags, bool& grouped) const;
     int launchNeighbor(const GroupLaunch& l, GroupKind kind, fb::GroupArgs& a, bool ss, int flags, cudaStream_t s);
+    int launchNeighborV(const GroupLaunch& l, GroupKind kind, fb::GroupArgs& a, bool ss, int flags, cudaStream_t s);
+    int neighborVCheck(GroupKind kind, const NeighborVItem* items, size_t nItems, int dtype, size_t& window) const;
+    int neighborVBatch(GroupKind kind,
+                       const NeighborVItem* items,
+                       size_t nItems,
+                       size_t esize,
+                       uint64_t agreed,
+                       std::vector<fb::GroupSeg>& segs,
+                       GroupLaunch& l) const;
+    int addPlanLaunch(GroupPlan& plan, const std::vector<fb::GroupSeg>& segs, GroupLaunch& l);
     int groupBatch(GroupKind kind,
                    const GroupItem* items,
                    size_t nItems,
@@ -735,6 +818,11 @@ class Communicator : public std::enable_shared_from_this<Communicator>
 // this limit 24, so a list of many items on a high-degree graph takes several
 // launches.  (The MPI layer runs graphs above the limit on its host path.)
 #define FB_NEIGHBOR_MAX_IN_DEGREE 4000
+// Largest out-degree plus in-degree of the neighbour v kinds: a launch's table
+// holds every stream of a rank, one entry per item and one more, so at this
+// limit a launch window holds 6 items.  (The MPI layer runs graphs above it
+// on its host path.)
+#define FB_NEIGHBOR_V_MAX_DEGREE 256
 
 // Error codes
 #define FB_OK 0

@@ -417,6 +417,32 @@ extern "C"
                                 int recvcount, MPI_Datatype recvtype, MPI_Comm comm, MPI_Request* request);
     int MPI_Ineighbor_alltoall(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf, int recvcount,
                                MPI_Datatype recvtype, MPI_Comm comm, MPI_Request* request);
+    /* The v variants (MPI-3.1 7.6.2): counts and displacements in elements of
+     * sendtype / recvtype.  Recv block j (recvcounts[j] at displs[j] or
+     * rdispls[j]) gets the whole send of sources[j] (allgatherv), or send
+     * block i (sendcounts[i] at sdispls[i]) of sources[j] for the edge that
+     * names this rank as destinations[i] (alltoallv).  A block's size must
+     * equal its peer's for the same edge.  MPI_IN_PLACE or a negative count
+     * or displacement gives MPI_ERR_ARG, a communicator without a dist-graph
+     * topology MPI_ERR_TOPOLOGY, both before anything is sent or launched.
+     * Where a call runs depends on buffer placement only (the send buffer, or
+     * the recv buffer on a rank without destinations), never on counts: every
+     * member passes device buffers or every member passes host buffers, as
+     * for the other device collectives; a member whose counts are all 0
+     * passes a buffer of the same kind too.  On the device, each blocking call
+     * or burst of non-blocking calls agrees on its launches with one host
+     * reduction over the members. */
+    int MPI_Neighbor_allgatherv(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf,
+                                const int recvcounts[], const int displs[], MPI_Datatype recvtype, MPI_Comm comm);
+    int MPI_Neighbor_alltoallv(const void* sendbuf, const int sendcounts[], const int sdispls[],
+                               MPI_Datatype sendtype, void* recvbuf, const int recvcounts[], const int rdispls[],
+                               MPI_Datatype recvtype, MPI_Comm comm);
+    int MPI_Ineighbor_allgatherv(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf,
+                                 const int recvcounts[], const int displs[], MPI_Datatype recvtype, MPI_Comm comm,
+                                 MPI_Request* request);
+    int MPI_Ineighbor_alltoallv(const void* sendbuf, const int sendcounts[], const int sdispls[],
+                                MPI_Datatype sendtype, void* recvbuf, const int recvcounts[], const int rdispls[],
+                                MPI_Datatype recvtype, MPI_Comm comm, MPI_Request* request);
     /* Persistent collectives (MPI-4.0).  Each init call refuses what the
      * matching MPI_I* call refuses, before anything is created, and fixes
      * where the call runs; info is ignored.  A completed start leaves the

@@ -703,6 +703,28 @@ class MpiWorld
     // The blocking call: one grouped launch, waited for (false: no comm)
     bool deviceNeighbor(const DeviceComm& comm, int rank, faabric::device::Communicator::GroupKind kind,
                         const uint8_t* send, uint8_t* recv, size_t bytes);
+    // One MPI_Neighbor_allgatherv / MPI_Neighbor_alltoallv call in bytes
+    // (FB_U8 elements): an out-edge's count and displacement per send entry
+    // (the all-gather: one count), an in-edge's per recv entry.  The vectors
+    // are the call's own, so a deferred call outlives the caller's arrays.
+    struct NeighborVCall
+    {
+        const uint8_t* send;
+        uint8_t* recv;
+        std::vector<size_t> sendCounts, sendDispls, recvCounts, recvDispls;
+    };
+    // The host agreement of a v list over the communicator's members:
+    // `agreed` gets the elementwise maximum of every member's `mine`
+    using NeighborVAgree = std::function<void(const std::vector<uint64_t>& mine, std::vector<uint64_t>& agreed)>;
+    // MPI_Ineighbor_allgatherv / MPI_Ineighbor_alltoallv (`kind` a neighbour
+    // v GroupKind), with nbNeighbor's rules.  A burst of them is agreed on
+    // once, at its flush; with grouping off each call is agreed on at issue.
+    int nbNeighborV(const DeviceComm& comm, int rank, faabric::device::Communicator::GroupKind kind,
+                    NeighborVCall call, const NeighborVAgree& agree, const HostPath& host);
+    // The blocking call: one agreement, then the window's launches, waited
+    // for (false: no comm, or the communicator declines the call)
+    bool deviceNeighborV(const DeviceComm& comm, int rank, faabric::device::Communicator::GroupKind kind,
+                         const NeighborVCall& call, const NeighborVAgree& agree);
     // Issues this rank thread's pending burst if it is keyed to `comm`, and
     // waits for it (before `comm` is released: MPI_Comm_free)
     void settleDeviceBurst(const DeviceComm& comm);

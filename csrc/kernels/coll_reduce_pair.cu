@@ -70,6 +70,9 @@ cudaError_t preloadAllKernels()
         e = preloadNeighborKernels();
     }
     if (e == cudaSuccess) {
+        e = preloadNeighborVKernels();
+    }
+    if (e == cudaSuccess) {
         e = preloadMoveBulkKernel();
     }
     if (e == cudaSuccess) {

@@ -100,6 +100,10 @@ struct GroupArgs
     // follow the segments in the table, and the send blocks it stages
     uint32_t nEdges;
     uint32_t outDeg;
+    // neighbour v kinds only (see NeighborVSeg): the round's first stream
+    // byte and its width
+    uint64_t vBase;
+    uint64_t vWidth;
 };
 
 // vectors per warp-chunk for a world of n ranks (host and kernel must agree)
@@ -229,6 +233,41 @@ struct NeighborEdge
 #define FB_NEIGHBOR_EDGE_SLOTS(n) (((uint32_t)(n) + 3u) / 4u)
 cudaError_t launchGroupNeighbor(const GroupArgs& a, bool allToAll, int blocks, int threads, cudaStream_t stream);
 cudaError_t preloadNeighborKernels();
+
+// ---- grouped neighbourhood v-collectives: many MPI_Neighbor_allgatherv /
+// MPI_Neighbor_alltoallv calls, with a size per edge, ONE launch per round ----
+// A launch window of nSegs items.  A rank has S send streams (all-to-all: one
+// per out-edge, S = outDeg; all-gather: S = min(outDeg, 1)) and nEdges recv
+// streams, one per in-edge.  Stream k is the concatenation, in item order, of
+// the window's blocks of its edge.  The table holds, per stream, nSegs + 1
+// NeighborVSeg entries: {address of item m's block, offset of that block in
+// the stream}, and last {0, length of the stream}.  The send streams come
+// first, then the recv streams, then this rank's in-edges (NeighborEdge).  A round moves stream bytes [vBase, vBase + vWidth); staging slot
+// k (all-gather: 0) holds those bytes of send stream k at k * vWidth.  The
+// receiver of an edge knows its source's stream layout from its own recv
+// counts, which MPI requires to match the sender's, so no displacement
+// crosses ranks.  Chunk c (FB_NEIGHBOR_CHUNK bytes, totalChunks = vWidth /
+// CB per slot) of slot k is staged and pulled by warp (k * totalChunks + c) %
+// warps of the grid on every rank.
+//   LOCAL: stage the round's bytes of every send stream
+//   entry barrier
+//   MOVE:  in-edge j = (src, idx) fills the round's bytes of recv stream j
+//          from src's slot idx.  One rank: straight from send stream idx, no
+//          staging and no barrier.
+//   exit barrier
+// With noSync the launch runs the steps of `phase` with no barrier.
+struct NeighborVSeg
+{
+    uint64_t addr; // this rank's address of the item's block (0: empty block)
+    uint64_t off;  // the block's first byte in the stream
+};
+static_assert(2 * sizeof(NeighborVSeg) == sizeof(GroupSeg), "two v entries per GroupSeg slot");
+// GroupSeg slots of a v table of `streams` streams over n items, with nEdges
+// in-edges right after the last entry
+#define FB_NEIGHBOR_V_SLOTS(streams, n, nEdges)                                                                        \
+    (((uint32_t)(streams) * ((uint32_t)(n) + 1u) * 16u + (uint32_t)(nEdges) * 8u + 31u) / 32u)
+cudaError_t launchGroupNeighborV(const GroupArgs& a, bool allToAll, int blocks, int threads, cudaStream_t stream);
+cudaError_t preloadNeighborVKernels();
 
 struct ReduceLaunchers
 {

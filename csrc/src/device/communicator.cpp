@@ -1251,6 +1251,7 @@ const fb::KernelTable CUDA_KERNELS = {
     .groupReduce = cudaGroupReduce,
     .groupScan = cudaGroupScan,
     .groupNeighbor = fb::launchGroupNeighbor,
+    .groupNeighborV = fb::launchGroupNeighborV,
     .move = fb::launchMove,
     .moveBulk = fb::launchMoveBulk,
     .barrier = fb::launchBarrier,
@@ -1281,6 +1282,7 @@ const fb::KernelTable HOST_KERNELS = {
     .groupReduce = fb::host::groupReduce,
     .groupScan = fb::host::groupScan,
     .groupNeighbor = fb::host::groupNeighbor,
+    .groupNeighborV = fb::host::groupNeighborV,
     .move = fb::host::moveKernel,
     .moveBulk = fb::host::moveBulk,
     .barrier = fb::host::barrierKernel,
@@ -1810,6 +1812,10 @@ struct Communicator::GroupLaunch
     uint64_t bytes = 0;
     // rooted kinds: an item of the launch has no send (bit 0) / no recv (bit 1)
     uint32_t missing = 0;
+    // kernel launches: a neighbour v window runs as `rounds` launches of
+    // `width` stream bytes each
+    uint32_t rounds = 1;
+    uint64_t width = 0;
 };
 
 // A neighbourhood topology (setNeighbors)
@@ -1906,7 +1912,11 @@ Communicator::ManySlot* Communicator::nextManySlot()
 
 size_t Communicator::groupPlanLaunches(const GroupPlan& plan)
 {
-    return plan.launches.size();
+    size_t n = 0;
+    for (const auto& l : plan.launches) {
+        n += l.rounds;
+    }
+    return n;
 }
 
 namespace {
@@ -2092,6 +2102,16 @@ static bool neighborKind(Communicator::GroupKind kind)
     return kind == Communicator::GROUP_NEIGHBOR_ALLGATHER || kind == Communicator::GROUP_NEIGHBOR_ALLTOALL;
 }
 
+static bool neighborVKind(Communicator::GroupKind kind)
+{
+    return kind == Communicator::GROUP_NEIGHBOR_ALLGATHERV || kind == Communicator::GROUP_NEIGHBOR_ALLTOALLV;
+}
+
+std::pair<int, int> Communicator::neighborDegrees() const
+{
+    return topo_ != nullptr ? std::pair<int, int>{ (int)topo_->in.size(), (int)topo_->outDeg } : std::pair<int, int>{ 0, 0 };
+}
+
 int Communicator::setNeighbors(const std::vector<std::pair<int, int>>& inEdges,
                                int outDegree,
                                int maxOutDegree,
@@ -2253,34 +2273,41 @@ std::shared_ptr<Communicator::GroupPlan> Communicator::prepareGroup(
         if (rc != FB_OK) {
             return nullptr;
         }
-        stats_.segTables++;
-        // (a rank may own nothing of a tiny group: it still takes part in the
-        // barriers, with an empty table)
-        const size_t tb = std::max<size_t>(segs.size(), 1) * sizeof(fb::GroupSeg);
-        if (loop_) {
-            plan->hostTables = true;
-            l.dSegs = (fb::GroupSeg*)::malloc(tb);
-            if (!segs.empty()) {
-                memcpy(l.dSegs, segs.data(), segs.size() * sizeof(fb::GroupSeg));
-            }
-            plan->launches.push_back(l);
-            continue;
-        }
-        if (cudaMalloc((void**)&l.dSegs, tb) != cudaSuccess) {
-            cudaGetLastError();
-            rc = FB_E_CUDA;
-            return nullptr;
-        }
-        plan->launches.push_back(l);
-        if (!segs.empty() &&
-            cudaMemcpy(l.dSegs, segs.data(), segs.size() * sizeof(fb::GroupSeg), cudaMemcpyHostToDevice) !=
-              cudaSuccess) {
-            cudaGetLastError();
-            rc = FB_E_CUDA;
+        rc = addPlanLaunch(*plan, segs, l);
+        if (rc != FB_OK) {
             return nullptr;
         }
     }
     return plan;
+}
+
+// Uploads one launch's table into a plan, which owns it from then on
+int Communicator::addPlanLaunch(GroupPlan& plan, const std::vector<fb::GroupSeg>& segs, GroupLaunch& l)
+{
+    stats_.segTables++;
+    // (a rank may own nothing of a tiny group: it still takes part in the
+    // barriers, with an empty table)
+    const size_t tb = std::max<size_t>(segs.size(), 1) * sizeof(fb::GroupSeg);
+    if (loop_) {
+        plan.hostTables = true;
+        l.dSegs = (fb::GroupSeg*)::malloc(tb);
+        if (!segs.empty()) {
+            memcpy(l.dSegs, segs.data(), segs.size() * sizeof(fb::GroupSeg));
+        }
+        plan.launches.push_back(l);
+        return FB_OK;
+    }
+    if (cudaMalloc((void**)&l.dSegs, tb) != cudaSuccess) {
+        cudaGetLastError();
+        return FB_E_CUDA;
+    }
+    plan.launches.push_back(l);
+    if (!segs.empty() &&
+        cudaMemcpy(l.dSegs, segs.data(), segs.size() * sizeof(fb::GroupSeg), cudaMemcpyHostToDevice) != cudaSuccess) {
+        cudaGetLastError();
+        return FB_E_CUDA;
+    }
+    return FB_OK;
 }
 
 static int groupGrid(const CommConfig& cfg, int nranks, uint64_t vecsPerRank)
@@ -2321,6 +2348,9 @@ int Communicator::launchGroup(const GroupLaunch& l,
     }
     if (neighborKind(kind)) {
         return launchNeighbor(l, kind, a, ss, flags, s);
+    }
+    if (neighborVKind(kind)) {
+        return launchNeighborV(l, kind, a, ss, flags, s);
     }
     if (ss && streamBarrier(flags, s) != FB_OK) {
         return FB_E_CUDA;
@@ -2488,6 +2518,8 @@ const GroupKindNames kGroupNames[] = {
     FB_GROUP_NAMES("scan", "scan"), FB_GROUP_NAMES("exscan", "exscan"),
     FB_GROUP_NAMES("neighborAllGather", "neighbor-allgather"),
     FB_GROUP_NAMES("neighborAllToAll", "neighbor-alltoall"),
+    FB_GROUP_NAMES("neighborAllGatherV", "neighbor-allgatherv"),
+    FB_GROUP_NAMES("neighborAllToAllV", "neighbor-alltoallv"),
 };
 #undef FB_GROUP_NAMES
 
@@ -2497,7 +2529,7 @@ const int GROUP_NOTHING = 1;
 
 const char* Communicator::groupKindName(GroupKind kind)
 {
-    return kind >= GROUP_ALLREDUCE && kind <= GROUP_NEIGHBOR_ALLTOALL ? kGroupNames[kind].name : "unknown";
+    return kind >= GROUP_ALLREDUCE && kind <= GROUP_NEIGHBOR_ALLTOALLV ? kGroupNames[kind].name : "unknown";
 }
 
 // The rules runGroup and groupMany share (see the header).  FB_OK, with
@@ -2533,12 +2565,17 @@ int Communicator::groupCheck(GroupKind kind, int dtype, int op, int root, int fl
             return FB_E_INVALID;
         }
     }
-    if (neighborKind(kind)) {
+    if (neighborKind(kind) || neighborVKind(kind)) {
         if (topo_ == nullptr || FB_FLAG_GET_CHANNEL(flags) != 0) {
             return FB_E_INVALID;
         }
+        if (neighborVKind(kind) && topo_->maxOutDeg + topo_->maxInDeg > FB_NEIGHBOR_V_MAX_DEGREE) {
+            return FB_E_TOO_LARGE;
+        }
         // (the all-to-all stages a chunk per slot at least)
-        const uint64_t slots = kind == GROUP_NEIGHBOR_ALLTOALL ? std::max<uint32_t>(topo_->maxOutDeg, 1) : 1;
+        const uint64_t slots = kind == GROUP_NEIGHBOR_ALLTOALL || kind == GROUP_NEIGHBOR_ALLTOALLV
+                                 ? std::max<uint32_t>(topo_->maxOutDeg, 1)
+                                 : 1;
         if (std::min<uint64_t>(cfg_.stageBytes, (uint64_t)1 << 31) / FB_NEIGHBOR_CHUNK < slots) {
             return FB_E_TOO_LARGE;
         }
@@ -2714,6 +2751,302 @@ int Communicator::groupPerItem(GroupKind kind,
             return rc;
         }
     }
+    return FB_OK;
+}
+
+// ---------------------------------------------------------------------------
+// Grouped neighbourhood v-collectives
+// ---------------------------------------------------------------------------
+// Send streams of a rank with `outDeg` out-edges
+static uint32_t neighborVSends(Communicator::GroupKind kind, uint32_t outDeg)
+{
+    return kind == Communicator::GROUP_NEIGHBOR_ALLTOALLV ? outDeg : std::min(outDeg, 1u);
+}
+
+// This rank's streams over items[0..n): the table entries (send streams, then
+// recv streams, n + 1 entries each, NeighborVSeg in launch_api.h) into `out`
+// when given, and the length of the longest stream
+static uint64_t neighborVEntries(bool allToAll,
+                                 uint32_t sends,
+                                 size_t inDeg,
+                                 const Communicator::NeighborVItem* items,
+                                 size_t n,
+                                 size_t esize,
+                                 std::vector<fb::NeighborVSeg>* out)
+{
+    uint64_t longest = 0;
+    auto stream = [&](auto count, auto addr) {
+        uint64_t off = 0;
+        for (size_t m = 0; m < n; m++) {
+            const uint64_t bytes = (uint64_t)count(items[m]) * esize;
+            if (out != nullptr) {
+                out->push_back(fb::NeighborVSeg{ bytes > 0 ? addr(items[m]) : 0, off });
+            }
+            off += bytes;
+        }
+        if (out != nullptr) {
+            out->push_back(fb::NeighborVSeg{ 0, off });
+        }
+        longest = std::max(longest, off);
+    };
+    for (uint32_t k = 0; k < sends; k++) {
+        stream([&](const Communicator::NeighborVItem& it) { return it.sendCounts[k]; },
+               [&](const Communicator::NeighborVItem& it) {
+                   return (uint64_t)(uintptr_t)it.send + (allToAll ? it.sendDispls[k] * esize : 0);
+               });
+    }
+    for (size_t j = 0; j < inDeg; j++) {
+        stream([&](const Communicator::NeighborVItem& it) { return it.recvCounts[j]; },
+               [&](const Communicator::NeighborVItem& it) { return (uint64_t)(uintptr_t)it.recv + it.recvDispls[j] * esize; });
+    }
+    return longest;
+}
+
+// The refusals of a v list that do not depend on the agreement (see the
+// header), and its items per launch window: the streams of the largest
+// degrees, n + 1 entries each, and the largest in-degree's edges fill at most
+// FB_GROUP_MAX_SEGS slots, so every member cuts alike.  window 0: no member has
+// an edge.
+int Communicator::neighborVCheck(GroupKind kind, const NeighborVItem* items, size_t nItems, int dtype, size_t& window)
+  const
+{
+    window = 0;
+    bool grouped = false;
+    const int rc = neighborVKind(kind) ? groupCheck(kind, dtype, 0, 0, 0, grouped) : FB_E_INVALID;
+    if (rc != FB_OK) {
+        return rc == GROUP_NOTHING ? FB_OK : rc;
+    }
+    const NeighborTopo& t = *topo_;
+    const uint32_t sends = neighborVSends(kind, t.outDeg);
+    const bool a2a = kind == GROUP_NEIGHBOR_ALLTOALLV;
+    for (size_t i = 0; i < nItems; i++) {
+        const NeighborVItem& it = items[i];
+        if ((sends > 0 && (it.sendCounts == nullptr || (a2a && it.sendDispls == nullptr))) ||
+            (!t.in.empty() && (it.recvCounts == nullptr || it.recvDispls == nullptr))) {
+            return FB_E_INVALID;
+        }
+        for (uint32_t k = 0; k < sends; k++) {
+            if (it.sendCounts[k] != 0 && it.send == nullptr) {
+                return FB_E_INVALID;
+            }
+        }
+        for (size_t j = 0; j < t.in.size(); j++) {
+            if (it.recvCounts[j] != 0 && it.recv == nullptr) {
+                return FB_E_INVALID;
+            }
+        }
+    }
+    const uint64_t streams = neighborVSends(kind, t.maxOutDeg) + t.maxInDeg;
+    const uint64_t entries =
+      ((uint64_t)FB_GROUP_MAX_SEGS * sizeof(fb::GroupSeg) - (uint64_t)t.maxInDeg * sizeof(fb::NeighborEdge)) /
+      sizeof(fb::NeighborVSeg);
+    // (FB_NEIGHBOR_V_MAX_DEGREE leaves room for several items)
+    window = std::min<size_t>(entries / streams - 1, GROUP_ITEMS_PER_LAUNCH);
+    return FB_OK;
+}
+
+int Communicator::neighborVStreams(GroupKind kind,
+                                   const NeighborVItem* items,
+                                   size_t nItems,
+                                   int dtype,
+                                   std::vector<uint64_t>& out) const
+{
+    out.clear();
+    size_t window = 0;
+    const int rc = neighborVCheck(kind, items, nItems, dtype, window);
+    if (rc != FB_OK || window == 0) {
+        return rc;
+    }
+    const uint32_t sends = neighborVSends(kind, topo_->outDeg);
+    for (size_t b = 0; b < nItems; b += window) {
+        out.push_back(neighborVEntries(kind == GROUP_NEIGHBOR_ALLTOALLV, sends, topo_->in.size(), items + b,
+                                       std::min(window, nItems - b), fbDtypeSize(dtype), nullptr));
+    }
+    return FB_OK;
+}
+
+// One launch window, items[0..n): this rank's table in `segs` and the
+// window's rounds in `l`.  `agreed` (> 0) is the window's longest stream over
+// every member.
+int Communicator::neighborVBatch(GroupKind kind,
+                                 const NeighborVItem* items,
+                                 size_t n,
+                                 size_t esize,
+                                 uint64_t agreed,
+                                 std::vector<fb::GroupSeg>& segs,
+                                 GroupLaunch& l) const
+{
+    const NeighborTopo& t = *topo_;
+    const bool a2a = kind == GROUP_NEIGHBOR_ALLTOALLV;
+    const uint32_t sends = neighborVSends(kind, t.outDeg);
+    std::vector<fb::NeighborVSeg> entries;
+    neighborVEntries(a2a, sends, t.in.size(), items, n, esize, &entries);
+    // A slot's room in whole chunks (the all-to-all shares the staging buffer
+    // among the largest out-degree's slots), at most the agreed stream
+    const uint64_t cb = FB_NEIGHBOR_CHUNK;
+    const uint64_t slots = a2a ? std::max<uint32_t>(t.maxOutDeg, 1) : 1;
+    const uint64_t room = std::min<uint64_t>(cfg_.stageBytes, (uint64_t)1 << 31) / cb / slots * cb;
+    l.width = std::min(room, (agreed + cb - 1) / cb * cb);
+    l.rounds = (uint32_t)((agreed + l.width - 1) / l.width);
+    l.totalChunks = (uint32_t)(l.width / cb);
+    l.nSegs = (uint32_t)n;
+    l.bytes = 0;
+    for (size_t j = 0; j < t.in.size(); j++) {
+        l.bytes += entries[(sends + j) * (n + 1) + n].off;
+    }
+    segs.assign(FB_NEIGHBOR_V_SLOTS(sends + t.in.size(), n, t.in.size()), fb::GroupSeg{});
+    memcpy(segs.data(), entries.data(), entries.size() * sizeof(fb::NeighborVSeg));
+    memcpy(reinterpret_cast<uint8_t*>(segs.data()) + entries.size() * sizeof(fb::NeighborVSeg), t.in.data(),
+           t.in.size() * sizeof(fb::NeighborEdge));
+    return FB_OK;
+}
+
+// Whether `agreed` is an agreement this rank can take: one entry per window,
+// none below this rank's own streams
+static bool neighborVAgrees(const std::vector<uint64_t>& mine, const std::vector<uint64_t>& agreed)
+{
+    if (mine.size() != agreed.size()) {
+        return false;
+    }
+    for (size_t w = 0; w < mine.size(); w++) {
+        if (mine[w] > agreed[w]) {
+            return false;
+        }
+    }
+    return true;
+}
+
+std::shared_ptr<Communicator::GroupPlan> Communicator::prepareGroup(const NeighborVItem* items,
+                                                                    size_t nItems,
+                                                                    int dtype,
+                                                                    const std::vector<uint64_t>& agreed,
+                                                                    int* rcOut,
+                                                                    GroupKind kind)
+{
+    int rcLocal = FB_OK;
+    int& rc = rcOut ? *rcOut : rcLocal;
+    std::vector<uint64_t> mine;
+    rc = neighborVStreams(kind, items, nItems, dtype, mine);
+    if (rc != FB_OK) {
+        return nullptr;
+    }
+    if (!neighborVAgrees(mine, agreed)) {
+        rc = FB_E_INVALID;
+        return nullptr;
+    }
+    bindDevice();
+    auto plan = std::make_shared<GroupPlan>();
+    plan->kind = kind;
+    plan->dtype = dtype;
+    plan->device = device_;
+    plan->items = nItems;
+    size_t window = 0;
+    neighborVCheck(kind, items, nItems, dtype, window);
+    for (size_t w = 0; w < agreed.size(); w++) {
+        if (agreed[w] == 0) {
+            continue;
+        }
+        const size_t b = w * window;
+        std::vector<fb::GroupSeg> segs;
+        GroupLaunch l;
+        rc = neighborVBatch(kind, items + b, std::min(window, nItems - b), fbDtypeSize(dtype), agreed[w], segs, l);
+        rc = rc == FB_OK ? addPlanLaunch(*plan, segs, l) : rc;
+        if (rc != FB_OK) {
+            return nullptr;
+        }
+    }
+    return plan;
+}
+
+int Communicator::groupMany(GroupKind kind,
+                            const NeighborVItem* items,
+                            size_t nItems,
+                            int dtype,
+                            const std::vector<uint64_t>& agreed,
+                            int flags,
+                            cudaStream_t s)
+{
+    if (!neighborVKind(kind)) {
+        return FB_E_INVALID;
+    }
+    NvtxRange nvtxRange(kGroupNames[kind].many);
+    bool grouped = false;
+    int rc = groupCheck(kind, dtype, 0, 0, flags, grouped);
+    if (rc != FB_OK) {
+        return rc == GROUP_NOTHING ? FB_OK : rc;
+    }
+    std::vector<uint64_t> mine;
+    rc = neighborVStreams(kind, items, nItems, dtype, mine);
+    if (rc != FB_OK) {
+        return rc;
+    }
+    if (!neighborVAgrees(mine, agreed)) {
+        return FB_E_INVALID;
+    }
+    bindDevice();
+    size_t window = 0;
+    neighborVCheck(kind, items, nItems, dtype, window);
+    for (size_t w = 0; w < agreed.size(); w++) {
+        if (agreed[w] == 0) {
+            continue;
+        }
+        const size_t b = w * window;
+        std::vector<fb::GroupSeg> segs;
+        GroupLaunch l;
+        neighborVBatch(kind, items + b, std::min(window, nItems - b), fbDtypeSize(dtype), agreed[w], segs, l);
+        stats_.segTables++;
+        ManySlot* slot = nullptr;
+        l.dSegs = (fb::GroupSeg*)stageManyTable(segs.data(), segs.size() * sizeof(fb::GroupSeg), s, &slot);
+        if (l.dSegs == nullptr && !loop_) {
+            return FB_E_CUDA;
+        }
+        rc = launchGroup(l, kind, dtype, 0, 0, flags, s);
+        if (rc != FB_OK) {
+            return rc;
+        }
+        releaseManySlot(slot, s);
+    }
+    return FB_OK;
+}
+
+// A window's rounds: each is a launch, LOCAL, barrier, MOVE, barrier (two
+// launches around stream-ordered barriers).  The grid follows from the
+// window's chunks per slot and the largest degrees, the same on every rank.
+int Communicator::launchNeighborV(const GroupLaunch& l, GroupKind kind, fb::GroupArgs& a, bool ss, int flags,
+                                  cudaStream_t s)
+{
+    const NeighborTopo& t = *topo_;
+    const bool a2a = kind == GROUP_NEIGHBOR_ALLTOALLV;
+    a.stageOff = stageSendOff_;
+    a.nEdges = (uint32_t)t.in.size();
+    a.outDeg = t.outDeg;
+    a.vWidth = l.width;
+    const uint64_t warps = (uint64_t)cfg_.threads / 32;
+    const uint64_t units = (uint64_t)l.totalChunks * std::max(neighborVSends(kind, t.maxOutDeg), t.maxInDeg);
+    const int blocks = (int)std::clamp<uint64_t>(
+      (units + warps - 1) / warps, 1, (uint64_t)groupGrid(cfg_, dev_.nranks, units * (FB_NEIGHBOR_CHUNK / 16)));
+    auto run = [&](int phase) {
+        a.phase = phase;
+        return k_->groupNeighborV(a, a2a, blocks, cfg_.threads, s) == cudaSuccess ? FB_OK : FB_E_CUDA;
+    };
+    for (uint32_t r = 0; r < l.rounds; r++) {
+        a.vBase = (uint64_t)r * l.width;
+        int rc;
+        if (!ss) {
+            rc = run(GROUP_PHASE_LOCAL | GROUP_PHASE_MOVE);
+        } else {
+            rc = run(GROUP_PHASE_LOCAL);
+            rc = rc == FB_OK ? streamBarrier(flags, s) : rc;
+            rc = rc == FB_OK ? run(GROUP_PHASE_MOVE) : rc;
+            rc = rc == FB_OK ? streamBarrier(flags, s) : rc;
+            stats_.stagedCopies++;
+        }
+        if (rc != FB_OK) {
+            return FB_E_CUDA;
+        }
+        stats_.launches++;
+    }
+    stats_.bytes += l.bytes;
     return FB_OK;
 }
 

@@ -746,6 +746,62 @@ cudaError_t groupNeighbor(const GroupArgs& a, bool allToAll, int blocks, int, cu
     return cudaSuccess;
 }
 
+// The twin of groupNeighborVKernel: the round's bytes [vBase, vBase + vWidth)
+// of every stream, between the streams' blocks and the staging slots
+cudaError_t groupNeighborV(const GroupArgs& a, bool allToAll, int blocks, int, cudaStream_t)
+{
+    const FbCommDev& c = a.comm;
+    if ((uintptr_t)(c.heap[c.rank] + a.stageOff) & 15) {
+        return cudaErrorMisalignedAddress;
+    }
+    const uint32_t n = a.nSegs;
+    const uint32_t sends = allToAll ? a.outDeg : std::min(a.outDeg, 1u);
+    const NeighborVSeg* tbl = reinterpret_cast<const NeighborVSeg*>(a.segs);
+    const NeighborEdge* edges = reinterpret_cast<const NeighborEdge*>(tbl + (uint64_t)(sends + a.nEdges) * (n + 1));
+    const bool direct = c.nranks == 1;
+    const uint64_t W = a.vWidth;
+    // stream bytes [pos, end) of stream e (n + 1 entries), block by block,
+    // to or from the flat range whose byte pos is at flat + pos - vBase
+    auto walk = [&](const NeighborVSeg* e, uint64_t pos, uint64_t end, auto&& copy) {
+        for (uint32_t m = 0; m < n && pos < end; m++) {
+            const uint64_t from = std::max(pos, e[m].off);
+            const uint64_t to = std::min(end, e[m + 1].off);
+            if (from < to) {
+                copy(reinterpret_cast<uint8_t*>(e[m].addr) + (from - e[m].off), from, to - from);
+            }
+        }
+    };
+    if (!direct && (a.phase & GROUP_PHASE_LOCAL)) {
+        for (uint32_t k = 0; k < sends; k++) {
+            const NeighborVSeg* e = tbl + (uint64_t)k * (n + 1);
+            uint8_t* const slot = c.heap[c.rank] + a.stageOff + k * W;
+            walk(e, a.vBase, std::min(a.vBase + W, e[n].off),
+                 [&](uint8_t* user, uint64_t p, uint64_t len) { memcpy(slot + (p - a.vBase), user, len); });
+        }
+    }
+    bool ok = a.noSync || gridBarrier(c, blocks);
+    if (ok && (a.phase & GROUP_PHASE_MOVE)) {
+        for (uint32_t j = 0; j < a.nEdges; j++) {
+            const uint64_t k = allToAll ? edges[j].idx : 0;
+            const NeighborVSeg* re = tbl + (uint64_t)(sends + j) * (n + 1);
+            const NeighborVSeg* se = tbl + k * (n + 1);
+            const uint64_t end = std::min(a.vBase + W, direct ? std::min(re[n].off, se[n].off) : re[n].off);
+            walk(re, a.vBase, end, [&](uint8_t* user, uint64_t p, uint64_t len) {
+                if (!direct) {
+                    memcpy(user, c.heap[edges[j].src] + a.stageOff + k * W + (p - a.vBase), len);
+                    return;
+                }
+                walk(se, p, p + len,
+                     [&](uint8_t* from, uint64_t q, uint64_t l2) { memcpy(user + (q - p), from, l2); });
+            });
+        }
+    }
+    if (!a.noSync) {
+        gridBarrier(c, blocks);
+    }
+    return cudaSuccess;
+}
+
 // The twin of groupReduceKernel: every rank stages its pieces; after the
 // entry barrier this rank folds the chunks it owns (the kernel's rule, with
 // the same grid) into the root's result slices; after the exit barrier the

@@ -25,6 +25,7 @@ struct KernelTable
     cudaError_t (*groupReduce)(const GroupArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s);
     cudaError_t (*groupScan)(const GroupArgs& a, int dtype, int op, int blocks, int threads, cudaStream_t s);
     cudaError_t (*groupNeighbor)(const GroupArgs& a, bool allToAll, int blocks, int threads, cudaStream_t s);
+    cudaError_t (*groupNeighborV)(const GroupArgs& a, bool allToAll, int blocks, int threads, cudaStream_t s);
     cudaError_t (*move)(const MoveArgs& a, int width, int blocks, int threads, cudaStream_t s);
     // TMA bulk-copy engine (fixed block size, 16-byte aligned ranges)
     cudaError_t (*moveBulk)(const MoveArgs& a, int blocks, cudaStream_t s);
@@ -72,6 +73,7 @@ cudaError_t groupScan(const GroupArgs& a, int dtype, int op, int blocks, int thr
 // this rank's staging buffer is not 16-byte aligned (the kernel stores whole
 // vectors there)
 cudaError_t groupNeighbor(const GroupArgs& a, bool allToAll, int blocks, int threads, cudaStream_t s);
+cudaError_t groupNeighborV(const GroupArgs& a, bool allToAll, int blocks, int threads, cudaStream_t s);
 // The move, p2p and put twins return cudaErrorMisalignedAddress, before they
 // copy or synchronise, when an address the kernel reads or writes in words of
 // `width` bytes is not aligned to it (moveBulk: 16 bytes)

@@ -140,6 +140,10 @@ struct RankState
     void* groupStream = nullptr;
     std::vector<faabric::device::Communicator::GroupItem> groupItems;
     std::vector<int> groupRequests;
+    // A burst of a neighbour v kind: its calls (groupItems then holds one
+    // placeholder per call) and how its members agree on the launch rounds
+    std::vector<MpiWorld::NeighborVCall> groupVCalls;
+    MpiWorld::NeighborVAgree groupAgree;
     // every call of the pending burst is a persistent start
     bool groupAllPersistent = false;
     // Plans of such bursts, most recently used first, and plans dropped from
@@ -179,6 +183,8 @@ struct RankState
         groupComm = nullptr;
         groupItems.clear();
         groupRequests.clear();
+        groupVCalls.clear();
+        groupAgree = nullptr;
         groupAllPersistent = false;
         plans.clear();
         retiredPlans.clear();
@@ -1072,6 +1078,40 @@ static int runPersistentBurst(faabric::device::Communicator& comm,
     return rc;
 }
 
+static bool neighborVKind(faabric::device::Communicator::GroupKind kind)
+{
+    return kind == faabric::device::Communicator::GROUP_NEIGHBOR_ALLGATHERV ||
+           kind == faabric::device::Communicator::GROUP_NEIGHBOR_ALLTOALLV;
+}
+
+// A list of neighbour v calls on `c`: one host agreement on every launch
+// window's longest stream, then its launches.  Every member runs it at the
+// same program point with the same number of calls, so every member agrees
+// on the same number of windows.
+static int runNeighborV(faabric::device::Communicator& c,
+                        faabric::device::Communicator::GroupKind kind,
+                        const std::vector<MpiWorld::NeighborVCall>& calls,
+                        const MpiWorld::NeighborVAgree& agree,
+                        cudaStream_t s)
+{
+    std::vector<faabric::device::Communicator::NeighborVItem> items;
+    items.reserve(calls.size());
+    for (const auto& v : calls) {
+        items.push_back({ v.send, v.recv, v.sendCounts.data(), v.sendDispls.data(), v.recvCounts.data(),
+                          v.recvDispls.data() });
+    }
+    std::vector<uint64_t> mine;
+    const int rc = c.neighborVStreams(kind, items.data(), items.size(), FB_U8, mine);
+    if (rc != FB_OK) {
+        return rc;
+    }
+    std::vector<uint64_t> agreed(mine.size(), 0);
+    if (!mine.empty()) {
+        agree(mine, agreed);
+    }
+    return c.groupMany(kind, items.data(), items.size(), FB_U8, agreed, 0, s);
+}
+
 // Issues the deferred burst of this rank thread as one grouped launch (every
 // rank defers and flushes at the same program points)
 static void flushPendingGroup()
@@ -1087,14 +1127,20 @@ static void flushPendingGroup()
     auto comm = tls.groupComm;
     auto items = std::move(tls.groupItems);
     auto reqs = std::move(tls.groupRequests);
+    auto vCalls = std::move(tls.groupVCalls);
+    auto agree = std::move(tls.groupAgree);
     tls.groupItems.clear();
     tls.groupRequests.clear();
+    tls.groupVCalls.clear();
+    tls.groupAgree = nullptr;
     tls.groupComm = nullptr;
     cudaSetDevice(comm->device());
     const cudaStream_t s = (cudaStream_t)tls.groupStream;
-    const int rc = tls.groupAllPersistent ? runPersistentBurst(*comm, items, reqs, s)
-                                          : comm->groupMany(tls.groupKind, items.data(), items.size(), tls.groupDtype,
-                                                            tls.groupOp, tls.groupRoot, FB_FLAG_SYMMETRIC, s);
+    const int rc = neighborVKind(tls.groupKind)  ? runNeighborV(*comm, tls.groupKind, vCalls, agree, s)
+                   : tls.groupAllPersistent      ? runPersistentBurst(*comm, items, reqs, s)
+                                                 : comm->groupMany(tls.groupKind, items.data(), items.size(),
+                                                                   tls.groupDtype, tls.groupOp, tls.groupRoot,
+                                                                   FB_FLAG_SYMMETRIC, s);
     if (rc != FB_OK) {
         const std::string what = std::string("Grouped device ") + Communicator::groupKindName(tls.groupKind);
         // (the burst's requests have no host path left: declining is an error too)
@@ -2066,6 +2112,42 @@ int MpiWorld::nbNeighbor(const DeviceComm& comm, int rank, faabric::device::Comm
         const faabric::device::Communicator::GroupItem item{ send, recv, bytes };
         return c.groupMany(kind, &item, 1, FB_U8, 0, 0, 0, st);
     }, host, 0);
+}
+
+int MpiWorld::nbNeighborV(const DeviceComm& comm, int rank, faabric::device::Communicator::GroupKind kind,
+                          NeighborVCall call, const NeighborVAgree& agree, const HostPath& host)
+{
+    cacheDeviceComm(rank);
+    const int requestId = tls.nextRequestId++;
+    AsyncRequest r = collectiveRequest(rank);
+    if (comm != nullptr && groupIallreduce) {
+        // the burst's key is (kind, communicator); a change of key flushes
+        // the pending burst before this call joins
+        const faabric::device::Communicator::GroupItem placeholder{ call.send, call.recv, 0 };
+        deferToGroup(kind, comm, FB_U8, -1, 0, placeholder, requestId, std::move(r), deviceCollectives);
+        tls.groupVCalls.push_back(std::move(call));
+        tls.groupAgree = agree;
+        return requestId;
+    }
+    void* s = tls.cachedStream0;
+    const std::vector<NeighborVCall> one{ call };
+    if (comm != nullptr && issueDevice(*comm, s, deviceCollectives, [&](auto& c, cudaStream_t st) {
+            return runNeighborV(c, kind, one, agree, st);
+        })) {
+        return recordDevice(requestId, std::move(r), comm, s);
+    }
+    host();
+    tls.requests[requestId] = std::move(r);
+    return requestId;
+}
+
+bool MpiWorld::deviceNeighborV(const DeviceComm& comm, int rank, faabric::device::Communicator::GroupKind kind,
+                               const NeighborVCall& call, const NeighborVAgree& agree)
+{
+    const std::vector<NeighborVCall> one{ call };
+    return issueAndWait(comm, streamForRank(rank), deviceCollectives, [&](auto& c, cudaStream_t s) {
+        return runNeighborV(c, kind, one, agree, s);
+    });
 }
 
 bool MpiWorld::deviceNeighbor(const DeviceComm& comm, int rank, faabric::device::Communicator::GroupKind kind,

@@ -2137,4 +2137,107 @@ int MPI_Ineighbor_alltoall(const void* sendbuf, int sendcount, MPI_Datatype send
     return neighborCall(true, sendbuf, sendcount, sendtype, recvbuf, recvcount, recvtype, comm, request);
 }
 
+// Blocking and non-blocking neighbourhood v-calls.  Where a call runs is
+// judged on buffer placement alone, with neighborCall's rule (a rank with all
+// counts zero still joins its peers' launches), and on degrees every member
+// holds alike; the device path agrees on its launch rounds over the members
+// with one host reduction per blocking call or per burst.  Counts and
+// displacements are checked before anything is sent or launched.
+static int neighborVCall(bool allToAll, const void* sendbuf, const int sendcounts[], const int sdispls[],
+                         MPI_Datatype sendtype, void* recvbuf, const int recvcounts[], const int rdispls[],
+                         MPI_Datatype recvtype, MPI_Comm comm, MPI_Request* request)
+{
+    if (sendbuf == MPI_IN_PLACE) {
+        return MPI_ERR_ARG;
+    }
+    std::shared_ptr<SubCommunicator> sub;
+    auto g = graphOf(comm, &sub);
+    if (g == nullptr) {
+        return MPI_ERR_TOPOLOGY;
+    }
+    MpiWorld& world = getExecutingWorld();
+    const int rank = executingContext.getRank();
+    const int cr = sub->commRankOf(rank);
+    const size_t outDeg = g->destinations[cr].size();
+    const size_t inDeg = g->in[cr].size();
+    const size_t sends = allToAll ? outDeg : 1;
+    MpiWorld::NeighborVCall call{ (const uint8_t*)sendbuf, (uint8_t*)recvbuf, {}, {}, {}, {} };
+    for (size_t i = 0; i < sends; i++) {
+        if (sendcounts[i] < 0 || (allToAll && sdispls[i] < 0)) {
+            return MPI_ERR_ARG;
+        }
+        call.sendCounts.push_back((size_t)sendcounts[i] * sendtype->size);
+        call.sendDispls.push_back(allToAll ? (size_t)sdispls[i] * sendtype->size : 0);
+    }
+    for (size_t j = 0; j < inDeg; j++) {
+        if (recvcounts[j] < 0 || rdispls[j] < 0) {
+            return MPI_ERR_ARG;
+        }
+        call.recvCounts.push_back((size_t)recvcounts[j] * recvtype->size);
+        call.recvDispls.push_back((size_t)rdispls[j] * recvtype->size);
+    }
+    const void* judged = outDeg == 0 ? recvbuf : sendbuf;
+    const bool device = g->maxIn + g->maxOut <= FB_NEIGHBOR_V_MAX_DEGREE && MpiWorld::isDevicePointer(judged);
+    auto dev = device ? sub->deviceComm(world, rank) : nullptr;
+    const auto kind = allToAll ? faabric::device::Communicator::GROUP_NEIGHBOR_ALLTOALLV
+                               : faabric::device::Communicator::GROUP_NEIGHBOR_ALLGATHERV;
+    // (the host path owns copies: a non-blocking call's arrays may go first)
+    const std::vector<int> sc(sendcounts, sendcounts + sends);
+    const std::vector<int> sd = allToAll ? std::vector<int>(sdispls, sdispls + sends) : std::vector<int>(1, 0);
+    const std::vector<int> rc(recvcounts, recvcounts + inDeg);
+    const std::vector<int> rd(rdispls, rdispls + inDeg);
+    const uint8_t* send = call.send;
+    uint8_t* recv = call.recv;
+    auto host = [=, &world] {
+        sub->neighborExchangeV(world, rank, allToAll, send, sc.data(), sd.data(), sendtype, recv, rc.data(), rd.data(),
+                               recvtype);
+    };
+    auto agree = [sub, &world, rank](const std::vector<uint64_t>& mine, std::vector<uint64_t>& agreed) {
+        sub->allReduce(world, rank, (const uint8_t*)mine.data(), (uint8_t*)agreed.data(), MPI_UINT64_T,
+                       (int)mine.size(), MPI_MAX);
+    };
+    if (request == nullptr) {
+        if (!world.deviceNeighborV(dev, rank, kind, call, agree)) {
+            host();
+        }
+        return MPI_SUCCESS;
+    }
+    return handOut(world.nbNeighborV(dev, rank, kind, std::move(call), agree, host), request);
+}
+
+int MPI_Neighbor_allgatherv(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf,
+                            const int recvcounts[], const int displs[], MPI_Datatype recvtype, MPI_Comm comm)
+{
+    SPDLOG_TRACE("MPI - MPI_Neighbor_allgatherv");
+    return neighborVCall(false, sendbuf, &sendcount, nullptr, sendtype, recvbuf, recvcounts, displs, recvtype, comm,
+                         nullptr);
+}
+
+int MPI_Neighbor_alltoallv(const void* sendbuf, const int sendcounts[], const int sdispls[], MPI_Datatype sendtype,
+                           void* recvbuf, const int recvcounts[], const int rdispls[], MPI_Datatype recvtype,
+                           MPI_Comm comm)
+{
+    SPDLOG_TRACE("MPI - MPI_Neighbor_alltoallv");
+    return neighborVCall(true, sendbuf, sendcounts, sdispls, sendtype, recvbuf, recvcounts, rdispls, recvtype, comm,
+                         nullptr);
+}
+
+int MPI_Ineighbor_allgatherv(const void* sendbuf, int sendcount, MPI_Datatype sendtype, void* recvbuf,
+                             const int recvcounts[], const int displs[], MPI_Datatype recvtype, MPI_Comm comm,
+                             MPI_Request* request)
+{
+    SPDLOG_TRACE("MPI - MPI_Ineighbor_allgatherv");
+    return neighborVCall(false, sendbuf, &sendcount, nullptr, sendtype, recvbuf, recvcounts, displs, recvtype, comm,
+                         request);
+}
+
+int MPI_Ineighbor_alltoallv(const void* sendbuf, const int sendcounts[], const int sdispls[], MPI_Datatype sendtype,
+                            void* recvbuf, const int recvcounts[], const int rdispls[], MPI_Datatype recvtype,
+                            MPI_Comm comm, MPI_Request* request)
+{
+    SPDLOG_TRACE("MPI - MPI_Ineighbor_alltoallv");
+    return neighborVCall(true, sendbuf, sendcounts, sdispls, sendtype, recvbuf, recvcounts, rdispls, recvtype, comm,
+                         request);
+}
+
 } // extern "C"

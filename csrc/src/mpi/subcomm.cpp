@@ -330,6 +330,31 @@ void SubCommunicator::neighborExchange(MpiWorld& w, int me, bool allToAll, const
     }
 }
 
+void SubCommunicator::neighborExchangeV(MpiWorld& w, int me, bool allToAll, const uint8_t* send,
+                                        const int* sendCounts, const int* sendDispls, faabric_datatype_t* sendType,
+                                        uint8_t* recv, const int* recvCounts, const int* recvDispls,
+                                        faabric_datatype_t* recvType)
+{
+    const int cr = commRankOf(me);
+    const auto& dst = topo->destinations[cr];
+    const auto& in = topo->in[cr];
+    auto sendBlock = [&](size_t i) { return send + (allToAll ? (size_t)sendDispls[i] * sendType->size : 0); };
+    for (size_t i = 0; i < dst.size(); i++) {
+        if (dst[i] != cr) {
+            w.send(me, worldRanks[dst[i]], sendBlock(i), sendType, sendCounts[allToAll ? i : 0]);
+        }
+    }
+    for (size_t j = 0; j < in.size(); j++) {
+        const auto [src, idx] = in[j];
+        uint8_t* block = recv + (size_t)recvDispls[j] * recvType->size;
+        if (src == cr) {
+            copyBytes(block, sendBlock(idx), (size_t)recvCounts[j] * recvType->size);
+        } else {
+            w.recv(worldRanks[src], me, block, recvType, recvCounts[j], nullptr);
+        }
+    }
+}
+
 std::shared_ptr<faabric::device::Communicator> SubCommunicator::currentDevice(int me)
 {
     std::lock_guard<std::mutex> lk(deviceMx);

@@ -105,6 +105,13 @@ class SubCommunicator
     // with the k-th; self-edges are local copies.  `count` x `dt` per block.
     void neighborExchange(MpiWorld& w, int me, bool allToAll, const uint8_t* send, uint8_t* recv,
                           faabric_datatype_t* dt, int count);
+    // MPI_Neighbor_allgatherv / MPI_Neighbor_alltoallv on the host path, in
+    // the same order: out-edge i sends sendCounts[i] x sendType at
+    // sendDispls[i] (the all-gather: sendCounts[0] at 0 on every edge), in-edge
+    // j receives recvCounts[j] x recvType at recvDispls[j]
+    void neighborExchangeV(MpiWorld& w, int me, bool allToAll, const uint8_t* send, const int* sendCounts,
+                           const int* sendDispls, faabric_datatype_t* sendType, uint8_t* recv, const int* recvCounts,
+                           const int* recvDispls, faabric_datatype_t* recvType);
 
     // ---- fused device path ----
     // This rank's child of its world device communicator over the members

@@ -126,6 +126,10 @@ def load():
     _sig(lib, "fb_group_plan_launches", i32, [vp])
     _sig(lib, "fb_group_plan_free", None, [vp])
     _sig(lib, "fb_comm_set_neighbors", i32, [vp, i32, C.POINTER(C.c_int), C.POINTER(C.c_int), i32, i32, i32])
+    _nv = [vp, i32, i32, vpp, vpp, u64p, u64p, i32, u64p, u64p, i32, i32]
+    _sig(lib, "fb_neighbor_v_streams", i32, _nv + [u64p, i32])
+    _sig(lib, "fb_group_prepare_v", vp, _nv + [u64p, i32])
+    _sig(lib, "fb_group_many_v", i32, _nv + [u64p, i32, i32, vp])
     _sig(lib, "fb_put_signal", i32, [vp, vp, u64, u64, i32, i32, i32, vp])
     _sig(lib, "fb_wait_signal", i32, [vp, i32, u32, vp])
     _sig(lib, "fb_accumulate", i32, [vp, vp, u64, u64, i32, i32, i32, vp, vp])

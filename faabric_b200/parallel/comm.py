@@ -98,6 +98,8 @@ GROUP_KINDS = {
     "exscan": 9,
     "neighbor_all_gather": 10,
     "neighbor_all_to_all": 11,
+    "neighbor_all_gather_v": 12,
+    "neighbor_all_to_all_v": 13,
 }
 ALGOS = {"auto": 0, "oneshot": 1, "twoshot": 2, "nvls": 3, "ll": 4}
 ALGO_NAMES = {v: k for k, v in ALGOS.items()}
@@ -947,6 +949,176 @@ class Communicator:
         :meth:`neighbor_all_to_all_group`."""
         self._neighbor_many("neighbor_all_to_all_many", "neighbor_all_to_all", sends, recvs, counts, dtype, stream)
 
+    # ------------------------------- neighbourhood v-collectives (per-edge sizes)
+    def _neighbor_v_items(self, what, kind, sends, recvs, sendcounts, sdispls, recvcounts, rdispls, dtype):
+        """The C arguments of a neighbour v list; raises before any native
+        call.  Counts and displacements are in elements of ``dtype`` (or of
+        the tensors' own dtype).  Item i: the all-gather's send holds
+        ``sendcounts[i]`` elements (default: all of it), the all-to-all's send
+        block k is ``sendcounts[i][k]`` elements at ``sdispls[i][k]``, one per
+        out-edge; recv block j is ``recvcounts[i][j]`` elements at
+        ``rdispls[i][j]``, one per in-edge.  A tensor may be None where all its
+        counts are 0."""
+        if self._neighbors is None:
+            raise CommError(f"{what}: no neighbourhood topology; call set_neighbors first")
+        indeg, outdeg = self._neighbors
+        a2a = kind == "neighbor_all_to_all_v"
+        n = len(sends) if sends is not None else 0
+        if n == 0 or recvs is None or len(recvs) != n:
+            raise CommError(f"{what}: need equally long, non-empty lists")
+        for name, v in (("recvcounts", recvcounts), ("rdispls", rdispls)) + (
+            (("sendcounts", sendcounts), ("sdispls", sdispls)) if a2a else ()
+        ):
+            if v is None or len(v) != n:
+                raise CommError(f"{what}: {name} needs one entry per item")
+        codes = set()
+        sw = outdeg if a2a else 1
+        sc, sd, rc, rd = [], [], [], []
+
+        def side(i, t, counts, displs, width, label):
+            counts = [int(x) for x in counts]
+            displs = [int(x) for x in displs]
+            if len(counts) != width or len(displs) != width:
+                raise CommError(f"{what}: item {i} needs {width} {label} counts and displacements")
+            if any(x < 0 for x in counts + displs):
+                raise CommError(f"{what}: item {i} has a negative {label} count or displacement")
+            if t is None:
+                if any(counts):
+                    raise CommError(f"{what}: item {i} has {label} counts but no {label} tensor")
+                return counts, displs
+            if not t.is_cuda or t.device.index != self.device or not t.is_contiguous():
+                raise CommError(f"{what}: item {i}: {label} must be a contiguous tensor on cuda:{self.device}")
+            numel, code = self._typed(t, dtype)
+            codes.add(code)
+            for c, d in zip(counts, displs):
+                if c and c + d > numel:
+                    raise CommError(f"{what}: item {i}: a {label} block of {c} at {d} overruns {numel} elements")
+            return counts, displs
+
+        for i in range(n):
+            s, r = sends[i], recvs[i]
+            if a2a:
+                c, d = side(i, s, sendcounts[i], sdispls[i], outdeg, "send")
+            else:
+                cnt = sendcounts[i] if sendcounts is not None else (self._typed(s, dtype)[0] if s is not None else 0)
+                c, d = side(i, s, [cnt], [0], 1, "send")
+            sc += c
+            sd += d
+            c, d = side(i, r, recvcounts[i], rdispls[i], indeg, "recv")
+            rc += c
+            rd += d
+        if len(codes) > 1:
+            raise CommError(f"{what}: every tensor must have the same dtype")
+        code = codes.pop() if codes else FB_DTYPES[dtype or "u8"][0]
+        u64 = lambda v: (C.c_uint64 * max(len(v), 1))(*v)  # noqa: E731
+        sp = (C.c_void_p * n)(*[(t.data_ptr() or None) if t is not None else None for t in sends])
+        rp = (C.c_void_p * n)(*[(t.data_ptr() or None) if t is not None else None for t in recvs])
+        return (self._h, GROUP_KINDS[kind], n, sp, rp, u64(sc), u64(sd), sw, u64(rc), u64(rd), indeg, code)
+
+    def _neighbor_v_streams(self, what, kind, args):
+        cap = len(args[3]) + 1
+        out = (C.c_uint64 * cap)()
+        w = self._lib.fb_neighbor_v_streams(*args, out, cap)
+        self._check(min(w, 0), what)
+        return [int(out[i]) for i in range(w)]
+
+    @staticmethod
+    def _agreed(agreed):
+        v = [int(x) for x in agreed]
+        return (C.c_uint64 * max(len(v), 1))(*v), len(v)
+
+    def _prepare_neighbor_v(self, what, kind, args, agreed, nbytes) -> "GroupPlan":
+        a, na = self._agreed(agreed)
+        h = self._lib.fb_group_prepare_v(*args, a, na)
+        if not h:
+            raise CommError(f"{what} failed [{_lib.last_error()}]")
+        plan = GroupPlan(self, h, args[2], nbytes)
+        plan.kind = kind
+        return plan
+
+    def _neighbor_v_many(self, what, args, agreed, stream):
+        a, na = self._agreed(agreed)
+        self._check(self._lib.fb_group_many_v(*args, a, na, 0, self._stream(stream)), what)
+
+    def neighbor_all_gather_v_streams(self, sends, recvs, recvcounts, rdispls, sendcounts=None, dtype=None):
+        """This rank's longest stream of every launch window of a neighbour
+        all-gatherv list, in bytes (see :meth:`prepare_neighbor_all_gather_v_group`).
+        Every member's lists are combined by an elementwise maximum, the
+        agreement (:meth:`LocalGroup.agree_neighbor_v` for a local group)."""
+        kind = "neighbor_all_gather_v"
+        args = self._neighbor_v_items(
+            "neighbor_all_gather_v_streams", kind, sends, recvs, sendcounts, None, recvcounts, rdispls, dtype
+        )
+        return self._neighbor_v_streams("neighbor_all_gather_v_streams", kind, args)
+
+    def prepare_neighbor_all_gather_v_group(
+        self, sends, recvs, recvcounts, rdispls, agreed, sendcounts=None, dtype=None
+    ) -> "GroupPlan":
+        """Plan MPI_Neighbor_allgatherv per item over this communicator's
+        topology: block j of ``recvs[i]`` (``recvcounts[i][j]`` elements at
+        ``rdispls[i][j]``) gets the send of in-edge j's source.  ``agreed`` is
+        the elementwise maximum over every member of their
+        :meth:`neighbor_all_gather_v_streams`; each launch window then takes
+        ``ceil(agreed[w] / W)`` launches, W the room of a staging slot.
+        Tensors are any device memory at any alignment; call collectively,
+        every member takes part, edges or not."""
+        what = "prepare_neighbor_all_gather_v_group"
+        kind = "neighbor_all_gather_v"
+        args = self._neighbor_v_items(what, kind, sends, recvs, sendcounts, None, recvcounts, rdispls, dtype)
+        nbytes = sum(t.numel() * t.element_size() for t in recvs if t is not None)
+        return self._prepare_neighbor_v(what, kind, args, agreed, nbytes)
+
+    def neighbor_all_gather_v_group(self, plan: "GroupPlan", stream=None, flags=0):
+        self._launch("neighbor_all_gather_v_group", "neighbor_all_gather_v", plan, 0, 0, stream, 0, flags)
+
+    def neighbor_all_gather_v_many(
+        self, sends, recvs, recvcounts, rdispls, agreed, sendcounts=None, stream=None, dtype=None
+    ):
+        """Transient variant of :meth:`prepare_neighbor_all_gather_v_group` +
+        :meth:`neighbor_all_gather_v_group`."""
+        what = "neighbor_all_gather_v_many"
+        args = self._neighbor_v_items(
+            what, "neighbor_all_gather_v", sends, recvs, sendcounts, None, recvcounts, rdispls, dtype
+        )
+        self._neighbor_v_many(what, args, agreed, stream)
+
+    def neighbor_all_to_all_v_streams(self, sends, recvs, sendcounts, sdispls, recvcounts, rdispls, dtype=None):
+        """As :meth:`neighbor_all_gather_v_streams`, for a neighbour
+        all-to-allv list."""
+        kind = "neighbor_all_to_all_v"
+        args = self._neighbor_v_items(
+            "neighbor_all_to_all_v_streams", kind, sends, recvs, sendcounts, sdispls, recvcounts, rdispls, dtype
+        )
+        return self._neighbor_v_streams("neighbor_all_to_all_v_streams", kind, args)
+
+    def prepare_neighbor_all_to_all_v_group(
+        self, sends, recvs, sendcounts, sdispls, recvcounts, rdispls, agreed, dtype=None
+    ) -> "GroupPlan":
+        """Plan MPI_Neighbor_alltoallv per item: send block k of ``sends[i]``
+        (``sendcounts[i][k]`` elements at ``sdispls[i][k]``) goes to out-edge
+        k, and recv block j gets the block of in-edge j = (source, idx), the
+        source's send block idx.  Otherwise as
+        :meth:`prepare_neighbor_all_gather_v_group`."""
+        what = "prepare_neighbor_all_to_all_v_group"
+        kind = "neighbor_all_to_all_v"
+        args = self._neighbor_v_items(what, kind, sends, recvs, sendcounts, sdispls, recvcounts, rdispls, dtype)
+        nbytes = sum(t.numel() * t.element_size() for t in recvs if t is not None)
+        return self._prepare_neighbor_v(what, kind, args, agreed, nbytes)
+
+    def neighbor_all_to_all_v_group(self, plan: "GroupPlan", stream=None, flags=0):
+        self._launch("neighbor_all_to_all_v_group", "neighbor_all_to_all_v", plan, 0, 0, stream, 0, flags)
+
+    def neighbor_all_to_all_v_many(
+        self, sends, recvs, sendcounts, sdispls, recvcounts, rdispls, agreed, stream=None, dtype=None
+    ):
+        """Transient variant of :meth:`prepare_neighbor_all_to_all_v_group` +
+        :meth:`neighbor_all_to_all_v_group`."""
+        what = "neighbor_all_to_all_v_many"
+        args = self._neighbor_v_items(
+            what, "neighbor_all_to_all_v", sends, recvs, sendcounts, sdispls, recvcounts, rdispls, dtype
+        )
+        self._neighbor_v_many(what, args, agreed, stream)
+
     def send_recv(self, send_buf, dst, recv_buf, src, stream=None):
         rc = self._lib.fb_sendrecv(
             self._h,
@@ -1219,7 +1391,7 @@ class Communicator:
 class GroupPlan:
     """Device-resident segment tables of a grouped all-reduce, reduce-scatter,
     all-gather, broadcast, all-to-all, gather, scatter, reduce, scan, exscan,
-    neighbourhood all-gather or neighbourhood all-to-all."""
+    or neighbourhood all-gather and all-to-all (equal blocks or v)."""
 
     def __init__(self, comm: Communicator, handle, n_tensors: int, nbytes: int):
         self._comm = comm
@@ -1318,6 +1490,17 @@ class LocalGroup:
         max_in = max(len(v) for v in edges)
         for r, c in enumerate(self.comms):
             c.set_neighbors(edges[r], len(destinations_per_rank[r]), max_out, max_in)
+
+    @staticmethod
+    def agree_neighbor_v(streams_per_rank):
+        """The agreement of a neighbour v list over the whole group: the
+        elementwise maximum of every rank's ``neighbor_*_v_streams``, which
+        every rank then passes as ``agreed``.  (An MPI program gets the same
+        from one host reduction over the members.)"""
+        lists = [[int(x) for x in v] for v in streams_per_rank]
+        if len({len(v) for v in lists}) > 1:
+            raise CommError(f"agree_neighbor_v: ranks have different window counts {[len(v) for v in lists]}")
+        return [max(col) for col in zip(*lists)] if lists else []
 
     def subset(self, members: Sequence[int]) -> "SubGroup":
         """The ranks ``members`` of this group as a group of their own (child
