@@ -596,18 +596,65 @@ inline std::vector<uint8_t> inputOf(const Case& c, int r, size_t n)
     return v;
 }
 
-// The fold of ranks [0, upto) in rank order
-inline std::vector<uint8_t> foldOf(const Case& c, int upto, size_t n)
+// The fold of the inputs of world ranks `ranks` (a communicator's members in
+// its order), in that order
+inline std::vector<uint8_t> foldOver(const Case& c, const std::vector<int>& ranks, size_t n)
 {
-    std::vector<uint8_t> acc = inputOf(c, 0, n);
+    std::vector<uint8_t> acc = inputOf(c, ranks[0], n);
     const size_t kb = kindSize(c.t->kind);
-    for (int r = 1; r < upto; r++) {
-        std::vector<uint8_t> in = inputOf(c, r, n);
+    for (size_t i = 1; i < ranks.size(); i++) {
+        std::vector<uint8_t> in = inputOf(c, ranks[i], n);
         for (size_t off = 0; off < acc.size(); off += kb) {
             combine(c.t->kind, c.opId(), acc.data() + off, in.data() + off);
         }
     }
     return acc;
+}
+
+// The fold of ranks [0, upto) in rank order
+inline std::vector<uint8_t> foldOf(const Case& c, int upto, size_t n)
+{
+    std::vector<int> ranks(std::max(upto, 1));
+    for (size_t r = 0; r < ranks.size(); r++) {
+        ranks[r] = (int)r;
+    }
+    return foldOver(c, ranks, n);
+}
+
+// A buffer image: each region's `want` at its offset (compared element by
+// element as `c`'s type), every other byte as in `before`
+struct Region
+{
+    size_t off;
+    std::vector<uint8_t> want;
+};
+
+inline void checkRegions(Ctx& x,
+                         const Case& c,
+                         const std::string& call,
+                         const std::vector<uint8_t>& got,
+                         const std::vector<uint8_t>& before,
+                         const std::vector<Region>& regions)
+{
+    std::vector<bool> result(got.size(), false);
+    for (const Region& r : regions) {
+        std::fill(result.begin() + (long)r.off, result.begin() + (long)(r.off + r.want.size()), true);
+    }
+    for (size_t i = 0; i < got.size(); i++) {
+        if (!result[i] && got[i] != before[i]) {
+            x.fail(c.name() + " " + call + ": byte " + std::to_string(i) + " outside the result changed");
+            return;
+        }
+    }
+    const size_t kb = kindSize(c.t->kind);
+    for (const Region& r : regions) {
+        for (size_t e = 0; e < r.want.size(); e += kb) {
+            if (!sameElem(c.t->kind, got.data() + r.off + e, r.want.data() + e)) {
+                x.fail(c.name() + " " + call + ": element " + std::to_string(e / kb) + " differs");
+                return;
+            }
+        }
+    }
 }
 
 // A buffer image: `want` at each of `offs`, every other byte as in `before`
@@ -619,26 +666,11 @@ inline void checkImage(Ctx& x,
                        const std::vector<size_t>& offs,
                        const std::vector<uint8_t>* want)
 {
-    const size_t n = want != nullptr ? want->size() : 0;
-    std::vector<bool> result(got.size(), false);
+    std::vector<Region> regions;
     for (size_t off : offs) {
-        std::fill(result.begin() + (long)off, result.begin() + (long)(off + n), true);
+        regions.push_back({ off, want != nullptr ? *want : std::vector<uint8_t>() });
     }
-    for (size_t i = 0; i < got.size(); i++) {
-        if (!result[i] && got[i] != before[i]) {
-            x.fail(c.name() + " " + call + ": byte " + std::to_string(i) + " outside the result changed");
-            return;
-        }
-    }
-    const size_t kb = kindSize(c.t->kind);
-    for (size_t off : offs) {
-        for (size_t e = 0; e < n; e += kb) {
-            if (!sameElem(c.t->kind, got.data() + off + e, want->data() + e)) {
-                x.fail(c.name() + " " + call + ": element " + std::to_string(e / kb) + " differs");
-                return;
-            }
-        }
-    }
+    checkRegions(x, c, call, got, before, regions);
 }
 
 // The world's count of device collectives, once every rank has reached this
