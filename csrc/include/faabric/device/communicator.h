@@ -17,6 +17,7 @@
 #include <cstdint>
 #include <cstddef>
 #include <deque>
+#include <initializer_list>
 #include <map>
 #include <memory>
 #include <mutex>
@@ -750,24 +751,39 @@ class Communicator : public std::enable_shared_from_this<Communicator>
                 std::shared_ptr<Backing> backing,
                 const std::string& kind);
     void finishSetup();
+    template<typename Run>
+    int runPhases(const GroupLaunch& l,
+                  std::initializer_list<int> steps,
+                  bool ss,
+                  int flags,
+                  cudaStream_t s,
+                  Run&& run);
     int launchGroup(const GroupLaunch& l, GroupKind kind, int dtype, int op, int root, int flags, cudaStream_t s);
-    int launchRooted(const GroupLaunch& l,
-                     GroupKind kind,
-                     int dtype,
-                     int op,
-                     fb::GroupArgs& a,
-                     bool ss,
-                     int flags,
-                     cudaStream_t s);
+    bool groupMissing(GroupKind kind, int root, uint32_t missing) const;
     int groupCheck(GroupKind kind, int dtype, int op, int root, int flags, bool& grouped) const;
-    int launchNeighbor(const GroupLaunch& l, GroupKind kind, fb::GroupArgs& a, bool ss, int flags, cudaStream_t s);
-    int launchNeighborV(const GroupLaunch& l, GroupKind kind, fb::GroupArgs& a, bool ss, int flags, cudaStream_t s);
-    int neighborVCheck(GroupKind kind, const NeighborVItem* items, size_t nItems, int dtype, size_t& window) const;
+    template<typename Next>
+    int groupWalk(GroupPlan* plan,
+                  GroupKind kind,
+                  int dtype,
+                  int op,
+                  int root,
+                  int flags,
+                  cudaStream_t s,
+                  Next&& next);
+    int neighborVCheck(GroupKind kind,
+                       const NeighborVItem* items,
+                       size_t nItems,
+                       int dtype,
+                       int flags,
+                       size_t& window,
+                       std::vector<uint64_t>& streams) const;
     int neighborVBatch(GroupKind kind,
                        const NeighborVItem* items,
                        size_t nItems,
                        size_t esize,
-                       uint64_t agreed,
+                       size_t window,
+                       const std::vector<uint64_t>& agreed,
+                       size_t& w,
                        std::vector<fb::GroupSeg>& segs,
                        GroupLaunch& l) const;
     int addPlanLaunch(GroupPlan& plan, const std::vector<fb::GroupSeg>& segs, GroupLaunch& l);

@@ -2107,6 +2107,12 @@ static bool neighborVKind(Communicator::GroupKind kind)
     return kind == Communicator::GROUP_NEIGHBOR_ALLGATHERV || kind == Communicator::GROUP_NEIGHBOR_ALLTOALLV;
 }
 
+// Send streams of a neighbour v rank with `outDeg` out-edges
+static uint32_t neighborVSends(Communicator::GroupKind kind, uint32_t outDeg)
+{
+    return kind == Communicator::GROUP_NEIGHBOR_ALLTOALLV ? outDeg : std::min(outDeg, 1u);
+}
+
 std::pair<int, int> Communicator::neighborDegrees() const
 {
     return topo_ != nullptr ? std::pair<int, int>{ (int)topo_->in.size(), (int)topo_->outDeg } : std::pair<int, int>{ 0, 0 };
@@ -2245,42 +2251,6 @@ int Communicator::groupBatch(GroupKind kind,
     return FB_OK;
 }
 
-std::shared_ptr<Communicator::GroupPlan> Communicator::prepareGroup(
-  const GroupItem* items,
-  size_t nItems,
-  int dtype,
-  int* rcOut,
-  GroupKind kind)
-{
-    int rcLocal = FB_OK;
-    int& rc = rcOut ? *rcOut : rcLocal;
-    rc = FB_OK;
-    const size_t esize = fbDtypeSize(dtype);
-    if (esize == 0 || kind < GROUP_ALLREDUCE || kind > GROUP_NEIGHBOR_ALLTOALL) {
-        rc = FB_E_INVALID;
-        return nullptr;
-    }
-    bindDevice();
-    auto plan = std::make_shared<GroupPlan>();
-    plan->kind = kind;
-    plan->dtype = dtype;
-    plan->device = device_;
-    plan->items = nItems;
-    for (GroupCursor at; at.item < nItems;) {
-        std::vector<fb::GroupSeg> segs;
-        GroupLaunch l;
-        rc = groupBatch(kind, items, nItems, esize, at, segs, l);
-        if (rc != FB_OK) {
-            return nullptr;
-        }
-        rc = addPlanLaunch(*plan, segs, l);
-        if (rc != FB_OK) {
-            return nullptr;
-        }
-    }
-    return plan;
-}
-
 // Uploads one launch's table into a plan, which owns it from then on
 int Communicator::addPlanLaunch(GroupPlan& plan, const std::vector<fb::GroupSeg>& segs, GroupLaunch& l)
 {
@@ -2324,6 +2294,59 @@ static int groupGrid(const CommConfig& cfg, int nranks, uint64_t vecsPerRank)
     return (int)std::clamp<uint64_t>(want, 1, (uint64_t)cap);
 }
 
+// No warp without a unit of work: `units` (the launch's chunks, times the
+// largest degree for the neighbour kinds) is the same on every rank
+static int chunkGrid(const CommConfig& cfg, int nranks, uint64_t units, uint64_t vecsPerRank)
+{
+    const uint64_t warps = (uint64_t)cfg.threads / 32;
+    return (int)std::clamp<uint64_t>((units + warps - 1) / warps, 1, (uint64_t)groupGrid(cfg, nranks, vecsPerRank));
+}
+
+// A stream-ordered barrier in a step list of runPhases
+static const int GROUP_BARRIER = -1;
+
+// One launch of a grouped kind.  With stream-ordered barriers (`ss`) it runs
+// `steps` in order: a kernel run of the phases a step names, or a
+// streamBarrier for GROUP_BARRIER; without them one kernel run does every
+// phase.  A neighbour v window does this once per round.  run(phases, round)
+// makes one kernel run and returns whether it was launched.  Counts a launch
+// per round, the kernel runs of a round beyond its first as staging copies,
+// and the launch's bytes once.
+template<typename Run>
+int Communicator::runPhases(const GroupLaunch& l,
+                            std::initializer_list<int> steps,
+                            bool ss,
+                            int flags,
+                            cudaStream_t s,
+                            Run&& run)
+{
+    int phases = 0;
+    int runs = 0;
+    for (const int step : steps) {
+        if (step != GROUP_BARRIER) {
+            phases |= step;
+            runs++;
+        }
+    }
+    for (uint32_t r = 0; r < l.rounds; r++) {
+        if (!ss) {
+            if (!run(phases, r)) {
+                return FB_E_CUDA;
+            }
+        } else {
+            for (const int step : steps) {
+                if (step == GROUP_BARRIER ? streamBarrier(flags, s) != FB_OK : !run(step, r)) {
+                    return FB_E_CUDA;
+                }
+            }
+            stats_.stagedCopies += runs - 1;
+        }
+        stats_.launches++;
+    }
+    stats_.bytes += l.bytes;
+    return FB_OK;
+}
+
 int Communicator::launchGroup(const GroupLaunch& l,
                               GroupKind kind,
                               int dtype,
@@ -2333,7 +2356,12 @@ int Communicator::launchGroup(const GroupLaunch& l,
                               cudaStream_t s)
 {
     const int n = dev_.nranks;
+    if (kind == GROUP_EXSCAN && n == 1) {
+        return FB_OK; // a one-member exscan writes nothing
+    }
     const bool ss = streamSync_ && !(flags & FB_FLAG_NOSYNC) && n > 1;
+    const bool rooted = rootedKind(kind);
+    const bool neighbor = neighborKind(kind) || neighborVKind(kind);
     fb::GroupArgs a;
     memset(&a, 0, sizeof(a));
     a.comm = devFor(flags);
@@ -2341,163 +2369,81 @@ int Communicator::launchGroup(const GroupLaunch& l,
     a.nSegs = l.nSegs;
     a.totalChunks = l.totalChunks;
     a.noSync = ((flags & FB_FLAG_NOSYNC) || ss || n == 1) ? 1 : 0;
-    a.root = (kind == GROUP_BROADCAST || (rootedKind(kind) && !scanKind(kind))) ? root : 0;
+    a.root = (kind == GROUP_BROADCAST || (rooted && !scanKind(kind))) ? root : 0;
     a.exclusive = kind == GROUP_EXSCAN ? 1 : 0;
-    if (rootedKind(kind)) {
-        return launchRooted(l, kind, dtype, op, a, ss, flags, s);
-    }
-    if (neighborKind(kind)) {
-        return launchNeighbor(l, kind, a, ss, flags, s);
-    }
-    if (neighborVKind(kind)) {
-        return launchNeighborV(l, kind, a, ss, flags, s);
-    }
-    if (ss && streamBarrier(flags, s) != FB_OK) {
-        return FB_E_CUDA;
-    }
-    int blocks = groupGrid(cfg_, n, l.vecsPerRank);
-    if (kind == GROUP_ALLTOALL) {
-        // no warp without a chunk (totalChunks is the same on every rank: one
-        // whole block per item)
-        const uint64_t warps = (uint64_t)cfg_.threads / 32;
-        blocks = (int)std::clamp<uint64_t>((l.totalChunks + warps - 1) / warps, 1, (uint64_t)blocks);
-    }
-    cudaError_t e;
-    if (kind == GROUP_REDUCE_SCATTER) {
-        e = k_->groupReduceScatter(a, dtype, op, blocks, cfg_.threads, s);
-    } else if (kind == GROUP_ALLGATHER) {
-        e = k_->groupAllGather(a, blocks, cfg_.threads, s);
-    } else if (kind == GROUP_BROADCAST) {
-        e = k_->groupBroadcast(a, blocks, cfg_.threads, s);
-    } else if (kind == GROUP_ALLTOALL) {
-        e = k_->groupAllToAll(a, blocks, cfg_.threads, s);
+    int blocks;
+    if (neighbor) {
+        const NeighborTopo& t = *topo_;
+        a.stageOff = stageSendOff_;
+        a.nEdges = (uint32_t)t.in.size();
+        a.outDeg = t.outDeg;
+        a.vWidth = l.width;
+        const uint32_t sends = neighborVKind(kind) ? neighborVSends(kind, t.maxOutDeg) : t.maxOutDeg;
+        const uint64_t units = (uint64_t)l.totalChunks * std::max(sends, t.maxInDeg);
+        blocks = chunkGrid(cfg_, n, units, units * (FB_NEIGHBOR_CHUNK / 16));
+    } else if (rooted || kind == GROUP_ALLTOALL) {
+        // (an all-to-all has one whole block per item on every rank)
+        a.stageOff = rooted ? stageSendOff_ : 0;
+        a.stageRecvOff = rooted ? stageRecvOff_ : 0;
+        blocks = chunkGrid(cfg_, n, l.totalChunks, l.vecsPerRank);
     } else {
-        e = k_->group(a, dtype, op, blocks, cfg_.threads, s);
+        blocks = groupGrid(cfg_, n, l.vecsPerRank);
     }
-    if (e != cudaSuccess) {
-        return FB_E_CUDA;
+    const int th = cfg_.threads;
+    const bool a2a = kind == GROUP_NEIGHBOR_ALLTOALL || kind == GROUP_NEIGHBOR_ALLTOALLV;
+    auto run = [&](int phases, uint32_t round) {
+        a.phase = phases;
+        a.vBase = (uint64_t)round * l.width;
+        const cudaError_t e = kind == GROUP_ALLREDUCE        ? k_->group(a, dtype, op, blocks, th, s)
+                              : kind == GROUP_REDUCE_SCATTER ? k_->groupReduceScatter(a, dtype, op, blocks, th, s)
+                              : kind == GROUP_ALLGATHER      ? k_->groupAllGather(a, blocks, th, s)
+                              : kind == GROUP_BROADCAST      ? k_->groupBroadcast(a, blocks, th, s)
+                              : kind == GROUP_ALLTOALL       ? k_->groupAllToAll(a, blocks, th, s)
+                              : kind == GROUP_GATHER         ? k_->groupGather(a, blocks, th, s)
+                              : kind == GROUP_SCATTER        ? k_->groupScatter(a, blocks, th, s)
+                              : kind == GROUP_REDUCE         ? k_->groupReduce(a, dtype, op, blocks, th, s)
+                              : scanKind(kind)               ? k_->groupScan(a, dtype, op, blocks, th, s)
+                              : neighborKind(kind)           ? k_->groupNeighbor(a, a2a, blocks, th, s)
+                                                             : k_->groupNeighborV(a, a2a, blocks, th, s);
+        return e == cudaSuccess;
+    };
+    const int L = GROUP_PHASE_LOCAL;
+    const int M = GROUP_PHASE_MOVE;
+    const int B = GROUP_BARRIER;
+    int rc;
+    if (kind == GROUP_SCATTER) {
+        rc = runPhases(l, { B, M, B, L }, ss, flags, s, run);
+    } else if (kind == GROUP_REDUCE || scanKind(kind)) {
+        rc = runPhases(l, { L, B, M, B, GROUP_PHASE_UNSTAGE }, ss, flags, s, run);
+    } else if (rooted || neighbor) {
+        // gather, and the neighbour kinds (each round of a v window)
+        rc = runPhases(l, { L, B, M, B }, ss, flags, s, run);
+    } else {
+        // the two-shot kinds: one kernel between the entry and exit barriers
+        rc = runPhases(l, { B, 0, B }, ss, flags, s, run);
     }
-    if (ss && streamBarrier(flags, s) != FB_OK) {
-        return FB_E_CUDA;
-    }
-    stats_.launches++;
-    stats_.bytes += l.bytes;
-    if (kind == GROUP_ALLREDUCE) {
+    if (rc == FB_OK && kind == GROUP_ALLREDUCE) {
         stats_.algoCount[FB_ALGO_TWOSHOT]++;
     }
-    return FB_OK;
+    return rc;
 }
 
-// Whether this rank lacks a buffer of a rooted list (`missing`:
-// GroupLaunch::missing over the list): every rank needs its own side (the
-// send of a gather or reduce), the root both, and every rank of a scan or
-// exscan both.  Checked before the list's first launch.
-static bool rootedMissing(Communicator::GroupKind kind, bool isRoot, uint32_t missing)
+// Whether this rank lacks a buffer of a list that it needs (`missing`:
+// GroupLaunch::missing over the list's launches, or the same over its
+// items), checked before the list's first launch.  Rooted kinds: every rank
+// needs its own side (the send of a gather or reduce), the root both, and
+// every rank of a scan or exscan both.  Neighbour kinds: the send with an
+// out-edge, the recv with an in-edge.  The v kinds check theirs, with their
+// counts, in neighborVCheck.
+bool Communicator::groupMissing(GroupKind kind, int root, uint32_t missing) const
 {
-    const uint32_t needed = isRoot || scanKind(kind) ? 3u : (kind == Communicator::GROUP_SCATTER ? 2u : 1u);
+    uint32_t needed = 0;
+    if (rootedKind(kind)) {
+        needed = dev_.rank == root || scanKind(kind) ? 3u : (kind == GROUP_SCATTER ? 2u : 1u);
+    } else if (neighborKind(kind)) {
+        needed = (topo_->outDeg > 0 ? 1u : 0u) | (topo_->in.empty() ? 0u : 2u);
+    }
     return (missing & needed) != 0;
-}
-
-// A rooted launch.  With stream-ordered barriers the kernel runs as one
-// launch per step: gather LOCAL, barrier, MOVE, barrier; scatter barrier,
-// MOVE, barrier, LOCAL; reduce, scan and exscan LOCAL, barrier, MOVE,
-// barrier, UNSTAGE.  A one-member exscan writes nothing: no launch.
-int Communicator::launchRooted(const GroupLaunch& l, GroupKind kind, int dtype, int op, fb::GroupArgs& a, bool ss,
-                               int flags, cudaStream_t s)
-{
-    const bool gather = kind == GROUP_GATHER;
-    const bool folds = kind == GROUP_REDUCE || scanKind(kind);
-    if (kind == GROUP_EXSCAN && dev_.nranks == 1) {
-        return FB_OK;
-    }
-    a.stageOff = stageSendOff_;
-    a.stageRecvOff = stageRecvOff_;
-    // no warp without a chunk (as the all-to-all)
-    const uint64_t warps = (uint64_t)cfg_.threads / 32;
-    const int blocks = (int)std::clamp<uint64_t>(
-      (l.totalChunks + warps - 1) / warps, 1, (uint64_t)groupGrid(cfg_, dev_.nranks, l.vecsPerRank));
-    auto run = [&](int phase) {
-        a.phase = phase;
-        const cudaError_t e = kind == GROUP_REDUCE ? k_->groupReduce(a, dtype, op, blocks, cfg_.threads, s)
-                              : scanKind(kind)     ? k_->groupScan(a, dtype, op, blocks, cfg_.threads, s)
-                              : gather             ? k_->groupGather(a, blocks, cfg_.threads, s)
-                                                   : k_->groupScatter(a, blocks, cfg_.threads, s);
-        return e == cudaSuccess ? FB_OK : FB_E_CUDA;
-    };
-    int rc;
-    int staged = 1; // launches beyond the first: staging copies
-    if (!ss) {
-        rc = run(GROUP_PHASE_LOCAL | GROUP_PHASE_MOVE | GROUP_PHASE_UNSTAGE);
-        staged = 0;
-    } else if (folds) {
-        rc = run(GROUP_PHASE_LOCAL);
-        rc = rc == FB_OK ? streamBarrier(flags, s) : rc;
-        rc = rc == FB_OK ? run(GROUP_PHASE_MOVE) : rc;
-        rc = rc == FB_OK ? streamBarrier(flags, s) : rc;
-        rc = rc == FB_OK ? run(GROUP_PHASE_UNSTAGE) : rc;
-        staged = 2;
-    } else if (gather) {
-        rc = run(GROUP_PHASE_LOCAL);
-        rc = rc == FB_OK ? streamBarrier(flags, s) : rc;
-        rc = rc == FB_OK ? run(GROUP_PHASE_MOVE) : rc;
-        rc = rc == FB_OK ? streamBarrier(flags, s) : rc;
-    } else {
-        rc = streamBarrier(flags, s);
-        rc = rc == FB_OK ? run(GROUP_PHASE_MOVE) : rc;
-        rc = rc == FB_OK ? streamBarrier(flags, s) : rc;
-        rc = rc == FB_OK ? run(GROUP_PHASE_LOCAL) : rc;
-    }
-    if (rc != FB_OK) {
-        return FB_E_CUDA;
-    }
-    stats_.launches++;
-    stats_.stagedCopies += staged;
-    stats_.bytes += l.bytes;
-    return FB_OK;
-}
-
-// A neighbour launch.  With stream-ordered barriers the kernel runs as two
-// launches: LOCAL, barrier, MOVE, barrier.  The grid follows from the launch's
-// chunks and the largest degrees, the same on every rank.
-int Communicator::launchNeighbor(const GroupLaunch& l, GroupKind kind, fb::GroupArgs& a, bool ss, int flags,
-                                 cudaStream_t s)
-{
-    const NeighborTopo& t = *topo_;
-    a.stageOff = stageSendOff_;
-    a.nEdges = (uint32_t)t.in.size();
-    a.outDeg = t.outDeg;
-    const uint64_t warps = (uint64_t)cfg_.threads / 32;
-    const uint64_t units = (uint64_t)l.totalChunks * std::max(t.maxOutDeg, t.maxInDeg);
-    const int blocks = (int)std::clamp<uint64_t>(
-      (units + warps - 1) / warps, 1, (uint64_t)groupGrid(cfg_, dev_.nranks, units * (FB_NEIGHBOR_CHUNK / 16)));
-    const bool a2a = kind == GROUP_NEIGHBOR_ALLTOALL;
-    auto run = [&](int phase) {
-        a.phase = phase;
-        return k_->groupNeighbor(a, a2a, blocks, cfg_.threads, s) == cudaSuccess ? FB_OK : FB_E_CUDA;
-    };
-    int rc;
-    if (!ss) {
-        rc = run(GROUP_PHASE_LOCAL | GROUP_PHASE_MOVE);
-    } else {
-        rc = run(GROUP_PHASE_LOCAL);
-        rc = rc == FB_OK ? streamBarrier(flags, s) : rc;
-        rc = rc == FB_OK ? run(GROUP_PHASE_MOVE) : rc;
-        rc = rc == FB_OK ? streamBarrier(flags, s) : rc;
-        stats_.stagedCopies++;
-    }
-    if (rc != FB_OK) {
-        return FB_E_CUDA;
-    }
-    stats_.launches++;
-    stats_.bytes += l.bytes;
-    return FB_OK;
-}
-
-// Whether this rank lacks a buffer of a neighbour list (`missing` as for the
-// rooted kinds): the send with an out-edge, the recv with an in-edge
-static bool neighborMissing(uint32_t outDeg, size_t inDeg, uint32_t missing)
-{
-    return (missing & ((outDeg > 0 ? 1u : 0u) | (inDeg > 0 ? 2u : 0u))) != 0;
 }
 
 namespace {
@@ -2523,7 +2469,8 @@ const GroupKindNames kGroupNames[] = {
 };
 #undef FB_GROUP_NAMES
 
-// groupCheck: a valid call with nothing to launch
+// groupCheck: a valid call with nothing to launch; groupWalk's producers: no
+// launch left
 const int GROUP_NOTHING = 1;
 }
 
@@ -2586,6 +2533,75 @@ int Communicator::groupCheck(GroupKind kind, int dtype, int op, int root, int fl
     return FB_OK;
 }
 
+// Walks the launches of a list: next(segs, l) makes the next launch's table
+// and sizes and returns FB_OK, or returns GROUP_NOTHING after the last launch,
+// or an error.  Each launch is uploaded into `plan`, or without a plan staged
+// in the table ring and launched.
+template<typename Next>
+int Communicator::groupWalk(GroupPlan* plan,
+                            GroupKind kind,
+                            int dtype,
+                            int op,
+                            int root,
+                            int flags,
+                            cudaStream_t s,
+                            Next&& next)
+{
+    std::vector<fb::GroupSeg> segs;
+    for (;;) {
+        GroupLaunch l;
+        int rc = next(segs, l);
+        if (rc != FB_OK) {
+            return rc == GROUP_NOTHING ? FB_OK : rc;
+        }
+        if (plan != nullptr) {
+            rc = addPlanLaunch(*plan, segs, l);
+        } else {
+            stats_.segTables++;
+            ManySlot* slot = nullptr;
+            l.dSegs = (fb::GroupSeg*)stageManyTable(segs.data(), segs.size() * sizeof(fb::GroupSeg), s, &slot);
+            // (on loopback an empty table is a null pointer the kernel never reads)
+            if (l.dSegs == nullptr && !loop_) {
+                return FB_E_CUDA;
+            }
+            rc = launchGroup(l, kind, dtype, op, root, flags, s);
+            if (rc == FB_OK) {
+                releaseManySlot(slot, s);
+            }
+        }
+        if (rc != FB_OK) {
+            return rc;
+        }
+    }
+}
+
+std::shared_ptr<Communicator::GroupPlan> Communicator::prepareGroup(
+  const GroupItem* items,
+  size_t nItems,
+  int dtype,
+  int* rcOut,
+  GroupKind kind)
+{
+    int rcLocal = FB_OK;
+    int& rc = rcOut ? *rcOut : rcLocal;
+    const size_t esize = fbDtypeSize(dtype);
+    if (esize == 0 || kind < GROUP_ALLREDUCE || kind > GROUP_NEIGHBOR_ALLTOALL) {
+        rc = FB_E_INVALID;
+        return nullptr;
+    }
+    bindDevice();
+    auto plan = std::make_shared<GroupPlan>();
+    plan->kind = kind;
+    plan->dtype = dtype;
+    plan->device = device_;
+    plan->items = nItems;
+    GroupCursor at;
+    rc = groupWalk(plan.get(), kind, dtype, 0, 0, 0, nullptr, [&](std::vector<fb::GroupSeg>& segs, GroupLaunch& l) {
+        return at.item < nItems ? groupBatch(kind, items, nItems, esize, at, segs, l) : GROUP_NOTHING;
+    });
+    return rc == FB_OK ? plan : nullptr;
+}
+
 int Communicator::runGroup(GroupKind kind, const GroupPlan& plan, int op, int root, int flags, cudaStream_t s)
 {
     if (plan.kind != kind) {
@@ -2600,23 +2616,12 @@ int Communicator::runGroup(GroupKind kind, const GroupPlan& plan, int op, int ro
     if (!grouped) {
         return FB_E_UNSUPPORTED;
     }
-    if (rootedKind(kind)) {
-        uint32_t missing = 0;
-        for (const auto& l : plan.launches) {
-            missing |= l.missing;
-        }
-        if (rootedMissing(kind, dev_.rank == root, missing)) {
-            return FB_E_INVALID;
-        }
+    uint32_t missing = 0;
+    for (const auto& l : plan.launches) {
+        missing |= l.missing;
     }
-    if (neighborKind(kind)) {
-        uint32_t missing = 0;
-        for (const auto& l : plan.launches) {
-            missing |= l.missing;
-        }
-        if (neighborMissing(topo_->outDeg, topo_->in.size(), missing)) {
-            return FB_E_INVALID;
-        }
+    if (groupMissing(kind, root, missing)) {
+        return FB_E_INVALID;
     }
     bindDevice();
     for (const auto& l : plan.launches) {
@@ -2649,50 +2654,40 @@ int Communicator::groupMany(GroupKind kind,
     if (rc != FB_OK) {
         return rc == GROUP_NOTHING ? FB_OK : rc;
     }
-    const size_t esize = fbDtypeSize(dtype);
-    if (rootedKind(kind) || neighborKind(kind)) {
-        uint32_t missing = 0;
-        for (size_t i = 0; i < nItems; i++) {
-            if (items[i].count != 0) {
-                missing |= (items[i].send == nullptr ? 1u : 0u) | (items[i].recv == nullptr ? 2u : 0u);
-            }
-        }
-        if (rootedKind(kind) ? rootedMissing(kind, dev_.rank == root, missing)
-                             : neighborMissing(topo_->outDeg, topo_->in.size(), missing)) {
-            return FB_E_INVALID;
+    uint32_t missing = 0;
+    for (size_t i = 0; i < nItems; i++) {
+        if (items[i].count != 0) {
+            missing |= (items[i].send == nullptr ? 1u : 0u) | (items[i].recv == nullptr ? 2u : 0u);
         }
     }
+    if (groupMissing(kind, root, missing)) {
+        return FB_E_INVALID;
+    }
     bindDevice();
+    const size_t esize = fbDtypeSize(dtype);
     // try the grouped path batch by batch; anything not symmetric / aligned
     // goes through the per-tensor calls (the choice depends only on arguments
     // that are symmetric across ranks)
-    for (GroupCursor at; at.item < nItems;) {
-        const size_t begin = at.item;
-        std::vector<fb::GroupSeg> segs;
-        GroupLaunch l;
-        rc = grouped ? groupBatch(kind, items, nItems, esize, at, segs, l) : FB_E_UNSUPPORTED;
-        if (rc != FB_OK) {
+    GroupCursor at;
+    rc = groupWalk(nullptr, kind, dtype, op, root, flags, s, [&](std::vector<fb::GroupSeg>& segs, GroupLaunch& l) {
+        while (at.item < nItems) {
+            const size_t begin = at.item;
+            int brc = grouped ? groupBatch(kind, items, nItems, esize, at, segs, l) : FB_E_UNSUPPORTED;
+            if (brc == FB_OK) {
+                return FB_OK;
+            }
             // (only the kinds that group a window of whole items fail here)
             const size_t cnt = std::min(GROUP_ITEMS_PER_LAUNCH, nItems - begin);
             at = GroupCursor{ begin + cnt, 0 };
-            rc = groupPerItem(kind, items + begin, cnt, dtype, op, root, flags, s);
-            if (rc != FB_OK) {
-                return rc;
+            brc = groupPerItem(kind, items + begin, cnt, dtype, op, root, flags, s);
+            if (brc != FB_OK) {
+                return brc;
             }
-            continue;
         }
-        stats_.segTables++;
-        ManySlot* slot = nullptr;
-        l.dSegs = (fb::GroupSeg*)stageManyTable(segs.data(), segs.size() * sizeof(fb::GroupSeg), s, &slot);
-        // (on loopback an empty table is a null pointer the kernel never reads)
-        if (l.dSegs == nullptr && !loop_) {
-            return FB_E_CUDA;
-        }
-        rc = launchGroup(l, kind, dtype, op, root, flags, s);
-        if (rc != FB_OK) {
-            return rc;
-        }
-        releaseManySlot(slot, s);
+        return GROUP_NOTHING;
+    });
+    if (rc != FB_OK) {
+        return rc;
     }
     if (kind == GROUP_ALLREDUCE) {
         lastAlgo_ = FB_ALGO_TWOSHOT;
@@ -2757,12 +2752,6 @@ int Communicator::groupPerItem(GroupKind kind,
 // ---------------------------------------------------------------------------
 // Grouped neighbourhood v-collectives
 // ---------------------------------------------------------------------------
-// Send streams of a rank with `outDeg` out-edges
-static uint32_t neighborVSends(Communicator::GroupKind kind, uint32_t outDeg)
-{
-    return kind == Communicator::GROUP_NEIGHBOR_ALLTOALLV ? outDeg : std::min(outDeg, 1u);
-}
-
 // This rank's streams over items[0..n): the table entries (send streams, then
 // recv streams, n + 1 entries each, NeighborVSeg in launch_api.h) into `out`
 // when given, and the length of the longest stream
@@ -2803,18 +2792,25 @@ static uint64_t neighborVEntries(bool allToAll,
 }
 
 // The refusals of a v list that do not depend on the agreement (see the
-// header), and its items per launch window: the streams of the largest
-// degrees, n + 1 entries each, and the largest in-degree's edges fill at most
-// FB_GROUP_MAX_SEGS slots, so every member cuts alike.  window 0: no member has
-// an edge.
-int Communicator::neighborVCheck(GroupKind kind, const NeighborVItem* items, size_t nItems, int dtype, size_t& window)
-  const
+// header; `flags` as for groupCheck), its items per launch window, and this
+// rank's longest stream of every window in `streams`.  The streams of the
+// largest degrees, n + 1 entries each, and the largest in-degree's edges fill
+// at most FB_GROUP_MAX_SEGS slots, so every member cuts alike.
+// GROUP_NOTHING, with no window: no member has an edge.
+int Communicator::neighborVCheck(GroupKind kind,
+                                 const NeighborVItem* items,
+                                 size_t nItems,
+                                 int dtype,
+                                 int flags,
+                                 size_t& window,
+                                 std::vector<uint64_t>& streams) const
 {
     window = 0;
+    streams.clear();
     bool grouped = false;
-    const int rc = neighborVKind(kind) ? groupCheck(kind, dtype, 0, 0, 0, grouped) : FB_E_INVALID;
+    const int rc = neighborVKind(kind) ? groupCheck(kind, dtype, 0, 0, flags, grouped) : FB_E_INVALID;
     if (rc != FB_OK) {
-        return rc == GROUP_NOTHING ? FB_OK : rc;
+        return rc;
     }
     const NeighborTopo& t = *topo_;
     const uint32_t sends = neighborVSends(kind, t.outDeg);
@@ -2836,12 +2832,16 @@ int Communicator::neighborVCheck(GroupKind kind, const NeighborVItem* items, siz
             }
         }
     }
-    const uint64_t streams = neighborVSends(kind, t.maxOutDeg) + t.maxInDeg;
+    const uint64_t streamsMax = neighborVSends(kind, t.maxOutDeg) + t.maxInDeg;
     const uint64_t entries =
       ((uint64_t)FB_GROUP_MAX_SEGS * sizeof(fb::GroupSeg) - (uint64_t)t.maxInDeg * sizeof(fb::NeighborEdge)) /
       sizeof(fb::NeighborVSeg);
     // (FB_NEIGHBOR_V_MAX_DEGREE leaves room for several items)
-    window = std::min<size_t>(entries / streams - 1, GROUP_ITEMS_PER_LAUNCH);
+    window = std::min<size_t>(entries / streamsMax - 1, GROUP_ITEMS_PER_LAUNCH);
+    for (size_t b = 0; b < nItems; b += window) {
+        const size_t n = std::min(window, nItems - b);
+        streams.push_back(neighborVEntries(a2a, sends, t.in.size(), items + b, n, fbDtypeSize(dtype), nullptr));
+    }
     return FB_OK;
 }
 
@@ -2851,43 +2851,46 @@ int Communicator::neighborVStreams(GroupKind kind,
                                    int dtype,
                                    std::vector<uint64_t>& out) const
 {
-    out.clear();
     size_t window = 0;
-    const int rc = neighborVCheck(kind, items, nItems, dtype, window);
-    if (rc != FB_OK || window == 0) {
-        return rc;
-    }
-    const uint32_t sends = neighborVSends(kind, topo_->outDeg);
-    for (size_t b = 0; b < nItems; b += window) {
-        out.push_back(neighborVEntries(kind == GROUP_NEIGHBOR_ALLTOALLV, sends, topo_->in.size(), items + b,
-                                       std::min(window, nItems - b), fbDtypeSize(dtype), nullptr));
-    }
-    return FB_OK;
+    const int rc = neighborVCheck(kind, items, nItems, dtype, 0, window, out);
+    return rc == GROUP_NOTHING ? FB_OK : rc;
 }
 
-// One launch window, items[0..n): this rank's table in `segs` and the
-// window's rounds in `l`.  `agreed` (> 0) is the window's longest stream over
-// every member.
+// The next launch window of a v list with a non-zero agreement, from window
+// `w` on, which it advances: this rank's table in `segs` and the window's
+// rounds in `l`; GROUP_NOTHING after the last.  agreed[w] is window w's
+// longest stream over every member, `window` the items per window.
 int Communicator::neighborVBatch(GroupKind kind,
                                  const NeighborVItem* items,
-                                 size_t n,
+                                 size_t nItems,
                                  size_t esize,
-                                 uint64_t agreed,
+                                 size_t window,
+                                 const std::vector<uint64_t>& agreed,
+                                 size_t& w,
                                  std::vector<fb::GroupSeg>& segs,
                                  GroupLaunch& l) const
 {
+    while (w < agreed.size() && agreed[w] == 0) {
+        w++;
+    }
+    if (w == agreed.size()) {
+        return GROUP_NOTHING;
+    }
+    const uint64_t longest = agreed[w];
+    const size_t b = w++ * window;
+    const size_t n = std::min(window, nItems - b);
     const NeighborTopo& t = *topo_;
     const bool a2a = kind == GROUP_NEIGHBOR_ALLTOALLV;
     const uint32_t sends = neighborVSends(kind, t.outDeg);
     std::vector<fb::NeighborVSeg> entries;
-    neighborVEntries(a2a, sends, t.in.size(), items, n, esize, &entries);
+    neighborVEntries(a2a, sends, t.in.size(), items + b, n, esize, &entries);
     // A slot's room in whole chunks (the all-to-all shares the staging buffer
     // among the largest out-degree's slots), at most the agreed stream
     const uint64_t cb = FB_NEIGHBOR_CHUNK;
     const uint64_t slots = a2a ? std::max<uint32_t>(t.maxOutDeg, 1) : 1;
     const uint64_t room = std::min<uint64_t>(cfg_.stageBytes, (uint64_t)1 << 31) / cb / slots * cb;
-    l.width = std::min(room, (agreed + cb - 1) / cb * cb);
-    l.rounds = (uint32_t)((agreed + l.width - 1) / l.width);
+    l.width = std::min(room, (longest + cb - 1) / cb * cb);
+    l.rounds = (uint32_t)((longest + l.width - 1) / l.width);
     l.totalChunks = (uint32_t)(l.width / cb);
     l.nSegs = (uint32_t)n;
     l.bytes = 0;
@@ -2925,8 +2928,10 @@ std::shared_ptr<Communicator::GroupPlan> Communicator::prepareGroup(const Neighb
 {
     int rcLocal = FB_OK;
     int& rc = rcOut ? *rcOut : rcLocal;
+    size_t window = 0;
     std::vector<uint64_t> mine;
-    rc = neighborVStreams(kind, items, nItems, dtype, mine);
+    rc = neighborVCheck(kind, items, nItems, dtype, 0, window, mine);
+    rc = rc == GROUP_NOTHING ? FB_OK : rc;
     if (rc != FB_OK) {
         return nullptr;
     }
@@ -2940,22 +2945,11 @@ std::shared_ptr<Communicator::GroupPlan> Communicator::prepareGroup(const Neighb
     plan->dtype = dtype;
     plan->device = device_;
     plan->items = nItems;
-    size_t window = 0;
-    neighborVCheck(kind, items, nItems, dtype, window);
-    for (size_t w = 0; w < agreed.size(); w++) {
-        if (agreed[w] == 0) {
-            continue;
-        }
-        const size_t b = w * window;
-        std::vector<fb::GroupSeg> segs;
-        GroupLaunch l;
-        rc = neighborVBatch(kind, items + b, std::min(window, nItems - b), fbDtypeSize(dtype), agreed[w], segs, l);
-        rc = rc == FB_OK ? addPlanLaunch(*plan, segs, l) : rc;
-        if (rc != FB_OK) {
-            return nullptr;
-        }
-    }
-    return plan;
+    size_t w = 0;
+    rc = groupWalk(plan.get(), kind, dtype, 0, 0, 0, nullptr, [&](std::vector<fb::GroupSeg>& segs, GroupLaunch& l) {
+        return neighborVBatch(kind, items, nItems, fbDtypeSize(dtype), window, agreed, w, segs, l);
+    });
+    return rc == FB_OK ? plan : nullptr;
 }
 
 int Communicator::groupMany(GroupKind kind,
@@ -2970,84 +2964,20 @@ int Communicator::groupMany(GroupKind kind,
         return FB_E_INVALID;
     }
     NvtxRange nvtxRange(kGroupNames[kind].many);
-    bool grouped = false;
-    int rc = groupCheck(kind, dtype, 0, 0, flags, grouped);
+    size_t window = 0;
+    std::vector<uint64_t> mine;
+    const int rc = neighborVCheck(kind, items, nItems, dtype, flags, window, mine);
     if (rc != FB_OK) {
         return rc == GROUP_NOTHING ? FB_OK : rc;
-    }
-    std::vector<uint64_t> mine;
-    rc = neighborVStreams(kind, items, nItems, dtype, mine);
-    if (rc != FB_OK) {
-        return rc;
     }
     if (!neighborVAgrees(mine, agreed)) {
         return FB_E_INVALID;
     }
     bindDevice();
-    size_t window = 0;
-    neighborVCheck(kind, items, nItems, dtype, window);
-    for (size_t w = 0; w < agreed.size(); w++) {
-        if (agreed[w] == 0) {
-            continue;
-        }
-        const size_t b = w * window;
-        std::vector<fb::GroupSeg> segs;
-        GroupLaunch l;
-        neighborVBatch(kind, items + b, std::min(window, nItems - b), fbDtypeSize(dtype), agreed[w], segs, l);
-        stats_.segTables++;
-        ManySlot* slot = nullptr;
-        l.dSegs = (fb::GroupSeg*)stageManyTable(segs.data(), segs.size() * sizeof(fb::GroupSeg), s, &slot);
-        if (l.dSegs == nullptr && !loop_) {
-            return FB_E_CUDA;
-        }
-        rc = launchGroup(l, kind, dtype, 0, 0, flags, s);
-        if (rc != FB_OK) {
-            return rc;
-        }
-        releaseManySlot(slot, s);
-    }
-    return FB_OK;
-}
-
-// A window's rounds: each is a launch, LOCAL, barrier, MOVE, barrier (two
-// launches around stream-ordered barriers).  The grid follows from the
-// window's chunks per slot and the largest degrees, the same on every rank.
-int Communicator::launchNeighborV(const GroupLaunch& l, GroupKind kind, fb::GroupArgs& a, bool ss, int flags,
-                                  cudaStream_t s)
-{
-    const NeighborTopo& t = *topo_;
-    const bool a2a = kind == GROUP_NEIGHBOR_ALLTOALLV;
-    a.stageOff = stageSendOff_;
-    a.nEdges = (uint32_t)t.in.size();
-    a.outDeg = t.outDeg;
-    a.vWidth = l.width;
-    const uint64_t warps = (uint64_t)cfg_.threads / 32;
-    const uint64_t units = (uint64_t)l.totalChunks * std::max(neighborVSends(kind, t.maxOutDeg), t.maxInDeg);
-    const int blocks = (int)std::clamp<uint64_t>(
-      (units + warps - 1) / warps, 1, (uint64_t)groupGrid(cfg_, dev_.nranks, units * (FB_NEIGHBOR_CHUNK / 16)));
-    auto run = [&](int phase) {
-        a.phase = phase;
-        return k_->groupNeighborV(a, a2a, blocks, cfg_.threads, s) == cudaSuccess ? FB_OK : FB_E_CUDA;
-    };
-    for (uint32_t r = 0; r < l.rounds; r++) {
-        a.vBase = (uint64_t)r * l.width;
-        int rc;
-        if (!ss) {
-            rc = run(GROUP_PHASE_LOCAL | GROUP_PHASE_MOVE);
-        } else {
-            rc = run(GROUP_PHASE_LOCAL);
-            rc = rc == FB_OK ? streamBarrier(flags, s) : rc;
-            rc = rc == FB_OK ? run(GROUP_PHASE_MOVE) : rc;
-            rc = rc == FB_OK ? streamBarrier(flags, s) : rc;
-            stats_.stagedCopies++;
-        }
-        if (rc != FB_OK) {
-            return FB_E_CUDA;
-        }
-        stats_.launches++;
-    }
-    stats_.bytes += l.bytes;
-    return FB_OK;
+    size_t w = 0;
+    return groupWalk(nullptr, kind, dtype, 0, 0, flags, s, [&](std::vector<fb::GroupSeg>& segs, GroupLaunch& l) {
+        return neighborVBatch(kind, items, nItems, fbDtypeSize(dtype), window, agreed, w, segs, l);
+    });
 }
 
 // ---------------------------------------------------------------------------
